@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py - benchmarks of the ELD synthetic-noise training path on B200 (one process per GPU).
+"""bench.py - benchmarks of the ELD synthetic-noise training path on H100 (one process per GPU).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload train|infer|noise|fullframe] [--impl reference]
+                    [--dump-outputs DIR]
 
 Workloads = BASELINE.json configs (a "frame" is one 4x512x512 packed raw tensor unless stated):
     train      configs[2]  G+P* noise -> U-Net fwd + L1 + bwd -> (all-reduce) -> Adam, batch 8 per GPU, bf16   [default]
@@ -10,7 +11,9 @@ Workloads = BASELINE.json configs (a "frame" is one 4x512x512 packed raw tensor 
     fullframe  configs[4]  4-camera sweep over 4256 x 2848 full frames (packed 4 x 1424 x 2128), noise synthesis only
 Prints ONE JSON line on rank 0.  DESIGN.md section 7 defines value / e2e / roofline / roofline_noise / onbox_baseline /
 cpu_baseline.  `--impl reference` times the reference's own CPU path (numpy / torch-CPU port under oracle/) and never
-imports the product package.
+imports the product package.  `--dump-outputs DIR` writes what the last timed step computed as DIR/<name>.npy (float32;
+arrays larger than their share of 60 MB as a fixed, seeded sample), so that two builds can be compared output for output:
+with the same arguments the inputs are the same on every run.
 """
 import argparse
 import json
@@ -34,17 +37,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d['hbm_gbs'], d['bf16_tflops'], d.get('bf16_tflops_sustained', d['bf16_tflops']), 'measured'
-    return 6650.0, 1590.0, 1400.0, 'fallback'
-
-
-def ncu_traffic():
-    """DRAM bytes per launch from the committed ncu capture of this command (profiles/ncu_traffic.json, written by
-    tools/ncu_step_table.py from an `ncu --set full`-metric pass); None if no capture is committed."""
-    p = os.path.join(REPO, 'profiles', 'ncu_traffic.json')
-    try:
-        return json.load(open(p))
-    except Exception:
-        return None
+    return 3350.0, 989.0, 989.0, 'H100 SXM data sheet (700 W)'
 
 
 class ClockSampler:
@@ -185,20 +178,20 @@ def config_dict(a):
     w = a.workload
     if w == 'noise':
         return {'workload': 'noise.py %s sampler, batch %d x 4x512x512 packed raw (SonyA7S2 params), f32 in/out' % (a.model, a.batch),
-                'frames_per_step_per_gpu': a.batch, 'cache': 'inputs+outputs %d MiB per step > 126 MiB L2' % (a.batch * 8)}
+                'frames_per_step_per_gpu': a.batch, 'cache': 'inputs+outputs %d MiB per step > 50 MiB L2' % (a.batch * 8)}
     if w == 'fullframe':
         return {'workload': '4-camera parameter sweep (include 1..4), %s noise synthesis on 4256x2848 full frames = packed 4x%dx%d f32, '
                             '%d frames per GPU per step, cameras round-robin (BASELINE configs[4])' % (a.model, FULL_H, FULL_W, a.batch),
-                'frames_per_step_per_gpu': a.batch, 'cache': 'inputs+outputs %d MiB per step > 126 MiB L2' % (a.batch * 93),
+                'frames_per_step_per_gpu': a.batch, 'cache': 'inputs+outputs %d MiB per step > 50 MiB L2' % (a.batch * 93),
                 'equiv_512_frames_per_full_frame': FULL_H * FULL_W / (512.0 * 512.0)}
     if w == 'infer':
-        return {'workload': 'U-Net inference 1x4x512x512 (BASELINE configs[1]); bf16 tcgen05 tiles with fp32 accumulation serve the '
+        return {'workload': 'U-Net inference 1x4x512x512 (BASELINE configs[1]); bf16 wgmma tiles with fp32 accumulation serve the '
                             'fp32 request at rel-L2 <= 2e-2 (DESIGN 5.2)', 'global_batch': a.batch * a.gpus,
                 'frames_per_step_per_gpu': a.batch, 'parallelism': 'dp%d' % a.gpus,
-                'cache': 'activations of one forward ~180 MB > 126 MiB L2; 4 rotating inputs'}
+                'cache': 'activations of one forward ~180 MB > 50 MiB L2; 4 rotating inputs'}
     return {'workload': 'train_syn.py step: %s noise + U-Net fwd+L1+bwd+Adam, batch %d x 4x512x512 bf16, L1 loss (BASELINE configs[2])' % (a.model, a.batch),
             'global_batch': a.batch * a.gpus, 'frames_per_step_per_gpu': a.batch, 'parallelism': 'dp%d' % a.gpus,
-            'cache': 'activations %s > 126 MiB L2' % 'of a step'}
+            'cache': 'activations %s > 50 MiB L2' % 'of a step'}
 
 
 def reference_arm(a):
@@ -275,8 +268,10 @@ def make_noise_steps(a, dev, rank, world, full):
     dev_in = torch.empty(B, 4, h, w, device=dev)
     dev_out = torch.empty_like(dev_in)
 
+    last = {}
+
     def step(i):
-        nm.batch_gpu(clean[i & 1], params=plist, frame_id0=(i * world + rank) * B, out=noisy[i & 1])
+        last['noisy'] = nm.batch_gpu(clean[i & 1], params=plist, frame_id0=(i * world + rank) * B, out=noisy[i & 1])
 
     def step_e2e(i):
         dev_in.copy_(host_in, non_blocking=True)
@@ -284,7 +279,23 @@ def make_noise_steps(a, dev, rank, world, full):
         host_out.copy_(dev_out, non_blocking=True)
         torch.cuda.current_stream().synchronize()
 
-    return step, step_e2e, host_in.numel() * 4, host_out.numel() * 4, B * 4 * h * w * 8
+    return step, step_e2e, host_in.numel() * 4, host_out.numel() * 4, B * 4 * h * w * 8, lambda: {'noisy': last['noisy']}
+
+
+def dump_outputs(d, arrays, budget_bytes=60 * 1000 * 1000):
+    """arrays: name -> tensor.  Each is written as d/<name>.npy in float32; one larger than its share of the budget is
+    replaced by a fixed sample of its flattened elements (np.unique of randint(0, numel, share) drawn with seed 0, so the
+    same shape always gives the same indices)."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    cap = budget_bytes // 4 // max(1, len(arrays))
+    for name, t in arrays.items():
+        v = t.detach().reshape(-1).float()
+        if v.numel() > cap:
+            idx = np.unique(np.random.RandomState(0).randint(0, v.numel(), cap))
+            v = v[torch.from_numpy(idx).to(v.device)]
+        np.save(os.path.join(d, name + '.npy'), v.cpu().numpy().astype(np.float32))
 
 
 def main():
@@ -299,6 +310,8 @@ def main():
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-onbox', action='store_true', help='skip the torch-eager/cuDNN on-box baseline')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help="write the last timed step's outputs to DIR/<name>.npy (float32, at most 60 MB in all)")
     a = ap.parse_args()
     if a.batch is None:
         a.batch = {'train': 8, 'infer': 1, 'noise': 32, 'fullframe': 4}[a.workload]
@@ -333,7 +346,7 @@ def main():
         sampler.start()                                        # before warm-up; returns after its first row
     extra = {}
     if a.workload in ('noise', 'fullframe'):
-        step, step_e2e, h2d, d2h, kernel_bytes = make_noise_steps(a, dev, rank, world, a.workload == 'fullframe')
+        step, step_e2e, h2d, d2h, kernel_bytes, outputs = make_noise_steps(a, dev, rank, world, a.workload == 'fullframe')
         dtype = 'f32'
     else:
         from eld_b200.noise import NoiseModel
@@ -341,6 +354,7 @@ def main():
         nm = NoiseModel(a.model, include=4, verbose=False, seed=2018)
         mk = make_train_steps if a.workload == 'train' else make_infer_steps
         step, step_e2e, h2d, d2h, extra = mk(a, nm, dev, rank, world)
+        outputs = extra.pop('outputs')
         kernel_bytes = None
         dtype = 'bf16'
 
@@ -369,6 +383,8 @@ def main():
         clocks['sm_mhz_device_probe'] = float(probe.item())
     ms = ev[0].elapsed_time(ev[1])
     launches = _lib.launch_count(local) - l0
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, outputs())
     t = torch.tensor([ms], device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -390,20 +406,15 @@ def main():
         dist.all_reduce(te, op=dist.ReduceOp.MAX)
     e2e_value = B * world * e2e_steps / float(te.item())
 
-    traffic = ncu_traffic()
     if a.workload in ('noise', 'fullframe'):
         ach = kernel_bytes * a.steps / (ms * 1e-3) / 1e9   # the step IS the kernel
         key = 'noise:%s:%s' % (a.workload, a.model)
         roof = {'bound': 'hbm', 'achieved': ach, 'peak': hbm_peak, 'unit': 'GB/s', 'frac': ach / hbm_peak,
-                'traffic': (traffic or {}).get(key), 'kernel': 'noise_packed_*_kernel<%s>' % a.model, 'peak_source': peak_src,
+                'traffic': None, 'kernel': 'noise_packed_*_kernel<%s>' % a.model, 'peak_source': peak_src,
                 'algorithmic_bytes_per_launch': kernel_bytes, 'peak_kind': 'hbm_gbs (measured copy bandwidth)'}
     else:
         roof = extra.pop('roofline')
         roof['peak_source'] = peak_src
-        if traffic and a.workload in traffic:
-            roof['traffic'] = traffic[a.workload].get('tensor_tile_bytes_per_step')
-            if 'roofline_noise' in extra:
-                extra['roofline_noise']['traffic'] = traffic[a.workload].get('noise_bytes_per_launch')
 
     out = {'metric': METRIC, 'value': value, 'unit': 'frames/s', 'n_gpus': world,
            'steps': a.steps, 'warmup': a.warmup, 'ms_per_step': ms / a.steps, 'higher_is_better': True,

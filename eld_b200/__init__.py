@@ -1,4 +1,4 @@
-"""eld_b200 - B200-native (sm_100a) implementation of ELD's synthetic-noise training path.
+"""eld_b200 - H100-native (sm_90a) implementation of ELD's synthetic-noise training path.
 
 Host-side mirror of the reference seams (SURVEY 8b) over the C ABI in include/eld_b200.h:
     eld_b200.noise.NoiseModel        <- noise.NoiseModel            (reference noise.py:174)

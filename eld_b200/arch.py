@@ -4,7 +4,7 @@
 The module keeps the reference's parameter names / shapes / default init (state_dict keys
 conv{1..9}_{1,2}.{weight,bias}, upv{6..9}.*, conv10_1.*; Conv2d OIHW, ConvTranspose2d IOHW) so
 released checkpoints load, but all parameters are views into ONE flat fp32 buffer and the forward
-runs the tcgen05 engine behind the C ABI (csrc/unet_engine.cu) on NHWC bf16 activations.
+runs the wgmma engine behind the C ABI (csrc/unet_engine.cu) on NHWC bf16 activations.
 """
 import ctypes
 
@@ -57,13 +57,13 @@ class _EngineFunction(torch.autograd.Function):
 
 
 class UNetSeeInDark(nn.Module):
-    """B200-native UNetSeeInDark(in_channels, out_channels) for 4-channel packed raw and 3-channel sRGB frames on either
+    """H100-native UNetSeeInDark(in_channels, out_channels) for 4-channel packed raw and 3-channel sRGB frames on either
     side (ELD_model.py:377-389: --stage_in / --stage_out raw | srgb with --channels 4)."""
 
     def __init__(self, in_channels=4, out_channels=4):
         super().__init__()
         if in_channels not in (3, 4) or out_channels not in (3, 4):
-            raise NotImplementedError('the B200 engine takes 4-channel (packed Bayer) or 3-channel (sRGB) frames; X-Trans '
+            raise NotImplementedError('the engine takes 4-channel (packed Bayer) or 3-channel (sRGB) frames; X-Trans '
                                       '(--channels 9) is out of scope (SURVEY 8a row a-X)')
         self.in_channels, self.out_channels = in_channels, out_channels
         # real torch layers, constructed in the reference ORDER, only to reproduce the default init
@@ -147,7 +147,7 @@ class UNetSeeInDark(nn.Module):
             self._drop_engines(keep=self._MAX_ENGINES - 1)
             lib = _lib.load()
             dev = self._flat.device
-            assert dev.type == 'cuda', 'the B200 engine has no CPU path'
+            assert dev.type == 'cuda', 'the engine has no CPU path'
             assert lib.eld_unet_param_count_io(self.in_channels, self.out_channels) == self._flat.numel()
             nbytes = lib.eld_unet_workspace_bytes(n, h, w, int(train))
             ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)

@@ -1,4 +1,4 @@
-"""Build libeld_b200.so (CUDA, sm_100a) and the CPU oracle in-tree.
+"""Build libeld_b200.so (CUDA, sm_90a) and the CPU oracle in-tree.
 
     python -m eld_b200.build            # both
 Called by __graft_entry__.build().  nvcc cross-compiles without a GPU.
@@ -12,7 +12,7 @@ REPO = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libeld_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-ARCH = ['-gencode', 'arch=compute_100a,code=sm_100a']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 FLAGS = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC', '-Xcompiler', '-Wall',
          '-Xptxas', '-v', '--expt-relaxed-constexpr']
 

@@ -36,8 +36,8 @@ int eld_ctx_create(int device, eld_ctx** out)
     ELD_CHECK_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     ELD_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-        eld::set_error("eld_ctx_create: device %d is sm_%d%d; this library is built for sm_100a only",
+    if (prop.major != 9 || prop.minor != 0) {
+        eld::set_error("eld_ctx_create: device %d is sm_%d%d; this library is built for sm_90a only",
                        device, prop.major, prop.minor);
         return ELD_E_UNSUPPORTED;
     }

@@ -1,19 +1,18 @@
-// conv_umma.cuh - persistent, warp-specialised tcgen05 implicit-GEMM tile for the U-Net's
-// conv3x3 / deconv2x2 (fprop and dgrad) on NHWC bf16 activations.
+// conv_umma.cuh - persistent, warp-specialised wgmma implicit-GEMM tile for the U-Net's conv3x3 / deconv2x2
+// (fprop and dgrad) on NHWC bf16 activations.
 //
-//   D[128 pixels x n_tile] (f32, TMEM)  +=  A[128 pixels x K] (bf16, smem via TMA)  *  B[n_tile x K]^T
+//   D[128 pixels x n_tile] (f32, registers)  +=  A[128 pixels x K] (bf16, smem via TMA)  *  B[n_tile x K]^T
 //
-// M tile  = an 8 x 16 pixel patch of one image (TMA box {kc, 16, 8}); every filter tap is one more
-//           box at shifted coordinates - TMA zero-fills out-of-image pixels, which IS the padding.
-// K       = taps x cin, walked in chunks of kc = 32 or 64 channels (one 64 B / 128 B swizzled row per
-//           pixel), each chunk = kc/16 tcgen05.mma.kind::f16 instructions (M=128, N=n_tile, K=16).
-// halo    = for conv3x3 with a small weight operand the three vertical taps of one filter column share ONE
-//           TMA box {kc, 16, 10}: tap kh is the same smem tile read 16 pixel rows (a multiple of the swizzle
-//           period) further down - 2.4x fewer L2->SM requests; weights can stay RESIDENT in smem for the
-//           whole persistent CTA (b_res) so thin full-resolution layers stream activations only.
-// roles   = warp 0: TMA producer | warp 1: MMA issuer (one elected lane) | warps 2-5: epilogue
-//           (tcgen05.ld -> bias / LeakyReLU / mask -> bf16 -> global).  Two TMEM accumulators so the
-//           epilogue of tile i overlaps the MMAs of tile i+1.
+// M tile  = an 8 x 16 pixel patch of one image (TMA box {kc, 16, 8}); every filter tap is one more box at shifted
+//           coordinates - TMA zero-fills out-of-image pixels, which IS the padding.
+// K       = taps x cin, walked in chunks of kc = 32 or 64 channels (one 64 B / 128 B swizzled row per pixel);
+//           each chunk = kc/16 wgmma.m64nNk16 per consumer warpgroup.
+// B       = the packed weights (unet_prims.h packed_index): one [n_tile x kc] block per (tap, chunk), already in the
+//           swizzled shared-memory image, one linear bulk copy each.
+// roles   = warpgroup 0: TMA producer (one thread) | warpgroups 1, 2: wgmma on pixel rows 0-63 / 64-127 of the tile,
+//           then the epilogue of those rows (accumulators -> smem -> one pixel x 32 channels per thread ->
+//           bias / LeakyReLU / mask -> bf16 -> global).  The producer runs ahead across tiles, so the next tile's
+//           operands load while the consumers run the epilogue.
 #pragma once
 #include "umma.cuh"
 #include "unet_prims.h"
@@ -21,15 +20,15 @@
 
 namespace eld {
 
-
 struct ConvGemmParams {
-    int n_img, H, W;      // output pixel grid (M space); H % 8 == 0, W % 16 == 0
-    int tiles_x, tiles_y;
+    int n_img, H, W;      // output pixel grid (M space)
+    int tiles_x, tiles_y; // 16 x 8 pixel tiles
     int taps, a_mode;     // 9/1 with A_CONV, 4 with A_GATHER
     int cin;              // K channels per tap
     int a_c0;             // first channel inside the A tensor (concat buffers)
     int kc;               // 32 or 64
-    int n_total, n_tile;  // GEMM N and per-CTA N (n_tile % 32 == 0, <= 256)
+    int n_total, n_tile;  // GEMM N and per-tile N (32, 64 or 128)
+    int b_rows;           // rows of one packed weight block (min(n_total, 256), unet_prims.h packed_index)
     int epi_mode, act;
     __nv_bfloat16* out;
     int out_pitch, out_c0;
@@ -40,265 +39,186 @@ struct ConvGemmParams {
                                // 2j+1 -> bit 16+j of its 32-channel chunk (what `sign_out` of the producing forward tile wrote)
     uint32_t* sign_out;        // optional (training): sign words of the activated output, same layout
     int cout;             // EPI_SHUFFLE: channels per sub-pixel
-    int stages;
-    int tmem_cols;
-    int halo;             // conv3x3: one {kc,16,10} box per filter column, kh taps = row-shifted views
-    int b_res;            // weights resident in smem (loaded once per CTA); requires n_total == n_tile
-    int tile_w;           // 16 (8x16 patch) or 8 (16x8 patch, full-halo mode)
-    int bo_mode;          // full-halo mode: 1 = put (start>>7)&7 into the descriptor's base_offset field
-    const uint8_t* b_ptr; // packed weights: blocks [n_tile][tap][chunk] in smem-image order (unet_prims.h packed_index)
-    int b_stages;         // halo == 3: depth of the separate weight ring (stages of b_group taps)
-    int b_group;          // halo == 3: filter taps per weight-ring stage (3, or 1 for n_tile == 256)
-    int l2_prefetch;      // full-halo mode: prefetch the A box this many tiles ahead into L2 (0 = off)
-    int dbg;              // experiments only (ELD_CONV_DBG): 1 = skip the global stores, 2 = skip bias, 4 = skip tcgen05.ld,
-                          // 8 = skip the activation TMA loads (full-halo modes), 16 = skip the MMAs
-    int acc_stages;       // TMEM accumulator ring depth (2..8, even): acc_stages * n_tile <= 512 columns
     int cout_shift;       // EPI_SHUFFLE: log2(cout) (cout must be a power of two)
+    int stages;
+    const uint8_t* b_ptr; // packed weights
     __nv_bfloat16* pool_out;   // optional fused MaxPool2d(2) of the (activated) output: bf16 NHWC [n][H/2][W/2][pool_pitch]
     int pool_pitch;
     uint32_t* pool_code;       // optional (training): 32 bytes per (pooled pixel, 32 channels) = which window element won and the
                                // four signs, all the pool backward needs of the activation (unet_ew.cu maxpool_bwd_code_kernel)
     __nv_bfloat16* out2;  // EPI_STORE split store: GEMM columns >= out_split go to out2[pix * out2_pitch + (col - out_split)]
     int out2_pitch, out_split;   // (planar halves of a concat gradient); out_split % 32 == 0, 0 = off
-    long long* prof;      // PROF instantiation only
-    int bias_smem_off;    // byte offset (from the 1024-aligned base) of the per-CTA bias copy
+    int bias_smem_off, stg_smem_off, bar_smem_off;   // byte offsets from the 1024-aligned base
 };
 
-// max of two packed bf16 pairs (HMNMX2.BF16)
+// max of two packed bf16 pairs
 __device__ __forceinline__ uint32_t bf2_max(uint32_t a, uint32_t b)
 {
     const __nv_bfloat162 m = __hmax2(*reinterpret_cast<const __nv_bfloat162*>(&a), *reinterpret_cast<const __nv_bfloat162*>(&b));
     return *reinterpret_cast<const uint32_t*>(&m);
 }
 
-// Two tiles at once: consecutive MMAs alternate between two accumulators, so an N = 32 tile's chain of
-// 18 dependent accumulates no longer runs at MMA latency (measured: ~100 cycles per dependent N=32 MMA).
-template <int KSUB>
-__device__ __forceinline__ void issue_halo2_pair(uint32_t d0, uint32_t d1, uint32_t a0_lo, uint32_t a1_lo, uint32_t a_hi,
-                                                 uint32_t b_lo, uint32_t b_hi, uint32_t b_tap_step, uint32_t idesc)
+constexpr int kConvThreads = 384;
+constexpr int kConvStg = 68;          // floats per staged pixel row (64 columns + 4: conflict-free 16-byte reads)
+constexpr int kConvTileW = 16;        // pixels per tile row; a warp of the epilogue holds two tile rows
+
+// One pixel x 32 GEMM columns of the epilogue: bias, activation / mask, bf16 rounding, sign words, fused pool, store.
+// All 32 lanes of the warp call it together (the pool's 2x2 window lives in lanes ^1 and ^16).
+__device__ __forceinline__ void conv_epilogue32(const ConvGemmParams& p, const float* s_bias, float (&v)[32],
+                                                int img, int x, int y, int col)
 {
-    constexpr uint32_t kRow = (uint32_t)(32 * KSUB) >> 4;
-#pragma unroll
-    for (int tap = 0; tap < 9; ++tap) {
-        const uint32_t off = (uint32_t)((tap / 3) * 10 + (tap % 3)) * kRow;
-#pragma unroll
-        for (int k = 0; k < KSUB; ++k) {
-            ptx::umma_bf16_lohi(d0, a0_lo + off + 2u * k, a_hi, b_lo + 2u * k, b_hi, idesc, !(tap == 0 && k == 0));
-            ptx::umma_bf16_lohi(d1, a1_lo + off + 2u * k, a_hi, b_lo + 2u * k, b_hi, idesc, !(tap == 0 && k == 0));
-        }
-        b_lo += b_tap_step;
+    const bool in_img = x < p.W && y < p.H;          // partial tiles at the right / bottom image border
+    const int pix = (img * p.H + y) * p.W + x;
+    __nv_bfloat16* dst;
+    int bcol;
+    if (p.epi_mode == EPI_STORE) {
+        dst = (p.out_split && col >= p.out_split) ? p.out2 + (size_t)pix * p.out2_pitch + (col - p.out_split)
+                                                  : p.out + (size_t)pix * p.out_pitch + (p.out_c0 + col);
+        bcol = col;
+    } else {
+        const int sub = col >> p.cout_shift, co = col & (p.cout - 1);   // sub = kh*2 + kw
+        const int oy = 2 * y + (sub >> 1), ox = 2 * x + (sub & 1);
+        dst = p.out + ((size_t)(img * 2 * p.H + oy) * (2 * p.W) + ox) * p.out_pitch + p.out_c0 + co;
+        bcol = co;
     }
-}
-
-constexpr int kConvThreads = 320;   // warp 0 TMA, warp 1 MMA, warps 2-5 and 6-9: two epilogue groups (alternate tiles)
-constexpr int kMaxAccStages = 8;
-
-// Full-halo issue: 9 taps x KSUB tcgen05.mma, fully unrolled so that every operand offset is an immediate
-// (the MMA issuer is ONE thread: for N = 32 tiles its instruction count per MMA is what bounds the layer).
-template <int KSUB>
-__device__ __forceinline__ void issue_halo2(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                            uint32_t b_tap_step, uint32_t idesc, bool first_chunk)
-{
-    constexpr uint32_t kRow = (uint32_t)(32 * KSUB) >> 4;          // one pixel row of kc = 16*KSUB channels, in 16 B units
+    if (p.bias) {
+        const float4* sb4 = reinterpret_cast<const float4*>(s_bias);
 #pragma unroll
-    for (int tap = 0; tap < 9; ++tap) {
-        const uint32_t a_tap = a_lo + (uint32_t)((tap / 3) * 10 + (tap % 3)) * kRow;
-#pragma unroll
-        for (int k = 0; k < KSUB; ++k)
-            ptx::umma_bf16_lohi(d_tmem, a_tap + 2u * k, a_hi, b_lo + 2u * k, b_hi, idesc, !(first_chunk && tap == 0 && k == 0));
-        b_lo += b_tap_step;
-    }
-}
-
-// halo == 3: the BG filter taps of one weight-ring stage (taps T0 .. T0+BG-1 of one channel chunk), fully unrolled
-// so that every descriptor offset is an immediate.  flag0 = accumulate flag of the very first MMA (tap 0, k 0).
-template <int KSUB, int BG, int T0>
-__device__ __forceinline__ void issue_halo3_group(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                                  uint32_t b_step, uint32_t idesc, uint32_t flag0)
-{
-    constexpr uint32_t kRow = (uint32_t)(32 * KSUB) >> 4;
-#pragma unroll
-    for (int t = 0; t < BG; ++t) {
-        constexpr int dummy = 0; (void)dummy;
-        const int tap = T0 + t;
-        const uint32_t a_tap = a_lo + (uint32_t)((tap / 3) * 10 + (tap % 3)) * kRow;
-        const uint32_t b_tap = b_lo + (uint32_t)t * b_step;
-#pragma unroll
-        for (int k = 0; k < KSUB; ++k) {
-            if (T0 == 0 && t == 0 && k == 0) {
-                const uint64_t ad = ((uint64_t)a_hi << 32) | a_tap, bd = ((uint64_t)b_hi << 32) | b_tap;
-                ptx::umma_bf16(d_tmem, ad, bd, idesc, flag0);
-            } else {
-                ptx::umma_bf16_lohi(d_tmem, a_tap + 2u * k, a_hi, b_tap + 2u * k, b_hi, idesc, true);
-            }
+        for (int j = 0; j < 8; ++j) {
+            const float4 b = sb4[(bcol >> 2) + j];
+            v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
         }
     }
+    if (p.act == ACT_LRELU) {
+#pragma unroll
+        for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.2f * v[j]);
+    } else if (p.act == ACT_MASK && in_img && p.aux_sign) {
+        const uint32_t sgw = __ldg(p.aux_sign + (size_t)pix * (size_t)(p.n_total >> 5) + (size_t)(col >> 5));
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            // slope = 0.6 + 0.4 * (+-1) = 1 or 0.2
+            const float s_lo = __uint_as_float(((sgw << (31 - j)) & 0x80000000u) | 0x3F800000u);
+            const float s_hi = __uint_as_float(((sgw << (15 - j)) & 0x80000000u) | 0x3F800000u);
+            v[2 * j] *= __fmaf_rn(s_lo, 0.4f, 0.6f);
+            v[2 * j + 1] *= __fmaf_rn(s_hi, 0.4f, 0.6f);
+        }
+    } else if (p.act == ACT_MASK && in_img) {
+        uint32_t mk[16];
+        const __nv_bfloat16* ap = p.aux + (size_t)pix * p.aux_pitch + (p.aux_c0 + col);
+        ptx::ld_global_nc_32B(ap, mk);
+        ptx::ld_global_nc_32B(ap + 16, mk + 8);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            // LeakyReLU keeps the sign: slope = 0.6 + 0.4 * sign(activation) = 1 or 0.2
+            // (activation == +0 counts as positive; the reference's tie is a measure-zero event)
+            const float s_lo = __uint_as_float(((mk[j] << 16) & 0x80000000u) | 0x3F800000u);
+            const float s_hi = __uint_as_float((mk[j] & 0x80000000u) | 0x3F800000u);
+            v[2 * j] *= __fmaf_rn(s_lo, 0.4f, 0.6f);
+            v[2 * j + 1] *= __fmaf_rn(s_hi, 0.4f, 0.6f);
+        }
+    }
+    // round once; the pool below works on the rounded (= stored) values
+    uint32_t wv[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        const __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
+        wv[j] = *reinterpret_cast<const uint32_t*>(&h);
+    }
+    if (p.sign_out && in_img) {
+        // sign words of the stored activation: all a later LeakyReLU' needs (1/16 of the tensor)
+        p.sign_out[(size_t)pix * (size_t)(p.n_total >> 5) + (size_t)(col >> 5)] = ptx::gather_msb16(wv);
+    }
+    if (p.pool_out) {
+        // MaxPool2d(2) fused: the 2x2 window of pixel (x, y) lives in lanes ^1 (x) and ^16 (y) of this warp; packed bf16x2
+        // max of the stored values.  H, W and the tile origin are even: a window is wholly in or out.
+        uint32_t pw[16];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const uint32_t a = bf2_max(wv[j], __shfl_xor_sync(0xffffffffu, wv[j], 1));
+            pw[j] = bf2_max(a, __shfl_xor_sync(0xffffffffu, a, kConvTileW));
+        }
+        const bool origin = in_img && !((x | y) & 1);
+        const size_t ppix = (size_t)(img * (p.H >> 1) + (y >> 1)) * (p.W >> 1) + (x >> 1);
+        if (origin) {
+            __nv_bfloat16* q4 = p.pool_out + ppix * p.pool_pitch + col;
+            ptx::st_global_32B(q4, pw);
+            ptx::st_global_32B(q4 + 16, pw + 8);
+        }
+        if (p.pool_code) {
+            // per lane two 32-bit masks over its 32 channels: "is not the window's maximum" and "is negative"
+            // (channel 2j -> bit j, channel 2j+1 -> bit 16+j); the window's origin lane collects the four lanes'
+            // masks in the order the backward walks the window: (0,0) (0,1) (1,0) (1,1)
+            uint32_t ne[16];
+#pragma unroll
+            for (int j = 0; j < 16; ++j)
+                ne[j] = __hne2_mask(*reinterpret_cast<const __nv_bfloat162*>(&wv[j]), *reinterpret_cast<const __nv_bfloat162*>(&pw[j]));
+            const uint32_t nm = ptx::gather_msb16(ne), sg = ptx::gather_msb16(wv);
+            uint32_t code[8];
+            code[0] = nm; code[4] = sg;
+            code[1] = __shfl_xor_sync(0xffffffffu, nm, 1);                code[5] = __shfl_xor_sync(0xffffffffu, sg, 1);
+            code[2] = __shfl_xor_sync(0xffffffffu, nm, kConvTileW);       code[6] = __shfl_xor_sync(0xffffffffu, sg, kConvTileW);
+            code[3] = __shfl_xor_sync(0xffffffffu, nm, kConvTileW | 1);   code[7] = __shfl_xor_sync(0xffffffffu, sg, kConvTileW | 1);
+            if (origin) ptx::st_global_32B(p.pool_code + (ppix * (size_t)(p.pool_pitch >> 5) + (size_t)(col >> 5)) * 8, code);
+        }
+    }
+    if (!in_img) return;
+    ptx::st_global_32B(dst, wv);                       // 64 bytes per pixel = two full 32-byte sectors
+    ptx::st_global_32B(dst + 16, wv + 8);
 }
 
-// PROF = true (ELD_CONV_PROF, debugging only): every role accumulates the cycles it spends blocked on each kind of
-// barrier and writes them to p.prof[blockIdx.x][16] - who waits for whom, per layer.
-#define ELD_WAIT(bar, par, ctr)                                                                    \
-    do {                                                                                           \
-        if (PROF) { const long long t_ = clock64(); ptx::mbar_wait((bar), (par)); (ctr) += clock64() - t_; } \
-        else ptx::mbar_wait((bar), (par));                                                         \
-    } while (0)
-
-template <bool PROF>
+template <int NT>
 __global__ void __launch_bounds__(kConvThreads, 1)
-conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParams p)
+conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParams p)
 {
-    long long pw0 = 0, pw1 = 0, pt0 = 0;
-    if (PROF) pt0 = clock64();
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = ptx::smem_u32(smem_raw);
     uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
 
     const int row_bytes = p.kc * 2;
-    // halo == 2 ("full halo"): ONE box {kc, 10, 18} per channel chunk; all nine taps are views of it
-    // (start shifted by (kh*10 + kw) pixel rows, 8-row groups 10 rows apart) - needs b_res.
-    const int a_bytes = p.halo >= 2 ? ((180 * row_bytes + 1023) & ~1023) : (p.halo ? 160 : 128) * row_bytes;
-    const int b_bytes = p.n_tile * row_bytes;                       // one tap, one channel chunk
+    const int a_bytes = 128 * row_bytes;
+    const int b_bytes = NT * row_bytes;                 // one tap, one channel chunk, this tile's NT weight rows
+    const int stage_bytes = a_bytes + b_bytes;
     const int kchunks = p.cin / p.kc;
-    // halo == 3: full-halo activations (one {kc,10,18} box per channel chunk, ring of `stages`) and weights
-    // STREAMED through their own ring of `b_stages` one-tap tiles - 180 + 9*n_tile TMA rows per chunk instead
-    // of 9*(128 + n_tile).
-    const int b_per_stage = (p.b_res || p.halo == 3) ? 0 : (p.halo ? 3 : 1);
-    const int stage_bytes = a_bytes + b_per_stage * b_bytes;
-    const int bres_bytes = p.b_res ? p.taps * kchunks * b_bytes : 0;
-    uint8_t* stage0 = smem + bres_bytes;
-    uint8_t* bring0 = stage0 + (size_t)p.stages * stage_bytes;
-    const int bring_bytes = p.halo == 3 ? p.b_stages * p.b_group * b_bytes : 0;
-    uint64_t* full = reinterpret_cast<uint64_t*>(bring0 + bring_bytes);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.bar_smem_off);
     uint64_t* empty = full + p.stages;
-    uint64_t* tmem_full = empty + p.stages;
-    uint64_t* tmem_empty = tmem_full + kMaxAccStages;
-    uint64_t* bres_full = tmem_empty + kMaxAccStages;
-    uint64_t* bfull = bres_full + 1;               // halo == 3 weight ring (<= 8 stages)
-    uint64_t* bempty = bfull + 8;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bempty + 8);
     float* s_bias = reinterpret_cast<float*>(smem + p.bias_smem_off);      // bias staged once per CTA (16-byte aligned)
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n_tiles = p.n_total / p.n_tile;
-    const int m_tiles = p.n_img * p.tiles_y * p.tiles_x;
-    const int total_tiles = m_tiles * n_tiles;
-    const int ksteps = (p.halo >= 2 ? 1 : (p.halo ? 3 : p.taps)) * kchunks;
-    const int tile_h = 128 / p.tile_w;
+    const int lane = threadIdx.x & 31;
+    const int n_tiles = p.n_total / NT;
+    const int total_tiles = p.n_img * p.tiles_y * p.tiles_x * n_tiles;
+    const int ksteps = p.taps * kchunks;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         ptx::prefetch_tmap(&tmA);
-        for (int s = 0; s < p.stages; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 1); }
-        for (int a = 0; a < p.acc_stages; ++a) { ptx::mbar_init(&tmem_full[a], 1); ptx::mbar_init(&tmem_empty[a], 4); }
-        ptx::mbar_init(bres_full, 1);
-        for (int b = 0; b < 8; ++b) { ptx::mbar_init(&bfull[b], 1); ptx::mbar_init(&bempty[b], 1); }
+        for (int s = 0; s < p.stages; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 8); }
         ptx::fence_barrier_init();
     }
-    if (warp == 2) ptx::tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
     if (p.bias) {
         const int nb = p.epi_mode == EPI_STORE ? p.n_total : p.cout;
         for (int i = threadIdx.x; i < nb; i += kConvThreads) s_bias[i] = __ldg(p.bias + i);
     }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    // PDL: everything above touched only this launch's parameters, the bias and nothing the previous kernel writes;
-    // the activations (TMA loads, mask reads) and the output must wait for it.  The packed weights were written before
-    // the forward pass started and only conv / wgrad tiles release their successor early, so they are stable too.
+    // PDL: everything above touched only this launch's parameters and the bias; the activations (TMA loads, mask
+    // reads) and the output must wait for the previous kernel.  The packed weights were written before the pass started.
     ptx::grid_dep_wait();
     ptx::grid_dep_launch();
 
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        if (lane == 0) {
-            if (p.b_res) {
-                ptx::mbar_arrive_expect_tx(bres_full, (uint32_t)bres_bytes);
-                for (int j = 0; j < p.taps; ++j)                    // the whole operand is one contiguous smem image
-                    ptx::bulk_load(smem + (size_t)j * kchunks * b_bytes, p.b_ptr + (size_t)j * kchunks * b_bytes,
-                                   (uint32_t)(kchunks * b_bytes), bres_full);
-            }
-            int s = 0, sb = 0;
-            uint32_t ph = 0, bph = 0;
-            uint8_t* sa = stage0;
+    if (threadIdx.x < 128) {
+        // ===================== TMA producer (warpgroup 0; one thread works) =====================
+        if (threadIdx.x == 0) {
+            int s = 0;
+            uint32_t ph = 0;
             const int tiles_xy = p.tiles_x * p.tiles_y;
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const int m_tile = tile / n_tiles, n_t = tile - m_tile * n_tiles;
                 const int img = m_tile / tiles_xy;
                 const int rem = m_tile - img * tiles_xy;
                 const int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
-                const int x0 = tx * p.tile_w, y0 = ty * tile_h;
-                if (p.halo == 3) {
-                    int c = p.a_c0;
-                    for (int kcI = 0; kcI < kchunks; ++kcI) {
-                        ELD_WAIT(&empty[s], ph ^ 1u, pw0);
-                        if (p.dbg & 8) ptx::mbar_arrive(&full[s]);
-                        else {
-                            ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)(180 * row_bytes));
-                            ptx::tma_load_5d(sa, &tmA, &full[s], c, x0 - 1, y0 - 1, img, 0);
-                        }
-                        for (int tap = 0; tap < 9; tap += p.b_group) {     // one ring stage = b_group taps
-                            ELD_WAIT(&bempty[sb], bph ^ 1u, pw1);
-                            ptx::mbar_arrive_expect_tx(&bfull[sb], (uint32_t)(p.b_group * b_bytes));
-                            for (int t = 0; t < p.b_group; ++t)
-                                ptx::bulk_load(bring0 + ((size_t)sb * p.b_group + t) * b_bytes,
-                                               p.b_ptr + ((size_t)(n_t * 9 + tap + t) * kchunks + kcI) * b_bytes, (uint32_t)b_bytes, &bfull[sb]);
-                            if (++sb == p.b_stages) { sb = 0; bph ^= 1u; }
-                        }
-                        c += p.kc;
-                        sa += stage_bytes;
-                        if (++s == p.stages) { s = 0; ph ^= 1u; sa = stage0; }
-                    }
-                    continue;
-                }
-                if (p.halo == 2) {
-                    if (p.l2_prefetch > 0) {
-                        // pull the box of the tile `l2_prefetch` iterations ahead into L2 (DRAM-sourced TMA rows are
-                        // ~2x slower than L2 hits; the stream is perfectly predictable)
-                        const int ft = tile + p.l2_prefetch * (int)gridDim.x;
-                        if (ft < total_tiles) {
-                            const int fm = ft / n_tiles;
-                            const int fimg = fm / tiles_xy, frem = fm - fimg * tiles_xy;
-                            const int fty = frem / p.tiles_x, ftx = frem - fty * p.tiles_x;
-                            for (int kcI = 0; kcI < kchunks; ++kcI)
-                                ptx::tma_prefetch_5d(&tmA, p.a_c0 + kcI * p.kc, ftx * p.tile_w - 1, fty * tile_h - 1, fimg, 0);
-                        }
-                    }
-                    int c = p.a_c0;
-                    for (int kcI = 0; kcI < kchunks; ++kcI) {
-                        ELD_WAIT(&empty[s], ph ^ 1u, pw0);
-                        if (p.dbg & 8) ptx::mbar_arrive(&full[s]);
-                        else {
-                            ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)(180 * row_bytes));
-                            ptx::tma_load_5d(sa, &tmA, &full[s], c, x0 - 1, y0 - 1, img, 0);
-                        }
-                        c += p.kc;
-                        sa += stage_bytes;
-                        if (++s == p.stages) { s = 0; ph ^= 1u; sa = stage0; }
-                    }
-                    continue;
-                }
-                if (p.halo) {
-                    for (int kw = 0; kw < 3; ++kw) {
-                        int c = p.a_c0;
-                        for (int kcI = 0; kcI < kchunks; ++kcI) {
-                            ELD_WAIT(&empty[s], ph ^ 1u, pw0);
-                            ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)stage_bytes);
-                            ptx::tma_load_5d(sa, &tmA, &full[s], c, x0 + kw - 1, y0 - 1, img, 0);
-                            if (!p.b_res) {
-                                for (int kh = 0; kh < 3; ++kh)
-                                    ptx::bulk_load(sa + a_bytes + kh * b_bytes,
-                                                   p.b_ptr + ((size_t)(n_t * 9 + kh * 3 + kw) * kchunks + kcI) * b_bytes,
-                                                   (uint32_t)b_bytes, &full[s]);
-                            }
-                            c += p.kc;
-                            sa += stage_bytes;
-                            if (++s == p.stages) { s = 0; ph ^= 1u; sa = stage0; }
-                        }
-                    }
-                    continue;
-                }
+                const int x0 = tx * kConvTileW, y0 = ty * 8;
                 const int gy = img * p.H + y0;
-                int kb = 0;                                   // K coordinate in the weight matrix
+                // weight rows n_t*NT .. +NT live in packed block n_t*NT / b_rows, from row n_t*NT % b_rows on
+                const int pb = (n_t * NT) / p.b_rows, pr = (n_t * NT) - pb * p.b_rows;
+                const uint8_t* bsrc = p.b_ptr + (size_t)pb * p.taps * kchunks * p.b_rows * row_bytes + (size_t)pr * row_bytes;
                 for (int tap = 0; tap < p.taps; ++tap) {
                     int c1, c2, c3, c4;
                     if (p.a_mode == A_CONV) {
@@ -311,352 +231,86 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParams p
                     }
                     int c = p.a_c0;
                     for (int kcI = 0; kcI < kchunks; ++kcI) {
-                        ELD_WAIT(&empty[s], ph ^ 1u, pw0);
+                        ptx::mbar_wait(&empty[s], ph ^ 1u);
+                        uint8_t* sa = smem + (size_t)s * stage_bytes;
                         ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)stage_bytes);
                         ptx::tma_load_5d(sa, &tmA, &full[s], c, c1, c2, c3, c4);
-                        if (!p.b_res) ptx::bulk_load(sa + a_bytes, p.b_ptr + ((size_t)(n_t * p.taps + tap) * kchunks + kcI) * b_bytes,
-                                                     (uint32_t)b_bytes, &full[s]);
-                        c += p.kc; kb += p.kc;
-                        sa += stage_bytes;
-                        if (++s == p.stages) { s = 0; ph ^= 1u; sa = stage0; }
+                        ptx::bulk_load(sa + a_bytes, bsrc + (size_t)(tap * kchunks + kcI) * p.b_rows * row_bytes,
+                                       (uint32_t)b_bytes, &full[s]);
+                        c += p.kc;
+                        if (++s == p.stages) { s = 0; ph ^= 1u; }
                     }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        const uint32_t idesc = ptx::make_idesc_bf16(128, (uint32_t)p.n_tile, 0, 0);
-        const uint32_t layout = (p.kc == 64) ? ptx::LAYOUT_SW128 : ptx::LAYOUT_SW64;
-        const uint32_t sbo = (p.kc == 64) ? 1024u : 512u;
-        const uint64_t desc_hi = ptx::make_smem_desc(0, 16, sbo, layout);   // everything but the address
-        const uint32_t stage_base = ptx::smem_u32(stage0);
-        const uint32_t bres_base = ptx::smem_u32(smem);
-        const int ksub = p.kc / 16;
-        const int nsub = p.halo ? 3 : 1;                                    // taps served by one stage
-        const uint32_t a_tap_step = (uint32_t)(16 * row_bytes) >> 4;        // one image row of the patch, in 16 B units
-        const uint32_t b_step = (uint32_t)b_bytes >> 4;
-        int s = 0;
-        uint32_t ph = 0, tile_it = 0;
-        uint32_t a_addr = stage_base;
-        if (p.b_res) { ptx::mbar_wait(bres_full, 0); ptx::tc_fence_after(); }
-        uint32_t acc = 0, acc_ph = 0;
-        int tile = blockIdx.x;
-        if (p.halo == 2 && kchunks == 1) {
-            // pairs of tiles (one stage each), interleaved issue
-            const uint64_t a_hi64 = ptx::make_smem_desc(0, 16, 10u * row_bytes, layout);
-            const uint32_t a_hi = (uint32_t)(a_hi64 >> 32);
-            const uint32_t b_lo = (uint32_t)desc_hi | ((bres_base & 0x3FFFFu) >> 4);
-            for (; tile + (int)gridDim.x < total_tiles; tile += 2 * gridDim.x, tile_it += 2) {
-                const uint32_t acc0 = acc, ph0 = acc_ph;
-                if (++acc == (uint32_t)p.acc_stages) { acc = 0; acc_ph ^= 1u; }
-                const uint32_t acc1 = acc, ph1 = acc_ph;
-                if (++acc == (uint32_t)p.acc_stages) { acc = 0; acc_ph ^= 1u; }
-                ELD_WAIT(&tmem_empty[acc0], ph0 ^ 1u, pw0);
-                ELD_WAIT(&tmem_empty[acc1], ph1 ^ 1u, pw0);
-                const int s0 = s; const uint32_t sph0 = ph; const uint32_t a0 = a_addr;
-                a_addr += (uint32_t)stage_bytes;
-                if (++s == p.stages) { s = 0; ph ^= 1u; a_addr = stage_base; }
-                const int s1 = s; const uint32_t sph1 = ph; const uint32_t a1 = a_addr;
-                a_addr += (uint32_t)stage_bytes;
-                if (++s == p.stages) { s = 0; ph ^= 1u; a_addr = stage_base; }
-                ELD_WAIT(&full[s0], sph0, pw1);
-                ELD_WAIT(&full[s1], sph1, pw1);
-                ptx::tc_fence_after();
-                if (ptx::elect_one()) {
-                    const uint32_t d0 = tmem_base + acc0 * (uint32_t)p.n_tile, d1 = tmem_base + acc1 * (uint32_t)p.n_tile;
-                    const uint32_t a0_lo = (uint32_t)a_hi64 | ((a0 & 0x3FFFFu) >> 4), a1_lo = (uint32_t)a_hi64 | ((a1 & 0x3FFFFu) >> 4);
-                    if (p.dbg & 16) { }
-                    else if (ksub == 2) issue_halo2_pair<2>(d0, d1, a0_lo, a1_lo, a_hi, b_lo, (uint32_t)(desc_hi >> 32), b_step, idesc);
-                    else                issue_halo2_pair<4>(d0, d1, a0_lo, a1_lo, a_hi, b_lo, (uint32_t)(desc_hi >> 32), b_step, idesc);
-                    ptx::umma_commit(&empty[s0]);
-                    ptx::umma_commit(&empty[s1]);
-                    ptx::umma_commit(&tmem_full[acc0]);
-                    ptx::umma_commit(&tmem_full[acc1]);
-                }
-                __syncwarp();
-            }
+        return;
+    }
+
+    // ===================== consumers: warpgroup cg = 0 / 1 owns pixel rows 64 cg .. 64 cg + 63 =====================
+    const int cg = (threadIdx.x >> 7) - 1;
+    const int t = threadIdx.x & 127;
+    const uint32_t layout = ptx::gmma_layout(row_bytes);
+    const uint32_t smem_base = ptx::smem_u32(smem);
+    const uint64_t desc0 = ptx::make_gmma_desc(0, 16, 8u * row_bytes, layout);     // everything but the address
+    float* stg = reinterpret_cast<float*>(smem + p.stg_smem_off) + (size_t)cg * 64 * kConvStg;
+    const int ksub = p.kc / 16;
+    int s = 0;
+    uint32_t ph = 0;
+    const int tiles_xy = p.tiles_x * p.tiles_y;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        float acc[NT / 2];
+#pragma unroll
+        for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+        int prev = -1;
+        for (int ks = 0; ks < ksteps; ++ks) {
+            ptx::mbar_wait(&full[s], ph);
+            const uint32_t st = smem_base + (uint32_t)s * (uint32_t)stage_bytes;
+            const uint64_t ad = desc0 | (uint64_t)(((st + (uint32_t)(cg * 64 * row_bytes)) & 0x3FFFFu) >> 4);
+            const uint64_t bd = desc0 | (uint64_t)(((st + (uint32_t)a_bytes) & 0x3FFFFu) >> 4);
+            ptx::wgmma_fence();
+            for (int k = 0; k < ksub; ++k)                  // +32 bytes along K inside the swizzle atom
+                ptx::wgmma_bf16<NT, 0, 0>(acc, ad + 2u * k, bd + 2u * k, 1u);
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<1>();                          // the previous stage's MMAs are done: release it
+            if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty[prev]);
+            prev = s;
+            if (++s == p.stages) { s = 0; ph ^= 1u; }
         }
-        int sb = 0;
-        uint32_t bph = 0;
-        const uint32_t bring_base = ptx::smem_u32(bring0);
-        for (; tile < total_tiles; tile += gridDim.x, ++tile_it) {
-            ELD_WAIT(&tmem_empty[acc], acc_ph ^ 1u, pw0);
-            ptx::tc_fence_after();
-            const uint32_t d_tmem = tmem_base + acc * (uint32_t)p.n_tile;
-            const uint32_t acc_cur = acc;
-            if (++acc == (uint32_t)p.acc_stages) { acc = 0; acc_ph ^= 1u; }
-            if (p.halo == 3) {
-                const uint64_t a_hi64 = ptx::make_smem_desc(0, 16, 10u * row_bytes, layout);
-                const uint32_t a_hi32 = (uint32_t)(a_hi64 >> 32), b_hi32 = (uint32_t)(desc_hi >> 32);
-                const uint32_t b_ring_lo = (uint32_t)desc_hi | ((bring_base & 0x3FFFFu) >> 4);
-                const uint32_t b_stage_step = (uint32_t)p.b_group * b_step;
-                for (int ks = 0; ks < ksteps; ++ks) {                 // ks = channel chunk
-                    ELD_WAIT(&full[s], ph, pw1);
-                    const uint32_t a_lo = (uint32_t)a_hi64 | ((a_addr & 0x3FFFFu) >> 4);
-                    const bool last = ks == ksteps - 1;
-                    const uint32_t flag0 = ks != 0 ? 1u : 0u;
-                    // one iteration per weight-ring stage; the taps of a stage are issued from a fully unrolled body
-#define ELD_H3_STAGE(KSUB_, BG_, T0_, LAST_)                                                                       \
-                    {                                                                                                  \
-                        ELD_WAIT(&bfull[sb], bph, pw1);                                                                \
-                        ptx::tc_fence_after();                                                                         \
-                        if (ptx::elect_one()) {                                                                        \
-                            if (!(p.dbg & 16))                                                                         \
-                                issue_halo3_group<KSUB_, BG_, T0_>(d_tmem, a_lo, a_hi32, b_ring_lo + (uint32_t)sb * b_stage_step, \
-                                                                   b_hi32, b_step, idesc, flag0);                     \
-                            ptx::umma_commit(&bempty[sb]);                                                             \
-                            if (LAST_) {                                                                               \
-                                ptx::umma_commit(&empty[s]);                                                           \
-                                if (last) ptx::umma_commit(&tmem_full[acc_cur]);                                       \
-                            }                                                                                          \
-                        }                                                                                              \
-                        __syncwarp();                                                                                  \
-                        if (++sb == p.b_stages) { sb = 0; bph ^= 1u; }                                                 \
-                    }
-                    if (p.b_group == 3) {
-                        if (ksub == 4) { ELD_H3_STAGE(4, 3, 0, false) ELD_H3_STAGE(4, 3, 3, false) ELD_H3_STAGE(4, 3, 6, true) }
-                        else           { ELD_H3_STAGE(2, 3, 0, false) ELD_H3_STAGE(2, 3, 3, false) ELD_H3_STAGE(2, 3, 6, true) }
-                    } else {
-                        if (ksub == 4) {
-                            ELD_H3_STAGE(4, 1, 0, false) ELD_H3_STAGE(4, 1, 1, false) ELD_H3_STAGE(4, 1, 2, false)
-                            ELD_H3_STAGE(4, 1, 3, false) ELD_H3_STAGE(4, 1, 4, false) ELD_H3_STAGE(4, 1, 5, false)
-                            ELD_H3_STAGE(4, 1, 6, false) ELD_H3_STAGE(4, 1, 7, false) ELD_H3_STAGE(4, 1, 8, true)
-                        } else {
-                            ELD_H3_STAGE(2, 1, 0, false) ELD_H3_STAGE(2, 1, 1, false) ELD_H3_STAGE(2, 1, 2, false)
-                            ELD_H3_STAGE(2, 1, 3, false) ELD_H3_STAGE(2, 1, 4, false) ELD_H3_STAGE(2, 1, 5, false)
-                            ELD_H3_STAGE(2, 1, 6, false) ELD_H3_STAGE(2, 1, 7, false) ELD_H3_STAGE(2, 1, 8, true)
-                        }
-                    }
-#undef ELD_H3_STAGE
-                    a_addr += (uint32_t)stage_bytes;
-                    if (++s == p.stages) { s = 0; ph ^= 1u; a_addr = stage_base; }
-                }
-                continue;
-            }
-            for (int ks = 0; ks < ksteps; ++ks) {
-                ELD_WAIT(&full[s], ph, pw1);
-                ptx::tc_fence_after();
-                const bool leader = ptx::elect_one();
-                if (leader && p.halo == 2) {
-                    // ks = channel chunk; 9 taps, each a shifted view of the same halo tile
-                    const uint64_t a_hi64 = ptx::make_smem_desc(0, 16, 10u * row_bytes, layout);
-                    const uint32_t a_lo = (uint32_t)a_hi64 | ((a_addr & 0x3FFFFu) >> 4);
-                    const uint32_t b_lo = (uint32_t)desc_hi | (((bres_base + (uint32_t)ks * (uint32_t)b_bytes) & 0x3FFFFu) >> 4);
-                    const uint32_t b_tap_step = (uint32_t)kchunks * b_step;
-                    if (p.dbg & 16) { }
-                    else if (ksub == 2) issue_halo2<2>(d_tmem, a_lo, (uint32_t)(a_hi64 >> 32), b_lo, (uint32_t)(desc_hi >> 32), b_tap_step, idesc, ks == 0);
-                    else           issue_halo2<4>(d_tmem, a_lo, (uint32_t)(a_hi64 >> 32), b_lo, (uint32_t)(desc_hi >> 32), b_tap_step, idesc, ks == 0);
-                    ptx::umma_commit(&empty[s]);
-                    if (ks == ksteps - 1) ptx::umma_commit(&tmem_full[acc_cur]);
-                } else if (leader) {
-                    uint64_t ad0 = desc_hi | (uint64_t)((a_addr & 0x3FFFFu) >> 4);
-                    uint64_t bd0;
-                    uint32_t b_sub_step;                       // descriptor units between the B tiles of taps kh, kh+1
-                    if (p.b_res) {
-                        // halo: ks = kw*kchunks + chunk, tap = kh*3 + kw -> tile index (kh*3+kw)*kchunks + chunk
-                        int j;
-                        if (p.halo) { const int kw = ks / kchunks; j = kw * kchunks + (ks - kw * kchunks); b_sub_step = 3u * kchunks * b_step; }
-                        else { j = ks; b_sub_step = 0; }
-                        bd0 = desc_hi | (uint64_t)(((bres_base + (uint32_t)j * (uint32_t)b_bytes) & 0x3FFFFu) >> 4);
-                    } else {
-                        bd0 = desc_hi | (uint64_t)(((a_addr + (uint32_t)a_bytes) & 0x3FFFFu) >> 4);
-                        b_sub_step = b_step;
-                    }
-                    for (int sub = 0; sub < nsub; ++sub) {
-                        uint64_t ad = ad0, bd = bd0;
-                        for (int k = 0; k < ksub; ++k) {
-                            ptx::umma_bf16(d_tmem, ad, bd, idesc, (ks | sub | k) != 0 ? 1u : 0u);
-                            ad += 2; bd += 2;                   // +32 bytes along K inside the swizzle atom
-                        }
-                        ad0 += a_tap_step; bd0 += b_sub_step;
-                    }
-                    ptx::umma_commit(&empty[s]);
-                    if (ks == ksteps - 1) ptx::umma_commit(&tmem_full[acc_cur]);
-                }
-                __syncwarp();
-                a_addr += (uint32_t)stage_bytes;
-                if (++s == p.stages) { s = 0; ph ^= 1u; a_addr = stage_base; }
-            }
-        }
-    } else {
-        // ===================== epilogue: group 0 = warps 2..5 (even tiles), group 1 = warps 6..9 (odd tiles) =====
-        // Two warps per scheduler cannot hide ALU latency, so the per-tile instruction count IS the epilogue's
-        // speed (measured: the old ~650-instruction body bounded every N = 32 layer).  No divisions (tile
-        // coordinates advance incrementally), bias from shared memory, LeakyReLU' from the sign bit.
-        const uint32_t egroup = (uint32_t)(warp - 2) >> 2;
-        const int q = warp & 3;                // TMEM lane quarter this warp may read
-        const int m = q * 32 + lane;           // pixel inside the patch
-        const int py = p.tile_w == 8 ? (m >> 3) : (m >> 4), px = m & (p.tile_w - 1);
-        // decomposition of this group's first tile and of its stride (2 * gridDim.x) into (n_t, tx, ty, img) digits
-        int t0 = (int)blockIdx.x + (int)egroup * (int)gridDim.x;
-        int n_t = t0 % n_tiles; t0 /= n_tiles;
-        int tx = t0 % p.tiles_x; t0 /= p.tiles_x;
-        int ty = t0 % p.tiles_y;
-        int img = t0 / p.tiles_y;
-        int g0 = 2 * (int)gridDim.x;
-        const int d_nt = g0 % n_tiles; g0 /= n_tiles;
-        const int d_tx = g0 % p.tiles_x; g0 /= p.tiles_x;
-        const int d_ty = g0 % p.tiles_y;
-        const int d_img = g0 / p.tiles_y;
-        uint32_t acc = egroup, acc_ph = 0;     // acc_stages is even: this group's accumulators are acc = egroup, +2, ...
-        const int tile_hh = 128 / p.tile_w;
-        const float4* sb4 = reinterpret_cast<const float4*>(s_bias);
-        for (int tile = (int)blockIdx.x + (int)egroup * (int)gridDim.x; tile < total_tiles; tile += 2 * (int)gridDim.x) {
-            const int x = tx * p.tile_w + px, y = ty * tile_hh + py;
-            const bool in_img = x < p.W && y < p.H;          // partial tiles at the right / bottom image border
-            const int pix = (img * p.H + y) * p.W + x;
-            const int col0 = n_t * p.n_tile;
-            const uint32_t t_addr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * (uint32_t)p.n_tile;
-            // the first chunk's sign word is requested before the wait for the accumulator: its DRAM latency hides there
-            uint32_t sg_first = 0;
-            if (p.aux_sign && in_img) sg_first = __ldg(p.aux_sign + (size_t)pix * (size_t)(p.n_total >> 5) + (size_t)(col0 >> 5));
-            ELD_WAIT(&tmem_full[acc], acc_ph, pw0);
-            ptx::tc_fence_after();
-            for (int c32 = 0; c32 < p.n_tile; c32 += 32) {
-                uint32_t r[32];
-                ptx::tmem_ld32(t_addr + c32, r);
-                const int col = col0 + c32;                   // first GEMM column of this chunk
-                __nv_bfloat16* dst;
-                int bcol;
-                if (p.epi_mode == EPI_STORE) {
-                    dst = (p.out_split && col >= p.out_split) ? p.out2 + (size_t)pix * p.out2_pitch + (col - p.out_split)
-                                                              : p.out + (size_t)pix * p.out_pitch + (p.out_c0 + col);
-                    bcol = col;
-                } else {
-                    const int sub = col >> p.cout_shift, co = col & (p.cout - 1);   // sub = kh*2 + kw
-                    const int oy = 2 * y + (sub >> 1), ox = 2 * x + (sub & 1);
-                    dst = p.out + ((size_t)(img * 2 * p.H + oy) * (2 * p.W) + ox) * p.out_pitch + p.out_c0 + co;
-                    bcol = co;
-                }
-                uint32_t mk[16];
-                uint32_t sgw = sg_first;
-                if (p.act == ACT_MASK && in_img) {
-                    if (p.aux_sign) {
-                        if (c32) sgw = __ldg(p.aux_sign + (size_t)pix * (size_t)(p.n_total >> 5) + (size_t)(col >> 5));
-                    } else {
-                        const __nv_bfloat16* ap = p.aux + (size_t)pix * p.aux_pitch + (p.aux_c0 + col);
-                        ptx::ld_global_nc_v8(ap, mk);
-                        ptx::ld_global_nc_v8(ap + 16, mk + 8);
-                    }
-                }
-                ptx::tmem_ld_wait();
+        ptx::wgmma_wait<0>();
+        ptx::reg_fence(acc);
+        if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty[prev]);
+
+        // ---- epilogue: 64 columns per pass through shared memory; thread t -> pixel t % 64, columns 32 (t / 64) ----
+        const int m_tile = tile / n_tiles, n_t = tile - m_tile * n_tiles;
+        const int img = m_tile / tiles_xy;
+        const int rem = m_tile - img * tiles_xy;
+        const int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
+        const int m = cg * 64 + (t & 63);                  // pixel inside the 8 x 16 tile
+        const int x = tx * kConvTileW + (m & 15), y = ty * 8 + (m >> 4);
+        const int wq = t >> 5, r0 = 16 * wq + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+        for (int pass = 0; pass < (NT + 63) / 64; ++pass) {
+            ptx::bar_sync(1 + cg, 128);                    // the previous pass / tile is done reading the staging rows
+#pragma unroll
+            for (int j = 0; j < 8 && 8 * pass + j < NT / 8; ++j)
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+                    *reinterpret_cast<float2*>(stg + (r0 + 8 * i) * kConvStg + 8 * j + c0) =
+                        make_float2(acc[4 * (8 * pass + j) + 2 * i], acc[4 * (8 * pass + j) + 2 * i + 1]);
+            ptx::bar_sync(1 + cg, 128);
+            const int half = t >> 6;
+            if (64 * pass + 32 * half < NT) {               // whole warps take part (the pool shuffles)
                 float v[32];
+                const float4* src = reinterpret_cast<const float4*>(stg + (t & 63) * kConvStg + 32 * half);
 #pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-                if (p.bias && !(p.dbg & 2)) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float4 b = sb4[(bcol >> 2) + j];
-                        v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
-                    }
+                for (int j = 0; j < 8; ++j) {
+                    const float4 q = src[j];
+                    v[4 * j] = q.x; v[4 * j + 1] = q.y; v[4 * j + 2] = q.z; v[4 * j + 3] = q.w;
                 }
-                if (p.act == ACT_LRELU) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.2f * v[j]);
-                } else if (p.act == ACT_MASK && in_img && p.aux_sign) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        // slope = 0.6 + 0.4 * (+-1) = 1 or 0.2
-                        const float s_lo = __uint_as_float(((sgw << (31 - j)) & 0x80000000u) | 0x3F800000u);
-                        const float s_hi = __uint_as_float(((sgw << (15 - j)) & 0x80000000u) | 0x3F800000u);
-                        v[2 * j] *= __fmaf_rn(s_lo, 0.4f, 0.6f);
-                        v[2 * j + 1] *= __fmaf_rn(s_hi, 0.4f, 0.6f);
-                    }
-                } else if (p.act == ACT_MASK && in_img) {
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        const uint32_t aw[4] = { mk[4 * g], mk[4 * g + 1], mk[4 * g + 2], mk[4 * g + 3] };
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            // LeakyReLU keeps the sign: slope = 0.6 + 0.4 * sign(activation) = 1 or 0.2
-                            // (activation == +0 counts as positive; the reference's tie is a measure-zero event)
-                            const float s_lo = __uint_as_float(((aw[j] << 16) & 0x80000000u) | 0x3F800000u);
-                            const float s_hi = __uint_as_float((aw[j] & 0x80000000u) | 0x3F800000u);
-                            v[g * 8 + 2 * j] *= __fmaf_rn(s_lo, 0.4f, 0.6f);
-                            v[g * 8 + 2 * j + 1] *= __fmaf_rn(s_hi, 0.4f, 0.6f);
-                        }
-                    }
-                }
-                // round once; the pool below works on the rounded (= stored) values
-                uint32_t wv[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-                    wv[j] = *reinterpret_cast<const uint32_t*>(&h);
-                }
-                if (p.sign_out && in_img) {
-                    // sign words of the stored activation: all a later LeakyReLU' needs (1/16 of the tensor)
-                    const uint32_t sg = ptx::gather_msb16(wv);
-                    p.sign_out[(size_t)pix * (size_t)(p.n_total >> 5) + (size_t)(col >> 5)] = sg;
-                }
-                if (p.pool_out) {
-                    // MaxPool2d(2) (Unet.py:13,51-63) fused: the 2x2 window of pixel (x, y) lives in lanes ^1 (x) and ^tile_w (y)
-                    // of this warp; packed bf16x2 max of the stored values.  H, W and the tile origin are even: a window is
-                    // wholly in or out.
-                    uint32_t pw[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const uint32_t a = bf2_max(wv[j], __shfl_xor_sync(0xffffffffu, wv[j], 1));
-                        pw[j] = bf2_max(a, __shfl_xor_sync(0xffffffffu, a, p.tile_w));
-                    }
-                    const bool origin = in_img && !((x | y) & 1);
-                    const size_t ppix = (size_t)(img * (p.H >> 1) + (y >> 1)) * (p.W >> 1) + (x >> 1);
-                    if (origin) {
-                        __nv_bfloat16* q4 = p.pool_out + ppix * p.pool_pitch + col;
-                        ptx::st_global_v8(q4, pw);
-                        ptx::st_global_v8(q4 + 16, pw + 8);
-                    }
-                    if (p.pool_code) {
-                        // per lane two 32-bit masks over its 32 channels: "is not the window's maximum" and "is negative"
-                        // (channel 2j -> bit j, channel 2j+1 -> bit 16+j); the window's origin lane collects the four lanes'
-                        // masks in the order the backward walks the window: (0,0) (0,1) (1,0) (1,1)
-                        uint32_t ne[16];
-#pragma unroll
-                        for (int j = 0; j < 16; ++j)
-                            ne[j] = __hne2_mask(*reinterpret_cast<const __nv_bfloat162*>(&wv[j]), *reinterpret_cast<const __nv_bfloat162*>(&pw[j]));
-                        const uint32_t nm = ptx::gather_msb16(ne), sg = ptx::gather_msb16(wv);
-                        uint32_t code[8];
-                        code[0] = nm; code[4] = sg;
-                        code[1] = __shfl_xor_sync(0xffffffffu, nm, 1);          code[5] = __shfl_xor_sync(0xffffffffu, sg, 1);
-                        code[2] = __shfl_xor_sync(0xffffffffu, nm, p.tile_w);   code[6] = __shfl_xor_sync(0xffffffffu, sg, p.tile_w);
-                        code[3] = __shfl_xor_sync(0xffffffffu, nm, p.tile_w | 1); code[7] = __shfl_xor_sync(0xffffffffu, sg, p.tile_w | 1);
-                        if (origin) ptx::st_global_v8(p.pool_code + (ppix * (size_t)(p.pool_pitch >> 5) + (size_t)(col >> 5)) * 8, code);
-                    }
-                }
-                if (!in_img || (p.dbg & 1)) continue;
-                // 64 bytes per pixel = two full 32-byte sectors, one 256-bit store each (four 16-byte stores sent four
-                // half-sector requests: 3.85 -> 3.70 ms per step).  Swapping halves between lane pairs so that one
-                // instruction covers a pixel's whole 64 bytes was measured too: no further gain (3.707 vs 3.713 ms).
-                ptx::st_global_v8(dst, wv);
-                ptx::st_global_v8(dst + 16, wv + 8);
+                conv_epilogue32(p, s_bias, v, img, x, y, n_t * NT + 64 * pass + 32 * half);
             }
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&tmem_empty[acc]);
-            acc += 2;
-            if (acc >= (uint32_t)p.acc_stages) { acc -= (uint32_t)p.acc_stages; acc_ph ^= 1u; }
-            // next tile of this group: add the stride digit-wise with carries
-            n_t += d_nt;
-            int cy = 0;
-            if (n_t >= n_tiles) { n_t -= n_tiles; cy = 1; }
-            tx += d_tx + cy; cy = 0;
-            if (tx >= p.tiles_x) { tx -= p.tiles_x; cy = 1; }
-            ty += d_ty + cy; cy = 0;
-            if (ty >= p.tiles_y) { ty -= p.tiles_y; cy = 1; }
-            img += d_img + cy;
         }
     }
-    if (PROF && lane == 0 && (warp <= 2 || warp == 6)) {
-        // slots: 0-2 producer (total, wait empty, wait bempty) | 3-5 MMA (total, wait tmem_empty, wait full) |
-        //        6-7 epilogue group 0 (total, wait tmem_full) | 8-9 epilogue group 1
-        const int base = warp == 0 ? 0 : warp == 1 ? 3 : warp == 2 ? 6 : 8;
-        long long* o = p.prof + (size_t)blockIdx.x * 16 + base;
-        o[0] = clock64() - pt0; o[1] = pw0;
-        if (warp <= 1) o[2] = pw1;
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) ptx::tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
 }
 
 }  // namespace eld

@@ -1,22 +1,17 @@
-// first_conv.cuh - conv1_1 (4 -> 32 channels, 3x3, Unet.py:11) fprop and wgrad as tcgen05 tiles fed by a SOFTWARE im2col.
+// first_conv.cuh - conv1_1 (4 -> 32 channels, 3x3, Unet.py:11) fprop and wgrad as wgmma tiles fed by a SOFTWARE im2col.
 //
-// The generic conv tile needs >= 32 input channels (one 64-byte TMA row per pixel), so round 1 ran conv1_1 on a
-// zero-padded 32-channel copy of the input: a 134 MB pack pass, 18 MMAs per 128-pixel tile of which 7/8 multiplied
-// zeros, and the same again for the weight gradient (216 us of a 4.1 ms step for 0.6 % of its FLOPs).  Here four
-// builder warps read the fp32 NCHW frame directly (16 B per pixel) and write the im2col tile
+// The generic conv tile needs >= 32 input channels (one 64-byte TMA row per pixel); conv1_1 has 4.  Instead of a
+// zero-padded 32-channel copy of the input (a pack pass, and 7/8 of the MMAs multiplying zeros), one thread per pixel
+// reads the fp32 NCHW frame (from a TMA-loaded halo patch in shared memory) and writes the im2col tile
 //     A[128 pixels][k = tap*4 + c  (36 real, k = 36 is a column of ones, the rest zero)]       bf16, 128-byte rows, SW128
 // into shared memory; that ONE tile is
-//     fprop : the K-major A operand   D[128 px][32 co]  = A[px][k] * W[co][k]            3 MMAs (K = 48) per tile
-//     wgrad : the MN-major A operand  D[k][32 co]      += A[px][k] * dZ[px][co]          8 MMAs (K = 128 pixels) per tile
-// (the ones column makes row 36 of the wgrad accumulator the bias gradient).  No padded copy, no pack pass.
-// The raw frame reaches the builders through a TMA ring of halo patches (zero-filled outside the image = the conv
-// padding): the first version loaded its 36 taps straight from global memory and every tile paid a DRAM round trip
-// (164 us); with the patches 8 tiles ahead the builders only read shared memory.  The fp32 planes are described to TMA
-// as bf16 PAIRS with the same geometry the other tiles use (128-byte rows, SWIZZLE_128B) - a {20 x 10 x 4} fp32 box
-// with SWIZZLE_NONE encodes fine but the copy instruction is rejected as illegal on B200 (measured) - so a patch is
-// [4 planes][10 rows][32 floats] with the 16-byte chunks of row r XOR-ed by (r & 7); the builders undo that.  The box
-// starts at column x0 - 4, not x0 - 1: the innermost start of a TMA box must be 16-byte aligned in global memory (a
-// start at x0 - 1 was the actual cause of the illegal-instruction fault; compute-sanitizer pinned it to UTMALDG).
+//     fprop : the K-major A operand   D[128 px][32 co]  = A[px][k] * W[co][k]            2 x 3 wgmma (K = 48) per tile
+//     wgrad : the MN-major A operand  D[k][32 co]      += A[px][k] * dZ[px][co]          8 wgmma (K = 128 pixels) per tile
+// (the ones column makes row 36 of the wgrad accumulator the bias gradient).
+// The fp32 planes are described to TMA as bf16 PAIRS with the same geometry the other tiles use (128-byte rows,
+// SWIZZLE_128B), so a patch is [4 planes][10 rows][32 floats] with the 16-byte chunks of row r XOR-ed by (r & 7); the
+// builders undo that.  The box starts at column x0 - 4, not x0 - 1: the innermost start of a TMA box must be 16-byte
+// aligned in global memory.
 #pragma once
 #include "umma.cuh"
 #include <cuda_bf16.h>
@@ -36,33 +31,17 @@ struct FirstConvParams {
                                 // LeakyReLU' mask conv1_2's data gradient needs (conv_umma.cuh aux_sign)
     float* dw;                  // wgrad: f32 OIHW [32][4][3][3], accumulated into
     float* db;                  // wgrad: f32 [32]
-    int stages;
-    int epi_groups;             // fprop: 1 or 2 epilogue groups (alternate tiles)
-    int groups;                 // wgrad: builder groups taking alternate tiles (1..2, or 3 with the joint producer)
-    int split_prod;             // wgrad: the dZ tiles have a TMA producer of their own (warp 8)
-    long long* prof;            // PROF instantiations only (ELD_FC_PROF): per-role totals and barrier waits, 16 slots per CTA
 };
 
-// A builder group (4 warps, one pixel per thread) needs ~1000 cycles per tile (36 shared-memory loads, packing, six
-// swizzled stores and - the long pole - a fence.proxy.async before it may signal the tensor core), all of it latency:
-// one group alone bounded the kernels at 70 us.  kFcGroups groups take alternate tiles, so that many are in flight.
-constexpr int kFcGroups = 2;
-constexpr int kFcBuilderWarps = 4 * kFcGroups;
-constexpr int kFcThreads = 32 * (kFcBuilderWarps + 6);   // + MMA issuer, 4 epilogue warps (fprop), TMA producer
-// fprop only: a second epilogue group (4 more warps) takes the odd tiles.  One warp per scheduler runs a tile's ~200
-// dependent instructions (tcgen05.ld, bias, LeakyReLU, pack, two 256-bit stores, sign word) in ~1000 cycles: with one
-// group that chain, not the builders or the MMAs, set the kernel's pace.
-constexpr int kFcThreadsFprop = kFcThreads + 128;
+// Two warpgroups per CTA take alternate tiles; inside a warpgroup one thread per pixel builds the im2col row, one
+// thread issues the TMA loads of the halo patches (and, for the wgrad, the dZ tiles) kFcRing tiles ahead, and the
+// warpgroup's wgmma consumes the tile.  While one warpgroup builds, the other's MMAs and epilogue run.
+constexpr int kFcThreads = 256;
 constexpr int kFcRaw = 4 * 10 * 128;      // bytes of one raw patch: [4 planes][10 rows][32 floats], SW128-swizzled rows
-constexpr int kFcRawStages = 8;
-constexpr int kFcATile = 128 * 128;  // bytes
-constexpr int kFcAcc = 4;            // fprop TMEM accumulator ring (4 x 32 columns)
-
-#define FC_WAIT(bar, par, ctr)                                                                     \
-    do {                                                                                           \
-        if (PROF) { const long long t_ = clock64(); ptx::mbar_wait((bar), (par)); (ctr) += clock64() - t_; } \
-        else ptx::mbar_wait((bar), (par));                                                         \
-    } while (0)
+constexpr int kFcQTile = 128 * 64;        // wgrad dZ tile: 128 pixel rows x 32 channels bf16 (SW64)
+constexpr int kFcRing = 4;                // patch ring depth per warpgroup
+constexpr int kFcATile = 128 * 128;       // bytes of one im2col tile
+constexpr int kFcStg = 36;                // fprop: floats per staged pixel row (32 columns + 4)
 
 __device__ __forceinline__ uint32_t fc_pack(float a, float b)
 {
@@ -106,347 +85,159 @@ __device__ __forceinline__ void fc_tile_coords(const FirstConvParams& p, int til
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// fprop: a1_1 = lrelu(conv1_1(x) + b)
+// WGRAD = false: a1_1 = lrelu(conv1_1(x) + b)
+// WGRAD = true : dW[co][c][tap] += sum_px dZ[px][co] * x[px + tap][c] ; db[co] += sum_px dZ[px][co]
 // ---------------------------------------------------------------------------------------------------------------------
-template <bool PROF>
-__global__ void __launch_bounds__(kFcThreadsFprop, 1)
-first_conv_fprop_kernel(const __grid_constant__ CUtensorMap tmX, const FirstConvParams p)
+template <bool WGRAD>
+__global__ void __launch_bounds__(kFcThreads, 1)
+first_conv_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmQ, const FirstConvParams p)
 {
-    long long w0 = 0, w1 = 0, t0 = 0;
-    if (PROF) t0 = clock64();
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = ptx::smem_u32(smem_raw);
     uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
-    uint8_t* w_s = smem;                                   // 4 KB weights
-    uint8_t* a_s = smem + 4096;                            // ring of A tiles
-    uint8_t* r_s = a_s + (size_t)p.stages * kFcATile;      // ring of raw halo patches
-    uint64_t* full = reinterpret_cast<uint64_t*>(r_s + ((kFcRawStages * kFcRaw + 1023) & ~1023));
-    uint64_t* empty = full + 8;
-    uint64_t* raw_full = empty + 8;
-    uint64_t* raw_empty = raw_full + kFcRawStages;
-    uint64_t* tmem_full = raw_empty + kFcRawStages;
-    uint64_t* tmem_empty = tmem_full + kFcAcc;
-    uint64_t* w_full = tmem_empty + kFcAcc;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(w_full + 1);
-    float* s_bias = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + 512);    // 16-byte aligned (float4 reads)
+    // per warpgroup: [A tile 16 KB][ring of kFcRing slots: raw patch 5 KB (+ dZ tile 8 KB)][fprop: staging 18 KB]
+    constexpr int slot_bytes = kFcRaw + (WGRAD ? kFcQTile : 0);
+    constexpr int stg_bytes = WGRAD ? 0 : ((128 * kFcStg * 4 + 1023) & ~1023);
+    constexpr int wg_bytes = kFcATile + kFcRing * slot_bytes + stg_bytes;
+    uint8_t* w_s = smem;                                   // fprop: 4 KB weights
+    const int wg = threadIdx.x >> 7, m = threadIdx.x & 127, lane = threadIdx.x & 31, wq = m >> 5;
+    uint8_t* my = smem + 4096 + (size_t)wg * wg_bytes;
+    uint8_t* a_s = my;
+    uint8_t* ring = my + kFcATile;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 4096 + 2 * wg_bytes);
+    uint64_t* w_full = bars;
+    uint64_t* slot_full = bars + 1 + wg * kFcRing;
+    float* s_bias = reinterpret_cast<float*>(bars + 1 + 2 * kFcRing + 1);      // 16-byte aligned (float4 reads)
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int total_tiles = p.n_img * p.tiles_x * p.tiles_y;
+    const int my_tiles = (int)blockIdx.x < total_tiles ? (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
+    const int n_mine = my_tiles > wg ? (my_tiles - wg + 1) / 2 : 0;     // this warpgroup's tiles: wg, wg + 2, ...
     if (threadIdx.x == 0) {
         ptx::prefetch_tmap(&tmX);
-        for (int s = 0; s < p.stages; ++s) { ptx::mbar_init(&full[s], 128); ptx::mbar_init(&empty[s], 1); }
-        for (int s = 0; s < kFcRawStages; ++s) { ptx::mbar_init(&raw_full[s], 1); ptx::mbar_init(&raw_empty[s], 128); }
-        for (int a = 0; a < kFcAcc; ++a) { ptx::mbar_init(&tmem_full[a], 1); ptx::mbar_init(&tmem_empty[a], 4); }
+        if (WGRAD) ptx::prefetch_tmap(&tmQ);
         ptx::mbar_init(w_full, 1);
+        for (int s = 0; s < 2 * kFcRing; ++s) ptx::mbar_init(&bars[1 + s], 1);
         ptx::fence_barrier_init();
     }
-    if (warp == kFcBuilderWarps + 1) ptx::tmem_alloc(tmem_slot, 128);
-    if (threadIdx.x < 32) s_bias[threadIdx.x] = __ldg(p.bias + threadIdx.x);
-    ptx::tc_fence_before();
+    if (!WGRAD && threadIdx.x < 32) s_bias[threadIdx.x] = __ldg(p.bias + threadIdx.x);
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    ptx::grid_dep_wait();          // PDL: x (noise kernel) and the packed weights (pack kernel) are complete past this point
+    ptx::grid_dep_wait();          // PDL: x (noise kernel), dZ and the packed weights are complete past this point
     ptx::grid_dep_launch();
 
-    const int my_tiles = (int)blockIdx.x < total_tiles ? (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
-    if (warp < kFcBuilderWarps) {
-        // ===================== im2col builders: group g builds this CTA's tiles g, g + kFcGroups, ... =====================
-        const int g = warp >> 2, m = threadIdx.x & 127, py = m >> 4, px = m & 15;
-        for (int i = g; i < my_tiles; i += kFcGroups) {
-            const int s = i % p.stages, rs = i % kFcRawStages;
-            const uint32_t ph = (uint32_t)(i / p.stages) & 1u, rph = (uint32_t)(i / kFcRawStages) & 1u;
-            FC_WAIT(&raw_full[rs], rph, w0);
-            FC_WAIT(&empty[s], ph ^ 1u, w1);
-            fc_build_row(reinterpret_cast<const float*>(r_s + (size_t)rs * kFcRaw), a_s + (size_t)s * kFcATile, m, py, px);
-            ptx::mbar_arrive(&raw_empty[rs]);              // this thread's patch reads are done (values are in the A tile)
-            ptx::fence_proxy_async();                      // generic-proxy stores -> visible to the tensor core's async proxy
-            ptx::mbar_arrive(&full[s]);
-        }
-    } else if (warp == kFcBuilderWarps) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
+    auto issue = [&](int i) {      // TMA loads of this warpgroup's i-th tile into ring slot i % kFcRing
+        int img, y0, x0;
+        fc_tile_coords(p, (int)blockIdx.x + (wg + 2 * i) * (int)gridDim.x, img, y0, x0);
+        uint8_t* slot = ring + (size_t)(i % kFcRing) * slot_bytes;
+        uint64_t* bar = &slot_full[i % kFcRing];
+        ptx::mbar_arrive_expect_tx(bar, (uint32_t)slot_bytes);
+        ptx::tma_load_5d(slot, &tmX, bar, 2 * (x0 - 4), y0 - 1, 0, img, 0);
+        if (WGRAD) ptx::tma_load_5d(slot + kFcRaw, &tmQ, bar, 0, x0, y0, img, 0);
+    };
+    if (m == 0) {
+        if (!WGRAD && wg == 0) {
             ptx::mbar_arrive_expect_tx(w_full, 4096u);
             ptx::bulk_load(w_s, p.w_img, 4096u, w_full);
         }
-        __syncwarp();
-        ptx::mbar_wait(w_full, 0);
-        const uint32_t idesc = ptx::make_idesc_bf16(128, 32, 0, 0);
-        const uint64_t desc_hi = ptx::make_smem_desc(0, 16, 1024, ptx::LAYOUT_SW128);
-        const uint32_t hi = (uint32_t)(desc_hi >> 32);
-        const uint32_t b_lo = (uint32_t)desc_hi | ((ptx::smem_u32(w_s) & 0x3FFFFu) >> 4);
-        const uint32_t a_base = ptx::smem_u32(a_s);
-        int s = 0;
-        uint32_t ph = 0, acc = 0, acc_ph = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            FC_WAIT(&tmem_empty[acc], acc_ph ^ 1u, w0);
-            FC_WAIT(&full[s], ph, w1);
-            ptx::tc_fence_after();
-            if (ptx::elect_one()) {
-                const uint32_t a_lo = (uint32_t)desc_hi | (((a_base + (uint32_t)s * kFcATile) & 0x3FFFFu) >> 4);
-                const uint32_t d = tmem_base + acc * 32u;
-                ptx::umma_bf16_lohi(d, a_lo, hi, b_lo, hi, idesc, false);
-                ptx::umma_bf16_lohi(d, a_lo + 2u, hi, b_lo + 2u, hi, idesc, true);
-                ptx::umma_bf16_lohi(d, a_lo + 4u, hi, b_lo + 4u, hi, idesc, true);
-                ptx::umma_commit(&empty[s]);
-                ptx::umma_commit(&tmem_full[acc]);
+        for (int i = 0; i < kFcRing && i < n_mine; ++i) issue(i);
+    }
+    if (!WGRAD) ptx::mbar_wait(w_full, 0);
+
+    const int py = m >> 4, px = m & 15;
+    const uint32_t a_addr = ptx::smem_u32(a_s);
+    float acc[2][16];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < 16; ++j) acc[h][j] = 0.f;
+    for (int i = 0; i < n_mine; ++i) {
+        const int rs = i % kFcRing;
+        const uint8_t* slot = ring + (size_t)rs * slot_bytes;
+        ptx::mbar_wait(&slot_full[rs], (uint32_t)(i / kFcRing) & 1u);
+        fc_build_row(reinterpret_cast<const float*>(slot), a_s, m, py, px);
+        ptx::fence_proxy_async();                      // generic-proxy stores -> visible to wgmma's operand reads
+        ptx::bar_sync(1 + wg, 128);
+        if (!WGRAD) {
+            // D[px][co] for pixel rows 0-63 and 64-127: K-major A and W, SBO = 8 rows of 128 B
+            if (m == 0 && i + kFcRing < n_mine) issue(i + kFcRing);     // the patch is consumed (it is in the A tile)
+            const uint64_t dsc = ptx::make_gmma_desc(0, 16, 1024, ptx::GMMA_SW128);
+            const uint64_t bd = dsc | (uint64_t)((ptx::smem_u32(w_s) & 0x3FFFFu) >> 4);
+            ptx::wgmma_fence();
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const uint64_t ad = dsc | (uint64_t)(((a_addr + 8192u * h) & 0x3FFFFu) >> 4);
+#pragma unroll
+                for (int k = 0; k < 3; ++k) ptx::wgmma_bf16<32, 0, 0>(acc[h], ad + 2u * k, bd + 2u * k, k != 0 ? 1u : 0u);
             }
-            __syncwarp();
-            if (++s == p.stages) { s = 0; ph ^= 1u; }
-            if (++acc == kFcAcc) { acc = 0; acc_ph ^= 1u; }
-        }
-    } else if (warp == kFcBuilderWarps + 5) {
-        // ===================== TMA producer of the raw halo patches =====================
-        if (lane == 0) {
-            int rs = 0;
-            uint32_t rph = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                int img, y0, x0;
-                fc_tile_coords(p, tile, img, y0, x0);
-                FC_WAIT(&raw_empty[rs], rph ^ 1u, w0);
-                ptx::mbar_arrive_expect_tx(&raw_full[rs], (uint32_t)kFcRaw);
-                ptx::tma_load_5d(r_s + (size_t)rs * kFcRaw, &tmX, &raw_full[rs], 2 * (x0 - 4), y0 - 1, 0, img, 0);
-                if (++rs == kFcRawStages) { rs = 0; rph ^= 1u; }
-            }
-        }
-    } else {
-        // ===================== epilogue: bias + LeakyReLU -> bf16 NHWC =====================
-        const int q = warp & 3;                            // TMEM lane quarter of this warp
-        const int m = q * 32 + lane, py = m >> 4, px = m & 15;
-        const float4* sb4 = reinterpret_cast<const float4*>(s_bias);
-        const int eg = warp > kFcBuilderWarps + 5 ? 1 : 0;  // warps +1..+4 = group 0, +6..+9 = group 1
-        for (int i = eg < p.epi_groups ? eg : my_tiles; i < my_tiles; i += p.epi_groups) {
-            const uint32_t acc = (uint32_t)i % kFcAcc, acc_ph = ((uint32_t)i / kFcAcc) & 1u;
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<0>();
+            ptx::reg_fence(acc[0]);
+            ptx::reg_fence(acc[1]);
+            // ---- epilogue: fragments -> staging -> one pixel x 32 channels per thread: bias + LeakyReLU -> bf16 NHWC ----
+            float* stg = reinterpret_cast<float*>(my + kFcATile + kFcRing * slot_bytes);
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+#pragma unroll
+                    for (int r = 0; r < 2; ++r)
+                        *reinterpret_cast<float2*>(stg + (64 * h + 16 * wq + (lane >> 2) + 8 * r) * kFcStg + 8 * j + 2 * (lane & 3)) =
+                            make_float2(acc[h][4 * j + 2 * r], acc[h][4 * j + 2 * r + 1]);
+            ptx::bar_sync(1 + wg, 128);
             int img, y0, x0;
-            fc_tile_coords(p, (int)blockIdx.x + i * (int)gridDim.x, img, y0, x0);
-            FC_WAIT(&tmem_full[acc], acc_ph, w0);
-            ptx::tc_fence_after();
-            uint32_t r[32];
-            ptx::tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + acc * 32u, r);
-            ptx::tmem_ld_wait();
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&tmem_empty[acc]);
-            __nv_bfloat16* dst = p.out + ((size_t)(img * p.H + y0 + py) * p.W + (x0 + px)) * p.out_pitch;
+            fc_tile_coords(p, (int)blockIdx.x + (wg + 2 * i) * (int)gridDim.x, img, y0, x0);
+            const float4* row = reinterpret_cast<const float4*>(stg + m * kFcStg);
+            const float4* sb4 = reinterpret_cast<const float4*>(s_bias);
             uint32_t wv[16];
 #pragma unroll
             for (int g = 0; g < 4; ++g) {
-                const float4 b0 = sb4[2 * g], b1 = sb4[2 * g + 1];
-                float v[8] = { __uint_as_float(r[8 * g]) + b0.x, __uint_as_float(r[8 * g + 1]) + b0.y,
-                               __uint_as_float(r[8 * g + 2]) + b0.z, __uint_as_float(r[8 * g + 3]) + b0.w,
-                               __uint_as_float(r[8 * g + 4]) + b1.x, __uint_as_float(r[8 * g + 5]) + b1.y,
-                               __uint_as_float(r[8 * g + 6]) + b1.z, __uint_as_float(r[8 * g + 7]) + b1.w };
+                const float4 a0 = row[2 * g], a1 = row[2 * g + 1], b0 = sb4[2 * g], b1 = sb4[2 * g + 1];
+                float v[8] = { a0.x + b0.x, a0.y + b0.y, a0.z + b0.z, a0.w + b0.w, a1.x + b1.x, a1.y + b1.y, a1.z + b1.z, a1.w + b1.w };
 #pragma unroll
                 for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.2f * v[j]);
                 wv[4 * g] = fc_pack(v[0], v[1]); wv[4 * g + 1] = fc_pack(v[2], v[3]);
                 wv[4 * g + 2] = fc_pack(v[4], v[5]); wv[4 * g + 3] = fc_pack(v[6], v[7]);
             }
-            ptx::st_global_v8(dst, wv);                    // 64 bytes = two full sectors, two 256-bit stores
-            ptx::st_global_v8(dst + 16, wv + 8);
-            if (p.sign_out) {
-                const uint32_t sg = ptx::gather_msb16(wv);
-                p.sign_out[(size_t)(img * p.H + y0 + py) * p.W + (x0 + px)] = sg;
-            }
-        }
-    }
-    if (PROF && lane == 0) {
-        // slots: 0-2 builders 0 (total, wait raw_full, wait empty) | 3-5 builders 1 | 6-8 MMA (total, wait tmem_empty, wait full)
-        //        9-10 producer (total, wait raw_empty) | 11-12 epilogue 0 (total, wait tmem_full) | 13-14 epilogue 1
-        const int base = warp == 0 ? 0 : warp == 4 ? 3 : warp == kFcBuilderWarps ? 6 : warp == kFcBuilderWarps + 5 ? 9
-                       : warp == kFcBuilderWarps + 1 ? 11 : warp == kFcBuilderWarps + 6 ? 13 : -1;
-        if (base >= 0) {
-            long long* o = p.prof + (size_t)blockIdx.x * 16 + base;
-            o[0] = clock64() - t0; o[1] = w0;
-            if (base <= 6) o[2] = w1;
-        }
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == kFcBuilderWarps + 1) ptx::tmem_dealloc(tmem_base, 128);
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// wgrad: dW[co][c][tap] += sum_px dZ[px][co] * x[px + tap][c] ; db[co] += sum_px dZ[px][co]
-// ---------------------------------------------------------------------------------------------------------------------
-constexpr int kFcQTile = 128 * 64;   // dZ tile: 128 pixel rows x 32 channels bf16 (SW64)
-// wgrad roles inside the same 14 warps: builders = warps [0, 4 * groups) with groups <= 3 (it has no per-tile epilogue, so the
-// four warps the fprop uses for one can build), MMA issuer = warp 12, TMA producer (+ TMEM allocation) = warp 13
-constexpr int kWgMmaWarp = 12, kWgProdWarp = 13, kWgDzWarp = 8;     // warp 8 builds when groups == 3 (joint producer only)
-static_assert(kFcThreads == 32 * 14, "wgrad role map assumes 14 warps");
-
-template <bool PROF>
-__global__ void __launch_bounds__(kFcThreads, 1)
-first_conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmQ, const FirstConvParams p)
-{
-    long long w0 = 0, w1 = 0, t0 = 0;
-    if (PROF) t0 = clock64();
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t raw = ptx::smem_u32(smem_raw);
-    uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
-    // stage = [A tile 16 KB][dZ tile 8 KB]; one spare A-sized block behind the ring keeps the (ignored) second M block
-    // of the last stage inside the allocation
-    const int stage_bytes = kFcATile + kFcQTile;
-    uint8_t* ring = smem;
-    uint8_t* r_s = ring + (size_t)p.stages * stage_bytes + kFcATile;
-    uint64_t* full_a = reinterpret_cast<uint64_t*>(r_s + ((kFcRawStages * kFcRaw + 1023) & ~1023));
-    uint64_t* full_q = full_a + 8;
-    uint64_t* empty = full_q + 8;
-    uint64_t* raw_full = empty + 8;
-    uint64_t* raw_empty = raw_full + kFcRawStages;
-    uint64_t* acc_full = raw_empty + kFcRawStages;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int total_tiles = p.n_img * p.tiles_x * p.tiles_y;
-    const int my_tiles = (int)blockIdx.x < total_tiles ? (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
-    if (threadIdx.x == 0) {
-        ptx::prefetch_tmap(&tmQ);
-        ptx::prefetch_tmap(&tmX);
-        for (int s = 0; s < p.stages; ++s) { ptx::mbar_init(&full_a[s], 128); ptx::mbar_init(&full_q[s], 1); ptx::mbar_init(&empty[s], 1); }
-        for (int s = 0; s < kFcRawStages; ++s) { ptx::mbar_init(&raw_full[s], 1); ptx::mbar_init(&raw_empty[s], 128); }
-        ptx::mbar_init(acc_full, 1);
-        ptx::fence_barrier_init();
-    }
-    if (warp == kWgProdWarp) ptx::tmem_alloc(tmem_slot, 32);
-    ptx::tc_fence_before();
-    __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    ptx::grid_dep_wait();
-    ptx::grid_dep_launch();
-
-    if (warp < 4 * p.groups) {
-        const int g = warp >> 2, m = threadIdx.x & 127, py = m >> 4, px = m & 15;
-        for (int i = g; i < my_tiles; i += p.groups) {
-            const int s = i % p.stages, rs = i % kFcRawStages;
-            const uint32_t ph = (uint32_t)(i / p.stages) & 1u, rph = (uint32_t)(i / kFcRawStages) & 1u;
-            FC_WAIT(&raw_full[rs], rph, w0);
-            FC_WAIT(&empty[s], ph ^ 1u, w1);
-            fc_build_row(reinterpret_cast<const float*>(r_s + (size_t)rs * kFcRaw), ring + (size_t)s * stage_bytes, m, py, px);
-            ptx::mbar_arrive(&raw_empty[rs]);
-            ptx::fence_proxy_async();
-            ptx::mbar_arrive(&full_a[s]);
-        }
-        // ===================== epilogue (after the last tile): rows 0..35 = dW, row 36 = db =====================
-        if (my_tiles > 0 && warp < 2) {
-            ptx::mbar_wait(acc_full, 0);
-            ptx::tc_fence_after();
-            uint32_t r[32];
-            ptx::tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16), r);
-            ptx::tmem_ld_wait();
-            const int k = warp * 32 + lane;
-            if (k < 36) {
-                const int tap = k >> 2, c = k & 3;
-                if (c < p.cin) {
+            const size_t pix = (size_t)(img * p.H + y0 + py) * p.W + (x0 + px);
+            __nv_bfloat16* dst = p.out + pix * p.out_pitch;
+            ptx::st_global_32B(dst, wv);                   // 64 bytes = two full sectors
+            ptx::st_global_32B(dst + 16, wv + 8);
+            if (p.sign_out) p.sign_out[pix] = ptx::gather_msb16(wv);
+            // the next tile's staging writes come after its build barrier: every thread has read its row by then
+        } else {
+            // D[k][co] += A^T (MN-major, k = 64 slots per 128-byte row) * dZ (MN-major, 32 co per 64-byte row);
+            // K = 128 pixels per tile: +2048 B in A and +1024 B in dZ per 16 pixel rows
+            const uint64_t ad0 = ptx::make_gmma_desc(a_addr, 8192, 1024, ptx::GMMA_SW128);
+            const uint64_t bd0 = ptx::make_gmma_desc(ptx::smem_u32(slot + kFcRaw), 4096, 512, ptx::GMMA_SW64);
+            ptx::wgmma_fence();
 #pragma unroll
-                    for (int co = 0; co < 32; ++co) atomicAdd(p.dw + (co * p.cin + c) * 9 + tap, __uint_as_float(r[co]));
+            for (int k = 0; k < 8; ++k) ptx::wgmma_bf16<32, 1, 1>(acc[0], ad0 + 128u * k, bd0 + 64u * k, 1u);
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<0>();
+            ptx::bar_sync(1 + wg, 128);                    // every warp's MMAs are done with the A tile and the dZ tile
+            if (m == 0 && i + kFcRing < n_mine) issue(i + kFcRing);
+        }
+    }
+    if (WGRAD && n_mine > 0) {
+        // ===================== epilogue: rows 0..35 = dW, row 36 = db =====================
+        ptx::reg_fence(acc[0]);
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const int k = 16 * wq + (lane >> 2) + 8 * r;
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int c2 = 0; c2 < 2; ++c2) {
+                    const int co = 8 * j + 2 * (lane & 3) + c2;
+                    const float v = acc[0][4 * j + 2 * r + c2];
+                    if (k < 36) {
+                        const int tap = k >> 2, c = k & 3;
+                        if (c < p.cin) atomicAdd(p.dw + (co * p.cin + c) * 9 + tap, v);
+                    } else if (k == 36) {
+                        atomicAdd(p.db + co, v);
+                    }
                 }
-            } else if (k == 36) {
-#pragma unroll
-                for (int co = 0; co < 32; ++co) atomicAdd(p.db + co, __uint_as_float(r[co]));
-            }
-        }
-    } else if (warp == kWgMmaWarp) {
-        // ===================== MMA issuer: D[k][co] += A^T (MN-major) * dZ (MN-major), K = 128 pixels per tile ==========
-        const uint32_t idesc = ptx::make_idesc_bf16(128, 32, 1, 1);
-        // A: 64 k-slots = one 128-byte M block per pixel row, 8-row groups 1024 B apart; M = 128 reads a second block
-        // LBO bytes further on (the next stage's tile - finite or not, rows 64..127 of D are never read)
-        const uint64_t a_desc = ptx::make_smem_desc(0, (uint32_t)stage_bytes, 1024, ptx::LAYOUT_SW128);
-        const uint64_t b_desc = ptx::make_smem_desc(0, (uint32_t)kFcQTile, 512, ptx::LAYOUT_SW64);
-        const uint32_t a_hi = (uint32_t)(a_desc >> 32), b_hi = (uint32_t)(b_desc >> 32);
-        const uint32_t base = ptx::smem_u32(ring);
-        int s = 0;
-        uint32_t ph = 0;
-        for (int i = 0; i < my_tiles; ++i) {
-            FC_WAIT(&full_a[s], ph, w0);
-            FC_WAIT(&full_q[s], ph, w1);
-            ptx::tc_fence_after();
-            if (ptx::elect_one()) {
-                const uint32_t st = base + (uint32_t)s * (uint32_t)stage_bytes;
-                const uint32_t a_lo = (uint32_t)a_desc | ((st & 0x3FFFFu) >> 4);
-                const uint32_t b_lo = (uint32_t)b_desc | (((st + kFcATile) & 0x3FFFFu) >> 4);
-#pragma unroll
-                for (int k = 0; k < 8; ++k)                 // 16 pixel rows per MMA: +2048 B in A, +1024 B in dZ
-                    ptx::umma_bf16(tmem_base, ((uint64_t)a_hi << 32) | (a_lo + 128u * k), ((uint64_t)b_hi << 32) | (b_lo + 64u * k),
-                                   idesc, (i | k) != 0 ? 1u : 0u);
-                ptx::umma_commit(&empty[s]);
-                if (i == my_tiles - 1) ptx::umma_commit(acc_full);
-            }
-            __syncwarp();
-            if (++s == p.stages) { s = 0; ph ^= 1u; }
-        }
-    } else if (warp == kWgProdWarp && p.split_prod) {
-        // ===================== TMA producer of the raw halo patches (its own warp: see below) =====================
-        if (lane == 0) {
-            int rs = 0;
-            uint32_t rph = 0;
-            for (int i = 0; i < my_tiles; ++i) {
-                int img, y0, x0;
-                fc_tile_coords(p, (int)blockIdx.x + i * (int)gridDim.x, img, y0, x0);
-                FC_WAIT(&raw_empty[rs], rph ^ 1u, w0);
-                ptx::mbar_arrive_expect_tx(&raw_full[rs], (uint32_t)kFcRaw);
-                ptx::tma_load_5d(r_s + (size_t)rs * kFcRaw, &tmX, &raw_full[rs], 2 * (x0 - 4), y0 - 1, 0, img, 0);
-                if (++rs == kFcRawStages) { rs = 0; rph ^= 1u; }
-            }
-        }
-    } else if (warp == kWgDzWarp && p.split_prod) {
-        // ===================== TMA producer of the dZ tiles =====================
-        // One thread used to feed both rings.  The in-kernel profile showed the convoy: blocked on a raw-ring slot (which
-        // the builders free only after they got an A stage, i.e. after the MMAs advanced) it did not issue the dZ tile the
-        // MMAs were waiting for - the issuer spent 44 % of the kernel waiting for dZ, the builders 45 % for patches.
-        if (lane == 0) {
-            int s = 0;
-            uint32_t ph = 0;
-            for (int i = 0; i < my_tiles; ++i) {
-                int img, y0, x0;
-                fc_tile_coords(p, (int)blockIdx.x + i * (int)gridDim.x, img, y0, x0);
-                FC_WAIT(&empty[s], ph ^ 1u, w1);
-                ptx::mbar_arrive_expect_tx(&full_q[s], (uint32_t)kFcQTile);
-                ptx::tma_load_5d(ring + (size_t)s * stage_bytes + kFcATile, &tmQ, &full_q[s], 0, x0, y0, img, 0);
-                if (++s == p.stages) { s = 0; ph ^= 1u; }
-            }
-        }
-    } else if (warp == kWgProdWarp) {
-        // ===================== one TMA producer for both rings (ELD_FC_WGRAD_JOINT=1: the A/B arm) =====================
-        if (lane == 0) {
-            int s = 0, rs = 0;
-            uint32_t ph = 0, rph = 0;
-            // the raw ring is deeper than the A / dZ ring: run it `lead` tiles ahead so a blocked dZ slot never starves it
-            const int lead = kFcRawStages - 1;
-            int t_raw = blockIdx.x, n_raw = 0;
-            auto issue_raw = [&]() {
-                int img, y0, x0;
-                fc_tile_coords(p, t_raw, img, y0, x0);
-                FC_WAIT(&raw_empty[rs], rph ^ 1u, w0);
-                ptx::mbar_arrive_expect_tx(&raw_full[rs], (uint32_t)kFcRaw);
-                ptx::tma_load_5d(r_s + (size_t)rs * kFcRaw, &tmX, &raw_full[rs], 2 * (x0 - 4), y0 - 1, 0, img, 0);
-                if (++rs == kFcRawStages) { rs = 0; rph ^= 1u; }
-                t_raw += gridDim.x; ++n_raw;
-            };
-            for (int i = 0; i < my_tiles; ++i) {
-                while (n_raw < my_tiles && n_raw <= i + lead - 1) issue_raw();
-                int img, y0, x0;
-                fc_tile_coords(p, (int)blockIdx.x + i * (int)gridDim.x, img, y0, x0);
-                FC_WAIT(&empty[s], ph ^ 1u, w1);
-                ptx::mbar_arrive_expect_tx(&full_q[s], (uint32_t)kFcQTile);
-                ptx::tma_load_5d(ring + (size_t)s * stage_bytes + kFcATile, &tmQ, &full_q[s], 0, x0, y0, img, 0);
-                if (++s == p.stages) { s = 0; ph ^= 1u; }
-            }
         }
     }
-    if (PROF && lane == 0) {
-        // slots: 0-2 builders 0 (total incl. the final epilogue, wait raw_full, wait empty) | 3-5 builders 1
-        //        6-8 MMA (total, wait full_a, wait full_q) | 9-11 producer (total, wait raw_empty, wait empty) | 12-14 dZ producer
-        const int base = warp == 0 ? 0 : warp == 4 ? 3 : warp == kWgMmaWarp ? 6 : warp == kWgProdWarp ? 9
-                       : (warp == kWgDzWarp && p.split_prod) ? 12 : -1;
-        if (base >= 0) {
-            long long* o = p.prof + (size_t)blockIdx.x * 16 + base;
-            o[0] = clock64() - t0; o[1] = w0; o[2] = w1;
-        }
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == kWgProdWarp) ptx::tmem_dealloc(tmem_base, 32);
 }
 
 }  // namespace eld

@@ -1,5 +1,5 @@
-// umma.cuh - inline-PTX wrappers for the Blackwell (sm_100a) async machinery used by the U-Net
-// tiles: mbarrier, TMA (cp.async.bulk.tensor), TMEM allocation, tcgen05.mma / commit / ld.
+// umma.cuh - inline-PTX wrappers for the Hopper (sm_90a) async machinery used by the U-Net tiles:
+// mbarrier, TMA (cp.async.bulk.tensor), programmatic dependent launch and warpgroup MMA (wgmma).
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -19,6 +19,7 @@ __device__ __forceinline__ void fence_barrier_init()
 {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
+// generic-proxy shared-memory stores -> visible to the async proxy (TMA, wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async()
 {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -46,19 +47,16 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity)
     while (!mbar_try_wait(bar, parity)) { }
 }
 
-// one lane of a CONVERGED warp (elect.sync): unlike `lane == 0`, ptxas knows a single thread is active and
-// issues the tcgen05 / TMA instruction straight from uniform registers (no per-instruction waterfall loop)
-__device__ __forceinline__ bool elect_one()
+// named barrier over `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void bar_sync(uint32_t id, uint32_t count)
 {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xFFFFFFFF;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // ---- programmatic dependent launch (PDL) -----------------------------------------------------------------
 // grid_dep_wait(): block until every grid this launch depends on has completed and flushed (no-op for a normal launch).
 // grid_dep_launch(): let the next kernel in the stream start launching (its CTAs become resident as ours retire and
-// run their prologue - barrier init, TMEM alloc, bias / resident-weight loads - before blocking in grid_dep_wait()).
+// run their prologue - barrier init, bias loads - before blocking in grid_dep_wait()).
 __device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
@@ -66,12 +64,6 @@ __device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m)
 {
     asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
 __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uint64_t* bar,
                                             int c0, int c1, int c2, int c3, int c4)
@@ -88,114 +80,87 @@ __device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t b
                  ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
-// L2 prefetch of a tensor box (no smem destination, no barrier)
-__device__ __forceinline__ void tma_prefetch_5d(const CUtensorMap* m, int c0, int c1, int c2, int c3, int c4)
+// ---- 32-byte global accesses (two 128-bit instructions; 32-byte aligned) ----------------------------------------
+// An epilogue thread owns 64 contiguous bytes of its pixel: it writes them as two full 32-byte sectors.
+__device__ __forceinline__ void st_global_32B(void* p, const uint32_t w[8])
 {
-    asm volatile("cp.async.bulk.prefetch.tensor.5d.L2.global [%0, {%1, %2, %3, %4, %5}];"
-                 ::"l"(m), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-
-// ---- TMEM -----------------------------------------------------------------------------------------
-// one full warp; writes the allocated base address (lane 0, column base) to *dst_smem
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols)
-{
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ---- MMA ------------------------------------------------------------------------------------------
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 inputs, f32 accumulate, issued by ONE thread
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// same, descriptors given as (lo, hi) 32-bit halves; `accumulate` is a compile-time-friendly flag
-__device__ __forceinline__ void umma_bf16_lohi(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                               uint32_t idesc, bool accumulate)
-{
-    if (accumulate) {
-        asm volatile(
-            "{\n\t.reg .b64 da, db;\n\t.reg .pred p;\n\t"
-            "mov.b64 da, {%1, %2};\n\tmov.b64 db, {%3, %4};\n\t"
-            "setp.eq.b32 p, 0, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-            ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc) : "memory");
-    } else {
-        asm volatile(
-            "{\n\t.reg .b64 da, db;\n\t.reg .pred p;\n\t"
-            "mov.b64 da, {%1, %2};\n\tmov.b64 db, {%3, %4};\n\t"
-            "setp.ne.b32 p, 0, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-            ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc) : "memory");
-    }
-}
-// arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// 32 lanes x 32 consecutive 32-bit columns: thread t of the warp receives lane (base_lane + t)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t r[32])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---- 256-bit global accesses (sm_100: STG.E.ENL2.256 / LDG.E.ENL2.256; 32-byte aligned) ------------------------------
-// An epilogue thread owns 64 contiguous bytes of its pixel: two of these write two FULL 32-byte sectors each, where
-// four 16-byte stores sent four half-sector requests to L2.
-__device__ __forceinline__ void st_global_v8(void* p, const uint32_t w[8])
-{
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
+    asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};\n\tst.global.v4.b32 [%0+16], {%5,%6,%7,%8};"
                  :: "l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
 }
-__device__ __forceinline__ void ld_global_nc_v8(const void* p, uint32_t w[8])
+__device__ __forceinline__ void ld_global_nc_32B(const void* p, uint32_t w[8])
 {
-    asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%8];\n\tld.global.nc.v4.b32 {%4,%5,%6,%7}, [%8+16];"
                  : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(p));
 }
 
-// ---- descriptors ----------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [49,52) base_offset |
-//   [61,64) layout: 0 none, 2 SW128, 4 SW64, 6 SW32
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout)
+// ---- wgmma ----------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor (sm_90 GMMA layout):
+//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [49,52) base_offset | [62,64) layout: 0 none, 1 SW128, 2 SW64, 3 SW32
+// K-major swizzled operand: SBO = 8 rows * row bytes, LBO unused.  MN-major swizzled operand (rows = K, the MN extent
+// contiguous inside a row): LBO = distance between swizzle atoms along MN, SBO = distance between 8-row groups along K.
+__device__ __forceinline__ uint64_t make_gmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout)
 {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)(layout & 7u) << 61;
+    d |= (uint64_t)(layout & 3u) << 62;
     return d;
 }
-constexpr uint32_t LAYOUT_SW128 = 2, LAYOUT_SW64 = 4, LAYOUT_SW32 = 6;
+constexpr uint32_t GMMA_SW128 = 1, GMMA_SW64 = 2;
+// swizzle mode of a TMA box / packed weight block whose rows are `row_bytes` (64 or 128) long
+__host__ __device__ constexpr uint32_t gmma_layout(int row_bytes) { return row_bytes == 128 ? GMMA_SW128 : GMMA_SW64; }
 
-// Instruction descriptor (cute::UMMA::InstrDescriptor): f32 accumulate, bf16 A and B.
-//   [4,6) c_format=1 (F32) | [7,10) a_format=1 (BF16) | [10,13) b_format=1 | [15] a_major | [16] b_major
-//   (0 = K-major, 1 = MN-major) | [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major, uint32_t b_mn_major)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulator registers must not be touched by ordinary instructions while a wgmma that writes them is in flight
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R])
 {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] (f32, registers of one warpgroup) (+)= A[64 x 16] * B[16 x N], bf16 operands from shared-memory descriptors.
+// TA / TB: 0 = K-major, 1 = MN-major.  scale_d == 0 overwrites D.
+// Fragment layout: warp w, lane l holds d[4j + 2i + c] = D[16w + l/4 + 8i][8j + 2(l%4) + c].
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB) : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB) : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB) : "memory");
+}
+
+// N selected at compile time: N in {32, 64, 128}
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d)
+{
+    if constexpr (N == 32) wgmma_m64n32k16<TA, TB>(d, a_desc, b_desc, scale_d);
+    else if constexpr (N == 64) wgmma_m64n64k16<TA, TB>(d, a_desc, b_desc, scale_d);
+    else wgmma_m64n128k16<TA, TB>(d, a_desc, b_desc, scale_d);
 }
 
 // bits 15 / 31 of 16 packed bf16x2 words gathered into one word: word j's low half -> bit j, high half -> bit 16 + j

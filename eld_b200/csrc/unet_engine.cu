@@ -1,5 +1,5 @@
 // unet_engine.cu - the UNetSeeInDark training / inference step as a fixed launch sequence over the
-// tcgen05 tiles (unet_prims.cu) and the HBM-bound helpers (unet_ew.cu).
+// wgmma tiles (unet_prims.cu) and the HBM-bound helpers (unet_ew.cu).
 //
 // Reference: models/arch/Unet.py:48-91 (forward), models/ELD_model.py:411-420,469-475 (L1 loss,
 // backward, Adam).  Activations NHWC bf16; torch.cat (Unet.py:69,74,79,84) is free: the deconv and
@@ -616,10 +616,10 @@ struct Runner {
     int finish_bucket(int k, float* g) const
     {
         // Single-GPU steps (no bucket events) move all conv gradients with ONE launch at the end: a permute launch over a
-        // few dozen tiles is latency-bound (~15 us whatever its size), four of them cost 61 us against 27 us for one.
+        // few dozen tiles is latency-bound whatever its size, so four of them cost more than one.
         // Data-parallel steps (bucket events on): the bucket's conv gradients move to the PyTorch layout right here, on
         // the compute stream, then an event marks the bucket final.  (Running this permute on the caller's communication
-        // stream instead was measured at 2 GPUs: +0.10 ms per step - any foreign kernel that overlaps the persistent
+        // stream instead would let it overlap the tiles - any foreign kernel that overlaps the persistent
         // one-CTA-per-SM tiles delays some of their CTAs, and a tile kernel is as slow as its slowest CTA.)
         const bool per_bucket = u->bucket_ev[0] != nullptr;
         if (!per_bucket && k != kGradBuckets - 1) return ELD_OK;

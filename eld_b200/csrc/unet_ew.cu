@@ -53,8 +53,7 @@ maxpool_kernel(const __nv_bfloat16* __restrict__ in, int in_pitch, int in_c0, __
 //   dskip : gradient that reached A through the skip connection (d_cat buffer, same pitch/offset)
 //   dP    : gradient of the pooled tensor (compact)
 // PyTorch's max_pool2d backward routes to the FIRST maximum in window scan order; so do we.
-// 16 channels (32 bytes) per thread and 256-bit accesses: half as many, twice as wide memory requests as the 16-byte
-// version (the same change took 150 us out of the conv epilogues) - C % 16 == 0, 32-byte aligned tensors.
+// 16 channels (32 bytes) per thread, moved as whole 32-byte sectors - C % 16 == 0, 32-byte aligned tensors.
 __global__ void __launch_bounds__(256)
 maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ A, const __nv_bfloat16* __restrict__ dskip, int a_pitch, int a_c0,
                    int s_pitch, int s_c0, const __nv_bfloat16* __restrict__ dP, __nv_bfloat16* __restrict__ dZ, int C, int n_img, int Ho, int Wo)
@@ -72,10 +71,10 @@ maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ A, const __nv_bfloat16* __r
         uint32_t a[4][8], s[4][8], dp[8];
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-            ptx::ld_global_nc_v8(A + offs[k] * a_pitch + a_c0 + gch * 16, a[k]);
-            ptx::ld_global_nc_v8(dskip + offs[k] * s_pitch + s_c0 + gch * 16, s[k]);
+            ptx::ld_global_nc_32B(A + offs[k] * a_pitch + a_c0 + gch * 16, a[k]);
+            ptx::ld_global_nc_32B(dskip + offs[k] * s_pitch + s_c0 + gch * 16, s[k]);
         }
-        ptx::ld_global_nc_v8(dP + (((size_t)n * Ho + yo) * Wo + xo) * C + gch * 16, dp);
+        ptx::ld_global_nc_32B(dP + (((size_t)n * Ho + yo) * Wo + xo) * C + gch * 16, dp);
         uint32_t o[4][8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -101,7 +100,7 @@ maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ A, const __nv_bfloat16* __r
             }
         }
 #pragma unroll
-        for (int k = 0; k < 4; ++k) ptx::st_global_v8(dZ + offs[k] * C + gch * 16, o[k]);
+        for (int k = 0; k < 4; ++k) ptx::st_global_32B(dZ + offs[k] * C + gch * 16, o[k]);
     }
 }
 
@@ -125,10 +124,10 @@ maxpool_bwd_code_kernel(const uint32_t* __restrict__ code, const __nv_bfloat16* 
         const size_t pix00 = ((size_t)n * 2 * Ho + 2 * yo) * (2 * Wo) + 2 * xo;
         const size_t offs[4] = { pix00, pix00 + 1, pix00 + (size_t)2 * Wo, pix00 + (size_t)2 * Wo + 1 };
         uint32_t cw[8], s[4][8], dp[8];
-        ptx::ld_global_nc_v8(code + ((size_t)ppix * (groups >> 1) + (gch >> 1)) * 8, cw);
+        ptx::ld_global_nc_32B(code + ((size_t)ppix * (groups >> 1) + (gch >> 1)) * 8, cw);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) ptx::ld_global_nc_v8(dskip + offs[k] * s_pitch + s_c0 + gch * 16, s[k]);
-        ptx::ld_global_nc_v8(dP + (size_t)ppix * C + gch * 16, dp);
+        for (int k = 0; k < 4; ++k) ptx::ld_global_nc_32B(dskip + offs[k] * s_pitch + s_c0 + gch * 16, s[k]);
+        ptx::ld_global_nc_32B(dP + (size_t)ppix * C + gch * 16, dp);
         // this thread's 16 channels are pairs 8*(gch&1) .. +7 of the chunk: bring their bits to positions 0..7 / 16..23
         const uint32_t sh = (gch & 1u) * 8u;
         const uint32_t m0 = cw[0] >> sh, m1 = cw[1] >> sh, m2 = cw[2] >> sh;
@@ -148,7 +147,7 @@ maxpool_bwd_code_kernel(const uint32_t* __restrict__ code, const __nv_bfloat16* 
                 const __nv_bfloat162 h = __floats2bfloat162_rn((bf_lo(s[k][j]) + g_lo) * f_lo, (bf_hi(s[k][j]) + g_hi) * f_hi);
                 o[j] = *reinterpret_cast<const uint32_t*>(&h);
             }
-            ptx::st_global_v8(dZ + offs[k] * C + gch * 16, o);
+            ptx::st_global_32B(dZ + offs[k] * C + gch * 16, o);
         }
     }
 }
@@ -238,7 +237,7 @@ head_kernel(const __nv_bfloat16* __restrict__ a, const float* __restrict__ w, co
 {
     // cout = 4 (packed raw) or 3 (sRGB out): lane q >= cout of a pixel's four carries zero weights and writes nothing.
     // The kernel is HBM-LATENCY bound (160 B per pixel, ~150 instructions): one register-prefetched pixel per thread
-    // kept only ~13 KB per SM in flight (37 % of the bandwidth-delay product).  Every thread now streams ITS OWN 16 bytes
+    // keeps too few bytes per SM in flight to cover the bandwidth-delay product.  Every thread streams ITS OWN 16 bytes
     // of the pixel and ITS OWN target value through a private slot of a kHeadStages-deep cp.async ring - 7 pixels ahead,
     // no registers, and no block barrier because a thread only ever reads what it copied itself.
     __shared__ uint4 ring_a[kHeadStages][kHeadThreads];

@@ -1,12 +1,10 @@
-// unet_prims.cu - host side of the tcgen05 conv/deconv tiles: TMA tensor-map construction, launch
+// unet_prims.cu - host side of the wgmma conv/deconv tiles: TMA tensor-map construction, launch
 // geometry, weight packing, and the C-ABI primitives (include/eld_b200_unet.h).
 #include "common.cuh"
 #include <cstdlib>
 #include <cstdio>
-#include <vector>
 #include "conv_umma.cuh"
 #include "wgrad_umma.cuh"
-#include "wgrad_conv.cuh"
 #include "first_conv.cuh"
 #include "unet_prims.h"
 
@@ -41,7 +39,7 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
     ELD_REQUIRE(op.cin % 32 == 0, "conv tile: cin=%d must be a multiple of 32", op.cin);
     ELD_REQUIRE(op.n_total % 32 == 0, "conv tile: GEMM N=%d must be a multiple of 32", op.n_total);
     ELD_REQUIRE(op.a_pitch % 8 == 0, "conv tile: the input pitch must be a multiple of 8 channels");
-    // the epilogue moves 64 bytes per pixel with two 256-bit accesses: 32-byte aligned pixel rows and channel offsets
+    // the epilogue moves 64 bytes per pixel as two 32-byte sectors: 32-byte aligned pixel rows and channel offsets
     ELD_REQUIRE(op.out_pitch % 16 == 0 && op.out_c0 % 16 == 0 && (reinterpret_cast<uintptr_t>(op.out) & 31) == 0,
                 "conv tile: output pitch / first channel must be multiples of 16 channels and the tensor 32-byte aligned");
     ELD_REQUIRE(op.aux == nullptr || (op.aux_pitch % 16 == 0 && op.aux_c0 % 16 == 0 && (reinterpret_cast<uintptr_t>(op.aux) & 31) == 0),
@@ -50,12 +48,10 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
                 "conv tile: pooled-output pitch must be a multiple of 16 channels and the tensor 32-byte aligned");
     ConvGemmParams p{};
     p.n_img = op.n_img; p.H = op.H; p.W = op.W;
-    p.tiles_x = op.W / 16; p.tiles_y = op.H / 8;
+    p.tiles_x = (op.W + 15) / 16; p.tiles_y = (op.H + 7) / 8;
     p.taps = op.taps; p.a_mode = op.a_mode; p.cin = op.cin; p.a_c0 = op.a_c0;
     p.kc = (op.cin % 64 == 0) ? 64 : 32;
     p.n_total = op.n_total;
-    p.n_tile = op.n_total <= 256 ? op.n_total : 256;
-    ELD_REQUIRE(op.n_total % p.n_tile == 0, "conv tile: N=%d not divisible by tile %d", op.n_total, p.n_tile);
     p.epi_mode = op.epi_mode; p.act = op.act;
     p.out = static_cast<__nv_bfloat16*>(op.out); p.out_pitch = op.out_pitch; p.out_c0 = op.out_c0;
     p.bias = op.bias;
@@ -75,54 +71,27 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
                                      (reinterpret_cast<uintptr_t>(op.out2) & 31) == 0),
                 "conv tile: split store needs a plain store epilogue, a second tensor and a split at a multiple of 32 columns");
     p.out2 = static_cast<__nv_bfloat16*>(op.out2); p.out2_pitch = op.out2_pitch; p.out_split = op.out_split;
+    p.b_rows = op.n_total <= 256 ? op.n_total : 256;
+    // N per tile: 32, 64 or 128 (a 64 x 256 f32 accumulator would take 128 registers per consumer thread and spill
+    // next to the epilogue)
+    p.n_tile = (op.n_total % 128 == 0) ? 128 : (op.n_total % 64 == 0) ? 64 : 32;
     const int rb = p.kc * 2;
-    const int b_tile = p.n_tile * rb;
-    const int b_total = op.taps * (op.cin / p.kc) * b_tile;
-    const int budget = 200 * 1024;
-    p.b_res = (op.a_mode == A_CONV && op.taps == 9 && p.n_total == p.n_tile && b_total <= 80 * 1024) ? 1 : 0;
-    p.halo = (op.a_mode == A_CONV && op.taps == 9 && (p.b_res || (160 * rb + 3 * b_tile) <= 64 * 1024)) ? 1 : 0;
-    if (getenv("ELD_CONV_V1")) { p.b_res = 0; p.halo = 0; }       // debugging aid: the plain 9-box path
-    p.tile_w = 16;
-    p.bo_mode = 0;
-    // Full halo: measured on B200 - the UMMA descriptor's swizzle is a function of the ABSOLUTE smem address
-    // bits, so a K-major operand may start at any 16-byte-aligned pixel row of a TMA-written tile and its
-    // 8-row groups may be any stride apart (base_offset left 0; setting it to (start>>7)&7 gives wrong
-    // results).  One {kc,10,18} box then serves all nine taps.
-    if (p.b_res && !getenv("ELD_CONV_NOHALO2")) {
-        p.halo = 2; p.tile_w = 8;
-        p.bo_mode = getenv("ELD_CONV_BO") ? atoi(getenv("ELD_CONV_BO")) : 0;
-    }
-    // streamed weights + full-halo activations for every other conv3x3 (two rings)
-    p.b_stages = 0;
-    // one weight-ring stage = 3 taps for n_tile <= 128 (12 MMAs per barrier round trip), 1 tap for n_tile == 256
-    p.b_group = 1;
-    if (!p.b_res && op.a_mode == A_CONV && op.taps == 9 && p.n_tile >= 64 && !getenv("ELD_CONV_NOHALO3")) {
-        p.halo = 3; p.tile_w = 8;
-        p.b_group = p.n_tile <= 128 ? 3 : 1;
-    }
-    p.tiles_x = (op.W + p.tile_w - 1) / p.tile_w;
-    p.tiles_y = (op.H + (128 / p.tile_w) - 1) / (128 / p.tile_w);
-    const int stage_bytes = p.halo >= 2 ? ((180 * rb + 1023) & ~1023)
-                                        : (p.halo ? 160 : 128) * rb + (p.b_res ? 0 : (p.halo ? 3 : 1) * b_tile);
-    int stages = (budget - (p.b_res ? b_total : 0)) / stage_bytes;
-    if (p.halo == 3) {
-        stages = 3;                                              // activations: 3 x 23 KB (kc = 64)
-        int bs = (216 * 1024 - stages * stage_bytes) / (p.b_group * b_tile);   // weights: the rest
-        if (bs > 8) bs = 8;
-        if (bs < 2) { stages = 2; bs = (216 * 1024 - stages * stage_bytes) / (p.b_group * b_tile); }
-        ELD_REQUIRE(bs >= 2, "conv tile: weight ring does not fit (n_tile %d, kc %d)", p.n_tile, p.kc);
-        p.b_stages = bs;
-    }
+    const int stage_bytes = 128 * rb + p.n_tile * rb;
+    const int stg_bytes = 2 * 64 * kConvStg * 4;
+    const int n_bias = op.epi_mode == EPI_STORE ? op.n_total : op.cout;
+    ELD_REQUIRE(n_bias <= 1024, "conv tile: %d bias entries exceed the 4 KB shared-memory copy", n_bias);
+    int stages = (200 * 1024 - stg_bytes - 4096) / stage_bytes;
     if (stages > 8) stages = 8;
     if (stages < 2) stages = 2;
     p.stages = stages;
-    p.l2_prefetch = getenv("ELD_CONV_PREFETCH") ? atoi(getenv("ELD_CONV_PREFETCH")) : 0;
-    p.dbg = getenv("ELD_CONV_DBG") ? atoi(getenv("ELD_CONV_DBG")) : 0;
-    p.acc_stages = 512 / p.n_tile;
-    if (p.acc_stages > kMaxAccStages) p.acc_stages = kMaxAccStages;
-    int cols = 32;
-    while (cols < p.acc_stages * p.n_tile) cols *= 2;
-    p.tmem_cols = cols;
+    p.stg_smem_off = stages * stage_bytes;
+    p.bias_smem_off = p.stg_smem_off + stg_bytes;
+    p.bar_smem_off = p.bias_smem_off + 4096;
+    p.cout_shift = 0;
+    if (op.epi_mode == EPI_SHUFFLE) {
+        ELD_REQUIRE(op.cout > 0 && (op.cout & (op.cout - 1)) == 0, "deconv tile: cout=%d must be a power of two", op.cout);
+        while ((1 << p.cout_shift) < op.cout) ++p.cout_shift;
+    }
 
     CUtensorMap tmA;
     const cuuint64_t eb = 2;  // bf16
@@ -131,8 +100,7 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
         cuuint64_t str[4] = { op.a_pitch * eb, (cuuint64_t)op.W * op.a_pitch * eb,
                               (cuuint64_t)op.H * op.W * op.a_pitch * eb,
                               (cuuint64_t)op.n_img * op.H * op.W * op.a_pitch * eb };
-        cuuint32_t box[5] = { (cuuint32_t)p.kc, (cuuint32_t)(p.halo >= 2 ? 10 : 16),
-                              (cuuint32_t)(p.halo >= 2 ? 18 : (p.halo ? 10 : 8)), 1, 1 };
+        cuuint32_t box[5] = { (cuuint32_t)p.kc, 16, 8, 1, 1 };
         int rc = encode(ctx, &tmA, op.a, 5, dims, str, box, p.kc * 2);
         if (rc) return rc;
     } else {
@@ -145,45 +113,14 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
         if (rc) return rc;
     }
     p.b_ptr = static_cast<const uint8_t*>(op.b);
-    const size_t ring_bytes = (size_t)stages * stage_bytes + (p.b_res ? b_total : 0) + (size_t)p.b_stages * p.b_group * b_tile;
-    p.bias_smem_off = (int)ring_bytes + 768;                      // barriers (<= 53 x 8 B + slot) live in the first 768 B
-    const int n_bias = op.epi_mode == EPI_STORE ? op.n_total : op.cout;
-    ELD_REQUIRE(n_bias <= 1024, "conv tile: %d bias entries exceed the 4 KB shared-memory copy", n_bias);
-    p.cout_shift = 0;
-    if (op.epi_mode == EPI_SHUFFLE) {
-        ELD_REQUIRE(op.cout > 0 && (op.cout & (op.cout - 1)) == 0, "deconv tile: cout=%d must be a power of two", op.cout);
-        while ((1 << p.cout_shift) < op.cout) ++p.cout_shift;
-    }
-    const size_t smem = ring_bytes + 1024 /*align slack*/ + 768 /*barriers*/ + 4096 /*bias*/;
+    const size_t smem = 1024 /*align slack*/ + (size_t)p.bar_smem_off + 256 /*barriers*/;
     const int total_tiles = op.n_img * p.tiles_x * p.tiles_y * (p.n_total / p.n_tile);
     const int grid = total_tiles < ctx->num_sms ? total_tiles : ctx->num_sms;
-    if (getenv("ELD_CONV_PROF")) {          // debugging: per-role barrier-wait cycles of this launch, printed to stderr
-        long long* d = nullptr;
-        ELD_CHECK_CUDA(cudaMalloc(&d, (size_t)grid * 16 * sizeof(long long)));
-        ELD_CHECK_CUDA(cudaMemsetAsync(d, 0, (size_t)grid * 16 * sizeof(long long), st));
-        p.prof = d;
-        cudaEvent_t e0, e1;
-        cudaEventCreate(&e0); cudaEventCreate(&e1);
-        cudaEventRecord(e0, st);
-        conv_umma_kernel<true><<<grid, kConvThreads, smem, st>>>(tmA, p);
-        cudaEventRecord(e1, st);
-        ELD_CHECK_CUDA(cudaStreamSynchronize(st));
-        float ev_ms = 0.f;
-        cudaEventElapsedTime(&ev_ms, e0, e1);
-        cudaEventDestroy(e0); cudaEventDestroy(e1);
-        fprintf(stderr, "[conv prof] event time %.1f us | ", ev_ms * 1e3);
-        std::vector<long long> h((size_t)grid * 16);
-        ELD_CHECK_CUDA(cudaMemcpy(h.data(), d, h.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-        cudaFree(d);
-        double m[16] = { 0 };
-        for (int b = 0; b < grid; ++b) for (int k = 0; k < 16; ++k) m[k] += (double)h[(size_t)b * 16 + k] / grid;
-        fprintf(stderr, "[conv prof] cin %d taps %d N %d/%d HxW %dx%d halo %d tiles/cta %.1f | kclk: prod tot %.1f wE %.1f wBE %.1f | "
-                        "mma tot %.1f wTE %.1f wF %.1f | epi0 tot %.1f wTF %.1f | epi1 tot %.1f wTF %.1f\n",
-                op.cin, op.taps, p.n_tile, p.n_total, op.H, op.W, p.halo, (double)total_tiles / grid,
-                m[0] / 1e3, m[1] / 1e3, m[2] / 1e3, m[3] / 1e3, m[4] / 1e3, m[5] / 1e3, m[6] / 1e3, m[7] / 1e3, m[8] / 1e3, m[9] / 1e3);
-    } else {
-        ELD_CHECK_CUDA(launch_pdl(conv_umma_kernel<false>, grid, kConvThreads, smem, st, tmA, p));
-    }
+    cudaError_t e;
+    if (p.n_tile == 128) e = launch_pdl(conv_gemm_kernel<128>, grid, kConvThreads, smem, st, tmA, p);
+    else if (p.n_tile == 64) e = launch_pdl(conv_gemm_kernel<64>, grid, kConvThreads, smem, st, tmA, p);
+    else e = launch_pdl(conv_gemm_kernel<32>, grid, kConvThreads, smem, st, tmA, p);
+    ELD_CHECK_CUDA(e);
     ELD_CHECK_CUDA(cudaGetLastError());
     count_launch(ctx);
     return ELD_OK;
@@ -191,7 +128,7 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
 
 // the fp32 NCHW frame [n][4][H][W] as (x in HALF floats, y, plane, image) of bf16: box = 64 halves (32 floats, 128 B,
 // SWIZZLE_128B - the geometry every other tile uses) x 10 rows x 4 planes around an 8 x 16 pixel tile; out-of-image
-// elements are zero-filled = the conv padding (see first_conv.cuh for why not a plain fp32 box)
+// elements are zero-filled = the conv padding
 static int encode_frame(eld_ctx* ctx, CUtensorMap* map, const float* x, int cin, int n, int H, int W)
 {
     ELD_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "first conv tile: the input frame must be 16-byte aligned");
@@ -201,36 +138,16 @@ static int encode_frame(eld_ctx* ctx, CUtensorMap* map, const float* x, int cin,
     return encode(ctx, map, x, 5, dims, str, box, 128);
 }
 
-// conv1_1 (4 -> 32): software-im2col tcgen05 tiles on the fp32 NCHW frame (first_conv.cuh)
-// debugging (ELD_FC_PROF): per-role totals and barrier-wait cycles of one first-layer launch, printed to stderr
-template <typename Launch>
-static int fc_prof_launch(eld_ctx* ctx, const char* what, int grid, double tiles_per_cta, cudaStream_t st, FirstConvParams p, Launch launch)
+// shared memory of the first-layer tiles (first_conv.cuh): align slack, weights, two warpgroups' A tile + patch ring
+// (+ staging), barriers and bias
+static size_t first_conv_smem(bool wgrad)
 {
-    long long* d = nullptr;
-    ELD_CHECK_CUDA(cudaMalloc(&d, (size_t)grid * 16 * sizeof(long long)));
-    ELD_CHECK_CUDA(cudaMemsetAsync(d, 0, (size_t)grid * 16 * sizeof(long long), st));
-    p.prof = d;
-    cudaEvent_t e0, e1;
-    cudaEventCreate(&e0); cudaEventCreate(&e1);
-    cudaEventRecord(e0, st);
-    launch(p);
-    cudaEventRecord(e1, st);
-    ELD_CHECK_CUDA(cudaStreamSynchronize(st));
-    float ev_ms = 0.f;
-    cudaEventElapsedTime(&ev_ms, e0, e1);
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    std::vector<long long> h((size_t)grid * 16);
-    ELD_CHECK_CUDA(cudaMemcpy(h.data(), d, h.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-    cudaFree(d);
-    double m[16] = { 0 };
-    for (int b = 0; b < grid; ++b) for (int k = 0; k < 16; ++k) m[k] += (double)h[(size_t)b * 16 + k] / grid / 1e3;
-    fprintf(stderr, "[first conv prof] %s event time %.1f us tiles/cta %.1f stages %d | kclk: bld0 tot %.1f wRF %.1f wE %.1f | bld1 tot %.1f wRF %.1f wE %.1f | "
-                    "mma tot %.1f w0 %.1f w1 %.1f | slots 9.. (fprop: prod tot wRE, epi0 tot wTF, epi1 tot wTF; wgrad: prod tot wRE wE, dz-prod tot - wE): %.1f %.1f %.1f %.1f %.1f %.1f\n",
-            what, ev_ms * 1e3, tiles_per_cta, p.stages, m[0], m[1], m[2], m[3], m[4], m[5], m[6], m[7], m[8], m[9], m[10], m[11], m[12], m[13], m[14]);
-    count_launch(ctx);
-    return ELD_OK;
+    const size_t slot = kFcRaw + (wgrad ? kFcQTile : 0);
+    const size_t stg = wgrad ? 0 : ((128 * kFcStg * 4 + 1023) & ~1023);
+    return 1024 + 4096 + 2 * (kFcATile + kFcRing * slot + stg) + 512;
 }
 
+// conv1_1 (4 -> 32): software-im2col wgmma tiles on the fp32 NCHW frame (first_conv.cuh)
 int launch_first_conv(eld_ctx* ctx, const float* x, int cin, const void* w_img, const float* bias, void* out, int out_pitch,
                       int n, int H, int W, cudaStream_t st, void* sign_out)
 {
@@ -239,17 +156,11 @@ int launch_first_conv(eld_ctx* ctx, const float* x, int cin, const void* w_img, 
     p.x = x; p.n_img = n; p.H = H; p.W = W; p.tiles_x = W / 16; p.tiles_y = H / 8; p.cin = cin;
     p.w_img = static_cast<const uint8_t*>(w_img); p.bias = bias;
     p.out = static_cast<__nv_bfloat16*>(out); p.out_pitch = out_pitch; p.sign_out = static_cast<uint32_t*>(sign_out);
-    p.stages = 8;
-    static const int epi_groups = getenv("ELD_FC_ONE_EPI") ? 1 : 2;      // (A/B: one epilogue group)
-    p.epi_groups = epi_groups;
     const int total = n * p.tiles_x * p.tiles_y;
     const int grid = total < ctx->num_sms ? total : ctx->num_sms;
     CUtensorMap tmX;
     { int rc = encode_frame(ctx, &tmX, x, cin, n, H, W); if (rc) return rc; }
-    const size_t smem = 1024 + 4096 + (size_t)p.stages * kFcATile + ((kFcRawStages * kFcRaw + 1023) & ~1023) + 1024;
-    if (getenv("ELD_FC_PROF")) return fc_prof_launch(ctx, "fprop", grid, (double)total / grid, st, p, [&](const FirstConvParams& q) {
-        first_conv_fprop_kernel<true><<<grid, kFcThreadsFprop, smem, st>>>(tmX, q); });
-    ELD_CHECK_CUDA(launch_pdl(first_conv_fprop_kernel<false>, grid, kFcThreadsFprop, smem, st, tmX, p));
+    ELD_CHECK_CUDA(launch_pdl(first_conv_kernel<false>, grid, kFcThreads, first_conv_smem(false), st, tmX, tmX, p));
     ELD_CHECK_CUDA(cudaGetLastError());
     count_launch(ctx);
     return ELD_OK;
@@ -262,12 +173,6 @@ int launch_first_conv_wgrad(eld_ctx* ctx, const float* x, int cin, const void* d
     FirstConvParams p{};
     p.x = x; p.n_img = n; p.H = H; p.W = W; p.tiles_x = W / 16; p.tiles_y = H / 8; p.cin = cin;
     p.dw = dw; p.db = db;
-    p.stages = 6;
-    static const int split = getenv("ELD_FC_WGRAD_JOINT") == nullptr;                               // (A/B: one producer for both rings)
-    static const int groups = getenv("ELD_FC_WGRAD_GROUPS") ? atoi(getenv("ELD_FC_WGRAD_GROUPS")) : 2;
-    ELD_REQUIRE(groups >= 1 && groups <= (split ? 2 : 3), "first conv wgrad: 1..2 builder groups (3 with the joint producer)");
-    p.split_prod = split;
-    p.groups = groups;
     CUtensorMap tmQ;
     const cuuint64_t eb = 2;
     cuuint64_t dims[5] = { (cuuint64_t)dz_pitch, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n, 1 };
@@ -279,10 +184,7 @@ int launch_first_conv_wgrad(eld_ctx* ctx, const float* x, int cin, const void* d
     const int grid = total < ctx->num_sms ? total : ctx->num_sms;
     CUtensorMap tmX;
     { int rc = encode_frame(ctx, &tmX, x, cin, n, H, W); if (rc) return rc; }
-    const size_t smem = 1024 + (size_t)p.stages * (kFcATile + kFcQTile) + kFcATile + ((kFcRawStages * kFcRaw + 1023) & ~1023) + 1024;
-    if (getenv("ELD_FC_PROF")) return fc_prof_launch(ctx, "wgrad", grid, (double)total / grid, st, p, [&](const FirstConvParams& q) {
-        first_conv_wgrad_kernel<true><<<grid, kFcThreads, smem, st>>>(tmX, tmQ, q); });
-    ELD_CHECK_CUDA(launch_pdl(first_conv_wgrad_kernel<false>, grid, kFcThreads, smem, st, tmX, tmQ, p));
+    ELD_CHECK_CUDA(launch_pdl(first_conv_kernel<true>, grid, kFcThreads, first_conv_smem(true), st, tmX, tmQ, p));
     ELD_CHECK_CUDA(cudaGetLastError());
     count_launch(ctx);
     return ELD_OK;
@@ -291,143 +193,22 @@ int launch_first_conv_wgrad(eld_ctx* ctx, const float* x, int cin, const void* d
 int init_gemm_kernels(eld_ctx* ctx)
 {
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(first_conv_fprop_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(first_conv_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(first_conv_fprop_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(first_conv_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv_umma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv_umma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-#define ELD_WG2_ATTR(PR, A, N) ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_conv_kernel<PR, A, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    ELD_WG2_ATTR(false, 64, 32) ELD_WG2_ATTR(false, 64, 64) ELD_WG2_ATTR(false, 64, 128) ELD_WG2_ATTR(false, 64, 256)
-    ELD_WG2_ATTR(false, 128, 32) ELD_WG2_ATTR(false, 128, 64) ELD_WG2_ATTR(false, 128, 128) ELD_WG2_ATTR(false, 128, 256)
-    ELD_WG2_ATTR(true, 64, 32) ELD_WG2_ATTR(true, 64, 64) ELD_WG2_ATTR(true, 64, 128) ELD_WG2_ATTR(true, 64, 256)
-    ELD_WG2_ATTR(true, 128, 32) ELD_WG2_ATTR(true, 128, 64) ELD_WG2_ATTR(true, 128, 128) ELD_WG2_ATTR(true, 128, 256)
-#undef ELD_WG2_ATTR
-    return ELD_OK;
-}
-
-template <bool PROF>
-static void launch_wg2(int grid, size_t smem, cudaStream_t st, const CUtensorMap& tmP, const CUtensorMap& tmQ, const Wgrad2Params& p)
-{
-    const int rbp = p.box_ch * 2;
-#define ELD_WG2_CASE(A, N) if (rbp == A && p.n_tile == N) { (void)launch_pdl(wgrad_conv_kernel<PROF, A, N>, grid, kWg2Threads, smem, st, tmP, tmQ, p); return; }
-    ELD_WG2_CASE(64, 32) ELD_WG2_CASE(64, 64) ELD_WG2_CASE(64, 128) ELD_WG2_CASE(64, 256)
-    ELD_WG2_CASE(128, 32) ELD_WG2_CASE(128, 64) ELD_WG2_CASE(128, 128) ELD_WG2_CASE(128, 256)
-#undef ELD_WG2_CASE
-}
-
-// conv3x3 weight gradient, full-halo generation (wgrad_conv.cuh)
-static int launch_wgrad_conv(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
-{
-    Wgrad2Params p{};
-    p.n_img = op.n_img; p.H = op.H; p.W = op.W;
-    p.chunks_x = op.W / 8; p.chunks_y = op.H / 8;
-    p.cin = op.p_ch; p.cout = op.q_ch; p.p_c0 = op.p_c0; p.q_c0 = op.q_c0;
-    if (op.p_ch == 32) { p.kind = 0; p.box_ch = 32; p.m_tiles = 3; p.cps = 1; p.p_boxes = 1; }
-    else if (op.p_ch == 64) { p.kind = 1; p.box_ch = 64; p.m_tiles = 5; p.cps = 1; p.p_boxes = 1; }
-    else { p.kind = 2; p.box_ch = 64; p.m_tiles = 9; p.cps = op.p_ch / 128; p.p_boxes = 2; }
-    p.q_box_ch = (op.q_ch % 64 == 0) ? 64 : 32;
-    p.n_tile = op.q_ch <= 256 ? op.q_ch : 256;
-    p.n_tiles = op.q_ch / p.n_tile;
-    p.q_boxes = p.n_tile / p.q_box_ch;
-    int gmax = 512 / p.n_tile;
-    if (gmax > kWg2MaxG) gmax = kWg2MaxG;
-    // the issue loop is specialised (wgrad_conv.cuh, WV_*): kind 0 -> 3 filter rows; kind 1 -> 5 / 3+2 / 2+2+1 tap pairs;
-    // kind 2 -> one filter row (3 taps) per CTA for N <= 128, tap pairs for N == 256
-    if (p.kind == 2) gmax = p.n_tile <= 128 ? 3 : 2;
-    if (p.kind == 1) gmax = p.n_tile <= 64 ? 5 : (p.n_tile == 128 ? 3 : 2);
-    if (p.kind == 0) gmax = 3;
-    p.G = gmax;
-    p.groups = (p.m_tiles + p.G - 1) / p.G;
-    const int rb_p = p.box_ch * 2, rb_q = p.q_box_ch * 2;
-    const int chunk_bytes = p.p_boxes * ((100 * rb_p + 1023) & ~1023) + p.q_boxes * 64 * rb_q;
-    // chunks per stage: as many as still leave a 3-deep ring (small-N layers are bound by the issuing thread's
-    // per-stage barrier round trip, not by the tensor pipe)
-    int cps_stage = (200 * 1024) / (3 * chunk_bytes);
-    if (cps_stage > 4) cps_stage = 4;
-    if (cps_stage < 1) cps_stage = 1;
-    if (p.kind == 0) cps_stage = 1;      // measured: the 32-channel layers lose with multi-chunk stages, the others gain
-    if (getenv("ELD_WGRAD_CPS") && atoi(getenv("ELD_WGRAD_CPS")) < cps_stage) cps_stage = atoi(getenv("ELD_WGRAD_CPS"));   // (experiments: cap)
-    p.cps_stage = cps_stage;
-    const int stage_bytes = cps_stage * chunk_bytes;
-    int stages = (200 * 1024) / stage_bytes;
-    if (stages > 8) stages = 8;
-    if (stages < 2) stages = 2;
-    p.stages = stages;
-    int cols = 32;
-    while (cols < p.G * p.n_tile) cols *= 2;
-    p.tmem_cols = cols;
-    const int items = p.cps * p.groups * p.n_tiles;
-    const int total_chunks = op.n_img * p.chunks_x * p.chunks_y;
-    // split-K: every split adds its whole [9*cin x cout] tile with red.add, so big outputs get one wave only
-    const size_t outputs = (size_t)9 * op.p_ch * op.q_ch;
-    // measured (profiles/): two waves of CTAs only pay for the full-resolution thin layers (>= 16K chunks, small outputs)
-    int waves = (outputs > (1u << 18) || total_chunks < 16384) ? 1 : 2;
-    if (getenv("ELD_WGRAD_WAVES")) waves = atoi(getenv("ELD_WGRAD_WAVES"));
-    int ksplit = (waves * ctx->num_sms) / items;
-    if (ksplit < 1) ksplit = 1;
-    if (ksplit > total_chunks) ksplit = total_chunks;
-    p.ksplit = ksplit;
-    p.dw = op.dw;
-    p.out_tco = op.out_tco;
-    p.dbg = getenv("ELD_CONV_DBG") ? atoi(getenv("ELD_CONV_DBG")) : 0;
-    p.db = getenv("ELD_WGRAD_NOBIAS") ? nullptr : op.db;     // (debugging: time the tile without the fused bias gradient)
-    CUtensorMap tmP, tmQ;
-    const cuuint64_t eb = 2;
-    {
-        cuuint64_t dims[5] = { (cuuint64_t)op.p_pitch, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.n_img, 1 };
-        cuuint64_t str[4] = { op.p_pitch * eb, (cuuint64_t)op.W * op.p_pitch * eb, (cuuint64_t)op.H * op.W * op.p_pitch * eb,
-                              (cuuint64_t)op.n_img * op.H * op.W * op.p_pitch * eb };
-        cuuint32_t box[5] = { (cuuint32_t)p.box_ch, 10, 10, 1, 1 };
-        int rc = encode(ctx, &tmP, op.p, 5, dims, str, box, p.box_ch * 2);
-        if (rc) return rc;
-    }
-    {
-        cuuint64_t dims[5] = { (cuuint64_t)op.q_pitch, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.n_img, 1 };
-        cuuint64_t str[4] = { op.q_pitch * eb, (cuuint64_t)op.W * op.q_pitch * eb, (cuuint64_t)op.H * op.W * op.q_pitch * eb,
-                              (cuuint64_t)op.n_img * op.H * op.W * op.q_pitch * eb };
-        cuuint32_t box[5] = { (cuuint32_t)p.q_box_ch, 8, 8, 1, 1 };
-        int rc = encode(ctx, &tmQ, op.q, 5, dims, str, box, p.q_box_ch * 2);
-        if (rc) return rc;
-    }
-    const size_t smem = (size_t)stages * stage_bytes + 1024 + 256;
-    if (getenv("ELD_CONV_PROF")) {
-        const int grid = items * p.ksplit;
-        long long* d = nullptr;
-        ELD_CHECK_CUDA(cudaMalloc(&d, (size_t)grid * 8 * sizeof(long long)));
-        ELD_CHECK_CUDA(cudaMemsetAsync(d, 0, (size_t)grid * 8 * sizeof(long long), st));
-        p.prof = d;
-        launch_wg2<true>(grid, smem, st, tmP, tmQ, p);
-        ELD_CHECK_CUDA(cudaStreamSynchronize(st));
-        std::vector<long long> h((size_t)grid * 8);
-        ELD_CHECK_CUDA(cudaMemcpy(h.data(), d, h.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-        cudaFree(d);
-        double m[8] = { 0 }, mx = 0;
-        for (int b = 0; b < grid; ++b) for (int k = 0; k < 8; ++k) m[k] += (double)h[(size_t)b * 8 + k] / grid;
-        for (int b = 0; b < grid; ++b) if ((double)h[(size_t)b * 8 + 4] > mx) mx = (double)h[(size_t)b * 8 + 4];
-        fprintf(stderr, "[wgrad prof] slowest cta %.1f kclk | ", mx / 1e3);
-        fprintf(stderr, "[wgrad prof] cin %d cout %d HxW %dx%d kind %d G %d groups %d n_tile %d items %d ksplit %d grid %d stages %d chunks/cta %.1f | kclk: "
-                        "prod tot %.1f wE %.1f | mma tot %.1f wF %.1f issue %.1f commit %.1f | epi tot %.1f red %.1f\n",
-                op.p_ch, op.q_ch, op.H, op.W, p.kind, p.G, p.groups, p.n_tile, items, p.ksplit, grid, p.stages,
-                (double)total_chunks / p.ksplit, m[0] / 1e3, m[1] / 1e3, m[2] / 1e3, m[3] / 1e3, m[6] / 1e3, m[7] / 1e3, m[4] / 1e3, m[5] / 1e3);
-    } else {
-        launch_wg2<false>(items * p.ksplit, smem, st, tmP, tmQ, p);
-    }
-    ELD_CHECK_CUDA(cudaGetLastError());
-    count_launch(ctx);
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(first_conv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_conv_smem(false)));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(first_conv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_conv_smem(true)));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     return ELD_OK;
 }
 
 int launch_wgrad(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
 {
-    if (op.mode == WG_CONV && op.H % 8 == 0 && op.W % 8 == 0 && (op.p_ch == 32 || op.p_ch == 64 || op.p_ch % 128 == 0) &&
-        (op.q_ch == 32 || op.q_ch == 64 || op.q_ch == 128 || op.q_ch % 256 == 0) && !(op.p_ch == 32 && op.q_ch > 128) &&
-        !getenv("ELD_WGRAD_V1"))
-        return launch_wgrad_conv(ctx, op, st);
-    ELD_REQUIRE(op.db == nullptr || op.mode == WG_DECONV, "wgrad tile: the first-generation tile fuses the bias gradient for deconvs only");
     ELD_REQUIRE(op.H % 4 == 0 && op.W % 16 == 0, "wgrad tile: H=%d must be a multiple of 4 and W=%d of 16", op.H, op.W);
     ELD_REQUIRE(op.p_ch % 32 == 0 && op.q_ch % 32 == 0, "wgrad tile: channel counts must be multiples of 32");
+    ELD_REQUIRE(op.out_tco == 0 || op.mode == WG_CONV, "wgrad tile: the [tap][ci][co] layout is a conv layout");
     WgradParams p{};
     p.n_img = op.n_img; p.H = op.H; p.W = op.W;
     p.chunks_x = op.W / 16; p.chunks_y = op.H / 4;
@@ -439,26 +220,22 @@ int launch_wgrad(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
     p.m_tiles = (total_boxes + p.boxes_per_mtile - 1) / p.boxes_per_mtile;
     p.q_ch = op.q_ch; p.q_c0 = op.q_c0;
     p.q_box_ch = (op.q_ch % 64 == 0) ? 64 : 32;
-    p.n_tile = op.q_ch <= 256 ? op.q_ch : 256;
-    ELD_REQUIRE(op.q_ch % p.n_tile == 0, "wgrad tile: N=%d not divisible by %d", op.q_ch, p.n_tile);
-    p.n_tiles = op.q_ch / p.n_tile;
+    const int n_tile = (op.q_ch % 128 == 0) ? 128 : (op.q_ch % 64 == 0) ? 64 : 32;
+    p.n_tiles = op.q_ch / n_tile;
+    const int items = p.m_tiles * p.n_tiles;
     const int total_chunks = op.n_img * p.chunks_x * p.chunks_y;
-    // every K split adds its whole 128 x n_tile tile with SCALAR atomics (the PyTorch IOHW layout leaves nothing contiguous
-    // to vectorise): one wave of CTAs instead of two halves those (e.g. upv7: 9.7 M -> 4.8 M atomics per step)
-    const int waves1 = getenv("ELD_WGRAD1_WAVES") ? atoi(getenv("ELD_WGRAD1_WAVES")) : 1;
-    int ksplit = (waves1 * ctx->num_sms) / (p.m_tiles * p.n_tiles);
+    // every K split adds its whole 128 x n_tile tile with atomics: one wave of CTAs
+    int ksplit = ctx->num_sms / items;
     if (ksplit < 1) ksplit = 1;
     if (ksplit > total_chunks) ksplit = total_chunks;
     p.ksplit = ksplit;
-    const int stage_bytes = kWgradKP * (256 + 2 * p.n_tile);
+    const int stage_bytes = kWgradKP * (256 + 2 * n_tile);
     int stages = (200 * 1024) / stage_bytes;
     if (stages > 8) stages = 8;
     if (stages < 2) stages = 2;
     p.stages = stages;
-    int cols = 32;
-    while (cols < p.n_tile) cols *= 2;
-    p.tmem_cols = cols;
     p.dw = op.dw;
+    p.out_tco = op.out_tco;
     p.db = op.db;
 
     CUtensorMap tmP, tmQ;
@@ -487,8 +264,12 @@ int launch_wgrad(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
         if (rc) return rc;
     }
     const size_t smem = (size_t)stages * stage_bytes + 1024 + 256;
-    const int grid = p.m_tiles * p.n_tiles * p.ksplit;
-    ELD_CHECK_CUDA(launch_pdl(wgrad_umma_kernel, grid, kWgradThreads, smem, st, tmP, tmQ, p));
+    const int grid = items * p.ksplit;
+    cudaError_t e;
+    if (n_tile == 128) e = launch_pdl(wgrad_gemm_kernel<128>, grid, kWgradThreads, smem, st, tmP, tmQ, p);
+    else if (n_tile == 64) e = launch_pdl(wgrad_gemm_kernel<64>, grid, kWgradThreads, smem, st, tmP, tmQ, p);
+    else e = launch_pdl(wgrad_gemm_kernel<32>, grid, kWgradThreads, smem, st, tmP, tmQ, p);
+    ELD_CHECK_CUDA(e);
     ELD_CHECK_CUDA(cudaGetLastError());
     count_launch(ctx);
     return ELD_OK;

@@ -1,4 +1,4 @@
-// unet_prims.h - internal (C++) interface of the tcgen05 tiles, shared by the C-ABI primitives and
+// unet_prims.h - internal (C++) interface of the wgmma tiles, shared by the C-ABI primitives and
 // the U-Net engine.
 #pragma once
 #include "common.cuh"
@@ -14,7 +14,7 @@ enum { PACK_CONV_FPROP = 0, PACK_CONV_DGRAD = 1, PACK_DECONV_FPROP = 2, PACK_DEC
 // Element index of logical B[n][tap][c] (n < rows, c < ck) inside the packed weight operand.
 // The operand is stored as the exact shared-memory IMAGE the conv tile consumes: contiguous blocks
 // [n_tile_idx][tap][channel chunk], each block = n_tile rows of kc channels (64 B / 128 B per row) with the
-// UMMA/TMA 64B / 128B swizzle already applied - so a whole block (or, for resident weights, a whole n-tile) is
+// wgmma/TMA 64B / 128B swizzle already applied - so a whole block is
 // ONE linear cp.async.bulk instead of n_tile TMA tensor rows.
 __host__ __device__ inline size_t packed_index(int rows, int ck, int taps, int n, int tap, int c)
 {

@@ -1,23 +1,23 @@
-// wgrad_umma.cuh - tcgen05 weight-gradient tile: a GEMM whose reduction (K) dimension is PIXELS.
+// wgrad_umma.cuh - wgmma weight-gradient tile: a GEMM whose reduction (K) dimension is PIXELS.
 //
-//   D[128 x n_tile] (f32, TMEM)  =  sum over pixels p   P[p, m] * Q[p, n]
+//   D[128 x n_tile] (f32, registers)  =  sum over pixels p   P[p, m] * Q[p, n]
 //
-// Both operands are pixel-major NHWC tensors, i.e. "MN-major" UMMA operands: a TMA box
-// {box_ch channels, 16, 4} lands in smem as 64 pixel rows of box_ch*2 bytes (64 B / 128 B swizzled) and is
-// consumed directly with a_major = b_major = MN.
+// Both operands are pixel-major NHWC tensors, i.e. MN-major wgmma operands: a TMA box {box_ch channels, 16, 4} lands
+// in smem as 64 pixel rows of box_ch*2 bytes (64 B / 128 B swizzled) and is consumed directly (transposed operands).
 //   conv3x3 wgrad : P = layer input X shifted by the filter tap (zero-filled halo = padding),
 //                   M rows = (tap, ci) packed 128 at a time;  Q = dZ, N = co.
 //   deconv  wgrad : P = d(up) gathered per sub-pixel (kh,kw) through a 5-D map, M rows = (s, co);
 //                   Q = deconv input X, N = ci.
-// Work item = (M tile, N tile, K split); each CTA accumulates its pixel range in TMEM and adds the
-// f32 tile into the PyTorch-layout gradient with red.global.add (dW is zeroed once per step).
+// Work item = (M tile, N tile, K split); warpgroups 1 and 2 accumulate M rows 0-63 / 64-127 of the item's pixel range
+// in registers and add the f32 tile into the gradient with red.global.add (the gradient is zeroed once per step).
+// The optional bias gradient (conv: column sums of dZ; deconv: column sums of d(up)) is summed from the same smem
+// tiles while the MMAs run.
 #pragma once
 #include "umma.cuh"
 #include "unet_prims.h"
 #include <cuda_bf16.h>
 
 namespace eld {
-
 
 struct WgradParams {
     int n_img, H, W;          // pixel grid of the K dimension (conv: layer grid; deconv: coarse grid)
@@ -32,20 +32,29 @@ struct WgradParams {
     int q_ch;                 // N total (conv: cout, deconv: cin)
     int q_c0;
     int q_box_ch;             // 32 or 64
-    int n_tile, n_tiles;
+    int n_tiles;
     int ksplit;
-    int stages, tmem_cols;
-    float* dw;                // f32 gradient, PyTorch layout (conv OIHW [q_ch][p_ch][3][3]; deconv IOHW [q_ch][p_ch][2][2])
-    float* db;                // deconv only, optional: bias gradient db[co] += sum over the FINE pixels of d(up)[., co] = column
-                              // sums of the P boxes, formed by the otherwise idle epilogue warps of the nt == 0 CTAs while the MMAs run
+    int stages;
+    float* dw;                // f32 gradient: conv OIHW [q_ch][p_ch][3][3] or (out_tco) [tap][p_ch][q_ch]; deconv IOHW [q_ch][p_ch][2][2]
+    int out_tco;
+    float* db;                // optional bias gradient (conv: db[co] += sum dZ; deconv: db[co] += sum d(up) over the fine pixels)
 };
 
-constexpr int kWgradThreads = 192;
+constexpr int kWgradThreads = 384;
 constexpr int kWgradKP = 64;  // pixels per stage
 
+// bf16 element (row, ch) of a swizzled TMA box with `rb`-byte rows, as f32
+__device__ __forceinline__ float box_elem(const uint8_t* box, int rb, int row, int ch)
+{
+    const uint32_t swz = rb == 128 ? (uint32_t)(row & 7) : (uint32_t)((row >> 1) & 3);
+    const uint32_t byte = (uint32_t)(ch * 2);
+    const unsigned short v = *reinterpret_cast<const unsigned short*>(box + row * rb + ((((byte >> 4) ^ swz)) << 4) + (byte & 15u));
+    return __uint_as_float((uint32_t)v << 16);
+}
+
+template <int NT>
 __global__ void __launch_bounds__(kWgradThreads, 1)
-wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmQ,
-                  const WgradParams p)
+wgrad_gemm_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmQ, const WgradParams p)
 {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = ptx::smem_u32(smem_raw);
@@ -53,15 +62,12 @@ wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_constant
 
     const int p_row = p.box_ch * 2, q_row = p.q_box_ch * 2;          // bytes per pixel row of one box
     const int p_box = kWgradKP * p_row, q_box = kWgradKP * q_row;
-    const int q_boxes = p.n_tile / p.q_box_ch;
+    const int q_boxes = NT / p.q_box_ch;
     const int a_bytes = p.boxes_per_mtile * p_box;                  // = 64 * 256 = 16 KB
     const int stage_bytes = a_bytes + q_boxes * q_box;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
     uint64_t* empty = full + p.stages;
-    uint64_t* acc_full = empty + p.stages;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     int item = blockIdx.x;
     const int ks = item % p.ksplit; item /= p.ksplit;
     const int nt = item % p.n_tiles;
@@ -73,45 +79,42 @@ wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_constant
     const int ch_end = min(total_chunks, ch_begin + per);
     const int nchunks = max(0, ch_end - ch_begin);
     const int boxes_per_tap = p.p_ch / p.box_ch;
-    const bool do_bias = p.db != nullptr && nt == 0;      // the P (d(up)) boxes are the same for every N tile: one of them sums
+    // the P (d(up)) boxes are the same for every N tile, the Q (dZ) boxes for every M tile: one CTA of each sums them
+    const int bias_kind = !p.db ? 0 : (p.mode == WG_DECONV ? (nt == 0 ? 1 : 0) : (mt == 0 ? 2 : 0));
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         ptx::prefetch_tmap(&tmP);
         ptx::prefetch_tmap(&tmQ);
-        for (int s = 0; s < p.stages; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], do_bias ? 5 : 1); }
-        ptx::mbar_init(acc_full, 1);
+        for (int s = 0; s < p.stages; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 8); }
         ptx::fence_barrier_init();
     }
-    if (warp == 2) ptx::tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     ptx::grid_dep_wait();       // PDL: the prologue above overlapped the previous kernel's tail
     ptx::grid_dep_launch();
 
-    if (warp == 0) {
-        if (lane == 0 && nchunks > 0) {
+    if (threadIdx.x < 128) {
+        // ===================== TMA producer (warpgroup 0; one thread works) =====================
+        if (threadIdx.x == 0 && nchunks > 0) {
             // per-box constants (tap shift, channel) do not depend on the chunk: hoist them
             int bc[4], bdx[4], bdy[4];
             for (int b = 0; b < p.boxes_per_mtile; ++b) {
                 const int gb = mt * p.boxes_per_mtile + b;
                 int tap = gb / boxes_per_tap;
                 bc[b] = p.p_c0 + (gb - tap * boxes_per_tap) * p.box_ch;
-                if (tap >= p.taps) tap = p.taps - 1;            // dummy rows: load something valid, result ignored
+                if (tap >= p.taps) { tap = p.taps - 1; bc[b] = p.p_c0; }   // dummy rows: load something valid, result ignored
                 if (p.mode == WG_CONV) { bdx[b] = (tap % 3) - 1; bdy[b] = (tap / 3) - 1; }
                 else { bdx[b] = tap & 1; bdy[b] = tap >> 1; }
             }
-            const int qc0 = p.q_c0 + nt * p.n_tile;
+            const int qc0 = p.q_c0 + nt * NT;
             const int cxy = p.chunks_x * p.chunks_y;
             int img = ch_begin / cxy;
             int rem = ch_begin - img * cxy;
             int cy = rem / p.chunks_x, cx = rem - cy * p.chunks_x;
             int s = 0;
             uint32_t ph = 0;
-            uint8_t* sa = smem;
             for (int i = 0; i < nchunks; ++i) {
                 const int x0 = cx * 16, y0 = cy * 4;
+                uint8_t* sa = smem + (size_t)s * stage_bytes;
                 ptx::mbar_wait(&empty[s], ph ^ 1u);
                 ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)stage_bytes);
                 if (p.mode == WG_CONV) {
@@ -124,93 +127,95 @@ wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_constant
                 uint8_t* sq = sa + a_bytes;
                 for (int b = 0; b < q_boxes; ++b)
                     ptx::tma_load_5d(sq + b * q_box, &tmQ, &full[s], qc0 + b * p.q_box_ch, x0, y0, img, 0);
-                sa += stage_bytes;
-                if (++s == p.stages) { s = 0; ph ^= 1u; sa = smem; }
+                if (++s == p.stages) { s = 0; ph ^= 1u; }
                 if (++cx == p.chunks_x) { cx = 0; if (++cy == p.chunks_y) { cy = 0; ++img; } }
             }
         }
-    } else if (warp == 1) {
-        const uint32_t idesc = ptx::make_idesc_bf16(128, (uint32_t)p.n_tile, 1, 1);   // both MN-major
-        const uint32_t a_layout = p.box_ch == 64 ? ptx::LAYOUT_SW128 : ptx::LAYOUT_SW64;
-        const uint32_t b_layout = p.q_box_ch == 64 ? ptx::LAYOUT_SW128 : ptx::LAYOUT_SW64;
-        // MN-major: LBO = distance between channel blocks (one TMA box), SBO = 8 pixel rows
-        const uint64_t a_hi = ptx::make_smem_desc(0, (uint32_t)p_box, 8u * p_row, a_layout);
-        const uint64_t b_hi = ptx::make_smem_desc(0, (uint32_t)q_box, 8u * q_row, b_layout);
-        const uint32_t a_step = (16u * p_row) >> 4, b_step = (16u * q_row) >> 4;       // 16 pixel rows per MMA
-        const uint32_t smem_base = ptx::smem_u32(smem);
-        uint32_t a_addr = smem_base;
-        int s = 0;
-        uint32_t ph = 0;
-        for (int i = 0; i < nchunks; ++i) {
-            ptx::mbar_wait(&full[s], ph);
-            ptx::tc_fence_after();
-            if (ptx::elect_one()) {
-                uint64_t ad = a_hi | (uint64_t)((a_addr & 0x3FFFFu) >> 4);
-                uint64_t bd = b_hi | (uint64_t)(((a_addr + (uint32_t)a_bytes) & 0x3FFFFu) >> 4);
+        return;
+    }
+    if (nchunks == 0) return;
+
+    // ===================== consumers: warpgroup cg = 0 / 1 owns M rows 64 cg .. 64 cg + 63 =====================
+    const int cg = (threadIdx.x >> 7) - 1;
+    const int t = threadIdx.x & 127, lane = threadIdx.x & 31;
+    // MN-major operands: LBO = next box (the next 32 / 64 channels), SBO = 8 pixel rows; one k16 step = 16 pixel rows
+    const uint64_t a_desc0 = ptx::make_gmma_desc(0, (uint32_t)p_box, 8u * p_row, ptx::gmma_layout(p_row));
+    const uint64_t b_desc0 = ptx::make_gmma_desc(0, (uint32_t)q_box, 8u * q_row, ptx::gmma_layout(q_row));
+    const uint32_t a_step = (16u * p_row) >> 4, b_step = (16u * q_row) >> 4;
+    const uint32_t smem_base = ptx::smem_u32(smem);
+    const uint32_t a_off = (uint32_t)((64 * cg / p.box_ch) * p_box);
+    // bias gradient: column `bcol` (a P row of the M tile, or a Q column) summed over pixel rows 32 bh .. 32 bh + 31
+    const int bct = cg * 128 + t, bcol = bct & 127, bh = bct >> 7;
+    const bool bias_on = (bias_kind == 1) || (bias_kind == 2 && bcol < NT);
+    float bsum = 0.f;
+    float acc[NT / 2];
 #pragma unroll
-                for (int k = 0; k < kWgradKP / 16; ++k) {
-                    ptx::umma_bf16(tmem_base, ad, bd, idesc, (i | k) != 0 ? 1u : 0u);
-                    ad += a_step; bd += b_step;
-                }
-                ptx::umma_commit(&empty[s]);
-                if (i == nchunks - 1) ptx::umma_commit(acc_full);
-            }
-            __syncwarp();
-            a_addr += (uint32_t)stage_bytes;
-            if (++s == p.stages) { s = 0; ph ^= 1u; a_addr = smem_base; }
+    for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+    int s = 0, prev = -1;
+    uint32_t ph = 0;
+    for (int i = 0; i < nchunks; ++i) {
+        ptx::mbar_wait(&full[s], ph);
+        const uint32_t st = smem_base + (uint32_t)s * (uint32_t)stage_bytes;
+        uint64_t ad = a_desc0 | (uint64_t)(((st + a_off) & 0x3FFFFu) >> 4);
+        uint64_t bd = b_desc0 | (uint64_t)(((st + (uint32_t)a_bytes) & 0x3FFFFu) >> 4);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kWgradKP / 16; ++k) {
+            ptx::wgmma_bf16<NT, 1, 1>(acc, ad, bd, 1u);
+            ad += a_step; bd += b_step;
         }
-    } else if (nchunks > 0) {
-        const int q = warp & 3;
-        const int r = q * 32 + lane;                       // D row = (box, channel in box)
+        ptx::wgmma_commit();
+        if (bias_on) {
+            const uint8_t* sb = smem + (size_t)s * stage_bytes;
+            if (bias_kind == 1) {
+                const uint8_t* box = sb + (size_t)(bcol / p.box_ch) * p_box;
+                for (int row = 32 * bh; row < 32 * bh + 32; ++row) bsum += box_elem(box, p_row, row, bcol % p.box_ch);
+            } else {
+                const uint8_t* box = sb + a_bytes + (size_t)(bcol / p.q_box_ch) * q_box;
+                for (int row = 32 * bh; row < 32 * bh + 32; ++row) bsum += box_elem(box, q_row, row, bcol % p.q_box_ch);
+            }
+        }
+        ptx::wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty[prev]);
+        prev = s;
+        if (++s == p.stages) { s = 0; ph ^= 1u; }
+    }
+    ptx::wgmma_wait<0>();
+    ptx::reg_fence(acc);
+    if (lane == 0) ptx::mbar_arrive(&empty[prev]);
+
+    if (bias_kind == 1 && bias_on) {
+        const int b = bcol / p.box_ch, gb = mt * p.boxes_per_mtile + b, tap = gb / boxes_per_tap;
+        if (tap < p.taps) atomicAdd(p.db + (gb - tap * boxes_per_tap) * p.box_ch + (bcol - b * p.box_ch), bsum);
+    } else if (bias_kind == 2 && bias_on) {
+        atomicAdd(p.db + nt * NT + bcol, bsum);
+    }
+
+    // ===================== epilogue: registers -> red.add into dW =====================
+    const int wq = t >> 5;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const int r = 64 * cg + 16 * wq + (lane >> 2) + 8 * i;     // D row = (box, channel in box)
         const int b = r / p.box_ch;
         const int gb = mt * p.boxes_per_mtile + b;
         const int tap = gb / boxes_per_tap;
+        if (tap >= p.taps) continue;
         const int pc = (gb - tap * boxes_per_tap) * p.box_ch + (r - b * p.box_ch);   // P-side channel
-        if (do_bias) {
-            // ---- bias gradient while the MMAs run: this thread's (tap, channel) column of the P boxes, all 64 pixel rows ----
-            const int cib = r - b * p.box_ch;                  // channel inside the box
-            const uint32_t chunk16 = (uint32_t)(cib * 2) >> 4, in16 = (uint32_t)(cib * 2) & 15u;
-            float acc = 0.f;
-            int s = 0;
-            uint32_t ph = 0;
-            for (int i = 0; i < nchunks; ++i) {
-                ptx::mbar_wait(&full[s], ph);
-                if (tap < p.taps) {
-                    const uint8_t* box = smem + (size_t)s * stage_bytes + (size_t)b * p_box;
-#pragma unroll 8
-                    for (int row = 0; row < kWgradKP; ++row) {
-                        const uint32_t swz = (p_row == 128) ? (uint32_t)(row & 7) : (uint32_t)((row >> 1) & 3);
-                        const unsigned short v = *reinterpret_cast<const unsigned short*>(box + row * p_row + ((chunk16 ^ swz) << 4) + in16);
-                        acc += __uint_as_float((uint32_t)v << 16);
-                    }
-                }
-                __syncwarp();
-                if (lane == 0) ptx::mbar_arrive(&empty[s]);
-                if (++s == p.stages) { s = 0; ph ^= 1u; }
-            }
-            if (tap < p.taps) atomicAdd(p.db + pc, acc);
-        }
-        ptx::mbar_wait(acc_full, 0);
-        ptx::tc_fence_after();
-        const uint32_t t_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-        for (int c32 = 0; c32 < p.n_tile / 32; ++c32) {
-            uint32_t v[32];
-            ptx::tmem_ld32(t_addr + c32 * 32, v);
-            ptx::tmem_ld_wait();
-            if (tap < p.taps) {
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int qc = nt * p.n_tile + c32 * 32 + j;   // Q-side channel
-                    // conv: dW[co=qc][ci=pc][tap] ; deconv: dWt[ci=qc][co=pc][s=tap]
-                    float* dst = p.dw + ((size_t)qc * p.p_ch + pc) * p.taps + tap;
-                    atomicAdd(dst, __uint_as_float(v[j]));
-                }
+        for (int j = 0; j < NT / 8; ++j) {
+            const int qc = nt * NT + 8 * j + 2 * (lane & 3);                           // Q-side channel
+            const float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+            if (p.out_tco) {
+                float* dst = p.dw + ((size_t)tap * p.p_ch + pc) * p.q_ch + qc;
+                atomicAdd(dst, v0);
+                atomicAdd(dst + 1, v1);
+            } else {
+                // conv: dW[co=qc][ci=pc][tap] ; deconv: dWt[ci=qc][co=pc][s=tap]
+                atomicAdd(p.dw + ((size_t)qc * p.p_ch + pc) * p.taps + tap, v0);
+                atomicAdd(p.dw + ((size_t)(qc + 1) * p.p_ch + pc) * p.taps + tap, v1);
             }
         }
     }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) ptx::tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
 }
 
 }  // namespace eld

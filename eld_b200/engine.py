@@ -51,8 +51,8 @@ class Engine(object):
         opt, model = self.opt, self.model
         epoch_start_time = time.time()
         # engine.py:40-55's loop; with opt.prefetch_noise it runs ONE batch of look-ahead: after step i has been queued, the
-        # synthesis of step i+1's noisy input starts on a side stream (ELDModel.prefetch_input).  Off by default: on B200
-        # the overlapped noise CTAs slow the tiles' epilogue warps by as much as they save (profiles/r02_overlap_ab.txt).
+        # synthesis of step i+1's noisy input starts on a side stream (ELDModel.prefetch_input).  Off by default: the
+        # overlapped noise CTAs take issue slots from the persistent tiles.
         it = iter(train_loader)
         data = next(it, None)
         while data is not None:

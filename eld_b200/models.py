@@ -3,7 +3,7 @@
 Reference: models/ELD_model.py:172-200 (set_input), :352-523 (ELDModel), models/base_model.py.
 
 Differences that are the point of this repo
-  * netG is eld_b200.arch.unet (tcgen05 engine); forward+L1+backward is ONE C-ABI call, Adam another;
+  * netG is eld_b200.arch.unet (wgmma engine); forward+L1+backward is ONE C-ABI call, Adam another;
   * noise can be synthesised ON THE TRAINING STREAM (opt.noise_on_gpu / a batch without 'input'):
     only the clean frame crosses PCIe, the fused CUDA kernel makes the noisy input (SURVEY F4);
   * data parallel: if torch.distributed is initialised the flat gradient buffer is all-reduced

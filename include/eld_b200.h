@@ -1,4 +1,4 @@
-/* eld_b200.h - C ABI of the B200-native ELD hot path (libeld_b200.so).
+/* eld_b200.h - C ABI of the H100-native ELD hot path (libeld_b200.so).
  *
  * The reference (Vandermode/ELD) has no FFI layer: its seams are Python duck-typed protocols
  * (SURVEY.md 8b).  This header is what a binding for that seam would call; every entry point

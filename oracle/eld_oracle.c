@@ -4,10 +4,10 @@
  * load this library; the product (libeld_b200.so) never links or calls it.
  *
  * What it restates
- *   - NoiseModelBase.__call__            /root/reference/noise.py:149-170  (scale, shot, read, unscale)
- *   - clip                               /root/reference/dataset/sid_dataset.py:277
- *   - RawPacker.pack_raw_bayer           /root/reference/noise.py:10-20     (RGBG plane order)
- *   - LMDB de-quantisation               /root/reference/dataset/lmdb_dataset.py:38-39
+ *   - NoiseModelBase.__call__            noise.py:149-170  (scale, shot, read, unscale)
+ *   - clip                               dataset/sid_dataset.py:277
+ *   - RawPacker.pack_raw_bayer           noise.py:10-20     (RGBG plane order)
+ *   - LMDB de-quantisation               dataset/lmdb_dataset.py:38-39
  *   - np.random.poisson                  third-party numpy (legacy RandomState): PTRS (Hormann 1993)
  *                                        for lam >= 10 as numpy does; for lam < 10 sequential-search
  *                                        inversion (one uniform) instead of numpy's multiplication

@@ -1,12 +1,12 @@
 """CPU ORACLE (test infrastructure, NOT product code) - numpy / torch restatement of the arithmetic of
 ELDModelBase.eval.  Only tests/ may import this module.
 
-    illuminance_correct   <- /root/reference/models/ELD_model.py:138-169  (IlluminanceCorrect.forward / .correct)
-    tensor2im             <- /root/reference/models/ELD_model.py:23-38
-    psnr                  <- /root/reference/util/index.py:76-79 -> skimage.metrics.peak_signal_noise_ratio(data_range=255)
+    illuminance_correct   <- models/ELD_model.py:138-169  (IlluminanceCorrect.forward / .correct)
+    tensor2im             <- models/ELD_model.py:23-38
+    psnr                  <- util/index.py:76-79 -> skimage.metrics.peak_signal_noise_ratio(data_range=255)
                              (third-party scikit-image, not installed: its published formula 10 log10(R^2 / mse) on float64)
-    crop_center           <- /root/reference/util/util.py crop_center
-    forward_chop          <- /root/reference/models/ELD_model.py:434-467
+    crop_center           <- util/util.py crop_center
+    forward_chop          <- models/ELD_model.py:434-467
 
 Pinned by tests/golden/eval_kat.npz, produced by importing the UNMODIFIED models/ELD_model.py with stub modules for its
 uninstalled imports (tests/golden/make_golden.py eval).

@@ -2,8 +2,8 @@
 reference network and training step.  Only tests/, __graft_entry__.smoke() and bench.py's
 cpu_baseline / --impl reference legs may import this module.
 
-    UNetSeeInDarkRef          <- /root/reference/models/arch/Unet.py:6-104
-    l1_train_step             <- /root/reference/models/ELD_model.py:411-420,469-475 + models/losses.py:31-32
+    UNetSeeInDarkRef          <- models/arch/Unet.py:6-104
+    l1_train_step             <- models/ELD_model.py:411-420,469-475 + models/losses.py:31-32
 
 Pinned by tests/golden/unet_kat.npz, produced by running the unmodified reference module
 (tests/golden/make_golden.py): same torch seed -> identical default init -> same output/loss/grads.

@@ -1,13 +1,13 @@
 #!/usr/bin/env python
 """Generate the golden fixtures under tests/golden/ by RUNNING THE UNMODIFIED REFERENCE.
 
-Run in the authoring container only (needs /root/reference):
+Needs a checkout of the reference (Vandermode/ELD), named by ELD_REFERENCE_ROOT:
 
-    python tests/golden/make_golden.py
+    ELD_REFERENCE_ROOT=<path to the ELD checkout> python tests/golden/make_golden.py
 
-It imports /root/reference/noise.py (CWD must be the reference root because of the
+It imports the reference's noise.py (CWD must be the reference root because of the
 relative `camera_params/release` path, noise.py:187) and loads
-/root/reference/models/arch/Unet.py by file path (``import models`` drags in
+models/arch/Unet.py by file path (``import models`` drags in
 tensorboardX/rawpy, SURVEY 8c).  Nothing here is shipped to the GPU box except the
 small files it writes; the GPU-side tests read only those files.
 
@@ -36,7 +36,7 @@ import sys
 
 import numpy as np
 
-REF = '/root/reference'
+REF = os.environ.get('ELD_REFERENCE_ROOT', '')
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(os.path.dirname(HERE))
 

@@ -1,5 +1,5 @@
-"""GPU parity tests of the tcgen05 conv / deconv tiles against plain PyTorch fp32 on the same
-bf16-rounded operands.  Tolerance: the tile accumulates in fp32 (TMEM) and rounds the result to
+"""GPU parity tests of the wgmma conv / deconv tiles against plain PyTorch fp32 on the same
+bf16-rounded operands.  Tolerance: the tile accumulates in fp32 (registers) and rounds the result to
 bf16 once, so |err| <= 2^-8 * |ref| + 1e-2 * rms(ref) (bf16 output rounding + accumulation order)."""
 import numpy as np
 import pytest
@@ -114,7 +114,7 @@ WGRAD_CASES = [  # n, h, w, cin, cout, x_c0, x_pitch
 
 @pytest.mark.parametrize('case', WGRAD_CASES)
 def test_conv3x3_wgrad(torch, case):
-    """tcgen05 wgrad (pixels are the GEMM K dimension, MN-major operands) vs autograd of F.conv2d."""
+    """wgmma wgrad (pixels are the GEMM K dimension, MN-major operands) vs autograd of F.conv2d."""
     from eld_b200 import prims
     n, h, w, cin, cout, x_c0, xp = case
     g = torch.Generator(device='cuda').manual_seed(17)

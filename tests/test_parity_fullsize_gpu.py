@@ -8,12 +8,11 @@
 Gates (bf16 operands / activations / stored gradients, fp32 accumulation):
   out        rel-L2 <= 2e-2 vs fp32 oracle, <= 3e-3 vs emulation
   loss       <= 1e-2 relative vs fp32 oracle, <= 2e-3 vs emulation
-  gradients  per tensor rel-L2 <= 2e-3 vs the emulated backward (measured on B200: 9e-6 .. 6.5e-4, fp32 atomics
+  gradients  per tensor rel-L2 <= 2e-3 vs the emulated backward (fp32 atomics
              reorder sums; a real indexing or masking bug moves a tensor by >= 1e-1), and <= 5e-2 vs the fp32 autograd
-             (the bf16 storage itself: measured 1e-3 .. 3e-2, largest at the 32 x 32 bottleneck)
+             (the bf16 storage itself, largest at the 32 x 32 bottleneck)
   dPSNR      <= 0.05 dB between engine and fp32 oracle on seeded synthetic pairs (input = batch_gpu(clean), target =
              clean) with weights TRAINED for 200 Adam steps - an untrained net vs a random target is insensitive.
-             Measured: 0.003 .. 0.005 dB with the same weights, -0.02 dB between the two training trajectories.
 """
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""GPU parity of the whole tcgen05 U-Net step (through the C ABI) against the CPU oracle
+"""GPU parity of the whole wgmma U-Net step (through the C ABI) against the CPU oracle
 (oracle/unet_ref.py, pinned to the reference by tests/golden/unet_kat.npz).
 
 Stated tolerances (bf16 activations / bf16 GEMM operands, fp32 accumulation, fp32 master weights):

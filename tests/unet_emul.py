@@ -1,7 +1,7 @@
 """Test infrastructure: torch restatements of the U-Net step with the ENGINE's rounding points, forward and
 backward, so that a gradient gate can be tight enough to fail (VERDICT r1: cosine 0.99 passes a 14 % error).
 
-Rounding points of the tcgen05 engine (csrc/unet_engine.cu):
+Rounding points of the wgmma engine (csrc/unet_engine.cu):
   forward : bf16 GEMM operands (weights and the 4-channel input), fp32 accumulation, every stored activation bf16;
             the 1x1 head reads bf16 a9_2 with fp32 weights and writes fp32.
   backward: every STORED gradient is bf16 - the pre-activation gradients dz (after the LeakyReLU' mask), the
