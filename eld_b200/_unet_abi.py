@@ -37,6 +37,7 @@ def declare_engine(lib):
     lib.eld_unet_bucket_events.argtypes = [vp, i32]
     lib.eld_unet_wait_bucket.argtypes = [vp, i32, vp]
     lib.eld_unet_backward.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.eld_unet_input_grad.argtypes = [vp, vp, vp, vp]
     lib.eld_unet_set_loss.argtypes = [vp, i32]
     lib.eld_clock_probe.argtypes = [vp, vp, vp]
     lib.eld_unet_profile.argtypes = [vp, i32]

@@ -7,6 +7,7 @@ released checkpoints load, but all parameters are views into ONE flat fp32 buffe
 runs the wgmma engine behind the C ABI (csrc/unet_engine.cu) on NHWC bf16 activations.
 """
 import ctypes
+import warnings
 
 import torch
 import torch.nn as nn
@@ -29,6 +30,8 @@ class _EngineFunction(torch.autograd.Function):
     """The netG seam as an autograd node (SURVEY 8b): forward = the training engine's forward (activations stay in its
     workspace), backward = eld_unet_backward on the incoming d(loss)/d(out) - so the reference's own
     `loss.backward(); optimizer.step()` (ELD_model.py:411-420,469-475) runs against this module unchanged, with any loss.
+    When the frame requires grad (a learnable stage upstream, test-time optimisation of the input), eld_unet_input_grad
+    follows and gives d(loss)/d(x) as well.
     Parameters enter as inputs only so that autograd routes their gradients; the math reads the flat buffer."""
 
     @staticmethod
@@ -48,17 +51,24 @@ class _EngineFunction(torch.autograd.Function):
         g = torch.empty_like(net._flat)
         _lib.check(_lib.load().eld_unet_backward(ctx.eng, net._flat.data_ptr(), x.data_ptr(), dout.contiguous().data_ptr(),
                                                 g.data_ptr(), _st()), 'eld_unet_backward')
+        dx = None
+        if ctx.needs_input_grad[1]:              # conv1_1's data gradient, one launch; skipped when nothing upstream wants it
+            dx = torch.empty_like(x)
+            _lib.check(_lib.load().eld_unet_input_grad(ctx.eng, net._flat.data_ptr(), dx.data_ptr(), _st()),
+                       'eld_unet_input_grad')
         grads, off = [], 0
         for p in net.parameters():
             k = p.numel()
             grads.append(g[off:off + k].view(p.shape))
             off += k
-        return (None, None) + tuple(grads)       # no gradient wrt the input frame (the reference never asks for one)
+        return (None, dx) + tuple(grads)
 
 
 class UNetSeeInDark(nn.Module):
     """H100-native UNetSeeInDark(in_channels, out_channels) for 4-channel packed raw and 3-channel sRGB frames on either
     side (ELD_model.py:377-389: --stage_in / --stage_out raw | srgb with --channels 4)."""
+
+    _warned_detached = False   # set on the first frame that requires grad at a shape the training tiles reject
 
     def __init__(self, in_channels=4, out_channels=4):
         super().__init__()
@@ -158,14 +168,20 @@ class UNetSeeInDark(nn.Module):
         return self._engines[key][0]
 
     def forward(self, x):
-        """x: cuda float32 NCHW [n,4,h,w] -> float32 NCHW [n,4,h,w].  Under torch.enable_grad() in training mode the call
-        is an autograd node (`_EngineFunction`: shapes the training tiles accept, H % 128 == 0 and W % 256 == 0);
-        otherwise plain inference."""
+        """x: cuda float32 NCHW [n,4,h,w] -> float32 NCHW [n,4,h,w].  Under torch.enable_grad(), in training mode or when
+        x requires grad (in eval mode too: the network has no batch norm or dropout), the call is an autograd node
+        (`_EngineFunction`) at the shapes the training tiles accept, H % 128 == 0 and W % 256 == 0; otherwise plain
+        inference, whose output is detached (a frame that requires grad gets a one-time warning then)."""
         assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == self.in_channels
         x = x.contiguous()
         n, _, h, w = x.shape
-        if self.training and torch.is_grad_enabled() and h % 128 == 0 and w % 256 == 0:
-            return _EngineFunction.apply(self, x, *self.parameters())
+        if torch.is_grad_enabled() and (self.training or x.requires_grad):
+            if h % 128 == 0 and w % 256 == 0:
+                return _EngineFunction.apply(self, x, *self.parameters())
+            if x.requires_grad and not self._warned_detached:
+                self._warned_detached = True
+                warnings.warn('UNetSeeInDark: back-propagation needs H %% 128 == 0 and W %% 256 == 0; this %d x %d frame '
+                              'runs inference and its output is detached, so x gets no gradient' % (h, w), stacklevel=2)
         out = torch.empty((n, self.out_channels, h, w), dtype=torch.float32, device=x.device)
         _lib.check(_lib.load().eld_unet_forward(self._engine(n, h, w, False), self._flat.data_ptr(), x.data_ptr(),
                                                out.data_ptr(), _st()), 'eld_unet_forward')

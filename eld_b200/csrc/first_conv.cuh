@@ -1,4 +1,5 @@
-// first_conv.cuh - conv1_1 (4 -> 32 channels, 3x3, Unet.py:11) fprop and wgrad as wgmma tiles fed by a SOFTWARE im2col.
+// first_conv.cuh - conv1_1 (4 -> 32 channels, 3x3, Unet.py:11) fprop and wgrad as wgmma tiles fed by a SOFTWARE im2col,
+// and its data gradient (the gradient of the input frame; see first_conv_dgrad_kernel at the end).
 //
 // The generic conv tile needs >= 32 input channels (one 64-byte TMA row per pixel); conv1_1 has 4.  Instead of a
 // zero-padded 32-channel copy of the input (a pack pass, and 7/8 of the MMAs multiplying zeros), one thread per pixel
@@ -31,6 +32,8 @@ struct FirstConvParams {
                                 // LeakyReLU' mask conv1_2's data gradient needs (conv_umma.cuh aux_sign)
     float* dw;                  // wgrad: f32 OIHW [32][4][3][3], accumulated into
     float* db;                  // wgrad: f32 [32]
+    const float* w;             // dgrad: the f32 master weights, OIHW [32][cin][3][3]
+    float* dx;                  // dgrad: f32 NCHW [n][cin][H][W], overwritten
 };
 
 // Two warpgroups per CTA take alternate tiles; inside a warpgroup one thread per pixel builds the im2col row, one
@@ -237,6 +240,117 @@ first_conv_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
                     }
                 }
         }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// DGRAD: dx[c][y][x] = sum_{co, kh, kw} dZ[y + 1 - kh][x + 1 - kw][co] * W[co][c][kh][kw]   (d loss / d frame)
+//
+// Here the A operand needs no im2col: dZ (conv1_1's pre-activation gradient, bf16 NHWC, 32 channels) is one 64-byte SW64
+// row per pixel, and K = 9 taps x 32 channels.  Per 8 x 16 pixel tile the producer loads three TMA boxes
+// {32 ch, 16 px, 10 rows}, one per column shift -1 / 0 / +1, each with a one-row halo above and below; out-of-image
+// elements are zero-filled, which is the transposed padding.  A row shift is then 16 pixel rows = 1 KB inside a box,
+// whole 8-row swizzle atoms, so each of the nine taps is a descriptor offset, and a tile moves 30 KB instead of nine
+// 8 KB boxes.  B = the weights in the dgrad arrangement [tap][8 rows = c, zero for c >= cin][32 co] (taps flipped), bf16
+// SW64, built once per CTA from the fp32 master weights.  wgmma m64n8k16: N = cin padded to 8.
+// The wgmma tile of conv_umma.cuh is not reused: it bulk-loads B per stage and ends in a 32-column bf16 epilogue
+// (bias, masks, pool, sign words); an N = 8 fp32 NCHW store would make both halves branch on this one caller.
+// Warpgroup 0 is the TMA producer (one thread); warpgroups 1 and 2 take pixel rows 0-63 / 64-127 of every tile and store
+// their fragments straight to the fp32 planes: per store instruction a warp writes 8 consecutive pixels of one plane
+// per lane quad position (full 32-byte sectors).
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int kDgThreads = 384;
+constexpr int kDgBox = 10 * 16 * 64;      // one {32 ch, 16, 10} box of dZ: 10 KB
+constexpr int kDgStage = 3 * kDgBox;      // the three column shifts of one tile
+constexpr int kDgStages = 6;
+constexpr int kDgB = 9 * 8 * 64;          // B image: [tap][8 rows][32 co] bf16
+
+__global__ void __launch_bounds__(kDgThreads, 1)
+first_conv_dgrad_kernel(const __grid_constant__ CUtensorMap tmZ, const FirstConvParams p)
+{
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t raw = ptx::smem_u32(smem_raw);
+    uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
+    uint8_t* b_s = smem + kDgStages * kDgStage;
+    uint64_t* full = reinterpret_cast<uint64_t*>(b_s + kDgB);
+    uint64_t* empty = full + kDgStages;
+    const int total_tiles = p.n_img * p.tiles_x * p.tiles_y;
+
+    if (threadIdx.x == 0) {
+        ptx::prefetch_tmap(&tmZ);
+        for (int s = 0; s < kDgStages; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 8); }
+        ptx::fence_barrier_init();
+    }
+    ptx::grid_dep_wait();          // PDL: dZ and the weights are final past this point
+    ptx::grid_dep_launch();
+    // B[tap][c][co] = bf16(W[co][c][8 - tap]): tap t of A is the shift (t / 3 - 1, t % 3 - 1), i.e. kh = 2 - t / 3, kw = 2 - t % 3
+    for (int i = threadIdx.x; i < 9 * 8 * 32; i += kDgThreads) {
+        const int tap = i >> 8, c = (i >> 5) & 7, co = i & 31;
+        const float v = c < p.cin ? __ldg(p.w + (co * p.cin + c) * 9 + (8 - tap)) : 0.0f;
+        const int byte = tap * 512 + c * 64 + ((((co >> 3) ^ ((c >> 1) & 3)) << 4) | ((co & 7) << 1));
+        *reinterpret_cast<__nv_bfloat16*>(b_s + byte) = __float2bfloat16_rn(v);
+    }
+    ptx::fence_proxy_async();      // generic-proxy stores -> visible to wgmma's operand reads
+    __syncthreads();
+
+    if (threadIdx.x < 128) {
+        // ===================== TMA producer (warpgroup 0; one thread works) =====================
+        if (threadIdx.x == 0) {
+            int s = 0;
+            uint32_t ph = 0;
+            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+                int img, y0, x0;
+                fc_tile_coords(p, tile, img, y0, x0);
+                ptx::mbar_wait(&empty[s], ph ^ 1u);
+                uint8_t* sa = smem + (size_t)s * kDgStage;
+                ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)kDgStage);
+                for (int b = 0; b < 3; ++b) ptx::tma_load_5d(sa + b * kDgBox, &tmZ, &full[s], 0, x0 + b - 1, y0 - 1, img, 0);
+                if (++s == kDgStages) { s = 0; ph ^= 1u; }
+            }
+        }
+        return;
+    }
+
+    // ===================== consumers: warpgroup cg = 0 / 1 owns pixel rows 64 cg .. 64 cg + 63 =====================
+    const int cg = (threadIdx.x >> 7) - 1;
+    const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+    const uint64_t desc0 = ptx::make_gmma_desc(0, 16, 512, ptx::GMMA_SW64);
+    const uint64_t bd0 = desc0 | (uint64_t)((ptx::smem_u32(b_s) & 0x3FFFFu) >> 4);
+    const uint32_t a0 = ptx::smem_u32(smem) + (uint32_t)(cg * 64 * 64);
+    const size_t plane = (size_t)p.H * p.W;
+    const int c0 = 2 * (lane & 3);                 // this lane's accumulator columns: input channels c0, c0 + 1
+    int s = 0;
+    uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        float acc[4] = { 0.f, 0.f, 0.f, 0.f };
+        ptx::mbar_wait(&full[s], ph);
+        const uint32_t sa = a0 + (uint32_t)(s * kDgStage);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap) {
+            const int ty = tap / 3, tx = tap - 3 * ty;     // box tx, 16 ty pixel rows down
+            const uint64_t ad = desc0 | (uint64_t)(((sa + (uint32_t)(tx * kDgBox + ty * 16 * 64)) & 0x3FFFFu) >> 4);
+            const uint64_t bd = bd0 + (uint64_t)((tap * 512) >> 4);
+#pragma unroll
+            for (int k = 0; k < 2; ++k)                    // +32 bytes along K inside the swizzle atom
+                ptx::wgmma_m64n8k16<0, 0>(acc, ad + 2u * k, bd + 2u * k, 1u);
+        }
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        ptx::reg_fence(acc);
+        if (lane == 0) ptx::mbar_arrive(&empty[s]);
+        if (++s == kDgStages) { s = 0; ph ^= 1u; }
+
+        // ---- epilogue: acc[2i + j] = D[pixel row 16 wq + lane / 4 + 8 i][column c0 + j] ----
+        int img, y0, x0;
+        fc_tile_coords(p, tile, img, y0, x0);
+        const int m = cg * 64 + 16 * wq + (lane >> 2);
+        float* dst = p.dx + (size_t)img * p.cin * plane + (size_t)(y0 + (m >> 4)) * p.W + (x0 + (m & 15));
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int j = 0; j < 2; ++j)
+                if (c0 + j < p.cin) dst[(size_t)(c0 + j) * plane + 8 * i] = acc[2 * i + j];
     }
 }
 

@@ -127,6 +127,15 @@ __device__ __forceinline__ void reg_fence(float (&d)[R])
 // TA / TB: 0 = K-major, 1 = MN-major.  scale_d == 0 overwrites D.
 // Fragment layout: warp w, lane l holds d[4j + 2i + c] = D[16w + l/4 + 8i][8j + 2(l%4) + c].
 template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n8k16(float (&d)[4], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0,%1,%2,%3}, %4, %5, p, 1, 1, %7, %8;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB) : "memory");
+}
+template <int TA, int TB>
 __device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d)
 {
     asm volatile(

@@ -238,6 +238,7 @@ struct eld_unet {
     cudaEvent_t bucket_ev[kGradBuckets] = { nullptr, nullptr, nullptr, nullptr };
     int cin0 = 4, cout_last = 4; // channels of the frame in / out: 4 = packed raw, 3 = sRGB (ELD_model.py:377-389)
     int l2_loss = 0;             // 0: nn.L1Loss (the reference default, losses.py:31-32), 1: nn.MSELoss (losses.py:33-34)
+    bool dz1_1_final = false;    // dz1_1 holds the last backward's conv1_1 gradient: set by a backward, cleared by a forward
     // optional per-launch profile (CUDA events on the launch stream)
     bool profile = false;
     struct Rec { char name[32]; double flops, bytes; cudaEvent_t e0, e1; };
@@ -744,6 +745,7 @@ struct Runner {
 extern "C" int eld_unet_forward(eld_unet* u, const float* params, const float* x, float* out, void* stream)
 {
     ELD_REQUIRE(u && params && x && out, "eld_unet_forward: NULL argument");
+    u->dz1_1_final = false;
     ELD_CHECK_CUDA(cudaSetDevice(u->ctx->device));
     Runner r{ u, params, static_cast<cudaStream_t>(stream) };
     TRY(r.forward(x));
@@ -758,6 +760,7 @@ extern "C" int eld_unet_train_step(eld_unet* u, const float* params, const float
 {
     ELD_REQUIRE(u && params && x && target && out && grads && loss, "eld_unet_train_step: NULL argument");
     ELD_REQUIRE(u->dz9_2 != nullptr, "eld_unet_train_step: the eld_unet was created with train = 0");
+    u->dz1_1_final = false;
     ELD_CHECK_CUDA(cudaSetDevice(u->ctx->device));
     Runner r{ u, params, static_cast<cudaStream_t>(stream) };
     ELD_CHECK_CUDA(cudaMemsetAsync(grads, 0, u->n_params * sizeof(float), r.st));
@@ -770,7 +773,9 @@ extern "C" int eld_unet_train_step(eld_unet* u, const float* params, const float
         TRY(launch_head(u->ctx, u->a9_2, params + u->L[I_C10].w_off, params + u->L[I_C10].b_off, out, target, u->dz9_2,
                         grads + u->L[I_C10].w_off, grads + u->L[I_C10].b_off, loss, u->n, (size_t)u->H * u->W, u->cout_last, u->l2_loss, r.st));
     }
-    return r.backward(x, grads);
+    TRY(r.backward(x, grads));
+    u->dz1_1_final = true;
+    return ELD_OK;
 }
 
 extern "C" int eld_unet_backward(eld_unet* u, const float* params, const float* x, const float* dout, float* grads, void* stream)
@@ -789,7 +794,21 @@ extern "C" int eld_unet_backward(eld_unet* u, const float* params, const float* 
                         reinterpret_cast<float*>(u->dz1_1), dout, u->dz9_2,
                         grads + u->L[I_C10].w_off, grads + u->L[I_C10].b_off, nullptr, u->n, (size_t)u->H * u->W, u->cout_last, 2, r.st));
     }
-    return r.backward(x, grads);
+    TRY(r.backward(x, grads));
+    u->dz1_1_final = true;
+    return ELD_OK;
+}
+
+extern "C" int eld_unet_input_grad(eld_unet* u, const float* params, float* dx, void* stream)
+{
+    ELD_REQUIRE(u && params && dx, "eld_unet_input_grad: NULL argument");
+    ELD_REQUIRE(u->dz9_2 != nullptr, "eld_unet_input_grad: the eld_unet was created with train = 0");
+    ELD_REQUIRE(u->dz1_1_final, "eld_unet_input_grad: no eld_unet_backward or eld_unet_train_step since the last forward");
+    ELD_CHECK_CUDA(cudaSetDevice(u->ctx->device));
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const double px = (double)u->n * u->H * u->W;
+    Scope sc(u, st, "conv1_1", "dgrad", 2.0 * px * 32 * 9 * u->cin0, px * (64 + 4 * u->cin0));
+    return launch_first_conv_dgrad(u->ctx, u->dz1_1, params + u->L[I_C11].w_off, u->cin0, dx, u->n, u->H, u->W, st);
 }
 
 extern "C" int eld_adam_step(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, size_t n,

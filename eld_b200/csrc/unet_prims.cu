@@ -190,9 +190,35 @@ int launch_first_conv_wgrad(eld_ctx* ctx, const float* x, int cin, const void* d
     return ELD_OK;
 }
 
+// align slack, the TMA ring, the B image, full / empty barriers
+static size_t first_conv_dgrad_smem() { return 1024 + kDgStages * kDgStage + kDgB + 2 * kDgStages * 8; }
+
+int launch_first_conv_dgrad(eld_ctx* ctx, const void* dz, const float* w, int cin, float* dx, int n, int H, int W,
+                            cudaStream_t st)
+{
+    ELD_REQUIRE(H % 8 == 0 && W % 16 == 0, "first conv dgrad tile: H=%d must be a multiple of 8 and W=%d of 16", H, W);
+    ELD_REQUIRE(cin >= 1 && cin <= 8, "first conv dgrad tile: cin=%d must be 1..8 (wgmma N = 8)", cin);
+    FirstConvParams p{};
+    p.n_img = n; p.H = H; p.W = W; p.tiles_x = W / 16; p.tiles_y = H / 8; p.cin = cin;
+    p.w = w; p.dx = dx;
+    CUtensorMap tmZ;
+    const cuuint64_t eb = 2;
+    cuuint64_t dims[5] = { 32, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n, 1 };
+    cuuint64_t str[4] = { 32 * eb, (cuuint64_t)W * 32 * eb, (cuuint64_t)H * W * 32 * eb, (cuuint64_t)n * H * W * 32 * eb };
+    cuuint32_t box[5] = { 32, 16, 10, 1, 1 };
+    { int rc = encode(ctx, &tmZ, dz, 5, dims, str, box, 64); if (rc) return rc; }
+    const int total = n * p.tiles_x * p.tiles_y;
+    const int grid = total < ctx->num_sms ? total : ctx->num_sms;
+    ELD_CHECK_CUDA(launch_pdl(first_conv_dgrad_kernel, grid, kDgThreads, first_conv_dgrad_smem(), st, tmZ, p));
+    ELD_CHECK_CUDA(cudaGetLastError());
+    count_launch(ctx);
+    return ELD_OK;
+}
+
 int init_gemm_kernels(eld_ctx* ctx)
 {
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(first_conv_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_conv_dgrad_smem()));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(first_conv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_conv_smem(false)));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(first_conv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_conv_smem(true)));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));

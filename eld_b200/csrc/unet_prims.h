@@ -69,6 +69,9 @@ int launch_first_conv(eld_ctx* ctx, const float* x, int cin, const void* w_img, 
                       int n, int H, int W, cudaStream_t st, void* sign_out = nullptr);
 int launch_first_conv_wgrad(eld_ctx* ctx, const float* x, int cin, const void* dz, int dz_pitch, float* dw, float* db,
                             int n, int H, int W, cudaStream_t st);
+// conv1_1's data gradient: dz bf16 NHWC [n][H][W][32], w f32 OIHW [32][cin][3][3] -> dx f32 NCHW [n][cin][H][W]
+int launch_first_conv_dgrad(eld_ctx* ctx, const void* dz, const float* w, int cin, float* dx, int n, int H, int W,
+                            cudaStream_t st);
 int launch_pack_weights(eld_ctx* ctx, const float* w, void* out, int cout, int cin, int kind, cudaStream_t st);
 
 }  // namespace eld

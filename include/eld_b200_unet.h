@@ -87,8 +87,13 @@ int    eld_unet_train_step(eld_unet* u, const float* params, const float* x, con
                            float* out, float* grads, float* loss, void* stream);
 /* The autograd seam (ELDModel.backward_G, ELD_model.py:411-420: `loss.backward()` through netG): after an
  * eld_unet_forward on a train = 1 object (activations stay in the workspace), back-propagate the caller's
- * dout = d(loss)/d(out) (f32 NCHW) into `grads` (zeroed and filled, like eld_unet_train_step).  Any loss the caller likes. */
+ * dout = d(loss)/d(out) (f32 NCHW) into `grads` (zeroed and filled, like eld_unet_train_step).  Any loss the caller likes.
+ * The gradient of the input frame is not computed here; eld_unet_input_grad gives it on request. */
 int    eld_unet_backward(eld_unet* u, const float* params, const float* x, const float* dout, float* grads, void* stream);
+/* d(loss)/d(x) of the last eld_unet_backward / eld_unet_train_step on this object, stream-ordered after it:
+ * dx f32 NCHW [n][cin][h][w], overwritten.  bf16 conv1_1 gradient and weights, fp32 accumulation.  Fails on an object
+ * created with train = 0 and when no backward or train step has run since the last forward. */
+int    eld_unet_input_grad(eld_unet* u, const float* params, float* dx, void* stream);
 /* Pixel loss of eld_unet_train_step (models/losses.py:29-36, --loss): 0 = nn.L1Loss (default), 1 = nn.MSELoss. */
 #define ELD_LOSS_L1 0
 #define ELD_LOSS_L2 1
