@@ -227,20 +227,6 @@ class UNetSeeInDark(nn.Module):
             self._ddp_ready = eng.value
             self._ddp_stream = torch.cuda.Stream(device=x.device)
             self._ddp_buckets = self.grad_buckets()
-            if group is None and getattr(self, '_ddp_group', None) is None:
-                # A communicator of its own for the gradient exchange, limited to a few CTAs: the all-reduce kernels run
-                # UNDER the persistent one-CTA-per-SM tiles, and every SM they occupy delays a tile kernel's slowest CTA.
-                # The exchange is hidden behind backward, so its own speed is worth less than the SMs it leaves alone.
-                import os
-                ctas = int(os.environ.get('ELD_NCCL_MAX_CTAS', '0'))
-                self._ddp_group = False
-                if ctas > 0:
-                    opts = dist.ProcessGroupNCCL.Options()
-                    opts.config.max_ctas = ctas
-                    opts.config.min_ctas = min(ctas, 4)
-                    self._ddp_group = dist.new_group(pg_options=opts)
-        if group is None and getattr(self, '_ddp_group', None):
-            group = self._ddp_group
         ev = (lambda: torch.cuda.Event(enable_timing=True)) if timeline is not None else None
         if ev:
             timeline['step_start'] = ev(); timeline['step_start'].record()

@@ -51,17 +51,16 @@ namespace eld {
 inline void count_launch(eld_ctx* ctx, int n = 1) { ctx->launches.fetch_add(n, std::memory_order_relaxed); }
 
 // Launch with programmatic stream serialization (PDL): the kernel may start while its predecessor drains; it blocks in
-// griddepcontrol.wait before touching anything the predecessor writes.  ELD_NO_PDL=1 restores plain launches.
+// griddepcontrol.wait before touching anything the predecessor writes.
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), int grid, int block, size_t smem, cudaStream_t st, Args... args)
 {
-    static const bool no_pdl = getenv("ELD_NO_PDL") != nullptr;
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3((unsigned)block); cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = no_pdl ? 0 : 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 

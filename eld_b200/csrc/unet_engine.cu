@@ -491,11 +491,9 @@ struct Runner {
     const __nv_bfloat16* wd(int i) const { return u->packed + u->L[i].wd_off; }
     const float* bias(int i) const { return params + u->L[i].b_off; }
 
-    // sign words of activation `act` (training engines; ELD_MASK_FROM_ACT=1 keeps the masks that re-read the activations: A/B)
+    // sign words of activation `act`, or nullptr: an inference engine keeps none, and a9_2's LeakyReLU' is the head's
     uint32_t* sign_of(const void* act) const
     {
-        static const bool off = getenv("ELD_MASK_FROM_ACT") != nullptr;
-        if (off || !u->dz9_2) return nullptr;
         for (int i = 0; i < u->n_signs; ++i) if (u->signs[i].act == act) return u->signs[i].words;
         return nullptr;
     }
@@ -526,12 +524,12 @@ struct Runner {
         Scope sc(u, st, l.name, "fprop", 2.0 * px * 4 * l.cout * l.cin, px * 2 * (l.cin + 4 * l.cout) + 8.0 * l.cin * l.cout);
         return launch_conv_gemm(ctx(), op, st);
     }
-    // data gradient of a conv: dz [cout] -> d(input) [cin channels at dxc0], optional lrelu' mask from `act_src`
+    // data gradient of a conv: dz [cout] -> d(input) [cin channels at dxc0], optional lrelu' mask from the sign words of
+    // activation `act_src`
     // dx2 != nullptr: the gradient of a concat input is stored as two PLANAR halves (dx = [up], dx2 = [skip], pitch cin/2
     // each) - every consumer reads exactly one half, and an interleaved buffer made each of them move whole 128-byte
     // lines for 64 useful bytes (ncu r01: level-1 pool.bwd 570 MB for 300, upv9 dgrad/wgrad 336 MB for 200)
-    int conv_dgrad(int li, const void* dz, void* dx, int dxp, int dxc0, const void* act_src, int asp, int asc0, int lvl,
-                   void* dx2 = nullptr) const
+    int conv_dgrad(int li, const void* dz, void* dx, int dxp, int dxc0, const void* act_src, int lvl, void* dx2 = nullptr) const
     {
         const Layer& l = u->L[li];
         GemmOp op{};
@@ -541,8 +539,8 @@ struct Runner {
         op.epi_mode = EPI_STORE; op.act = act_src ? ACT_MASK : ACT_NONE;
         op.out = dx; op.out_pitch = dxp; op.out_c0 = dxc0; op.bias = nullptr;
         if (dx2) { op.out2 = dx2; op.out2_pitch = dxp; op.out_split = l.cin / 2; }
-        op.aux = act_src; op.aux_pitch = asp; op.aux_c0 = asc0;
-        if (act_src && asc0 == 0 && asp == l.cin) op.aux_sign = sign_of(act_src);
+        op.aux_sign = act_src ? sign_of(act_src) : nullptr;
+        ELD_REQUIRE(!act_src || op.aux_sign, "eld_unet: %s dgrad: no sign words for its LeakyReLU' mask", l.name);
         const double px = (double)u->n * op.H * op.W;
         Scope sc(u, st, l.name, "dgrad", 2.0 * px * l.cout * 9 * l.cin, px * 2 * (l.cin * (act_src ? 2 : 1) + l.cout) + 18.0 * l.cin * l.cout);
         return launch_conv_gemm(ctx(), op, st);
@@ -555,7 +553,8 @@ struct Runner {
         op.n_img = u->n; op.H = u->H >> lvl_in; op.W = u->W >> lvl_in;
         op.b = wd(li); op.n_total = l.cin; op.cout = l.cin;
         op.epi_mode = EPI_STORE; op.act = ACT_MASK; op.out = dx; op.out_pitch = l.cin; op.out_c0 = 0;
-        op.aux = act_src; op.aux_pitch = l.cin; op.aux_c0 = 0; op.aux_sign = sign_of(act_src);
+        op.aux_sign = sign_of(act_src);
+        ELD_REQUIRE(op.aux_sign, "eld_unet: %s dgrad: no sign words for its LeakyReLU' mask", l.name);
         const double px = (double)u->n * op.H * op.W;
         Scope sc(u, st, l.name, "dgrad", 2.0 * px * 4 * l.cout * l.cin, px * 2 * (2 * l.cin + 4 * l.cout) + 8.0 * l.cin * l.cout);
         return launch_conv_gemm(ctx(), op, st);
@@ -580,31 +579,18 @@ struct Runner {
         op.mode = WG_DECONV; op.p = dy; op.p_pitch = dyp; op.p_c0 = 0; op.p_ch = l.cout;
         op.q = x; op.q_pitch = l.cin; op.q_c0 = 0; op.q_ch = l.cin;
         op.n_img = u->n; op.H = u->H >> lvl_in; op.W = u->W >> lvl_in; op.dw = grads + l.w_off;
-        static const bool fuse_bias = getenv("ELD_DECONV_COLSUM") == nullptr;    // (A/B: the stand-alone column-sum kernel)
-        op.db = fuse_bias ? grads + l.b_off : nullptr;           // bias gradient = column sums of the d(up) boxes, same launch
+        op.db = grads + l.b_off;                     // bias gradient = column sums of the d(up) boxes, same launch
         const double px = (double)u->n * op.H * op.W;
-        {
-            Scope sc(u, st, l.name, "wgrad", 2.0 * px * 4 * l.cout * l.cin, px * 2 * (l.cin + 4 * l.cout) + 16.0 * l.cin * l.cout);
-            TRY(launch_wgrad(ctx(), op, st));
-        }
-        if (fuse_bias) return ELD_OK;
-        Scope sc(u, st, l.name, "bgrad", 0.0, px * 8 * l.cout);
-        return launch_colsum(ctx(), dy, dyp, 0, l.cout, (size_t)u->n * op.H * op.W * 4, grads + l.b_off, st);
+        Scope sc(u, st, l.name, "wgrad", 2.0 * px * 4 * l.cout * l.cin, px * 2 * (l.cin + 4 * l.cout) + 16.0 * l.cin * l.cout);
+        return launch_wgrad(ctx(), op, st);
     }
-    int pool(const void* in, int pitch, int c0, void* out, int C, int lvl_out) const
+    // from the argmax + sign code the forward tile left (the activation is not read again); dskip = the PLANAR skip half
+    // of the concat gradient
+    int pool_bwd(const void* code, const void* dskip, const void* dP, void* dZ, int C, int lvl_out) const
     {
         const double pxo = (double)u->n * (u->H >> lvl_out) * (u->W >> lvl_out);
-        Scope sc(u, st, "pool", "fwd", 0.0, pxo * C * 2 * 5);
-        return launch_maxpool(ctx(), in, pitch, c0, out, C, u->n, u->H >> lvl_out, u->W >> lvl_out, st);
-    }
-    // A = the interleaved concat buffer's skip half (pitch 2C, offset C); dskip = the PLANAR skip half of its gradient
-    // code != nullptr: the forward tile left the argmax + sign code, the activation is not read again
-    int pool_bwd(const void* A, int pitch, int c0, const void* dskip, const void* dP, void* dZ, int C, int lvl_out, const void* code) const
-    {
-        const double pxo = (double)u->n * (u->H >> lvl_out) * (u->W >> lvl_out);
-        Scope sc(u, st, "pool", "bwd", 0.0, pxo * C * (code ? 2 * 9 + 1 : 2 * 13));
-        if (code) return launch_maxpool_bwd_code(ctx(), code, dskip, C, 0, dP, dZ, C, u->n, u->H >> lvl_out, u->W >> lvl_out, st);
-        return launch_maxpool_bwd(ctx(), A, pitch, c0, dskip, C, 0, dP, dZ, C, u->n, u->H >> lvl_out, u->W >> lvl_out, st);
+        Scope sc(u, st, "pool", "bwd", 0.0, pxo * C * (2 * 9 + 1));
+        return launch_maxpool_bwd_code(ctx(), code, dskip, C, 0, dP, dZ, C, u->n, u->H >> lvl_out, u->W >> lvl_out, st);
     }
     // second (skip) half of a planar concat gradient: [n][h][w][C] right behind the up half
     __nv_bfloat16* skip_half(__nv_bfloat16* dcat, int lvl, int C) const
@@ -648,7 +634,6 @@ struct Runner {
     int forward(const float* x) const
     {
         eld_unet* U = u;
-        static const bool fuse_pool = getenv("ELD_NO_FUSED_POOL") == nullptr;   // (A/B: the stand-alone pool kernel)
         TRY(pack());
         {
             // conv1_1 (4 -> 32): software-im2col tile straight from the fp32 NCHW frame (first_conv.cuh)
@@ -656,13 +641,13 @@ struct Runner {
             Scope sc(u, st, "conv1_1", "fprop", 2.0 * px * 32 * 9 * U->cin0, px * (4 * U->cin0 + 64));
             TRY(launch_first_conv(ctx(), x, U->cin0, wf(I_C11), bias(I_C11), U->a1_1, 32, U->n, U->H, U->W, st, sign_of(U->a1_1)));
         }
-        if (fuse_pool) { TRY(conv(I_C12, U->a1_1, 32, 0, U->cat9, 64, 32, 0, U->p1, U->pc1)); } else { TRY(conv(I_C12, U->a1_1, 32, 0, U->cat9, 64, 32, 0)); TRY(pool(U->cat9, 64, 32, U->p1, 32, 1)); }      // + pool (Unet.py:51)
+        TRY(conv(I_C12, U->a1_1, 32, 0, U->cat9, 64, 32, 0, U->p1, U->pc1));       // + pool (Unet.py:51)
         TRY(conv(I_C21, U->p1, 32, 0, U->a2_1, 64, 0, 1));
-        if (fuse_pool) { TRY(conv(I_C22, U->a2_1, 64, 0, U->cat8, 128, 64, 1, U->p2, U->pc2)); } else { TRY(conv(I_C22, U->a2_1, 64, 0, U->cat8, 128, 64, 1)); TRY(pool(U->cat8, 128, 64, U->p2, 64, 2)); }     // + pool (Unet.py:55)
+        TRY(conv(I_C22, U->a2_1, 64, 0, U->cat8, 128, 64, 1, U->p2, U->pc2));      // + pool (Unet.py:55)
         TRY(conv(I_C31, U->p2, 64, 0, U->a3_1, 128, 0, 2));
-        if (fuse_pool) { TRY(conv(I_C32, U->a3_1, 128, 0, U->cat7, 256, 128, 2, U->p3, U->pc3)); } else { TRY(conv(I_C32, U->a3_1, 128, 0, U->cat7, 256, 128, 2)); TRY(pool(U->cat7, 256, 128, U->p3, 128, 3)); }   // + pool (Unet.py:59)
+        TRY(conv(I_C32, U->a3_1, 128, 0, U->cat7, 256, 128, 2, U->p3, U->pc3));    // + pool (Unet.py:59)
         TRY(conv(I_C41, U->p3, 128, 0, U->a4_1, 256, 0, 3));
-        if (fuse_pool) { TRY(conv(I_C42, U->a4_1, 256, 0, U->cat6, 512, 256, 3, U->p4, U->pc4)); } else { TRY(conv(I_C42, U->a4_1, 256, 0, U->cat6, 512, 256, 3)); TRY(pool(U->cat6, 512, 256, U->p4, 256, 4)); }   // + pool (Unet.py:63)
+        TRY(conv(I_C42, U->a4_1, 256, 0, U->cat6, 512, 256, 3, U->p4, U->pc4));    // + pool (Unet.py:63)
         TRY(conv(I_C51, U->p4, 256, 0, U->a5_1, 512, 0, 4));
         TRY(conv(I_C52, U->a5_1, 512, 0, U->a5_2, 512, 0, 4));
         TRY(deconv(I_UP6, U->a5_2, 512, U->cat6, 512, 4));
@@ -679,58 +664,56 @@ struct Runner {
     int backward(const float* x, float* g) const
     {
         eld_unet* U = u;
-        // the fused pools leave their codes; ELD_POOL_BWD_FROM_ACT=1 keeps the backward that re-reads the activations (A/B)
-        static const bool coded = getenv("ELD_NO_FUSED_POOL") == nullptr && getenv("ELD_POOL_BWD_FROM_ACT") == nullptr;
         TRY(conv_wgrad(I_C92, U->a9_1, 32, 0, U->dz9_2, g, 0));
-        TRY(conv_dgrad(I_C92, U->dz9_2, U->dz9_1, 32, 0, U->a9_1, 32, 0, 0));
+        TRY(conv_dgrad(I_C92, U->dz9_2, U->dz9_1, 32, 0, U->a9_1, 0));
         TRY(conv_wgrad(I_C91, U->cat9, 64, 0, U->dz9_1, g, 0));
-        TRY(conv_dgrad(I_C91, U->dz9_1, U->dcat9, 32, 0, nullptr, 0, 0, 0, skip_half(U->dcat9, 0, 32)));
+        TRY(conv_dgrad(I_C91, U->dz9_1, U->dcat9, 32, 0, nullptr, 0, skip_half(U->dcat9, 0, 32)));
         TRY(deconv_wgrad(I_UP9, U->a8_2, U->dcat9, 32, g, 1));
         TRY(deconv_dgrad(I_UP9, U->dcat9, 32, U->dz8_2, U->a8_2, 1));
         TRY(conv_wgrad(I_C82, U->a8_1, 64, 0, U->dz8_2, g, 1));
-        TRY(conv_dgrad(I_C82, U->dz8_2, U->dz8_1, 64, 0, U->a8_1, 64, 0, 1));
+        TRY(conv_dgrad(I_C82, U->dz8_2, U->dz8_1, 64, 0, U->a8_1, 1));
         TRY(conv_wgrad(I_C81, U->cat8, 128, 0, U->dz8_1, g, 1));
-        TRY(conv_dgrad(I_C81, U->dz8_1, U->dcat8, 64, 0, nullptr, 0, 0, 1, skip_half(U->dcat8, 1, 64)));
+        TRY(conv_dgrad(I_C81, U->dz8_1, U->dcat8, 64, 0, nullptr, 1, skip_half(U->dcat8, 1, 64)));
         TRY(deconv_wgrad(I_UP8, U->a7_2, U->dcat8, 64, g, 2));
         TRY(deconv_dgrad(I_UP8, U->dcat8, 64, U->dz7_2, U->a7_2, 2));
         TRY(conv_wgrad(I_C72, U->a7_1, 128, 0, U->dz7_2, g, 2));
-        TRY(conv_dgrad(I_C72, U->dz7_2, U->dz7_1, 128, 0, U->a7_1, 128, 0, 2));
+        TRY(conv_dgrad(I_C72, U->dz7_2, U->dz7_1, 128, 0, U->a7_1, 2));
         TRY(conv_wgrad(I_C71, U->cat7, 256, 0, U->dz7_1, g, 2));
-        TRY(conv_dgrad(I_C71, U->dz7_1, U->dcat7, 128, 0, nullptr, 0, 0, 2, skip_half(U->dcat7, 2, 128)));
+        TRY(conv_dgrad(I_C71, U->dz7_1, U->dcat7, 128, 0, nullptr, 2, skip_half(U->dcat7, 2, 128)));
         TRY(deconv_wgrad(I_UP7, U->a6_2, U->dcat7, 128, g, 3));
         TRY(deconv_dgrad(I_UP7, U->dcat7, 128, U->dz6_2, U->a6_2, 3));
         TRY(conv_wgrad(I_C62, U->a6_1, 256, 0, U->dz6_2, g, 3));
-        TRY(conv_dgrad(I_C62, U->dz6_2, U->dz6_1, 256, 0, U->a6_1, 256, 0, 3));
+        TRY(conv_dgrad(I_C62, U->dz6_2, U->dz6_1, 256, 0, U->a6_1, 3));
         TRY(conv_wgrad(I_C61, U->cat6, 512, 0, U->dz6_1, g, 3));
-        TRY(conv_dgrad(I_C61, U->dz6_1, U->dcat6, 256, 0, nullptr, 0, 0, 3, skip_half(U->dcat6, 3, 256)));
+        TRY(conv_dgrad(I_C61, U->dz6_1, U->dcat6, 256, 0, nullptr, 3, skip_half(U->dcat6, 3, 256)));
         TRY(deconv_wgrad(I_UP6, U->a5_2, U->dcat6, 256, g, 4));
         TRY(finish_bucket(0, g));
         TRY(deconv_dgrad(I_UP6, U->dcat6, 256, U->dz5_2, U->a5_2, 4));
         // bottleneck + encoder
         TRY(conv_wgrad(I_C52, U->a5_1, 512, 0, U->dz5_2, g, 4));
-        TRY(conv_dgrad(I_C52, U->dz5_2, U->dz5_1, 512, 0, U->a5_1, 512, 0, 4));
+        TRY(conv_dgrad(I_C52, U->dz5_2, U->dz5_1, 512, 0, U->a5_1, 4));
         TRY(conv_wgrad(I_C51, U->p4, 256, 0, U->dz5_1, g, 4));
         TRY(finish_bucket(1, g));
-        TRY(conv_dgrad(I_C51, U->dz5_1, U->dp4, 256, 0, nullptr, 0, 0, 4));
-        TRY(pool_bwd(U->cat6, 512, 256, skip_half(U->dcat6, 3, 256), U->dp4, U->dz4_2, 256, 4, coded ? U->pc4 : nullptr));
+        TRY(conv_dgrad(I_C51, U->dz5_1, U->dp4, 256, 0, nullptr, 4));
+        TRY(pool_bwd(U->pc4, skip_half(U->dcat6, 3, 256), U->dp4, U->dz4_2, 256, 4));
         TRY(conv_wgrad(I_C42, U->a4_1, 256, 0, U->dz4_2, g, 3));
-        TRY(conv_dgrad(I_C42, U->dz4_2, U->dz4_1, 256, 0, U->a4_1, 256, 0, 3));
+        TRY(conv_dgrad(I_C42, U->dz4_2, U->dz4_1, 256, 0, U->a4_1, 3));
         TRY(conv_wgrad(I_C41, U->p3, 128, 0, U->dz4_1, g, 3));
-        TRY(conv_dgrad(I_C41, U->dz4_1, U->dp3, 128, 0, nullptr, 0, 0, 3));
-        TRY(pool_bwd(U->cat7, 256, 128, skip_half(U->dcat7, 2, 128), U->dp3, U->dz3_2, 128, 3, coded ? U->pc3 : nullptr));
+        TRY(conv_dgrad(I_C41, U->dz4_1, U->dp3, 128, 0, nullptr, 3));
+        TRY(pool_bwd(U->pc3, skip_half(U->dcat7, 2, 128), U->dp3, U->dz3_2, 128, 3));
         TRY(conv_wgrad(I_C32, U->a3_1, 128, 0, U->dz3_2, g, 2));
-        TRY(conv_dgrad(I_C32, U->dz3_2, U->dz3_1, 128, 0, U->a3_1, 128, 0, 2));
+        TRY(conv_dgrad(I_C32, U->dz3_2, U->dz3_1, 128, 0, U->a3_1, 2));
         TRY(conv_wgrad(I_C31, U->p2, 64, 0, U->dz3_1, g, 2));
-        TRY(conv_dgrad(I_C31, U->dz3_1, U->dp2, 64, 0, nullptr, 0, 0, 2));
-        TRY(pool_bwd(U->cat8, 128, 64, skip_half(U->dcat8, 1, 64), U->dp2, U->dz2_2, 64, 2, coded ? U->pc2 : nullptr));
+        TRY(conv_dgrad(I_C31, U->dz3_1, U->dp2, 64, 0, nullptr, 2));
+        TRY(pool_bwd(U->pc2, skip_half(U->dcat8, 1, 64), U->dp2, U->dz2_2, 64, 2));
         TRY(conv_wgrad(I_C22, U->a2_1, 64, 0, U->dz2_2, g, 1));
-        TRY(conv_dgrad(I_C22, U->dz2_2, U->dz2_1, 64, 0, U->a2_1, 64, 0, 1));
+        TRY(conv_dgrad(I_C22, U->dz2_2, U->dz2_1, 64, 0, U->a2_1, 1));
         TRY(conv_wgrad(I_C21, U->p1, 32, 0, U->dz2_1, g, 1));
         TRY(finish_bucket(2, g));
-        TRY(conv_dgrad(I_C21, U->dz2_1, U->dp1, 32, 0, nullptr, 0, 0, 1));
-        TRY(pool_bwd(U->cat9, 64, 32, skip_half(U->dcat9, 0, 32), U->dp1, U->dz1_2, 32, 1, coded ? U->pc1 : nullptr));
+        TRY(conv_dgrad(I_C21, U->dz2_1, U->dp1, 32, 0, nullptr, 1));
+        TRY(pool_bwd(U->pc1, skip_half(U->dcat9, 0, 32), U->dp1, U->dz1_2, 32, 1));
         TRY(conv_wgrad(I_C12, U->a1_1, 32, 0, U->dz1_2, g, 0));
-        TRY(conv_dgrad(I_C12, U->dz1_2, U->dz1_1, 32, 0, U->a1_1, 32, 0, 0));
+        TRY(conv_dgrad(I_C12, U->dz1_2, U->dz1_1, 32, 0, U->a1_1, 0));
         {
             const double px = (double)U->n * U->H * U->W;
             Scope sc(u, st, "conv1_1", "wgrad", 2.0 * px * 32 * 9 * U->cin0, px * (4 * U->cin0 + 64));

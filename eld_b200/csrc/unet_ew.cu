@@ -1,5 +1,5 @@
 // unet_ew.cu - the non-GEMM kernels of the U-Net step (all HBM-bound, CUDA cores):
-//   2x2 max-pool fwd / bwd(+skip add + LeakyReLU'), 1x1 head + L1 loss + its whole backward, deconv bias gradients,
+//   2x2 max-pool bwd (+skip add + LeakyReLU') from the forward's pool code, 1x1 head + L1 loss + its whole backward,
 //   fused Adam.
 #include "common.cuh"
 #include "unet_ew.h"
@@ -18,96 +18,18 @@ __device__ __forceinline__ uint32_t pack_bf2(float a, float b)
 }
 
 // ---------------------------------------------------------------------------------------------------
-// 2x2 max pool, NHWC bf16, 8 channels (16 B) per thread                                 (Unet.py:51-63)
+// 2x2 max-pool backward, NHWC bf16                                                      (Unet.py:51-63)
 // ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint4 ld16(const __nv_bfloat16* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }
-
-__global__ void __launch_bounds__(256)
-maxpool_kernel(const __nv_bfloat16* __restrict__ in, int in_pitch, int in_c0, __nv_bfloat16* __restrict__ out,
-               int C, int n_img, int Ho, int Wo)
-{
-    const int groups = C / 8;
-    const size_t total = (size_t)n_img * Ho * Wo * groups;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int gch = i % groups;
-        size_t r = i / groups;
-        const int xo = r % Wo; r /= Wo;
-        const int yo = r % Ho;
-        const int n = r / Ho;
-        const __nv_bfloat16* p00 = in + (((size_t)n * 2 * Ho + 2 * yo) * (2 * Wo) + 2 * xo) * in_pitch + in_c0 + gch * 8;
-        const uint4 a = ld16(p00), b = ld16(p00 + in_pitch), c = ld16(p00 + (size_t)2 * Wo * in_pitch), d = ld16(p00 + (size_t)(2 * Wo + 1) * in_pitch);
-        const uint32_t aw[4] = { a.x, a.y, a.z, a.w }, bw[4] = { b.x, b.y, b.z, b.w }, cw[4] = { c.x, c.y, c.z, c.w }, dw[4] = { d.x, d.y, d.z, d.w };
-        uint32_t o[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const float lo = fmaxf(fmaxf(bf_lo(aw[j]), bf_lo(bw[j])), fmaxf(bf_lo(cw[j]), bf_lo(dw[j])));
-            const float hi = fmaxf(fmaxf(bf_hi(aw[j]), bf_hi(bw[j])), fmaxf(bf_hi(cw[j]), bf_hi(dw[j])));
-            o[j] = pack_bf2(lo, hi);
-        }
-        *reinterpret_cast<uint4*>(out + (((size_t)n * Ho + yo) * Wo + xo) * C + gch * 8) = make_uint4(o[0], o[1], o[2], o[3]);
-    }
-}
-
 // dZ[full res] = ( dskip + (first arg-max of the window ? dP : 0) ) * lrelu'(A)
-//   A     : activation that was pooled (lives in a concat buffer: pitch a_pitch, offset a_c0)
-//   dskip : gradient that reached A through the skip connection (d_cat buffer, same pitch/offset)
+//   A     : activation that was pooled - never read: the forward tile's epilogue (conv_umma.cuh) leaves a 1-byte-per-
+//           pooled-element code instead, per (pooled pixel, 32 channels) eight words - "not the maximum" masks of the
+//           window's four pixels, then their sign masks (channel 2j -> bit j, 2j+1 -> bit 16+j).  That is 1/16 of what
+//           the activation costs (and the level-1 skip half of an interleaved concat buffer cost double: 128-byte lines
+//           for 64 useful bytes).
+//   dskip : gradient that reached A through the skip connection (pitch s_pitch, offset s_c0)
 //   dP    : gradient of the pooled tensor (compact)
 // PyTorch's max_pool2d backward routes to the FIRST maximum in window scan order; so do we.
-// 16 channels (32 bytes) per thread, moved as whole 32-byte sectors - C % 16 == 0, 32-byte aligned tensors.
-__global__ void __launch_bounds__(256)
-maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ A, const __nv_bfloat16* __restrict__ dskip, int a_pitch, int a_c0,
-                   int s_pitch, int s_c0, const __nv_bfloat16* __restrict__ dP, __nv_bfloat16* __restrict__ dZ, int C, int n_img, int Ho, int Wo)
-{
-    const uint32_t groups = (uint32_t)C / 16u;
-    const uint32_t total = (uint32_t)n_img * (uint32_t)Ho * (uint32_t)Wo * groups;      // 32-bit index math (launcher checks the range)
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-        const uint32_t gch = i % groups;
-        uint32_t r = i / groups;
-        const uint32_t xo = r % (uint32_t)Wo; r /= (uint32_t)Wo;
-        const uint32_t yo = r % (uint32_t)Ho;
-        const uint32_t n = r / (uint32_t)Ho;
-        const size_t pix00 = ((size_t)n * 2 * Ho + 2 * yo) * (2 * Wo) + 2 * xo;
-        const size_t offs[4] = { pix00, pix00 + 1, pix00 + (size_t)2 * Wo, pix00 + (size_t)2 * Wo + 1 };
-        uint32_t a[4][8], s[4][8], dp[8];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            ptx::ld_global_nc_32B(A + offs[k] * a_pitch + a_c0 + gch * 16, a[k]);
-            ptx::ld_global_nc_32B(dskip + offs[k] * s_pitch + s_c0 + gch * 16, s[k]);
-        }
-        ptx::ld_global_nc_32B(dP + (((size_t)n * Ho + yo) * Wo + xo) * C + gch * 16, dp);
-        uint32_t o[4][8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-#pragma unroll
-            for (int half = 0; half < 2; ++half) {
-                float av[4], sv[4];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    av[k] = half ? bf_hi(a[k][j]) : bf_lo(a[k][j]);
-                    sv[k] = half ? bf_hi(s[k][j]) : bf_lo(s[k][j]);
-                }
-                const float g = half ? bf_hi(dp[j]) : bf_lo(dp[j]);
-                int arg = 0;
-                float m = av[0];
-#pragma unroll
-                for (int k = 1; k < 4; ++k) if (av[k] > m) { m = av[k]; arg = k; }
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const float v = (sv[k] + (k == arg ? g : 0.0f)) * (av[k] > 0.0f ? 1.0f : 0.2f);
-                    const uint32_t bits = (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v));
-                    if (half) o[k][j] |= bits << 16; else o[k][j] = bits;
-                }
-            }
-        }
-#pragma unroll
-        for (int k = 0; k < 4; ++k) ptx::st_global_32B(dZ + offs[k] * C + gch * 16, o[k]);
-    }
-}
-
-// Same backward from the 1-byte-per-pooled-element code the forward tile's epilogue leaves (conv_umma.cuh): per (pooled
-// pixel, 32 channels) eight words - "not the maximum" masks of the window's four pixels, then their sign masks
-// (channel 2j -> bit j, 2j+1 -> bit 16+j).  Reads 1/16 of what the activation itself costs (and the level-1 skip half
-// of an interleaved concat buffer cost double: 128-byte lines for 64 useful bytes).
+// 16 channels (32 bytes) per thread, moved as whole 32-byte sectors - C % 32 == 0, 32-byte aligned tensors.
 __global__ void __launch_bounds__(256)
 maxpool_bwd_code_kernel(const uint32_t* __restrict__ code, const __nv_bfloat16* __restrict__ dskip, int s_pitch, int s_c0,
                         const __nv_bfloat16* __restrict__ dP, __nv_bfloat16* __restrict__ dZ, int C, int n_img, int Ho, int Wo)
@@ -149,43 +71,6 @@ maxpool_bwd_code_kernel(const uint32_t* __restrict__ code, const __nv_bfloat16* 
             }
             ptx::st_global_32B(dZ + offs[k] * C + gch * 16, o);
         }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------
-// bias gradient: out[c] += sum over pixels of g[p][c0 + c]   (NHWC bf16, C % 8 == 0, C <= 512)
-// thread handles 8 channels of a pixel; block = (C/8) x (256/(C/8)) ; smem reduce; atomics per block.
-// ---------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-colsum_kernel(const __nv_bfloat16* __restrict__ g, int pitch, int c0, int C, size_t npix, float* __restrict__ out)
-{
-    __shared__ float red[256][8 + 1];
-    const int groups = C / 8;                 // <= 64
-    const int lanes = 256 / groups;           // pixel lanes per block
-    const int gch = threadIdx.x % groups, pl = threadIdx.x / groups;
-    float acc[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
-    if (pl < lanes) {
-        for (size_t p = (size_t)blockIdx.x * lanes + pl; p < npix; p += (size_t)gridDim.x * lanes) {
-            const uint4 v = ld16(g + p * pitch + c0 + gch * 8);
-            const uint32_t w[4] = { v.x, v.y, v.z, v.w };
-#pragma unroll
-            for (int j = 0; j < 4; ++j) { acc[2 * j] += bf_lo(w[j]); acc[2 * j + 1] += bf_hi(w[j]); }
-        }
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) red[threadIdx.x][j] = acc[j];
-    __syncthreads();
-    if (threadIdx.x < C) {
-        const int c = threadIdx.x, gq = c / 8, j = c % 8;
-        float s = 0.f;
-        for (int l = 0; l < lanes; ++l) s += red[l * groups + gq][j];
-        atomicAdd(out + c, s);
-    }
-    if (C > 256 && threadIdx.x + 256 < C) {
-        const int c = threadIdx.x + 256, gq = c / 8, j = c % 8;
-        float s = 0.f;
-        for (int l = 0; l < lanes; ++l) s += red[l * groups + gq][j];
-        atomicAdd(out + c, s);
     }
 }
 
@@ -407,31 +292,6 @@ static inline int grid_for(size_t work, int per_block, int cap)
     return (int)b;
 }
 
-int launch_maxpool(eld_ctx* ctx, const void* in, int in_pitch, int in_c0, void* out, int C, int n, int Ho, int Wo, cudaStream_t st)
-{
-    const size_t work = (size_t)n * Ho * Wo * (C / 8);
-    maxpool_kernel<<<grid_for(work, 256, 16 * ctx->num_sms), 256, 0, st>>>(
-        static_cast<const __nv_bfloat16*>(in), in_pitch, in_c0, static_cast<__nv_bfloat16*>(out), C, n, Ho, Wo);
-    ELD_CHECK_CUDA(cudaGetLastError());
-    count_launch(ctx);
-    return ELD_OK;
-}
-
-int launch_maxpool_bwd(eld_ctx* ctx, const void* A, int a_pitch, int a_c0, const void* dskip, int s_pitch, int s_c0,
-                       const void* dP, void* dZ, int C, int n, int Ho, int Wo, cudaStream_t st)
-{
-    ELD_REQUIRE(C % 16 == 0 && a_pitch % 16 == 0 && a_c0 % 16 == 0 && s_pitch % 16 == 0 && s_c0 % 16 == 0,
-                "pool backward: channel counts, pitches and offsets must be multiples of 16 (256-bit accesses)");
-    const size_t work = (size_t)n * Ho * Wo * (C / 16);
-    ELD_REQUIRE(work < (1ull << 31), "pool backward: %zu work items exceed the kernel's 32-bit index range", work);
-    maxpool_bwd_kernel<<<grid_for(work, 256, 16 * ctx->num_sms), 256, 0, st>>>(
-        static_cast<const __nv_bfloat16*>(A), static_cast<const __nv_bfloat16*>(dskip), a_pitch, a_c0, s_pitch, s_c0,
-        static_cast<const __nv_bfloat16*>(dP), static_cast<__nv_bfloat16*>(dZ), C, n, Ho, Wo);
-    ELD_CHECK_CUDA(cudaGetLastError());
-    count_launch(ctx);
-    return ELD_OK;
-}
-
 int launch_maxpool_bwd_code(eld_ctx* ctx, const void* code, const void* dskip, int s_pitch, int s_c0,
                             const void* dP, void* dZ, int C, int n, int Ho, int Wo, cudaStream_t st)
 {
@@ -442,17 +302,6 @@ int launch_maxpool_bwd_code(eld_ctx* ctx, const void* code, const void* dskip, i
     maxpool_bwd_code_kernel<<<grid_for(work, 256, 16 * ctx->num_sms), 256, 0, st>>>(
         static_cast<const uint32_t*>(code), static_cast<const __nv_bfloat16*>(dskip), s_pitch, s_c0,
         static_cast<const __nv_bfloat16*>(dP), static_cast<__nv_bfloat16*>(dZ), C, n, Ho, Wo);
-    ELD_CHECK_CUDA(cudaGetLastError());
-    count_launch(ctx);
-    return ELD_OK;
-}
-
-int launch_colsum(eld_ctx* ctx, const void* g, int pitch, int c0, int C, size_t npix, float* out, cudaStream_t st)
-{
-    ELD_REQUIRE(C % 8 == 0 && C <= 512, "colsum: C=%d must be a multiple of 8 and <= 512", C);
-    const int lanes = 256 / (C / 8);
-    colsum_kernel<<<grid_for(npix, lanes * 8, 4 * ctx->num_sms), 256, 0, st>>>(
-        static_cast<const __nv_bfloat16*>(g), pitch, c0, C, npix, out);
     ELD_CHECK_CUDA(cudaGetLastError());
     count_launch(ctx);
     return ELD_OK;

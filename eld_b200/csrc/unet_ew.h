@@ -3,12 +3,8 @@
 #include "common.cuh"
 
 namespace eld {
-int launch_maxpool(eld_ctx* ctx, const void* in, int in_pitch, int in_c0, void* out, int C, int n, int Ho, int Wo, cudaStream_t st);
 int launch_maxpool_bwd_code(eld_ctx* ctx, const void* code, const void* dskip, int s_pitch, int s_c0,
                             const void* dP, void* dZ, int C, int n, int Ho, int Wo, cudaStream_t st);
-int launch_maxpool_bwd(eld_ctx* ctx, const void* A, int a_pitch, int a_c0, const void* dskip, int s_pitch, int s_c0,
-                       const void* dP, void* dZ, int C, int n, int Ho, int Wo, cudaStream_t st);
-int launch_colsum(eld_ctx* ctx, const void* g, int pitch, int c0, int C, size_t npix, float* out, cudaStream_t st);
 int launch_head(eld_ctx* ctx, const void* a, const float* w, const float* b, float* out, const float* target, void* dz,
                 float* dw, float* db, float* loss, int n, size_t plane, int cout, int l2_loss, cudaStream_t st);
 int launch_clock_probe(eld_ctx* ctx, float* out_mhz, cudaStream_t st);

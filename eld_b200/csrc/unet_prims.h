@@ -59,8 +59,8 @@ struct WgradOp {
     int q_pitch, q_c0, q_ch;
     int n_img, H, W;     // pixel grid of the reduction (deconv: coarse)
     float* dw;           // f32, PyTorch layout, accumulated into (zero it first)
-    int out_tco;         // conv only: 1 = dw is the [tap][ci][co] staging layout (vector red.add), see wgrad_conv.cuh
-    float* db;           // conv (full-halo generation) only: optional fused bias gradient, db[co] += sum_pixels dz
+    int out_tco;         // conv only: 1 = dw is the [tap][ci][co] staging layout (the engine permutes it to OIHW afterwards)
+    float* db;           // optional fused bias gradient: conv db[co] += sum_pixels dz, deconv db[co] += sum_fine_pixels d(up)
 };
 int init_gemm_kernels(eld_ctx* ctx);   // opt in to large dynamic smem (call once, outside graph capture)
 int launch_wgrad(eld_ctx* ctx, const WgradOp& op, cudaStream_t st);

@@ -1,8 +1,6 @@
 """bench.py's U-Net workloads: the training step (BASELINE configs[2]) - noise kernel -> U-Net fwd + L1 + bwd ->
 (bucketed NCCL all-reduce overlapped with backward) -> fused Adam - and the inference step (configs[1]), one process
 per GPU; plus the ON-BOX baseline: the reference module through PyTorch-eager / cuDNN on the same GPU (SURVEY 2.2)."""
-import os
-
 import torch
 
 from . import arch
@@ -109,52 +107,17 @@ def make_train_steps(a, nm, dev, rank, world):
     host_losses = [torch.zeros(1).pin_memory() for _ in range(2)]
     loss_read = [torch.cuda.Event() for _ in range(2)]
 
-    # Optional software pipeline (ELD_OVERLAP=1): the noise kernel of step i+1 on a side stream WHILE step i's network runs
-    # (one noise launch per step, all inside the timed region; double-buffered `noisy`, events both ways).  Off by default:
-    # the noise CTAs that co-reside with the persistent tiles take issue slots from them.
-    overlap = os.environ.get('ELD_OVERLAP') is not None
-    noise_stream = torch.cuda.Stream(device=dev)
-    noisy2 = [noisy, torch.empty_like(noisy)]
-    made = [torch.cuda.Event() for _ in range(2)]
-    used = [torch.cuda.Event() for _ in range(2)]
-    pipe = {'have': None}
-
-    def issue_noise(i, target, after=None):
-        k = i & 1
-        with torch.cuda.stream(noise_stream):
-            noise_stream.wait_event(used[k])                 # the step that last read noisy2[k] has consumed it
-            if after is not None:
-                noise_stream.wait_event(after)               # e2e: the H2D copy of this clean batch
-            nm.batch_gpu(target, params=plist, frame_id0=(i * world + rank) * B, out=noisy2[k])
-            made[k].record(noise_stream)
-        pipe['have'] = i
-
-    def body(target, i, next_target=None, next_after=None):
-        cur = torch.cuda.current_stream()
-        k = i & 1
-        if overlap:
-            if pipe['have'] != i:                            # pipeline start: nothing was made ahead for this step
-                here = torch.cuda.Event()
-                here.record(cur)
-                issue_noise(i, target, here)                 # `target` is ready on the current stream at this point
-            cur.wait_event(made[k])
-            x = noisy2[k]
-        else:
-            x = noisy
-            nm.batch_gpu(target, params=plist, frame_id0=(i * world + rank) * B, out=noisy)
+    def body(target, i):
+        nm.batch_gpu(target, params=plist, frame_id0=(i * world + rank) * B, out=noisy)
         if world > 1:
-            out, _ = net.train_step_ddp(x, target, loss_out=loss)
+            out, _ = net.train_step_ddp(noisy, target, loss_out=loss)
         else:
-            out, _ = net.train_step(x, target, loss_out=loss)
-        last.update(noisy=x, out=out, loss=loss)
-        if overlap:
-            used[k].record(cur)
-            if next_target is not None:
-                issue_noise(i + 1, next_target, next_after)  # queued behind nothing: runs next to this step's tiles
+            out, _ = net.train_step(noisy, target, loss_out=loss)
+        last.update(noisy=noisy, out=out, loss=loss)
         opt.step(grad_scale=1.0 / world)
 
     def step(i):
-        body(clean[i & 1], i, clean[(i + 1) & 1])
+        body(clean[i & 1], i)
 
     # end to end: every step's clean batch comes from pinned host memory.  Like a DataLoader with
     # pin_memory + prefetch (train_syn.py:78-80) the copy of batch i+1 runs on a side stream while step i
@@ -176,12 +139,11 @@ def make_train_steps(a, nm, dev, rank, world):
         k = i & 1
         if state['next'] != i:
             issue_copy(i)
-            pipe['have'] = None                            # (re)start of an e2e run: no pre-made input
         cur = torch.cuda.current_stream()
         cur.wait_event(copied[k])
         issue_copy(i + 1)
         state['next'] = i + 1
-        body(dev_bufs[k], i, dev_bufs[(i + 1) & 1], copied[(i + 1) & 1])
+        body(dev_bufs[k], i)
         consumed[k].record(cur)
         # the loss of EVERY step is read back to the host; the host waits for step i-1's value after it has queued step i
         # (a training loop that logs with one step of lag), so its launch work never leaves the GPU idle.  bench.py's
