@@ -48,6 +48,8 @@ class _EngineFunction(torch.autograd.Function):
     def backward(ctx, dout):
         net = ctx.net
         (x,) = ctx.saved_tensors
+        need = ctx.needs_input_grad[2:]              # frozen parameters: no weight-gradient launch, None returned
+        net._set_trainable(ctx.eng, need, ctx.needs_input_grad[1])
         g = torch.empty_like(net._flat)
         _lib.check(_lib.load().eld_unet_backward(ctx.eng, net._flat.data_ptr(), x.data_ptr(), dout.contiguous().data_ptr(),
                                                 g.data_ptr(), _st()), 'eld_unet_backward')
@@ -56,12 +58,9 @@ class _EngineFunction(torch.autograd.Function):
             dx = torch.empty_like(x)
             _lib.check(_lib.load().eld_unet_input_grad(ctx.eng, net._flat.data_ptr(), dx.data_ptr(), _st()),
                        'eld_unet_input_grad')
-        grads, off = [], 0
-        for p in net.parameters():
-            k = p.numel()
-            grads.append(g[off:off + k].view(p.shape))
-            off += k
-        return (None, dx) + tuple(grads)
+        grads = tuple(g[off:off + k].view(p.shape) if want else None
+                      for p, (off, k), want in zip(net.parameters(), net._spans, need))
+        return (None, dx) + grads
 
 
 class UNetSeeInDark(nn.Module):
@@ -91,6 +90,7 @@ class UNetSeeInDark(nn.Module):
         self._flat = None
         self._flat_grad = None
         self._engines = {}
+        self._masks = {}          # engine handle -> (trainable flags, input_grad) it was last given
         self._ddp_ready = None
         self._flatten()
 
@@ -102,14 +102,36 @@ class UNetSeeInDark(nn.Module):
         flat = torch.empty(total, dtype=torch.float32, device=dev)
         grad = torch.zeros(total, dtype=torch.float32, device=dev)
         off = 0
+        self._spans, self._grad_views = [], []        # (offset, count) of every parameter; its view into flat_grads
         for p in params:
             n = p.numel()
             flat[off:off + n].copy_(p.data.reshape(-1).float())
             p.data = flat[off:off + n].view(p.shape)
-            p.grad = grad[off:off + n].view(p.shape)
+            view = grad[off:off + n].view(p.shape)
+            p.grad = view if p.requires_grad else None
+            self._spans.append((off, n))
+            self._grad_views.append(view)
             off += n
         self._flat, self._flat_grad = flat, grad
         self._drop_engines()
+
+    # ---- frozen parameters (p.requires_grad_(False)) ---------------------------------------------
+    def _set_trainable(self, eng, flags, input_grad):
+        """Tell engine `eng` which gradients the next backward computes (eld_unet_set_trainable; host-side, only when the
+        mask changed): one flag per parameter in state_dict order, and whether d(loss)/d(x) is wanted."""
+        key = (tuple(bool(f) for f in flags), bool(input_grad))
+        if self._masks.get(eng.value) != key:
+            arr = (ctypes.c_uint8 * len(key[0]))(*key[0])
+            _lib.check(_lib.load().eld_unet_set_trainable(eng, arr, len(key[0]), int(key[1])), 'eld_unet_set_trainable')
+            self._masks[eng.value] = key
+
+    def _sync_grads(self, flags):
+        """torch's contract for a fused step: a frozen parameter's .grad is None, a trainable one's is its flat_grads view"""
+        for p, view, f in zip(self.parameters(), self._grad_views, flags):
+            if not f:
+                p.grad = None
+            elif p.grad is None or p.grad.data_ptr() != view.data_ptr():
+                p.grad = view
 
     _MAX_ENGINES = 4      # (n, h, w, train) launch plans kept alive, least recently used evicted (each owns a workspace)
 
@@ -118,6 +140,7 @@ class UNetSeeInDark(nn.Module):
         while len(eng) > keep:
             key = next(iter(eng))
             handle, _ws = eng.pop(key)
+            self._masks.pop(handle.value, None)
             try:
                 _lib.load().eld_unet_destroy(handle)
             except Exception:
@@ -165,6 +188,7 @@ class UNetSeeInDark(nn.Module):
             _lib.check(lib.eld_unet_create_io(_lib.ctx(dev.index or 0), n, h, w, int(train), ws.data_ptr(), nbytes,
                                               self.in_channels, self.out_channels, ctypes.byref(handle)), 'eld_unet_create_io')
             self._engines[key] = (handle, ws)
+            self._masks[handle.value] = ((True,) * len(self._spans), True)      # a new engine computes every gradient
         return self._engines[key][0]
 
     def forward(self, x):
@@ -190,14 +214,19 @@ class UNetSeeInDark(nn.Module):
     loss_kind = 'l1'      # 'l1' (nn.L1Loss, the reference default) or 'l2' (nn.MSELoss) - models/losses.py:29-36
 
     def train_step(self, x, target, loss_out=None):
-        """forward + pixel loss + backward in one launch sequence.  Fills self.flat_grads (== every
-        parameter's .grad) and returns (out, loss) with loss a 0-dim cuda tensor (no host sync)."""
+        """forward + pixel loss + backward in one launch sequence.  Fills self.flat_grads (== every trainable
+        parameter's .grad) and returns (out, loss) with loss a 0-dim cuda tensor (no host sync).  Parameters with
+        requires_grad == False are frozen: no gradient is computed for them, their .grad is None and their range of
+        flat_grads reads zero."""
         n, _, h, w = x.shape
         assert x.is_cuda and x.dtype == torch.float32 and x.shape[1] == self.in_channels
         assert target.shape == (n, self.out_channels, h, w) and target.dtype == torch.float32
         x, target = x.contiguous(), target.contiguous()
         out = torch.empty_like(target)
         loss = loss_out if loss_out is not None else torch.empty((), dtype=torch.float32, device=x.device)
+        flags = self._last_flags = [p.requires_grad for p in self.parameters()]
+        self._set_trainable(self._engine(n, h, w, True), flags, False)
+        self._sync_grads(flags)
         _lib.check(_lib.load().eld_unet_set_loss(self._engine(n, h, w, True), 1 if self.loss_kind == 'l2' else 0), 'eld_unet_set_loss')
         _lib.check(_lib.load().eld_unet_train_step(self._engine(n, h, w, True), self._flat.data_ptr(), x.data_ptr(),
                                                    target.data_ptr(), out.data_ptr(), self._flat_grad.data_ptr(),
@@ -234,9 +263,15 @@ class UNetSeeInDark(nn.Module):
         if ev:
             timeline['backward_end'] = ev(); timeline['backward_end'].record()
             timeline['buckets'] = []
-        works = []
+        # a bucket whose parameters are all frozen has nothing to exchange: no wait, no all-reduce
+        live = [any(f and o < off + cnt and off < o + k for (o, k), f in zip(self._spans, self._last_flags))
+                for off, cnt in self._ddp_buckets]
+        works, sent = [], []
         with torch.cuda.stream(self._ddp_stream):
             for k, (off, cnt) in enumerate(self._ddp_buckets):
+                if not live[k]:
+                    continue
+                sent.append((off, cnt))
                 _lib.check(lib.eld_unet_wait_bucket(eng, k, ctypes.c_void_p(self._ddp_stream.cuda_stream)), 'eld_unet_wait_bucket')
                 if ev:
                     e0 = ev(); e0.record(self._ddp_stream)
@@ -252,7 +287,7 @@ class UNetSeeInDark(nn.Module):
             works = []
         # FusedAdam.step joins them bucket by bucket: Adam on the first buckets runs while the last, tiny one (conv1_*:
         # final only when backward ends, its all-reduce pure latency) is still in flight
-        self._pending_allreduce = [(off, cnt, wk) for (off, cnt), wk in zip(self._ddp_buckets, works)]
+        self._pending_allreduce = [(off, cnt, wk) for (off, cnt), wk in zip(sent, works)]
         return out, loss
 
     def join_allreduce(self):
@@ -304,30 +339,58 @@ class UNetSeeInDark(nn.Module):
 
 class FusedAdam(torch.optim.Optimizer):
     """torch.optim.Adam semantics (ELD_model.py:400-401) as ONE kernel over the flat buffers.
-    Keeps `param_groups` so Engine.set_learning_rate / util.set_opt_param keep working."""
+    Keeps `param_groups` so Engine.set_learning_rate / util.set_opt_param keep working.  Frozen parameters
+    (requires_grad == False) are skipped: the trainable runs of the buffer go to eld_adam_step_segments, each with the
+    per-parameter step count torch keeps in state['step']."""
 
     def __init__(self, net, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
         super().__init__(list(net.parameters()), dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
         self.net = net
         self.m = torch.zeros_like(net.flat_params)
         self.v = torch.zeros_like(net.flat_params)
-        self.t = 0
+        self.t = 0                                     # step() calls
+        self.steps = [0] * len(net._spans)             # Adam steps taken by each parameter (torch's state['step'])
 
     @torch.no_grad()
     def step(self, closure=None, grad_scale=1.0):
+        """One Adam step on every parameter that requires grad; a frozen parameter, its moments and its step count stay
+        as they are (torch.optim.Adam skips a parameter whose .grad is None)."""
         g = self.param_groups[0]
         if self.m.data_ptr() == 0 or self.m.device != self.net.flat_params.device:
             self.m = torch.zeros_like(self.net.flat_params)
             self.v = torch.zeros_like(self.net.flat_params)
         self.t += 1
+        flags = [q.requires_grad for q in self.net.parameters()]
+        for i, f in enumerate(flags):
+            self.steps[i] += 1 if f else 0
+        uniform = all(flags) and len(set(self.steps)) == 1
         p = self.net.flat_params
+        hp = (float(g['lr']), float(g['betas'][0]), float(g['betas'][1]), float(g['eps']), float(g['weight_decay']))
 
-        def adam(off, cnt):
-            _lib.check(_lib.load().eld_adam_step(_lib.ctx(p.device.index or 0), p.data_ptr() + 4 * off,
-                                                 self.net.flat_grads.data_ptr() + 4 * off, self.m.data_ptr() + 4 * off,
-                                                 self.v.data_ptr() + 4 * off, cnt, float(g['lr']),
-                                                 float(g['betas'][0]), float(g['betas'][1]), float(g['eps']),
-                                                 float(g['weight_decay']), self.t, float(grad_scale), _st()), 'eld_adam_step')
+        def adam(lo, hi):
+            lib, dev = _lib.load(), _lib.ctx(p.device.index or 0)
+            if uniform:                                # one range, one step count
+                _lib.check(lib.eld_adam_step(dev, p.data_ptr() + 4 * lo, self.net.flat_grads.data_ptr() + 4 * lo,
+                                             self.m.data_ptr() + 4 * lo, self.v.data_ptr() + 4 * lo, hi - lo, *hp,
+                                             self.steps[0], float(grad_scale), _st()), 'eld_adam_step')
+                return
+            segs = []                                  # trainable runs inside [lo, hi), merged while the step count agrees
+            for (off, n), f, s in zip(self.net._spans, flags, self.steps):
+                a, b = max(off, lo), min(off + n, hi)
+                if not f or a >= b:
+                    continue
+                if segs and segs[-1][2] == s and segs[-1][0] + segs[-1][1] == a:
+                    segs[-1][1] += b - a
+                else:
+                    segs.append([a, b - a, s])
+            if not segs:
+                return
+            k = len(segs)
+            table = (ctypes.c_size_t * (2 * k))(*[x for a, c, _ in segs for x in (a, c)])
+            steps = (ctypes.c_int * k)(*[s for _, _, s in segs])
+            _lib.check(lib.eld_adam_step_segments(dev, p.data_ptr(), self.net.flat_grads.data_ptr(), self.m.data_ptr(),
+                                                  self.v.data_ptr(), table, steps, k, *hp, float(grad_scale), _st()),
+                       'eld_adam_step_segments')
         pend = getattr(self.net, '_pending_allreduce', None)
         if pend:
             # data parallel: buckets arrive in backward-completion order and tile the buffer from its end towards its start;
@@ -337,7 +400,7 @@ class FusedAdam(torch.optim.Optimizer):
                 wk.wait()
             lo = min(off for off, _, _ in pend[:-1]) if len(pend) > 1 else p.numel()
             if lo < p.numel():
-                adam(lo, p.numel() - lo)
+                adam(lo, p.numel())
             pend[-1][2].wait()
             if lo > 0:
                 adam(0, lo)
@@ -347,28 +410,32 @@ class FusedAdam(torch.optim.Optimizer):
     def zero_grad(self, set_to_none=False):
         self.net.flat_grads.zero_()
 
-    # checkpoint format of torch.optim.Adam ('opt_g' in ELD_model.py:516-523)
+    # checkpoint format of torch.optim.Adam ('opt_g' in ELD_model.py:516-523): per-parameter step; a parameter that has
+    # never taken a step has no state entry
     def state_dict(self):
-        state, off = {}, 0
-        for i, p in enumerate(self.net.parameters()):
-            n = p.numel()
-            state[i] = {'step': torch.tensor(float(self.t)), 'exp_avg': self.m[off:off + n].view(p.shape).clone(),
+        state = {}
+        params = list(self.net.parameters())
+        for i, (p, (off, n), s) in enumerate(zip(params, self.net._spans, self.steps)):
+            if s == 0:
+                continue
+            state[i] = {'step': torch.tensor(float(s)), 'exp_avg': self.m[off:off + n].view(p.shape).clone(),
                         'exp_avg_sq': self.v[off:off + n].view(p.shape).clone()}
-            off += n
         groups = [dict((k, v) for k, v in self.param_groups[0].items() if k != 'params')]
-        groups[0]['params'] = list(range(len(state)))
+        groups[0]['params'] = list(range(len(params)))
         return {'state': state, 'param_groups': groups}
 
     def load_state_dict(self, sd):
-        off = 0
-        for i, p in enumerate(self.net.parameters()):
-            n = p.numel()
+        for i, (off, n) in enumerate(self.net._spans):
             st = sd['state'].get(i)
             if st is not None:
                 self.m[off:off + n].copy_(st['exp_avg'].reshape(-1))
                 self.v[off:off + n].copy_(st['exp_avg_sq'].reshape(-1))
-                self.t = int(float(st['step']))
-            off += n
+                self.steps[i] = int(float(st['step']))
+            else:
+                self.m[off:off + n].zero_()
+                self.v[off:off + n].zero_()
+                self.steps[i] = 0
+        self.t = max(self.steps)
         for k, v in sd['param_groups'][0].items():
             if k != 'params':
                 self.param_groups[0][k] = v

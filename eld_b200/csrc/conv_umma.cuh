@@ -28,7 +28,8 @@ struct ConvGemmParams {
     int a_c0;             // first channel inside the A tensor (concat buffers)
     int kc;               // 32 or 64
     int n_total, n_tile;  // GEMM N and per-tile N (32, 64 or 128)
-    int b_rows;           // rows of one packed weight block (min(n_total, 256), unet_prims.h packed_index)
+    int b_rows;           // rows of one packed weight block = the block stride (min(rows of the operand, 256), unet_prims.h
+                          // packed_index); n_total may be a prefix of them (GemmOp::b_block_rows)
     int epi_mode, act;
     __nv_bfloat16* out;
     int out_pitch, out_c0;

@@ -41,6 +41,14 @@ constexpr int kBucketEntry1[kGradBuckets] = { 21, 9, 7, 1 };
 constexpr int kBucketLayer0[kGradBuckets] = { 10 /*upv6*/, 8 /*conv5_1*/, 2 /*conv2_1*/, 0 /*conv1_1*/ };
 constexpr int kBucketLayer1[kGradBuckets] = { 23, 10, 8, 2 };   // one past the last layer
 
+// The forward graph the backward walks in reverse: the layer whose output each layer reads (-1 = the input frame x; a
+// pool between two encoder levels does not change who produced the tensor), and for the four concatenating convs the
+// encoder layer behind the skip half of their input (Unet.py:69,74,79,84).  State_dict order is a topological order.
+constexpr int kSrc[kNumLayers] = { -1, I_C11, I_C12, I_C21, I_C22, I_C31, I_C32, I_C41, I_C42, I_C51, I_C52, I_UP6, I_C61,
+                                   I_C62, I_UP7, I_C71, I_C72, I_UP8, I_C81, I_C82, I_UP9, I_C91, I_C92 };
+constexpr int kSkip[kNumLayers] = { -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, I_C42 /*conv6_1*/, -1, -1, I_C32 /*conv7_1*/,
+                                    -1, -1, I_C22 /*conv8_1*/, -1, -1, I_C12 /*conv9_1*/, -1, -1 };
+
 struct PackEntry { unsigned long long src, dst_f, dst_d; int cout, cin, type; int pad; };
 struct PackTable {
     PackEntry e[kNumLayers];
@@ -239,6 +247,13 @@ struct eld_unet {
     int cin0 = 4, cout_last = 4; // channels of the frame in / out: 4 = packed raw, 3 = sRGB (ELD_model.py:377-389)
     int l2_loss = 0;             // 0: nn.L1Loss (the reference default, losses.py:31-32), 1: nn.MSELoss (losses.py:33-34)
     bool dz1_1_final = false;    // dz1_1 holds the last backward's conv1_1 gradient: set by a backward, cleared by a forward
+    // what the backward computes (eld_unet_set_trainable; default: everything).  wgrad[l]: layer l's weight or bias
+    // requires grad.  reach[l]: the gradient of layer l's output is needed - l trains, or something upstream of it does
+    // (or the frame, when input_grad).  perm_t0 / perm_t1: tile span of the gradient permute per bucket ([kGradBuckets]
+    // = the whole table), over the layers that train.
+    bool wgrad[kNumLayers], reach[kNumLayers];
+    bool input_grad = true;
+    int perm_t0[kGradBuckets + 1], perm_t1[kGradBuckets + 1];
     // optional per-launch profile (CUDA events on the launch stream)
     bool profile = false;
     struct Rec { char name[32]; double flops, bytes; cudaEvent_t e0, e1; };
@@ -364,6 +379,29 @@ extern "C" size_t eld_unet_workspace_bytes(int n, int h, int w, int train)
     return layout(&tmp, nullptr, train != 0) + 1024;
 }
 
+// The per-launch plan of the backward from the trainable flags (one per parameter tensor, state_dict order), by one
+// walk of the forward graph (kSrc / kSkip) in topological order: a layer's output gradient is needed when the layer
+// trains or when the gradient of one of its inputs is.  Runner::backward launches a weight gradient where wgrad[] says
+// so and a data gradient towards every input whose producer is reached.
+static void derive_needs(eld_unet* u, const uint8_t* flags, bool input_grad)
+{
+    u->input_grad = input_grad;
+    for (int l = 0; l < kNumLayers; ++l) {
+        u->wgrad[l] = flags[2 * l] || flags[2 * l + 1];
+        const bool in = kSrc[l] < 0 ? input_grad : u->reach[kSrc[l]];
+        u->reach[l] = u->wgrad[l] || in || (kSkip[l] >= 0 && u->reach[kSkip[l]]);
+    }
+    // the table holds conv1_2 .. conv9_2 in state_dict order: entry e is layer e + 1
+    for (int k = 0; k <= kGradBuckets; ++k) {
+        const int e0 = k < kGradBuckets ? kBucketEntry0[k] : 0, e1 = k < kGradBuckets ? kBucketEntry1[k] : u->table.n;
+        int a = e1, b = e0;
+        for (int e = e0; e < e1; ++e)
+            if (u->wgrad[e + 1]) { a = a < e ? a : e; b = e + 1; }
+        u->perm_t0[k] = a < b ? u->table.tile0[a] : 0;
+        u->perm_t1[k] = a < b ? u->table.tile0[b] : 0;
+    }
+}
+
 extern "C" int eld_unet_create_io(eld_ctx* ctx, int n, int h, int w, int train, void* workspace, size_t bytes,
                                   int cin, int cout, eld_unet** out);
 extern "C" int eld_unet_create(eld_ctx* ctx, int n, int h, int w, int train, void* workspace, size_t bytes, eld_unet** out)
@@ -406,6 +444,11 @@ extern "C" int eld_unet_create_io(eld_ctx* ctx, int n, int h, int w, int train, 
     u->table.first_dst = u->L[I_C11].w_off;
     u->table.first_wf = u->L[I_C11].wf_off;
     u->table.first_cin = u->cin0;
+    {
+        uint8_t all[2 * kNumLayers];
+        memset(all, 1, sizeof(all));
+        derive_needs(u, all, true);
+    }
     // conv1_1's operand image: zero once (pack_all rewrites all of it every step anyway)
     ELD_CHECK_CUDA(cudaMemset(u->packed + u->L[I_C11].wf_off, 0, 32 * 9 * 32 * sizeof(__nv_bfloat16)));
     // opt in to large dynamic shared memory once (not inside a captured region)
@@ -529,21 +572,34 @@ struct Runner {
     // dx2 != nullptr: the gradient of a concat input is stored as two PLANAR halves (dx = [up], dx2 = [skip], pitch cin/2
     // each) - every consumer reads exactly one half, and an interleaved buffer made each of them move whole 128-byte
     // lines for 64 useful bytes (ncu r01: level-1 pool.bwd 570 MB for 300, upv9 dgrad/wgrad 336 MB for 200)
-    int conv_dgrad(int li, const void* dz, void* dx, int dxp, int dxc0, const void* act_src, int lvl, void* dx2 = nullptr) const
+    // n_cols != 0: only the first n_cols input channels (the up half of a concat input whose skip half nobody needs),
+    // read as a row prefix of every block of the same packed dgrad operand
+    int conv_dgrad(int li, const void* dz, void* dx, int dxp, int dxc0, const void* act_src, int lvl, void* dx2 = nullptr,
+                   int n_cols = 0) const
     {
         const Layer& l = u->L[li];
+        const int nc = n_cols ? n_cols : l.cin;
         GemmOp op{};
         op.a = dz; op.a_pitch = l.cout; op.a_c0 = 0; op.a_mode = A_CONV; op.taps = 9; op.cin = l.cout;
         op.n_img = u->n; op.H = u->H >> lvl; op.W = u->W >> lvl;
-        op.b = wd(li); op.n_total = l.cin; op.cout = l.cin;
+        op.b = wd(li); op.n_total = nc; op.cout = nc;
+        if (n_cols) op.b_block_rows = l.cin <= 256 ? l.cin : 256;
         op.epi_mode = EPI_STORE; op.act = act_src ? ACT_MASK : ACT_NONE;
         op.out = dx; op.out_pitch = dxp; op.out_c0 = dxc0; op.bias = nullptr;
         if (dx2) { op.out2 = dx2; op.out2_pitch = dxp; op.out_split = l.cin / 2; }
         op.aux_sign = act_src ? sign_of(act_src) : nullptr;
         ELD_REQUIRE(!act_src || op.aux_sign, "eld_unet: %s dgrad: no sign words for its LeakyReLU' mask", l.name);
         const double px = (double)u->n * op.H * op.W;
-        Scope sc(u, st, l.name, "dgrad", 2.0 * px * l.cout * 9 * l.cin, px * 2 * (l.cin * (act_src ? 2 : 1) + l.cout) + 18.0 * l.cin * l.cout);
+        Scope sc(u, st, l.name, "dgrad", 2.0 * px * l.cout * 9 * nc, px * 2 * (nc * (act_src ? 2 : 1) + l.cout) + 18.0 * nc * l.cout);
         return launch_conv_gemm(ctx(), op, st);
+    }
+    // data gradient of a concatenating conv (conv6_1 .. conv9_1) into the planar [up | skip] halves of dcat; the skip half
+    // only when the encoder layer behind it, or something upstream of it, needs a gradient
+    int concat_dgrad(int li, const void* dz, __nv_bfloat16* dcat, int lvl) const
+    {
+        const int half = u->L[li].cin / 2;
+        if (!u->reach[kSkip[li]]) return conv_dgrad(li, dz, dcat, half, 0, nullptr, lvl, nullptr, half);
+        return conv_dgrad(li, dz, dcat, half, 0, nullptr, lvl, skip_half(dcat, lvl, half));
     }
     int deconv_dgrad(int li, const void* dy, int dyp, void* dx, const void* act_src, int lvl_in) const
     {
@@ -608,11 +664,13 @@ struct Runner {
         // the compute stream, then an event marks the bucket final.  (Running this permute on the caller's communication
         // stream instead would let it overlap the tiles - any foreign kernel that overlaps the persistent
         // one-CTA-per-SM tiles delays some of their CTAs, and a tile kernel is as slow as its slowest CTA.)
+        // Only the span of layers that train is moved (a frozen layer's range of grads keeps the zeros of the memset); a
+        // bucket with nothing to move still records its event, so a waiter never sees one from an earlier step.
         const bool per_bucket = u->bucket_ev[0] != nullptr;
         if (!per_bucket && k != kGradBuckets - 1) return ELD_OK;
-        const int t0 = per_bucket ? u->table.tile0[kBucketEntry0[k]] : 0;
-        const int t1 = per_bucket ? u->table.tile0[kBucketEntry1[k]] : u->table.tile0[u->table.n];
-        {
+        const int t0 = u->perm_t0[per_bucket ? k : kGradBuckets];
+        const int t1 = u->perm_t1[per_bucket ? k : kGradBuckets];
+        if (t1 > t0) {
             Scope sc(u, st, "weights", "gperm", 0.0, 0.0);
             wgrad_permute_kernel<<<t1 - t0, 256, 0, st>>>(u->gtmp, g, u->table, t0, t1);
             ELD_CHECK_CUDA(cudaGetLastError());
@@ -661,60 +719,65 @@ struct Runner {
         return ELD_OK;
     }
 
+    // The fixed backward sequence; every launch runs only when the plan (derive_needs) asks for what it produces:
+    // W(l) = layer l's weight gradient, D(s) = the data gradient towards the output of layer s (the gradient of an
+    // input produced by s).  With every parameter trainable all of them run, in this order.
     int backward(const float* x, float* g) const
     {
         eld_unet* U = u;
-        TRY(conv_wgrad(I_C92, U->a9_1, 32, 0, U->dz9_2, g, 0));
-        TRY(conv_dgrad(I_C92, U->dz9_2, U->dz9_1, 32, 0, U->a9_1, 0));
-        TRY(conv_wgrad(I_C91, U->cat9, 64, 0, U->dz9_1, g, 0));
-        TRY(conv_dgrad(I_C91, U->dz9_1, U->dcat9, 32, 0, nullptr, 0, skip_half(U->dcat9, 0, 32)));
-        TRY(deconv_wgrad(I_UP9, U->a8_2, U->dcat9, 32, g, 1));
-        TRY(deconv_dgrad(I_UP9, U->dcat9, 32, U->dz8_2, U->a8_2, 1));
-        TRY(conv_wgrad(I_C82, U->a8_1, 64, 0, U->dz8_2, g, 1));
-        TRY(conv_dgrad(I_C82, U->dz8_2, U->dz8_1, 64, 0, U->a8_1, 1));
-        TRY(conv_wgrad(I_C81, U->cat8, 128, 0, U->dz8_1, g, 1));
-        TRY(conv_dgrad(I_C81, U->dz8_1, U->dcat8, 64, 0, nullptr, 1, skip_half(U->dcat8, 1, 64)));
-        TRY(deconv_wgrad(I_UP8, U->a7_2, U->dcat8, 64, g, 2));
-        TRY(deconv_dgrad(I_UP8, U->dcat8, 64, U->dz7_2, U->a7_2, 2));
-        TRY(conv_wgrad(I_C72, U->a7_1, 128, 0, U->dz7_2, g, 2));
-        TRY(conv_dgrad(I_C72, U->dz7_2, U->dz7_1, 128, 0, U->a7_1, 2));
-        TRY(conv_wgrad(I_C71, U->cat7, 256, 0, U->dz7_1, g, 2));
-        TRY(conv_dgrad(I_C71, U->dz7_1, U->dcat7, 128, 0, nullptr, 2, skip_half(U->dcat7, 2, 128)));
-        TRY(deconv_wgrad(I_UP7, U->a6_2, U->dcat7, 128, g, 3));
-        TRY(deconv_dgrad(I_UP7, U->dcat7, 128, U->dz6_2, U->a6_2, 3));
-        TRY(conv_wgrad(I_C62, U->a6_1, 256, 0, U->dz6_2, g, 3));
-        TRY(conv_dgrad(I_C62, U->dz6_2, U->dz6_1, 256, 0, U->a6_1, 3));
-        TRY(conv_wgrad(I_C61, U->cat6, 512, 0, U->dz6_1, g, 3));
-        TRY(conv_dgrad(I_C61, U->dz6_1, U->dcat6, 256, 0, nullptr, 3, skip_half(U->dcat6, 3, 256)));
-        TRY(deconv_wgrad(I_UP6, U->a5_2, U->dcat6, 256, g, 4));
+        auto W = [U](int l) { return U->wgrad[l]; };
+        auto D = [U](int s) { return U->reach[s]; };
+        if (W(I_C92)) TRY(conv_wgrad(I_C92, U->a9_1, 32, 0, U->dz9_2, g, 0));
+        if (D(I_C91)) TRY(conv_dgrad(I_C92, U->dz9_2, U->dz9_1, 32, 0, U->a9_1, 0));
+        if (W(I_C91)) TRY(conv_wgrad(I_C91, U->cat9, 64, 0, U->dz9_1, g, 0));
+        if (D(I_UP9)) TRY(concat_dgrad(I_C91, U->dz9_1, U->dcat9, 0));
+        if (W(I_UP9)) TRY(deconv_wgrad(I_UP9, U->a8_2, U->dcat9, 32, g, 1));
+        if (D(I_C82)) TRY(deconv_dgrad(I_UP9, U->dcat9, 32, U->dz8_2, U->a8_2, 1));
+        if (W(I_C82)) TRY(conv_wgrad(I_C82, U->a8_1, 64, 0, U->dz8_2, g, 1));
+        if (D(I_C81)) TRY(conv_dgrad(I_C82, U->dz8_2, U->dz8_1, 64, 0, U->a8_1, 1));
+        if (W(I_C81)) TRY(conv_wgrad(I_C81, U->cat8, 128, 0, U->dz8_1, g, 1));
+        if (D(I_UP8)) TRY(concat_dgrad(I_C81, U->dz8_1, U->dcat8, 1));
+        if (W(I_UP8)) TRY(deconv_wgrad(I_UP8, U->a7_2, U->dcat8, 64, g, 2));
+        if (D(I_C72)) TRY(deconv_dgrad(I_UP8, U->dcat8, 64, U->dz7_2, U->a7_2, 2));
+        if (W(I_C72)) TRY(conv_wgrad(I_C72, U->a7_1, 128, 0, U->dz7_2, g, 2));
+        if (D(I_C71)) TRY(conv_dgrad(I_C72, U->dz7_2, U->dz7_1, 128, 0, U->a7_1, 2));
+        if (W(I_C71)) TRY(conv_wgrad(I_C71, U->cat7, 256, 0, U->dz7_1, g, 2));
+        if (D(I_UP7)) TRY(concat_dgrad(I_C71, U->dz7_1, U->dcat7, 2));
+        if (W(I_UP7)) TRY(deconv_wgrad(I_UP7, U->a6_2, U->dcat7, 128, g, 3));
+        if (D(I_C62)) TRY(deconv_dgrad(I_UP7, U->dcat7, 128, U->dz6_2, U->a6_2, 3));
+        if (W(I_C62)) TRY(conv_wgrad(I_C62, U->a6_1, 256, 0, U->dz6_2, g, 3));
+        if (D(I_C61)) TRY(conv_dgrad(I_C62, U->dz6_2, U->dz6_1, 256, 0, U->a6_1, 3));
+        if (W(I_C61)) TRY(conv_wgrad(I_C61, U->cat6, 512, 0, U->dz6_1, g, 3));
+        if (D(I_UP6)) TRY(concat_dgrad(I_C61, U->dz6_1, U->dcat6, 3));
+        if (W(I_UP6)) TRY(deconv_wgrad(I_UP6, U->a5_2, U->dcat6, 256, g, 4));
         TRY(finish_bucket(0, g));
-        TRY(deconv_dgrad(I_UP6, U->dcat6, 256, U->dz5_2, U->a5_2, 4));
+        if (D(I_C52)) TRY(deconv_dgrad(I_UP6, U->dcat6, 256, U->dz5_2, U->a5_2, 4));
         // bottleneck + encoder
-        TRY(conv_wgrad(I_C52, U->a5_1, 512, 0, U->dz5_2, g, 4));
-        TRY(conv_dgrad(I_C52, U->dz5_2, U->dz5_1, 512, 0, U->a5_1, 4));
-        TRY(conv_wgrad(I_C51, U->p4, 256, 0, U->dz5_1, g, 4));
+        if (W(I_C52)) TRY(conv_wgrad(I_C52, U->a5_1, 512, 0, U->dz5_2, g, 4));
+        if (D(I_C51)) TRY(conv_dgrad(I_C52, U->dz5_2, U->dz5_1, 512, 0, U->a5_1, 4));
+        if (W(I_C51)) TRY(conv_wgrad(I_C51, U->p4, 256, 0, U->dz5_1, g, 4));
         TRY(finish_bucket(1, g));
-        TRY(conv_dgrad(I_C51, U->dz5_1, U->dp4, 256, 0, nullptr, 4));
-        TRY(pool_bwd(U->pc4, skip_half(U->dcat6, 3, 256), U->dp4, U->dz4_2, 256, 4));
-        TRY(conv_wgrad(I_C42, U->a4_1, 256, 0, U->dz4_2, g, 3));
-        TRY(conv_dgrad(I_C42, U->dz4_2, U->dz4_1, 256, 0, U->a4_1, 3));
-        TRY(conv_wgrad(I_C41, U->p3, 128, 0, U->dz4_1, g, 3));
-        TRY(conv_dgrad(I_C41, U->dz4_1, U->dp3, 128, 0, nullptr, 3));
-        TRY(pool_bwd(U->pc3, skip_half(U->dcat7, 2, 128), U->dp3, U->dz3_2, 128, 3));
-        TRY(conv_wgrad(I_C32, U->a3_1, 128, 0, U->dz3_2, g, 2));
-        TRY(conv_dgrad(I_C32, U->dz3_2, U->dz3_1, 128, 0, U->a3_1, 2));
-        TRY(conv_wgrad(I_C31, U->p2, 64, 0, U->dz3_1, g, 2));
-        TRY(conv_dgrad(I_C31, U->dz3_1, U->dp2, 64, 0, nullptr, 2));
-        TRY(pool_bwd(U->pc2, skip_half(U->dcat8, 1, 64), U->dp2, U->dz2_2, 64, 2));
-        TRY(conv_wgrad(I_C22, U->a2_1, 64, 0, U->dz2_2, g, 1));
-        TRY(conv_dgrad(I_C22, U->dz2_2, U->dz2_1, 64, 0, U->a2_1, 1));
-        TRY(conv_wgrad(I_C21, U->p1, 32, 0, U->dz2_1, g, 1));
+        if (D(I_C42)) TRY(conv_dgrad(I_C51, U->dz5_1, U->dp4, 256, 0, nullptr, 4));
+        if (D(I_C42)) TRY(pool_bwd(U->pc4, skip_half(U->dcat6, 3, 256), U->dp4, U->dz4_2, 256, 4));
+        if (W(I_C42)) TRY(conv_wgrad(I_C42, U->a4_1, 256, 0, U->dz4_2, g, 3));
+        if (D(I_C41)) TRY(conv_dgrad(I_C42, U->dz4_2, U->dz4_1, 256, 0, U->a4_1, 3));
+        if (W(I_C41)) TRY(conv_wgrad(I_C41, U->p3, 128, 0, U->dz4_1, g, 3));
+        if (D(I_C32)) TRY(conv_dgrad(I_C41, U->dz4_1, U->dp3, 128, 0, nullptr, 3));
+        if (D(I_C32)) TRY(pool_bwd(U->pc3, skip_half(U->dcat7, 2, 128), U->dp3, U->dz3_2, 128, 3));
+        if (W(I_C32)) TRY(conv_wgrad(I_C32, U->a3_1, 128, 0, U->dz3_2, g, 2));
+        if (D(I_C31)) TRY(conv_dgrad(I_C32, U->dz3_2, U->dz3_1, 128, 0, U->a3_1, 2));
+        if (W(I_C31)) TRY(conv_wgrad(I_C31, U->p2, 64, 0, U->dz3_1, g, 2));
+        if (D(I_C22)) TRY(conv_dgrad(I_C31, U->dz3_1, U->dp2, 64, 0, nullptr, 2));
+        if (D(I_C22)) TRY(pool_bwd(U->pc2, skip_half(U->dcat8, 1, 64), U->dp2, U->dz2_2, 64, 2));
+        if (W(I_C22)) TRY(conv_wgrad(I_C22, U->a2_1, 64, 0, U->dz2_2, g, 1));
+        if (D(I_C21)) TRY(conv_dgrad(I_C22, U->dz2_2, U->dz2_1, 64, 0, U->a2_1, 1));
+        if (W(I_C21)) TRY(conv_wgrad(I_C21, U->p1, 32, 0, U->dz2_1, g, 1));
         TRY(finish_bucket(2, g));
-        TRY(conv_dgrad(I_C21, U->dz2_1, U->dp1, 32, 0, nullptr, 1));
-        TRY(pool_bwd(U->pc1, skip_half(U->dcat9, 0, 32), U->dp1, U->dz1_2, 32, 1));
-        TRY(conv_wgrad(I_C12, U->a1_1, 32, 0, U->dz1_2, g, 0));
-        TRY(conv_dgrad(I_C12, U->dz1_2, U->dz1_1, 32, 0, U->a1_1, 0));
-        {
+        if (D(I_C12)) TRY(conv_dgrad(I_C21, U->dz2_1, U->dp1, 32, 0, nullptr, 1));
+        if (D(I_C12)) TRY(pool_bwd(U->pc1, skip_half(U->dcat9, 0, 32), U->dp1, U->dz1_2, 32, 1));
+        if (W(I_C12)) TRY(conv_wgrad(I_C12, U->a1_1, 32, 0, U->dz1_2, g, 0));
+        if (D(I_C11)) TRY(conv_dgrad(I_C12, U->dz1_2, U->dz1_1, 32, 0, U->a1_1, 0));
+        if (W(I_C11)) {
             const double px = (double)U->n * U->H * U->W;
             Scope sc(u, st, "conv1_1", "wgrad", 2.0 * px * 32 * 9 * U->cin0, px * (4 * U->cin0 + 64));
             TRY(launch_first_conv_wgrad(ctx(), x, U->cin0, U->dz1_1, 32, g + U->L[I_C11].w_off, g + U->L[I_C11].b_off, U->n, U->H, U->W, st));
@@ -751,13 +814,17 @@ extern "C" int eld_unet_train_step(eld_unet* u, const float* params, const float
     ELD_CHECK_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), r.st));
     TRY(r.forward(x));
     {
+        // conv10_1 frozen: no dW10 / db10 reduction; nothing below it needed: no dz9_2 (then the step is forward + loss)
+        const bool dz = u->reach[I_C92], dw = u->wgrad[I_C10];
         const double hpx = (double)u->n * u->H * u->W;
-        Scope sc(u, r.st, "conv10_1", "fwd+loss+bwd", 6.0 * hpx * 128, hpx * (64 + 16 + 16 + 64));
-        TRY(launch_head(u->ctx, u->a9_2, params + u->L[I_C10].w_off, params + u->L[I_C10].b_off, out, target, u->dz9_2,
-                        grads + u->L[I_C10].w_off, grads + u->L[I_C10].b_off, loss, u->n, (size_t)u->H * u->W, u->cout_last, u->l2_loss, r.st));
+        Scope sc(u, r.st, "conv10_1", dz || dw ? "fwd+loss+bwd" : "fwd+loss", (dz || dw ? 6.0 : 2.0) * hpx * 128,
+                 hpx * (64 + 16 + 16 + (dz ? 64 : 0)));
+        TRY(launch_head(u->ctx, u->a9_2, params + u->L[I_C10].w_off, params + u->L[I_C10].b_off, out, target, dz ? u->dz9_2 : nullptr,
+                        dw ? grads + u->L[I_C10].w_off : nullptr, dw ? grads + u->L[I_C10].b_off : nullptr, loss, u->n,
+                        (size_t)u->H * u->W, u->cout_last, u->l2_loss, r.st));
     }
     TRY(r.backward(x, grads));
-    u->dz1_1_final = true;
+    u->dz1_1_final = u->reach[I_C11];
     return ELD_OK;
 }
 
@@ -769,16 +836,27 @@ extern "C" int eld_unet_backward(eld_unet* u, const float* params, const float* 
     Runner r{ u, params, static_cast<cudaStream_t>(stream) };
     ELD_CHECK_CUDA(cudaMemsetAsync(grads, 0, u->n_params * sizeof(float), r.st));
     ELD_CHECK_CUDA(cudaMemsetAsync(u->gtmp, 0, u->n_params * sizeof(float), r.st));
-    {
+    if (u->reach[I_C10]) {
+        const bool dz = u->reach[I_C92], dw = u->wgrad[I_C10];
         const double hpx = (double)u->n * u->H * u->W;
-        Scope sc(u, r.st, "conv10_1", "bwd", 4.0 * hpx * 128, hpx * (64 + 16 + 64));
+        Scope sc(u, r.st, "conv10_1", "bwd", 4.0 * hpx * 128, hpx * (64 + 16 + (dz ? 64 : 0)));
         // the head re-forms `out` into scratch (dz1_1 is not written before the very end of backward) and back-propagates dout
         TRY(launch_head(u->ctx, u->a9_2, params + u->L[I_C10].w_off, params + u->L[I_C10].b_off,
-                        reinterpret_cast<float*>(u->dz1_1), dout, u->dz9_2,
-                        grads + u->L[I_C10].w_off, grads + u->L[I_C10].b_off, nullptr, u->n, (size_t)u->H * u->W, u->cout_last, 2, r.st));
+                        reinterpret_cast<float*>(u->dz1_1), dout, dz ? u->dz9_2 : nullptr,
+                        dw ? grads + u->L[I_C10].w_off : nullptr, dw ? grads + u->L[I_C10].b_off : nullptr, nullptr, u->n,
+                        (size_t)u->H * u->W, u->cout_last, 2, r.st));
     }
     TRY(r.backward(x, grads));
-    u->dz1_1_final = true;
+    u->dz1_1_final = u->reach[I_C11];
+    return ELD_OK;
+}
+
+extern "C" int eld_unet_set_trainable(eld_unet* u, const uint8_t* flags, int n_flags, int input_grad)
+{
+    ELD_REQUIRE(u && flags, "eld_unet_set_trainable: NULL argument");
+    ELD_REQUIRE(n_flags == 2 * kNumLayers, "eld_unet_set_trainable: %d flags; want %d (weight, bias of every layer in state_dict order)",
+                n_flags, 2 * kNumLayers);
+    derive_needs(u, flags, input_grad != 0);
     return ELD_OK;
 }
 
@@ -803,6 +881,16 @@ extern "C" int eld_adam_step(eld_ctx* ctx, float* params, const float* grads, fl
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     return launch_adam(ctx, params, grads, m, v, n, lr, beta1, beta2, eps, weight_decay, step, grad_scale,
                        static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int eld_adam_step_segments(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, const size_t* segs,
+                                      const int* steps, int n_segs, float lr, float beta1, float beta2, float eps,
+                                      float weight_decay, float grad_scale, void* stream)
+{
+    ELD_REQUIRE(ctx && params && grads && m && v && (n_segs == 0 || (segs && steps)), "eld_adam_step_segments: NULL argument");
+    ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
+    return launch_adam_segments(ctx, params, grads, m, v, segs, steps, n_segs, lr, beta1, beta2, eps, weight_decay, grad_scale,
+                                static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int eld_unet_set_loss(eld_unet* u, int kind)

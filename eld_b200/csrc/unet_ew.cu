@@ -230,32 +230,34 @@ head_kernel(const __nv_bfloat16* __restrict__ a, const float* __restrict__ w, co
                 g1 *= (av[j + 1] > 0.f ? 1.0f : 0.2f);
                 zo[j >> 1] = pack_bf2(g0, g1);
             }
-            if (valid) reinterpret_cast<uint4*>(dz + (size_t)p * 32)[q] = make_uint4(zo[0], zo[1], zo[2], zo[3]);
+            if (valid && dz) reinterpret_cast<uint4*>(dz + (size_t)p * 32)[q] = make_uint4(zo[0], zo[1], zo[2], zo[3]);
         }
     }
     cp_async_wait<0>();
     if (TRAIN) {
         // reduce over the 8 lanes of a warp that share `q` (lane ^ 4, 8, 16), then shared atomics, then one global
-        // atomic per value per block
+        // atomic per value per block.  dw == db == nullptr: conv10_1 is frozen, only the loss is reduced.
+        if (dw) {
 #pragma unroll
-        for (int co = 0; co < 4; ++co)
+            for (int co = 0; co < 4; ++co)
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                float x = pdw[co][j];
-                x += __shfl_xor_sync(0xffffffffu, x, 4);
-                x += __shfl_xor_sync(0xffffffffu, x, 8);
-                x += __shfl_xor_sync(0xffffffffu, x, 16);
-                if (lane < 4) atomicAdd(&red[co * 32 + q * 8 + j], x);
-            }
-        float x = pdb;
-        x += __shfl_xor_sync(0xffffffffu, x, 4); x += __shfl_xor_sync(0xffffffffu, x, 8); x += __shfl_xor_sync(0xffffffffu, x, 16);
-        if (lane < 4) atomicAdd(&red[128 + q], x);
+                for (int j = 0; j < 8; ++j) {
+                    float x = pdw[co][j];
+                    x += __shfl_xor_sync(0xffffffffu, x, 4);
+                    x += __shfl_xor_sync(0xffffffffu, x, 8);
+                    x += __shfl_xor_sync(0xffffffffu, x, 16);
+                    if (lane < 4) atomicAdd(&red[co * 32 + q * 8 + j], x);
+                }
+            float x = pdb;
+            x += __shfl_xor_sync(0xffffffffu, x, 4); x += __shfl_xor_sync(0xffffffffu, x, 8); x += __shfl_xor_sync(0xffffffffu, x, 16);
+            if (lane < 4) atomicAdd(&red[128 + q], x);
+        }
         float ls = ploss;
 #pragma unroll
         for (int sft = 16; sft > 0; sft >>= 1) ls += __shfl_xor_sync(0xffffffffu, ls, sft);
         if (lane == 0) atomicAdd(&red[132], ls);
         __syncthreads();
-        for (int i = tid; i < 133; i += kHeadThreads) {
+        for (int i = dw ? tid : 132 + tid; i < 133; i += kHeadThreads) {
             if (i < 128) { if ((i >> 5) < cout) atomicAdd(dw + i, red[i]); }
             else if (i < 132) { if (i - 128 < cout) atomicAdd(db + (i - 128), red[i]); }
             else if (loss) atomicAdd(loss, red[132] * inv_numel);
@@ -266,20 +268,41 @@ head_kernel(const __nv_bfloat16* __restrict__ a, const float* __restrict__ w, co
 // ---------------------------------------------------------------------------------------------------
 // Adam (torch.optim.Adam semantics, ELD_model.py:400-401): one pass over the flat parameter buffer.
 // ---------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void adam_elem(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                                          float* __restrict__ v, size_t i, float lr, float b1, float b2, float eps, float wd,
+                                          float bc1, float bc2_sqrt, float gscale)
+{
+    float gi = g[i] * gscale;
+    const float pi = p[i];
+    if (wd != 0.f) gi = fmaf(wd, pi, gi);
+    const float mi = fmaf(b1, m[i], (1.f - b1) * gi);
+    const float vi = fmaf(b2, v[i], (1.f - b2) * gi * gi);
+    m[i] = mi;
+    v[i] = vi;
+    const float denom = sqrtf(vi) / bc2_sqrt + eps;
+    p[i] = pi - (lr / bc1) * (mi / denom);
+}
+
 __global__ void __launch_bounds__(256)
 adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
             size_t n, float lr, float b1, float b2, float eps, float wd, float bc1, float bc2_sqrt, float gscale)
 {
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        float gi = g[i] * gscale;
-        const float pi = p[i];
-        if (wd != 0.f) gi = fmaf(wd, pi, gi);
-        const float mi = fmaf(b1, m[i], (1.f - b1) * gi);
-        const float vi = fmaf(b2, v[i], (1.f - b2) * gi * gi);
-        m[i] = mi;
-        v[i] = vi;
-        const float denom = sqrtf(vi) / bc2_sqrt + eps;
-        p[i] = pi - (lr / bc1) * (mi / denom);
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        adam_elem(p, g, m, v, i, lr, b1, b2, eps, wd, bc1, bc2_sqrt, gscale);
+}
+
+// The same update on a list of (offset, count) ranges, each with its own step count (torch.optim.Adam keeps
+// state['step'] per parameter: a tensor that was frozen for a while has taken fewer steps than its neighbours).
+// Every segment is walked by the whole grid; the table travels in the kernel parameters.
+__global__ void __launch_bounds__(256)
+adam_segments_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                     const __grid_constant__ AdamSegments S, float lr, float b1, float b2, float eps, float wd, float gscale)
+{
+    const size_t t0 = blockIdx.x * (size_t)blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
+    for (int s = 0; s < S.n; ++s) {
+        const size_t off = S.off[s], end = S.off[s] + S.cnt[s];
+        for (size_t i = off + t0; i < end; i += stride)
+            adam_elem(p, g, m, v, i, lr, b1, b2, eps, wd, S.bc1[s], S.bc2_sqrt[s], gscale);
     }
 }
 
@@ -352,6 +375,27 @@ int launch_adam(eld_ctx* ctx, float* p, const float* g, float* m, float* v, size
     const float bc1 = 1.0f - powf(b1, (float)step);
     const float bc2 = 1.0f - powf(b2, (float)step);
     adam_kernel<<<grid_for(n, 256 * 4, 8 * ctx->num_sms), 256, 0, st>>>(p, g, m, v, n, lr, b1, b2, eps, wd, bc1, sqrtf(bc2), gscale);
+    ELD_CHECK_CUDA(cudaGetLastError());
+    count_launch(ctx);
+    return ELD_OK;
+}
+
+int launch_adam_segments(eld_ctx* ctx, float* p, const float* g, float* m, float* v, const size_t* segs, const int* steps,
+                         int n_segs, float lr, float b1, float b2, float eps, float wd, float gscale, cudaStream_t st)
+{
+    ELD_REQUIRE(n_segs >= 0 && n_segs <= kAdamMaxSegments, "adam: %d segments (at most %d)", n_segs, kAdamMaxSegments);
+    AdamSegments S{};
+    size_t total = 0;
+    for (int s = 0; s < n_segs; ++s) {
+        ELD_REQUIRE(steps[s] >= 1, "adam: segment %d: step counts from 1", s);
+        S.off[s] = segs[2 * s]; S.cnt[s] = segs[2 * s + 1];
+        S.bc1[s] = 1.0f - powf(b1, (float)steps[s]);                 // the bias corrections of launch_adam, per segment
+        S.bc2_sqrt[s] = sqrtf(1.0f - powf(b2, (float)steps[s]));
+        total += S.cnt[s];
+    }
+    S.n = n_segs;
+    if (total == 0) return ELD_OK;
+    adam_segments_kernel<<<grid_for(total, 256 * 4, 8 * ctx->num_sms), 256, 0, st>>>(p, g, m, v, S, lr, b1, b2, eps, wd, gscale);
     ELD_CHECK_CUDA(cudaGetLastError());
     count_launch(ctx);
     return ELD_OK;

@@ -10,4 +10,13 @@ int launch_head(eld_ctx* ctx, const void* a, const float* w, const float* b, flo
 int launch_clock_probe(eld_ctx* ctx, float* out_mhz, cudaStream_t st);
 int launch_adam(eld_ctx* ctx, float* p, const float* g, float* m, float* v, size_t n, float lr, float b1, float b2,
                 float eps, float wd, int step, float gscale, cudaStream_t st);
+// Adam over (offset, count) ranges of the flat buffers with one step count per range, one launch
+constexpr int kAdamMaxSegments = 64;    // one per parameter tensor of the U-Net (46) fits
+struct AdamSegments {
+    unsigned long long off[kAdamMaxSegments], cnt[kAdamMaxSegments];
+    float bc1[kAdamMaxSegments], bc2_sqrt[kAdamMaxSegments];
+    int n;
+};
+int launch_adam_segments(eld_ctx* ctx, float* p, const float* g, float* m, float* v, const size_t* segs, const int* steps,
+                         int n_segs, float lr, float b1, float b2, float eps, float wd, float gscale, cudaStream_t st);
 }  // namespace eld

@@ -71,7 +71,13 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
                                      (reinterpret_cast<uintptr_t>(op.out2) & 31) == 0),
                 "conv tile: split store needs a plain store epilogue, a second tensor and a split at a multiple of 32 columns");
     p.out2 = static_cast<__nv_bfloat16*>(op.out2); p.out2_pitch = op.out2_pitch; p.out_split = op.out_split;
-    p.b_rows = op.n_total <= 256 ? op.n_total : 256;
+    // block stride of the packed operand: its own row count (min(rows, 256)), whatever prefix of the rows the GEMM reads.
+    // A prefix starts at row 0 of every block and covers whole 32-row groups, so each tile's rows keep the swizzle
+    // phase (row & 7, or (row >> 1) & 3) they were packed with.
+    ELD_REQUIRE(op.b_block_rows == 0 || (op.b_block_rows % 32 == 0 && op.b_block_rows <= 256 &&
+                                         (op.n_total <= op.b_block_rows || op.b_block_rows == 256) && op.aux_sign == nullptr),
+                "conv tile: a row prefix of the packed operand needs whole 32-row groups of its blocks and no sign-word mask");
+    p.b_rows = op.b_block_rows ? op.b_block_rows : (op.n_total <= 256 ? op.n_total : 256);
     // N per tile: 32, 64 or 128 (a 64 x 256 f32 accumulator would take 128 registers per consumer thread and spill
     // next to the epilogue)
     p.n_tile = (op.n_total % 128 == 0) ? 128 : (op.n_total % 64 == 0) ? 64 : 32;

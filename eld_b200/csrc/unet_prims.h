@@ -49,6 +49,8 @@ struct GemmOp {
     void* pool_code = nullptr;  // optional with pool_out: 1 byte per pooled element (argmax + signs) for the pool backward
     void* out2 = nullptr;       // EPI_STORE split store: columns >= out_split go to out2 (planar halves of a concat gradient)
     int out2_pitch = 0, out_split = 0;
+    int b_block_rows = 0;       // rows of one packed weight block when the GEMM reads only the first n_total rows of each
+                                // (a prefix of the output channels); 0 = the operand has exactly n_total rows
 };
 
 struct WgradOp {

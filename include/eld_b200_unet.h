@@ -94,6 +94,15 @@ int    eld_unet_backward(eld_unet* u, const float* params, const float* x, const
  * dx f32 NCHW [n][cin][h][w], overwritten.  bf16 conv1_1 gradient and weights, fp32 accumulation.  Fails on an object
  * created with train = 0 and when no backward or train step has run since the last forward. */
 int    eld_unet_input_grad(eld_unet* u, const float* params, float* dx, void* stream);
+/* Frozen parameters (p.requires_grad_(False) in the reference, ELD_model.py:473-475): which gradients the following
+ * eld_unet_train_step / eld_unet_backward compute.  flags: one byte per parameter tensor in state_dict order (46: weight
+ * and bias of every layer), nonzero = trainable; input_grad != 0 keeps the data-gradient chain running down to conv1_1
+ * so that eld_unet_input_grad stays valid.  A layer's weight-gradient launch runs when its weight or its bias trains;
+ * the data-gradient chain runs from the head down to the deepest tensor something still needs (a trainable layer below
+ * it, or the frame), and a concat's skip half only when the encoder side needs it.  The `grads` range of a frozen tensor
+ * reads zero; every bucket event is still recorded.  Default (and after all ones, input_grad = 1): everything, as
+ * before.  Host-side only: no launch, no synchronisation. */
+int    eld_unet_set_trainable(eld_unet* u, const uint8_t* flags, int n_flags, int input_grad);
 /* Pixel loss of eld_unet_train_step (models/losses.py:29-36, --loss): 0 = nn.L1Loss (default), 1 = nn.MSELoss. */
 #define ELD_LOSS_L1 0
 #define ELD_LOSS_L2 1
@@ -122,5 +131,11 @@ int    eld_unet_profile_read(eld_unet* u, int max, char* names32, float* ms, dou
 int    eld_adam_step(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, size_t n,
                      float lr, float beta1, float beta2, float eps, float weight_decay, int step,
                      float grad_scale, void* stream);
+/* The same update on n_segs ranges of the flat buffers in ONE launch: segs (host) = (offset, count) pairs, steps (host) =
+ * each range's own step count (torch.optim.Adam's per-parameter state['step']: a tensor that was frozen for a while has
+ * taken fewer steps).  Elements outside the ranges are not touched.  n_segs <= 64. */
+int    eld_adam_step_segments(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, const size_t* segs,
+                              const int* steps, int n_segs, float lr, float beta1, float beta2, float eps,
+                              float weight_decay, float grad_scale, void* stream);
 
 #endif
