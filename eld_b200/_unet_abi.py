@@ -45,3 +45,4 @@ def declare_engine(lib):
     lib.eld_clock_probe.argtypes = [vp, vp, vp]
     lib.eld_unet_profile.argtypes = [vp, i32]
     lib.eld_unet_profile_read.argtypes = [vp, i32, c.c_char_p, vp, vp, vp, c.POINTER(i32)]
+    lib.eld_unet_buffer.argtypes = [vp, c.c_char_p, c.POINTER(vp), c.POINTER(i32), c.POINTER(i32)]

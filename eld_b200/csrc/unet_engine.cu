@@ -872,6 +872,81 @@ extern "C" int eld_unet_input_grad(eld_unet* u, const float* params, float* dx, 
     return launch_first_conv_dgrad(u->ctx, u->dz1_1, params + u->L[I_C11].w_off, u->cin0, dx, u->n, u->H, u->W, st);
 }
 
+// The intermediate tensors of the step by name: member, level (1/2^lvl of the frame), units per pixel, training only.
+// A gradient of a concat input (dcat*) is the whole planar buffer: [n][h][w][C/2] up plane, then the skip plane.
+static const struct { const char* name; __nv_bfloat16* eld_unet::*p; int lvl, ch; bool train; } kBuffers[] = {
+    { "a1_1", &eld_unet::a1_1, 0, 32, false },  { "cat9", &eld_unet::cat9, 0, 64, false },   { "p1", &eld_unet::p1, 1, 32, false },
+    { "a2_1", &eld_unet::a2_1, 1, 64, false },  { "cat8", &eld_unet::cat8, 1, 128, false },  { "p2", &eld_unet::p2, 2, 64, false },
+    { "a3_1", &eld_unet::a3_1, 2, 128, false }, { "cat7", &eld_unet::cat7, 2, 256, false },  { "p3", &eld_unet::p3, 3, 128, false },
+    { "a4_1", &eld_unet::a4_1, 3, 256, false }, { "cat6", &eld_unet::cat6, 3, 512, false },  { "p4", &eld_unet::p4, 4, 256, false },
+    { "a5_1", &eld_unet::a5_1, 4, 512, false }, { "a5_2", &eld_unet::a5_2, 4, 512, false },
+    { "a6_1", &eld_unet::a6_1, 3, 256, false }, { "a6_2", &eld_unet::a6_2, 3, 256, false },
+    { "a7_1", &eld_unet::a7_1, 2, 128, false }, { "a7_2", &eld_unet::a7_2, 2, 128, false },
+    { "a8_1", &eld_unet::a8_1, 1, 64, false },  { "a8_2", &eld_unet::a8_2, 1, 64, false },
+    { "a9_1", &eld_unet::a9_1, 0, 32, false },  { "a9_2", &eld_unet::a9_2, 0, 32, false },
+    { "dz9_2", &eld_unet::dz9_2, 0, 32, true },  { "dz9_1", &eld_unet::dz9_1, 0, 32, true },  { "dcat9", &eld_unet::dcat9, 0, 64, true },
+    { "dz8_2", &eld_unet::dz8_2, 1, 64, true },  { "dz8_1", &eld_unet::dz8_1, 1, 64, true },  { "dcat8", &eld_unet::dcat8, 1, 128, true },
+    { "dz7_2", &eld_unet::dz7_2, 2, 128, true }, { "dz7_1", &eld_unet::dz7_1, 2, 128, true }, { "dcat7", &eld_unet::dcat7, 2, 256, true },
+    { "dz6_2", &eld_unet::dz6_2, 3, 256, true }, { "dz6_1", &eld_unet::dz6_1, 3, 256, true }, { "dcat6", &eld_unet::dcat6, 3, 512, true },
+    { "dz5_2", &eld_unet::dz5_2, 4, 512, true }, { "dz5_1", &eld_unet::dz5_1, 4, 512, true }, { "dp4", &eld_unet::dp4, 4, 256, true },
+    { "dz4_2", &eld_unet::dz4_2, 3, 256, true }, { "dz4_1", &eld_unet::dz4_1, 3, 256, true }, { "dp3", &eld_unet::dp3, 3, 128, true },
+    { "dz3_2", &eld_unet::dz3_2, 2, 128, true }, { "dz3_1", &eld_unet::dz3_1, 2, 128, true }, { "dp2", &eld_unet::dp2, 2, 64, true },
+    { "dz2_2", &eld_unet::dz2_2, 1, 64, true },  { "dz2_1", &eld_unet::dz2_1, 1, 64, true },  { "dp1", &eld_unet::dp1, 1, 32, true },
+    { "dz1_2", &eld_unet::dz1_2, 0, 32, true },  { "dz1_1", &eld_unet::dz1_1, 0, 32, true },
+};
+
+/* Host-side view of the workspace for tests and debugging: where tensor `name` of the last step lives.  No launch. */
+extern "C" int eld_unet_buffer(const eld_unet* u, const char* name, void** ptr, int dims[4], int* elem_bytes)
+{
+    ELD_REQUIRE(u && name && ptr && dims && elem_bytes, "eld_unet_buffer: NULL argument");
+    const bool train = u->dz9_2 != nullptr;
+    auto put = [&](const void* p, int n, int h, int w, int units, int eb) {
+        *ptr = const_cast<void*>(p); dims[0] = n; dims[1] = h; dims[2] = w; dims[3] = units; *elem_bytes = eb;
+        return ELD_OK;
+    };
+    for (const auto& b : kBuffers) {
+        if (strcmp(name, b.name) != 0) continue;
+        ELD_REQUIRE(train || !b.train, "eld_unet_buffer: '%s' exists only in a training workspace", name);
+        return put(u->*b.p, u->n, u->H >> b.lvl, u->W >> b.lvl, b.ch, 2);
+    }
+    // pool codes: one byte per pooled element (32 bytes per pooled pixel and 32 channels)
+    static const struct { const char* name; __nv_bfloat16* eld_unet::*p; int lvl, ch; } kCodes[] = {
+        { "pc1", &eld_unet::pc1, 1, 32 }, { "pc2", &eld_unet::pc2, 2, 64 }, { "pc3", &eld_unet::pc3, 3, 128 }, { "pc4", &eld_unet::pc4, 4, 256 },
+    };
+    for (const auto& c : kCodes) {
+        if (strcmp(name, c.name) != 0) continue;
+        ELD_REQUIRE(train, "eld_unet_buffer: '%s' exists only in a training workspace", name);
+        return put(u->*c.p, u->n, u->H >> c.lvl, u->W >> c.lvl, c.ch, 1);
+    }
+    if (strncmp(name, "sign:", 5) == 0) {            // sign words of an activation: uint32 [pixel][channels / 32]
+        for (const auto& b : kBuffers) {
+            if (b.train || strcmp(name + 5, b.name) != 0) continue;
+            for (int i = 0; i < u->n_signs; ++i)
+                if (u->signs[i].act == u->*b.p) return put(u->signs[i].words, u->n, u->H >> b.lvl, u->W >> b.lvl, b.ch / 32, 4);
+        }
+        set_error("eld_unet_buffer: no sign words '%s' in this workspace", name);
+        return ELD_E_ARG;
+    }
+    if (strncmp(name, "wf:", 3) == 0 || strncmp(name, "wd:", 3) == 0) {   // packed bf16 operands of one layer
+        const bool fprop = name[1] == 'f';
+        for (int i = 0; i < kNumLayers; ++i) {
+            const Layer& l = u->L[i];
+            if (strcmp(name + 3, l.name) != 0 || l.type == L_CONV1 || (i == I_C11 && !fprop)) continue;
+            // conv1_1: the [32 co][64 k] K-major image of first_conv.cuh; the others: the operand packed_index describes
+            const int count = i == I_C11 ? 32 * 64 : l.cin * l.cout * (l.type == L_CONV3 ? 9 : 4);
+            return put(u->packed + (fprop ? l.wf_off : l.wd_off), 1, 1, 1, count, 2);
+        }
+        set_error("eld_unet_buffer: no packed operand '%s'", name);
+        return ELD_E_ARG;
+    }
+    if (strcmp(name, "gtmp") == 0) {                 // [tap][ci][co] staging of the conv3x3 weight gradients, parameter offsets
+        ELD_REQUIRE(train, "eld_unet_buffer: 'gtmp' exists only in a training workspace");
+        return put(u->gtmp, 1, 1, 1, (int)u->n_params, 4);
+    }
+    set_error("eld_unet_buffer: unknown tensor '%s'", name);
+    return ELD_E_ARG;
+}
+
 extern "C" int eld_adam_step(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, size_t n,
                              float lr, float beta1, float beta2, float eps, float weight_decay, int step,
                              float grad_scale, void* stream)

@@ -128,6 +128,14 @@ int    eld_unet_profile(eld_unet* u, int enable);
  * for ~20 us and writes the SM clock in MHz that the preceding kernels were running at to *out_mhz_device. */
 int    eld_clock_probe(eld_ctx* ctx, float* out_mhz_device, void* stream);
 int    eld_unet_profile_read(eld_unet* u, int max, char* names32, float* ms, double* flops, double* bytes, int* count);
+/* Where intermediate tensor `name` of the last step lives in the caller's workspace (for tests and debugging; no launch,
+ * no synchronisation).  dims = {n, h, w, units per pixel}, *elem_bytes = 2 (bf16) / 4 (f32, uint32) / 1 (bytes).
+ * Names: activations a1_1, cat9, p1, ... a9_2; gradients dz9_2 ... dz1_1, dcat9 ... dcat6 (the whole planar buffer: up
+ * plane [n][h][w][units/2], then the skip plane), dp1 ... dp4; pool codes pc1 ... pc4 (one byte per pooled element);
+ * sign words sign:<activation> (uint32, one per pixel and 32 channels); packed operands wf:<layer>, wd:<layer> (dims
+ * {1, 1, 1, element count}); the [tap][ci][co] staging of the conv weight gradients gtmp (f32, parameter offsets).
+ * ELD_E_ARG for an unknown name and, on an object created with train = 0, for a training-only one. */
+int    eld_unet_buffer(const eld_unet* u, const char* name, void** ptr, int dims[4], int* elem_bytes);
 int    eld_adam_step(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, size_t n,
                      float lr, float beta1, float beta2, float eps, float weight_decay, int step,
                      float grad_scale, void* stream);

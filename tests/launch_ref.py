@@ -1,0 +1,273 @@
+"""Float64 references of every launch kind of the U-Net step, one function per kind, for test_launches_gpu.py.
+
+Each reference takes the launch's ACTUAL inputs as the engine stored them (teacher forcing: the bf16 activation or
+gradient tensors read from the workspace, the bf16-rounded weights the packed operands hold), computes in float64 and
+returns (r, S): r = the exact value before the kernel's single rounding point, S = the same linear operation on
+|inputs| x |weights| (the scale of the fp32 accumulation error).  Tensors are NHWC, like the engine's, so that a
+reference lines up with the workspace view element for element; the convolutions are sums of per-tap matrix products.
+
+`buffer()` maps an engine tensor name to a torch view of the module's workspace; the layout itself is the engine's
+(eld_unet_buffer), never restated here.
+"""
+import ctypes
+
+import torch
+import torch.nn.functional as F
+
+_DT = {1: torch.uint8, 2: torch.bfloat16, 4: torch.float32}
+
+
+def buffer(lib, eng, ws, name):
+    """torch view [n, h, w, units] of tensor `name` inside workspace `ws` (uint8 tensor) of engine `eng`; sign words
+    are int32, pool codes uint8, gtmp float32, everything else bf16.  Raises EldError for a name the engine lacks."""
+    from eld_b200 import _lib
+    ptr, dims, eb = ctypes.c_void_p(), (ctypes.c_int * 4)(), ctypes.c_int()
+    _lib.check(lib.eld_unet_buffer(eng, name.encode(), ctypes.byref(ptr), dims, ctypes.byref(eb)), 'eld_unet_buffer')
+    n, h, w, u = list(dims)
+    off, count = ptr.value - ws.data_ptr(), n * h * w * u * eb.value
+    assert 0 <= off and off + count <= ws.numel(), (name, off, count, ws.numel())
+    dt = torch.int32 if name.startswith('sign:') else _DT[eb.value]
+    return ws[off:off + count].view(dt).view(n, h, w, u)
+
+
+# ---- rounding -------------------------------------------------------------------------------------------------------
+def bf(t):
+    """fp32 -> bf16 (round to nearest even) -> float64: what a packed operand or an im2col tile holds"""
+    return t.float().bfloat16().double()
+
+
+def ulp_bf16(r):
+    """spacing of bf16 numbers at |r| (8 significant bits), normal range"""
+    _, e = torch.frexp(r.abs().clamp_min(2.0 ** -126))
+    return torch.ldexp(torch.ones_like(r), (e - 8).to(torch.int32))
+
+
+def slope(a):
+    """LeakyReLU' from the sign of the stored activation: 1, or 0.2 where the sign bit is set (+0 counts positive)"""
+    return 1.0 - 0.8 * torch.signbit(a.float()).double()
+
+
+def lrelu(v):
+    return torch.maximum(v, 0.2 * v)
+
+
+# ---- conv3x3 (pad 1) and deconv2x2 (stride 2) as per-tap matrix products on NHWC float64 --------------------------
+def _conv(x, w):
+    """x [n,h,w,ci], w [co,ci,3,3] -> [n,h,w,co]: y[p] = sum_taps x[p + (kh-1, kw-1)] W[:, :, kh, kw]^T"""
+    n, h, wd, _ = x.shape
+    xp = F.pad(x, (0, 0, 1, 1, 1, 1))
+    out = None
+    for kh in range(3):
+        for kw in range(3):
+            t = xp[:, kh:kh + h, kw:kw + wd, :] @ w[:, :, kh, kw].t()
+            out = t if out is None else out + t
+    return out
+
+
+def _conv_t(dz, w):
+    """data gradient of _conv: dz [n,h,w,co], w [co,ci,3,3] -> [n,h,w,ci]"""
+    n, h, wd, _ = dz.shape
+    dp = F.pad(dz, (0, 0, 1, 1, 1, 1))
+    out = None
+    for kh in range(3):
+        for kw in range(3):
+            t = dp[:, 2 - kh:2 - kh + h, 2 - kw:2 - kw + wd, :] @ w[:, :, kh, kw]
+            out = t if out is None else out + t
+    return out
+
+
+def _conv_w(x, dz):
+    """weight gradient of _conv: -> [co, ci, 3, 3]"""
+    n, h, wd, ci = x.shape
+    xp = F.pad(x, (0, 0, 1, 1, 1, 1))
+    q = dz.reshape(-1, dz.shape[-1])
+    g = torch.empty(dz.shape[-1], ci, 3, 3, dtype=torch.float64, device=x.device)
+    for kh in range(3):
+        for kw in range(3):
+            g[:, :, kh, kw] = q.t() @ xp[:, kh:kh + h, kw:kw + wd, :].reshape(-1, ci)
+    return g
+
+
+def _deconv(x, wt):
+    """x [n,h,w,ci], wt [ci,co,2,2] -> [n,2h,2w,co]"""
+    n, h, wd, _ = x.shape
+    y = torch.empty(n, 2 * h, 2 * wd, wt.shape[1], dtype=torch.float64, device=x.device)
+    for kh in range(2):
+        for kw in range(2):
+            y[:, kh::2, kw::2, :] = x @ wt[:, :, kh, kw]
+    return y
+
+
+def _deconv_t(dy, wt):
+    """data gradient of _deconv: dy [n,2h,2w,co] -> [n,h,w,ci]"""
+    out = None
+    for kh in range(2):
+        for kw in range(2):
+            t = dy[:, kh::2, kw::2, :] @ wt[:, :, kh, kw].t()
+            out = t if out is None else out + t
+    return out
+
+
+def _deconv_w(x, dy):
+    """weight gradient of _deconv: -> [ci, co, 2, 2]"""
+    ci, co = x.shape[-1], dy.shape[-1]
+    p = x.reshape(-1, ci)
+    g = torch.empty(ci, co, 2, 2, dtype=torch.float64, device=x.device)
+    for kh in range(2):
+        for kw in range(2):
+            g[:, :, kh, kw] = p.t() @ dy[:, kh::2, kw::2, :].reshape(-1, co)
+    return g
+
+
+# ---- references, one per launch kind ---------------------------------------------------------------------------------
+def conv_fprop(x, w, b, act=True):
+    """conv3x3 + bias (+ LeakyReLU): x stored bf16 NHWC, w fp32 master OIHW (the operand holds it rounded to bf16)"""
+    x, w, b = x.double(), bf(w), b.double()
+    r = _conv(x, w) + b
+    S = _conv(x.abs(), w.abs()) + b.abs()
+    return (lrelu(r) if act else r), S
+
+
+def first_conv_fprop(frame, w, b):
+    """conv1_1 from the fp32 NCHW frame: the im2col tile rounds the frame to bf16, the weights too; -> NHWC"""
+    return conv_fprop(bf(frame).permute(0, 2, 3, 1), w, b)
+
+
+def pool(a):
+    """MaxPool2d(2) of the stored activation a [n,h,w,c] -> (pooled [n,h/2,w/2,c] exact, window [..., 4] in the order
+    (0,0) (0,1) (1,0) (1,1), one-hot first arg-max [..., 4])"""
+    n, h, w, c = a.shape
+    win = a.float().reshape(n, h // 2, 2, w // 2, 2, c).permute(0, 1, 3, 5, 2, 4).reshape(n, h // 2, w // 2, c, 4)
+    m = win.amax(-1)
+    eq = win == m.unsqueeze(-1)
+    first = eq & (eq.int().cumsum(-1) == 1)
+    return m, win, first
+
+
+def _pack_bits(bits):
+    """bool [..., 32 channels] -> int32 word: channel 2j -> bit j, channel 2j+1 -> bit 16 + j"""
+    b = bits.long()
+    sh = torch.tensor([j // 2 + (16 if j % 2 else 0) for j in range(32)], device=bits.device)
+    w = (b << sh).sum(-1)
+    return torch.where(w >= 2 ** 31, w - 2 ** 32, w).int()
+
+
+def sign_words(a):
+    """sign words of the stored activation a [n,h,w,c] -> int32 [n,h,w,c/32]"""
+    n, h, w, c = a.shape
+    return _pack_bits(torch.signbit(a.float()).reshape(n, h, w, c // 32, 32))
+
+
+def pool_code(a):
+    """the 32-byte pool code per (pooled pixel, 32 channels) as int32 [n,h/2,w/2,c/32,8]: words 0-3 = "is not the
+    window's maximum" of the window elements (0,0) (0,1) (1,0) (1,1), words 4-7 = their sign bits (channel bits as in
+    sign_words).  The pool backward takes the first window element whose bit is clear."""
+    m, win, _ = pool(a)
+    n, h2, w2, c, _ = win.shape
+    ne = (win != m.unsqueeze(-1)).reshape(n, h2, w2, c // 32, 32, 4)
+    sg = torch.signbit(win).reshape(n, h2, w2, c // 32, 32, 4)
+    return torch.stack([_pack_bits(ne[..., k]) for k in range(4)] + [_pack_bits(sg[..., k]) for k in range(4)], -1)
+
+
+def deconv_fprop(x, wt, b):
+    """ConvTranspose2d(2, stride 2) + bias, pixel-shuffled: x stored bf16 [n,h,w,ci], wt fp32 IOHW"""
+    x, wt, b = x.double(), bf(wt), b.double()
+    return _deconv(x, wt) + b, _deconv(x.abs(), wt.abs()) + b.abs()
+
+
+def conv_dgrad(dz, w, act=None):
+    """conv3x3 data gradient (transposed, pad 1) of the stored bf16 dz [n,h,w,co] with the bf16 weights, times the
+    LeakyReLU' of the stored activation `act` (None: no mask) -> [n,h,w,ci]"""
+    dz, w = dz.double(), bf(w)
+    r, S = _conv_t(dz, w), _conv_t(dz.abs(), w.abs())
+    if act is not None:
+        s = slope(act)
+        r, S = r * s, S * s
+    return r, S
+
+
+def deconv_dgrad(dy, wt, act):
+    """deconv data gradient: gather of the up plane dy [n,2h,2w,co], bf16 weights, LeakyReLU' of `act` [n,h,w,ci]"""
+    dy, wt = dy.double(), bf(wt)
+    s = slope(act)
+    return _deconv_t(dy, wt) * s, _deconv_t(dy.abs(), wt.abs()) * s
+
+
+def pool_bwd(a, dskip, dp):
+    """dZ = (dskip + dp routed to the first arg-max of its window) * LeakyReLU'(a); a = the pooled activation"""
+    _, _, first = pool(a)
+    n, h, w, c = a.shape
+    g = (first.double() * dp.double().unsqueeze(-1)).reshape(n, h // 2, w // 2, c, 2, 2)
+    g = g.permute(0, 1, 4, 2, 5, 3).reshape(n, h, w, c)
+    s = slope(a)
+    r = (dskip.double() + g) * s
+    return r, (dskip.double().abs() + g.abs()) * s
+
+
+def conv_wgrad(x, dz):
+    """-> (dW OIHW, S, db, S_b) from the stored bf16 layer input x [n,h,w,ci] and dz [n,h,w,co]"""
+    x, dz = x.double(), dz.double()
+    return _conv_w(x, dz), _conv_w(x.abs(), dz.abs()), dz.sum((0, 1, 2)), dz.abs().sum((0, 1, 2))
+
+
+def first_conv_wgrad(frame, dz):
+    """conv1_1 weight / bias gradient: the frame rounded to bf16 (the im2col tile), dz1_1 stored bf16"""
+    return conv_wgrad(bf(frame).permute(0, 2, 3, 1), dz)
+
+
+def first_conv_dgrad(dz, w):
+    """d(loss)/d(frame), fp32 NCHW: the stored bf16 dz1_1 and the weights rounded to bf16"""
+    r, S = conv_dgrad(dz, w)
+    return r.permute(0, 3, 1, 2), S.permute(0, 3, 1, 2)
+
+
+def deconv_wgrad(x, dy):
+    """-> (dWt IOHW, S, db, S_b): x stored bf16 [n,h,w,ci] (the deconv input), dy the up plane [n,2h,2w,co]"""
+    x, dy = x.double(), dy.double()
+    return _deconv_w(x, dy), _deconv_w(x.abs(), dy.abs()), dy.sum((0, 1, 2)), dy.abs().sum((0, 1, 2))
+
+
+def head(a, w, b):
+    """conv10_1 (1x1, fp32 weights) on the stored bf16 a9_2 [n,h,w,32] -> (out NCHW, S)"""
+    a, w, b = a.double(), w.double().reshape(w.shape[0], -1), b.double()
+    r = a @ w.t() + b
+    S = a.abs() @ w.abs().t() + b.abs()
+    return r.permute(0, 3, 1, 2), S.permute(0, 3, 1, 2)
+
+
+def head_dout(out, target, kind):
+    """d(loss)/d(out) the kernel forms from ITS out (fp32) and the target: L1 sign(e) / numel, MSE 2 e / numel"""
+    e = out.double() - target.double()
+    inv = 1.0 / out.numel()
+    return torch.sign(e) * inv if kind == 'l1' else 2.0 * e * inv
+
+
+def head_loss(out, target, kind):
+    e = out.double() - target.double()
+    return (e.abs() if kind == 'l1' else e * e).mean()
+
+
+def head_bwd(a, w, dout):
+    """-> (dz9_2 r, S, dW10, S_w, db10, S_b): dout [n,co,h,w] (fp32), a stored bf16 a9_2; a9_2's LeakyReLU' is a > 0"""
+    a, w = a.double(), w.double().reshape(w.shape[0], -1)
+    d = dout.double().permute(0, 2, 3, 1)
+    s = 1.0 - 0.8 * (a <= 0).double()
+    dz, S = (d @ w) * s, (d.abs() @ w.abs()) * s
+    p, q = a.reshape(-1, a.shape[-1]), d.reshape(-1, d.shape[-1])
+    return dz, S, q.t() @ p, q.abs().t() @ p.abs(), q.sum(0), q.abs().sum(0)
+
+
+def first_layer_image(w):
+    """conv1_1's fprop operand as first_conv.cuh consumes it: K-major [32 co][64 k], k = tap * 4 + c (k >= 36 and
+    c >= cin zero), 128-byte rows with the 16-byte chunks of row co XOR-ed by co & 7; bf16 bit patterns"""
+    co_n, cin = w.shape[0], w.shape[1]
+    img = torch.zeros(co_n, 64, dtype=torch.bfloat16, device=w.device)
+    k = torch.arange(36, device=w.device)
+    tap, c = k // 4, k % 4
+    live = c < cin
+    src = torch.zeros(co_n, 36, dtype=torch.float32, device=w.device)
+    src[:, live] = w.reshape(co_n, cin, 9)[:, c[live], tap[live]]
+    for co in range(co_n):
+        col = ((k >> 3) ^ (co & 7)) << 3 | (k & 7)
+        img[co, col] = src[co].bfloat16()
+    return img.reshape(-1)

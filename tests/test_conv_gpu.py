@@ -34,6 +34,11 @@ CONV_CASES = [  # n, h, w, cin, cout, x_c0, x_pitch, y_c0, y_pitch
     (1, 16, 16, 512, 512, 0, 512, 0, 512),
     (1, 8, 16, 512, 256, 0, 512, 0, 256),
     (3, 64, 64, 32, 64, 32, 64, 0, 64),
+    # partial 8 x 16 tiles at the right and bottom borders (h % 8 != 0, w % 16 != 0)
+    (1, 5, 7, 32, 32, 0, 32, 0, 32),
+    (2, 13, 40, 64, 128, 0, 64, 0, 128),
+    (1, 3, 100, 128, 64, 0, 128, 64, 128),
+    (2, 1, 1, 512, 256, 0, 512, 0, 256),
 ]
 
 
@@ -46,8 +51,10 @@ def test_conv3x3_fprop(torch, case, act):
     x = torch.randn(n, h, w, xp, device='cuda', generator=g).bfloat16()
     W = (torch.randn(cout, cin, 3, 3, device='cuda', generator=g) / (3 * cin ** 0.5))
     b = torch.randn(cout, device='cuda', generator=g)
-    y = torch.full((n, h, w, yp), 7.0, device='cuda').bfloat16()
+    y_all = torch.full((n + 1, h, w, yp), 7.0, device='cuda').bfloat16()       # one more image: a sentinel
+    y = y_all[:n]
     prims.conv3x3(x, x_c0, cin, prims.pack_weights(W, prims.PACK_CONV_FPROP), b, y, y_c0, cout, act=act)
+    assert (y_all[n] == 7.0).all()                                                # nothing past the last image
     xin = x[..., x_c0:x_c0 + cin].float().permute(0, 3, 1, 2)
     ref = torch.nn.functional.conv2d(xin, W.bfloat16().float(), b, padding=1)
     if act:
@@ -76,21 +83,30 @@ def test_conv3x3_dgrad_with_mask(torch, case):
     _close(torch, dx.permute(0, 3, 1, 2), ref)
 
 
-@pytest.mark.parametrize('case', [(1, 8, 16, 64, 32), (2, 16, 16, 128, 64), (1, 8, 16, 256, 128), (1, 8, 16, 512, 256)])
+@pytest.mark.parametrize('case', [(1, 8, 16, 64, 32), (2, 16, 16, 128, 64), (1, 8, 16, 256, 128), (1, 8, 16, 512, 256),
+                                  (1, 5, 7, 64, 32), (2, 13, 40, 128, 64), (1, 3, 100, 256, 128)])
 def test_deconv2x2_fprop_and_dgrad(torch, case):
-    from eld_b200 import prims
+    """fprop at any h, w (partial input tiles are masked); the data gradient's gather needs whole 8 x 16 input tiles and
+    refuses other shapes"""
+    from eld_b200 import prims, _lib
     n, h, w, cin, cout = case
     g = torch.Generator(device='cuda').manual_seed(11)
     Wt = torch.randn(cin, cout, 2, 2, device='cuda', generator=g) / cin ** 0.5
     b = torch.randn(cout, device='cuda', generator=g)
     x = torch.randn(n, h, w, cin, device='cuda', generator=g).bfloat16()
-    y = torch.zeros(n, 2 * h, 2 * w, 2 * cout, device='cuda').bfloat16()          # concat buffer: up | skip
+    y_all = torch.zeros(n + 1, 2 * h, 2 * w, 2 * cout, device='cuda').bfloat16()  # concat buffer: up | skip; + a sentinel image
+    y = y_all[:n]
     prims.deconv2x2(x, 0, cin, prims.pack_weights(Wt, prims.PACK_DECONV_FPROP), b, y, 0, cout)
     ref = torch.nn.functional.conv_transpose2d(x.float().permute(0, 3, 1, 2), Wt.bfloat16().float(), b, stride=2)
     _close(torch, y[..., :cout].permute(0, 3, 1, 2), ref)
-    assert (y[..., cout:] == 0).all()
+    assert (y[..., cout:] == 0).all() and (y_all[n] == 0).all()
     dy = torch.randn(n, 2 * h, 2 * w, 2 * cout, device='cuda', generator=g).bfloat16()
     dx = torch.empty(n, h, w, cin, device='cuda').bfloat16()
+    if h % 8 or w % 16:
+        with pytest.raises(_lib.EldError):
+            prims.deconv2x2_dgrad(dy, 0, cout, prims.pack_weights(Wt, prims.PACK_DECONV_DGRAD), dx, 0, cin,
+                                  act=prims.ACT_MASK, aux=x)
+        return
     prims.deconv2x2_dgrad(dy, 0, cout, prims.pack_weights(Wt, prims.PACK_DECONV_DGRAD), dx, 0, cin,
                           act=prims.ACT_MASK, aux=x)
     refdx = torch.nn.functional.conv2d(dy[..., :cout].float().permute(0, 3, 1, 2),
@@ -109,6 +125,7 @@ WGRAD_CASES = [  # n, h, w, cin, cout, x_c0, x_pitch
     (1, 8, 16, 32, 32, 0, 32), (2, 16, 32, 32, 64, 0, 32), (1, 16, 16, 64, 64, 0, 64), (2, 16, 16, 64, 32, 32, 128),
     (1, 8, 32, 128, 128, 0, 128), (1, 8, 16, 256, 256, 0, 256), (1, 8, 16, 512, 512, 0, 512), (2, 8, 16, 512, 256, 0, 512),
     (3, 32, 32, 128, 64, 0, 128), (1, 64, 64, 32, 32, 0, 32),
+    (1, 6, 16, 32, 32, 0, 32), (1, 8, 24, 64, 64, 0, 64),       # not whole 4 x 16 reduction chunks: refused
 ]
 
 
@@ -121,6 +138,15 @@ def test_conv3x3_wgrad(torch, case):
     x = torch.randn(n, h, w, xp, device='cuda', generator=g).bfloat16()
     dz = torch.randn(n, h, w, cout, device='cuda', generator=g).bfloat16()
     dw = torch.zeros(cout, cin, 3, 3, device='cuda')
+    if h % 4 or w % 16:
+        from eld_b200 import _lib
+        with pytest.raises(_lib.EldError):
+            prims.conv3x3_wgrad(x, x_c0, cin, dz, 0, cout, dw)
+        with pytest.raises(_lib.EldError):
+            prims.deconv2x2_wgrad(x, x_c0, cin, torch.zeros(n, 2 * h, 2 * w, cout, device='cuda').bfloat16(), 0, cout,
+                                  torch.zeros(cin, cout, 2, 2, device='cuda'))
+        assert (dw == 0).all()
+        return
     prims.conv3x3_wgrad(x, x_c0, cin, dz, 0, cout, dw)
     xin = x[..., x_c0:x_c0 + cin].float().permute(0, 3, 1, 2).contiguous()
     ref = torch.nn.grad.conv2d_weight(xin, (cout, cin, 3, 3), dz.float().permute(0, 3, 1, 2).contiguous(), padding=1)
