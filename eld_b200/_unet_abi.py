@@ -38,6 +38,10 @@ def declare_engine(lib):
     lib.eld_unet_wait_bucket.argtypes = [vp, i32, vp]
     lib.eld_unet_backward.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.eld_unet_input_grad.argtypes = [vp, vp, vp, vp]
+    lib.eld_unet_state_bytes.argtypes = [i32, i32, i32, i32, i32]
+    lib.eld_unet_state_bytes.restype = sz
+    lib.eld_unet_forward_state.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.eld_unet_backward_state.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.eld_unet_set_trainable.argtypes = [vp, c.POINTER(c.c_uint8), i32, i32]
     lib.eld_adam_step_segments.argtypes = [vp, vp, vp, vp, vp, c.POINTER(sz), c.POINTER(i32), i32, f32, f32, f32, f32, f32,
                                            f32, vp]

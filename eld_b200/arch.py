@@ -8,6 +8,7 @@ runs the wgmma engine behind the C ABI (csrc/unet_engine.cu) on NHWC bf16 activa
 """
 import ctypes
 import warnings
+import weakref
 
 import torch
 import torch.nn as nn
@@ -26,41 +27,106 @@ def _st():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+class _Claim:
+    """What a call that holds an engine's built-in forward state keeps (the engine refers to it weakly, so a call whose
+    graph is dropped without a backward gives the state up)."""
+    __slots__ = ('done', '__weakref__')
+
+    def __init__(self):
+        self.done = False                  # the call has run its backward
+
+
+class _Engine(tuple):
+    """(handle, workspace) of one launch plan, kept by the module's cache and by every autograd call that may still
+    run its backward; the handle is destroyed when the last of them drops it, so neither the cache's eviction nor
+    _flatten() frees a plan a pending backward needs.  A training plan's workspace holds one forward state (the built-in
+    one); `owner` refers to the call it belongs to."""
+
+    def __new__(cls, handle, ws, masks):
+        self = super().__new__(cls, (handle, ws))
+        self.masks, self.owner = masks, None
+        return self
+
+    def claim(self):
+        """A _Claim on the built-in state for a new call, or None while it belongs to a call that has not back-propagated"""
+        cur = self.owner() if self.owner is not None else None
+        if cur is not None and not cur.done:
+            return None
+        c = _Claim()
+        self.owner = weakref.ref(c)
+        return c
+
+    def holds(self, c):
+        """the built-in state still holds the forward of the call with claim `c`"""
+        return c is not None and self.owner is not None and self.owner() is c
+
+    def __del__(self):
+        self.masks.pop(self[0].value, None)
+        try:
+            _lib.load().eld_unet_destroy(self[0])
+        except Exception:
+            pass
+
+
 class _EngineFunction(torch.autograd.Function):
-    """The netG seam as an autograd node (SURVEY 8b): forward = the training engine's forward (activations stay in its
-    workspace), backward = eld_unet_backward on the incoming d(loss)/d(out) - so the reference's own
-    `loss.backward(); optimizer.step()` (ELD_model.py:411-420,469-475) runs against this module unchanged, with any loss.
+    """The netG seam as an autograd node (SURVEY 8b): forward = the training engine's forward, backward =
+    eld_unet_backward on the incoming d(loss)/d(out) - so the reference's own `loss.backward(); optimizer.step()`
+    (ELD_model.py:411-420,469-475) runs against this module unchanged, with any loss.
     When the frame requires grad (a learnable stage upstream, test-time optimisation of the input), eld_unet_input_grad
     follows and gives d(loss)/d(x) as well.
-    Parameters enter as inputs only so that autograd routes their gradients; the math reads the flat buffer."""
+    Every call keeps its forward state until its backward: the engine's built-in state when no other call still needs it
+    (the one-call-per-backward loop: no allocation, no extra launch), otherwise a state of its own
+    (eld_unet_forward_state), released when its backward ends.  A call whose state is gone by the time of a backward
+    (the built-in state went to a newer call or a train_step after a retain_graph backward, or its own state was released
+    by an earlier backward) runs its forward again from the saved x into a fresh state: the forward tiles have no
+    atomics, so that state is bit-identical.
+    Parameters enter as inputs so that autograd routes their gradients, and are saved so that changing them in place
+    before the backward is torch's usual error; the math reads the flat buffer."""
 
     @staticmethod
     def forward(ctx, net, x, *params):
         n, _, h, w = x.shape
-        eng = net._engine(n, h, w, True)
+        eng = net._plan(n, h, w, True)
         out = torch.empty((n, net.out_channels, h, w), dtype=torch.float32, device=x.device)
-        _lib.check(_lib.load().eld_unet_forward(eng, net._flat.data_ptr(), x.data_ptr(), out.data_ptr(), _st()), 'eld_unet_forward')
         ctx.net, ctx.eng = net, eng
-        ctx.save_for_backward(x)
+        ctx.claim = eng.claim()
+        # not through save_for_backward: torch.utils.checkpoint pairs the tensors a recomputed forward saves with the
+        # original's, and whether a call gets the built-in state can differ between the two
+        ctx.state = None if ctx.claim is not None else net._new_state(x)
+        _lib.check(_lib.load().eld_unet_forward_state(eng[0], _ptr(ctx.state), net._flat.data_ptr(), x.data_ptr(),
+                                                      out.data_ptr(), _st()), 'eld_unet_forward_state')
+        ctx.save_for_backward(x, *params)
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        net = ctx.net
-        (x,) = ctx.saved_tensors
-        need = ctx.needs_input_grad[2:]              # frozen parameters: no weight-gradient launch, None returned
-        net._set_trainable(ctx.eng, need, ctx.needs_input_grad[1])
+        net, eng, lib = ctx.net, ctx.eng, _lib.load()
+        x = ctx.saved_tensors[0]                 # raises if x or a parameter was changed in place since the forward
+        need = ctx.needs_input_grad[2:]          # frozen parameters: no weight-gradient launch, None returned
+        net._set_trainable(eng[0], need, ctx.needs_input_grad[1])
+        state = ctx.state
+        if state is None and not eng.holds(ctx.claim):
+            state = net._new_state(x)
+            scratch = torch.empty((x.shape[0], net.out_channels) + tuple(x.shape[2:]), dtype=torch.float32, device=x.device)
+            _lib.check(lib.eld_unet_forward_state(eng[0], state.data_ptr(), net._flat.data_ptr(), x.data_ptr(),
+                                                  scratch.data_ptr(), _st()), 'eld_unet_forward_state')
         g = torch.empty_like(net._flat)
-        _lib.check(_lib.load().eld_unet_backward(ctx.eng, net._flat.data_ptr(), x.data_ptr(), dout.contiguous().data_ptr(),
-                                                g.data_ptr(), _st()), 'eld_unet_backward')
+        _lib.check(lib.eld_unet_backward_state(eng[0], _ptr(state), net._flat.data_ptr(), x.data_ptr(),
+                                               dout.contiguous().data_ptr(), g.data_ptr(), _st()), 'eld_unet_backward_state')
         dx = None
         if ctx.needs_input_grad[1]:              # conv1_1's data gradient, one launch; skipped when nothing upstream wants it
             dx = torch.empty_like(x)
-            _lib.check(_lib.load().eld_unet_input_grad(ctx.eng, net._flat.data_ptr(), dx.data_ptr(), _st()),
-                       'eld_unet_input_grad')
+            _lib.check(lib.eld_unet_input_grad(eng[0], net._flat.data_ptr(), dx.data_ptr(), _st()), 'eld_unet_input_grad')
+        if ctx.claim is not None:
+            ctx.claim.done = True
+        ctx.state = None
         grads = tuple(g[off:off + k].view(p.shape) if want else None
                       for p, (off, k), want in zip(net.parameters(), net._spans, need))
         return (None, dx) + grads
+
+
+def _ptr(t):
+    return None if t is None else t.data_ptr()
 
 
 class UNetSeeInDark(nn.Module):
@@ -133,18 +199,13 @@ class UNetSeeInDark(nn.Module):
             elif p.grad is None or p.grad.data_ptr() != view.data_ptr():
                 p.grad = view
 
-    _MAX_ENGINES = 4      # (n, h, w, train) launch plans kept alive, least recently used evicted (each owns a workspace)
+    _MAX_ENGINES = 4      # (n, h, w, train) launch plans cached, least recently used evicted (each owns a workspace)
 
     def _drop_engines(self, keep=0):
+        """evict from the cache; a plan is destroyed when no pending backward holds it either (_Engine)"""
         eng = getattr(self, '_engines', None) or {}
         while len(eng) > keep:
-            key = next(iter(eng))
-            handle, _ws = eng.pop(key)
-            self._masks.pop(handle.value, None)
-            try:
-                _lib.load().eld_unet_destroy(handle)
-            except Exception:
-                pass
+            eng.pop(next(iter(eng)))
         self._engines = eng
         self._ddp_ready = None
 
@@ -173,6 +234,16 @@ class UNetSeeInDark(nn.Module):
 
     # ---- engine ------------------------------------------------------------------------------------
     def _engine(self, n, h, w, train):
+        """the eld_unet handle of the (n, h, w, train) launch plan"""
+        return self._plan(n, h, w, train)[0]
+
+    def _new_state(self, x):
+        """device memory for one forward state of frame batch x (eld_unet_forward_state)"""
+        n, _, h, w = x.shape
+        nbytes = _lib.load().eld_unet_state_bytes(n, h, w, self.in_channels, self.out_channels)
+        return torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+
+    def _plan(self, n, h, w, train):
         key = (n, h, w, bool(train))
         if key in self._engines:
             self._engines[key] = self._engines.pop(key)          # most recently used last
@@ -187,9 +258,9 @@ class UNetSeeInDark(nn.Module):
             handle = ctypes.c_void_p()
             _lib.check(lib.eld_unet_create_io(_lib.ctx(dev.index or 0), n, h, w, int(train), ws.data_ptr(), nbytes,
                                               self.in_channels, self.out_channels, ctypes.byref(handle)), 'eld_unet_create_io')
-            self._engines[key] = (handle, ws)
+            self._engines[key] = _Engine(handle, ws, self._masks)
             self._masks[handle.value] = ((True,) * len(self._spans), True)      # a new engine computes every gradient
-        return self._engines[key][0]
+        return self._engines[key]
 
     def forward(self, x):
         """x: cuda float32 NCHW [n,4,h,w] -> float32 NCHW [n,4,h,w].  Under torch.enable_grad(), in training mode or when
@@ -225,10 +296,12 @@ class UNetSeeInDark(nn.Module):
         out = torch.empty_like(target)
         loss = loss_out if loss_out is not None else torch.empty((), dtype=torch.float32, device=x.device)
         flags = self._last_flags = [p.requires_grad for p in self.parameters()]
-        self._set_trainable(self._engine(n, h, w, True), flags, False)
+        plan = self._plan(n, h, w, True)
+        plan.owner = None              # the step overwrites the built-in forward state: a call still needing it recomputes
+        self._set_trainable(plan[0], flags, False)
         self._sync_grads(flags)
-        _lib.check(_lib.load().eld_unet_set_loss(self._engine(n, h, w, True), 1 if self.loss_kind == 'l2' else 0), 'eld_unet_set_loss')
-        _lib.check(_lib.load().eld_unet_train_step(self._engine(n, h, w, True), self._flat.data_ptr(), x.data_ptr(),
+        _lib.check(_lib.load().eld_unet_set_loss(plan[0], 1 if self.loss_kind == 'l2' else 0), 'eld_unet_set_loss')
+        _lib.check(_lib.load().eld_unet_train_step(plan[0], self._flat.data_ptr(), x.data_ptr(),
                                                    target.data_ptr(), out.data_ptr(), self._flat_grad.data_ptr(),
                                                    loss.data_ptr(), _st()), 'eld_unet_train_step')
         return out, loss
@@ -360,9 +433,13 @@ class FusedAdam(torch.optim.Optimizer):
             self.m = torch.zeros_like(self.net.flat_params)
             self.v = torch.zeros_like(self.net.flat_params)
         self.t += 1
-        flags = [q.requires_grad for q in self.net.parameters()]
+        params = list(self.net.parameters())
+        flags = [q.requires_grad for q in params]
         for i, f in enumerate(flags):
             self.steps[i] += 1 if f else 0
+        # the kernels write the flat buffer behind autograd's back: mark the parameters modified in place, so that a
+        # retained graph that saved them raises torch's usual error instead of back-propagating through new weights
+        torch.autograd.graph.increment_version([q for q, f in zip(params, flags) if f])
         uniform = all(flags) and len(set(self.steps)) == 1
         p = self.net.flat_params
         hp = (float(g['lr']), float(g['betas'][0]), float(g['betas'][1]), float(g['eps']), float(g['weight_decay']))

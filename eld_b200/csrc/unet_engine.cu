@@ -222,6 +222,21 @@ wgrad_permute_kernel(const float* __restrict__ gtmp, float* __restrict__ grads, 
 
 using namespace eld;
 
+// Everything a forward leaves for the backward of the same call: activations and concat buffers, pool codes, sign words
+// and the packed weights.  layout() places one inside the workspace (the built-in state, eld_unet_forward) or in memory
+// the caller owns (eld_unet_forward_state).  The backward writes none of it, so a state stays valid after a backward
+// that read it.
+struct FwdState {
+    __nv_bfloat16 *a1_1, *cat9, *p1, *a2_1, *cat8, *p2, *a3_1, *cat7, *p3, *a4_1, *cat6, *p4, *a5_1, *a5_2,
+        *a6_1, *a6_2, *a7_1, *a7_2, *a8_1, *a8_2, *a9_1, *a9_2;
+    __nv_bfloat16 *pc1 = nullptr, *pc2 = nullptr, *pc3 = nullptr, *pc4 = nullptr;   // pool codes, 1 byte per pooled element (training)
+    // sign words (1 bit per element) of the activations whose LeakyReLU' a data gradient applies (training): the dgrad
+    // tiles read these instead of the activation itself
+    struct SignBuf { const void* act; uint32_t* words; } signs[16];
+    int n_signs = 0;
+    __nv_bfloat16* packed;
+};
+
 struct eld_unet {
     eld_ctx* ctx;
     int n, H, W;
@@ -229,17 +244,10 @@ struct eld_unet {
     size_t n_params;
     char* ws;
     size_t ws_bytes;
-    // activations / gradients (bf16), offsets in bytes into ws
-    __nv_bfloat16 *a1_1, *cat9, *p1, *a2_1, *cat8, *p2, *a3_1, *cat7, *p3, *a4_1, *cat6, *p4, *a5_1, *a5_2,
-        *a6_1, *a6_2, *a7_1, *a7_2, *a8_1, *a8_2, *a9_1, *a9_2;
+    FwdState fs;                 // the built-in forward state, in ws
+    // backward scratch (bf16), in ws
     __nv_bfloat16 *dz9_2, *dz9_1, *dcat9, *dz8_2, *dz8_1, *dcat8, *dz7_2, *dz7_1, *dcat7, *dz6_2, *dz6_1, *dcat6,
         *dz5_2, *dz5_1, *dp4, *dz4_2, *dz4_1, *dp3, *dz3_2, *dz3_1, *dp2, *dz2_2, *dz2_1, *dp1, *dz1_2, *dz1_1;
-    __nv_bfloat16 *pc1 = nullptr, *pc2 = nullptr, *pc3 = nullptr, *pc4 = nullptr;   // pool codes, 1 byte per pooled element (training)
-    // sign words (1 bit per element) of the activations whose LeakyReLU' a data gradient applies (training): the dgrad
-    // tiles read these instead of the activation itself
-    struct SignBuf { const void* act; uint32_t* words; } signs[16];
-    int n_signs = 0;
-    __nv_bfloat16* packed;
     float* gtmp = nullptr;
     PackTable table;
     // gradient buckets in backward-completion order (data-parallel overlap, SURVEY 8e): decoder, bottleneck, encoder
@@ -261,7 +269,10 @@ struct eld_unet {
     size_t rec_used = 0;
 };
 
-static size_t layout(eld_unet* u, char* base, bool train)
+// Places forward state `s` at `base` and, with `scratch`, the backward scratch of `u` (dz*, dcat*, dp*, gtmp) among it in
+// the workspace's order; returns the bytes used.  Without `scratch` the state's buffers are packed back to back
+// (eld_unet_state_bytes).  train = false: activations and packed weights only.
+static size_t layout(eld_unet* u, FwdState* s, char* base, bool train, bool scratch)
 {
     size_t off = 0;
     const size_t n = u->n;
@@ -271,14 +282,14 @@ static size_t layout(eld_unet* u, char* base, bool train)
         if (p) *p = reinterpret_cast<__nv_bfloat16*>(base + off);
         off += bytes;
     };
-    take(&u->a1_1, 0, 32); take(&u->cat9, 0, 64); take(&u->p1, 1, 32);
-    take(&u->a2_1, 1, 64); take(&u->cat8, 1, 128); take(&u->p2, 2, 64);
-    take(&u->a3_1, 2, 128); take(&u->cat7, 2, 256); take(&u->p3, 3, 128);
-    take(&u->a4_1, 3, 256); take(&u->cat6, 3, 512); take(&u->p4, 4, 256);
-    take(&u->a5_1, 4, 512); take(&u->a5_2, 4, 512);
-    take(&u->a6_1, 3, 256); take(&u->a6_2, 3, 256); take(&u->a7_1, 2, 128); take(&u->a7_2, 2, 128);
-    take(&u->a8_1, 1, 64); take(&u->a8_2, 1, 64); take(&u->a9_1, 0, 32); take(&u->a9_2, 0, 32);
-    if (train) {
+    take(&s->a1_1, 0, 32); take(&s->cat9, 0, 64); take(&s->p1, 1, 32);
+    take(&s->a2_1, 1, 64); take(&s->cat8, 1, 128); take(&s->p2, 2, 64);
+    take(&s->a3_1, 2, 128); take(&s->cat7, 2, 256); take(&s->p3, 3, 128);
+    take(&s->a4_1, 3, 256); take(&s->cat6, 3, 512); take(&s->p4, 4, 256);
+    take(&s->a5_1, 4, 512); take(&s->a5_2, 4, 512);
+    take(&s->a6_1, 3, 256); take(&s->a6_2, 3, 256); take(&s->a7_1, 2, 128); take(&s->a7_2, 2, 128);
+    take(&s->a8_1, 1, 64); take(&s->a8_2, 1, 64); take(&s->a9_1, 0, 32); take(&s->a9_2, 0, 32);
+    if (train && scratch) {
         take(&u->dz9_2, 0, 32); take(&u->dz9_1, 0, 32); take(&u->dcat9, 0, 64);
         take(&u->dz8_2, 1, 64); take(&u->dz8_1, 1, 64); take(&u->dcat8, 1, 128);
         take(&u->dz7_2, 2, 128); take(&u->dz7_1, 2, 128); take(&u->dcat7, 2, 256);
@@ -288,17 +299,19 @@ static size_t layout(eld_unet* u, char* base, bool train)
         take(&u->dz3_2, 2, 128); take(&u->dz3_1, 2, 128); take(&u->dp2, 2, 64);
         take(&u->dz2_2, 1, 64); take(&u->dz2_1, 1, 64); take(&u->dp1, 1, 32);
         take(&u->dz1_2, 0, 32); take(&u->dz1_1, 0, 32);
-        take(&u->pc1, 1, 16); take(&u->pc2, 2, 32); take(&u->pc3, 3, 64); take(&u->pc4, 4, 128);
-        u->n_signs = 0;
+    }
+    if (train) {
+        take(&s->pc1, 1, 16); take(&s->pc2, 2, 32); take(&s->pc3, 3, 64); take(&s->pc4, 4, 128);
+        s->n_signs = 0;
         auto take_signs = [&](__nv_bfloat16* act, int lvl, int ch) {      // ch / 32 words per pixel = ch / 16 bf16-sized units
             __nv_bfloat16* w = nullptr;
             take(&w, lvl, ch / 16);
-            u->signs[u->n_signs++] = { act, reinterpret_cast<uint32_t*>(w) };
+            s->signs[s->n_signs++] = { act, reinterpret_cast<uint32_t*>(w) };
         };
-        take_signs(u->a1_1, 0, 32); take_signs(u->a2_1, 1, 64); take_signs(u->a3_1, 2, 128); take_signs(u->a4_1, 3, 256);
-        take_signs(u->a5_1, 4, 512); take_signs(u->a5_2, 4, 512); take_signs(u->a6_1, 3, 256); take_signs(u->a6_2, 3, 256);
-        take_signs(u->a7_1, 2, 128); take_signs(u->a7_2, 2, 128); take_signs(u->a8_1, 1, 64); take_signs(u->a8_2, 1, 64);
-        take_signs(u->a9_1, 0, 32);
+        take_signs(s->a1_1, 0, 32); take_signs(s->a2_1, 1, 64); take_signs(s->a3_1, 2, 128); take_signs(s->a4_1, 3, 256);
+        take_signs(s->a5_1, 4, 512); take_signs(s->a5_2, 4, 512); take_signs(s->a6_1, 3, 256); take_signs(s->a6_2, 3, 256);
+        take_signs(s->a7_1, 2, 128); take_signs(s->a7_2, 2, 128); take_signs(s->a8_1, 1, 64); take_signs(s->a8_2, 1, 64);
+        take_signs(s->a9_1, 0, 32);
     }
     // packed weights
     size_t pk = 0;
@@ -310,9 +323,9 @@ static size_t layout(eld_unet* u, char* base, bool train)
         l.wf_off = pk; pk += cnt;
         l.wd_off = pk; pk += cnt;
     }
-    u->packed = reinterpret_cast<__nv_bfloat16*>(base + off);
+    s->packed = reinterpret_cast<__nv_bfloat16*>(base + off);
     off += (pk * 2 + 1023) & ~(size_t)1023;
-    if (train) {   // [tap][ci][co] staging of the conv3x3 weight gradients (same offsets as the fp32 parameters)
+    if (train && scratch) {   // [tap][ci][co] staging of the conv3x3 weight gradients (same offsets as the fp32 parameters)
         u->gtmp = reinterpret_cast<float*>(base + off);
         off += (u->n_params * 4 + 1023) & ~(size_t)1023;
     }
@@ -376,7 +389,16 @@ extern "C" size_t eld_unet_workspace_bytes(int n, int h, int w, int train)
     eld_unet tmp{};
     tmp.n = n; tmp.H = h; tmp.W = w;
     init_layers(&tmp);
-    return layout(&tmp, nullptr, train != 0) + 1024;
+    return layout(&tmp, &tmp.fs, nullptr, train != 0, true) + 1024;
+}
+
+extern "C" size_t eld_unet_state_bytes(int n, int h, int w, int cin, int cout)
+{
+    if (!io_ok(cin, cout) || n <= 0 || h <= 0 || w <= 0) return 0;
+    eld_unet tmp{};
+    tmp.n = n; tmp.H = h; tmp.W = w; tmp.cin0 = cin; tmp.cout_last = cout;
+    init_layers(&tmp);
+    return layout(&tmp, &tmp.fs, nullptr, true, false) + 1024;      // + room to align the caller's pointer to 1 KB
 }
 
 // The per-launch plan of the backward from the trainable flags (one per parameter tensor, state_dict order), by one
@@ -423,7 +445,7 @@ extern "C" int eld_unet_create_io(eld_ctx* ctx, int n, int h, int w, int train, 
     u->ctx = ctx; u->n = n; u->H = h; u->W = w; u->cin0 = cin; u->cout_last = cout;
     init_layers(u);
     char* base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~(uintptr_t)1023);
-    const size_t need = layout(u, base, train != 0) + (base - static_cast<char*>(workspace));
+    const size_t need = layout(u, &u->fs, base, train != 0, true) + (base - static_cast<char*>(workspace));
     if (need > bytes) {
         set_error("eld_unet_create: workspace %zu bytes < required %zu", bytes, need);
         delete u;
@@ -450,7 +472,7 @@ extern "C" int eld_unet_create_io(eld_ctx* ctx, int n, int h, int w, int train, 
         derive_needs(u, all, true);
     }
     // conv1_1's operand image: zero once (pack_all rewrites all of it every step anyway)
-    ELD_CHECK_CUDA(cudaMemset(u->packed + u->L[I_C11].wf_off, 0, 32 * 9 * 32 * sizeof(__nv_bfloat16)));
+    ELD_CHECK_CUDA(cudaMemset(u->fs.packed + u->L[I_C11].wf_off, 0, 32 * 9 * 32 * sizeof(__nv_bfloat16)));
     // opt in to large dynamic shared memory once (not inside a captured region)
     { int rc = init_gemm_kernels(ctx); if (rc != ELD_OK) { delete u; return rc; } }
     *out = u;
@@ -527,17 +549,18 @@ struct Scope {
 
 struct Runner {
     eld_unet* u;
+    const FwdState* s;           // the forward state this call writes (forward) or reads (backward)
     const float* params;
     cudaStream_t st;
     eld_ctx* ctx() const { return u->ctx; }
-    const __nv_bfloat16* wf(int i) const { return u->packed + u->L[i].wf_off; }
-    const __nv_bfloat16* wd(int i) const { return u->packed + u->L[i].wd_off; }
+    const __nv_bfloat16* wf(int i) const { return s->packed + u->L[i].wf_off; }
+    const __nv_bfloat16* wd(int i) const { return s->packed + u->L[i].wd_off; }
     const float* bias(int i) const { return params + u->L[i].b_off; }
 
     // sign words of activation `act`, or nullptr: an inference engine keeps none, and a9_2's LeakyReLU' is the head's
     uint32_t* sign_of(const void* act) const
     {
-        for (int i = 0; i < u->n_signs; ++i) if (u->signs[i].act == act) return u->signs[i].words;
+        for (int i = 0; i < s->n_signs; ++i) if (s->signs[i].act == act) return s->signs[i].words;
         return nullptr;
     }
     // pool_dst != nullptr: MaxPool2d(2) of the output fused into the tile's epilogue (pooled tensor has cout channels)
@@ -683,7 +706,7 @@ struct Runner {
     int pack() const
     {
         Scope sc(u, st, "weights", "pack", 0.0, (double)u->n_params * 8);
-        pack_all_kernel<<<u->table.tile0[u->table.n] + 2, 256, 0, st>>>(params, u->packed, u->table);
+        pack_all_kernel<<<u->table.tile0[u->table.n] + 2, 256, 0, st>>>(params, s->packed, u->table);
         ELD_CHECK_CUDA(cudaGetLastError());
         count_launch(ctx());
         return ELD_OK;
@@ -692,30 +715,31 @@ struct Runner {
     int forward(const float* x) const
     {
         eld_unet* U = u;
+        const FwdState* S = s;
         TRY(pack());
         {
             // conv1_1 (4 -> 32): software-im2col tile straight from the fp32 NCHW frame (first_conv.cuh)
             const double px = (double)U->n * U->H * U->W;
             Scope sc(u, st, "conv1_1", "fprop", 2.0 * px * 32 * 9 * U->cin0, px * (4 * U->cin0 + 64));
-            TRY(launch_first_conv(ctx(), x, U->cin0, wf(I_C11), bias(I_C11), U->a1_1, 32, U->n, U->H, U->W, st, sign_of(U->a1_1)));
+            TRY(launch_first_conv(ctx(), x, U->cin0, wf(I_C11), bias(I_C11), S->a1_1, 32, U->n, U->H, U->W, st, sign_of(S->a1_1)));
         }
-        TRY(conv(I_C12, U->a1_1, 32, 0, U->cat9, 64, 32, 0, U->p1, U->pc1));       // + pool (Unet.py:51)
-        TRY(conv(I_C21, U->p1, 32, 0, U->a2_1, 64, 0, 1));
-        TRY(conv(I_C22, U->a2_1, 64, 0, U->cat8, 128, 64, 1, U->p2, U->pc2));      // + pool (Unet.py:55)
-        TRY(conv(I_C31, U->p2, 64, 0, U->a3_1, 128, 0, 2));
-        TRY(conv(I_C32, U->a3_1, 128, 0, U->cat7, 256, 128, 2, U->p3, U->pc3));    // + pool (Unet.py:59)
-        TRY(conv(I_C41, U->p3, 128, 0, U->a4_1, 256, 0, 3));
-        TRY(conv(I_C42, U->a4_1, 256, 0, U->cat6, 512, 256, 3, U->p4, U->pc4));    // + pool (Unet.py:63)
-        TRY(conv(I_C51, U->p4, 256, 0, U->a5_1, 512, 0, 4));
-        TRY(conv(I_C52, U->a5_1, 512, 0, U->a5_2, 512, 0, 4));
-        TRY(deconv(I_UP6, U->a5_2, 512, U->cat6, 512, 4));
-        TRY(conv(I_C61, U->cat6, 512, 0, U->a6_1, 256, 0, 3)); TRY(conv(I_C62, U->a6_1, 256, 0, U->a6_2, 256, 0, 3));
-        TRY(deconv(I_UP7, U->a6_2, 256, U->cat7, 256, 3));
-        TRY(conv(I_C71, U->cat7, 256, 0, U->a7_1, 128, 0, 2)); TRY(conv(I_C72, U->a7_1, 128, 0, U->a7_2, 128, 0, 2));
-        TRY(deconv(I_UP8, U->a7_2, 128, U->cat8, 128, 2));
-        TRY(conv(I_C81, U->cat8, 128, 0, U->a8_1, 64, 0, 1));  TRY(conv(I_C82, U->a8_1, 64, 0, U->a8_2, 64, 0, 1));
-        TRY(deconv(I_UP9, U->a8_2, 64, U->cat9, 64, 1));
-        TRY(conv(I_C91, U->cat9, 64, 0, U->a9_1, 32, 0, 0));   TRY(conv(I_C92, U->a9_1, 32, 0, U->a9_2, 32, 0, 0));
+        TRY(conv(I_C12, S->a1_1, 32, 0, S->cat9, 64, 32, 0, S->p1, S->pc1));       // + pool (Unet.py:51)
+        TRY(conv(I_C21, S->p1, 32, 0, S->a2_1, 64, 0, 1));
+        TRY(conv(I_C22, S->a2_1, 64, 0, S->cat8, 128, 64, 1, S->p2, S->pc2));      // + pool (Unet.py:55)
+        TRY(conv(I_C31, S->p2, 64, 0, S->a3_1, 128, 0, 2));
+        TRY(conv(I_C32, S->a3_1, 128, 0, S->cat7, 256, 128, 2, S->p3, S->pc3));    // + pool (Unet.py:59)
+        TRY(conv(I_C41, S->p3, 128, 0, S->a4_1, 256, 0, 3));
+        TRY(conv(I_C42, S->a4_1, 256, 0, S->cat6, 512, 256, 3, S->p4, S->pc4));    // + pool (Unet.py:63)
+        TRY(conv(I_C51, S->p4, 256, 0, S->a5_1, 512, 0, 4));
+        TRY(conv(I_C52, S->a5_1, 512, 0, S->a5_2, 512, 0, 4));
+        TRY(deconv(I_UP6, S->a5_2, 512, S->cat6, 512, 4));
+        TRY(conv(I_C61, S->cat6, 512, 0, S->a6_1, 256, 0, 3)); TRY(conv(I_C62, S->a6_1, 256, 0, S->a6_2, 256, 0, 3));
+        TRY(deconv(I_UP7, S->a6_2, 256, S->cat7, 256, 3));
+        TRY(conv(I_C71, S->cat7, 256, 0, S->a7_1, 128, 0, 2)); TRY(conv(I_C72, S->a7_1, 128, 0, S->a7_2, 128, 0, 2));
+        TRY(deconv(I_UP8, S->a7_2, 128, S->cat8, 128, 2));
+        TRY(conv(I_C81, S->cat8, 128, 0, S->a8_1, 64, 0, 1));  TRY(conv(I_C82, S->a8_1, 64, 0, S->a8_2, 64, 0, 1));
+        TRY(deconv(I_UP9, S->a8_2, 64, S->cat9, 64, 1));
+        TRY(conv(I_C91, S->cat9, 64, 0, S->a9_1, 32, 0, 0));   TRY(conv(I_C92, S->a9_1, 32, 0, S->a9_2, 32, 0, 0));
         return ELD_OK;
     }
 
@@ -725,58 +749,59 @@ struct Runner {
     int backward(const float* x, float* g) const
     {
         eld_unet* U = u;
+        const FwdState* S = s;
         auto W = [U](int l) { return U->wgrad[l]; };
-        auto D = [U](int s) { return U->reach[s]; };
-        if (W(I_C92)) TRY(conv_wgrad(I_C92, U->a9_1, 32, 0, U->dz9_2, g, 0));
-        if (D(I_C91)) TRY(conv_dgrad(I_C92, U->dz9_2, U->dz9_1, 32, 0, U->a9_1, 0));
-        if (W(I_C91)) TRY(conv_wgrad(I_C91, U->cat9, 64, 0, U->dz9_1, g, 0));
+        auto D = [U](int src) { return U->reach[src]; };
+        if (W(I_C92)) TRY(conv_wgrad(I_C92, S->a9_1, 32, 0, U->dz9_2, g, 0));
+        if (D(I_C91)) TRY(conv_dgrad(I_C92, U->dz9_2, U->dz9_1, 32, 0, S->a9_1, 0));
+        if (W(I_C91)) TRY(conv_wgrad(I_C91, S->cat9, 64, 0, U->dz9_1, g, 0));
         if (D(I_UP9)) TRY(concat_dgrad(I_C91, U->dz9_1, U->dcat9, 0));
-        if (W(I_UP9)) TRY(deconv_wgrad(I_UP9, U->a8_2, U->dcat9, 32, g, 1));
-        if (D(I_C82)) TRY(deconv_dgrad(I_UP9, U->dcat9, 32, U->dz8_2, U->a8_2, 1));
-        if (W(I_C82)) TRY(conv_wgrad(I_C82, U->a8_1, 64, 0, U->dz8_2, g, 1));
-        if (D(I_C81)) TRY(conv_dgrad(I_C82, U->dz8_2, U->dz8_1, 64, 0, U->a8_1, 1));
-        if (W(I_C81)) TRY(conv_wgrad(I_C81, U->cat8, 128, 0, U->dz8_1, g, 1));
+        if (W(I_UP9)) TRY(deconv_wgrad(I_UP9, S->a8_2, U->dcat9, 32, g, 1));
+        if (D(I_C82)) TRY(deconv_dgrad(I_UP9, U->dcat9, 32, U->dz8_2, S->a8_2, 1));
+        if (W(I_C82)) TRY(conv_wgrad(I_C82, S->a8_1, 64, 0, U->dz8_2, g, 1));
+        if (D(I_C81)) TRY(conv_dgrad(I_C82, U->dz8_2, U->dz8_1, 64, 0, S->a8_1, 1));
+        if (W(I_C81)) TRY(conv_wgrad(I_C81, S->cat8, 128, 0, U->dz8_1, g, 1));
         if (D(I_UP8)) TRY(concat_dgrad(I_C81, U->dz8_1, U->dcat8, 1));
-        if (W(I_UP8)) TRY(deconv_wgrad(I_UP8, U->a7_2, U->dcat8, 64, g, 2));
-        if (D(I_C72)) TRY(deconv_dgrad(I_UP8, U->dcat8, 64, U->dz7_2, U->a7_2, 2));
-        if (W(I_C72)) TRY(conv_wgrad(I_C72, U->a7_1, 128, 0, U->dz7_2, g, 2));
-        if (D(I_C71)) TRY(conv_dgrad(I_C72, U->dz7_2, U->dz7_1, 128, 0, U->a7_1, 2));
-        if (W(I_C71)) TRY(conv_wgrad(I_C71, U->cat7, 256, 0, U->dz7_1, g, 2));
+        if (W(I_UP8)) TRY(deconv_wgrad(I_UP8, S->a7_2, U->dcat8, 64, g, 2));
+        if (D(I_C72)) TRY(deconv_dgrad(I_UP8, U->dcat8, 64, U->dz7_2, S->a7_2, 2));
+        if (W(I_C72)) TRY(conv_wgrad(I_C72, S->a7_1, 128, 0, U->dz7_2, g, 2));
+        if (D(I_C71)) TRY(conv_dgrad(I_C72, U->dz7_2, U->dz7_1, 128, 0, S->a7_1, 2));
+        if (W(I_C71)) TRY(conv_wgrad(I_C71, S->cat7, 256, 0, U->dz7_1, g, 2));
         if (D(I_UP7)) TRY(concat_dgrad(I_C71, U->dz7_1, U->dcat7, 2));
-        if (W(I_UP7)) TRY(deconv_wgrad(I_UP7, U->a6_2, U->dcat7, 128, g, 3));
-        if (D(I_C62)) TRY(deconv_dgrad(I_UP7, U->dcat7, 128, U->dz6_2, U->a6_2, 3));
-        if (W(I_C62)) TRY(conv_wgrad(I_C62, U->a6_1, 256, 0, U->dz6_2, g, 3));
-        if (D(I_C61)) TRY(conv_dgrad(I_C62, U->dz6_2, U->dz6_1, 256, 0, U->a6_1, 3));
-        if (W(I_C61)) TRY(conv_wgrad(I_C61, U->cat6, 512, 0, U->dz6_1, g, 3));
+        if (W(I_UP7)) TRY(deconv_wgrad(I_UP7, S->a6_2, U->dcat7, 128, g, 3));
+        if (D(I_C62)) TRY(deconv_dgrad(I_UP7, U->dcat7, 128, U->dz6_2, S->a6_2, 3));
+        if (W(I_C62)) TRY(conv_wgrad(I_C62, S->a6_1, 256, 0, U->dz6_2, g, 3));
+        if (D(I_C61)) TRY(conv_dgrad(I_C62, U->dz6_2, U->dz6_1, 256, 0, S->a6_1, 3));
+        if (W(I_C61)) TRY(conv_wgrad(I_C61, S->cat6, 512, 0, U->dz6_1, g, 3));
         if (D(I_UP6)) TRY(concat_dgrad(I_C61, U->dz6_1, U->dcat6, 3));
-        if (W(I_UP6)) TRY(deconv_wgrad(I_UP6, U->a5_2, U->dcat6, 256, g, 4));
+        if (W(I_UP6)) TRY(deconv_wgrad(I_UP6, S->a5_2, U->dcat6, 256, g, 4));
         TRY(finish_bucket(0, g));
-        if (D(I_C52)) TRY(deconv_dgrad(I_UP6, U->dcat6, 256, U->dz5_2, U->a5_2, 4));
+        if (D(I_C52)) TRY(deconv_dgrad(I_UP6, U->dcat6, 256, U->dz5_2, S->a5_2, 4));
         // bottleneck + encoder
-        if (W(I_C52)) TRY(conv_wgrad(I_C52, U->a5_1, 512, 0, U->dz5_2, g, 4));
-        if (D(I_C51)) TRY(conv_dgrad(I_C52, U->dz5_2, U->dz5_1, 512, 0, U->a5_1, 4));
-        if (W(I_C51)) TRY(conv_wgrad(I_C51, U->p4, 256, 0, U->dz5_1, g, 4));
+        if (W(I_C52)) TRY(conv_wgrad(I_C52, S->a5_1, 512, 0, U->dz5_2, g, 4));
+        if (D(I_C51)) TRY(conv_dgrad(I_C52, U->dz5_2, U->dz5_1, 512, 0, S->a5_1, 4));
+        if (W(I_C51)) TRY(conv_wgrad(I_C51, S->p4, 256, 0, U->dz5_1, g, 4));
         TRY(finish_bucket(1, g));
         if (D(I_C42)) TRY(conv_dgrad(I_C51, U->dz5_1, U->dp4, 256, 0, nullptr, 4));
-        if (D(I_C42)) TRY(pool_bwd(U->pc4, skip_half(U->dcat6, 3, 256), U->dp4, U->dz4_2, 256, 4));
-        if (W(I_C42)) TRY(conv_wgrad(I_C42, U->a4_1, 256, 0, U->dz4_2, g, 3));
-        if (D(I_C41)) TRY(conv_dgrad(I_C42, U->dz4_2, U->dz4_1, 256, 0, U->a4_1, 3));
-        if (W(I_C41)) TRY(conv_wgrad(I_C41, U->p3, 128, 0, U->dz4_1, g, 3));
+        if (D(I_C42)) TRY(pool_bwd(S->pc4, skip_half(U->dcat6, 3, 256), U->dp4, U->dz4_2, 256, 4));
+        if (W(I_C42)) TRY(conv_wgrad(I_C42, S->a4_1, 256, 0, U->dz4_2, g, 3));
+        if (D(I_C41)) TRY(conv_dgrad(I_C42, U->dz4_2, U->dz4_1, 256, 0, S->a4_1, 3));
+        if (W(I_C41)) TRY(conv_wgrad(I_C41, S->p3, 128, 0, U->dz4_1, g, 3));
         if (D(I_C32)) TRY(conv_dgrad(I_C41, U->dz4_1, U->dp3, 128, 0, nullptr, 3));
-        if (D(I_C32)) TRY(pool_bwd(U->pc3, skip_half(U->dcat7, 2, 128), U->dp3, U->dz3_2, 128, 3));
-        if (W(I_C32)) TRY(conv_wgrad(I_C32, U->a3_1, 128, 0, U->dz3_2, g, 2));
-        if (D(I_C31)) TRY(conv_dgrad(I_C32, U->dz3_2, U->dz3_1, 128, 0, U->a3_1, 2));
-        if (W(I_C31)) TRY(conv_wgrad(I_C31, U->p2, 64, 0, U->dz3_1, g, 2));
+        if (D(I_C32)) TRY(pool_bwd(S->pc3, skip_half(U->dcat7, 2, 128), U->dp3, U->dz3_2, 128, 3));
+        if (W(I_C32)) TRY(conv_wgrad(I_C32, S->a3_1, 128, 0, U->dz3_2, g, 2));
+        if (D(I_C31)) TRY(conv_dgrad(I_C32, U->dz3_2, U->dz3_1, 128, 0, S->a3_1, 2));
+        if (W(I_C31)) TRY(conv_wgrad(I_C31, S->p2, 64, 0, U->dz3_1, g, 2));
         if (D(I_C22)) TRY(conv_dgrad(I_C31, U->dz3_1, U->dp2, 64, 0, nullptr, 2));
-        if (D(I_C22)) TRY(pool_bwd(U->pc2, skip_half(U->dcat8, 1, 64), U->dp2, U->dz2_2, 64, 2));
-        if (W(I_C22)) TRY(conv_wgrad(I_C22, U->a2_1, 64, 0, U->dz2_2, g, 1));
-        if (D(I_C21)) TRY(conv_dgrad(I_C22, U->dz2_2, U->dz2_1, 64, 0, U->a2_1, 1));
-        if (W(I_C21)) TRY(conv_wgrad(I_C21, U->p1, 32, 0, U->dz2_1, g, 1));
+        if (D(I_C22)) TRY(pool_bwd(S->pc2, skip_half(U->dcat8, 1, 64), U->dp2, U->dz2_2, 64, 2));
+        if (W(I_C22)) TRY(conv_wgrad(I_C22, S->a2_1, 64, 0, U->dz2_2, g, 1));
+        if (D(I_C21)) TRY(conv_dgrad(I_C22, U->dz2_2, U->dz2_1, 64, 0, S->a2_1, 1));
+        if (W(I_C21)) TRY(conv_wgrad(I_C21, S->p1, 32, 0, U->dz2_1, g, 1));
         TRY(finish_bucket(2, g));
         if (D(I_C12)) TRY(conv_dgrad(I_C21, U->dz2_1, U->dp1, 32, 0, nullptr, 1));
-        if (D(I_C12)) TRY(pool_bwd(U->pc1, skip_half(U->dcat9, 0, 32), U->dp1, U->dz1_2, 32, 1));
-        if (W(I_C12)) TRY(conv_wgrad(I_C12, U->a1_1, 32, 0, U->dz1_2, g, 0));
-        if (D(I_C11)) TRY(conv_dgrad(I_C12, U->dz1_2, U->dz1_1, 32, 0, U->a1_1, 0));
+        if (D(I_C12)) TRY(pool_bwd(S->pc1, skip_half(U->dcat9, 0, 32), U->dp1, U->dz1_2, 32, 1));
+        if (W(I_C12)) TRY(conv_wgrad(I_C12, S->a1_1, 32, 0, U->dz1_2, g, 0));
+        if (D(I_C11)) TRY(conv_dgrad(I_C12, U->dz1_2, U->dz1_1, 32, 0, S->a1_1, 0));
         if (W(I_C11)) {
             const double px = (double)U->n * U->H * U->W;
             Scope sc(u, st, "conv1_1", "wgrad", 2.0 * px * 32 * 9 * U->cin0, px * (4 * U->cin0 + 64));
@@ -788,16 +813,33 @@ struct Runner {
 
 }  // namespace
 
+// The forward state a call works on: the built-in one (state == NULL), or one laid out in the caller's memory by the
+// same layout() (into `tmp`; host-side only)
+static const FwdState* state_at(eld_unet* u, void* state, FwdState& tmp)
+{
+    if (!state) return &u->fs;
+    char* base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(state) + 1023) & ~(uintptr_t)1023);
+    layout(u, &tmp, base, true, false);
+    return &tmp;
+}
+
 extern "C" int eld_unet_forward(eld_unet* u, const float* params, const float* x, float* out, void* stream)
 {
+    return eld_unet_forward_state(u, nullptr, params, x, out, stream);
+}
+
+extern "C" int eld_unet_forward_state(eld_unet* u, void* state, const float* params, const float* x, float* out, void* stream)
+{
     ELD_REQUIRE(u && params && x && out, "eld_unet_forward: NULL argument");
+    ELD_REQUIRE(!state || u->dz9_2 != nullptr, "eld_unet_forward_state: a caller state needs an eld_unet created with train = 1");
     u->dz1_1_final = false;
     ELD_CHECK_CUDA(cudaSetDevice(u->ctx->device));
-    Runner r{ u, params, static_cast<cudaStream_t>(stream) };
+    FwdState tmp;
+    Runner r{ u, state_at(u, state, tmp), params, static_cast<cudaStream_t>(stream) };
     TRY(r.forward(x));
     const double hpx = (double)u->n * u->H * u->W;
     Scope sc(u, r.st, "conv10_1", "fprop", 2.0 * hpx * 128, hpx * (64 + 16));
-    return launch_head(u->ctx, u->a9_2, params + u->L[I_C10].w_off, params + u->L[I_C10].b_off, out, nullptr, nullptr,
+    return launch_head(u->ctx, r.s->a9_2, params + u->L[I_C10].w_off, params + u->L[I_C10].b_off, out, nullptr, nullptr,
                        nullptr, nullptr, nullptr, u->n, (size_t)u->H * u->W, u->cout_last, 0, r.st);
 }
 
@@ -808,7 +850,7 @@ extern "C" int eld_unet_train_step(eld_unet* u, const float* params, const float
     ELD_REQUIRE(u->dz9_2 != nullptr, "eld_unet_train_step: the eld_unet was created with train = 0");
     u->dz1_1_final = false;
     ELD_CHECK_CUDA(cudaSetDevice(u->ctx->device));
-    Runner r{ u, params, static_cast<cudaStream_t>(stream) };
+    Runner r{ u, &u->fs, params, static_cast<cudaStream_t>(stream) };
     ELD_CHECK_CUDA(cudaMemsetAsync(grads, 0, u->n_params * sizeof(float), r.st));
     ELD_CHECK_CUDA(cudaMemsetAsync(u->gtmp, 0, u->n_params * sizeof(float), r.st));
     ELD_CHECK_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), r.st));
@@ -819,7 +861,7 @@ extern "C" int eld_unet_train_step(eld_unet* u, const float* params, const float
         const double hpx = (double)u->n * u->H * u->W;
         Scope sc(u, r.st, "conv10_1", dz || dw ? "fwd+loss+bwd" : "fwd+loss", (dz || dw ? 6.0 : 2.0) * hpx * 128,
                  hpx * (64 + 16 + 16 + (dz ? 64 : 0)));
-        TRY(launch_head(u->ctx, u->a9_2, params + u->L[I_C10].w_off, params + u->L[I_C10].b_off, out, target, dz ? u->dz9_2 : nullptr,
+        TRY(launch_head(u->ctx, u->fs.a9_2, params + u->L[I_C10].w_off, params + u->L[I_C10].b_off, out, target, dz ? u->dz9_2 : nullptr,
                         dw ? grads + u->L[I_C10].w_off : nullptr, dw ? grads + u->L[I_C10].b_off : nullptr, loss, u->n,
                         (size_t)u->H * u->W, u->cout_last, u->l2_loss, r.st));
     }
@@ -830,10 +872,17 @@ extern "C" int eld_unet_train_step(eld_unet* u, const float* params, const float
 
 extern "C" int eld_unet_backward(eld_unet* u, const float* params, const float* x, const float* dout, float* grads, void* stream)
 {
+    return eld_unet_backward_state(u, nullptr, params, x, dout, grads, stream);
+}
+
+extern "C" int eld_unet_backward_state(eld_unet* u, void* state, const float* params, const float* x, const float* dout,
+                                       float* grads, void* stream)
+{
     ELD_REQUIRE(u && params && x && dout && grads, "eld_unet_backward: NULL argument");
     ELD_REQUIRE(u->dz9_2 != nullptr, "eld_unet_backward: the eld_unet was created with train = 0");
     ELD_CHECK_CUDA(cudaSetDevice(u->ctx->device));
-    Runner r{ u, params, static_cast<cudaStream_t>(stream) };
+    FwdState tmp;
+    Runner r{ u, state_at(u, state, tmp), params, static_cast<cudaStream_t>(stream) };
     ELD_CHECK_CUDA(cudaMemsetAsync(grads, 0, u->n_params * sizeof(float), r.st));
     ELD_CHECK_CUDA(cudaMemsetAsync(u->gtmp, 0, u->n_params * sizeof(float), r.st));
     if (u->reach[I_C10]) {
@@ -841,7 +890,7 @@ extern "C" int eld_unet_backward(eld_unet* u, const float* params, const float* 
         const double hpx = (double)u->n * u->H * u->W;
         Scope sc(u, r.st, "conv10_1", "bwd", 4.0 * hpx * 128, hpx * (64 + 16 + (dz ? 64 : 0)));
         // the head re-forms `out` into scratch (dz1_1 is not written before the very end of backward) and back-propagates dout
-        TRY(launch_head(u->ctx, u->a9_2, params + u->L[I_C10].w_off, params + u->L[I_C10].b_off,
+        TRY(launch_head(u->ctx, r.s->a9_2, params + u->L[I_C10].w_off, params + u->L[I_C10].b_off,
                         reinterpret_cast<float*>(u->dz1_1), dout, dz ? u->dz9_2 : nullptr,
                         dw ? grads + u->L[I_C10].w_off : nullptr, dw ? grads + u->L[I_C10].b_off : nullptr, nullptr, u->n,
                         (size_t)u->H * u->W, u->cout_last, 2, r.st));
@@ -872,27 +921,30 @@ extern "C" int eld_unet_input_grad(eld_unet* u, const float* params, float* dx, 
     return launch_first_conv_dgrad(u->ctx, u->dz1_1, params + u->L[I_C11].w_off, u->cin0, dx, u->n, u->H, u->W, st);
 }
 
-// The intermediate tensors of the step by name: member, level (1/2^lvl of the frame), units per pixel, training only.
+// The intermediate tensors of the step by name: member, level (1/2^lvl of the frame), units per pixel.  Activations
+// belong to the built-in forward state; the gradients are backward scratch (training only).
 // A gradient of a concat input (dcat*) is the whole planar buffer: [n][h][w][C/2] up plane, then the skip plane.
-static const struct { const char* name; __nv_bfloat16* eld_unet::*p; int lvl, ch; bool train; } kBuffers[] = {
-    { "a1_1", &eld_unet::a1_1, 0, 32, false },  { "cat9", &eld_unet::cat9, 0, 64, false },   { "p1", &eld_unet::p1, 1, 32, false },
-    { "a2_1", &eld_unet::a2_1, 1, 64, false },  { "cat8", &eld_unet::cat8, 1, 128, false },  { "p2", &eld_unet::p2, 2, 64, false },
-    { "a3_1", &eld_unet::a3_1, 2, 128, false }, { "cat7", &eld_unet::cat7, 2, 256, false },  { "p3", &eld_unet::p3, 3, 128, false },
-    { "a4_1", &eld_unet::a4_1, 3, 256, false }, { "cat6", &eld_unet::cat6, 3, 512, false },  { "p4", &eld_unet::p4, 4, 256, false },
-    { "a5_1", &eld_unet::a5_1, 4, 512, false }, { "a5_2", &eld_unet::a5_2, 4, 512, false },
-    { "a6_1", &eld_unet::a6_1, 3, 256, false }, { "a6_2", &eld_unet::a6_2, 3, 256, false },
-    { "a7_1", &eld_unet::a7_1, 2, 128, false }, { "a7_2", &eld_unet::a7_2, 2, 128, false },
-    { "a8_1", &eld_unet::a8_1, 1, 64, false },  { "a8_2", &eld_unet::a8_2, 1, 64, false },
-    { "a9_1", &eld_unet::a9_1, 0, 32, false },  { "a9_2", &eld_unet::a9_2, 0, 32, false },
-    { "dz9_2", &eld_unet::dz9_2, 0, 32, true },  { "dz9_1", &eld_unet::dz9_1, 0, 32, true },  { "dcat9", &eld_unet::dcat9, 0, 64, true },
-    { "dz8_2", &eld_unet::dz8_2, 1, 64, true },  { "dz8_1", &eld_unet::dz8_1, 1, 64, true },  { "dcat8", &eld_unet::dcat8, 1, 128, true },
-    { "dz7_2", &eld_unet::dz7_2, 2, 128, true }, { "dz7_1", &eld_unet::dz7_1, 2, 128, true }, { "dcat7", &eld_unet::dcat7, 2, 256, true },
-    { "dz6_2", &eld_unet::dz6_2, 3, 256, true }, { "dz6_1", &eld_unet::dz6_1, 3, 256, true }, { "dcat6", &eld_unet::dcat6, 3, 512, true },
-    { "dz5_2", &eld_unet::dz5_2, 4, 512, true }, { "dz5_1", &eld_unet::dz5_1, 4, 512, true }, { "dp4", &eld_unet::dp4, 4, 256, true },
-    { "dz4_2", &eld_unet::dz4_2, 3, 256, true }, { "dz4_1", &eld_unet::dz4_1, 3, 256, true }, { "dp3", &eld_unet::dp3, 3, 128, true },
-    { "dz3_2", &eld_unet::dz3_2, 2, 128, true }, { "dz3_1", &eld_unet::dz3_1, 2, 128, true }, { "dp2", &eld_unet::dp2, 2, 64, true },
-    { "dz2_2", &eld_unet::dz2_2, 1, 64, true },  { "dz2_1", &eld_unet::dz2_1, 1, 64, true },  { "dp1", &eld_unet::dp1, 1, 32, true },
-    { "dz1_2", &eld_unet::dz1_2, 0, 32, true },  { "dz1_1", &eld_unet::dz1_1, 0, 32, true },
+static const struct { const char* name; __nv_bfloat16* FwdState::*p; int lvl, ch; } kStateBuffers[] = {
+    { "a1_1", &FwdState::a1_1, 0, 32 },  { "cat9", &FwdState::cat9, 0, 64 },   { "p1", &FwdState::p1, 1, 32 },
+    { "a2_1", &FwdState::a2_1, 1, 64 },  { "cat8", &FwdState::cat8, 1, 128 },  { "p2", &FwdState::p2, 2, 64 },
+    { "a3_1", &FwdState::a3_1, 2, 128 }, { "cat7", &FwdState::cat7, 2, 256 },  { "p3", &FwdState::p3, 3, 128 },
+    { "a4_1", &FwdState::a4_1, 3, 256 }, { "cat6", &FwdState::cat6, 3, 512 },  { "p4", &FwdState::p4, 4, 256 },
+    { "a5_1", &FwdState::a5_1, 4, 512 }, { "a5_2", &FwdState::a5_2, 4, 512 },
+    { "a6_1", &FwdState::a6_1, 3, 256 }, { "a6_2", &FwdState::a6_2, 3, 256 },
+    { "a7_1", &FwdState::a7_1, 2, 128 }, { "a7_2", &FwdState::a7_2, 2, 128 },
+    { "a8_1", &FwdState::a8_1, 1, 64 },  { "a8_2", &FwdState::a8_2, 1, 64 },
+    { "a9_1", &FwdState::a9_1, 0, 32 },  { "a9_2", &FwdState::a9_2, 0, 32 },
+};
+static const struct { const char* name; __nv_bfloat16* eld_unet::*p; int lvl, ch; } kScratchBuffers[] = {
+    { "dz9_2", &eld_unet::dz9_2, 0, 32 },  { "dz9_1", &eld_unet::dz9_1, 0, 32 },  { "dcat9", &eld_unet::dcat9, 0, 64 },
+    { "dz8_2", &eld_unet::dz8_2, 1, 64 },  { "dz8_1", &eld_unet::dz8_1, 1, 64 },  { "dcat8", &eld_unet::dcat8, 1, 128 },
+    { "dz7_2", &eld_unet::dz7_2, 2, 128 }, { "dz7_1", &eld_unet::dz7_1, 2, 128 }, { "dcat7", &eld_unet::dcat7, 2, 256 },
+    { "dz6_2", &eld_unet::dz6_2, 3, 256 }, { "dz6_1", &eld_unet::dz6_1, 3, 256 }, { "dcat6", &eld_unet::dcat6, 3, 512 },
+    { "dz5_2", &eld_unet::dz5_2, 4, 512 }, { "dz5_1", &eld_unet::dz5_1, 4, 512 }, { "dp4", &eld_unet::dp4, 4, 256 },
+    { "dz4_2", &eld_unet::dz4_2, 3, 256 }, { "dz4_1", &eld_unet::dz4_1, 3, 256 }, { "dp3", &eld_unet::dp3, 3, 128 },
+    { "dz3_2", &eld_unet::dz3_2, 2, 128 }, { "dz3_1", &eld_unet::dz3_1, 2, 128 }, { "dp2", &eld_unet::dp2, 2, 64 },
+    { "dz2_2", &eld_unet::dz2_2, 1, 64 },  { "dz2_1", &eld_unet::dz2_1, 1, 64 },  { "dp1", &eld_unet::dp1, 1, 32 },
+    { "dz1_2", &eld_unet::dz1_2, 0, 32 },  { "dz1_1", &eld_unet::dz1_1, 0, 32 },
 };
 
 /* Host-side view of the workspace for tests and debugging: where tensor `name` of the last step lives.  No launch. */
@@ -900,29 +952,32 @@ extern "C" int eld_unet_buffer(const eld_unet* u, const char* name, void** ptr, 
 {
     ELD_REQUIRE(u && name && ptr && dims && elem_bytes, "eld_unet_buffer: NULL argument");
     const bool train = u->dz9_2 != nullptr;
+    const FwdState& fs = u->fs;
     auto put = [&](const void* p, int n, int h, int w, int units, int eb) {
         *ptr = const_cast<void*>(p); dims[0] = n; dims[1] = h; dims[2] = w; dims[3] = units; *elem_bytes = eb;
         return ELD_OK;
     };
-    for (const auto& b : kBuffers) {
+    for (const auto& b : kStateBuffers)
+        if (strcmp(name, b.name) == 0) return put(fs.*b.p, u->n, u->H >> b.lvl, u->W >> b.lvl, b.ch, 2);
+    for (const auto& b : kScratchBuffers) {
         if (strcmp(name, b.name) != 0) continue;
-        ELD_REQUIRE(train || !b.train, "eld_unet_buffer: '%s' exists only in a training workspace", name);
+        ELD_REQUIRE(train, "eld_unet_buffer: '%s' exists only in a training workspace", name);
         return put(u->*b.p, u->n, u->H >> b.lvl, u->W >> b.lvl, b.ch, 2);
     }
     // pool codes: one byte per pooled element (32 bytes per pooled pixel and 32 channels)
-    static const struct { const char* name; __nv_bfloat16* eld_unet::*p; int lvl, ch; } kCodes[] = {
-        { "pc1", &eld_unet::pc1, 1, 32 }, { "pc2", &eld_unet::pc2, 2, 64 }, { "pc3", &eld_unet::pc3, 3, 128 }, { "pc4", &eld_unet::pc4, 4, 256 },
+    static const struct { const char* name; __nv_bfloat16* FwdState::*p; int lvl, ch; } kCodes[] = {
+        { "pc1", &FwdState::pc1, 1, 32 }, { "pc2", &FwdState::pc2, 2, 64 }, { "pc3", &FwdState::pc3, 3, 128 }, { "pc4", &FwdState::pc4, 4, 256 },
     };
     for (const auto& c : kCodes) {
         if (strcmp(name, c.name) != 0) continue;
         ELD_REQUIRE(train, "eld_unet_buffer: '%s' exists only in a training workspace", name);
-        return put(u->*c.p, u->n, u->H >> c.lvl, u->W >> c.lvl, c.ch, 1);
+        return put(fs.*c.p, u->n, u->H >> c.lvl, u->W >> c.lvl, c.ch, 1);
     }
     if (strncmp(name, "sign:", 5) == 0) {            // sign words of an activation: uint32 [pixel][channels / 32]
-        for (const auto& b : kBuffers) {
-            if (b.train || strcmp(name + 5, b.name) != 0) continue;
-            for (int i = 0; i < u->n_signs; ++i)
-                if (u->signs[i].act == u->*b.p) return put(u->signs[i].words, u->n, u->H >> b.lvl, u->W >> b.lvl, b.ch / 32, 4);
+        for (const auto& b : kStateBuffers) {
+            if (strcmp(name + 5, b.name) != 0) continue;
+            for (int i = 0; i < fs.n_signs; ++i)
+                if (fs.signs[i].act == fs.*b.p) return put(fs.signs[i].words, u->n, u->H >> b.lvl, u->W >> b.lvl, b.ch / 32, 4);
         }
         set_error("eld_unet_buffer: no sign words '%s' in this workspace", name);
         return ELD_E_ARG;
@@ -934,7 +989,7 @@ extern "C" int eld_unet_buffer(const eld_unet* u, const char* name, void** ptr, 
             if (strcmp(name + 3, l.name) != 0 || l.type == L_CONV1 || (i == I_C11 && !fprop)) continue;
             // conv1_1: the [32 co][64 k] K-major image of first_conv.cuh; the others: the operand packed_index describes
             const int count = i == I_C11 ? 32 * 64 : l.cin * l.cout * (l.type == L_CONV3 ? 9 : 4);
-            return put(u->packed + (fprop ? l.wf_off : l.wd_off), 1, 1, 1, count, 2);
+            return put(fs.packed + (fprop ? l.wf_off : l.wd_off), 1, 1, 1, count, 2);
         }
         set_error("eld_unet_buffer: no packed operand '%s'", name);
         return ELD_E_ARG;

@@ -94,6 +94,20 @@ int    eld_unet_backward(eld_unet* u, const float* params, const float* x, const
  * dx f32 NCHW [n][cin][h][w], overwritten.  bf16 conv1_1 gradient and weights, fp32 accumulation.  Fails on an object
  * created with train = 0 and when no backward or train step has run since the last forward. */
 int    eld_unet_input_grad(eld_unet* u, const float* params, float* dx, void* stream);
+/* Several forwards before their backwards (a loss that calls the network twice, torch.utils.checkpoint, a retained
+ * graph): what a forward leaves for its backward - activations, pool codes, sign words, packed weights - is its FORWARD
+ * STATE.  A train = 1 object holds one in its workspace (the built-in state, which eld_unet_forward / eld_unet_backward /
+ * eld_unet_train_step use); a caller may give a forward a state of its own and later back-propagate from that state,
+ * whatever ran on the object in between.  state == NULL means the built-in state, so eld_unet_forward(u, ...) is
+ * eld_unet_forward_state(u, NULL, ...) and eld_unet_backward likewise.  A caller state is device memory of
+ * eld_unet_state_bytes(n, h, w, cin, cout) bytes at any address (laid out from its first 1 KB boundary); a non-NULL state
+ * needs an object created with train = 1.  The backward writes only its own scratch and `grads`, so a state stays valid
+ * after a backward that read it and may be back-propagated again.  Launches, grids and tiles are those of
+ * eld_unet_forward / eld_unet_backward; eld_unet_input_grad follows either backward as before. */
+size_t eld_unet_state_bytes(int n, int h, int w, int cin, int cout);   /* 0 for bad arguments */
+int    eld_unet_forward_state(eld_unet* u, void* state, const float* params, const float* x, float* out, void* stream);
+int    eld_unet_backward_state(eld_unet* u, void* state, const float* params, const float* x, const float* dout,
+                               float* grads, void* stream);
 /* Frozen parameters (p.requires_grad_(False) in the reference, ELD_model.py:473-475): which gradients the following
  * eld_unet_train_step / eld_unet_backward compute.  flags: one byte per parameter tensor in state_dict order (46: weight
  * and bias of every layer), nonzero = trainable; input_grad != 0 keeps the data-gradient chain running down to conv1_1
