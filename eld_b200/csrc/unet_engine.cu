@@ -16,38 +16,59 @@
 namespace eld {
 
 enum { L_CONV3 = 0, L_DECONV = 1, L_CONV1 = 2 };
-struct Layer { const char* name; int type, cin, cout; size_t w_off, b_off, wf_off, wd_off; };
-
-// state_dict order of UNetSeeInDark (Unet.py:11-46)
-static const struct { const char* name; int type, cin, cout; } kLayers[] = {
-    { "conv1_1", L_CONV3, 4, 32 },    { "conv1_2", L_CONV3, 32, 32 },   { "conv2_1", L_CONV3, 32, 64 },
-    { "conv2_2", L_CONV3, 64, 64 },   { "conv3_1", L_CONV3, 64, 128 },  { "conv3_2", L_CONV3, 128, 128 },
-    { "conv4_1", L_CONV3, 128, 256 }, { "conv4_2", L_CONV3, 256, 256 }, { "conv5_1", L_CONV3, 256, 512 },
-    { "conv5_2", L_CONV3, 512, 512 }, { "upv6", L_DECONV, 512, 256 },   { "conv6_1", L_CONV3, 512, 256 },
-    { "conv6_2", L_CONV3, 256, 256 }, { "upv7", L_DECONV, 256, 128 },   { "conv7_1", L_CONV3, 256, 128 },
-    { "conv7_2", L_CONV3, 128, 128 }, { "upv8", L_DECONV, 128, 64 },    { "conv8_1", L_CONV3, 128, 64 },
-    { "conv8_2", L_CONV3, 64, 64 },   { "upv9", L_DECONV, 64, 32 },     { "conv9_1", L_CONV3, 64, 32 },
-    { "conv9_2", L_CONV3, 32, 32 },   { "conv10_1", L_CONV1, 32, 4 },
-};
-constexpr int kNumLayers = sizeof(kLayers) / sizeof(kLayers[0]);
 enum { I_C11 = 0, I_C12, I_C21, I_C22, I_C31, I_C32, I_C41, I_C42, I_C51, I_C52, I_UP6, I_C61, I_C62, I_UP7,
        I_C71, I_C72, I_UP8, I_C81, I_C82, I_UP9, I_C91, I_C92, I_C10 };
+struct LayerSpec { const char* name; int type, cin, cout, lvl, src, skip; };
+struct Layer : LayerSpec { size_t w_off, b_off, wf_off, wd_off; };
+
+// UNetSeeInDark (Unet.py:11-46) in state_dict order, which is a topological order of its forward graph.  lvl: the grid of
+// the layer's output, 1/2^lvl of the frame (a deconv's is the fine grid it writes).  src: the layer whose output it reads
+// (-1 = the input frame x; a pool between two encoder levels does not change who produced the tensor).  skip: for the four
+// concatenating convs, the encoder layer behind the skip half of their input (Unet.py:69,74,79,84).  Every buffer, launch
+// and backward step of the engine is derived from this table.
+static const LayerSpec kLayers[] = {
+    //  name       type      cin  cout lvl  src    skip
+    { "conv1_1",  L_CONV3,    4,  32, 0, -1,    -1 },
+    { "conv1_2",  L_CONV3,   32,  32, 0, I_C11, -1 },
+    { "conv2_1",  L_CONV3,   32,  64, 1, I_C12, -1 },
+    { "conv2_2",  L_CONV3,   64,  64, 1, I_C21, -1 },
+    { "conv3_1",  L_CONV3,   64, 128, 2, I_C22, -1 },
+    { "conv3_2",  L_CONV3,  128, 128, 2, I_C31, -1 },
+    { "conv4_1",  L_CONV3,  128, 256, 3, I_C32, -1 },
+    { "conv4_2",  L_CONV3,  256, 256, 3, I_C41, -1 },
+    { "conv5_1",  L_CONV3,  256, 512, 4, I_C42, -1 },
+    { "conv5_2",  L_CONV3,  512, 512, 4, I_C51, -1 },
+    { "upv6",     L_DECONV, 512, 256, 3, I_C52, -1 },
+    { "conv6_1",  L_CONV3,  512, 256, 3, I_UP6, I_C42 },
+    { "conv6_2",  L_CONV3,  256, 256, 3, I_C61, -1 },
+    { "upv7",     L_DECONV, 256, 128, 2, I_C62, -1 },
+    { "conv7_1",  L_CONV3,  256, 128, 2, I_UP7, I_C32 },
+    { "conv7_2",  L_CONV3,  128, 128, 2, I_C71, -1 },
+    { "upv8",     L_DECONV, 128,  64, 1, I_C72, -1 },
+    { "conv8_1",  L_CONV3,  128,  64, 1, I_UP8, I_C22 },
+    { "conv8_2",  L_CONV3,   64,  64, 1, I_C81, -1 },
+    { "upv9",     L_DECONV,  64,  32, 0, I_C82, -1 },
+    { "conv9_1",  L_CONV3,   64,  32, 0, I_UP9, I_C12 },
+    { "conv9_2",  L_CONV3,   32,  32, 0, I_C91, -1 },
+    { "conv10_1", L_CONV1,   32,   4, 0, I_C92, -1 },
+};
+constexpr int kNumLayers = sizeof(kLayers) / sizeof(kLayers[0]);
+constexpr int kLevels = 5;       // the frame and the grids of the four 2x2 pools
+
+// An encoder layer behind the skip half of a concat writes channels [cout, 2 cout) of that concat buffer, and the 2x2
+// max-pool fused into its tile feeds the next level.
+static bool pooled(int l)
+{
+    for (const LayerSpec& m : kLayers) if (m.skip == l) return true;
+    return false;
+}
 
 constexpr int kGradBuckets = 4;
-// first table entry (state_dict order without conv1_1 / conv10_1) of each bucket's tile range: upv6.., conv5_1.., conv2_1..,
-// conv1_2.  The last bucket (conv1_1 + conv1_2, 42 KB) is all that is still in flight when backward ends.
-constexpr int kBucketEntry0[kGradBuckets] = { 9, 7, 1, 0 };
-constexpr int kBucketEntry1[kGradBuckets] = { 21, 9, 7, 1 };
-constexpr int kBucketLayer0[kGradBuckets] = { 10 /*upv6*/, 8 /*conv5_1*/, 2 /*conv2_1*/, 0 /*conv1_1*/ };
-constexpr int kBucketLayer1[kGradBuckets] = { 23, 10, 8, 2 };   // one past the last layer
-
-// The forward graph the backward walks in reverse: the layer whose output each layer reads (-1 = the input frame x; a
-// pool between two encoder levels does not change who produced the tensor), and for the four concatenating convs the
-// encoder layer behind the skip half of their input (Unet.py:69,74,79,84).  State_dict order is a topological order.
-constexpr int kSrc[kNumLayers] = { -1, I_C11, I_C12, I_C21, I_C22, I_C31, I_C32, I_C41, I_C42, I_C51, I_C52, I_UP6, I_C61,
-                                   I_C62, I_UP7, I_C71, I_C72, I_UP8, I_C81, I_C82, I_UP9, I_C91, I_C92 };
-constexpr int kSkip[kNumLayers] = { -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, I_C42 /*conv6_1*/, -1, -1, I_C32 /*conv7_1*/,
-                                    -1, -1, I_C22 /*conv8_1*/, -1, -1, I_C12 /*conv9_1*/, -1, -1 };
+// The first layer of each gradient bucket, in backward-completion order; a bucket runs up to the first layer of the one
+// before it: upv6..conv10_1, conv5_1..conv5_2, conv2_1..conv4_2, conv1_1..conv1_2.  The last bucket (42 KB) is all that
+// is still in flight when backward ends.
+constexpr int kBucketFirst[kGradBuckets] = { I_UP6, I_C51, I_C21, I_C11 };
+static int bucket_end(int k) { return k == 0 ? kNumLayers : kBucketFirst[k - 1]; }
 
 struct PackEntry { unsigned long long src, dst_f, dst_d; int cout, cin, type; int pad; };
 struct PackTable {
@@ -227,14 +248,13 @@ using namespace eld;
 // the caller owns (eld_unet_forward_state).  The backward writes none of it, so a state stays valid after a backward
 // that read it.
 struct FwdState {
-    __nv_bfloat16 *a1_1, *cat9, *p1, *a2_1, *cat8, *p2, *a3_1, *cat7, *p3, *a4_1, *cat6, *p4, *a5_1, *a5_2,
-        *a6_1, *a6_2, *a7_1, *a7_2, *a8_1, *a8_2, *a9_1, *a9_2;
-    __nv_bfloat16 *pc1 = nullptr, *pc2 = nullptr, *pc3 = nullptr, *pc4 = nullptr;   // pool codes, 1 byte per pooled element (training)
+    __nv_bfloat16* act[kNumLayers] = {};     // the output of each layer that has a buffer of its own
     // sign words (1 bit per element) of the activations whose LeakyReLU' a data gradient applies (training): the dgrad
     // tiles read these instead of the activation itself
-    struct SignBuf { const void* act; uint32_t* words; } signs[16];
-    int n_signs = 0;
-    __nv_bfloat16* packed;
+    uint32_t* sign[kNumLayers] = {};
+    // per level: the concat buffer, and the pooled tensor with its pool codes (1 byte per pooled element, training)
+    __nv_bfloat16 *cat[kLevels] = {}, *pool[kLevels] = {}, *code[kLevels] = {};
+    __nv_bfloat16* packed = nullptr;
 };
 
 struct eld_unet {
@@ -244,10 +264,11 @@ struct eld_unet {
     size_t n_params;
     char* ws;
     size_t ws_bytes;
+    bool train = false;
     FwdState fs;                 // the built-in forward state, in ws
-    // backward scratch (bf16), in ws
-    __nv_bfloat16 *dz9_2, *dz9_1, *dcat9, *dz8_2, *dz8_1, *dcat8, *dz7_2, *dz7_1, *dcat7, *dz6_2, *dz6_1, *dcat6,
-        *dz5_2, *dz5_1, *dp4, *dz4_2, *dz4_1, *dp3, *dz3_2, *dz3_1, *dp2, *dz2_2, *dz2_1, *dp1, *dz1_2, *dz1_1;
+    // backward scratch (bf16), in ws: the gradient of each layer's output, and per level of the concat buffer (two planar
+    // halves, see Runner::conv_dgrad) and of the pooled tensor
+    __nv_bfloat16 *dz[kNumLayers] = {}, *dcat[kLevels] = {}, *dp[kLevels] = {};
     float* gtmp = nullptr;
     PackTable table;
     // gradient buckets in backward-completion order (data-parallel overlap, SURVEY 8e): decoder, bottleneck, encoder
@@ -269,49 +290,43 @@ struct eld_unet {
     size_t rec_used = 0;
 };
 
-// Places forward state `s` at `base` and, with `scratch`, the backward scratch of `u` (dz*, dcat*, dp*, gtmp) among it in
+// Places forward state `s` at `base` and, with `scratch`, the backward scratch of `u` (dz, dcat, dp, gtmp) among it in
 // the workspace's order; returns the bytes used.  Without `scratch` the state's buffers are packed back to back
 // (eld_unet_state_bytes).  train = false: activations and packed weights only.
 static size_t layout(eld_unet* u, FwdState* s, char* base, bool train, bool scratch)
 {
     size_t off = 0;
-    const size_t n = u->n;
-    auto take = [&](__nv_bfloat16** p, int lvl, int ch) {
-        const size_t h = u->H >> lvl, w = u->W >> lvl;
-        const size_t bytes = (n * h * w * ch * 2 + 1023) & ~(size_t)1023;
-        if (p) *p = reinterpret_cast<__nv_bfloat16*>(base + off);
-        off += bytes;
+    auto take = [&](int lvl, int ch) {       // ch bf16-sized units per pixel of the level's grid
+        __nv_bfloat16* p = reinterpret_cast<__nv_bfloat16*>(base + off);
+        off += ((size_t)u->n * (u->H >> lvl) * (u->W >> lvl) * ch * 2 + 1023) & ~(size_t)1023;
+        return p;
     };
-    take(&s->a1_1, 0, 32); take(&s->cat9, 0, 64); take(&s->p1, 1, 32);
-    take(&s->a2_1, 1, 64); take(&s->cat8, 1, 128); take(&s->p2, 2, 64);
-    take(&s->a3_1, 2, 128); take(&s->cat7, 2, 256); take(&s->p3, 3, 128);
-    take(&s->a4_1, 3, 256); take(&s->cat6, 3, 512); take(&s->p4, 4, 256);
-    take(&s->a5_1, 4, 512); take(&s->a5_2, 4, 512);
-    take(&s->a6_1, 3, 256); take(&s->a6_2, 3, 256); take(&s->a7_1, 2, 128); take(&s->a7_2, 2, 128);
-    take(&s->a8_1, 1, 64); take(&s->a8_2, 1, 64); take(&s->a9_1, 0, 32); take(&s->a9_2, 0, 32);
-    if (train && scratch) {
-        take(&u->dz9_2, 0, 32); take(&u->dz9_1, 0, 32); take(&u->dcat9, 0, 64);
-        take(&u->dz8_2, 1, 64); take(&u->dz8_1, 1, 64); take(&u->dcat8, 1, 128);
-        take(&u->dz7_2, 2, 128); take(&u->dz7_1, 2, 128); take(&u->dcat7, 2, 256);
-        take(&u->dz6_2, 3, 256); take(&u->dz6_1, 3, 256); take(&u->dcat6, 3, 512);
-        take(&u->dz5_2, 4, 512); take(&u->dz5_1, 4, 512); take(&u->dp4, 4, 256);
-        take(&u->dz4_2, 3, 256); take(&u->dz4_1, 3, 256); take(&u->dp3, 3, 128);
-        take(&u->dz3_2, 2, 128); take(&u->dz3_1, 2, 128); take(&u->dp2, 2, 64);
-        take(&u->dz2_2, 1, 64); take(&u->dz2_1, 1, 64); take(&u->dp1, 1, 32);
-        take(&u->dz1_2, 0, 32); take(&u->dz1_1, 0, 32);
+    // activations in state_dict order; a deconv writes into the concat buffer its level's pooled layer placed
+    for (int i = 0; i < kNumLayers; ++i) {
+        const Layer& l = u->L[i];
+        if (l.type == L_CONV1 || l.type == L_DECONV) continue;
+        if (!pooled(i)) { s->act[i] = take(l.lvl, l.cout); continue; }
+        s->cat[l.lvl] = take(l.lvl, 2 * l.cout);
+        s->pool[l.lvl + 1] = take(l.lvl + 1, l.cout);
+    }
+    if (train && scratch) {       // in the order the backward reaches them
+        for (int i = kNumLayers - 1; i >= 0; --i) {
+            const Layer& l = u->L[i];
+            if (l.type == L_CONV1) continue;
+            if (l.type == L_DECONV) { u->dcat[l.lvl] = take(l.lvl, 2 * l.cout); continue; }
+            if (pooled(i)) u->dp[l.lvl + 1] = take(l.lvl + 1, l.cout);
+            u->dz[i] = take(l.lvl, l.cout);
+        }
     }
     if (train) {
-        take(&s->pc1, 1, 16); take(&s->pc2, 2, 32); take(&s->pc3, 3, 64); take(&s->pc4, 4, 128);
-        s->n_signs = 0;
-        auto take_signs = [&](__nv_bfloat16* act, int lvl, int ch) {      // ch / 32 words per pixel = ch / 16 bf16-sized units
-            __nv_bfloat16* w = nullptr;
-            take(&w, lvl, ch / 16);
-            s->signs[s->n_signs++] = { act, reinterpret_cast<uint32_t*>(w) };
-        };
-        take_signs(s->a1_1, 0, 32); take_signs(s->a2_1, 1, 64); take_signs(s->a3_1, 2, 128); take_signs(s->a4_1, 3, 256);
-        take_signs(s->a5_1, 4, 512); take_signs(s->a5_2, 4, 512); take_signs(s->a6_1, 3, 256); take_signs(s->a6_2, 3, 256);
-        take_signs(s->a7_1, 2, 128); take_signs(s->a7_2, 2, 128); take_signs(s->a8_1, 1, 64); take_signs(s->a8_2, 1, 64);
-        take_signs(s->a9_1, 0, 32);
+        for (int i = 0; i < kNumLayers; ++i)
+            if (pooled(i)) s->code[u->L[i].lvl + 1] = take(u->L[i].lvl + 1, u->L[i].cout / 2);
+        // every activation with a buffer of its own, except the head's input: the head applies that LeakyReLU'
+        for (int i = 0; i < kNumLayers; ++i) {
+            const Layer& l = u->L[i];
+            if (l.type == L_CONV3 && !pooled(i) && i != u->L[I_C10].src)
+                s->sign[i] = reinterpret_cast<uint32_t*>(take(l.lvl, l.cout / 16));   // cout / 32 words per pixel
+        }
     }
     // packed weights
     size_t pk = 0;
@@ -337,7 +352,7 @@ static void init_layers(eld_unet* u)
     size_t off = 0;
     for (int i = 0; i < kNumLayers; ++i) {
         Layer& l = u->L[i];
-        l.name = kLayers[i].name; l.type = kLayers[i].type; l.cin = kLayers[i].cin; l.cout = kLayers[i].cout;
+        static_cast<LayerSpec&>(l) = kLayers[i];
         if (i == 0) l.cin = u->cin0;
         if (i == kNumLayers - 1) l.cout = u->cout_last;
         const size_t ksz = l.type == L_CONV3 ? 9 : (l.type == L_DECONV ? 4 : 1);
@@ -402,23 +417,24 @@ extern "C" size_t eld_unet_state_bytes(int n, int h, int w, int cin, int cout)
 }
 
 // The per-launch plan of the backward from the trainable flags (one per parameter tensor, state_dict order), by one
-// walk of the forward graph (kSrc / kSkip) in topological order: a layer's output gradient is needed when the layer
+// walk of the forward graph (src / skip) in topological order: a layer's output gradient is needed when the layer
 // trains or when the gradient of one of its inputs is.  Runner::backward launches a weight gradient where wgrad[] says
 // so and a data gradient towards every input whose producer is reached.
 static void derive_needs(eld_unet* u, const uint8_t* flags, bool input_grad)
 {
     u->input_grad = input_grad;
-    for (int l = 0; l < kNumLayers; ++l) {
-        u->wgrad[l] = flags[2 * l] || flags[2 * l + 1];
-        const bool in = kSrc[l] < 0 ? input_grad : u->reach[kSrc[l]];
-        u->reach[l] = u->wgrad[l] || in || (kSkip[l] >= 0 && u->reach[kSkip[l]]);
+    for (int i = 0; i < kNumLayers; ++i) {
+        const Layer& l = u->L[i];
+        u->wgrad[i] = flags[2 * i] || flags[2 * i + 1];
+        const bool in = l.src < 0 ? input_grad : u->reach[l.src];
+        u->reach[i] = u->wgrad[i] || in || (l.skip >= 0 && u->reach[l.skip]);
     }
     // the table holds conv1_2 .. conv9_2 in state_dict order: entry e is layer e + 1
     for (int k = 0; k <= kGradBuckets; ++k) {
-        const int e0 = k < kGradBuckets ? kBucketEntry0[k] : 0, e1 = k < kGradBuckets ? kBucketEntry1[k] : u->table.n;
-        int a = e1, b = e0;
-        for (int e = e0; e < e1; ++e)
-            if (u->wgrad[e + 1]) { a = a < e ? a : e; b = e + 1; }
+        const int l0 = k < kGradBuckets ? kBucketFirst[k] : 0, l1 = k < kGradBuckets ? bucket_end(k) : kNumLayers;
+        int a = u->table.n, b = 0;
+        for (int e = 0; e < u->table.n; ++e)
+            if (e + 1 >= l0 && e + 1 < l1 && u->wgrad[e + 1]) { a = a < e ? a : e; b = e + 1; }
         u->perm_t0[k] = a < b ? u->table.tile0[a] : 0;
         u->perm_t1[k] = a < b ? u->table.tile0[b] : 0;
     }
@@ -451,8 +467,7 @@ extern "C" int eld_unet_create_io(eld_ctx* ctx, int n, int h, int w, int train, 
         delete u;
         return ELD_E_WORKSPACE;
     }
-    u->ws = base; u->ws_bytes = bytes;
-    if (!train) u->dz9_2 = nullptr;
+    u->ws = base; u->ws_bytes = bytes; u->train = train != 0;
     int k = 0;
     for (int i = 0; i < kNumLayers; ++i) {
         const Layer& l = u->L[i];
@@ -498,8 +513,8 @@ extern "C" int eld_unet_grad_buckets_io(int cin, int cout, size_t* offsets, int 
     if (offsets) {
         ELD_REQUIRE(max_offsets >= 2 * kGradBuckets, "eld_unet_grad_buckets: need room for %d (offset, count) pairs", kGradBuckets);
         for (int k = 0; k < kGradBuckets; ++k) {
-            const size_t b = tmp.L[kBucketLayer0[k]].w_off;
-            const size_t e = kBucketLayer1[k] == kNumLayers ? tmp.n_params : tmp.L[kBucketLayer1[k]].w_off;
+            const size_t b = tmp.L[kBucketFirst[k]].w_off;
+            const size_t e = bucket_end(k) == kNumLayers ? tmp.n_params : tmp.L[bucket_end(k)].w_off;
             offsets[2 * k] = b; offsets[2 * k + 1] = e - b;
         }
     }
@@ -557,124 +572,163 @@ struct Runner {
     const __nv_bfloat16* wd(int i) const { return s->packed + u->L[i].wd_off; }
     const float* bias(int i) const { return params + u->L[i].b_off; }
 
-    // sign words of activation `act`, or nullptr: an inference engine keeps none, and a9_2's LeakyReLU' is the head's
-    uint32_t* sign_of(const void* act) const
-    {
-        for (int i = 0; i < s->n_signs; ++i) if (s->signs[i].act == act) return s->signs[i].words;
-        return nullptr;
-    }
-    // pool_dst != nullptr: MaxPool2d(2) of the output fused into the tile's epilogue (pooled tensor has cout channels)
-    int conv(int li, const void* x, int xp, int xc0, void* y, int yp, int yc0, int lvl, void* pool_dst = nullptr, void* pool_code = nullptr) const
+    // a tensor as a launch addresses it: base, channel pitch, first channel
+    struct View { __nv_bfloat16* p; int pitch, c0; };
+    // where layer li writes its output: the concat buffer of its level for a deconv (channels [0, cout)) and for a pooled
+    // layer ([cout, 2 cout)), else a buffer of its own
+    View out_of(int li) const
     {
         const Layer& l = u->L[li];
+        if (l.type == L_DECONV) return { s->cat[l.lvl], 2 * l.cout, 0 };
+        if (pooled(li)) return { s->cat[l.lvl], 2 * l.cout, l.cout };
+        return { s->act[li], l.cout, 0 };
+    }
+    // what layer li reads: the whole concat buffer for a concatenating conv, the pooled tensor of a pooled producer, else
+    // its producer's output
+    View in_of(int li) const
+    {
+        const Layer& l = u->L[li];
+        if (l.skip >= 0) return { s->cat[l.lvl], l.cin, 0 };
+        if (pooled(l.src)) return { s->pool[l.lvl], l.cin, 0 };
+        return out_of(l.src);
+    }
+
+    // a pooled layer's MaxPool2d(2) is fused into the tile's epilogue (pooled tensor has cout channels)
+    int conv(int li) const
+    {
+        const Layer& l = u->L[li];
+        const View x = in_of(li), y = out_of(li);
         GemmOp op{};
-        op.a = x; op.a_pitch = xp; op.a_c0 = xc0; op.a_mode = A_CONV; op.taps = 9; op.cin = l.cin;
-        op.n_img = u->n; op.H = u->H >> lvl; op.W = u->W >> lvl;
+        op.a = x.p; op.a_pitch = x.pitch; op.a_c0 = x.c0; op.a_mode = A_CONV; op.taps = 9; op.cin = l.cin;
+        op.n_img = u->n; op.H = u->H >> l.lvl; op.W = u->W >> l.lvl;
         op.b = wf(li); op.n_total = l.cout; op.cout = l.cout;
-        op.epi_mode = EPI_STORE; op.act = ACT_LRELU; op.out = y; op.out_pitch = yp; op.out_c0 = yc0; op.bias = bias(li);
-        op.pool_out = pool_dst; op.pool_pitch = l.cout; op.pool_code = pool_code;
-        if (yc0 == 0 && yp == l.cout) op.sign_out = sign_of(y);
+        op.epi_mode = EPI_STORE; op.act = ACT_LRELU; op.out = y.p; op.out_pitch = y.pitch; op.out_c0 = y.c0; op.bias = bias(li);
+        if (pooled(li)) { op.pool_out = s->pool[l.lvl + 1]; op.pool_code = s->code[l.lvl + 1]; }
+        op.pool_pitch = l.cout;
+        op.sign_out = s->sign[li];
         const double px = (double)u->n * op.H * op.W;
         Scope sc(u, st, l.name, "fprop", 2.0 * px * l.cout * 9 * l.cin, px * 2 * (l.cin + l.cout) + 18.0 * l.cin * l.cout);
         return launch_conv_gemm(ctx(), op, st);
     }
-    int deconv(int li, const void* x, int xp, void* y, int yp, int lvl_in) const
+    int deconv(int li) const
     {
         const Layer& l = u->L[li];
+        const View x = in_of(li), y = out_of(li);
         GemmOp op{};
-        op.a = x; op.a_pitch = xp; op.a_c0 = 0; op.a_mode = A_CONV; op.taps = 1; op.cin = l.cin;
-        op.n_img = u->n; op.H = u->H >> lvl_in; op.W = u->W >> lvl_in;
+        op.a = x.p; op.a_pitch = x.pitch; op.a_c0 = x.c0; op.a_mode = A_CONV; op.taps = 1; op.cin = l.cin;
+        op.n_img = u->n; op.H = u->H >> (l.lvl + 1); op.W = u->W >> (l.lvl + 1);
         op.b = wf(li); op.n_total = 4 * l.cout; op.cout = l.cout;
-        op.epi_mode = EPI_SHUFFLE; op.act = ACT_NONE; op.out = y; op.out_pitch = yp; op.out_c0 = 0; op.bias = bias(li);
+        op.epi_mode = EPI_SHUFFLE; op.act = ACT_NONE; op.out = y.p; op.out_pitch = y.pitch; op.out_c0 = y.c0; op.bias = bias(li);
         const double px = (double)u->n * op.H * op.W;
         Scope sc(u, st, l.name, "fprop", 2.0 * px * 4 * l.cout * l.cin, px * 2 * (l.cin + 4 * l.cout) + 8.0 * l.cin * l.cout);
         return launch_conv_gemm(ctx(), op, st);
     }
-    // data gradient of a conv: dz [cout] -> d(input) [cin channels at dxc0], optional lrelu' mask from the sign words of
-    // activation `act_src`
-    // dx2 != nullptr: the gradient of a concat input is stored as two PLANAR halves (dx = [up], dx2 = [skip], pitch cin/2
-    // each) - every consumer reads exactly one half, and an interleaved buffer made each of them move whole 128-byte
-    // lines for 64 useful bytes (ncu r01: level-1 pool.bwd 570 MB for 300, upv9 dgrad/wgrad 336 MB for 200)
-    // n_cols != 0: only the first n_cols input channels (the up half of a concat input whose skip half nobody needs),
-    // read as a row prefix of every block of the same packed dgrad operand
-    int conv_dgrad(int li, const void* dz, void* dx, int dxp, int dxc0, const void* act_src, int lvl, void* dx2 = nullptr,
-                   int n_cols = 0) const
+    // data gradient of conv li towards its input, dz [cout] -> [cin]:
+    // - a concatenating conv: into the two PLANAR halves of its level's dcat ([up], [skip], pitch cin/2 each) - every
+    //   consumer reads exactly one half, and an interleaved buffer made each of them move whole 128-byte lines for 64 useful
+    //   bytes (ncu r01: level-1 pool.bwd 570 MB for 300, upv9 dgrad/wgrad 336 MB for 200).  When nothing needs the skip
+    //   half (reach[skip]), only the up half's cin/2 columns, read as a row prefix of every block of the same packed operand.
+    // - a pooled input: into dp of its level, unmasked (pool_bwd applies the pool code)
+    // - else: into the producer's dz, with the LeakyReLU' mask from the producer's sign words
+    int conv_dgrad(int li) const
     {
         const Layer& l = u->L[li];
-        const int nc = n_cols ? n_cols : l.cin;
         GemmOp op{};
-        op.a = dz; op.a_pitch = l.cout; op.a_c0 = 0; op.a_mode = A_CONV; op.taps = 9; op.cin = l.cout;
-        op.n_img = u->n; op.H = u->H >> lvl; op.W = u->W >> lvl;
+        int nc = l.cin;
+        const bool mask = l.skip < 0 && !pooled(l.src);
+        if (l.skip >= 0) {
+            op.out = u->dcat[l.lvl]; op.out_pitch = l.cin / 2;
+            if (u->reach[l.skip]) {
+                op.out2 = skip_half(u->dcat[l.lvl], l.lvl, l.cin / 2); op.out2_pitch = l.cin / 2; op.out_split = l.cin / 2;
+            } else {
+                nc = l.cin / 2; op.b_block_rows = l.cin <= 256 ? l.cin : 256;
+            }
+        } else {
+            op.out = mask ? u->dz[l.src] : u->dp[l.lvl]; op.out_pitch = l.cin;
+        }
+        op.a = u->dz[li]; op.a_pitch = l.cout; op.a_c0 = 0; op.a_mode = A_CONV; op.taps = 9; op.cin = l.cout;
+        op.n_img = u->n; op.H = u->H >> l.lvl; op.W = u->W >> l.lvl;
         op.b = wd(li); op.n_total = nc; op.cout = nc;
-        if (n_cols) op.b_block_rows = l.cin <= 256 ? l.cin : 256;
-        op.epi_mode = EPI_STORE; op.act = act_src ? ACT_MASK : ACT_NONE;
-        op.out = dx; op.out_pitch = dxp; op.out_c0 = dxc0; op.bias = nullptr;
-        if (dx2) { op.out2 = dx2; op.out2_pitch = dxp; op.out_split = l.cin / 2; }
-        op.aux_sign = act_src ? sign_of(act_src) : nullptr;
-        ELD_REQUIRE(!act_src || op.aux_sign, "eld_unet: %s dgrad: no sign words for its LeakyReLU' mask", l.name);
+        op.epi_mode = EPI_STORE; op.act = mask ? ACT_MASK : ACT_NONE; op.out_c0 = 0; op.bias = nullptr;
+        op.aux_sign = mask ? s->sign[l.src] : nullptr;
+        ELD_REQUIRE(!mask || op.aux_sign, "eld_unet: %s dgrad: no sign words for its LeakyReLU' mask", l.name);
         const double px = (double)u->n * op.H * op.W;
-        Scope sc(u, st, l.name, "dgrad", 2.0 * px * l.cout * 9 * nc, px * 2 * (nc * (act_src ? 2 : 1) + l.cout) + 18.0 * nc * l.cout);
+        Scope sc(u, st, l.name, "dgrad", 2.0 * px * l.cout * 9 * nc, px * 2 * (nc * (mask ? 2 : 1) + l.cout) + 18.0 * nc * l.cout);
         return launch_conv_gemm(ctx(), op, st);
     }
-    // data gradient of a concatenating conv (conv6_1 .. conv9_1) into the planar [up | skip] halves of dcat; the skip half
-    // only when the encoder layer behind it, or something upstream of it, needs a gradient
-    int concat_dgrad(int li, const void* dz, __nv_bfloat16* dcat, int lvl) const
-    {
-        const int half = u->L[li].cin / 2;
-        if (!u->reach[kSkip[li]]) return conv_dgrad(li, dz, dcat, half, 0, nullptr, lvl, nullptr, half);
-        return conv_dgrad(li, dz, dcat, half, 0, nullptr, lvl, skip_half(dcat, lvl, half));
-    }
-    int deconv_dgrad(int li, const void* dy, int dyp, void* dx, const void* act_src, int lvl_in) const
+    // data gradient of a deconv: the up half of its level's dcat -> the producer's dz, with its LeakyReLU' mask
+    int deconv_dgrad(int li) const
     {
         const Layer& l = u->L[li];
         GemmOp op{};
-        op.a = dy; op.a_pitch = dyp; op.a_c0 = 0; op.a_mode = A_GATHER; op.taps = 4; op.cin = l.cout;
-        op.n_img = u->n; op.H = u->H >> lvl_in; op.W = u->W >> lvl_in;
+        op.a = u->dcat[l.lvl]; op.a_pitch = l.cout; op.a_c0 = 0; op.a_mode = A_GATHER; op.taps = 4; op.cin = l.cout;
+        op.n_img = u->n; op.H = u->H >> (l.lvl + 1); op.W = u->W >> (l.lvl + 1);
         op.b = wd(li); op.n_total = l.cin; op.cout = l.cin;
-        op.epi_mode = EPI_STORE; op.act = ACT_MASK; op.out = dx; op.out_pitch = l.cin; op.out_c0 = 0;
-        op.aux_sign = sign_of(act_src);
+        op.epi_mode = EPI_STORE; op.act = ACT_MASK; op.out = u->dz[l.src]; op.out_pitch = l.cin; op.out_c0 = 0;
+        op.aux_sign = s->sign[l.src];
         ELD_REQUIRE(op.aux_sign, "eld_unet: %s dgrad: no sign words for its LeakyReLU' mask", l.name);
         const double px = (double)u->n * op.H * op.W;
         Scope sc(u, st, l.name, "dgrad", 2.0 * px * 4 * l.cout * l.cin, px * 2 * (2 * l.cin + 4 * l.cout) + 8.0 * l.cin * l.cout);
         return launch_conv_gemm(ctx(), op, st);
     }
-    int conv_wgrad(int li, const void* x, int xp, int xc0, const void* dz, float* grads, int lvl) const
+    int conv_wgrad(int li, float* grads) const
     {
         const Layer& l = u->L[li];
+        const View x = in_of(li);
         WgradOp op{};
-        op.mode = WG_CONV; op.p = x; op.p_pitch = xp; op.p_c0 = xc0; op.p_ch = l.cin;
-        op.q = dz; op.q_pitch = l.cout; op.q_c0 = 0; op.q_ch = l.cout;
-        op.n_img = u->n; op.H = u->H >> lvl; op.W = u->W >> lvl;
+        op.mode = WG_CONV; op.p = x.p; op.p_pitch = x.pitch; op.p_c0 = x.c0; op.p_ch = l.cin;
+        op.q = u->dz[li]; op.q_pitch = l.cout; op.q_c0 = 0; op.q_ch = l.cout;
+        op.n_img = u->n; op.H = u->H >> l.lvl; op.W = u->W >> l.lvl;
         op.dw = u->gtmp + l.w_off; op.out_tco = 1;
         op.db = grads + l.b_off;                     // bias gradient fused into the same launch
         const double px = (double)u->n * op.H * op.W;
         Scope sc(u, st, l.name, "wgrad", 2.0 * px * l.cout * 9 * l.cin, px * 2 * (l.cin + l.cout) + 36.0 * l.cin * l.cout);
         return launch_wgrad(ctx(), op, st);
     }
-    int deconv_wgrad(int li, const void* x, const void* dy, int dyp, float* grads, int lvl_in) const
+    int deconv_wgrad(int li, float* grads) const
     {
         const Layer& l = u->L[li];
         WgradOp op{};
-        op.mode = WG_DECONV; op.p = dy; op.p_pitch = dyp; op.p_c0 = 0; op.p_ch = l.cout;
-        op.q = x; op.q_pitch = l.cin; op.q_c0 = 0; op.q_ch = l.cin;
-        op.n_img = u->n; op.H = u->H >> lvl_in; op.W = u->W >> lvl_in; op.dw = grads + l.w_off;
+        op.mode = WG_DECONV; op.p = u->dcat[l.lvl]; op.p_pitch = l.cout; op.p_c0 = 0; op.p_ch = l.cout;
+        op.q = in_of(li).p; op.q_pitch = l.cin; op.q_c0 = 0; op.q_ch = l.cin;
+        op.n_img = u->n; op.H = u->H >> (l.lvl + 1); op.W = u->W >> (l.lvl + 1); op.dw = grads + l.w_off;
         op.db = grads + l.b_off;                     // bias gradient = column sums of the d(up) boxes, same launch
         const double px = (double)u->n * op.H * op.W;
         Scope sc(u, st, l.name, "wgrad", 2.0 * px * 4 * l.cout * l.cin, px * 2 * (l.cin + 4 * l.cout) + 16.0 * l.cin * l.cout);
         return launch_wgrad(ctx(), op, st);
     }
-    // from the argmax + sign code the forward tile left (the activation is not read again); dskip = the PLANAR skip half
-    // of the concat gradient
-    int pool_bwd(const void* code, const void* dskip, const void* dP, void* dZ, int C, int lvl_out) const
+    // conv1_1's weight gradient: software-im2col tile straight from the fp32 NCHW frame (first_conv.cuh)
+    int first_conv_wgrad(const float* x, float* grads) const
     {
-        const double pxo = (double)u->n * (u->H >> lvl_out) * (u->W >> lvl_out);
+        const Layer& l = u->L[I_C11];
+        const double px = (double)u->n * u->H * u->W;
+        Scope sc(u, st, "conv1_1", "wgrad", 2.0 * px * 32 * 9 * u->cin0, px * (4 * u->cin0 + 64));
+        return launch_first_conv_wgrad(ctx(), x, u->cin0, u->dz[I_C11], l.cout, grads + l.w_off, grads + l.b_off, u->n, u->H,
+                                       u->W, st);
+    }
+    // pooled layer li's pool backward, from the argmax + sign code the forward tile left (the activation is not read
+    // again): dp and the PLANAR skip half of the concat gradient -> li's dz
+    int pool_bwd(int li) const
+    {
+        const Layer& l = u->L[li];
+        const int lvl = l.lvl + 1, C = l.cout;
+        const double pxo = (double)u->n * (u->H >> lvl) * (u->W >> lvl);
         Scope sc(u, st, "pool", "bwd", 0.0, pxo * C * (2 * 9 + 1));
-        return launch_maxpool_bwd_code(ctx(), code, dskip, C, 0, dP, dZ, C, u->n, u->H >> lvl_out, u->W >> lvl_out, st);
+        return launch_maxpool_bwd_code(ctx(), s->code[lvl], skip_half(u->dcat[l.lvl], l.lvl, C), C, 0, u->dp[lvl], u->dz[li],
+                                       C, u->n, u->H >> lvl, u->W >> lvl, st);
     }
     // second (skip) half of a planar concat gradient: [n][h][w][C] right behind the up half
     __nv_bfloat16* skip_half(__nv_bfloat16* dcat, int lvl, int C) const
     {
         return dcat + (size_t)u->n * (u->H >> lvl) * (u->W >> lvl) * C;
+    }
+    // the data gradient towards the output of layer li's producer
+    int data_grad(int li) const
+    {
+        const Layer& l = u->L[li];
+        if (l.type == L_DECONV) return deconv_dgrad(li);
+        TRY(conv_dgrad(li));
+        return l.skip < 0 && pooled(l.src) ? pool_bwd(l.src) : ELD_OK;
     }
 
     // gradients of bucket k are complete in the staging area: move its conv tiles to the PyTorch layout and mark the
@@ -714,100 +768,32 @@ struct Runner {
 
     int forward(const float* x) const
     {
-        eld_unet* U = u;
-        const FwdState* S = s;
         TRY(pack());
         {
             // conv1_1 (4 -> 32): software-im2col tile straight from the fp32 NCHW frame (first_conv.cuh)
-            const double px = (double)U->n * U->H * U->W;
-            Scope sc(u, st, "conv1_1", "fprop", 2.0 * px * 32 * 9 * U->cin0, px * (4 * U->cin0 + 64));
-            TRY(launch_first_conv(ctx(), x, U->cin0, wf(I_C11), bias(I_C11), S->a1_1, 32, U->n, U->H, U->W, st, sign_of(S->a1_1)));
+            const double px = (double)u->n * u->H * u->W;
+            Scope sc(u, st, "conv1_1", "fprop", 2.0 * px * 32 * 9 * u->cin0, px * (4 * u->cin0 + 64));
+            TRY(launch_first_conv(ctx(), x, u->cin0, wf(I_C11), bias(I_C11), s->act[I_C11], u->L[I_C11].cout, u->n, u->H, u->W,
+                                  st, s->sign[I_C11]));
         }
-        TRY(conv(I_C12, S->a1_1, 32, 0, S->cat9, 64, 32, 0, S->p1, S->pc1));       // + pool (Unet.py:51)
-        TRY(conv(I_C21, S->p1, 32, 0, S->a2_1, 64, 0, 1));
-        TRY(conv(I_C22, S->a2_1, 64, 0, S->cat8, 128, 64, 1, S->p2, S->pc2));      // + pool (Unet.py:55)
-        TRY(conv(I_C31, S->p2, 64, 0, S->a3_1, 128, 0, 2));
-        TRY(conv(I_C32, S->a3_1, 128, 0, S->cat7, 256, 128, 2, S->p3, S->pc3));    // + pool (Unet.py:59)
-        TRY(conv(I_C41, S->p3, 128, 0, S->a4_1, 256, 0, 3));
-        TRY(conv(I_C42, S->a4_1, 256, 0, S->cat6, 512, 256, 3, S->p4, S->pc4));    // + pool (Unet.py:63)
-        TRY(conv(I_C51, S->p4, 256, 0, S->a5_1, 512, 0, 4));
-        TRY(conv(I_C52, S->a5_1, 512, 0, S->a5_2, 512, 0, 4));
-        TRY(deconv(I_UP6, S->a5_2, 512, S->cat6, 512, 4));
-        TRY(conv(I_C61, S->cat6, 512, 0, S->a6_1, 256, 0, 3)); TRY(conv(I_C62, S->a6_1, 256, 0, S->a6_2, 256, 0, 3));
-        TRY(deconv(I_UP7, S->a6_2, 256, S->cat7, 256, 3));
-        TRY(conv(I_C71, S->cat7, 256, 0, S->a7_1, 128, 0, 2)); TRY(conv(I_C72, S->a7_1, 128, 0, S->a7_2, 128, 0, 2));
-        TRY(deconv(I_UP8, S->a7_2, 128, S->cat8, 128, 2));
-        TRY(conv(I_C81, S->cat8, 128, 0, S->a8_1, 64, 0, 1));  TRY(conv(I_C82, S->a8_1, 64, 0, S->a8_2, 64, 0, 1));
-        TRY(deconv(I_UP9, S->a8_2, 64, S->cat9, 64, 1));
-        TRY(conv(I_C91, S->cat9, 64, 0, S->a9_1, 32, 0, 0));   TRY(conv(I_C92, S->a9_1, 32, 0, S->a9_2, 32, 0, 0));
+        for (int li = I_C11 + 1; li < I_C10; ++li) TRY(u->L[li].type == L_DECONV ? deconv(li) : conv(li));
         return ELD_OK;
     }
 
-    // The fixed backward sequence; every launch runs only when the plan (derive_needs) asks for what it produces:
-    // W(l) = layer l's weight gradient, D(s) = the data gradient towards the output of layer s (the gradient of an
-    // input produced by s).  With every parameter trainable all of them run, in this order.
+    // The layers in reverse state_dict order, each with: its weight gradient if it trains; the finish of the gradient
+    // bucket it is the first layer of; the data gradient towards its producer if that one is reached (derive_needs).
+    // With every parameter trainable all of them run.
     int backward(const float* x, float* g) const
     {
-        eld_unet* U = u;
-        const FwdState* S = s;
-        auto W = [U](int l) { return U->wgrad[l]; };
-        auto D = [U](int src) { return U->reach[src]; };
-        if (W(I_C92)) TRY(conv_wgrad(I_C92, S->a9_1, 32, 0, U->dz9_2, g, 0));
-        if (D(I_C91)) TRY(conv_dgrad(I_C92, U->dz9_2, U->dz9_1, 32, 0, S->a9_1, 0));
-        if (W(I_C91)) TRY(conv_wgrad(I_C91, S->cat9, 64, 0, U->dz9_1, g, 0));
-        if (D(I_UP9)) TRY(concat_dgrad(I_C91, U->dz9_1, U->dcat9, 0));
-        if (W(I_UP9)) TRY(deconv_wgrad(I_UP9, S->a8_2, U->dcat9, 32, g, 1));
-        if (D(I_C82)) TRY(deconv_dgrad(I_UP9, U->dcat9, 32, U->dz8_2, S->a8_2, 1));
-        if (W(I_C82)) TRY(conv_wgrad(I_C82, S->a8_1, 64, 0, U->dz8_2, g, 1));
-        if (D(I_C81)) TRY(conv_dgrad(I_C82, U->dz8_2, U->dz8_1, 64, 0, S->a8_1, 1));
-        if (W(I_C81)) TRY(conv_wgrad(I_C81, S->cat8, 128, 0, U->dz8_1, g, 1));
-        if (D(I_UP8)) TRY(concat_dgrad(I_C81, U->dz8_1, U->dcat8, 1));
-        if (W(I_UP8)) TRY(deconv_wgrad(I_UP8, S->a7_2, U->dcat8, 64, g, 2));
-        if (D(I_C72)) TRY(deconv_dgrad(I_UP8, U->dcat8, 64, U->dz7_2, S->a7_2, 2));
-        if (W(I_C72)) TRY(conv_wgrad(I_C72, S->a7_1, 128, 0, U->dz7_2, g, 2));
-        if (D(I_C71)) TRY(conv_dgrad(I_C72, U->dz7_2, U->dz7_1, 128, 0, S->a7_1, 2));
-        if (W(I_C71)) TRY(conv_wgrad(I_C71, S->cat7, 256, 0, U->dz7_1, g, 2));
-        if (D(I_UP7)) TRY(concat_dgrad(I_C71, U->dz7_1, U->dcat7, 2));
-        if (W(I_UP7)) TRY(deconv_wgrad(I_UP7, S->a6_2, U->dcat7, 128, g, 3));
-        if (D(I_C62)) TRY(deconv_dgrad(I_UP7, U->dcat7, 128, U->dz6_2, S->a6_2, 3));
-        if (W(I_C62)) TRY(conv_wgrad(I_C62, S->a6_1, 256, 0, U->dz6_2, g, 3));
-        if (D(I_C61)) TRY(conv_dgrad(I_C62, U->dz6_2, U->dz6_1, 256, 0, S->a6_1, 3));
-        if (W(I_C61)) TRY(conv_wgrad(I_C61, S->cat6, 512, 0, U->dz6_1, g, 3));
-        if (D(I_UP6)) TRY(concat_dgrad(I_C61, U->dz6_1, U->dcat6, 3));
-        if (W(I_UP6)) TRY(deconv_wgrad(I_UP6, S->a5_2, U->dcat6, 256, g, 4));
-        TRY(finish_bucket(0, g));
-        if (D(I_C52)) TRY(deconv_dgrad(I_UP6, U->dcat6, 256, U->dz5_2, S->a5_2, 4));
-        // bottleneck + encoder
-        if (W(I_C52)) TRY(conv_wgrad(I_C52, S->a5_1, 512, 0, U->dz5_2, g, 4));
-        if (D(I_C51)) TRY(conv_dgrad(I_C52, U->dz5_2, U->dz5_1, 512, 0, S->a5_1, 4));
-        if (W(I_C51)) TRY(conv_wgrad(I_C51, S->p4, 256, 0, U->dz5_1, g, 4));
-        TRY(finish_bucket(1, g));
-        if (D(I_C42)) TRY(conv_dgrad(I_C51, U->dz5_1, U->dp4, 256, 0, nullptr, 4));
-        if (D(I_C42)) TRY(pool_bwd(S->pc4, skip_half(U->dcat6, 3, 256), U->dp4, U->dz4_2, 256, 4));
-        if (W(I_C42)) TRY(conv_wgrad(I_C42, S->a4_1, 256, 0, U->dz4_2, g, 3));
-        if (D(I_C41)) TRY(conv_dgrad(I_C42, U->dz4_2, U->dz4_1, 256, 0, S->a4_1, 3));
-        if (W(I_C41)) TRY(conv_wgrad(I_C41, S->p3, 128, 0, U->dz4_1, g, 3));
-        if (D(I_C32)) TRY(conv_dgrad(I_C41, U->dz4_1, U->dp3, 128, 0, nullptr, 3));
-        if (D(I_C32)) TRY(pool_bwd(S->pc3, skip_half(U->dcat7, 2, 128), U->dp3, U->dz3_2, 128, 3));
-        if (W(I_C32)) TRY(conv_wgrad(I_C32, S->a3_1, 128, 0, U->dz3_2, g, 2));
-        if (D(I_C31)) TRY(conv_dgrad(I_C32, U->dz3_2, U->dz3_1, 128, 0, S->a3_1, 2));
-        if (W(I_C31)) TRY(conv_wgrad(I_C31, S->p2, 64, 0, U->dz3_1, g, 2));
-        if (D(I_C22)) TRY(conv_dgrad(I_C31, U->dz3_1, U->dp2, 64, 0, nullptr, 2));
-        if (D(I_C22)) TRY(pool_bwd(S->pc2, skip_half(U->dcat8, 1, 64), U->dp2, U->dz2_2, 64, 2));
-        if (W(I_C22)) TRY(conv_wgrad(I_C22, S->a2_1, 64, 0, U->dz2_2, g, 1));
-        if (D(I_C21)) TRY(conv_dgrad(I_C22, U->dz2_2, U->dz2_1, 64, 0, S->a2_1, 1));
-        if (W(I_C21)) TRY(conv_wgrad(I_C21, S->p1, 32, 0, U->dz2_1, g, 1));
-        TRY(finish_bucket(2, g));
-        if (D(I_C12)) TRY(conv_dgrad(I_C21, U->dz2_1, U->dp1, 32, 0, nullptr, 1));
-        if (D(I_C12)) TRY(pool_bwd(S->pc1, skip_half(U->dcat9, 0, 32), U->dp1, U->dz1_2, 32, 1));
-        if (W(I_C12)) TRY(conv_wgrad(I_C12, S->a1_1, 32, 0, U->dz1_2, g, 0));
-        if (D(I_C11)) TRY(conv_dgrad(I_C12, U->dz1_2, U->dz1_1, 32, 0, S->a1_1, 0));
-        if (W(I_C11)) {
-            const double px = (double)U->n * U->H * U->W;
-            Scope sc(u, st, "conv1_1", "wgrad", 2.0 * px * 32 * 9 * U->cin0, px * (4 * U->cin0 + 64));
-            TRY(launch_first_conv_wgrad(ctx(), x, U->cin0, U->dz1_1, 32, g + U->L[I_C11].w_off, g + U->L[I_C11].b_off, U->n, U->H, U->W, st));
+        int k = 0;                   // the next gradient bucket to finish
+        for (int li = I_C10 - 1; li >= I_C11; --li) {
+            const Layer& l = u->L[li];
+            if (u->wgrad[li])
+                TRY(li == I_C11 ? first_conv_wgrad(x, g) : l.type == L_DECONV ? deconv_wgrad(li, g) : conv_wgrad(li, g));
+            if (li == kBucketFirst[k]) TRY(finish_bucket(k++, g));
+            if (l.src >= 0 && u->reach[l.src]) TRY(data_grad(li));
         }
-        return finish_bucket(3, g);
+        return ELD_OK;
     }
 };
 
@@ -831,7 +817,7 @@ extern "C" int eld_unet_forward(eld_unet* u, const float* params, const float* x
 extern "C" int eld_unet_forward_state(eld_unet* u, void* state, const float* params, const float* x, float* out, void* stream)
 {
     ELD_REQUIRE(u && params && x && out, "eld_unet_forward: NULL argument");
-    ELD_REQUIRE(!state || u->dz9_2 != nullptr, "eld_unet_forward_state: a caller state needs an eld_unet created with train = 1");
+    ELD_REQUIRE(!state || u->train, "eld_unet_forward_state: a caller state needs an eld_unet created with train = 1");
     u->dz1_1_final = false;
     ELD_CHECK_CUDA(cudaSetDevice(u->ctx->device));
     FwdState tmp;
@@ -839,7 +825,7 @@ extern "C" int eld_unet_forward_state(eld_unet* u, void* state, const float* par
     TRY(r.forward(x));
     const double hpx = (double)u->n * u->H * u->W;
     Scope sc(u, r.st, "conv10_1", "fprop", 2.0 * hpx * 128, hpx * (64 + 16));
-    return launch_head(u->ctx, r.s->a9_2, params + u->L[I_C10].w_off, params + u->L[I_C10].b_off, out, nullptr, nullptr,
+    return launch_head(u->ctx, r.s->act[I_C92], params + u->L[I_C10].w_off, params + u->L[I_C10].b_off, out, nullptr, nullptr,
                        nullptr, nullptr, nullptr, u->n, (size_t)u->H * u->W, u->cout_last, 0, r.st);
 }
 
@@ -847,7 +833,7 @@ extern "C" int eld_unet_train_step(eld_unet* u, const float* params, const float
                                    float* out, float* grads, float* loss, void* stream)
 {
     ELD_REQUIRE(u && params && x && target && out && grads && loss, "eld_unet_train_step: NULL argument");
-    ELD_REQUIRE(u->dz9_2 != nullptr, "eld_unet_train_step: the eld_unet was created with train = 0");
+    ELD_REQUIRE(u->train, "eld_unet_train_step: the eld_unet was created with train = 0");
     u->dz1_1_final = false;
     ELD_CHECK_CUDA(cudaSetDevice(u->ctx->device));
     Runner r{ u, &u->fs, params, static_cast<cudaStream_t>(stream) };
@@ -861,9 +847,9 @@ extern "C" int eld_unet_train_step(eld_unet* u, const float* params, const float
         const double hpx = (double)u->n * u->H * u->W;
         Scope sc(u, r.st, "conv10_1", dz || dw ? "fwd+loss+bwd" : "fwd+loss", (dz || dw ? 6.0 : 2.0) * hpx * 128,
                  hpx * (64 + 16 + 16 + (dz ? 64 : 0)));
-        TRY(launch_head(u->ctx, u->fs.a9_2, params + u->L[I_C10].w_off, params + u->L[I_C10].b_off, out, target, dz ? u->dz9_2 : nullptr,
-                        dw ? grads + u->L[I_C10].w_off : nullptr, dw ? grads + u->L[I_C10].b_off : nullptr, loss, u->n,
-                        (size_t)u->H * u->W, u->cout_last, u->l2_loss, r.st));
+        TRY(launch_head(u->ctx, u->fs.act[I_C92], params + u->L[I_C10].w_off, params + u->L[I_C10].b_off, out, target,
+                        dz ? u->dz[I_C92] : nullptr, dw ? grads + u->L[I_C10].w_off : nullptr,
+                        dw ? grads + u->L[I_C10].b_off : nullptr, loss, u->n, (size_t)u->H * u->W, u->cout_last, u->l2_loss, r.st));
     }
     TRY(r.backward(x, grads));
     u->dz1_1_final = u->reach[I_C11];
@@ -879,7 +865,7 @@ extern "C" int eld_unet_backward_state(eld_unet* u, void* state, const float* pa
                                        float* grads, void* stream)
 {
     ELD_REQUIRE(u && params && x && dout && grads, "eld_unet_backward: NULL argument");
-    ELD_REQUIRE(u->dz9_2 != nullptr, "eld_unet_backward: the eld_unet was created with train = 0");
+    ELD_REQUIRE(u->train, "eld_unet_backward: the eld_unet was created with train = 0");
     ELD_CHECK_CUDA(cudaSetDevice(u->ctx->device));
     FwdState tmp;
     Runner r{ u, state_at(u, state, tmp), params, static_cast<cudaStream_t>(stream) };
@@ -890,8 +876,8 @@ extern "C" int eld_unet_backward_state(eld_unet* u, void* state, const float* pa
         const double hpx = (double)u->n * u->H * u->W;
         Scope sc(u, r.st, "conv10_1", "bwd", 4.0 * hpx * 128, hpx * (64 + 16 + (dz ? 64 : 0)));
         // the head re-forms `out` into scratch (dz1_1 is not written before the very end of backward) and back-propagates dout
-        TRY(launch_head(u->ctx, r.s->a9_2, params + u->L[I_C10].w_off, params + u->L[I_C10].b_off,
-                        reinterpret_cast<float*>(u->dz1_1), dout, dz ? u->dz9_2 : nullptr,
+        TRY(launch_head(u->ctx, r.s->act[I_C92], params + u->L[I_C10].w_off, params + u->L[I_C10].b_off,
+                        reinterpret_cast<float*>(u->dz[I_C11]), dout, dz ? u->dz[I_C92] : nullptr,
                         dw ? grads + u->L[I_C10].w_off : nullptr, dw ? grads + u->L[I_C10].b_off : nullptr, nullptr, u->n,
                         (size_t)u->H * u->W, u->cout_last, 2, r.st));
     }
@@ -912,73 +898,56 @@ extern "C" int eld_unet_set_trainable(eld_unet* u, const uint8_t* flags, int n_f
 extern "C" int eld_unet_input_grad(eld_unet* u, const float* params, float* dx, void* stream)
 {
     ELD_REQUIRE(u && params && dx, "eld_unet_input_grad: NULL argument");
-    ELD_REQUIRE(u->dz9_2 != nullptr, "eld_unet_input_grad: the eld_unet was created with train = 0");
+    ELD_REQUIRE(u->train, "eld_unet_input_grad: the eld_unet was created with train = 0");
     ELD_REQUIRE(u->dz1_1_final, "eld_unet_input_grad: no eld_unet_backward or eld_unet_train_step since the last forward");
     ELD_CHECK_CUDA(cudaSetDevice(u->ctx->device));
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     const double px = (double)u->n * u->H * u->W;
     Scope sc(u, st, "conv1_1", "dgrad", 2.0 * px * 32 * 9 * u->cin0, px * (64 + 4 * u->cin0));
-    return launch_first_conv_dgrad(u->ctx, u->dz1_1, params + u->L[I_C11].w_off, u->cin0, dx, u->n, u->H, u->W, st);
+    return launch_first_conv_dgrad(u->ctx, u->dz[I_C11], params + u->L[I_C11].w_off, u->cin0, dx, u->n, u->H, u->W, st);
 }
 
-// The intermediate tensors of the step by name: member, level (1/2^lvl of the frame), units per pixel.  Activations
-// belong to the built-in forward state; the gradients are backward scratch (training only).
-// A gradient of a concat input (dcat*) is the whole planar buffer: [n][h][w][C/2] up plane, then the skip plane.
-static const struct { const char* name; __nv_bfloat16* FwdState::*p; int lvl, ch; } kStateBuffers[] = {
-    { "a1_1", &FwdState::a1_1, 0, 32 },  { "cat9", &FwdState::cat9, 0, 64 },   { "p1", &FwdState::p1, 1, 32 },
-    { "a2_1", &FwdState::a2_1, 1, 64 },  { "cat8", &FwdState::cat8, 1, 128 },  { "p2", &FwdState::p2, 2, 64 },
-    { "a3_1", &FwdState::a3_1, 2, 128 }, { "cat7", &FwdState::cat7, 2, 256 },  { "p3", &FwdState::p3, 3, 128 },
-    { "a4_1", &FwdState::a4_1, 3, 256 }, { "cat6", &FwdState::cat6, 3, 512 },  { "p4", &FwdState::p4, 4, 256 },
-    { "a5_1", &FwdState::a5_1, 4, 512 }, { "a5_2", &FwdState::a5_2, 4, 512 },
-    { "a6_1", &FwdState::a6_1, 3, 256 }, { "a6_2", &FwdState::a6_2, 3, 256 },
-    { "a7_1", &FwdState::a7_1, 2, 128 }, { "a7_2", &FwdState::a7_2, 2, 128 },
-    { "a8_1", &FwdState::a8_1, 1, 64 },  { "a8_2", &FwdState::a8_2, 1, 64 },
-    { "a9_1", &FwdState::a9_1, 0, 32 },  { "a9_2", &FwdState::a9_2, 0, 32 },
-};
-static const struct { const char* name; __nv_bfloat16* eld_unet::*p; int lvl, ch; } kScratchBuffers[] = {
-    { "dz9_2", &eld_unet::dz9_2, 0, 32 },  { "dz9_1", &eld_unet::dz9_1, 0, 32 },  { "dcat9", &eld_unet::dcat9, 0, 64 },
-    { "dz8_2", &eld_unet::dz8_2, 1, 64 },  { "dz8_1", &eld_unet::dz8_1, 1, 64 },  { "dcat8", &eld_unet::dcat8, 1, 128 },
-    { "dz7_2", &eld_unet::dz7_2, 2, 128 }, { "dz7_1", &eld_unet::dz7_1, 2, 128 }, { "dcat7", &eld_unet::dcat7, 2, 256 },
-    { "dz6_2", &eld_unet::dz6_2, 3, 256 }, { "dz6_1", &eld_unet::dz6_1, 3, 256 }, { "dcat6", &eld_unet::dcat6, 3, 512 },
-    { "dz5_2", &eld_unet::dz5_2, 4, 512 }, { "dz5_1", &eld_unet::dz5_1, 4, 512 }, { "dp4", &eld_unet::dp4, 4, 256 },
-    { "dz4_2", &eld_unet::dz4_2, 3, 256 }, { "dz4_1", &eld_unet::dz4_1, 3, 256 }, { "dp3", &eld_unet::dp3, 3, 128 },
-    { "dz3_2", &eld_unet::dz3_2, 2, 128 }, { "dz3_1", &eld_unet::dz3_1, 2, 128 }, { "dp2", &eld_unet::dp2, 2, 64 },
-    { "dz2_2", &eld_unet::dz2_2, 1, 64 },  { "dz2_1", &eld_unet::dz2_1, 1, 64 },  { "dp1", &eld_unet::dp1, 1, 32 },
-    { "dz1_2", &eld_unet::dz1_2, 0, 32 },  { "dz1_1", &eld_unet::dz1_1, 0, 32 },
-};
-
-/* Host-side view of the workspace for tests and debugging: where tensor `name` of the last step lives.  No launch. */
+/* Host-side view of the workspace for tests and debugging: where tensor `name` of the last step lives.  No launch.
+   The names come from the layer table: aX_Y / dzX_Y / sign:aX_Y for convX_Y's own output, its gradient and its sign words;
+   catN / dcatN for the concat buffer upvN writes into and its gradient; pN / pcN / dpN for the pooled tensor at level N,
+   its pool codes and its gradient.  Activations belong to the built-in forward state; the gradients are backward scratch. */
 extern "C" int eld_unet_buffer(const eld_unet* u, const char* name, void** ptr, int dims[4], int* elem_bytes)
 {
     ELD_REQUIRE(u && name && ptr && dims && elem_bytes, "eld_unet_buffer: NULL argument");
-    const bool train = u->dz9_2 != nullptr;
     const FwdState& fs = u->fs;
     auto put = [&](const void* p, int n, int h, int w, int units, int eb) {
         *ptr = const_cast<void*>(p); dims[0] = n; dims[1] = h; dims[2] = w; dims[3] = units; *elem_bytes = eb;
         return ELD_OK;
     };
-    for (const auto& b : kStateBuffers)
-        if (strcmp(name, b.name) == 0) return put(fs.*b.p, u->n, u->H >> b.lvl, u->W >> b.lvl, b.ch, 2);
-    for (const auto& b : kScratchBuffers) {
-        if (strcmp(name, b.name) != 0) continue;
-        ELD_REQUIRE(train, "eld_unet_buffer: '%s' exists only in a training workspace", name);
-        return put(u->*b.p, u->n, u->H >> b.lvl, u->W >> b.lvl, b.ch, 2);
-    }
-    // pool codes: one byte per pooled element (32 bytes per pooled pixel and 32 channels)
-    static const struct { const char* name; __nv_bfloat16* FwdState::*p; int lvl, ch; } kCodes[] = {
-        { "pc1", &FwdState::pc1, 1, 32 }, { "pc2", &FwdState::pc2, 2, 64 }, { "pc3", &FwdState::pc3, 3, 128 }, { "pc4", &FwdState::pc4, 4, 256 },
+    auto at = [&](const void* p, int lvl, int units, int eb) { return put(p, u->n, u->H >> lvl, u->W >> lvl, units, eb); };
+    auto train_only = [&](const void* p, int lvl, int units, int eb) {
+        ELD_REQUIRE(u->train, "eld_unet_buffer: '%s' exists only in a training workspace", name);
+        return at(p, lvl, units, eb);
     };
-    for (const auto& c : kCodes) {
-        if (strcmp(name, c.name) != 0) continue;
-        ELD_REQUIRE(train, "eld_unet_buffer: '%s' exists only in a training workspace", name);
-        return put(fs.*c.p, u->n, u->H >> c.lvl, u->W >> c.lvl, c.ch, 1);
-    }
-    if (strncmp(name, "sign:", 5) == 0) {            // sign words of an activation: uint32 [pixel][channels / 32]
-        for (const auto& b : kStateBuffers) {
-            if (strcmp(name + 5, b.name) != 0) continue;
-            for (int i = 0; i < fs.n_signs; ++i)
-                if (fs.signs[i].act == fs.*b.p) return put(fs.signs[i].words, u->n, u->H >> b.lvl, u->W >> b.lvl, b.ch / 32, 4);
+    auto is = [name](const char* prefix, const char* id) {     // name == prefix followed by id
+        const size_t k = strlen(prefix);
+        return strncmp(name, prefix, k) == 0 && strcmp(name + k, id) == 0;
+    };
+    for (int i = 0; i < kNumLayers; ++i) {
+        const Layer& l = u->L[i];
+        if (l.type == L_CONV1) continue;
+        if (l.type == L_DECONV) {
+            if (is("cat", l.name + 3)) return at(fs.cat[l.lvl], l.lvl, 2 * l.cout, 2);
+            if (is("dcat", l.name + 3)) return train_only(u->dcat[l.lvl], l.lvl, 2 * l.cout, 2);
+            continue;
         }
+        if (is("dz", l.name + 4)) return train_only(u->dz[i], l.lvl, l.cout, 2);
+        if (pooled(i)) {
+            const char pool_lvl[2] = { char('1' + l.lvl), 0 };
+            if (is("p", pool_lvl)) return at(fs.pool[l.lvl + 1], l.lvl + 1, l.cout, 2);
+            if (is("pc", pool_lvl)) return train_only(fs.code[l.lvl + 1], l.lvl + 1, l.cout, 1);
+            if (is("dp", pool_lvl)) return train_only(u->dp[l.lvl + 1], l.lvl + 1, l.cout, 2);
+        } else {
+            if (is("a", l.name + 4)) return at(fs.act[i], l.lvl, l.cout, 2);
+            if (is("sign:a", l.name + 4) && fs.sign[i]) return at(fs.sign[i], l.lvl, l.cout / 32, 4);
+        }
+    }
+    if (strncmp(name, "sign:", 5) == 0) {
         set_error("eld_unet_buffer: no sign words '%s' in this workspace", name);
         return ELD_E_ARG;
     }
@@ -995,7 +964,7 @@ extern "C" int eld_unet_buffer(const eld_unet* u, const char* name, void** ptr, 
         return ELD_E_ARG;
     }
     if (strcmp(name, "gtmp") == 0) {                 // [tap][ci][co] staging of the conv3x3 weight gradients, parameter offsets
-        ELD_REQUIRE(train, "eld_unet_buffer: 'gtmp' exists only in a training workspace");
+        ELD_REQUIRE(u->train, "eld_unet_buffer: 'gtmp' exists only in a training workspace");
         return put(u->gtmp, 1, 1, 1, (int)u->n_params, 4);
     }
     set_error("eld_unet_buffer: unknown tensor '%s'", name);
