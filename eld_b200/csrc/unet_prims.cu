@@ -4,6 +4,7 @@
 #include <cstdlib>
 #include <cstdio>
 #include "conv_umma.cuh"
+#include "conv3x3_thin.cuh"
 #include "wgrad_umma.cuh"
 #include "first_conv.cuh"
 #include "unet_prims.h"
@@ -98,9 +99,44 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
         ELD_REQUIRE(op.cout > 0 && (op.cout & (op.cout - 1)) == 0, "deconv tile: cout=%d must be a power of two", op.cout);
         while ((1 << p.cout_shift) < op.cout) ++p.cout_shift;
     }
+    p.b_ptr = static_cast<const uint8_t*>(op.b);
 
+    // the thin 3x3 layers (one channel chunk, one N block) run the halo tile with resident weights (conv3x3_thin.cuh)
+    const bool thin = op.a_mode == A_CONV && op.taps == 9 && (op.cin == 32 || op.cin == 64) &&
+                      (op.n_total == 32 || op.n_total == 64);
     CUtensorMap tmA;
     const cuuint64_t eb = 2;  // bf16
+    if (thin) {
+        cuuint64_t dims[5] = { (cuuint64_t)op.a_pitch, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.n_img, 1 };
+        cuuint64_t str[4] = { op.a_pitch * eb, (cuuint64_t)op.W * op.a_pitch * eb,
+                              (cuuint64_t)op.H * op.W * op.a_pitch * eb,
+                              (cuuint64_t)op.n_img * op.H * op.W * op.a_pitch * eb };
+        cuuint32_t box[5] = { (cuuint32_t)p.kc, 16, kThinBoxRows, 1, 1 };
+        int rc = encode(ctx, &tmA, op.a, 5, dims, str, box, p.kc * 2);
+        if (rc) return rc;
+        // [resident weights][halo slots][staging of both consumer warpgroups][bias][barriers] after the 1024-byte alignment
+        const int slot_bytes = 3 * kThinBoxRows * 16 * rb;
+        const int fixed = 9 * p.n_tile * rb + 2 * kThinStgBytes + 256;
+        int slots = (kThinSmemBytes - 1024 - fixed - 256) / slot_bytes;
+        if (slots > kThinMaxSlots) slots = kThinMaxSlots;
+        ELD_REQUIRE(slots >= 2, "thin conv tile: no room for two halo slots");
+        p.stages = slots;
+        p.stg_smem_off = 9 * p.n_tile * rb + slots * slot_bytes;
+        p.bias_smem_off = p.stg_smem_off + 2 * kThinStgBytes;
+        p.bar_smem_off = p.bias_smem_off + 256;
+        const size_t smem = 1024 + (size_t)p.bar_smem_off + 256;
+        const int total_tiles = op.n_img * p.tiles_x * p.tiles_y;
+        const int grid = total_tiles < ctx->num_sms ? total_tiles : ctx->num_sms;
+        cudaError_t e;
+        if (p.n_tile == 64) e = p.kc == 64 ? launch_pdl(conv3x3_thin_kernel<64, 64>, grid, kConvThreads, smem, st, tmA, p)
+                                           : launch_pdl(conv3x3_thin_kernel<64, 32>, grid, kConvThreads, smem, st, tmA, p);
+        else e = p.kc == 64 ? launch_pdl(conv3x3_thin_kernel<32, 64>, grid, kConvThreads, smem, st, tmA, p)
+                            : launch_pdl(conv3x3_thin_kernel<32, 32>, grid, kConvThreads, smem, st, tmA, p);
+        ELD_CHECK_CUDA(e);
+        ELD_CHECK_CUDA(cudaGetLastError());
+        count_launch(ctx);
+        return ELD_OK;
+    }
     if (op.a_mode == A_CONV) {
         cuuint64_t dims[5] = { (cuuint64_t)op.a_pitch, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.n_img, 1 };
         cuuint64_t str[4] = { op.a_pitch * eb, (cuuint64_t)op.W * op.a_pitch * eb,
@@ -118,7 +154,6 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
         int rc = encode(ctx, &tmA, op.a, 5, dims, str, box, p.kc * 2);
         if (rc) return rc;
     }
-    p.b_ptr = static_cast<const uint8_t*>(op.b);
     const size_t smem = 1024 /*align slack*/ + (size_t)p.bar_smem_off + 256 /*barriers*/;
     const int total_tiles = op.n_img * p.tiles_x * p.tiles_y * (p.n_total / p.n_tile);
     const int grid = total_tiles < ctx->num_sms ? total_tiles : ctx->num_sms;
@@ -230,6 +265,10 @@ int init_gemm_kernels(eld_ctx* ctx)
     ELD_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_thin_kernel<32, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_thin_kernel<32, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_thin_kernel<64, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_thin_kernel<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
