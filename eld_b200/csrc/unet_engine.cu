@@ -70,7 +70,8 @@ constexpr int kGradBuckets = 4;
 constexpr int kBucketFirst[kGradBuckets] = { I_UP6, I_C51, I_C21, I_C11 };
 static int bucket_end(int k) { return k == 0 ? kNumLayers : kBucketFirst[k - 1]; }
 
-struct PackEntry { unsigned long long src, dst_f, dst_d; int cout, cin, type; int pad; };
+// perm: the layer's weight trains, so the gradient permute moves its tiles (derive_needs)
+struct PackEntry { unsigned long long src, dst_f, dst_d; int cout, cin, type; int perm; };
 struct PackTable {
     PackEntry e[kNumLayers];
     int tile0[kNumLayers + 1];   // prefix sum of (cout/32 x cin/32) tiles per entry: one block per tile, whatever the layer
@@ -206,7 +207,7 @@ wgrad_permute_kernel(const float* __restrict__ gtmp, float* __restrict__ grads, 
     if (gtile >= tile_end) return;
     int t;
     const PackEntry& e = T.e[find_entry(T, gtile, t)];
-    if (e.type != L_CONV3) return;
+    if (e.type != L_CONV3 || !e.perm) return;     // a frozen weight's range of grads keeps the zeros of the step's memset
     const int ct = e.cout / 32;
     {
         const int co0 = (t % ct) * 32, ci0 = (t / ct) * 32;
@@ -276,11 +277,11 @@ struct eld_unet {
     int cin0 = 4, cout_last = 4; // channels of the frame in / out: 4 = packed raw, 3 = sRGB (ELD_model.py:377-389)
     int l2_loss = 0;             // 0: nn.L1Loss (the reference default, losses.py:31-32), 1: nn.MSELoss (losses.py:33-34)
     bool dz1_1_final = false;    // dz1_1 holds the last backward's conv1_1 gradient: set by a backward, cleared by a forward
-    // what the backward computes (eld_unet_set_trainable; default: everything).  wgrad[l]: layer l's weight or bias
-    // requires grad.  reach[l]: the gradient of layer l's output is needed - l trains, or something upstream of it does
-    // (or the frame, when input_grad).  perm_t0 / perm_t1: tile span of the gradient permute per bucket ([kGradBuckets]
-    // = the whole table), over the layers that train.
-    bool wgrad[kNumLayers], reach[kNumLayers];
+    // what the backward computes (eld_unet_set_trainable; default: everything).  train_w[l] / train_b[l]: layer l's
+    // weight / bias requires grad; wgrad[l]: either does (one launch computes both).  reach[l]: the gradient of layer l's
+    // output is needed - l trains, or something upstream of it does (or the frame, when input_grad).  perm_t0 / perm_t1:
+    // tile span of the gradient permute per bucket ([kGradBuckets] = the whole table), over the layers that train.
+    bool train_w[kNumLayers], train_b[kNumLayers], wgrad[kNumLayers], reach[kNumLayers];
     bool input_grad = true;
     int perm_t0[kGradBuckets + 1], perm_t1[kGradBuckets + 1];
     // optional per-launch profile (CUDA events on the launch stream)
@@ -425,11 +426,14 @@ static void derive_needs(eld_unet* u, const uint8_t* flags, bool input_grad)
     u->input_grad = input_grad;
     for (int i = 0; i < kNumLayers; ++i) {
         const Layer& l = u->L[i];
-        u->wgrad[i] = flags[2 * i] || flags[2 * i + 1];
+        u->train_w[i] = flags[2 * i] != 0;
+        u->train_b[i] = flags[2 * i + 1] != 0;
+        u->wgrad[i] = u->train_w[i] || u->train_b[i];
         const bool in = l.src < 0 ? input_grad : u->reach[l.src];
         u->reach[i] = u->wgrad[i] || in || (l.skip >= 0 && u->reach[l.skip]);
     }
     // the table holds conv1_2 .. conv9_2 in state_dict order: entry e is layer e + 1
+    for (int e = 0; e < u->table.n; ++e) u->table.e[e].perm = u->train_w[e + 1];
     for (int k = 0; k <= kGradBuckets; ++k) {
         const int l0 = k < kGradBuckets ? kBucketFirst[k] : 0, l1 = k < kGradBuckets ? bucket_end(k) : kNumLayers;
         int a = u->table.n, b = 0;
@@ -473,7 +477,7 @@ extern "C" int eld_unet_create_io(eld_ctx* ctx, int n, int h, int w, int train, 
         const Layer& l = u->L[i];
         if (i == I_C11 || l.type == L_CONV1) continue;
         u->table.tile0[k] = k == 0 ? 0 : u->table.tile0[k - 1] + (u->table.e[k - 1].cout / 32) * (u->table.e[k - 1].cin / 32);
-        u->table.e[k++] = PackEntry{ l.w_off, l.wf_off, l.wd_off, l.cout, l.cin, l.type, 0 };
+        u->table.e[k++] = PackEntry{ l.w_off, l.wf_off, l.wd_off, l.cout, l.cin, l.type, 1 };
     }
     u->table.tile0[k] = u->table.tile0[k - 1] + (u->table.e[k - 1].cout / 32) * (u->table.e[k - 1].cin / 32);
     u->table.n = k;
@@ -571,6 +575,12 @@ struct Runner {
     const __nv_bfloat16* wf(int i) const { return s->packed + u->L[i].wf_off; }
     const __nv_bfloat16* wd(int i) const { return s->packed + u->L[i].wd_off; }
     const float* bias(int i) const { return params + u->L[i].b_off; }
+    // where a weight-gradient launch puts layer li's dW / db: the layer's range of grads when that tensor trains, else the
+    // same range of gtmp, which nothing reads.  One launch computes both, so a layer with one frozen tensor still
+    // computes it, and the frozen range of grads keeps the zeros of the step's memset.  (A conv3x3's dW is staged in gtmp
+    // either way; the permute skips a frozen one.)
+    float* dw_to(int li, float* grads) const { return (u->train_w[li] ? grads : u->gtmp) + u->L[li].w_off; }
+    float* db_to(int li, float* grads) const { return (u->train_b[li] ? grads : u->gtmp) + u->L[li].b_off; }
 
     // a tensor as a launch addresses it: base, channel pitch, first channel
     struct View { __nv_bfloat16* p; int pitch, c0; };
@@ -680,7 +690,7 @@ struct Runner {
         op.q = u->dz[li]; op.q_pitch = l.cout; op.q_c0 = 0; op.q_ch = l.cout;
         op.n_img = u->n; op.H = u->H >> l.lvl; op.W = u->W >> l.lvl;
         op.dw = u->gtmp + l.w_off; op.out_tco = 1;
-        op.db = grads + l.b_off;                     // bias gradient fused into the same launch
+        op.db = db_to(li, grads);                    // bias gradient fused into the same launch
         const double px = (double)u->n * op.H * op.W;
         Scope sc(u, st, l.name, "wgrad", 2.0 * px * l.cout * 9 * l.cin, px * 2 * (l.cin + l.cout) + 36.0 * l.cin * l.cout);
         return launch_wgrad(ctx(), op, st);
@@ -691,8 +701,8 @@ struct Runner {
         WgradOp op{};
         op.mode = WG_DECONV; op.p = u->dcat[l.lvl]; op.p_pitch = l.cout; op.p_c0 = 0; op.p_ch = l.cout;
         op.q = in_of(li).p; op.q_pitch = l.cin; op.q_c0 = 0; op.q_ch = l.cin;
-        op.n_img = u->n; op.H = u->H >> (l.lvl + 1); op.W = u->W >> (l.lvl + 1); op.dw = grads + l.w_off;
-        op.db = grads + l.b_off;                     // bias gradient = column sums of the d(up) boxes, same launch
+        op.n_img = u->n; op.H = u->H >> (l.lvl + 1); op.W = u->W >> (l.lvl + 1); op.dw = dw_to(li, grads);
+        op.db = db_to(li, grads);                    // bias gradient = column sums of the d(up) boxes, same launch
         const double px = (double)u->n * op.H * op.W;
         Scope sc(u, st, l.name, "wgrad", 2.0 * px * 4 * l.cout * l.cin, px * 2 * (l.cin + 4 * l.cout) + 16.0 * l.cin * l.cout);
         return launch_wgrad(ctx(), op, st);
@@ -703,8 +713,8 @@ struct Runner {
         const Layer& l = u->L[I_C11];
         const double px = (double)u->n * u->H * u->W;
         Scope sc(u, st, "conv1_1", "wgrad", 2.0 * px * 32 * 9 * u->cin0, px * (4 * u->cin0 + 64));
-        return launch_first_conv_wgrad(ctx(), x, u->cin0, u->dz[I_C11], l.cout, grads + l.w_off, grads + l.b_off, u->n, u->H,
-                                       u->W, st);
+        return launch_first_conv_wgrad(ctx(), x, u->cin0, u->dz[I_C11], l.cout, dw_to(I_C11, grads), db_to(I_C11, grads), u->n,
+                                       u->H, u->W, st);
     }
     // pooled layer li's pool backward, from the argmax + sign code the forward tile left (the activation is not read
     // again): dp and the PLANAR skip half of the concat gradient -> li's dz
@@ -741,8 +751,9 @@ struct Runner {
         // the compute stream, then an event marks the bucket final.  (Running this permute on the caller's communication
         // stream instead would let it overlap the tiles - any foreign kernel that overlaps the persistent
         // one-CTA-per-SM tiles delays some of their CTAs, and a tile kernel is as slow as its slowest CTA.)
-        // Only the span of layers that train is moved (a frozen layer's range of grads keeps the zeros of the memset); a
-        // bucket with nothing to move still records its event, so a waiter never sees one from an earlier step.
+        // Only the span of layers that train is moved, and inside it only the layers whose weight trains (a frozen
+        // weight's range of grads keeps the zeros of the memset); a bucket with nothing to move still records its event,
+        // so a waiter never sees one from an earlier step.
         const bool per_bucket = u->bucket_ev[0] != nullptr;
         if (!per_bucket && k != kGradBuckets - 1) return ELD_OK;
         const int t0 = u->perm_t0[per_bucket ? k : kGradBuckets];
@@ -848,8 +859,8 @@ extern "C" int eld_unet_train_step(eld_unet* u, const float* params, const float
         Scope sc(u, r.st, "conv10_1", dz || dw ? "fwd+loss+bwd" : "fwd+loss", (dz || dw ? 6.0 : 2.0) * hpx * 128,
                  hpx * (64 + 16 + 16 + (dz ? 64 : 0)));
         TRY(launch_head(u->ctx, u->fs.act[I_C92], params + u->L[I_C10].w_off, params + u->L[I_C10].b_off, out, target,
-                        dz ? u->dz[I_C92] : nullptr, dw ? grads + u->L[I_C10].w_off : nullptr,
-                        dw ? grads + u->L[I_C10].b_off : nullptr, loss, u->n, (size_t)u->H * u->W, u->cout_last, u->l2_loss, r.st));
+                        dz ? u->dz[I_C92] : nullptr, dw ? r.dw_to(I_C10, grads) : nullptr,
+                        dw ? r.db_to(I_C10, grads) : nullptr, loss, u->n, (size_t)u->H * u->W, u->cout_last, u->l2_loss, r.st));
     }
     TRY(r.backward(x, grads));
     u->dz1_1_final = u->reach[I_C11];
@@ -878,7 +889,7 @@ extern "C" int eld_unet_backward_state(eld_unet* u, void* state, const float* pa
         // the head re-forms `out` into scratch (dz1_1 is not written before the very end of backward) and back-propagates dout
         TRY(launch_head(u->ctx, r.s->act[I_C92], params + u->L[I_C10].w_off, params + u->L[I_C10].b_off,
                         reinterpret_cast<float*>(u->dz[I_C11]), dout, dz ? u->dz[I_C92] : nullptr,
-                        dw ? grads + u->L[I_C10].w_off : nullptr, dw ? grads + u->L[I_C10].b_off : nullptr, nullptr, u->n,
+                        dw ? r.dw_to(I_C10, grads) : nullptr, dw ? r.db_to(I_C10, grads) : nullptr, nullptr, u->n,
                         (size_t)u->H * u->W, u->cout_last, 2, r.st));
     }
     TRY(r.backward(x, grads));

@@ -73,15 +73,24 @@ def _dz(layer):
     return 'dz' + layer[4:]
 
 
+def _level(cat):
+    """the grid level of a concat buffer: cat9 -> 0 (full resolution) .. cat6 -> 3"""
+    return 9 - int(cat[-1])
+
+
 class Step:
-    """One finished step (or forward) of engine `eng` and the checks of its launches."""
+    """One finished step (or forward) of engine `eng` and the checks of its launches.
+    skip_elided: the concat levels whose data gradient is a row-prefix launch (the up half only; the caller filled the
+    skip plane with NAN_BITS), split stores elsewhere.  frozen: the parameter names that do not train - a weight-gradient
+    launch still computes them (one launch per layer), but their range of grads must read zero."""
 
     def __init__(self, torch, net, eng, ws, x, out, grads=None, target=None, loss=None, kind='l1', dout=None, dx=None,
-                 skip_elided=False, tag=''):
+                 skip_elided=frozenset(), frozen=frozenset(), tag=''):
         from eld_b200 import _lib
         self.t, self.net, self.lib, self.eng, self.ws = torch, net, _lib.load(), eng, ws
         self.x, self.out, self.grads, self.target, self.loss, self.kind = x, out, grads, target, loss, kind
-        self.dout, self.dx, self.skip_elided, self.tag = dout, dx, skip_elided, tag
+        self.dout, self.dx, self.skip_elided, self.frozen, self.tag = dout, dx, set(skip_elided), set(frozen), tag
+        self.dz9_2 = True       # the head wrote dz9_2 (something below conv10_1 needs it); set from the launch list
         self.params = dict(net.named_parameters())
         self.span = {k: sp for k, sp in zip(self.params, net._spans)}
         self.fail = []
@@ -138,6 +147,14 @@ class Step:
             rel_max, abs_max = (PRODUCTION_WGRAD, PRODUCTION_WGRAD) if self.tag else (WGRAD_REL_L2, MAX_ABS)
         if not (rel <= rel_max and mx <= abs_max):
             self.fail.append('%s (%s): rel-L2 %.3g, max-abs / max|r| %.3g' % (where, kind, rel, mx))
+
+    def grad(self, kind, pname, r, S):
+        """a parameter's range of grads: the fp32 rule when it trains, all zero bits when it is frozen"""
+        got = self.G(pname)
+        if pname in self.frozen:
+            self.exact('frozen range', pname, got.view(self.t.int32), self.t.zeros_like(got).view(self.t.int32))
+        else:
+            self.f32(kind, pname, got, r, S)
 
     def exact(self, kind, where, got, want):
         STATS['exact ' + kind]['elements'] += got.numel()
@@ -212,7 +229,7 @@ class Step:
             up, skip = self.planes('d' + src)
             r, S = R.conv_dgrad(dz, self.W(layer))
             half = up.shape[-1]
-            if self.skip_elided:      # the row-prefix launch: the up half only, the skip plane keeps its sentinel
+            if _level(src) in self.skip_elided:   # the row-prefix launch: the up half only, the skip plane keeps its sentinel
                 self.bf16('conv.dgrad.prefix', layer, up, r[..., :half], S[..., :half])
                 self.exact('sentinel', 'd%s skip plane' % src, self.bits(skip), self.t.full_like(self.bits(skip), NAN_BITS))
             else:
@@ -239,18 +256,18 @@ class Step:
         if layer.startswith('upv'):
             up, _ = self.planes('dcat' + layer[3:])
             dW, S, db, Sb = R.deconv_wgrad(self.V(src), up)
-            self.f32('deconv.wgrad', layer, self.G(layer + '.weight'), dW, S)
-            self.f32('deconv.bias_grad', layer, self.G(layer + '.bias'), db, Sb)
+            self.grad('deconv.wgrad', layer + '.weight', dW, S)
+            self.grad('deconv.bias_grad', layer + '.bias', db, Sb)
             return
         cout, cin = self.W(layer).shape[:2]
         dW, S, db, Sb = R.conv_wgrad(self.V(src)[..., sc0:sc0 + cin], self.V(_dz(layer)))
         off = self.span[layer + '.weight'][0]
         staged = self.V('gtmp').reshape(-1)[off:off + dW.numel()].view(3, 3, cin, cout).permute(3, 2, 0, 1)
-        self.f32('conv.wgrad', layer + ' (gtmp)', staged, dW, S)
-        self.f32('conv.bias_grad', layer, self.G(layer + '.bias'), db, Sb)
+        self.f32('conv.wgrad', layer + ' (gtmp)', staged, dW, S)    # staged whether or not the weight trains
+        self.grad('conv.bias_grad', layer + '.bias', db, Sb)
 
     def gperm(self, trained):
-        """grads (OIHW) of every trained conv3x3 layer == its [tap][ci][co] staging, permuted; a frozen layer's range zero"""
+        """grads (OIHW) of every trained conv3x3 weight == its [tap][ci][co] staging, permuted; a frozen one's range zero"""
         gtmp = self.V('gtmp').reshape(-1)
         for layer in FWD:
             if layer.startswith('upv'):
@@ -264,8 +281,8 @@ class Step:
     def first_wgrad(self):
         import tests.launch_ref as R
         dW, S, db, Sb = R.first_conv_wgrad(self.x, self.V('dz1_1'))
-        self.f32('conv1_1.wgrad', 'conv1_1', self.G('conv1_1.weight'), dW, S)
-        self.f32('conv1_1.bias_grad', 'conv1_1', self.G('conv1_1.bias'), db, Sb)
+        self.grad('conv1_1.wgrad', 'conv1_1.weight', dW, S)
+        self.grad('conv1_1.bias_grad', 'conv1_1.bias', db, Sb)
 
     def first_dgrad(self):
         import tests.launch_ref as R
@@ -287,15 +304,18 @@ class Step:
             return
         dout = self.dout if what == 'bwd' else R.head_dout(self.out, self.target, self.kind)
         dz, S, dW, Sw, db, Sb = R.head_bwd(a, w, dout)
-        self.bf16('head.dz9_2' + ('.seam' if what == 'bwd' else '.' + self.kind), 'dz9_2', self.V('dz9_2'), dz, S)
-        self.f32('head.dW10', 'conv10_1 dW', self.G('conv10_1.weight'), dW, Sw)
-        self.f32('head.db10', 'conv10_1 db', self.G('conv10_1.bias'), db, Sb)
+        if self.dz9_2:
+            self.bf16('head.dz9_2' + ('.seam' if what == 'bwd' else '.' + self.kind), 'dz9_2', self.V('dz9_2'), dz, S)
+        self.grad('head.dW10', 'conv10_1.weight', dW, Sw)
+        self.grad('head.db10', 'conv10_1.bias', db, Sb)
 
     def check(self, names):
         """every launch in `names` (the engine's profile, in issue order)"""
         self.names = names
         pools = 0
-        trained = {n.split('.')[0] for n in names if n.endswith('.wgrad')}
+        trained = {n.split('.')[0] for n in names if n.endswith('.wgrad')} - {p.split('.')[0] for p in self.frozen
+                                                                               if p.endswith('.weight')}
+        self.dz9_2 = 'conv9_2.wgrad' in names or 'conv9_2.dgrad' in names
         for name in names:
             layer, what = name.split('.', 1)
             if name == 'weights.pack':
@@ -344,7 +364,8 @@ def _train(torch, n, cin, cout, h, w, loss='l1', frozen=()):
     x, t = _frames(torch, n, cin, h, w, 1), _frames(torch, n, cout, h, w, 2)
     eng = net._engine(n, h, w, True)
     ws = _ws(net, n, h, w, True)
-    st = Step(torch, net, eng, ws, x, None, net.flat_grads, t, None, loss, skip_elided=bool(frozen),
+    st = Step(torch, net, eng, ws, x, None, net.flat_grads, t, None, loss, skip_elided={0, 1, 2, 3} if frozen else (),
+              frozen={k for k, p in net.named_parameters() if not p.requires_grad},
               tag=' @8x512^2' if n * h * w >= 8 * 512 * 512 else '')
     if frozen:
         for d in ('dcat6', 'dcat7', 'dcat8', 'dcat9'):
