@@ -6,6 +6,7 @@
 #include "conv_umma.cuh"
 #include "conv3x3_thin.cuh"
 #include "wgrad_umma.cuh"
+#include "wgrad_thin.cuh"
 #include "first_conv.cuh"
 #include "unet_prims.h"
 
@@ -272,6 +273,61 @@ int init_gemm_kernels(eld_ctx* ctx)
     ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wgrad_thin_kernel<32, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wgrad_thin_kernel<32, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wgrad_thin_kernel<64, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wgrad_thin_kernel<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    return ELD_OK;
+}
+
+// the thin 3x3 weight gradients (cin, cout in {32, 64}): one halo load per pixel tile for all nine taps (wgrad_thin.cuh)
+static int launch_wgrad_thin(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
+{
+    // the [tap][ci][co] flush and the bias gradient add four contiguous floats at a time
+    ELD_REQUIRE(op.out_tco == 0 || (reinterpret_cast<uintptr_t>(op.dw) & 15) == 0,
+                "thin wgrad tile: the [tap][ci][co] gradient must be 16-byte aligned");
+    ELD_REQUIRE(op.db == nullptr || (reinterpret_cast<uintptr_t>(op.db) & 15) == 0,
+                "thin wgrad tile: the bias gradient must be 16-byte aligned");
+    WgradThinParams p{};
+    p.n_img = op.n_img; p.H = op.H; p.W = op.W;
+    p.tiles_x = op.W / 16; p.tiles_y = (op.H + 7) / 8;       // H % 8 == 4: the last tile row overhangs, zero-filled
+    p.p_c0 = op.p_c0; p.q_c0 = op.q_c0; p.p_ch = op.p_ch; p.q_ch = op.q_ch;
+    p.dw = op.dw; p.out_tco = op.out_tco; p.db = op.db;
+    const int slot_bytes = wgrad_thin_slot_bytes(op.p_ch, op.q_ch);
+    int stages = (kThinSmemBytes - 1024 - 256) / slot_bytes;
+    if (stages > kThinMaxSlots) stages = kThinMaxSlots;
+    ELD_REQUIRE(stages >= 2, "thin wgrad tile: no room for two stages");
+    p.stages = stages;
+
+    CUtensorMap tmP, tmQ;
+    const cuuint64_t eb = 2;
+    {
+        cuuint64_t dims[5] = { (cuuint64_t)op.p_pitch, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.n_img, 1 };
+        cuuint64_t str[4] = { op.p_pitch * eb, (cuuint64_t)op.W * op.p_pitch * eb, (cuuint64_t)op.H * op.W * op.p_pitch * eb,
+                              (cuuint64_t)op.n_img * op.H * op.W * op.p_pitch * eb };
+        cuuint32_t box[5] = { (cuuint32_t)op.p_ch, 16, kThinBoxRows, 1, 1 };
+        int rc = encode(ctx, &tmP, op.p, 5, dims, str, box, op.p_ch * 2);
+        if (rc) return rc;
+    }
+    {
+        cuuint64_t dims[5] = { (cuuint64_t)op.q_pitch, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.n_img, 1 };
+        cuuint64_t str[4] = { op.q_pitch * eb, (cuuint64_t)op.W * op.q_pitch * eb, (cuuint64_t)op.H * op.W * op.q_pitch * eb,
+                              (cuuint64_t)op.n_img * op.H * op.W * op.q_pitch * eb };
+        cuuint32_t box[5] = { (cuuint32_t)op.q_ch, 16, 8, 1, 1 };
+        int rc = encode(ctx, &tmQ, op.q, 5, dims, str, box, op.q_ch * 2);
+        if (rc) return rc;
+    }
+    const size_t smem = 1024 + (size_t)stages * slot_bytes + 256;
+    const int total_tiles = op.n_img * p.tiles_x * p.tiles_y;
+    const int grid = total_tiles < ctx->num_sms ? total_tiles : ctx->num_sms;
+    cudaError_t e;
+    if (op.q_ch == 64) e = op.p_ch == 64 ? launch_pdl(conv3x3_wgrad_thin_kernel<64, 64>, grid, kWgThinThreads, smem, st, tmP, tmQ, p)
+                                         : launch_pdl(conv3x3_wgrad_thin_kernel<64, 32>, grid, kWgThinThreads, smem, st, tmP, tmQ, p);
+    else e = op.p_ch == 64 ? launch_pdl(conv3x3_wgrad_thin_kernel<32, 64>, grid, kWgThinThreads, smem, st, tmP, tmQ, p)
+                           : launch_pdl(conv3x3_wgrad_thin_kernel<32, 32>, grid, kWgThinThreads, smem, st, tmP, tmQ, p);
+    ELD_CHECK_CUDA(e);
+    ELD_CHECK_CUDA(cudaGetLastError());
+    count_launch(ctx);
     return ELD_OK;
 }
 
@@ -280,6 +336,8 @@ int launch_wgrad(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
     ELD_REQUIRE(op.H % 4 == 0 && op.W % 16 == 0, "wgrad tile: H=%d must be a multiple of 4 and W=%d of 16", op.H, op.W);
     ELD_REQUIRE(op.p_ch % 32 == 0 && op.q_ch % 32 == 0, "wgrad tile: channel counts must be multiples of 32");
     ELD_REQUIRE(op.out_tco == 0 || op.mode == WG_CONV, "wgrad tile: the [tap][ci][co] layout is a conv layout");
+    if (op.mode == WG_CONV && (op.p_ch == 32 || op.p_ch == 64) && (op.q_ch == 32 || op.q_ch == 64))
+        return launch_wgrad_thin(ctx, op, st);
     WgradParams p{};
     p.n_img = op.n_img; p.H = op.H; p.W = op.W;
     p.chunks_x = op.W / 16; p.chunks_y = op.H / 4;

@@ -1,0 +1,247 @@
+// wgrad_thin.cuh - wgmma weight-gradient tile for the thin 3x3 convolutions (cin and cout in {32, 64}): the
+// full- and half-resolution layers, where the generic tile (wgrad_umma.cuh) loads every pixel of X once per filter tap.
+//
+//   D[(tap, ci) x co] (f32, registers)  =  sum over pixels p   X[p + tap shift, ci] * dZ[p, co]
+//
+// Grid    = one persistent CTA per SM; CTA b owns tiles [b T / G, (b + 1) T / G) of the T 8 x 16 pixel tiles (a
+//           contiguous run, so vertically neighbouring halos meet in L2) and the layer's whole dW (+ db) for them.
+// P (X)   = per tile three TMA boxes {KC, 16, 10} at columns x0 - 1, x0, x0 + 1 and rows y0 - 1 .. y0 + 8 (zero-filled
+//           outside the image = the padding), the fprop thin tile's geometry.  Consumed MN-major: tap (dy, dx) is box
+//           dx + 1 from pixel row 16 (dy + 1) on, a whole number of swizzle atoms (1 KB at SW64, 2 KB at SW128), and k16
+//           step k is tile row k.  KC = 64: one tap = one m64 unit (9 units).  KC = 32: two taps share one m64 unit, the
+//           second 32 rows at the descriptor's LBO: (dy = -1, dx) + (0, dx) at LBO = 1 KB for each dx, (1, -1) + (1, 0)
+//           and (1, 0) + (1, 1) at LBO = one box (5 units; the first half of the last duplicates a tap and is dropped).
+// Q (dZ)  = one {NT, 16, 8} box per tile, MN-major.  Its column sums are the bias gradient, summed from shared memory
+//           while the MMAs run.
+// roles   = warpgroup 0: TMA producer (one thread) | warpgroups 1, 2 consume every stage and split the m64 units
+//           (5 / 4 at KC = 64, 3 / 2 at KC = 32).  There is no per-tile epilogue: at the end each consumer adds its f32
+//           units into the gradient with vector red.global.add.  The 160 accumulator registers of (64 -> 64) need more
+//           than the 168 a 384-thread CTA gets evenly: setmaxnreg moves registers from the producer to the consumers.
+#pragma once
+#include "umma.cuh"
+#include "unet_prims.h"
+#include "conv3x3_thin.cuh"
+#include <cuda_bf16.h>
+
+namespace eld {
+
+struct WgradThinParams {
+    int n_img, H, W;
+    int tiles_x, tiles_y;
+    int p_c0, q_c0;
+    int p_ch, q_ch;           // cin, cout (= KC, NT)
+    int stages;
+    float* dw;                // out_tco: [tap][ci][co]; otherwise OIHW [co][ci][3][3]
+    int out_tco;
+    float* db;                // optional: db[co] += sum over pixels of dZ
+};
+
+constexpr int kWgThinThreads = 384;
+constexpr int kWgThinProducerRegs = 40;
+constexpr int kWgThinConsumerRegs = 232;      // 128 x 40 + 256 x 232 <= 64 K registers
+
+// bytes of one pipeline slot: three halo boxes of X and the dZ box
+__host__ __device__ constexpr int wgrad_thin_box_bytes(int kc) { return kThinBoxRows * 16 * kc * 2; }
+__host__ __device__ constexpr int wgrad_thin_slot_bytes(int kc, int nt) { return 3 * wgrad_thin_box_bytes(kc) + 128 * nt * 2; }
+__host__ __device__ constexpr int wgrad_thin_units(int kc) { return kc == 64 ? 9 : 5; }
+
+// m64 unit u: byte offset of its first half inside a slot, and the LBO to its second 32 rows (KC = 32)
+template <int KC>
+__device__ __forceinline__ constexpr uint32_t wg_unit_off(int u)
+{
+    constexpr int box = wgrad_thin_box_bytes(KC), row = KC * 2;
+    if (KC == 64) return (uint32_t)((u % 3) * box + (u / 3) * 16 * row);
+    return (uint32_t)(u < 3 ? u * box : (u - 3) * box + 32 * row);
+}
+template <int KC>
+__device__ __forceinline__ constexpr uint32_t wg_unit_lbo(int u)
+{
+    return KC == 64 ? 0u : (u < 3 ? 16u * KC * 2 : (uint32_t)wgrad_thin_box_bytes(KC));
+}
+// filter tap (kh * 3 + kw) of row m of unit u, and its input channel; -1 = a duplicated half, dropped
+template <int KC>
+__device__ __forceinline__ int wg_unit_tap(int u, int m)
+{
+    if (KC == 64) return u;
+    const int half = m >> 5;
+    return u < 3 ? 3 * half + u : (u == 3 ? 6 + half : (half ? 8 : -1));
+}
+
+// One consumer warpgroup: units U0 .. U0 + NU - 1 of every stage, accumulated over the CTA's tiles, then flushed.
+template <int NT, int KC, int U0, int NU>
+__device__ __forceinline__ void wgrad_thin_consume(const WgradThinParams& p, uint8_t* smem, uint64_t* full, uint64_t* empty,
+                                                   int ntiles, int bt)
+{
+    constexpr int box_bytes = wgrad_thin_box_bytes(KC), slot_bytes = wgrad_thin_slot_bytes(KC, NT);
+    constexpr int p_row = KC * 2, q_row = NT * 2;
+    constexpr uint32_t a_step = (16u * p_row) >> 4, b_step = (16u * q_row) >> 4;   // one k16 step = one tile row
+    const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+    const uint32_t smem_base = ptx::smem_u32(smem);
+    uint64_t a_desc0[NU];
+#pragma unroll
+    for (int u = 0; u < NU; ++u)
+        a_desc0[u] = ptx::make_gmma_desc(0, wg_unit_lbo<KC>(U0 + u), 8u * p_row, ptx::gmma_layout(p_row));
+    const uint64_t b_desc0 = ptx::make_gmma_desc(0, 0, 8u * q_row, ptx::gmma_layout(q_row));
+
+    // bias gradient: consumer thread bt sums 16-byte chunk bc (8 columns) of the dZ rows br, br + BR, ...
+    constexpr int CH = NT / 8, BR = 256 / CH;
+    const int bc = bt % CH, br = bt / CH;
+    const uint32_t bswz = NT == 64 ? (uint32_t)(br & 7) : (uint32_t)((br >> 1) & 3);   // BR is a multiple of 8
+    const bool bias_on = p.db != nullptr;
+    float bsum[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) bsum[i] = 0.f;
+
+    float acc[NU][NT / 2];
+#pragma unroll
+    for (int u = 0; u < NU; ++u)
+#pragma unroll
+        for (int i = 0; i < NT / 2; ++i) acc[u][i] = 0.f;
+
+    int s = 0, prev = -1;
+    uint32_t ph = 0;
+    for (int i = 0; i < ntiles; ++i) {
+        ptx::mbar_wait(&full[s], ph);
+        const uint32_t st = smem_base + (uint32_t)(s * slot_bytes);
+        const uint64_t bd = b_desc0 | (uint64_t)(((st + (uint32_t)(3 * box_bytes)) & 0x3FFFFu) >> 4);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+#pragma unroll
+            for (int u = 0; u < NU; ++u) {
+                const uint64_t ad = a_desc0[u] | (uint64_t)(((st + wg_unit_off<KC>(U0 + u)) & 0x3FFFFu) >> 4);
+                ptx::wgmma_bf16<NT, 1, 1>(acc[u], ad + (uint64_t)(k * a_step), bd + (uint64_t)(k * b_step), 1u);
+            }
+        ptx::wgmma_commit();
+        if (bias_on) {
+            const uint8_t* q = smem + (size_t)s * slot_bytes + 3 * box_bytes;
+#pragma unroll
+            for (int r = 0; r < 128 / BR; ++r) {
+                const int row = br + r * BR;
+                const uint4 v = *reinterpret_cast<const uint4*>(q + row * q_row + (((uint32_t)bc ^ bswz) << 4));
+                const uint32_t w[4] = { v.x, v.y, v.z, v.w };
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    bsum[2 * j] += __uint_as_float(w[j] << 16);
+                    bsum[2 * j + 1] += __uint_as_float(w[j] & 0xFFFF0000u);
+                }
+            }
+        }
+        ptx::wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty[prev]);
+        prev = s;
+        if (++s == p.stages) { s = 0; ph ^= 1u; }
+    }
+    ptx::wgmma_wait<0>();
+#pragma unroll
+    for (int u = 0; u < NU; ++u) ptx::reg_fence(acc[u]);
+
+    if (bias_on) {
+        // lanes with the same chunk: lane % CH; fold them onto lanes 0 .. CH - 1, one pair of float4 reds each
+#pragma unroll
+        for (int o = CH; o < 32; o <<= 1)
+#pragma unroll
+            for (int i = 0; i < 8; ++i) bsum[i] += __shfl_xor_sync(0xffffffffu, bsum[i], o);
+        if (lane < CH) {
+            float4* d = reinterpret_cast<float4*>(p.db + 8 * bc);
+            atomicAdd(d, make_float4(bsum[0], bsum[1], bsum[2], bsum[3]));
+            atomicAdd(d + 1, make_float4(bsum[4], bsum[5], bsum[6], bsum[7]));
+        }
+    }
+
+    // ===================== flush: registers -> red.add into dW =====================
+    // fragment: lane holds D[16 wq + lane / 4 + 8 i][8 j + 2 (lane % 4) + c] in acc[u][4 j + 2 i + c].  For the
+    // [tap][ci][co] layout, lanes l and l ^ 1 swap a pair so that each holds four contiguous co of one row: the even
+    // lane row i = 0, the odd lane row i = 1.
+    const bool odd = lane & 1;
+#pragma unroll
+    for (int u = 0; u < NU; ++u) {
+#pragma unroll
+        for (int j = 0; j < NT / 8; ++j) {
+            const float v00 = acc[u][4 * j], v01 = acc[u][4 * j + 1], v10 = acc[u][4 * j + 2], v11 = acc[u][4 * j + 3];
+            if (p.out_tco) {
+                const float s0 = __shfl_xor_sync(0xffffffffu, odd ? v00 : v10, 1);
+                const float s1 = __shfl_xor_sync(0xffffffffu, odd ? v01 : v11, 1);
+                const int m = 16 * wq + (lane >> 2) + (odd ? 8 : 0);
+                const int tap = wg_unit_tap<KC>(U0 + u, m);
+                if (tap < 0) continue;
+                const int ci = m & (KC - 1), co = 8 * j + 2 * ((lane & 3) & ~1);
+                const float4 v = odd ? make_float4(s0, s1, v10, v11) : make_float4(v00, v01, s0, s1);
+                atomicAdd(reinterpret_cast<float4*>(p.dw + ((size_t)tap * KC + ci) * NT + co), v);
+            } else {
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int m = 16 * wq + (lane >> 2) + 8 * i;
+                    const int tap = wg_unit_tap<KC>(U0 + u, m);
+                    if (tap < 0) continue;
+                    const int ci = m & (KC - 1), co = 8 * j + 2 * (lane & 3);
+                    atomicAdd(p.dw + ((size_t)co * KC + ci) * 9 + tap, i ? v10 : v00);
+                    atomicAdd(p.dw + ((size_t)(co + 1) * KC + ci) * 9 + tap, i ? v11 : v01);
+                }
+            }
+        }
+    }
+}
+
+// NT = cout, KC = cin, each 32 or 64
+template <int NT, int KC>
+__global__ void __launch_bounds__(kWgThinThreads, 1)
+conv3x3_wgrad_thin_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmQ,
+                          const WgradThinParams p)
+{
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t raw = ptx::smem_u32(smem_raw);
+    uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
+
+    constexpr int box_bytes = wgrad_thin_box_bytes(KC), slot_bytes = wgrad_thin_slot_bytes(KC, NT);
+    constexpr int units = wgrad_thin_units(KC), u_first = (units + 1) / 2;
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * slot_bytes);
+    uint64_t* empty = full + p.stages;
+
+    const int tiles_xy = p.tiles_x * p.tiles_y;
+    const int total_tiles = p.n_img * tiles_xy;
+    const int t_begin = (int)((long long)blockIdx.x * total_tiles / gridDim.x);
+    const int t_end = (int)((long long)(blockIdx.x + 1) * total_tiles / gridDim.x);
+
+    if (threadIdx.x == 0) {
+        ptx::prefetch_tmap(&tmP);
+        ptx::prefetch_tmap(&tmQ);
+        for (int s = 0; s < p.stages; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 8); }
+        ptx::fence_barrier_init();
+    }
+    __syncthreads();
+    ptx::grid_dep_wait();       // PDL: X and dZ belong to the previous kernels
+    ptx::grid_dep_launch();
+
+    if (threadIdx.x < 128) {
+        // ===================== TMA producer (warpgroup 0; one thread works) =====================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kWgThinProducerRegs));
+        if (threadIdx.x == 0) {
+            int img = t_begin / tiles_xy;
+            const int rem = t_begin - img * tiles_xy;
+            int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
+            int s = 0;
+            uint32_t ph = 0;
+            for (int tile = t_begin; tile < t_end; ++tile) {
+                const int x0 = tx * 16, y0 = ty * 8;
+                uint8_t* sa = smem + (size_t)s * slot_bytes;
+                ptx::mbar_wait(&empty[s], ph ^ 1u);
+                ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)slot_bytes);
+                for (int b = 0; b < 3; ++b) ptx::tma_load_5d(sa + b * box_bytes, &tmP, &full[s], p.p_c0, x0 + b - 1, y0 - 1, img, 0);
+                ptx::tma_load_5d(sa + 3 * box_bytes, &tmQ, &full[s], p.q_c0, x0, y0, img, 0);
+                if (++s == p.stages) { s = 0; ph ^= 1u; }
+                if (++tx == p.tiles_x) { tx = 0; if (++ty == p.tiles_y) { ty = 0; ++img; } }
+            }
+        }
+        return;
+    }
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kWgThinConsumerRegs));
+
+    // broadcast from lane 0: the compiler then knows cg to be warp-uniform (no wgmma serialisation)
+    const int cg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7) - 1, 0);
+    const int bt = threadIdx.x - 128;
+    if (cg == 0) wgrad_thin_consume<NT, KC, 0, u_first>(p, smem, full, empty, t_end - t_begin, bt);
+    else wgrad_thin_consume<NT, KC, u_first, units - u_first>(p, smem, full, empty, t_end - t_begin, bt);
+}
+
+}  // namespace eld
