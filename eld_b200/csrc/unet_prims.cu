@@ -79,6 +79,9 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
     ELD_REQUIRE(op.b_block_rows == 0 || (op.b_block_rows % 32 == 0 && op.b_block_rows <= 256 &&
                                          (op.n_total <= op.b_block_rows || op.b_block_rows == 256) && op.aux_sign == nullptr),
                 "conv tile: a row prefix of the packed operand needs whole 32-row groups of its blocks and no sign-word mask");
+    // a whole operand of more than 256 rows is whole 256-row blocks (packed_index gives every block a full 256-row slot)
+    ELD_REQUIRE(op.b_block_rows != 0 || op.n_total <= 256 || op.n_total % 256 == 0,
+                "conv tile: GEMM N=%d above 256 must be a multiple of 256", op.n_total);
     p.b_rows = op.b_block_rows ? op.b_block_rows : (op.n_total <= 256 ? op.n_total : 256);
     // N per tile: 32, 64 or 128 (a 64 x 256 f32 accumulator would take 128 registers per consumer thread and spill
     // next to the epilogue)
@@ -97,7 +100,8 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
     p.bar_smem_off = p.bias_smem_off + 4096;
     p.cout_shift = 0;
     if (op.epi_mode == EPI_SHUFFLE) {
-        ELD_REQUIRE(op.cout > 0 && (op.cout & (op.cout - 1)) == 0, "deconv tile: cout=%d must be a power of two", op.cout);
+        // the epilogue stores 32 GEMM columns of one sub-pixel at a time: cout must fill whole groups of 32
+        ELD_REQUIRE(op.cout >= 32 && (op.cout & (op.cout - 1)) == 0, "deconv tile: cout=%d must be a power of two >= 32", op.cout);
         while ((1 << p.cout_shift) < op.cout) ++p.cout_shift;
     }
     p.b_ptr = static_cast<const uint8_t*>(op.b);
@@ -449,10 +453,22 @@ int launch_pack_weights(eld_ctx* ctx, const float* w, void* out, int cout, int c
 
 using namespace eld;
 
+// the channels [c0, c0 + c) a primitive reads or writes lie inside each pixel's `pitch` channels
+static bool in_pitch(int pitch, int c0, int c) { return c > 0 && c0 >= 0 && c0 + c <= pitch; }
+
 extern "C" int eld_pack_weights(eld_ctx* ctx, const float* w, void* packed, int cout, int cin, int kind, void* stream)
 {
     ELD_REQUIRE(ctx && w && packed, "eld_pack_weights: NULL argument");
     ELD_REQUIRE(kind >= 0 && kind <= 3 && cout > 0 && cin > 0, "eld_pack_weights: bad kind/shape");
+    // the operand is whole [n_tile][kc] blocks (packed_index): K channels in chunks of 32 or 64, and above 256 rows whole
+    // 256-row blocks - a partial last block would still span the address range of 256 rows, past the operand's end
+    const int rows = kind == PACK_CONV_FPROP ? cout : kind == PACK_DECONV_FPROP ? 4 * cout : cin;
+    const int ck = (kind == PACK_CONV_FPROP || kind == PACK_DECONV_FPROP) ? cin : cout;
+    ELD_REQUIRE(ck % 32 == 0 && rows % 32 == 0, "eld_pack_weights: cout=%d, cin=%d (kind %d) must be multiples of 32",
+                cout, cin, kind);
+    ELD_REQUIRE(rows <= 256 || rows % 256 == 0,
+                "eld_pack_weights: cout=%d, cin=%d (kind %d) gives %d operand rows; above 256 they must be a multiple of 256",
+                cout, cin, kind, rows);
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     return launch_pack_weights(ctx, w, packed, cout, cin, kind, static_cast<cudaStream_t>(stream));
 }
@@ -463,6 +479,10 @@ extern "C" int eld_conv3x3_bf16(eld_ctx* ctx, const void* x, int x_pitch, int x_
 {
     ELD_REQUIRE(ctx && x && w_packed && y, "eld_conv3x3_bf16: NULL argument");
     ELD_REQUIRE(act >= 0 && act <= 2 && (act != ACT_MASK || aux), "eld_conv3x3_bf16: bad act / missing aux");
+    ELD_REQUIRE(n > 0 && h > 0 && w > 0, "eld_conv3x3_bf16: empty grid %d x %d x %d", n, h, w);
+    ELD_REQUIRE(in_pitch(x_pitch, x_c0, cin) && in_pitch(y_pitch, y_c0, cout) &&
+                (act != ACT_MASK || in_pitch(aux_pitch, aux_c0, cout)),
+                "eld_conv3x3_bf16: a channel range [c0, c0 + c) lies outside its tensor's pitch");
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     GemmOp op{};
     op.a = x; op.a_pitch = x_pitch; op.a_c0 = x_c0; op.a_mode = A_CONV; op.taps = 9; op.cin = cin;
@@ -478,6 +498,9 @@ extern "C" int eld_deconv2x2_bf16(eld_ctx* ctx, const void* x, int x_pitch, int 
                                   void* stream)
 {
     ELD_REQUIRE(ctx && x && w_packed && y, "eld_deconv2x2_bf16: NULL argument");
+    ELD_REQUIRE(n > 0 && h > 0 && w > 0, "eld_deconv2x2_bf16: empty grid %d x %d x %d", n, h, w);
+    ELD_REQUIRE(in_pitch(x_pitch, x_c0, cin) && in_pitch(y_pitch, y_c0, cout),
+                "eld_deconv2x2_bf16: a channel range [c0, c0 + c) lies outside its tensor's pitch");
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     GemmOp op{};
     op.a = x; op.a_pitch = x_pitch; op.a_c0 = x_c0; op.a_mode = A_CONV; op.taps = 1; op.cin = cin;
@@ -494,6 +517,10 @@ extern "C" int eld_deconv2x2_dgrad_bf16(eld_ctx* ctx, const void* dy, int dy_pit
 {
     ELD_REQUIRE(ctx && dy && w_packed && dx, "eld_deconv2x2_dgrad_bf16: NULL argument");
     ELD_REQUIRE(act == ACT_NONE || (act == ACT_MASK && aux), "eld_deconv2x2_dgrad_bf16: act must be 0 or 2 (+aux)");
+    ELD_REQUIRE(n > 0 && h > 0 && w > 0, "eld_deconv2x2_dgrad_bf16: empty grid %d x %d x %d", n, h, w);
+    ELD_REQUIRE(in_pitch(dy_pitch, dy_c0, cout) && in_pitch(dx_pitch, dx_c0, cin) &&
+                (act != ACT_MASK || in_pitch(aux_pitch, aux_c0, cin)),
+                "eld_deconv2x2_dgrad_bf16: a channel range [c0, c0 + c) lies outside its tensor's pitch");
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     GemmOp op{};
     op.a = dy; op.a_pitch = dy_pitch; op.a_c0 = dy_c0; op.a_mode = A_GATHER; op.taps = 4; op.cin = cout;
@@ -509,6 +536,9 @@ extern "C" int eld_conv3x3_wgrad_bf16(eld_ctx* ctx, const void* x, int x_pitch, 
                                       float* dw, int n, int h, int w, void* stream)
 {
     ELD_REQUIRE(ctx && x && dz && dw, "eld_conv3x3_wgrad_bf16: NULL argument");
+    ELD_REQUIRE(n > 0 && h > 0 && w > 0, "eld_conv3x3_wgrad_bf16: empty grid %d x %d x %d", n, h, w);
+    ELD_REQUIRE(in_pitch(x_pitch, x_c0, cin) && in_pitch(dz_pitch, dz_c0, cout),
+                "eld_conv3x3_wgrad_bf16: a channel range [c0, c0 + c) lies outside its tensor's pitch");
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     WgradOp op{};
     op.mode = WG_CONV; op.p = x; op.p_pitch = x_pitch; op.p_c0 = x_c0; op.p_ch = cin;
@@ -522,6 +552,9 @@ extern "C" int eld_deconv2x2_wgrad_bf16(eld_ctx* ctx, const void* x, int x_pitch
                                         float* dw, int n, int h, int w, void* stream)
 {
     ELD_REQUIRE(ctx && x && dy && dw, "eld_deconv2x2_wgrad_bf16: NULL argument");
+    ELD_REQUIRE(n > 0 && h > 0 && w > 0, "eld_deconv2x2_wgrad_bf16: empty grid %d x %d x %d", n, h, w);
+    ELD_REQUIRE(in_pitch(x_pitch, x_c0, cin) && in_pitch(dy_pitch, dy_c0, cout),
+                "eld_deconv2x2_wgrad_bf16: a channel range [c0, c0 + c) lies outside its tensor's pitch");
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     WgradOp op{};
     op.mode = WG_DECONV; op.p = dy; op.p_pitch = dy_pitch; op.p_c0 = dy_c0; op.p_ch = cout;

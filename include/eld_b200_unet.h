@@ -12,7 +12,11 @@
 /* kinds for eld_pack_weights: source layout is PyTorch's (Conv2d OIHW, ConvTranspose2d IOHW).  The packed
  * operand is OPAQUE: the logical K-major matrix listed below, stored as the shared-memory image the tiles
  * consume (blocks [n_tile][tap][64-channel chunk], 64B/128B swizzle applied) so that a block is one linear
- * bulk copy.  Same element count as the source. */
+ * bulk copy.  Same element count as the source.  The K side of the operand (cin for the fprop kinds, cout for the
+ * dgrad kinds) and its row count must be multiples of 32, and a row count above 256 a multiple of 256 (a block holds
+ * up to 256 rows; a partial last block would span the addresses of a whole one, past the operand's end): conv fprop
+ * cout, conv / deconv dgrad cin in {32, 64, ..., 256, 512, 768, ...}; deconv fprop 4*cout likewise.  Other shapes:
+ * ELD_E_ARG, nothing written. */
 #define ELD_PACK_CONV_FPROP    0  /* [cout][ (kh*3+kw)*cin + ci ]            <- W[co][ci][kh][kw]      */
 #define ELD_PACK_CONV_DGRAD    1  /* [cin ][ (kh*3+kw)*cout + co ]           <- W[co][ci][2-kh][2-kw]  */
 #define ELD_PACK_DECONV_FPROP  2  /* [(kh*2+kw)*cout + co][ci]               <- Wt[ci][co][kh][kw]     */
@@ -25,20 +29,26 @@ int eld_pack_weights(eld_ctx* ctx, const float* w, void* packed_bf16, int cout, 
 
 /* y[n,h,w,y_c0:y_c0+cout] = act( conv3x3_pad1(x[n,h,w,x_c0:x_c0+cin]) + bias )   nn.Conv2d(k=3,p=1), Unet.py:11-44.
  * With ELD_PACK_CONV_DGRAD weights (cin/cout swapped) the same tile is the data gradient.
- * cin % 32 == 0, cout % 32 == 0; any h, w (partial tiles are masked).  bias may be NULL.  y (and aux): 32-byte aligned,
- * pitch and first channel multiples of 16 (the epilogue uses 256-bit accesses). */
+ * cin % 32 == 0, cout % 32 == 0 (above 256 a multiple of 256, as the packed operand); any h, w >= 1 (partial tiles are
+ * masked).  bias may be NULL, at most 1024 entries.  y (and aux): 32-byte aligned, pitch and first channel multiples
+ * of 16 (the epilogue uses 256-bit accesses).  Every channel range [c0, c0 + c) lies inside its tensor's pitch.
+ * A call that breaks one of these rules returns ELD_E_ARG and writes nothing; the same holds for the calls below. */
 int eld_conv3x3_bf16(eld_ctx* ctx, const void* x, int x_pitch, int x_c0, int cin, const void* w_packed,
                      const float* bias, void* y, int y_pitch, int y_c0, int cout, int n, int h, int w,
                      int act, const void* aux, int aux_pitch, int aux_c0, void* stream);
 
 /* nn.ConvTranspose2d(cin, cout, 2, stride=2) (Unet.py:30,34,38,42) as GEMM + pixel-shuffle epilogue:
- * y[n, 2h+kh, 2w+kw, y_c0+co] = sum_ci x[n,h,w,ci] Wt[ci][co][kh][kw] + bias[co].  (h, w) = INPUT grid. */
+ * y[n, 2h+kh, 2w+kw, y_c0+co] = sum_ci x[n,h,w,ci] Wt[ci][co][kh][kw] + bias[co].  (h, w) = INPUT grid.
+ * cin % 32 == 0; cout a power of two >= 32 (the epilogue stores 32 channels of one output sub-pixel at a time) and at
+ * most 1024; any h, w >= 1.  bias may be NULL.  y: as for eld_conv3x3_bf16. */
 int eld_deconv2x2_bf16(eld_ctx* ctx, const void* x, int x_pitch, int x_c0, int cin, const void* w_packed,
                        const float* bias, void* y, int y_pitch, int y_c0, int cout, int n, int h, int w,
                        void* stream);
 
 /* data gradient of the above: dx[n,h,w,ci] = sum_{kh,kw,co} dy[n,2h+kh,2w+kw,co] Wt[ci][co][kh][kw],
- * optionally times the LeakyReLU derivative of aux (the deconv input activation). */
+ * optionally times the LeakyReLU derivative of aux (the deconv input activation; act = ELD_ACT_NONE or ELD_ACT_MASK).
+ * cin % 32 == 0 (above 256 a multiple of 256), cout % 32 == 0; h % 8 == 0 and w % 16 == 0 (the gather loads whole
+ * 8 x 16 tiles of the input grid).  dx and aux: as y and aux of eld_conv3x3_bf16. */
 int eld_deconv2x2_dgrad_bf16(eld_ctx* ctx, const void* dy, int dy_pitch, int dy_c0, int cout,
                              const void* w_packed, void* dx, int dx_pitch, int dx_c0, int cin,
                              int n, int h, int w, int act, const void* aux, int aux_pitch, int aux_c0,
@@ -46,7 +56,8 @@ int eld_deconv2x2_dgrad_bf16(eld_ctx* ctx, const void* dy, int dy_pitch, int dy_
 
 /* Weight gradients, accumulated (+=) in f32 into the PyTorch-layout gradient `dw` (zero it once per
  * step): conv dW[co][ci][kh][kw] += sum_pixels dz[.,co] * x[. + (kh-1,kw-1), ci]   (autograd of Unet.py:11-44);
- * deconv dWt[ci][co][kh][kw] += sum_pixels x[n,h,w,ci] * dy[n,2h+kh,2w+kw,co].  (h, w) = x's grid. */
+ * deconv dWt[ci][co][kh][kw] += sum_pixels x[n,h,w,ci] * dy[n,2h+kh,2w+kw,co].  (h, w) = x's grid.
+ * cin % 32 == 0, cout % 32 == 0, h % 4 == 0, w % 16 == 0 (whole 4 x 16 reduction chunks). */
 int eld_conv3x3_wgrad_bf16(eld_ctx* ctx, const void* x, int x_pitch, int x_c0, int cin,
                            const void* dz, int dz_pitch, int dz_c0, int cout,
                            float* dw, int n, int h, int w, void* stream);

@@ -42,6 +42,26 @@ def ulp_bf16(r):
     return torch.ldexp(torch.ones_like(r), (e - 8).to(torch.int32))
 
 
+def bf16_rule(got, r, S):
+    """the statistics of the bf16 rule for a bf16 output `got` against the float64 value r before the kernel's single
+    rounding and its scale S: (max |got - r| / (ulp_bf16(r) + 2^-20 S), share of elements that differ from
+    round-to-nearest-even(r), every element finite)"""
+    assert got.shape == r.shape, (got.shape, r.shape)
+    g = got.double()
+    ratio = ((g - r).abs() / (ulp_bf16(r) + 2.0 ** -20 * S)).max().item()
+    mism = (got != r.float().bfloat16()).double().mean().item()
+    return ratio, mism, bool(torch.isfinite(g).all())
+
+
+def f32_rule(got, r, S):
+    """the statistics of the fp32 rule: (rel-L2 of got - r, max |got - r| / max |r|, max |got - r| / S)"""
+    d = got.double().reshape(r.shape) - r
+    rel = (d.norm() / r.norm().clamp_min(1e-300)).item()
+    mx = (d.abs().max() / r.abs().max().clamp_min(1e-300)).item()
+    ms = (d.abs() / S.clamp_min(1e-300)).max().item()
+    return rel, mx, ms
+
+
 def slope(a):
     """LeakyReLU' from the sign of the stored activation: 1, or 0.2 where the sign bit is set (+0 counts positive)"""
     return 1.0 - 0.8 * torch.signbit(a.float()).double()
@@ -121,10 +141,12 @@ def _deconv_w(x, dy):
 
 # ---- references, one per launch kind ---------------------------------------------------------------------------------
 def conv_fprop(x, w, b, act=True):
-    """conv3x3 + bias (+ LeakyReLU): x stored bf16 NHWC, w fp32 master OIHW (the operand holds it rounded to bf16)"""
-    x, w, b = x.double(), bf(w), b.double()
-    r = _conv(x, w) + b
-    S = _conv(x.abs(), w.abs()) + b.abs()
+    """conv3x3 + bias (+ LeakyReLU): x stored bf16 NHWC, w fp32 master OIHW (the operand holds it rounded to bf16),
+    b fp32 or None (no bias)"""
+    x, w = x.double(), bf(w)
+    r, S = _conv(x, w), _conv(x.abs(), w.abs())
+    if b is not None:
+        r, S = r + b.double(), S + b.double().abs()
     return (lrelu(r) if act else r), S
 
 
@@ -170,9 +192,12 @@ def pool_code(a):
 
 
 def deconv_fprop(x, wt, b):
-    """ConvTranspose2d(2, stride 2) + bias, pixel-shuffled: x stored bf16 [n,h,w,ci], wt fp32 IOHW"""
-    x, wt, b = x.double(), bf(wt), b.double()
-    return _deconv(x, wt) + b, _deconv(x.abs(), wt.abs()) + b.abs()
+    """ConvTranspose2d(2, stride 2) + bias, pixel-shuffled: x stored bf16 [n,h,w,ci], wt fp32 IOHW, b fp32 or None"""
+    x, wt = x.double(), bf(wt)
+    r, S = _deconv(x, wt), _deconv(x.abs(), wt.abs())
+    if b is not None:
+        r, S = r + b.double(), S + b.double().abs()
+    return r, S
 
 
 def conv_dgrad(dz, w, act=None):
@@ -186,11 +211,15 @@ def conv_dgrad(dz, w, act=None):
     return r, S
 
 
-def deconv_dgrad(dy, wt, act):
-    """deconv data gradient: gather of the up plane dy [n,2h,2w,co], bf16 weights, LeakyReLU' of `act` [n,h,w,ci]"""
+def deconv_dgrad(dy, wt, act=None):
+    """deconv data gradient: gather of the up plane dy [n,2h,2w,co], bf16 weights, LeakyReLU' of `act` [n,h,w,ci]
+    (None: no mask)"""
     dy, wt = dy.double(), bf(wt)
-    s = slope(act)
-    return _deconv_t(dy, wt) * s, _deconv_t(dy.abs(), wt.abs()) * s
+    r, S = _deconv_t(dy, wt), _deconv_t(dy.abs(), wt.abs())
+    if act is not None:
+        s = slope(act)
+        r, S = r * s, S * s
+    return r, S
 
 
 def pool_bwd(a, dskip, dp):

@@ -88,3 +88,46 @@ def test_ulp_and_first_layer_image():
     img = R.first_layer_image(w).view(32, 64)
     # row 5, k = tap 2 * 4 + channel 1 = 9: chunk 1 XOR (5 & 7) = 4 -> column 4 * 8 + 1
     assert img[5, 33] == w[5, 1, 0, 2].bfloat16() and (img.float() != 0).sum() <= 32 * 27
+
+
+def test_reference_variants_without_bias_or_mask():
+    """conv_fprop / deconv_fprop with b = None and deconv_dgrad without a mask: torch's float64 ops on the bf16 operands"""
+    g = torch.Generator().manual_seed(3)
+    x = torch.randn(2, 5, 7, 32, generator=g).bfloat16()
+    w = torch.randn(16, 32, 3, 3, generator=g)
+    r, S = R.conv_fprop(x, w, None, act=False)
+    ref = F.conv2d(_nchw(x.double()), w.bfloat16().double(), padding=1)
+    assert torch.allclose(_nchw(r), ref, rtol=1e-12, atol=1e-12)
+    assert torch.allclose(_nchw(S), F.conv2d(_nchw(x.double()).abs(), w.bfloat16().double().abs(), padding=1),
+                          rtol=1e-12, atol=1e-12)
+    r, _ = R.conv_fprop(x, w, None)
+    assert torch.allclose(_nchw(r), torch.maximum(ref, 0.2 * ref), rtol=1e-12, atol=1e-12)
+    wt = torch.randn(32, 16, 2, 2, generator=g)
+    r, S = R.deconv_fprop(x, wt, None)
+    ref = F.conv_transpose2d(_nchw(x.double()), wt.bfloat16().double(), stride=2)
+    assert torch.allclose(_nchw(r), ref, rtol=1e-12, atol=1e-12) and (S >= r.abs() - 1e-9).all()
+    dy = torch.randn(2, 10, 14, 16, generator=g).bfloat16()
+    r, S = R.deconv_dgrad(dy, wt)
+    xg = _nchw(x.double()).clone().requires_grad_()
+    F.conv_transpose2d(xg, wt.bfloat16().double(), stride=2).backward(_nchw(dy.double()))
+    assert torch.allclose(_nchw(r), xg.grad, rtol=1e-12, atol=1e-12) and (S >= r.abs() - 1e-9).all()
+    # with the mask: the same gradient times LeakyReLU' of the stored activation
+    rm, _ = R.deconv_dgrad(dy, wt, x)
+    s = torch.where(torch.signbit(x.float()), torch.tensor(0.2, dtype=torch.float64), torch.tensor(1.0, dtype=torch.float64))
+    assert torch.allclose(rm, r * s, rtol=1e-12, atol=1e-12)
+
+
+def test_rules_on_known_errors():
+    """bf16_rule / f32_rule: an element one ulp off passes the ulp bound and counts as a mismatch; two ulps fail it"""
+    r = torch.tensor([1.0, 3.0, -0.5, 100.0], dtype=torch.float64)
+    got = r.float().bfloat16().clone()
+    ratio, mism, finite = R.bf16_rule(got, r, torch.zeros_like(r))
+    assert ratio == 0 and mism == 0 and finite
+    got[1] = 3.0 + 2.0 ** -6                      # one ulp at 3
+    ratio, mism, _ = R.bf16_rule(got, r, torch.zeros_like(r))
+    assert ratio == 1.0 and mism == 0.25
+    got[1] = 3.0 + 2.0 ** -5
+    assert R.bf16_rule(got, r, torch.zeros_like(r))[0] == 2.0
+    rel, mx, ms = R.f32_rule(torch.tensor([1.0, 2.0]), torch.tensor([1.0, 2.5], dtype=torch.float64),
+                             torch.tensor([1.0, 1.0], dtype=torch.float64))
+    assert abs(rel - 0.5 / (1 + 2.5 ** 2) ** 0.5) < 1e-12 and mx == 0.2 and ms == 0.5

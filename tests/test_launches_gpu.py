@@ -120,24 +120,18 @@ class Step:
 
     # ---- the three acceptance rules ----
     def bf16(self, kind, where, got, r, S):
-        from tests.launch_ref import ulp_bf16
-        torch = self.t
+        from tests.launch_ref import bf16_rule
         assert got.shape == r.shape, (where, got.shape, r.shape)
-        g = got.double()
-        ratio = ((g - r).abs() / (ulp_bf16(r) + 2.0 ** -20 * S)).max().item()
-        mism = (got != r.float().bfloat16()).double().mean().item()
+        ratio, mism, finite = bf16_rule(got, r, S)
         st = STATS['bf16 ' + kind + self.tag]
         st['ulp_ratio'] = max(st['ulp_ratio'], ratio)
         st['mismatch'] = max(st['mismatch'], mism)
-        if not (ratio <= 1.0 and mism <= MISMATCH[kind]) or not torch.isfinite(g).all():
+        if not (ratio <= 1.0 and mism <= MISMATCH[kind]) or not finite:
             self.fail.append('%s (%s): max |got-r|/(ulp+2^-20 S) = %.3g, mismatch %.3g' % (where, kind, ratio, mism))
 
     def f32(self, kind, where, got, r, S):
-        g = got.double().reshape(r.shape)
-        d = g - r
-        rel = (d.norm() / r.norm().clamp_min(1e-300)).item()
-        mx = (d.abs().max() / r.abs().max().clamp_min(1e-300)).item()
-        ms = (d.abs() / S.clamp_min(1e-300)).max().item()
+        from tests.launch_ref import f32_rule
+        rel, mx, ms = f32_rule(got, r, S)
         st = STATS['fp32 ' + kind + self.tag]
         st['rel_l2'] = max(st['rel_l2'], rel)
         st['max_abs_rel'] = max(st['max_abs_rel'], mx)

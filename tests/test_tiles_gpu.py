@@ -1,0 +1,351 @@
+"""The C-ABI conv primitives (eld_pack_weights, eld_conv3x3_bf16, eld_deconv2x2_bf16, eld_deconv2x2_dgrad_bf16,
+eld_conv3x3_wgrad_bf16, eld_deconv2x2_wgrad_bf16) against the float64 references of tests/launch_ref.py on the same bf16
+operands, across the shapes and options their header admits - including those the U-Net engine never uses.
+
+The case table (tests/tile_cases.py) reaches every kernel instantiation the dispatch can choose, with more tiles than two
+rounds of SMs for each thin tile and each generic N tile, partial 8 x 16 tiles (H % 8 in {1, 3, 4, 7}, W % 16 in
+{1, 8, 15}, H = 1, W = 1), channel offsets and pitches on every operand, and batches whose odd images hold values 1000x
+larger than their neighbours (a halo row read from the wrong image is a large error).  Every output is a slice of a
+larger allocation: the guard image before and after it and the channels outside its range hold a bf16 NaN payload
+and must come back bit-identical; a weight gradient accumulates into a non-zero dW between two fp32 NaN guards.
+
+Acceptance, the rules of test_launches_gpu.py:
+  bf16  every element |got - r| <= ulp_bf16(r) + 2^-20 S (r = the float64 value before the kernel's single rounding,
+        S = the same sum over |terms|), and at most MISMATCH[kernel] of the elements differ from round-to-nearest(r).
+  fp32  (weight gradients) rel-L2 vs float64 <= WGRAD_REL_L2[kernel] and max |got - r| <= WGRAD_MAX_ABS[kernel] max|r|.
+  exact the thin 3x3 tile equals the first N block of the generic tile bit for bit; eld_pack_weights equals the Python
+        restatement of packed_index bit for bit; a refused call writes nothing.
+The gates are about 4x the worst case measured on an H100 80GB HBM3 (SXM, 132 SMs) at its 700 W power limit over this
+file and test_conv_gpu.py: a max |got-r| / (ulp + 2^-20 S) of 0.5 for every kernel (the final rounding alone); mismatch
+shares of 1.8e-4 to 4.3e-4 for the thin tiles, 4.3e-4 / 7.9e-4 / 2.8e-3 for conv_gemm<32 / 64 / 128> (the deep K of
+the 512-channel layers); weight gradients at rel-L2 2.8e-7 to 4.9e-7 and max-abs 3.0e-7 to 8.0e-7 of max|r|.  The whole
+file runs in about 8 s there.  The worst case per kernel is printed at the end (pytest -s)."""
+from collections import defaultdict
+
+import pytest
+
+from tests import tile_cases as T
+
+pytestmark = pytest.mark.gpu
+
+MISMATCH = {'conv3x3_thin<32,32>': 1.1e-3, 'conv3x3_thin<32,64>': 1.7e-3, 'conv3x3_thin<64,32>': 7e-4,
+            'conv3x3_thin<64,64>': 1.7e-3, 'conv_gemm<32>': 1.7e-3, 'conv_gemm<64>': 3.2e-3, 'conv_gemm<128>': 1.1e-2}
+WGRAD_REL_L2 = {'conv3x3_wgrad_thin<32,32>': 1.2e-6, 'conv3x3_wgrad_thin<32,64>': 1.2e-6,
+                'conv3x3_wgrad_thin<64,32>': 1.2e-6, 'conv3x3_wgrad_thin<64,64>': 1.2e-6,
+                'wgrad_gemm<32>': 2e-6, 'wgrad_gemm<64>': 1.2e-6, 'wgrad_gemm<128>': 1.2e-6}
+WGRAD_MAX_ABS = {'conv3x3_wgrad_thin<32,32>': 3.2e-6, 'conv3x3_wgrad_thin<32,64>': 2.3e-6,
+                 'conv3x3_wgrad_thin<64,32>': 3e-6, 'conv3x3_wgrad_thin<64,64>': 2.9e-6,
+                 'wgrad_gemm<32>': 2.4e-6, 'wgrad_gemm<64>': 1.7e-6, 'wgrad_gemm<128>': 1.3e-6}
+NAN16 = 0x7FA5                 # bf16 NaN with a payload: what no launch may write
+NAN32 = 0x7FC0A5A5             # its fp32 counterpart around a weight gradient
+BIG = 1000.0                   # scale of the odd images
+
+STATS = defaultdict(lambda: defaultdict(float))     # kernel -> worst measured value per statistic
+
+
+@pytest.fixture(scope='module')
+def torch():
+    import torch
+    if not torch.cuda.is_available():
+        pytest.skip('no GPU')
+    yield torch
+    print('\nworst case per kernel (bf16: max |got-r| / (ulp + 2^-20 S), mismatch rate; fp32: rel-L2, max-abs / max|r|)')
+    for k in sorted(STATS):
+        print('  %-28s %s' % (k, '  '.join('%s=%.3g' % kv for kv in sorted(STATS[k].items()))))
+
+
+def _sms(torch):
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def _operand(torch, g, n, h, w, pitch, big_odd=True):
+    """bf16 NHWC [n,h,w,pitch]: standard normal, the odd (or even) images x BIG"""
+    scale = torch.ones(n, 1, 1, 1, device='cuda')
+    scale[(1 if big_odd else 0)::2] = BIG
+    return (torch.randn(n, h, w, pitch, device='cuda', generator=g) * scale).bfloat16()
+
+
+def _guarded(torch, n, h, w, pitch):
+    """(the whole allocation [n+2,h,w,pitch] filled with NAN16, the output view = images 1..n)"""
+    full = torch.full((n + 2, h, w, pitch), NAN16, dtype=torch.int16, device='cuda').view(torch.bfloat16)
+    return full, full[1:n + 1]
+
+
+def _untouched(torch, full, c0=None, c=None):
+    """bits of `full` that are not images 1..n, channels [c0, c0 + c) still NAN16 -> number of elements that are not"""
+    b = full.view(torch.int16).clone()
+    if c0 is not None:
+        b[1:-1, ..., c0:c0 + c] = NAN16
+    return int((b != NAN16).sum().item())
+
+
+def _bf16_check(kernel, where, got, r, S):
+    from tests.launch_ref import bf16_rule
+    ratio, mism, finite = bf16_rule(got, r, S)
+    st = STATS['bf16 ' + kernel]
+    st['ulp_ratio'] = max(st['ulp_ratio'], ratio)
+    st['mismatch'] = max(st['mismatch'], mism)
+    assert ratio <= 1.0 and mism <= MISMATCH[kernel] and finite, \
+        '%s (%s): max |got-r|/(ulp+2^-20 S) = %.3g, mismatch %.3g, finite %s' % (where, kernel, ratio, mism, finite)
+
+
+def _f32_check(kernel, where, got, r, S):
+    from tests.launch_ref import f32_rule
+    rel, mx, _ = f32_rule(got, r, S)
+    st = STATS['fp32 ' + kernel]
+    st['rel_l2'] = max(st['rel_l2'], rel)
+    st['max_abs_rel'] = max(st['max_abs_rel'], mx)
+    assert rel <= WGRAD_REL_L2[kernel] and mx <= WGRAD_MAX_ABS[kernel], \
+        '%s (%s): rel-L2 %.3g, max-abs / max|r| %.3g' % (where, kernel, rel, mx)
+
+
+def run_case(torch, c, seed):
+    """one primitive call of case c, checked against its float64 reference and its guards"""
+    from eld_b200 import prims
+    import tests.launch_ref as R
+    g = torch.Generator(device='cuda').manual_seed(seed)
+    kern = T.kernel(c)[0]
+    where = T.case_id(c)
+    fine = c.op.startswith('deconv')
+    if c.op.endswith('wgrad'):
+        x = _operand(torch, g, c.n, c.h, c.w, c.x_pitch)
+        f = 2 if fine else 1
+        # the second operand is large on the EVEN images: a product across an image border is BIG^2
+        q = _operand(torch, g, c.n, f * c.h, f * c.w, c.y_pitch, big_odd=False)
+        xs, qs = x[..., c.x_c0:c.x_c0 + c.ci], q[..., c.y_c0:c.y_c0 + c.co]
+        if fine:
+            r, S, _, _ = R.deconv_wgrad(xs, qs)
+        else:
+            r, S, _, _ = R.conv_wgrad(xs, qs)
+        dw0 = torch.randn(r.shape, device='cuda', generator=g) * r.abs().max().float()
+        k, G = r.numel(), 256
+        full = torch.full((k + 2 * G,), NAN32, dtype=torch.int32, device='cuda').view(torch.float32)
+        dw = full[G:G + k].view(r.shape)
+        dw.copy_(dw0)
+        if fine:
+            prims.deconv2x2_wgrad(x, c.x_c0, c.ci, q, c.y_c0, c.co, dw)
+        else:
+            prims.conv3x3_wgrad(x, c.x_c0, c.ci, q, c.y_c0, c.co, dw)
+        guard = full.view(torch.int32)
+        assert (guard[:G] == NAN32).all() and (guard[G + k:] == NAN32).all(), '%s: dW guard written' % where
+        _f32_check(kern, where, dw, r + dw0.double(), S + dw0.double().abs())
+        return
+    ih, iw = (2 * c.h, 2 * c.w) if c.op == 'deconv.dgrad' else (c.h, c.w)
+    oh, ow = (2 * c.h, 2 * c.w) if c.op == 'deconv' else (c.h, c.w)
+    x = _operand(torch, g, c.n, ih, iw, c.x_pitch)
+    xs = x[..., c.x_c0:c.x_c0 + c.ci]
+    full, y = _guarded(torch, c.n, oh, ow, c.y_pitch)
+    aux = _operand(torch, g, c.n, c.h, c.w, c.aux_pitch) if c.act == prims.ACT_MASK else None
+    auxs = aux[..., c.aux_c0:c.aux_c0 + c.co] if aux is not None else None
+    if c.op == 'conv':
+        W = torch.randn(c.co, c.ci, 3, 3, device='cuda', generator=g) / (3 * c.ci ** 0.5)
+        b = torch.randn(c.co, device='cuda', generator=g) if c.bias else None
+        prims.conv3x3(x, c.x_c0, c.ci, prims.pack_weights(W, prims.PACK_CONV_FPROP), b, y, c.y_c0, c.co, act=c.act)
+        r, S = R.conv_fprop(xs, W, b, act=c.act == prims.ACT_LRELU)
+    elif c.op == 'conv.dgrad':
+        W = torch.randn(c.ci, c.co, 3, 3, device='cuda', generator=g) / (3 * c.ci ** 0.5)
+        prims.conv3x3(x, c.x_c0, c.ci, prims.pack_weights(W, prims.PACK_CONV_DGRAD), None, y, c.y_c0, c.co, act=c.act,
+                      aux=aux, aux_c0=c.aux_c0)
+        r, S = R.conv_dgrad(xs, W, auxs)
+    elif c.op == 'deconv':
+        Wt = torch.randn(c.ci, c.co, 2, 2, device='cuda', generator=g) / c.ci ** 0.5
+        b = torch.randn(c.co, device='cuda', generator=g) if c.bias else None
+        prims.deconv2x2(x, c.x_c0, c.ci, prims.pack_weights(Wt, prims.PACK_DECONV_FPROP), b, y, c.y_c0, c.co)
+        r, S = R.deconv_fprop(xs, Wt, b)
+    else:
+        Wt = torch.randn(c.co, c.ci, 2, 2, device='cuda', generator=g) / c.ci ** 0.5
+        prims.deconv2x2_dgrad(x, c.x_c0, c.ci, prims.pack_weights(Wt, prims.PACK_DECONV_DGRAD), y, c.y_c0, c.co,
+                              act=c.act, aux=aux, aux_c0=c.aux_c0)
+        r, S = R.deconv_dgrad(xs, Wt, auxs)
+    bad = _untouched(torch, full, c.y_c0, c.co)
+    assert bad == 0, '%s: %d guard elements written' % (where, bad)
+    _bf16_check(kern, where, y[..., c.y_c0:c.y_c0 + c.co], r, S)
+
+
+@pytest.mark.parametrize('c', T.CASES, ids=T.case_id)
+def test_primitive(torch, c):
+    run_case(torch, c, T.CASES.index(c) + 1)
+
+
+def test_large_cases_outnumber_the_sms(torch):
+    """with this GPU's SM count: every thin instantiation and every generic N tile has a case with more tiles than two
+    rounds of SMs, an odd count, not a multiple of the SM count"""
+    sms = _sms(torch)
+    kernels = {T.kernel(c)[0] for c in T.CASES}
+    covered = {T.kernel(c)[0] for c in T.CASES if T.many_tiles(c, sms)}
+    assert kernels <= covered, sorted(kernels - covered)
+
+
+@pytest.mark.parametrize('case', T.THIN_VS_GENERIC, ids=lambda t: '%s-%dx%dx%d-%d>%d' % t)
+def test_thin_tile_equals_generic_tile_bitwise(torch, case):
+    """the thin tile runs the generic tile's wgmma sequence (K order taps 0..8, k16 steps, one chunk; the same N): its
+    output equals the first N block of the generic tile, reached by appending output channels (96 for N = 32, 192 for
+    N = 64), bit for bit.  fprop with bias and LeakyReLU; dgrad with the mask."""
+    from eld_b200 import prims
+    op, n, h, w, ci, co = case
+    wide = 96 if co == 32 else 192
+    assert T.kernel(T.case(op, n, h, w, ci, co))[0] == 'conv3x3_thin<%d,%d>' % (co, ci)
+    assert T.kernel(T.case(op, n, h, w, ci, wide))[0] == 'conv_gemm<%d>' % co
+    g = torch.Generator(device='cuda').manual_seed(7)
+    x = _operand(torch, g, n, h, w, ci)
+    y_thin = torch.empty(n, h, w, co, device='cuda', dtype=torch.bfloat16)
+    y_wide = torch.empty(n, h, w, wide, device='cuda', dtype=torch.bfloat16)
+    if op == 'conv':
+        W = torch.randn(wide, ci, 3, 3, device='cuda', generator=g) / (3 * ci ** 0.5)
+        b = torch.randn(wide, device='cuda', generator=g)
+        prims.conv3x3(x, 0, ci, prims.pack_weights(W[:co], prims.PACK_CONV_FPROP), b[:co].contiguous(), y_thin, 0, co,
+                      act=prims.ACT_LRELU)
+        prims.conv3x3(x, 0, ci, prims.pack_weights(W, prims.PACK_CONV_FPROP), b, y_wide, 0, wide, act=prims.ACT_LRELU)
+    else:
+        W = torch.randn(ci, wide, 3, 3, device='cuda', generator=g) / (3 * ci ** 0.5)
+        aux = _operand(torch, g, n, h, w, wide)
+        prims.conv3x3(x, 0, ci, prims.pack_weights(W[:, :co], prims.PACK_CONV_DGRAD), None, y_thin, 0, co,
+                      act=prims.ACT_MASK, aux=aux, aux_c0=0)
+        prims.conv3x3(x, 0, ci, prims.pack_weights(W, prims.PACK_CONV_DGRAD), None, y_wide, 0, wide,
+                      act=prims.ACT_MASK, aux=aux, aux_c0=0)
+    a, b_ = y_thin.view(torch.int16), y_wide[..., :co].contiguous().view(torch.int16)
+    diff = int((a != b_).sum().item())
+    STATS['exact thin vs generic']['elements'] += a.numel()
+    assert diff == 0, '%s: %d of %d elements differ' % (case, diff, a.numel())
+
+
+PACK_SHAPES = [(k, co, ci) for k in range(4) for (co, ci) in [(32, 32), (64, 96), (96, 64), (256, 160), (512, 64),
+                                                               (64, 512), (128, 256)]
+               if T.pack_accepts(k, co, ci)]
+
+
+@pytest.mark.parametrize('shape', PACK_SHAPES, ids=lambda s: 'kind%d-%dx%d' % s)
+def test_pack_weights_matches_packed_index(torch, shape):
+    """eld_pack_weights against the Python restatement of packed_index, bit for bit"""
+    from eld_b200 import prims
+    kind, cout, cin = shape
+    g = torch.Generator(device='cuda').manual_seed(3)
+    W = torch.randn(*((cout, cin, 3, 3) if kind < 2 else (cin, cout, 2, 2)), device='cuda', generator=g)
+    got = prims.pack_weights(W, kind).reshape(-1)
+    src, dst = T.pack_order(kind, cout, cin)
+    want = torch.empty_like(got)
+    want[torch.from_numpy(dst).cuda()] = W.reshape(-1)[torch.from_numpy(src).cuda()].bfloat16()
+    assert torch.equal(got.view(torch.int16), want.view(torch.int16))
+
+
+# ---- the contract: right, or refused with nothing written --------------------------------------------------------------
+def _refused(torch, what, call, *guards):
+    """call() must raise EldError and leave every guard tensor (filled with NAN16 or NAN32) untouched; a guard is a
+    tensor or a (name, tensor) pair"""
+    from eld_b200 import _lib
+    raised = False
+    try:
+        call()
+    except _lib.EldError:
+        raised = True
+    torch.cuda.synchronize()
+    written = []
+    for i, t in enumerate(guards):
+        name, t = t if isinstance(t, tuple) else ('guard %d' % i, t)
+        bits = t.view(torch.int16 if t.element_size() == 2 else torch.int32)
+        written.append((name, int((bits != (NAN16 if t.element_size() == 2 else NAN32)).sum().item())))
+    assert raised and not any(k for _, k in written), '%s: %s; elements written: %s' % (
+        what, 'accepted' if not raised else 'refused', ', '.join('%s %d' % nk for nk in written))
+
+
+@pytest.mark.parametrize('shape', [(0, 384, 32), (0, 320, 64), (1, 32, 384), (2, 96, 32), (3, 32, 320), (0, 48, 32),
+                                   (2, 8, 48)], ids=lambda s: 'kind%d-cout%d-cin%d' % s)
+def test_pack_refuses_partial_256_row_blocks(torch, shape):
+    """an operand of more than 256 rows that is not whole 256-row blocks (or K channels not in chunks of 32): packed_index
+    spans the address range of the rows rounded up to 256, past the operand's end.  The buffer here is the exact operand
+    followed by a guard out to that padded extent, inside one allocation."""
+    from eld_b200 import _lib, prims
+    kind, cout, cin = shape
+    rows, ck, taps = T.pack_geometry(kind, cout, cin)
+    exact = rows * taps * ck
+    padded = (-(-rows // 256) * 256) * taps * max(ck, 64) * 2
+    buf = torch.full((padded,), NAN16, dtype=torch.int16, device='cuda')
+    W = torch.randn(*((cout, cin, 3, 3) if kind < 2 else (cin, cout, 2, 2)), device='cuda')
+    lib = _lib.load()
+    _refused(torch, 'eld_pack_weights(kind %d, cout %d, cin %d): %d rows, operand %d elements' % (kind, cout, cin, rows, exact),
+             lambda: _lib.check(lib.eld_pack_weights(_lib.ctx(0), W.data_ptr(), buf.data_ptr(), cout, cin, kind,
+                                                     prims._st()), 'eld_pack_weights'),
+             ('in the operand', buf[:exact]), ('past its end', buf[exact:]))
+
+
+@pytest.mark.parametrize('cout', [8, 16, 96])
+def test_deconv_refuses_cout_the_shuffle_cannot_store(torch, cout):
+    """the pixel-shuffle epilogue stores 32 GEMM columns of one sub-pixel at a time: cout must be a power of two >= 32"""
+    from eld_b200 import prims
+    n, h, w, cin = 1, 8, 16, 32
+    x = torch.randn(n, h, w, cin, device='cuda').bfloat16()
+    Wt = torch.randn(cin, cout, 2, 2, device='cuda')
+    wp = prims.pack_weights(Wt, prims.PACK_DECONV_FPROP) if cout != 96 else torch.zeros(4 * 256 * cin, device='cuda').bfloat16()
+    b = torch.randn(cout, device='cuda')
+    full, y = _guarded(torch, n, 2 * h, 2 * w, 64)
+    _refused(torch, 'eld_deconv2x2_bf16(cin %d, cout %d, y pitch 64)' % (cin, cout),
+             lambda: prims.deconv2x2(x, 0, cin, wp, b, y, 0, cout), full)
+
+
+def _conv_call(torch, n=1, h=8, w=16, ci=32, co=32, x_pitch=None, x_c0=0, y_pitch=None, y_c0=0, y_offset=0, act=0,
+               aux_pitch=None, aux_c0=0, bias=True):
+    """-> (callable running eld_conv3x3_bf16 with these arguments, the guarded output allocation, aux or None)"""
+    from eld_b200 import prims
+    x_pitch, y_pitch = x_pitch or ci, y_pitch or co
+    x = torch.randn(n, h, w, x_pitch, device='cuda').bfloat16()
+    wp = torch.zeros(-(-co // 256) * 256 * 9 * max(ci, 64), device='cuda').bfloat16()   # any bits: the call is refused
+    b = torch.randn(co, device='cuda') if bias else None
+    numel = n * h * w * y_pitch
+    full = torch.full((numel + 64,), NAN16, dtype=torch.int16, device='cuda').view(torch.bfloat16)
+    y = full[y_offset:y_offset + numel].view(n, h, w, y_pitch)
+    aux = torch.randn(n, h, w, aux_pitch, device='cuda').bfloat16() if aux_pitch else None
+    return (lambda: prims.conv3x3(x, x_c0, ci, wp, b, y, y_c0, co, act=act, aux=aux, aux_c0=aux_c0)), full
+
+
+CONV_REFUSED = {
+    'cin 48': dict(ci=48, x_pitch=64),
+    'cout 48': dict(co=48, y_pitch=64),
+    'y pitch 40': dict(y_pitch=40),
+    'y_c0 8': dict(y_c0=8, y_pitch=64),
+    'y 16-byte aligned': dict(y_offset=8),
+    'mask pitch 40': dict(act=2, aux_pitch=40, bias=False),
+    'mask aux_c0 8': dict(act=2, aux_pitch=64, aux_c0=8, bias=False),
+    'x channels past the pitch': dict(x_c0=32, x_pitch=32),
+    'y channels past the pitch': dict(y_c0=16, y_pitch=32),
+    'mask channels past the pitch': dict(act=2, aux_pitch=32, aux_c0=16, bias=False),
+    'cout 384: 1.5 operand blocks': dict(co=384),
+    'cout 2048: bias entries': dict(co=2048),
+    'empty grid': dict(h=0),
+}
+
+
+@pytest.mark.parametrize('what', sorted(CONV_REFUSED))
+def test_conv_refuses(torch, what):
+    call, full = _conv_call(torch, **CONV_REFUSED[what])
+    _refused(torch, 'eld_conv3x3_bf16 with ' + what, call, full)
+
+
+@pytest.mark.parametrize('hw', [(5, 7), (13, 40), (3, 100), (8, 24), (12, 16)])
+def test_deconv_dgrad_refuses_partial_tiles(torch, hw):
+    """the gather merges (image, row) into one tensor-map dimension: whole 8 x 16 input tiles only"""
+    from eld_b200 import prims
+    (h, w), cin, cout = hw, 64, 32
+    Wt = torch.randn(cin, cout, 2, 2, device='cuda')
+    dy = torch.randn(1, 2 * h, 2 * w, cout, device='cuda').bfloat16()
+    aux = torch.randn(1, h, w, cin, device='cuda').bfloat16()
+    full, dx = _guarded(torch, 1, h, w, cin)
+    _refused(torch, 'eld_deconv2x2_dgrad_bf16 at %d x %d' % (h, w),
+             lambda: prims.deconv2x2_dgrad(dy, 0, cout, prims.pack_weights(Wt, prims.PACK_DECONV_DGRAD), dx, 0, cin,
+                                           act=prims.ACT_MASK, aux=aux), full)
+
+
+@pytest.mark.parametrize('shape', [(6, 16, 32, 32), (8, 24, 64, 64), (8, 16, 48, 32), (8, 16, 32, 40)],
+                         ids=lambda s: '%dx%d-%d>%d' % s)
+def test_wgrad_refuses(torch, shape):
+    """whole 4 x 16 reduction chunks and channel counts in multiples of 32; dW is left as it was"""
+    from eld_b200 import prims
+    h, w, cin, cout = shape
+    x = torch.randn(1, h, w, cin, device='cuda').bfloat16()
+    dz = torch.randn(1, h, w, cout, device='cuda').bfloat16()
+    dy = torch.randn(1, 2 * h, 2 * w, cout, device='cuda').bfloat16()
+    dw = torch.full((cout * cin * 9,), NAN32, dtype=torch.int32, device='cuda').view(torch.float32)
+    _refused(torch, 'eld_conv3x3_wgrad_bf16 %s' % (shape,),
+             lambda: prims.conv3x3_wgrad(x, 0, cin, dz, 0, cout, dw.view(cout, cin, 3, 3)), dw)
+    dwt = torch.full((cin * cout * 4,), NAN32, dtype=torch.int32, device='cuda').view(torch.float32)
+    _refused(torch, 'eld_deconv2x2_wgrad_bf16 %s' % (shape,),
+             lambda: prims.deconv2x2_wgrad(x, 0, cin, dy, 0, cout, dwt.view(cin, cout, 2, 2)), dwt)
