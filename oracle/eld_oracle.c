@@ -278,6 +278,24 @@ void eld_oracle_noise_mosaic(const void* mosaic, int in_dtype, float black, floa
     }
 }
 
+/* Poisson photon counts of the 'P' term, packed [n][4][h][w] float32 clean in -> counts out: the sampler's
+ * accept/reject decisions are float32 by design, so tests/noise_ref.py builds its float64 value on these. */
+void eld_oracle_shot_counts(const float* clean, float* counts, int n, int h, int w,
+                            const oracle_noise_params* params, uint64_t seed, uint64_t frame_id0)
+{
+    size_t plane = (size_t)h * (size_t)w;
+    for (int f = 0; f < n; ++f) {
+        stream_t s = mk_stream(seed, frame_id0 + (uint64_t)f);
+        const oracle_noise_params* p = &params[f];
+        float scale_in = p->saturation / p->ratio, invK = 1.0f / p->K;
+        for (uint32_t c = 0; c < 4; ++c)
+            for (size_t l = 0; l < plane; ++l) {
+                size_t o = ((size_t)f * 4 + c) * plane + l;
+                counts[o] = eld_oracle_poisson_px(&s, (uint32_t)l, c, clean[o] * scale_in * invK);
+            }
+    }
+}
+
 /* --- sampler probes for the distribution tests ------------------------------------------------ */
 void eld_oracle_poisson_stream(float lam, uint64_t seed, uint64_t frame, uint32_t l0, int count, float* out)
 {

@@ -44,6 +44,8 @@ class Oracle:
         lib.eld_oracle_tukey_stream.argtypes = [c.c_float, c.c_uint64, c.c_uint64, c.c_uint32, c.c_int, c.c_void_p]
         lib.eld_oracle_pack_bayer_f32.argtypes = [c.c_void_p, c.c_void_p, c.c_int, c.c_int]
         lib.eld_oracle_pack_bayer_u16.argtypes = [c.c_void_p, c.c_void_p, c.c_int, c.c_int]
+        lib.eld_oracle_shot_counts.argtypes = [c.c_void_p, c.c_void_p, c.c_int, c.c_int, c.c_int,
+                                               c.POINTER(OracleParams), c.c_uint64, c.c_uint64]
 
     def philox(self, ctr, key):
         C = (ctypes.c_uint32 * 4)(*ctr)
@@ -71,6 +73,14 @@ class Oracle:
         self.lib.eld_oracle_noise_mosaic(mosaic.ctypes.data, dt, black, white, noisy.ctypes.data, clean.ctypes.data,
                                          n, H, W, to_params(plist), mask, seed, frame0, int(clip))
         return noisy, clean
+
+    def shot_counts(self, clean, plist, seed, frame0):
+        """Poisson photon counts of the 'P' term for packed clean [n,4,h,w], frames frame0 .. frame0+n-1"""
+        clean = np.ascontiguousarray(clean, np.float32)
+        n, _, h, w = clean.shape
+        out = np.empty_like(clean)
+        self.lib.eld_oracle_shot_counts(clean.ctypes.data, out.ctypes.data, n, h, w, to_params(plist), seed, frame0)
+        return out
 
     def poisson_stream(self, lam, seed, frame, l0, count):
         out = np.empty(count, np.float32)
