@@ -50,6 +50,17 @@ struct eld_ctx {
 namespace eld {
 inline void count_launch(eld_ctx* ctx, int n = 1) { ctx->launches.fetch_add(n, std::memory_order_relaxed); }
 
+// whether the byte ranges [a, a + a_bytes) and [b, b + b_bytes) share an address
+inline bool ranges_overlap(const void* a, size_t a_bytes, const void* b, size_t b_bytes)
+{
+    const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+    return a_bytes > 0 && b_bytes > 0 && x < y + b_bytes && y < x + a_bytes;
+}
+
+// max / clamp that keep NaN, as torch.clamp and np.clip do (fmaxf / fminf return the other operand for a NaN)
+__device__ __forceinline__ float fmax_nan(float x, float lo) { return x != x ? x : fmaxf(x, lo); }
+__device__ __forceinline__ float clamp_nan(float x, float lo, float hi) { return x != x ? x : fminf(fmaxf(x, lo), hi); }
+
 // Launch with programmatic stream serialization (PDL): the kernel may start while its predecessor drains; it blocks in
 // griddepcontrol.wait before touching anything the predecessor writes.
 template <typename... KArgs, typename... Args>

@@ -3,6 +3,8 @@
 //   IlluminanceCorrect.correct (ELD_model.py:156-169): gain = <p, s> / <p, p> over the elements where s != 1, with
 //       p = clamp(predict, 0, 1);  output = gain * p
 //   tensor2im (ELD_model.py:23-38): clip(255 * x, 0, 255), no rounding
+// Every clamp keeps NaN, as torch.clamp and np.clip do: a diverged prediction, or a frame whose mask is empty or whose
+// clamped prediction is all zero (<p, p> = 0, gain NaN), reports PSNR NaN, as the reference does.
 //   quality_assess -> skimage peak_signal_noise_ratio(data_range = 255) (util/index.py:76-79):
 //       PSNR = 10 log10(255^2 / mean((a - b)^2))
 // Three launches (two reductions + a finalise), double accumulation, no host synchronisation.
@@ -38,7 +40,7 @@ eval_dots_kernel(const float* __restrict__ pred, const float* __restrict__ src, 
     double num = 0.0, den = 0.0;
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < per_frame; i += (size_t)gridDim.x * blockDim.x) {
         const float sv = __ldg(s + i);
-        const float pv = fminf(fmaxf(__ldg(p + i), 0.0f), 1.0f);
+        const float pv = clamp_nan(__ldg(p + i), 0.0f, 1.0f);
         if (sv != 1.0f) { num += (double)pv * (double)sv; den += (double)pv * (double)pv; }
     }
     const double a = block_sum(num, sh);
@@ -61,10 +63,10 @@ eval_apply_kernel(const float* __restrict__ pred, const float* __restrict__ src,
     double sq = 0.0;
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < per_frame; i += (size_t)gridDim.x * blockDim.x) {
         float v = __ldg(p + i);
-        if (correct) v = gain * fminf(fmaxf(v, 0.0f), 1.0f);
+        if (correct) v = gain * clamp_nan(v, 0.0f, 1.0f);
         if (o) o[i] = v;
-        const float a = fminf(fmaxf(v * 255.0f, 0.0f), 255.0f);
-        const float b = fminf(fmaxf(__ldg(s + i) * 255.0f, 0.0f), 255.0f);
+        const float a = clamp_nan(v * 255.0f, 0.0f, 255.0f);
+        const float b = clamp_nan(__ldg(s + i) * 255.0f, 0.0f, 255.0f);
         const double d = (double)a - (double)b;
         sq += d * d;
     }
@@ -91,6 +93,12 @@ extern "C" int eld_eval_correct_psnr(eld_ctx* ctx, const float* pred, const floa
 {
     ELD_REQUIRE(ctx && pred && target && scratch && psnr, "eld_eval_correct_psnr: NULL argument");
     ELD_REQUIRE(n > 0 && per_frame > 0, "eld_eval_correct_psnr: empty batch");
+    ELD_REQUIRE(n <= 65535, "eld_eval_correct_psnr: %d frames (at most 65535, one grid row each)", n);
+    // out is written while other blocks still read pred and target: only the element-for-element out == pred is safe
+    const size_t bytes = (size_t)n * per_frame * sizeof(float);
+    ELD_REQUIRE(!out || !ranges_overlap(out, bytes, target, bytes), "eld_eval_correct_psnr: out overlaps target");
+    ELD_REQUIRE(!out || out == pred || !ranges_overlap(out, bytes, pred, bytes),
+                "eld_eval_correct_psnr: out overlaps pred without being pred");
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     ELD_CHECK_CUDA(cudaMemsetAsync(scratch, 0, (size_t)n * 4 * sizeof(double), st));

@@ -20,7 +20,9 @@ struct IspLaunch {
     int h, w;
 };
 
-__device__ __forceinline__ float clamp01(float x) { return fminf(fmaxf(x, 0.0f), 1.0f); }
+// torch.clamp keeps NaN (process.py:56,61); a NaN then reaches the `.int()` of :38 / :83, whose INT_MIN the final clamp
+// turns into 0 - so a NaN in any of a pixel's four packed values makes all three of its outputs 0, here as there
+__device__ __forceinline__ float clamp01(float x) { return clamp_nan(x, 0.0f, 1.0f); }
 
 // torchinterp1d.Interp1d semantics: ind = clamp(searchsorted(x, v) - 1, 0, L-2); y[ind] + slope[ind] * (v - x[ind]),
 // slope = (y[i+1] - y[i]) / (eps + x[i+1] - x[i])
@@ -40,7 +42,7 @@ __device__ __forceinline__ float crf_lookup(const float* __restrict__ E, const f
 
 __device__ __forceinline__ float quant8(float v)          // clamp((v*255).int(), 0, 255).float() / 255
 {
-    int q = (int)__fmul_rn(v, 255.0f);                    // truncation toward zero, like Tensor.int()
+    int q = (int)__fmul_rn(v, 255.0f);                    // truncation toward zero, like Tensor.int(); NaN -> 0
     q = q < 0 ? 0 : (q > 255 ? 255 : q);
     return __fdiv_rn((float)q, 255.0f);
 }
@@ -85,7 +87,7 @@ isp_kernel(const float* __restrict__ packed, float* __restrict__ rgb, const __gr
             float v = (float)(((double)__fmul_rn(r, F.ccm[3 * c]) + (double)__fmul_rn(g, F.ccm[3 * c + 1])) + (double)__fmul_rn(b, F.ccm[3 * c + 2]));
             v = clamp01(v);                                               // :61
             if (L.crf_len > 0) v = crf_lookup(crf_E, crf_f + (size_t)c * L.crf_len, L.crf_len, v);   // :71-84
-            else v = powf(fmaxf(v, 1e-8f), L.inv_gamma);                  // :34-36
+            else v = powf(fmax_nan(v, 1e-8f), L.inv_gamma);                // :34-36
             out[c][k] = clamp01(quant8(v));                               // :38 / :83, ISPDataset's clip (sid_dataset.py:311)
         }
     }
@@ -113,9 +115,12 @@ extern "C" int eld_isp_process(eld_ctx* ctx, const float* packed, float* rgb, in
     ELD_REQUIRE(packed && rgb && wb && ccm, "eld_isp_process: NULL buffer");
     ELD_REQUIRE(gamma > 0.f, "eld_isp_process: gamma must be positive");
     ELD_REQUIRE(crf_len == 0 || (crf_len >= 2 && crf_E && crf_f), "eld_isp_process: a CRF needs >= 2 samples and both arrays");
+    const size_t plane = (size_t)h * w;
+    // frame f writes the planes 3f..3f+2 of rgb while another block may still read frame f' < f from the same addresses
+    ELD_REQUIRE(!ranges_overlap(packed, (size_t)n * 4 * plane * sizeof(float), rgb, (size_t)n * 3 * plane * sizeof(float)),
+                "eld_isp_process: packed and rgb overlap");
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const size_t plane = (size_t)h * w;
     const bool vec = (plane % 4 == 0) && ((reinterpret_cast<uintptr_t>(packed) | reinterpret_cast<uintptr_t>(rgb)) % 16 == 0);
     for (int f0 = 0; f0 < n; f0 += kIspMaxFrames) {
         const int nf = n - f0 < kIspMaxFrames ? n - f0 : kIspMaxFrames;

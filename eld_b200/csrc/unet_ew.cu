@@ -5,6 +5,7 @@
 #include "unet_ew.h"
 #include "umma.cuh"
 #include <cuda_bf16.h>
+#include <algorithm>
 
 namespace eld {
 
@@ -392,6 +393,18 @@ int launch_adam_segments(eld_ctx* ctx, float* p, const float* g, float* m, float
         S.bc1[s] = 1.0f - powf(b1, (float)steps[s]);                 // the bias corrections of launch_adam, per segment
         S.bc2_sqrt[s] = sqrtf(1.0f - powf(b2, (float)steps[s]));
         total += S.cnt[s];
+    }
+    // an element in two ranges would be updated twice, by two threads, without ordering: refuse overlapping ranges
+    int order[kAdamMaxSegments];
+    for (int s = 0; s < n_segs; ++s) order[s] = s;
+    std::sort(order, order + n_segs, [&](int a, int b) { return S.off[a] < S.off[b]; });
+    unsigned long long end = 0;
+    for (int k = 0; k < n_segs; ++k) {
+        const int s = order[k];
+        if (S.cnt[s] == 0) continue;
+        ELD_REQUIRE(S.off[s] >= end && S.cnt[s] <= ~0ull - S.off[s], "adam: segment %d [%llu, +%llu) overlaps another", s,
+                    S.off[s], S.cnt[s]);
+        end = S.off[s] + S.cnt[s];
     }
     S.n = n_segs;
     if (total == 0) return ELD_OK;

@@ -126,7 +126,13 @@ int eld_noise_packed_aug(eld_ctx* ctx, const float* clean, float* noisy, float* 
  *   packed: device f32 [n][4][h][w] (RGBG planes)   rgb: device f32 [n][3][h][w]
  *   wb: HOST [n][4] white-balance gains   ccm: HOST [n][9] cam2rgb, row-major   gamma: 2.2 in the reference
  *   crf_len == 0: gamma curve.  crf_len >= 2: crf_E device [crf_len] (irradiance grid, ascending),
- *   crf_f device [3][crf_len] (per-channel response) - linear interpolation with torchinterp1d's formula. */
+ *   crf_f device [3][crf_len] (per-channel response) - linear interpolation with torchinterp1d's formula.
+ * NaN as in the reference: torch.clamp keeps it and `.int()` of NaN is INT_MIN, clamped to 0, so a NaN in any of a pixel's
+ * four packed values makes all three of its outputs 0.  The exponent is the float 1/gamma, one ulp off the reference's
+ * double 1/2.2 for gamma = 2.2 (an ABI limit: gamma is a float); an 8-bit output can differ by one level where that ulp
+ * moves pow() across a level boundary.
+ * ELD_E_ARG, nothing written: a negative size, a NULL buffer, gamma <= 0 or NaN, crf_len < 0 or 1, a CRF array NULL,
+ * packed and rgb overlapping.  n, h or w == 0: ELD_OK, nothing launched. */
 int eld_isp_process(eld_ctx* ctx, const float* packed, float* rgb, int n, int h, int w,
                     const float* wb, const float* ccm, float gamma,
                     const float* crf_E, const float* crf_f, int crf_len, void* stream);
@@ -135,10 +141,16 @@ int eld_isp_process(eld_ctx* ctx, const float* packed, float* rgb, int n, int h,
  * Metric side of ELDModelBase.eval (models/ELD_model.py:203-243), per frame f of a batch of `n` frames with
  * `per_frame` = C*H*W elements each (f32, any layout, pred and target alike):
  *   correct != 0: IlluminanceCorrect.correct (:156-169): gain = <p,s>/<p,p> over the elements where s != 1,
- *                 p = clamp(pred,0,1); corrected = gain * p (written to `out` if out != NULL, may alias pred)
+ *                 p = clamp(pred,0,1); corrected = gain * p (written to `out` if out != NULL)
+ *   correct == 0: x = pred; a non-NULL `out` receives pred bit for bit, and gain[f] = 1
  *   psnr[f] = 10 log10(255^2 / mean((clip(255 x,0,255) - clip(255 target,0,255))^2)), x = corrected (or pred):
  *             tensor2im (:23-38, no rounding) + skimage's peak_signal_noise_ratio(data_range = 255) (util/index.py:76-79)
- * scratch: device, n * 4 doubles (zeroed here).  psnr, gain (may be NULL): device f32 [n].  No host synchronisation. */
+ * NaN as in the reference (torch.clamp, torch.dot and np.clip keep it): a NaN in a frame's prediction, or an empty
+ * <p, p> (target 1 everywhere, prediction <= 0 everywhere) makes that frame's gain, corrected output and PSNR NaN;
+ * pred == target gives PSNR +inf.
+ * scratch: device, n * 4 doubles (zeroed here).  psnr, gain (may be NULL): device f32 [n].  No host synchronisation.
+ * ELD_E_ARG, nothing written: a NULL ctx / pred / target / scratch / psnr, n == 0, n > 65535, per_frame == 0, `out`
+ * overlapping target, `out` overlapping pred other than out == pred (which is allowed). */
 int eld_eval_correct_psnr(eld_ctx* ctx, const float* pred, const float* target, float* out, int n, size_t per_frame,
                           int correct, double* scratch, float* psnr, float* gain, void* stream);
 

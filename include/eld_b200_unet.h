@@ -143,8 +143,6 @@ int    eld_unet_set_loss(eld_unet* u, int kind);
 int    eld_unet_grad_buckets(size_t* offsets, int max_offsets);      /* returns the bucket count (4) */
 int    eld_unet_bucket_events(eld_unet* u, int enable);
 int    eld_unet_wait_bucket(eld_unet* u, int bucket, void* stream);
-/* torch.optim.Adam step (ELD_model.py:400-401,475) on the flat buffers; grads are multiplied by
- * grad_scale first (1/world_size after a SUM all-reduce).  step counts from 1. */
 /* Per-launch timing (CUDA events on the launch stream) of the steps issued after eld_unet_profile(u, 1);
  * eld_unet_profile_read synchronises, returns name[32] / ms / algorithmic FLOPs / algorithmic bytes per
  * launch and clears the log.  Used by bench.py for the live roofline numbers. */
@@ -161,12 +159,16 @@ int    eld_unet_profile_read(eld_unet* u, int max, char* names32, float* ms, dou
  * {1, 1, 1, element count}); the [tap][ci][co] staging of the conv weight gradients gtmp (f32, parameter offsets).
  * ELD_E_ARG for an unknown name and, on an object created with train = 0, for a training-only one. */
 int    eld_unet_buffer(const eld_unet* u, const char* name, void** ptr, int dims[4], int* elem_bytes);
+/* torch.optim.Adam step (ELD_model.py:400-401,475) on the flat buffers; grads are multiplied by
+ * grad_scale first (1/world_size after a SUM all-reduce), then weight_decay * params is added.  step counts from 1.
+ * ELD_E_ARG, nothing written: a NULL argument, step < 1. */
 int    eld_adam_step(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, size_t n,
                      float lr, float beta1, float beta2, float eps, float weight_decay, int step,
                      float grad_scale, void* stream);
 /* The same update on n_segs ranges of the flat buffers in ONE launch: segs (host) = (offset, count) pairs, steps (host) =
  * each range's own step count (torch.optim.Adam's per-parameter state['step']: a tensor that was frozen for a while has
- * taken fewer steps).  Elements outside the ranges are not touched.  n_segs <= 64. */
+ * taken fewer steps).  Elements outside the ranges are not touched.  n_segs <= 64.  ELD_E_ARG, nothing written: a NULL
+ * argument, a step count < 1, more than 64 ranges, two ranges that share an element (empty ranges share none). */
 int    eld_adam_step_segments(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, const size_t* segs,
                               const int* steps, int n_segs, float lr, float beta1, float beta2, float eps,
                               float weight_decay, float grad_scale, void* stream);

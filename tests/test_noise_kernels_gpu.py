@@ -138,11 +138,23 @@ def _call(torch, entry, inp, out, aux, n, h, w, plist, mask, seed, fid0, clip, d
     return lib.eld_noise_packed_aug(L.ctx(0), inp, out, aux, n, h, w, pa, mask, seed, fid0, clip, fl, st)
 
 
+TRACE_ATTEMPTS = 4
+# later in a long run the profiler drops the first kernel records of a trace, trace after trace (seen on the H100 for
+# the first launch of a call, whatever it was): a few of torch's own kernels go first, and the cached device memory is
+# handed back before each trace
+LEAD_IN = 8
+
+
 def _traced(torch, fn):
     """-> (fn(), canonical names of the noise kernels it launched)"""
     from torch.profiler import ProfilerActivity, profile
     torch.cuda.synchronize()
+    torch.cuda.empty_cache()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        lead = torch.ones(LEAD_IN, device='cuda')
+        for _ in range(LEAD_IN):
+            lead.add_(1)
+        torch.cuda.synchronize()
         rc = fn()
         torch.cuda.synchronize()
     names = {T.canonical(e.key) for e in prof.key_averages() if 'noise_' in e.key}
@@ -205,14 +217,22 @@ def run_case(torch, oracle, c):
     else:
         _, inp = _input(torch, src, c.offs[0])
     flags = np.asarray(c.aug, np.uint8) if c.aug is not None else None
-    n0 = _lib().launch_count(0)
-    rc, names = _traced(torch, lambda: _call(
-        torch, c.entry, inp.data_ptr(), out.view.data_ptr(), aux.view.data_ptr() if aux else None, n, h, w, plist,
-        c.mask, c.seed, c.fid0, c.clip, dtype=0 if c.dtype == 'u16' else 1, black=c.black, white=c.white,
-        scale=c.scale, flags=flags))
-    assert rc == 0, '%s: rc %d: %s' % (where, rc, _lib().load().eld_last_error())
-    assert names == {kern}, '%s: launched %s, the dispatch restatement says %s' % (where, sorted(names), kern)
-    assert _lib().launch_count(0) - n0 == T.launches(c), where
+    # torch.profiler can lose a trace's kernel records (about 1 trace in 100 on the H100) but never invents one: a trace
+    # that names no noise kernel is taken again, the in-place input restored first; a wrong kernel fails at once
+    for attempt in range(TRACE_ATTEMPTS):
+        if attempt and c.inplace:
+            out.view.copy_(torch.from_numpy(src.reshape(-1)).cuda())
+        n0 = _lib().launch_count(0)
+        rc, names = _traced(torch, lambda: _call(
+            torch, c.entry, inp.data_ptr(), out.view.data_ptr(), aux.view.data_ptr() if aux else None, n, h, w, plist,
+            c.mask, c.seed, c.fid0, c.clip, dtype=0 if c.dtype == 'u16' else 1, black=c.black, white=c.white,
+            scale=c.scale, flags=flags))
+        assert rc == 0, '%s: rc %d: %s' % (where, rc, _lib().load().eld_last_error())
+        assert names <= {kern}, '%s: launched %s, the dispatch restatement says %s' % (where, sorted(names), kern)
+        assert _lib().launch_count(0) - n0 == T.launches(c), where
+        if names:
+            break
+    assert names == {kern}, '%s: %d traces in a row lost their kernel records' % (where, TRACE_ATTEMPTS)
     assert out.written_guards() == 0, '%s: %d output guard words written' % (where, out.written_guards())
     if aux is not None:
         assert aux.written_guards() == 0, '%s: %d clean_out / target_out guard words written' % (where, aux.written_guards())
