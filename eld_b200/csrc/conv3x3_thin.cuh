@@ -10,8 +10,8 @@
 //           moves 30 rows of 16 pixels instead of 9 x 8.
 // B       = the layer's whole packed operand for its one N block (9 tap blocks of NT x kc, unet_prims.h packed_index),
 //           bulk-copied once per CTA and resident for every tile (at most 72 KB).
-// K order = the generic tile's: taps 0..8, k16 steps inside a tap, one channel chunk (cin = kc), so every output row
-//           accumulates the same wgmma sequence and the results are bit-identical to conv_gemm_kernel's.
+// K order = the wide tile's with one channel chunk (cin = kc): taps 0..8, k16 steps inside a tap, so every output row
+//           accumulates the same wgmma sequence and the results are bit-identical to conv3x3_wide_kernel's.
 // roles   = warpgroup 0: TMA producer (one thread) | warpgroups 1, 2 take whole tiles in turn (ping-pong): per k16 step
 //           two m64nNTk16 (pixel rows 0-63 / 64-127), then the epilogue of the tile, while the other warpgroup runs its
 //           MMAs.  Each has its own staging area: 128 pixel rows x 32 floats per pass, the 16-byte chunks of row r XOR-ed

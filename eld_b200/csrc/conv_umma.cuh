@@ -1,10 +1,11 @@
-// conv_umma.cuh - persistent, warp-specialised wgmma implicit-GEMM tile for the U-Net's conv3x3 / deconv2x2
-// (fprop and dgrad) on NHWC bf16 activations.
+// conv_umma.cuh - persistent, warp-specialised wgmma implicit-GEMM tile for the U-Net's deconv2x2 (fprop and dgrad) on
+// NHWC bf16 activations, and the epilogue every conv / deconv tile shares.  The 3x3 convolutions run the halo tiles of
+// conv3x3_thin.cuh and conv3x3_wide.cuh.
 //
 //   D[128 pixels x n_tile] (f32, registers)  +=  A[128 pixels x K] (bf16, smem via TMA)  *  B[n_tile x K]^T
 //
-// M tile  = an 8 x 16 pixel patch of one image (TMA box {kc, 16, 8}); every filter tap is one more box at shifted
-//           coordinates - TMA zero-fills out-of-image pixels, which IS the padding.
+// M tile  = an 8 x 16 pixel patch of one image: the fprop's box {kc, 16, 8} of the coarse grid (one tap), or the dgrad's
+//           gather of one sub-pixel (kh, kw) of the fine grid per tap.
 // K       = taps x cin, walked in chunks of kc = 32 or 64 channels (one 64 B / 128 B swizzled row per pixel);
 //           each chunk = kc/16 wgmma.m64nNk16 per consumer warpgroup.
 // B       = the packed weights (unet_prims.h packed_index): one [n_tile x kc] block per (tap, chunk), already in the
@@ -23,7 +24,7 @@ namespace eld {
 struct ConvGemmParams {
     int n_img, H, W;      // output pixel grid (M space)
     int tiles_x, tiles_y; // 16 x 8 pixel tiles
-    int taps, a_mode;     // 9/1 with A_CONV, 4 with A_GATHER
+    int taps, a_mode;     // A_CONV: 9 (the halo tiles) or 1 (conv_gemm_kernel, the deconv fprop); A_GATHER: 4
     int cin;              // K channels per tap
     int a_c0;             // first channel inside the A tensor (concat buffers)
     int kc;               // 32 or 64
@@ -167,6 +168,47 @@ __device__ __forceinline__ void conv_epilogue32(const ConvGemmParams& p, const f
     ptx::st_global_32B(dst + 16, wv + 8);
 }
 
+// Epilogue of one 128 x NT work tile whose accumulators two consumer warpgroups hold (cg = 0 / 1: pixel rows
+// 64 cg .. 64 cg + 63): 64 columns per pass through this warpgroup's staging rows `stg`; thread t -> pixel t % 64,
+// columns 32 (t / 64).
+template <int NT>
+__device__ __forceinline__ void conv_tile_epilogue(const ConvGemmParams& p, const float* s_bias, float* stg,
+                                                   const float (&acc)[NT / 2], int cg, int tile, int n_tiles)
+{
+    const int t = threadIdx.x & 127;
+    const int lane = threadIdx.x & 31;
+    const int tiles_xy = p.tiles_x * p.tiles_y;
+    const int m_tile = tile / n_tiles, n_t = tile - m_tile * n_tiles;
+    const int img = m_tile / tiles_xy;
+    const int rem = m_tile - img * tiles_xy;
+    const int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
+    const int m = cg * 64 + (t & 63);                  // pixel inside the 8 x 16 tile
+    const int x = tx * kConvTileW + (m & 15), y = ty * 8 + (m >> 4);
+    const int wq = t >> 5, r0 = 16 * wq + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int pass = 0; pass < (NT + 63) / 64; ++pass) {
+        ptx::bar_sync(1 + cg, 128);                    // the previous pass / tile is done reading the staging rows
+#pragma unroll
+        for (int j = 0; j < 8 && 8 * pass + j < NT / 8; ++j)
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+                *reinterpret_cast<float2*>(stg + (r0 + 8 * i) * kConvStg + 8 * j + c0) =
+                    make_float2(acc[4 * (8 * pass + j) + 2 * i], acc[4 * (8 * pass + j) + 2 * i + 1]);
+        ptx::bar_sync(1 + cg, 128);
+        const int half = t >> 6;
+        if (64 * pass + 32 * half < NT) {               // whole warps take part (the pool shuffles)
+            float v[32];
+            const float4* src = reinterpret_cast<const float4*>(stg + (t & 63) * kConvStg + 32 * half);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const float4 q = src[j];
+                v[4 * j] = q.x; v[4 * j + 1] = q.y; v[4 * j + 2] = q.z; v[4 * j + 3] = q.w;
+            }
+            conv_epilogue32(p, s_bias, v, img, x, y, n_t * NT + 64 * pass + 32 * half);
+        }
+    }
+}
+
 template <int NT>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParams p)
@@ -222,11 +264,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParams p
                 const uint8_t* bsrc = p.b_ptr + (size_t)pb * p.taps * kchunks * p.b_rows * row_bytes + (size_t)pr * row_bytes;
                 for (int tap = 0; tap < p.taps; ++tap) {
                     int c1, c2, c3, c4;
-                    if (p.a_mode == A_CONV) {
-                        const int t3 = tap / 3;
-                        c1 = x0 + ((p.taps == 9) ? (tap - 3 * t3) - 1 : 0);
-                        c2 = y0 + ((p.taps == 9) ? t3 - 1 : 0);
-                        c3 = img; c4 = 0;
+                    if (p.a_mode == A_CONV) {               // the deconv fprop: one tap, the tile itself
+                        c1 = x0; c2 = y0; c3 = img; c4 = 0;
                     } else {
                         c1 = tap & 1; c2 = x0; c3 = tap >> 1; c4 = gy;
                     }
@@ -249,7 +288,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParams p
 
     // ===================== consumers: warpgroup cg = 0 / 1 owns pixel rows 64 cg .. 64 cg + 63 =====================
     const int cg = (threadIdx.x >> 7) - 1;
-    const int t = threadIdx.x & 127;
     const uint32_t layout = ptx::gmma_layout(row_bytes);
     const uint32_t smem_base = ptx::smem_u32(smem);
     const uint64_t desc0 = ptx::make_gmma_desc(0, 16, 8u * row_bytes, layout);     // everything but the address
@@ -257,7 +295,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParams p
     const int ksub = p.kc / 16;
     int s = 0;
     uint32_t ph = 0;
-    const int tiles_xy = p.tiles_x * p.tiles_y;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         float acc[NT / 2];
 #pragma unroll
@@ -280,37 +317,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParams p
         ptx::wgmma_wait<0>();
         ptx::reg_fence(acc);
         if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty[prev]);
-
-        // ---- epilogue: 64 columns per pass through shared memory; thread t -> pixel t % 64, columns 32 (t / 64) ----
-        const int m_tile = tile / n_tiles, n_t = tile - m_tile * n_tiles;
-        const int img = m_tile / tiles_xy;
-        const int rem = m_tile - img * tiles_xy;
-        const int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
-        const int m = cg * 64 + (t & 63);                  // pixel inside the 8 x 16 tile
-        const int x = tx * kConvTileW + (m & 15), y = ty * 8 + (m >> 4);
-        const int wq = t >> 5, r0 = 16 * wq + (lane >> 2), c0 = 2 * (lane & 3);
-#pragma unroll
-        for (int pass = 0; pass < (NT + 63) / 64; ++pass) {
-            ptx::bar_sync(1 + cg, 128);                    // the previous pass / tile is done reading the staging rows
-#pragma unroll
-            for (int j = 0; j < 8 && 8 * pass + j < NT / 8; ++j)
-#pragma unroll
-                for (int i = 0; i < 2; ++i)
-                    *reinterpret_cast<float2*>(stg + (r0 + 8 * i) * kConvStg + 8 * j + c0) =
-                        make_float2(acc[4 * (8 * pass + j) + 2 * i], acc[4 * (8 * pass + j) + 2 * i + 1]);
-            ptx::bar_sync(1 + cg, 128);
-            const int half = t >> 6;
-            if (64 * pass + 32 * half < NT) {               // whole warps take part (the pool shuffles)
-                float v[32];
-                const float4* src = reinterpret_cast<const float4*>(stg + (t & 63) * kConvStg + 32 * half);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const float4 q = src[j];
-                    v[4 * j] = q.x; v[4 * j + 1] = q.y; v[4 * j + 2] = q.z; v[4 * j + 3] = q.w;
-                }
-                conv_epilogue32(p, s_bias, v, img, x, y, n_t * NT + 64 * pass + 32 * half);
-            }
-        }
+        conv_tile_epilogue<NT>(p, s_bias, stg, acc, cg, tile, n_tiles);
     }
 }
 

@@ -5,6 +5,7 @@
 #include <cstdio>
 #include "conv_umma.cuh"
 #include "conv3x3_thin.cuh"
+#include "conv3x3_wide.cuh"
 #include "wgrad_umma.cuh"
 #include "wgrad_thin.cuh"
 #include "first_conv.cuh"
@@ -87,17 +88,11 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
     // next to the epilogue)
     p.n_tile = (op.n_total % 128 == 0) ? 128 : (op.n_total % 64 == 0) ? 64 : 32;
     const int rb = p.kc * 2;
-    const int stage_bytes = 128 * rb + p.n_tile * rb;
     const int stg_bytes = 2 * 64 * kConvStg * 4;
     const int n_bias = op.epi_mode == EPI_STORE ? op.n_total : op.cout;
     ELD_REQUIRE(n_bias <= 1024, "conv tile: %d bias entries exceed the 4 KB shared-memory copy", n_bias);
-    int stages = (200 * 1024 - stg_bytes - 4096) / stage_bytes;
-    if (stages > 8) stages = 8;
-    if (stages < 2) stages = 2;
-    p.stages = stages;
-    p.stg_smem_off = stages * stage_bytes;
-    p.bias_smem_off = p.stg_smem_off + stg_bytes;
-    p.bar_smem_off = p.bias_smem_off + 4096;
+    // the 3x3 convolutions (9 taps) run the halo tiles; conv_gemm_kernel's A_CONV mode loads the tile itself: one tap
+    ELD_REQUIRE(op.a_mode != A_CONV || op.taps == 9 || op.taps == 1, "conv tile: %d taps on the coarse grid", op.taps);
     p.cout_shift = 0;
     if (op.epi_mode == EPI_SHUFFLE) {
         // the epilogue stores 32 GEMM columns of one sub-pixel at a time: cout must fill whole groups of 32
@@ -106,19 +101,30 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
     }
     p.b_ptr = static_cast<const uint8_t*>(op.b);
 
-    // the thin 3x3 layers (one channel chunk, one N block) run the halo tile with resident weights (conv3x3_thin.cuh)
-    const bool thin = op.a_mode == A_CONV && op.taps == 9 && (op.cin == 32 || op.cin == 64) &&
-                      (op.n_total == 32 || op.n_total == 64);
+    // the 3x3 layers read halo boxes {kc, 16, 10} around each 8 x 16 tile: the thin ones (one channel chunk, one N block)
+    // with resident weights (conv3x3_thin.cuh), the others with a weight ring (conv3x3_wide.cuh)
+    const bool halo = op.a_mode == A_CONV && op.taps == 9;
+    const bool thin = halo && (op.cin == 32 || op.cin == 64) && (op.n_total == 32 || op.n_total == 64);
     CUtensorMap tmA;
     const cuuint64_t eb = 2;  // bf16
-    if (thin) {
+    if (op.a_mode == A_CONV) {
         cuuint64_t dims[5] = { (cuuint64_t)op.a_pitch, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.n_img, 1 };
         cuuint64_t str[4] = { op.a_pitch * eb, (cuuint64_t)op.W * op.a_pitch * eb,
                               (cuuint64_t)op.H * op.W * op.a_pitch * eb,
                               (cuuint64_t)op.n_img * op.H * op.W * op.a_pitch * eb };
-        cuuint32_t box[5] = { (cuuint32_t)p.kc, 16, kThinBoxRows, 1, 1 };
+        cuuint32_t box[5] = { (cuuint32_t)p.kc, 16, halo ? (cuuint32_t)kThinBoxRows : 8u, 1, 1 };
         int rc = encode(ctx, &tmA, op.a, 5, dims, str, box, p.kc * 2);
         if (rc) return rc;
+    } else {
+        // fine tensor [n][2H][2W][pitch] viewed as (c, kw, x, kh, n*H + y)
+        cuuint64_t dims[5] = { (cuuint64_t)op.a_pitch, 2, (cuuint64_t)op.W, 2, (cuuint64_t)op.n_img * op.H };
+        cuuint64_t str[4] = { op.a_pitch * eb, 2 * op.a_pitch * eb, (cuuint64_t)2 * op.W * op.a_pitch * eb,
+                              (cuuint64_t)4 * op.W * op.a_pitch * eb };
+        cuuint32_t box[5] = { (cuuint32_t)p.kc, 1, 16, 1, 8 };
+        int rc = encode(ctx, &tmA, op.a, 5, dims, str, box, p.kc * 2);
+        if (rc) return rc;
+    }
+    if (thin) {
         // [resident weights][halo slots][staging of both consumer warpgroups][bias][barriers] after the 1024-byte alignment
         const int slot_bytes = 3 * kThinBoxRows * 16 * rb;
         const int fixed = 9 * p.n_tile * rb + 2 * kThinStgBytes + 256;
@@ -142,27 +148,46 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
         count_launch(ctx);
         return ELD_OK;
     }
-    if (op.a_mode == A_CONV) {
-        cuuint64_t dims[5] = { (cuuint64_t)op.a_pitch, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.n_img, 1 };
-        cuuint64_t str[4] = { op.a_pitch * eb, (cuuint64_t)op.W * op.a_pitch * eb,
-                              (cuuint64_t)op.H * op.W * op.a_pitch * eb,
-                              (cuuint64_t)op.n_img * op.H * op.W * op.a_pitch * eb };
-        cuuint32_t box[5] = { (cuuint32_t)p.kc, 16, 8, 1, 1 };
-        int rc = encode(ctx, &tmA, op.a, 5, dims, str, box, p.kc * 2);
-        if (rc) return rc;
-    } else {
-        // fine tensor [n][2H][2W][pitch] viewed as (c, kw, x, kh, n*H + y)
-        cuuint64_t dims[5] = { (cuuint64_t)op.a_pitch, 2, (cuuint64_t)op.W, 2, (cuuint64_t)op.n_img * op.H };
-        cuuint64_t str[4] = { op.a_pitch * eb, 2 * op.a_pitch * eb, (cuuint64_t)2 * op.W * op.a_pitch * eb,
-                              (cuuint64_t)4 * op.W * op.a_pitch * eb };
-        cuuint32_t box[5] = { (cuuint32_t)p.kc, 1, 16, 1, 8 };
-        int rc = encode(ctx, &tmA, op.a, 5, dims, str, box, p.kc * 2);
-        if (rc) return rc;
+    cudaError_t e;
+    if (halo) {
+        // [halo slots][weight ring][staging of both consumer warpgroups][bias][barriers] after the 1024-byte alignment;
+        // the weight ring takes what the opt-in maximum leaves
+        const int slot_bytes = 3 * kThinBoxRows * 16 * rb;
+        const int b_bytes = p.n_tile * rb;
+        const int fixed = kWideHaloSlots * slot_bytes + stg_bytes + 4096;
+        int wstages = (kThinSmemBytes - 1024 - 256 - fixed) / b_bytes;
+        if (wstages > 8) wstages = 8;
+        ELD_REQUIRE(wstages >= 2, "wide conv tile: no room for two weight stages");
+        p.stages = wstages;
+        p.stg_smem_off = kWideHaloSlots * slot_bytes + wstages * b_bytes;
+        p.bias_smem_off = p.stg_smem_off + stg_bytes;
+        p.bar_smem_off = p.bias_smem_off + 4096;
+        const size_t smem = 1024 + (size_t)p.bar_smem_off + 256;
+        const int total_tiles = op.n_img * p.tiles_x * p.tiles_y * (p.n_total / p.n_tile);
+        const int grid = total_tiles < ctx->num_sms ? total_tiles : ctx->num_sms;
+        if (p.n_tile == 128) e = p.kc == 64 ? launch_pdl(conv3x3_wide_kernel<128, 64>, grid, kConvThreads, smem, st, tmA, p)
+                                            : launch_pdl(conv3x3_wide_kernel<128, 32>, grid, kConvThreads, smem, st, tmA, p);
+        else if (p.n_tile == 64) e = p.kc == 64 ? launch_pdl(conv3x3_wide_kernel<64, 64>, grid, kConvThreads, smem, st, tmA, p)
+                                                : launch_pdl(conv3x3_wide_kernel<64, 32>, grid, kConvThreads, smem, st, tmA, p);
+        else e = p.kc == 64 ? launch_pdl(conv3x3_wide_kernel<32, 64>, grid, kConvThreads, smem, st, tmA, p)
+                            : launch_pdl(conv3x3_wide_kernel<32, 32>, grid, kConvThreads, smem, st, tmA, p);
+        ELD_CHECK_CUDA(e);
+        ELD_CHECK_CUDA(cudaGetLastError());
+        count_launch(ctx);
+        return ELD_OK;
     }
-    const size_t smem = 1024 /*align slack*/ + (size_t)p.bar_smem_off + 256 /*barriers*/;
+    // the deconv tile: A and the weight block of one (tap, chunk) share a ring stage; stage count from a 200 KB budget
+    const int stage_bytes = 128 * rb + p.n_tile * rb;
+    int stages = (200 * 1024 - stg_bytes - 4096) / stage_bytes;
+    if (stages > 8) stages = 8;
+    if (stages < 2) stages = 2;
+    p.stages = stages;
+    p.stg_smem_off = stages * stage_bytes;
+    p.bias_smem_off = p.stg_smem_off + stg_bytes;
+    p.bar_smem_off = p.bias_smem_off + 4096;
     const int total_tiles = op.n_img * p.tiles_x * p.tiles_y * (p.n_total / p.n_tile);
     const int grid = total_tiles < ctx->num_sms ? total_tiles : ctx->num_sms;
-    cudaError_t e;
+    const size_t smem = 1024 /*align slack*/ + (size_t)p.bar_smem_off + 256 /*barriers*/;
     if (p.n_tile == 128) e = launch_pdl(conv_gemm_kernel<128>, grid, kConvThreads, smem, st, tmA, p);
     else if (p.n_tile == 64) e = launch_pdl(conv_gemm_kernel<64>, grid, kConvThreads, smem, st, tmA, p);
     else e = launch_pdl(conv_gemm_kernel<32>, grid, kConvThreads, smem, st, tmA, p);
@@ -274,6 +299,12 @@ int init_gemm_kernels(eld_ctx* ctx)
     ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_thin_kernel<32, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_thin_kernel<64, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_thin_kernel<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wide_kernel<32, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wide_kernel<32, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wide_kernel<64, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wide_kernel<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wide_kernel<128, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wide_kernel<128, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
