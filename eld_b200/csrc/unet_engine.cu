@@ -609,10 +609,10 @@ struct Runner {
         const Layer& l = u->L[li];
         const View x = in_of(li), y = out_of(li);
         GemmOp op{};
-        op.a = x.p; op.a_pitch = x.pitch; op.a_c0 = x.c0; op.a_mode = A_CONV; op.taps = 9; op.cin = l.cin;
+        op.kind = GEMM_CONV3X3; op.a = x.p; op.a_pitch = x.pitch; op.a_c0 = x.c0; op.cin = l.cin;
         op.n_img = u->n; op.H = u->H >> l.lvl; op.W = u->W >> l.lvl;
-        op.b = wf(li); op.n_total = l.cout; op.cout = l.cout;
-        op.epi_mode = EPI_STORE; op.act = ACT_LRELU; op.out = y.p; op.out_pitch = y.pitch; op.out_c0 = y.c0; op.bias = bias(li);
+        op.b = wf(li); op.cout = l.cout;
+        op.act = ACT_LRELU; op.out = y.p; op.out_pitch = y.pitch; op.out_c0 = y.c0; op.bias = bias(li);
         if (pooled(li)) { op.pool_out = s->pool[l.lvl + 1]; op.pool_code = s->code[l.lvl + 1]; }
         op.pool_pitch = l.cout;
         op.sign_out = s->sign[li];
@@ -625,10 +625,10 @@ struct Runner {
         const Layer& l = u->L[li];
         const View x = in_of(li), y = out_of(li);
         GemmOp op{};
-        op.a = x.p; op.a_pitch = x.pitch; op.a_c0 = x.c0; op.a_mode = A_CONV; op.taps = 1; op.cin = l.cin;
+        op.kind = GEMM_DECONV; op.a = x.p; op.a_pitch = x.pitch; op.a_c0 = x.c0; op.cin = l.cin;
         op.n_img = u->n; op.H = u->H >> (l.lvl + 1); op.W = u->W >> (l.lvl + 1);
-        op.b = wf(li); op.n_total = 4 * l.cout; op.cout = l.cout;
-        op.epi_mode = EPI_SHUFFLE; op.act = ACT_NONE; op.out = y.p; op.out_pitch = y.pitch; op.out_c0 = y.c0; op.bias = bias(li);
+        op.b = wf(li); op.cout = l.cout;
+        op.act = ACT_NONE; op.out = y.p; op.out_pitch = y.pitch; op.out_c0 = y.c0; op.bias = bias(li);
         const double px = (double)u->n * op.H * op.W;
         Scope sc(u, st, l.name, "fprop", 2.0 * px * 4 * l.cout * l.cin, px * 2 * (l.cin + 4 * l.cout) + 8.0 * l.cin * l.cout);
         return launch_conv_gemm(ctx(), op, st);
@@ -656,10 +656,10 @@ struct Runner {
         } else {
             op.out = mask ? u->dz[l.src] : u->dp[l.lvl]; op.out_pitch = l.cin;
         }
-        op.a = u->dz[li]; op.a_pitch = l.cout; op.a_c0 = 0; op.a_mode = A_CONV; op.taps = 9; op.cin = l.cout;
+        op.kind = GEMM_CONV3X3; op.a = u->dz[li]; op.a_pitch = l.cout; op.a_c0 = 0; op.cin = l.cout;
         op.n_img = u->n; op.H = u->H >> l.lvl; op.W = u->W >> l.lvl;
-        op.b = wd(li); op.n_total = nc; op.cout = nc;
-        op.epi_mode = EPI_STORE; op.act = mask ? ACT_MASK : ACT_NONE; op.out_c0 = 0; op.bias = nullptr;
+        op.b = wd(li); op.cout = nc;
+        op.act = mask ? ACT_MASK : ACT_NONE; op.out_c0 = 0; op.bias = nullptr;
         op.aux_sign = mask ? s->sign[l.src] : nullptr;
         ELD_REQUIRE(!mask || op.aux_sign, "eld_unet: %s dgrad: no sign words for its LeakyReLU' mask", l.name);
         const double px = (double)u->n * op.H * op.W;
@@ -671,10 +671,10 @@ struct Runner {
     {
         const Layer& l = u->L[li];
         GemmOp op{};
-        op.a = u->dcat[l.lvl]; op.a_pitch = l.cout; op.a_c0 = 0; op.a_mode = A_GATHER; op.taps = 4; op.cin = l.cout;
+        op.kind = GEMM_DECONV_DGRAD; op.a = u->dcat[l.lvl]; op.a_pitch = l.cout; op.a_c0 = 0; op.cin = l.cout;
         op.n_img = u->n; op.H = u->H >> (l.lvl + 1); op.W = u->W >> (l.lvl + 1);
-        op.b = wd(li); op.n_total = l.cin; op.cout = l.cin;
-        op.epi_mode = EPI_STORE; op.act = ACT_MASK; op.out = u->dz[l.src]; op.out_pitch = l.cin; op.out_c0 = 0;
+        op.b = wd(li); op.cout = l.cin;
+        op.act = ACT_MASK; op.out = u->dz[l.src]; op.out_pitch = l.cin; op.out_c0 = 0;
         op.aux_sign = s->sign[l.src];
         ELD_REQUIRE(op.aux_sign, "eld_unet: %s dgrad: no sign words for its LeakyReLU' mask", l.name);
         const double px = (double)u->n * op.H * op.W;

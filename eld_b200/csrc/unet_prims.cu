@@ -1,6 +1,7 @@
 // unet_prims.cu - host side of the wgmma conv/deconv tiles: TMA tensor-map construction, launch
 // geometry, weight packing, and the C-ABI primitives (include/eld_b200_unet.h).
 #include "common.cuh"
+#include <algorithm>
 #include <cstdlib>
 #include <cstdio>
 #include "conv_umma.cuh"
@@ -12,6 +13,23 @@
 #include "unet_prims.h"
 
 namespace eld {
+
+// Every instantiation of each kernel family, indexed by NT / 64 and KC / 64 (32 -> 0, 64 -> 1, 128 -> 2): the launchers
+// pick from these tables and init_gemm_kernels opts each entry in to its shared memory.
+using ConvKernel = void (*)(CUtensorMap, ConvGemmParams);
+using WgradKernel = void (*)(CUtensorMap, CUtensorMap, WgradParams);
+using WgradThinKernel = void (*)(CUtensorMap, CUtensorMap, WgradThinParams);
+using FirstConvKernel = void (*)(CUtensorMap, CUtensorMap, FirstConvParams);
+static const ConvKernel kConvGemm[3] = { conv_gemm_kernel<32>, conv_gemm_kernel<64>, conv_gemm_kernel<128> };
+static const ConvKernel kConvThin[2][2] = { { conv3x3_thin_kernel<32, 32>, conv3x3_thin_kernel<32, 64> },
+                                            { conv3x3_thin_kernel<64, 32>, conv3x3_thin_kernel<64, 64> } };
+static const ConvKernel kConvWide[3][2] = { { conv3x3_wide_kernel<32, 32>, conv3x3_wide_kernel<32, 64> },
+                                            { conv3x3_wide_kernel<64, 32>, conv3x3_wide_kernel<64, 64> },
+                                            { conv3x3_wide_kernel<128, 32>, conv3x3_wide_kernel<128, 64> } };
+static const WgradKernel kWgradGemm[3] = { wgrad_gemm_kernel<32>, wgrad_gemm_kernel<64>, wgrad_gemm_kernel<128> };
+static const WgradThinKernel kWgradThin[2][2] = { { conv3x3_wgrad_thin_kernel<32, 32>, conv3x3_wgrad_thin_kernel<32, 64> },
+                                                  { conv3x3_wgrad_thin_kernel<64, 32>, conv3x3_wgrad_thin_kernel<64, 64> } };
+static const FirstConvKernel kFirstConv[2] = { first_conv_kernel<false>, first_conv_kernel<true> };   // [wgrad]
 
 static int encode(eld_ctx* ctx, CUtensorMap* map, const void* ptr, int rank, const cuuint64_t* dims,
                   const cuuint64_t* strides_bytes, const cuuint32_t* box, int inner_bytes,
@@ -33,14 +51,49 @@ static int encode(eld_ctx* ctx, CUtensorMap* map, const void* ptr, int rank, con
     return ELD_OK;
 }
 
-int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
+// a bf16 NHWC tensor [n][H][W][pitch] as (c, x, y, image): boxes of {c, w, h} inside one image, swizzled by the box's
+// row of c channels; out-of-image elements are zero-filled
+static int encode_nhwc(eld_ctx* ctx, CUtensorMap* map, const void* t, int pitch, int n, int H, int W,
+                       int box_c, int box_w, int box_h)
 {
-    // Partial tiles are fine for the A_CONV modes (TMA zero-fills out-of-image rows, the epilogue masks its stores);
-    // the gather mode merges (image, row) into one tensor-map dimension and therefore needs whole 8-row tiles.
-    ELD_REQUIRE(op.a_mode == A_CONV || (op.H % 8 == 0 && op.W % 16 == 0),
-                "deconv dgrad tile: H=%d must be a multiple of 8 and W=%d of 16", op.H, op.W);
+    const cuuint64_t eb = 2;
+    cuuint64_t dims[5] = { (cuuint64_t)pitch, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n, 1 };
+    cuuint64_t str[4] = { pitch * eb, (cuuint64_t)W * pitch * eb, (cuuint64_t)H * W * pitch * eb,
+                          (cuuint64_t)n * H * W * pitch * eb };
+    cuuint32_t box[5] = { (cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1, 1 };
+    return encode(ctx, map, t, 5, dims, str, box, box_c * 2);
+}
+
+// the sub-pixel gather view of a fine bf16 NHWC tensor [n][2H][2W][pitch] on its coarse H x W grid: (c, kw, x, kh,
+// n*H + y), boxes of {c, 1, 16, 1, rows} = one sub-pixel (kh, kw) of 16 coarse columns and `rows` coarse rows.  Images
+// and rows share one dimension, so a box must not run past the last row of an image.
+static int encode_subpixel(eld_ctx* ctx, CUtensorMap* map, const void* t, int pitch, int n, int H, int W,
+                           int box_c, int box_rows)
+{
+    const cuuint64_t eb = 2;
+    cuuint64_t dims[5] = { (cuuint64_t)pitch, 2, (cuuint64_t)W, 2, (cuuint64_t)n * H };
+    cuuint64_t str[4] = { pitch * eb, 2 * pitch * eb, (cuuint64_t)2 * W * pitch * eb, (cuuint64_t)4 * W * pitch * eb };
+    cuuint32_t box[5] = { (cuuint32_t)box_c, 1, 16, 1, (cuuint32_t)box_rows };
+    return encode(ctx, map, t, 5, dims, str, box, box_c * 2);
+}
+
+// launches `kernel` on `grid` CTAs with PDL (common.cuh) and counts the launch
+template <typename Kernel, typename... Args>
+static int launch(eld_ctx* ctx, Kernel kernel, int grid, int block, size_t smem, cudaStream_t st, Args... args)
+{
+    ELD_CHECK_CUDA(launch_pdl(kernel, grid, block, smem, st, args...));
+    ELD_CHECK_CUDA(cudaGetLastError());
+    count_launch(ctx);
+    return ELD_OK;
+}
+
+// checks the epilogue options and fills ConvGemmParams for both paths below, all but the shared-memory layout and stages
+static int conv_gemm_params(const GemmOp& op, ConvGemmParams& p)
+{
+    const int n_total = op.kind == GEMM_DECONV ? 4 * op.cout : op.cout;   // the deconv: four sub-pixels of cout columns
+    const bool store = op.kind != GEMM_DECONV;                            // else the deconv's pixel-shuffle epilogue
     ELD_REQUIRE(op.cin % 32 == 0, "conv tile: cin=%d must be a multiple of 32", op.cin);
-    ELD_REQUIRE(op.n_total % 32 == 0, "conv tile: GEMM N=%d must be a multiple of 32", op.n_total);
+    ELD_REQUIRE(n_total % 32 == 0, "conv tile: GEMM N=%d must be a multiple of 32", n_total);
     ELD_REQUIRE(op.a_pitch % 8 == 0, "conv tile: the input pitch must be a multiple of 8 channels");
     // the epilogue moves 64 bytes per pixel as two 32-byte sectors: 32-byte aligned pixel rows and channel offsets
     ELD_REQUIRE(op.out_pitch % 16 == 0 && op.out_c0 % 16 == 0 && (reinterpret_cast<uintptr_t>(op.out) & 31) == 0,
@@ -49,28 +102,29 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
                 "conv tile: mask-source pitch / first channel must be multiples of 16 channels and the tensor 32-byte aligned");
     ELD_REQUIRE(op.pool_out == nullptr || (op.pool_pitch % 16 == 0 && (reinterpret_cast<uintptr_t>(op.pool_out) & 31) == 0),
                 "conv tile: pooled-output pitch must be a multiple of 16 channels and the tensor 32-byte aligned");
-    ConvGemmParams p{};
     p.n_img = op.n_img; p.H = op.H; p.W = op.W;
     p.tiles_x = (op.W + 15) / 16; p.tiles_y = (op.H + 7) / 8;
-    p.taps = op.taps; p.a_mode = op.a_mode; p.cin = op.cin; p.a_c0 = op.a_c0;
+    p.taps = op.kind == GEMM_CONV3X3 ? 9 : op.kind == GEMM_DECONV ? 1 : 4;
+    p.a_mode = op.kind == GEMM_DECONV_DGRAD ? A_GATHER : A_CONV;
+    p.cin = op.cin; p.a_c0 = op.a_c0;
     p.kc = (op.cin % 64 == 0) ? 64 : 32;
-    p.n_total = op.n_total;
-    p.epi_mode = op.epi_mode; p.act = op.act;
+    p.n_total = n_total;
+    p.epi_mode = store ? EPI_STORE : EPI_SHUFFLE; p.act = op.act;
     p.out = static_cast<__nv_bfloat16*>(op.out); p.out_pitch = op.out_pitch; p.out_c0 = op.out_c0;
     p.bias = op.bias;
     p.aux = static_cast<const __nv_bfloat16*>(op.aux); p.aux_pitch = op.aux_pitch; p.aux_c0 = op.aux_c0;
-    ELD_REQUIRE(op.aux_sign == nullptr || (op.act == ACT_MASK && op.epi_mode == EPI_STORE), "conv tile: sign words are a mask source of a plain store epilogue");
-    ELD_REQUIRE(op.sign_out == nullptr || (op.act == ACT_LRELU && op.epi_mode == EPI_STORE && op.out_split == 0),
+    ELD_REQUIRE(op.aux_sign == nullptr || (op.act == ACT_MASK && store), "conv tile: sign words are a mask source of a plain store epilogue");
+    ELD_REQUIRE(op.sign_out == nullptr || (op.act == ACT_LRELU && store && op.out_split == 0),
                 "conv tile: sign words are written behind LeakyReLU by a plain store epilogue");
     p.aux_sign = static_cast<const uint32_t*>(op.aux_sign); p.sign_out = static_cast<uint32_t*>(op.sign_out);
     p.cout = op.cout;
-    ELD_REQUIRE(op.pool_out == nullptr || (op.epi_mode == EPI_STORE && op.H % 2 == 0 && op.W % 2 == 0),
+    ELD_REQUIRE(op.pool_out == nullptr || (store && op.H % 2 == 0 && op.W % 2 == 0),
                 "conv tile: the fused max pool needs a plain store epilogue and even H, W");
     p.pool_out = static_cast<__nv_bfloat16*>(op.pool_out); p.pool_pitch = op.pool_pitch;
     ELD_REQUIRE(op.pool_code == nullptr || (op.pool_out && op.pool_pitch % 32 == 0 && (reinterpret_cast<uintptr_t>(op.pool_code) & 31) == 0),
                 "conv tile: the pool code needs the fused pool, a multiple of 32 channels and a 32-byte aligned buffer");
     p.pool_code = static_cast<uint32_t*>(op.pool_code);
-    ELD_REQUIRE(op.out_split == 0 || (op.epi_mode == EPI_STORE && op.out2 && op.out_split % 32 == 0 && op.out2_pitch % 16 == 0 &&
+    ELD_REQUIRE(op.out_split == 0 || (store && op.out2 && op.out_split % 32 == 0 && op.out2_pitch % 16 == 0 &&
                                      (reinterpret_cast<uintptr_t>(op.out2) & 31) == 0),
                 "conv tile: split store needs a plain store epilogue, a second tensor and a split at a multiple of 32 columns");
     p.out2 = static_cast<__nv_bfloat16*>(op.out2); p.out2_pitch = op.out2_pitch; p.out_split = op.out_split;
@@ -78,53 +132,35 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
     // A prefix starts at row 0 of every block and covers whole 32-row groups, so each tile's rows keep the swizzle
     // phase (row & 7, or (row >> 1) & 3) they were packed with.
     ELD_REQUIRE(op.b_block_rows == 0 || (op.b_block_rows % 32 == 0 && op.b_block_rows <= 256 &&
-                                         (op.n_total <= op.b_block_rows || op.b_block_rows == 256) && op.aux_sign == nullptr),
+                                         (n_total <= op.b_block_rows || op.b_block_rows == 256) && op.aux_sign == nullptr),
                 "conv tile: a row prefix of the packed operand needs whole 32-row groups of its blocks and no sign-word mask");
     // a whole operand of more than 256 rows is whole 256-row blocks (packed_index gives every block a full 256-row slot)
-    ELD_REQUIRE(op.b_block_rows != 0 || op.n_total <= 256 || op.n_total % 256 == 0,
-                "conv tile: GEMM N=%d above 256 must be a multiple of 256", op.n_total);
-    p.b_rows = op.b_block_rows ? op.b_block_rows : (op.n_total <= 256 ? op.n_total : 256);
+    ELD_REQUIRE(op.b_block_rows != 0 || n_total <= 256 || n_total % 256 == 0,
+                "conv tile: GEMM N=%d above 256 must be a multiple of 256", n_total);
+    p.b_rows = op.b_block_rows ? op.b_block_rows : (n_total <= 256 ? n_total : 256);
     // N per tile: 32, 64 or 128 (a 64 x 256 f32 accumulator would take 128 registers per consumer thread and spill
     // next to the epilogue)
-    p.n_tile = (op.n_total % 128 == 0) ? 128 : (op.n_total % 64 == 0) ? 64 : 32;
-    const int rb = p.kc * 2;
-    const int stg_bytes = 2 * 64 * kConvStg * 4;
-    const int n_bias = op.epi_mode == EPI_STORE ? op.n_total : op.cout;
+    p.n_tile = (n_total % 128 == 0) ? 128 : (n_total % 64 == 0) ? 64 : 32;
+    const int n_bias = store ? n_total : op.cout;
     ELD_REQUIRE(n_bias <= 1024, "conv tile: %d bias entries exceed the 4 KB shared-memory copy", n_bias);
-    // the 3x3 convolutions (9 taps) run the halo tiles; conv_gemm_kernel's A_CONV mode loads the tile itself: one tap
-    ELD_REQUIRE(op.a_mode != A_CONV || op.taps == 9 || op.taps == 1, "conv tile: %d taps on the coarse grid", op.taps);
     p.cout_shift = 0;
-    if (op.epi_mode == EPI_SHUFFLE) {
+    if (!store) {
         // the epilogue stores 32 GEMM columns of one sub-pixel at a time: cout must fill whole groups of 32
         ELD_REQUIRE(op.cout >= 32 && (op.cout & (op.cout - 1)) == 0, "deconv tile: cout=%d must be a power of two >= 32", op.cout);
         while ((1 << p.cout_shift) < op.cout) ++p.cout_shift;
     }
     p.b_ptr = static_cast<const uint8_t*>(op.b);
+    return ELD_OK;
+}
 
-    // the 3x3 layers read halo boxes {kc, 16, 10} around each 8 x 16 tile: the thin ones (one channel chunk, one N block)
-    // with resident weights (conv3x3_thin.cuh), the others with a weight ring (conv3x3_wide.cuh)
-    const bool halo = op.a_mode == A_CONV && op.taps == 9;
-    const bool thin = halo && (op.cin == 32 || op.cin == 64) && (op.n_total == 32 || op.n_total == 64);
+// the 3x3 convolutions read halo boxes {kc, 16, 10} around each 8 x 16 tile: the thin ones (one channel chunk, one N block)
+// with resident weights (conv3x3_thin.cuh), the others with a weight ring (conv3x3_wide.cuh)
+static int launch_conv3x3(eld_ctx* ctx, const GemmOp& op, ConvGemmParams& p, cudaStream_t st)
+{
     CUtensorMap tmA;
-    const cuuint64_t eb = 2;  // bf16
-    if (op.a_mode == A_CONV) {
-        cuuint64_t dims[5] = { (cuuint64_t)op.a_pitch, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.n_img, 1 };
-        cuuint64_t str[4] = { op.a_pitch * eb, (cuuint64_t)op.W * op.a_pitch * eb,
-                              (cuuint64_t)op.H * op.W * op.a_pitch * eb,
-                              (cuuint64_t)op.n_img * op.H * op.W * op.a_pitch * eb };
-        cuuint32_t box[5] = { (cuuint32_t)p.kc, 16, halo ? (cuuint32_t)kThinBoxRows : 8u, 1, 1 };
-        int rc = encode(ctx, &tmA, op.a, 5, dims, str, box, p.kc * 2);
-        if (rc) return rc;
-    } else {
-        // fine tensor [n][2H][2W][pitch] viewed as (c, kw, x, kh, n*H + y)
-        cuuint64_t dims[5] = { (cuuint64_t)op.a_pitch, 2, (cuuint64_t)op.W, 2, (cuuint64_t)op.n_img * op.H };
-        cuuint64_t str[4] = { op.a_pitch * eb, 2 * op.a_pitch * eb, (cuuint64_t)2 * op.W * op.a_pitch * eb,
-                              (cuuint64_t)4 * op.W * op.a_pitch * eb };
-        cuuint32_t box[5] = { (cuuint32_t)p.kc, 1, 16, 1, 8 };
-        int rc = encode(ctx, &tmA, op.a, 5, dims, str, box, p.kc * 2);
-        if (rc) return rc;
-    }
-    if (thin) {
+    { int rc = encode_nhwc(ctx, &tmA, op.a, op.a_pitch, op.n_img, op.H, op.W, p.kc, 16, kThinBoxRows); if (rc) return rc; }
+    const int rb = p.kc * 2;
+    if ((op.cin == 32 || op.cin == 64) && (p.n_total == 32 || p.n_total == 64)) {
         // [resident weights][halo slots][staging of both consumer warpgroups][bias][barriers] after the 1024-byte alignment
         const int slot_bytes = 3 * kThinBoxRows * 16 * rb;
         const int fixed = 9 * p.n_tile * rb + 2 * kThinStgBytes + 256;
@@ -137,46 +173,43 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
         p.bar_smem_off = p.bias_smem_off + 256;
         const size_t smem = 1024 + (size_t)p.bar_smem_off + 256;
         const int total_tiles = op.n_img * p.tiles_x * p.tiles_y;
-        const int grid = total_tiles < ctx->num_sms ? total_tiles : ctx->num_sms;
-        cudaError_t e;
-        if (p.n_tile == 64) e = p.kc == 64 ? launch_pdl(conv3x3_thin_kernel<64, 64>, grid, kConvThreads, smem, st, tmA, p)
-                                           : launch_pdl(conv3x3_thin_kernel<64, 32>, grid, kConvThreads, smem, st, tmA, p);
-        else e = p.kc == 64 ? launch_pdl(conv3x3_thin_kernel<32, 64>, grid, kConvThreads, smem, st, tmA, p)
-                            : launch_pdl(conv3x3_thin_kernel<32, 32>, grid, kConvThreads, smem, st, tmA, p);
-        ELD_CHECK_CUDA(e);
-        ELD_CHECK_CUDA(cudaGetLastError());
-        count_launch(ctx);
-        return ELD_OK;
+        return launch(ctx, kConvThin[p.n_tile / 64][p.kc / 64], std::min(total_tiles, ctx->num_sms), kConvThreads, smem, st,
+                      tmA, p);
     }
-    cudaError_t e;
-    if (halo) {
-        // [halo slots][weight ring][staging of both consumer warpgroups][bias][barriers] after the 1024-byte alignment;
-        // the weight ring takes what the opt-in maximum leaves
-        const int slot_bytes = 3 * kThinBoxRows * 16 * rb;
-        const int b_bytes = p.n_tile * rb;
-        const int fixed = kWideHaloSlots * slot_bytes + stg_bytes + 4096;
-        int wstages = (kThinSmemBytes - 1024 - 256 - fixed) / b_bytes;
-        if (wstages > 8) wstages = 8;
-        ELD_REQUIRE(wstages >= 2, "wide conv tile: no room for two weight stages");
-        p.stages = wstages;
-        p.stg_smem_off = kWideHaloSlots * slot_bytes + wstages * b_bytes;
-        p.bias_smem_off = p.stg_smem_off + stg_bytes;
-        p.bar_smem_off = p.bias_smem_off + 4096;
-        const size_t smem = 1024 + (size_t)p.bar_smem_off + 256;
-        const int total_tiles = op.n_img * p.tiles_x * p.tiles_y * (p.n_total / p.n_tile);
-        const int grid = total_tiles < ctx->num_sms ? total_tiles : ctx->num_sms;
-        if (p.n_tile == 128) e = p.kc == 64 ? launch_pdl(conv3x3_wide_kernel<128, 64>, grid, kConvThreads, smem, st, tmA, p)
-                                            : launch_pdl(conv3x3_wide_kernel<128, 32>, grid, kConvThreads, smem, st, tmA, p);
-        else if (p.n_tile == 64) e = p.kc == 64 ? launch_pdl(conv3x3_wide_kernel<64, 64>, grid, kConvThreads, smem, st, tmA, p)
-                                                : launch_pdl(conv3x3_wide_kernel<64, 32>, grid, kConvThreads, smem, st, tmA, p);
-        else e = p.kc == 64 ? launch_pdl(conv3x3_wide_kernel<32, 64>, grid, kConvThreads, smem, st, tmA, p)
-                            : launch_pdl(conv3x3_wide_kernel<32, 32>, grid, kConvThreads, smem, st, tmA, p);
-        ELD_CHECK_CUDA(e);
-        ELD_CHECK_CUDA(cudaGetLastError());
-        count_launch(ctx);
-        return ELD_OK;
-    }
-    // the deconv tile: A and the weight block of one (tap, chunk) share a ring stage; stage count from a 200 KB budget
+    // [halo slots][weight ring][staging of both consumer warpgroups][bias][barriers] after the 1024-byte alignment;
+    // the weight ring takes what the opt-in maximum leaves
+    const int stg_bytes = 2 * 64 * kConvStg * 4;
+    const int slot_bytes = 3 * kThinBoxRows * 16 * rb;
+    const int b_bytes = p.n_tile * rb;
+    const int fixed = kWideHaloSlots * slot_bytes + stg_bytes + 4096;
+    int wstages = (kThinSmemBytes - 1024 - 256 - fixed) / b_bytes;
+    if (wstages > 8) wstages = 8;
+    ELD_REQUIRE(wstages >= 2, "wide conv tile: no room for two weight stages");
+    p.stages = wstages;
+    p.stg_smem_off = kWideHaloSlots * slot_bytes + wstages * b_bytes;
+    p.bias_smem_off = p.stg_smem_off + stg_bytes;
+    p.bar_smem_off = p.bias_smem_off + 4096;
+    const size_t smem = 1024 + (size_t)p.bar_smem_off + 256;
+    const int total_tiles = op.n_img * p.tiles_x * p.tiles_y * (p.n_total / p.n_tile);
+    return launch(ctx, kConvWide[p.n_tile / 64][p.kc / 64], std::min(total_tiles, ctx->num_sms), kConvThreads, smem, st,
+                  tmA, p);
+}
+
+// the deconv fprop (one {kc, 16, 8} box of the coarse tile) and the deconv dgrad (the sub-pixel gather of the fine
+// gradient): conv_gemm_kernel, A and the weight block of one (tap, chunk) in one ring stage
+static int launch_deconv(eld_ctx* ctx, const GemmOp& op, ConvGemmParams& p, cudaStream_t st)
+{
+    // partial tiles are fine for the fprop (TMA zero-fills out-of-image rows, the epilogue masks its stores); the gather
+    // merges (image, row) into one tensor-map dimension and therefore needs whole 8-row tiles
+    ELD_REQUIRE(op.kind == GEMM_DECONV || (op.H % 8 == 0 && op.W % 16 == 0),
+                "deconv dgrad tile: H=%d must be a multiple of 8 and W=%d of 16", op.H, op.W);
+    CUtensorMap tmA;
+    { int rc = op.kind == GEMM_DECONV ? encode_nhwc(ctx, &tmA, op.a, op.a_pitch, op.n_img, op.H, op.W, p.kc, 16, 8)
+                                      : encode_subpixel(ctx, &tmA, op.a, op.a_pitch, op.n_img, op.H, op.W, p.kc, 8);
+      if (rc) return rc; }
+    // stage count from a 200 KB budget
+    const int rb = p.kc * 2;
+    const int stg_bytes = 2 * 64 * kConvStg * 4;
     const int stage_bytes = 128 * rb + p.n_tile * rb;
     int stages = (200 * 1024 - stg_bytes - 4096) / stage_bytes;
     if (stages > 8) stages = 8;
@@ -186,15 +219,15 @@ int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
     p.bias_smem_off = p.stg_smem_off + stg_bytes;
     p.bar_smem_off = p.bias_smem_off + 4096;
     const int total_tiles = op.n_img * p.tiles_x * p.tiles_y * (p.n_total / p.n_tile);
-    const int grid = total_tiles < ctx->num_sms ? total_tiles : ctx->num_sms;
     const size_t smem = 1024 /*align slack*/ + (size_t)p.bar_smem_off + 256 /*barriers*/;
-    if (p.n_tile == 128) e = launch_pdl(conv_gemm_kernel<128>, grid, kConvThreads, smem, st, tmA, p);
-    else if (p.n_tile == 64) e = launch_pdl(conv_gemm_kernel<64>, grid, kConvThreads, smem, st, tmA, p);
-    else e = launch_pdl(conv_gemm_kernel<32>, grid, kConvThreads, smem, st, tmA, p);
-    ELD_CHECK_CUDA(e);
-    ELD_CHECK_CUDA(cudaGetLastError());
-    count_launch(ctx);
-    return ELD_OK;
+    return launch(ctx, kConvGemm[p.n_tile / 64], std::min(total_tiles, ctx->num_sms), kConvThreads, smem, st, tmA, p);
+}
+
+int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st)
+{
+    ConvGemmParams p{};
+    { int rc = conv_gemm_params(op, p); if (rc) return rc; }
+    return op.kind == GEMM_CONV3X3 ? launch_conv3x3(ctx, op, p, st) : launch_deconv(ctx, op, p, st);
 }
 
 // the fp32 NCHW frame [n][4][H][W] as (x in HALF floats, y, plane, image) of bf16: box = 64 halves (32 floats, 128 B,
@@ -228,13 +261,9 @@ int launch_first_conv(eld_ctx* ctx, const float* x, int cin, const void* w_img, 
     p.w_img = static_cast<const uint8_t*>(w_img); p.bias = bias;
     p.out = static_cast<__nv_bfloat16*>(out); p.out_pitch = out_pitch; p.sign_out = static_cast<uint32_t*>(sign_out);
     const int total = n * p.tiles_x * p.tiles_y;
-    const int grid = total < ctx->num_sms ? total : ctx->num_sms;
     CUtensorMap tmX;
     { int rc = encode_frame(ctx, &tmX, x, cin, n, H, W); if (rc) return rc; }
-    ELD_CHECK_CUDA(launch_pdl(first_conv_kernel<false>, grid, kFcThreads, first_conv_smem(false), st, tmX, tmX, p));
-    ELD_CHECK_CUDA(cudaGetLastError());
-    count_launch(ctx);
-    return ELD_OK;
+    return launch(ctx, kFirstConv[0], std::min(total, ctx->num_sms), kFcThreads, first_conv_smem(false), st, tmX, tmX, p);
 }
 
 int launch_first_conv_wgrad(eld_ctx* ctx, const float* x, int cin, const void* dz, int dz_pitch, float* dw, float* db,
@@ -245,20 +274,11 @@ int launch_first_conv_wgrad(eld_ctx* ctx, const float* x, int cin, const void* d
     p.x = x; p.n_img = n; p.H = H; p.W = W; p.tiles_x = W / 16; p.tiles_y = H / 8; p.cin = cin;
     p.dw = dw; p.db = db;
     CUtensorMap tmQ;
-    const cuuint64_t eb = 2;
-    cuuint64_t dims[5] = { (cuuint64_t)dz_pitch, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n, 1 };
-    cuuint64_t str[4] = { dz_pitch * eb, (cuuint64_t)W * dz_pitch * eb, (cuuint64_t)H * W * dz_pitch * eb,
-                          (cuuint64_t)n * H * W * dz_pitch * eb };
-    cuuint32_t box[5] = { 32, 16, 8, 1, 1 };
-    { int rc = encode(ctx, &tmQ, dz, 5, dims, str, box, 64); if (rc) return rc; }
+    { int rc = encode_nhwc(ctx, &tmQ, dz, dz_pitch, n, H, W, 32, 16, 8); if (rc) return rc; }
     const int total = n * p.tiles_x * p.tiles_y;
-    const int grid = total < ctx->num_sms ? total : ctx->num_sms;
     CUtensorMap tmX;
     { int rc = encode_frame(ctx, &tmX, x, cin, n, H, W); if (rc) return rc; }
-    ELD_CHECK_CUDA(launch_pdl(first_conv_kernel<true>, grid, kFcThreads, first_conv_smem(true), st, tmX, tmQ, p));
-    ELD_CHECK_CUDA(cudaGetLastError());
-    count_launch(ctx);
-    return ELD_OK;
+    return launch(ctx, kFirstConv[1], std::min(total, ctx->num_sms), kFcThreads, first_conv_smem(true), st, tmX, tmQ, p);
 }
 
 // align slack, the TMA ring, the B image, full / empty barriers
@@ -273,45 +293,23 @@ int launch_first_conv_dgrad(eld_ctx* ctx, const void* dz, const float* w, int ci
     p.n_img = n; p.H = H; p.W = W; p.tiles_x = W / 16; p.tiles_y = H / 8; p.cin = cin;
     p.w = w; p.dx = dx;
     CUtensorMap tmZ;
-    const cuuint64_t eb = 2;
-    cuuint64_t dims[5] = { 32, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n, 1 };
-    cuuint64_t str[4] = { 32 * eb, (cuuint64_t)W * 32 * eb, (cuuint64_t)H * W * 32 * eb, (cuuint64_t)n * H * W * 32 * eb };
-    cuuint32_t box[5] = { 32, 16, 10, 1, 1 };
-    { int rc = encode(ctx, &tmZ, dz, 5, dims, str, box, 64); if (rc) return rc; }
+    { int rc = encode_nhwc(ctx, &tmZ, dz, 32, n, H, W, 32, 16, 10); if (rc) return rc; }
     const int total = n * p.tiles_x * p.tiles_y;
-    const int grid = total < ctx->num_sms ? total : ctx->num_sms;
-    ELD_CHECK_CUDA(launch_pdl(first_conv_dgrad_kernel, grid, kDgThreads, first_conv_dgrad_smem(), st, tmZ, p));
-    ELD_CHECK_CUDA(cudaGetLastError());
-    count_launch(ctx);
-    return ELD_OK;
+    return launch(ctx, first_conv_dgrad_kernel, std::min(total, ctx->num_sms), kDgThreads, first_conv_dgrad_smem(), st, tmZ, p);
 }
 
 int init_gemm_kernels(eld_ctx* ctx)
 {
+    const auto attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(first_conv_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_conv_dgrad_smem()));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(first_conv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_conv_smem(false)));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(first_conv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_conv_smem(true)));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_thin_kernel<32, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_thin_kernel<32, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_thin_kernel<64, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_thin_kernel<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wide_kernel<32, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wide_kernel<32, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wide_kernel<64, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wide_kernel<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wide_kernel<128, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wide_kernel<128, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wgrad_thin_kernel<32, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wgrad_thin_kernel<32, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wgrad_thin_kernel<64, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
-    ELD_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_wgrad_thin_kernel<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kThinSmemBytes));
+    ELD_CHECK_CUDA(cudaFuncSetAttribute(first_conv_dgrad_kernel, attr, (int)first_conv_dgrad_smem()));
+    for (int wgrad = 0; wgrad < 2; ++wgrad)
+        ELD_CHECK_CUDA(cudaFuncSetAttribute(kFirstConv[wgrad], attr, (int)first_conv_smem(wgrad)));
+    for (auto k : kConvGemm) ELD_CHECK_CUDA(cudaFuncSetAttribute(k, attr, 220 * 1024));
+    for (auto& nt : kConvThin) for (auto k : nt) ELD_CHECK_CUDA(cudaFuncSetAttribute(k, attr, kThinSmemBytes));
+    for (auto& nt : kConvWide) for (auto k : nt) ELD_CHECK_CUDA(cudaFuncSetAttribute(k, attr, kThinSmemBytes));
+    for (auto k : kWgradGemm) ELD_CHECK_CUDA(cudaFuncSetAttribute(k, attr, 220 * 1024));
+    for (auto& nt : kWgradThin) for (auto k : nt) ELD_CHECK_CUDA(cudaFuncSetAttribute(k, attr, kThinSmemBytes));
     return ELD_OK;
 }
 
@@ -335,35 +333,12 @@ static int launch_wgrad_thin(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
     p.stages = stages;
 
     CUtensorMap tmP, tmQ;
-    const cuuint64_t eb = 2;
-    {
-        cuuint64_t dims[5] = { (cuuint64_t)op.p_pitch, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.n_img, 1 };
-        cuuint64_t str[4] = { op.p_pitch * eb, (cuuint64_t)op.W * op.p_pitch * eb, (cuuint64_t)op.H * op.W * op.p_pitch * eb,
-                              (cuuint64_t)op.n_img * op.H * op.W * op.p_pitch * eb };
-        cuuint32_t box[5] = { (cuuint32_t)op.p_ch, 16, kThinBoxRows, 1, 1 };
-        int rc = encode(ctx, &tmP, op.p, 5, dims, str, box, op.p_ch * 2);
-        if (rc) return rc;
-    }
-    {
-        cuuint64_t dims[5] = { (cuuint64_t)op.q_pitch, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.n_img, 1 };
-        cuuint64_t str[4] = { op.q_pitch * eb, (cuuint64_t)op.W * op.q_pitch * eb, (cuuint64_t)op.H * op.W * op.q_pitch * eb,
-                              (cuuint64_t)op.n_img * op.H * op.W * op.q_pitch * eb };
-        cuuint32_t box[5] = { (cuuint32_t)op.q_ch, 16, 8, 1, 1 };
-        int rc = encode(ctx, &tmQ, op.q, 5, dims, str, box, op.q_ch * 2);
-        if (rc) return rc;
-    }
+    { int rc = encode_nhwc(ctx, &tmP, op.p, op.p_pitch, op.n_img, op.H, op.W, op.p_ch, 16, kThinBoxRows); if (rc) return rc; }
+    { int rc = encode_nhwc(ctx, &tmQ, op.q, op.q_pitch, op.n_img, op.H, op.W, op.q_ch, 16, 8); if (rc) return rc; }
     const size_t smem = 1024 + (size_t)stages * slot_bytes + 256;
     const int total_tiles = op.n_img * p.tiles_x * p.tiles_y;
-    const int grid = total_tiles < ctx->num_sms ? total_tiles : ctx->num_sms;
-    cudaError_t e;
-    if (op.q_ch == 64) e = op.p_ch == 64 ? launch_pdl(conv3x3_wgrad_thin_kernel<64, 64>, grid, kWgThinThreads, smem, st, tmP, tmQ, p)
-                                         : launch_pdl(conv3x3_wgrad_thin_kernel<64, 32>, grid, kWgThinThreads, smem, st, tmP, tmQ, p);
-    else e = op.p_ch == 64 ? launch_pdl(conv3x3_wgrad_thin_kernel<32, 64>, grid, kWgThinThreads, smem, st, tmP, tmQ, p)
-                           : launch_pdl(conv3x3_wgrad_thin_kernel<32, 32>, grid, kWgThinThreads, smem, st, tmP, tmQ, p);
-    ELD_CHECK_CUDA(e);
-    ELD_CHECK_CUDA(cudaGetLastError());
-    count_launch(ctx);
-    return ELD_OK;
+    return launch(ctx, kWgradThin[op.q_ch / 64][op.p_ch / 64], std::min(total_tiles, ctx->num_sms), kWgThinThreads, smem, st,
+                  tmP, tmQ, p);
 }
 
 int launch_wgrad(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
@@ -403,40 +378,12 @@ int launch_wgrad(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
     p.db = op.db;
 
     CUtensorMap tmP, tmQ;
-    const cuuint64_t eb = 2;
-    if (op.mode == WG_CONV) {
-        cuuint64_t dims[5] = { (cuuint64_t)op.p_pitch, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.n_img, 1 };
-        cuuint64_t str[4] = { op.p_pitch * eb, (cuuint64_t)op.W * op.p_pitch * eb, (cuuint64_t)op.H * op.W * op.p_pitch * eb,
-                              (cuuint64_t)op.n_img * op.H * op.W * op.p_pitch * eb };
-        cuuint32_t box[5] = { (cuuint32_t)p.box_ch, 16, 4, 1, 1 };
-        int rc = encode(ctx, &tmP, op.p, 5, dims, str, box, p.box_ch * 2);
-        if (rc) return rc;
-    } else {
-        cuuint64_t dims[5] = { (cuuint64_t)op.p_pitch, 2, (cuuint64_t)op.W, 2, (cuuint64_t)op.n_img * op.H };
-        cuuint64_t str[4] = { op.p_pitch * eb, 2 * op.p_pitch * eb, (cuuint64_t)2 * op.W * op.p_pitch * eb,
-                              (cuuint64_t)4 * op.W * op.p_pitch * eb };
-        cuuint32_t box[5] = { (cuuint32_t)p.box_ch, 1, 16, 1, 4 };
-        int rc = encode(ctx, &tmP, op.p, 5, dims, str, box, p.box_ch * 2);
-        if (rc) return rc;
-    }
-    {
-        cuuint64_t dims[5] = { (cuuint64_t)op.q_pitch, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.n_img, 1 };
-        cuuint64_t str[4] = { op.q_pitch * eb, (cuuint64_t)op.W * op.q_pitch * eb, (cuuint64_t)op.H * op.W * op.q_pitch * eb,
-                              (cuuint64_t)op.n_img * op.H * op.W * op.q_pitch * eb };
-        cuuint32_t box[5] = { (cuuint32_t)p.q_box_ch, 16, 4, 1, 1 };
-        int rc = encode(ctx, &tmQ, op.q, 5, dims, str, box, p.q_box_ch * 2);
-        if (rc) return rc;
-    }
+    { int rc = op.mode == WG_CONV ? encode_nhwc(ctx, &tmP, op.p, op.p_pitch, op.n_img, op.H, op.W, p.box_ch, 16, 4)
+                                  : encode_subpixel(ctx, &tmP, op.p, op.p_pitch, op.n_img, op.H, op.W, p.box_ch, 4);
+      if (rc) return rc; }
+    { int rc = encode_nhwc(ctx, &tmQ, op.q, op.q_pitch, op.n_img, op.H, op.W, p.q_box_ch, 16, 4); if (rc) return rc; }
     const size_t smem = (size_t)stages * stage_bytes + 1024 + 256;
-    const int grid = items * p.ksplit;
-    cudaError_t e;
-    if (n_tile == 128) e = launch_pdl(wgrad_gemm_kernel<128>, grid, kWgradThreads, smem, st, tmP, tmQ, p);
-    else if (n_tile == 64) e = launch_pdl(wgrad_gemm_kernel<64>, grid, kWgradThreads, smem, st, tmP, tmQ, p);
-    else e = launch_pdl(wgrad_gemm_kernel<32>, grid, kWgradThreads, smem, st, tmP, tmQ, p);
-    ELD_CHECK_CUDA(e);
-    ELD_CHECK_CUDA(cudaGetLastError());
-    count_launch(ctx);
-    return ELD_OK;
+    return launch(ctx, kWgradGemm[n_tile / 64], items * p.ksplit, kWgradThreads, smem, st, tmP, tmQ, p);
 }
 
 // ---- weight packing: fp32 master (PyTorch layout) -> bf16 K-major GEMM operand -------------------
@@ -516,10 +463,10 @@ extern "C" int eld_conv3x3_bf16(eld_ctx* ctx, const void* x, int x_pitch, int x_
                 "eld_conv3x3_bf16: a channel range [c0, c0 + c) lies outside its tensor's pitch");
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     GemmOp op{};
-    op.a = x; op.a_pitch = x_pitch; op.a_c0 = x_c0; op.a_mode = A_CONV; op.taps = 9; op.cin = cin;
+    op.kind = GEMM_CONV3X3; op.a = x; op.a_pitch = x_pitch; op.a_c0 = x_c0; op.cin = cin;
     op.n_img = n; op.H = h; op.W = w;
-    op.b = w_packed; op.n_total = cout; op.cout = cout;
-    op.epi_mode = EPI_STORE; op.act = act; op.out = y; op.out_pitch = y_pitch; op.out_c0 = y_c0; op.bias = bias;
+    op.b = w_packed; op.cout = cout;
+    op.act = act; op.out = y; op.out_pitch = y_pitch; op.out_c0 = y_c0; op.bias = bias;
     op.aux = aux; op.aux_pitch = aux_pitch; op.aux_c0 = aux_c0;
     return launch_conv_gemm(ctx, op, static_cast<cudaStream_t>(stream));
 }
@@ -534,10 +481,10 @@ extern "C" int eld_deconv2x2_bf16(eld_ctx* ctx, const void* x, int x_pitch, int 
                 "eld_deconv2x2_bf16: a channel range [c0, c0 + c) lies outside its tensor's pitch");
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     GemmOp op{};
-    op.a = x; op.a_pitch = x_pitch; op.a_c0 = x_c0; op.a_mode = A_CONV; op.taps = 1; op.cin = cin;
+    op.kind = GEMM_DECONV; op.a = x; op.a_pitch = x_pitch; op.a_c0 = x_c0; op.cin = cin;
     op.n_img = n; op.H = h; op.W = w;
-    op.b = w_packed; op.n_total = 4 * cout; op.cout = cout;
-    op.epi_mode = EPI_SHUFFLE; op.act = ACT_NONE; op.out = y; op.out_pitch = y_pitch; op.out_c0 = y_c0; op.bias = bias;
+    op.b = w_packed; op.cout = cout;
+    op.act = ACT_NONE; op.out = y; op.out_pitch = y_pitch; op.out_c0 = y_c0; op.bias = bias;
     return launch_conv_gemm(ctx, op, static_cast<cudaStream_t>(stream));
 }
 
@@ -554,10 +501,10 @@ extern "C" int eld_deconv2x2_dgrad_bf16(eld_ctx* ctx, const void* dy, int dy_pit
                 "eld_deconv2x2_dgrad_bf16: a channel range [c0, c0 + c) lies outside its tensor's pitch");
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     GemmOp op{};
-    op.a = dy; op.a_pitch = dy_pitch; op.a_c0 = dy_c0; op.a_mode = A_GATHER; op.taps = 4; op.cin = cout;
+    op.kind = GEMM_DECONV_DGRAD; op.a = dy; op.a_pitch = dy_pitch; op.a_c0 = dy_c0; op.cin = cout;
     op.n_img = n; op.H = h; op.W = w;
-    op.b = w_packed; op.n_total = cin; op.cout = cin;
-    op.epi_mode = EPI_STORE; op.act = act; op.out = dx; op.out_pitch = dx_pitch; op.out_c0 = dx_c0; op.bias = nullptr;
+    op.b = w_packed; op.cout = cin;
+    op.act = act; op.out = dx; op.out_pitch = dx_pitch; op.out_c0 = dx_c0; op.bias = nullptr;
     op.aux = aux; op.aux_pitch = aux_pitch; op.aux_c0 = aux_c0;
     return launch_conv_gemm(ctx, op, static_cast<cudaStream_t>(stream));
 }

@@ -29,28 +29,35 @@ __host__ __device__ inline size_t packed_index(int rows, int ck, int taps, int n
     return block * ((size_t)n_tile * kc) + (size_t)(byte >> 1);
 }
 
+// what a GemmOp computes: a 3x3 conv (fprop or dgrad: 9 taps around each pixel, GEMM N = cout), a 2x2 stride-2 deconv
+// fprop (1 tap, GEMM N = 4 * cout, pixel-shuffle epilogue) or a deconv dgrad (4 taps gathered from the fine gradient's
+// sub-pixels, GEMM N = cout)
+enum { GEMM_CONV3X3 = 0, GEMM_DECONV = 1, GEMM_DECONV_DGRAD = 2 };
+
 struct GemmOp {
+    int kind;           // GEMM_CONV3X3 / GEMM_DECONV / GEMM_DECONV_DGRAD
     const void* a;      // bf16 NHWC activation (or gradient) tensor
     int a_pitch, a_c0;  // channels per pixel in memory, first channel used
-    int a_mode, taps, cin;
-    int n_img, H, W;    // M space (output pixel grid)
-    const void* b;      // bf16 packed weights [n_total][taps*cin]
-    int n_total, cout;
-    int epi_mode, act;
+    int cin;            // GEMM K channels per tap
+    int n_img, H, W;    // M space (output pixel grid; the coarse grid of the deconvolutions)
+    const void* b;      // bf16 packed weights [GEMM N][taps*cin]
+    int cout;
+    int act;
     void* out;
     int out_pitch, out_c0;
     const float* bias;
     const void* aux;
     int aux_pitch, aux_c0;
-    const void* aux_sign = nullptr;   // ACT_MASK from sign words (uint32 [pixel][n_total / 32]) instead of `aux`
-    void* sign_out = nullptr;         // EPI_STORE + ACT_LRELU: also write the output's sign words
-    void* pool_out = nullptr;   // optional fused 2x2 max pool of the activated output (EPI_STORE only)
+    const void* aux_sign = nullptr;   // ACT_MASK from sign words (uint32 [pixel][GEMM N / 32]) instead of `aux`
+    void* sign_out = nullptr;         // ACT_LRELU, not the deconv: also write the output's sign words
+    void* pool_out = nullptr;   // optional fused 2x2 max pool of the activated output (not the deconv)
     int pool_pitch = 0;
     void* pool_code = nullptr;  // optional with pool_out: 1 byte per pooled element (argmax + signs) for the pool backward
-    void* out2 = nullptr;       // EPI_STORE split store: columns >= out_split go to out2 (planar halves of a concat gradient)
+    void* out2 = nullptr;       // split store (not the deconv): columns >= out_split go to out2 (planar halves of a concat
+                                // gradient)
     int out2_pitch = 0, out_split = 0;
-    int b_block_rows = 0;       // rows of one packed weight block when the GEMM reads only the first n_total rows of each
-                                // (a prefix of the output channels); 0 = the operand has exactly n_total rows
+    int b_block_rows = 0;       // rows of one packed weight block when the GEMM reads only the first GEMM N rows of each
+                                // (a prefix of the output channels); 0 = the operand has exactly GEMM N rows
 };
 
 struct WgradOp {

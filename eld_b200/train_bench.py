@@ -25,7 +25,8 @@ def _tensor_roofline(recs, exclude=('conv10',)):
     ach = fl / (t_ms * 1e-3) / 1e12
     return {'bound': 'tensor', 'achieved': ach, 'peak': tf_peak, 'unit': 'TFLOP/s', 'frac': ach / tf_peak,
             'frac_of_sustained_peak': ach / tf_sus, 'traffic': None,
-            'kernel': 'conv_gemm_kernel + wgrad_gemm_kernel (all %d wgmma launches of a step)' % len(tens),
+            'kernel': ('first_conv_kernel + conv3x3_thin_kernel + conv3x3_wide_kernel + conv_gemm_kernel + '
+                       'conv3x3_wgrad_thin_kernel + wgrad_gemm_kernel (all %d wgmma launches of a step)' % len(tens)),
             'algorithmic_flops_per_step': fl, 'tensor_ms_per_step': t_ms, 'all_kernels_ms_per_step': total_ms,
             'share_of_step': t_ms / total_ms,
             'peak_kind': 'bf16_tflops (dense)'}

@@ -4,8 +4,8 @@ several channel chunks of 32 and of 64 with partial tiles at the right and botto
 three (N = 96), and the engine's split stores into planar concat gradients and its row-prefix dgrads.
 
 The C-ABI cases run through tests/test_tiles_gpu.py's run_case: the float64 references of tests/launch_ref.py under its
-bf16 rule and conv_gemm<NT> mismatch gates, with every output a slice of a NaN-payload guard that must come back bit for
-bit.  The engine cases check every launch of one training step as tests/test_launches_gpu.py does."""
+bf16 rule and conv3x3_wide<NT,KC> mismatch gates, with every output a slice of a NaN-payload guard that must come back
+bit for bit.  The engine cases check every launch of one training step as tests/test_launches_gpu.py does."""
 import pytest
 
 from tests import tile_cases as T
@@ -37,7 +37,7 @@ def test_cases_reach_the_wide_tile():
     """every case is a 9-tap launch the thin predicate leaves to the generic N tiles, and the shapes the docstring names
     are there"""
     for c in WIDE_CASES:
-        assert T.kernel(c)[0].startswith('conv_gemm<'), T.case_id(c)
+        assert T.kernel(c)[0].startswith('conv3x3_wide<'), T.case_id(c)
     feats = [T.kernel(c)[1] for c in WIDE_CASES]
     assert {(f['kc'], f['chunks'] > 1) for f in feats} >= {(32, True), (64, True)}
     tiles = [T.tiles(c) for c in WIDE_CASES]

@@ -6,6 +6,7 @@ import numpy as np
 from tests import tile_cases as T
 
 THIN = ['conv3x3_thin<%d,%d>' % (nt, kc) for nt in (32, 64) for kc in (32, 64)]
+WIDE = ['conv3x3_wide<%d,%d>' % (nt, kc) for nt in (32, 64, 128) for kc in (32, 64)]
 WGRAD_THIN = ['conv3x3_wgrad_thin<%d,%d>' % (nt, kc) for nt in (32, 64) for kc in (32, 64)]
 GENERIC = ['conv_gemm<%d>' % nt for nt in (32, 64, 128)]
 WGRAD_GENERIC = ['wgrad_gemm<%d>' % nt for nt in (32, 64, 128)]
@@ -19,8 +20,8 @@ def test_dispatch_restatement():
     """kernel() follows launch_conv_gemm / launch_wgrad on the shapes the engine uses"""
     assert T.kernel(T.case('conv', 1, 8, 16, 32, 32))[0] == 'conv3x3_thin<32,32>'
     assert T.kernel(T.case('conv', 1, 8, 16, 64, 32))[0] == 'conv3x3_thin<32,64>'
-    assert T.kernel(T.case('conv', 1, 8, 16, 128, 64)) == ('conv_gemm<64>', {'kc': 64, 'chunks': 2, 'a_mode': 'conv',
-                                                                             'epi': 'store'})
+    assert T.kernel(T.case('conv', 1, 8, 16, 128, 64)) == ('conv3x3_wide<64,64>', {'kc': 64, 'chunks': 2})
+    assert T.kernel(T.case('conv.dgrad', 1, 8, 16, 32, 96)) == ('conv3x3_wide<32,32>', {'kc': 32, 'chunks': 1})
     assert T.kernel(T.case('deconv', 1, 8, 16, 512, 256))[1]['epi'] == 'shuffle'
     assert T.kernel(T.case('deconv.dgrad', 1, 8, 16, 64, 128)) == ('conv_gemm<128>', {'kc': 64, 'chunks': 1,
                                                                                      'a_mode': 'gather', 'epi': 'store'})
@@ -29,15 +30,16 @@ def test_dispatch_restatement():
     assert T.kernel(T.case('conv.wgrad', 1, 8, 16, 96, 64)) == ('wgrad_gemm<64>', {'mode': 'conv', 'partial_m': True,
                                                                                    'n_blocks': 1})
     assert T.tiles(T.case('conv', 3, 71, 200, 32, 96)) == 3 * 9 * 13 * 3
+    assert T.tiles(T.case('deconv', 1, 8, 16, 64, 64)) == 2
 
 
 def test_cases_reach_every_instantiation():
     reached = {T.kernel(c)[0] for c in T.CASES}
-    assert set(THIN + WGRAD_THIN + GENERIC + WGRAD_GENERIC) == reached, reached
-    for name in GENERIC:
-        assert {f['kc'] for f in _features(name)} == {32, 64}, name
+    assert set(THIN + WIDE + WGRAD_THIN + GENERIC + WGRAD_GENERIC) == reached, reached
+    wide = [f for name in WIDE for f in _features(name)]
+    assert {f['kc'] for f in wide if f['chunks'] >= 3} == {32, 64}
     gen = [f for name in GENERIC for f in _features(name)]
-    assert any(f['chunks'] >= 3 for f in gen)
+    assert {f['kc'] for f in gen} == {32, 64} and any(f['chunks'] >= 3 for f in gen)
     assert {f['a_mode'] for f in gen} == {'conv', 'gather'} and {f['epi'] for f in gen} == {'store', 'shuffle'}
     for name in WGRAD_GENERIC:
         assert {f['mode'] for f in _features(name)} == {'conv', 'deconv'}, name
@@ -49,7 +51,7 @@ def test_cases_reach_every_instantiation():
 
 def test_every_instantiation_outnumbers_the_sms():
     """an odd tile count above 2 x 132, not a multiple of 132, for every instantiation"""
-    for name in THIN + WGRAD_THIN + GENERIC + WGRAD_GENERIC:
+    for name in THIN + WIDE + WGRAD_THIN + GENERIC + WGRAD_GENERIC:
         assert any(T.kernel(c)[0] == name and T.many_tiles(c, T.SMS_H100) for c in T.CASES), name
 
 

@@ -2,12 +2,12 @@
 eld_conv3x3_wgrad_bf16, eld_deconv2x2_wgrad_bf16) against the float64 references of tests/launch_ref.py on the same bf16
 operands, across the shapes and options their header admits - including those the U-Net engine never uses.
 
-The case table (tests/tile_cases.py) reaches every kernel instantiation the dispatch can choose, with more tiles than two
-rounds of SMs for each thin tile and each generic N tile, partial 8 x 16 tiles (H % 8 in {1, 3, 4, 7}, W % 16 in
-{1, 8, 15}, H = 1, W = 1), channel offsets and pitches on every operand, and batches whose odd images hold values 1000x
-larger than their neighbours (a halo row read from the wrong image is a large error).  Every output is a slice of a
-larger allocation: the guard image before and after it and the channels outside its range hold a bf16 NaN payload
-and must come back bit-identical; a weight gradient accumulates into a non-zero dW between two fp32 NaN guards.
+The case table (tests/tile_cases.py) reaches every kernel instantiation the dispatch can choose, each with more tiles
+than two rounds of SMs, partial 8 x 16 tiles (H % 8 in {1, 3, 4, 7}, W % 16 in {1, 8, 15}, H = 1, W = 1), channel
+offsets and pitches on every operand, and batches whose odd images hold values 1000x larger than their neighbours (a
+halo row read from the wrong image is a large error).  Every output is a slice of a larger allocation: the guard image
+before and after it and the channels outside its range hold a bf16 NaN payload and must come back bit-identical; a
+weight gradient accumulates into a non-zero dW between two fp32 NaN guards.
 
 Acceptance, the rules of test_launches_gpu.py:
   bf16  every element |got - r| <= ulp_bf16(r) + 2^-20 S (r = the float64 value before the kernel's single rounding,
@@ -17,9 +17,10 @@ Acceptance, the rules of test_launches_gpu.py:
         restatement of packed_index bit for bit; a refused call writes nothing.
 The gates are about 4x the worst case measured on an H100 80GB HBM3 (SXM, 132 SMs) at its 700 W power limit over this
 file and test_conv_gpu.py: a max |got-r| / (ulp + 2^-20 S) of 0.5 for every kernel (the final rounding alone); mismatch
-shares of 1.8e-4 to 4.3e-4 for the thin tiles, 4.3e-4 / 7.9e-4 / 2.8e-3 for conv_gemm<32 / 64 / 128> (the deep K of
-the 512-channel layers); weight gradients at rel-L2 2.8e-7 to 4.9e-7 and max-abs 3.0e-7 to 8.0e-7 of max|r|.  The whole
-file runs in about 8 s there.  The worst case per kernel is printed at the end (pytest -s)."""
+shares of 1.8e-4 to 4.3e-4 for the thin tiles, 4.3e-4 / 7.9e-4 / 2.8e-3 for the wide and deconv tiles of N tile 32 /
+64 / 128 together (the deep K of the 512-channel layers), which share a gate per N tile; weight gradients at rel-L2
+2.8e-7 to 4.9e-7 and max-abs 3.0e-7 to 8.0e-7 of max|r|.  The whole file runs in about 8 s there.  The worst case per
+kernel is printed at the end (pytest -s)."""
 from collections import defaultdict
 
 import pytest
@@ -29,7 +30,9 @@ from tests import tile_cases as T
 pytestmark = pytest.mark.gpu
 
 MISMATCH = {'conv3x3_thin<32,32>': 1.1e-3, 'conv3x3_thin<32,64>': 1.7e-3, 'conv3x3_thin<64,32>': 7e-4,
-            'conv3x3_thin<64,64>': 1.7e-3, 'conv_gemm<32>': 1.7e-3, 'conv_gemm<64>': 3.2e-3, 'conv_gemm<128>': 1.1e-2}
+            'conv3x3_thin<64,64>': 1.7e-3, 'conv3x3_wide<32,32>': 1.7e-3, 'conv3x3_wide<32,64>': 1.7e-3,
+            'conv3x3_wide<64,32>': 3.2e-3, 'conv3x3_wide<64,64>': 3.2e-3, 'conv3x3_wide<128,32>': 1.1e-2,
+            'conv3x3_wide<128,64>': 1.1e-2, 'conv_gemm<32>': 1.7e-3, 'conv_gemm<64>': 3.2e-3, 'conv_gemm<128>': 1.1e-2}
 WGRAD_REL_L2 = {'conv3x3_wgrad_thin<32,32>': 1.2e-6, 'conv3x3_wgrad_thin<32,64>': 1.2e-6,
                 'conv3x3_wgrad_thin<64,32>': 1.2e-6, 'conv3x3_wgrad_thin<64,64>': 1.2e-6,
                 'wgrad_gemm<32>': 2e-6, 'wgrad_gemm<64>': 1.2e-6, 'wgrad_gemm<128>': 1.2e-6}
@@ -168,8 +171,8 @@ def test_primitive(torch, c):
 
 
 def test_large_cases_outnumber_the_sms(torch):
-    """with this GPU's SM count: every thin instantiation and every generic N tile has a case with more tiles than two
-    rounds of SMs, an odd count, not a multiple of the SM count"""
+    """with this GPU's SM count: every instantiation has a case with more tiles than two rounds of SMs, an odd count,
+    not a multiple of the SM count"""
     sms = _sms(torch)
     kernels = {T.kernel(c)[0] for c in T.CASES}
     covered = {T.kernel(c)[0] for c in T.CASES if T.many_tiles(c, sms)}
@@ -185,7 +188,7 @@ def test_thin_tile_equals_generic_tile_bitwise(torch, case):
     op, n, h, w, ci, co = case
     wide = 96 if co == 32 else 192
     assert T.kernel(T.case(op, n, h, w, ci, co))[0] == 'conv3x3_thin<%d,%d>' % (co, ci)
-    assert T.kernel(T.case(op, n, h, w, ci, wide))[0] == 'conv_gemm<%d>' % co
+    assert T.kernel(T.case(op, n, h, w, ci, wide))[0] == 'conv3x3_wide<%d,%d>' % (co, ci)
     g = torch.Generator(device='cuda').manual_seed(7)
     x = _operand(torch, g, n, h, w, ci)
     y_thin = torch.empty(n, h, w, co, device='cuda', dtype=torch.bfloat16)

@@ -56,9 +56,9 @@ def n_tile(n):
 
 
 def kernel(c):
-    """the kernel instantiation a case reaches, as (name, features): conv3x3_thin<NT,KC>, conv_gemm<NT>,
-    conv3x3_wgrad_thin<NT,KC> or wgrad_gemm<NT>, with the template arguments in the name and the run-time options that
-    matter in `features`"""
+    """the kernel instantiation a case reaches, as (name, features): conv3x3_thin<NT,KC>, conv3x3_wide<NT,KC>,
+    conv_gemm<NT> (the deconvolutions), conv3x3_wgrad_thin<NT,KC> or wgrad_gemm<NT>, with the template arguments in the
+    name and the run-time options that matter in `features`"""
     if c.op.endswith('wgrad'):
         conv = c.op == 'conv.wgrad'
         p_ch, q_ch = (c.ci, c.co) if conv else (c.co, c.ci)      # P: the M side (taps x channels), Q: the N side
@@ -72,20 +72,23 @@ def kernel(c):
                                        'n_blocks': q_ch // nt}
     a_mode, taps, k, n, epi = gemm_shape(c)
     kc = 64 if k % 64 == 0 else 32
-    if a_mode == 'conv' and taps == 9 and k in (32, 64) and n in (32, 64):
-        return 'conv3x3_thin<%d,%d>' % (n, k), {}
+    if taps == 9:
+        if k in (32, 64) and n in (32, 64):
+            return 'conv3x3_thin<%d,%d>' % (n, k), {}
+        return 'conv3x3_wide<%d,%d>' % (n_tile(n), kc), {'kc': kc, 'chunks': k // kc}
     return 'conv_gemm<%d>' % n_tile(n), {'kc': kc, 'chunks': k // kc, 'a_mode': a_mode, 'epi': epi}
 
 
 def tiles(c):
-    """work tiles the persistent grid walks: 8 x 16 pixel tiles (times the N blocks for conv_gemm); for wgrad_gemm the
-    4 x 16 pixel chunks of the reduction, which its K splits walk through their stage rings"""
+    """work tiles the persistent grid walks: 8 x 16 pixel tiles (times the N blocks for the wide and deconv tiles); for
+    wgrad_gemm the 4 x 16 pixel chunks of the reduction, which its K splits walk through their stage rings"""
     name, _ = kernel(c)
     if name.startswith('wgrad_gemm'):
         return c.n * (c.h // 4) * (c.w // 16)
     t = c.n * -(-c.h // 8) * -(-c.w // 16)
-    if name.startswith('conv_gemm'):
-        t *= gemm_shape(c)[3] // n_tile(gemm_shape(c)[3])
+    if not c.op.endswith('wgrad'):
+        n = gemm_shape(c)[3]
+        t *= n // n_tile(n)
     return t
 
 
@@ -150,10 +153,13 @@ CASES = [
     case('conv', 3, 12, 15, 32, 32, act=1, bias=False, x_c0=32, x_pitch=64),
     case('conv.dgrad', 2, 13, 17, 64, 32, x_c0=64, x_pitch=192),
     case('conv.dgrad', 1, 1, 47, 32, 32, act=2),
-    # --- conv_gemm<NT>: kc 32 / 64, 3 and 5 channel chunks, several N blocks, both A modes, both epilogues ---
+    # --- conv3x3_wide<NT, KC>: 3 and 5 channel chunks, several N blocks ---
     case('conv', 3, 71, 200, 32, 96, act=1, x_c0=16, x_pitch=64, y_c0=32, y_pitch=160),   # NT 32, kc 32, 1053 tiles
     case('conv', 3, 39, 175, 64, 192, act=1),                                     # NT 64, kc 64, 495 tiles
     case('conv', 5, 65, 129, 160, 128, act=1, x_c0=32, x_pitch=256),              # NT 128, 5 chunks of 32, 405 tiles
+    case('conv', 1, 72, 240, 128, 96, act=1, y_c0=32, y_pitch=128),               # NT 32, kc 64, 405 tiles
+    case('conv.dgrad', 1, 135, 263, 96, 64, act=2, aux_c0=64, aux_pitch=128),     # NT 64, 3 chunks of 32, 289 tiles
+    case('conv', 1, 135, 263, 128, 128, bias=False, y_c0=64, y_pitch=256),        # NT 128, kc 64, 289 tiles
     case('conv', 2, 7, 33, 96, 64, bias=False),                                   # NT 64, 3 chunks of 32
     case('conv', 1, 4, 24, 128, 96, y_c0=16, y_pitch=128),                        # NT 32, kc 64
     case('conv', 2, 9, 1, 32, 128),                                               # NT 128, kc 32
@@ -162,7 +168,9 @@ CASES = [
     case('conv.dgrad', 2, 11, 40, 96, 64, act=2, aux_c0=32, aux_pitch=128),       # NT 64, 3 chunks of 32
     case('conv.dgrad', 1, 8, 16, 256, 512, act=2),
     case('conv.dgrad', 3, 7, 49, 64, 96),                                         # NT 32, kc 64
+    # --- conv_gemm<NT>: the deconv fprop and the deconv dgrad's gather, kc 32 / 64, several N blocks ---
     case('deconv', 3, 23, 45, 64, 32, x_c0=64, x_pitch=128, y_c0=32, y_pitch=64),  # NT 128, 3 x 3 x 3 = 27 tiles
+    case('deconv', 1, 135, 263, 64, 32, x_c0=32, x_pitch=96),                     # NT 128, 289 tiles
     case('deconv', 1, 9, 17, 96, 64, bias=False),                                 # NT 128, 2 N blocks, 3 chunks
     case('deconv', 2, 1, 1, 512, 256, y_c0=256, y_pitch=512),                     # 8 N blocks, 2 operand blocks
     case('deconv', 1, 4, 33, 128, 128),
@@ -171,6 +179,8 @@ CASES = [
     case('deconv.dgrad', 1, 8, 32, 256, 128, act=2, aux_c0=128, aux_pitch=256),   # NT 128
     case('deconv.dgrad', 2, 8, 16, 160, 96),                                      # NT 32, 5 chunks of 32
     case('deconv.dgrad', 1, 24, 16, 512, 256, act=2),
+    case('deconv.dgrad', 1, 72, 176, 64, 96, act=2),                              # NT 32, 3 N blocks, 297 tiles
+    case('deconv.dgrad', 1, 136, 272, 64, 64, y_c0=64, y_pitch=128),              # NT 64, 289 tiles
     # --- conv3x3_wgrad_thin<NT, KC> ---
     case('conv.wgrad', 3, 36, 304, 32, 32),                                       # 285 tiles
     case('conv.wgrad', 3, 68, 272, 64, 32, x_c0=64, x_pitch=128),                 # 459 tiles
