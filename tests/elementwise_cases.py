@@ -1,6 +1,7 @@
 """Case tables of tests/test_elementwise_gpu.py and a restatement of the host dispatch of eld_isp_process,
 eld_eval_correct_psnr and eld_adam_step(_segments): which kernels a call launches and how often.
 tests/test_elementwise_ref_cpu.py checks that the tables reach every kernel and every dispatch branch."""
+import re
 from collections import namedtuple
 
 import numpy as np
@@ -196,3 +197,9 @@ def adam_dispatch(total, segments):
     if not segments:
         return {'adam_kernel': 1}
     return {'adam_segments_kernel': 1} if total else {}
+
+
+def canonical(demangled):
+    """a demangled kernel name (as the CUDA trace reports it) -> the form the dispatch restatements use, or None"""
+    m = re.search(r'(isp_kernel<(?:true|false)>|eval_\w+?_kernel|adam(?:_segments)?_kernel)', demangled)
+    return m.group(1) if m else None

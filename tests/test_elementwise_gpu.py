@@ -1,8 +1,8 @@
 """eld_isp_process, eld_eval_correct_psnr, eld_adam_step and eld_adam_step_segments against the float64 restatements of
 tests/elementwise_ref.py, called directly through ctypes so that pointers, offsets and aliasing are under the test's
 control.  The case tables (tests/elementwise_cases.py) reach every kernel and dispatch branch; each case traces its
-launches with torch.profiler and requires the kernel names and launch counts that elementwise_cases restates from the
-host side.  Every output is a view inside a larger allocation between guard regions filled with an fp32 NaN payload that
+launches and requires the kernel names and launch counts that elementwise_cases restates from the host side.  Every
+output is a view inside a larger allocation between guard regions filled with an fp32 NaN payload that
 must come back bit-identical; a misaligned case offsets its view.
 
 Rules
@@ -24,26 +24,20 @@ Gates: D and EPS are 4x the worst values measured on an H100 80GB HBM3 (SXM, 400
 DELTA_MEASURED and EPS_MEASURED.  The Adam parameter error is set by powf's rounding of beta2^step before the
 1 - beta2^step cancellation (1.9e-5 of the update at step 2); the moments stay within a few float32 roundings.  The ISP
 window needed at most 0.22 of its unit propagated bound.  The worst value per kernel and rule is printed at the end
-(pytest -s); the file runs in about 80 s there.
-
-Launch tracing: torch.profiler can lose kernel records - a whole trace, torch's own kernels included, in about 1 of
-100 traces on the H100, and at times for long stretches of a run - but never invents one.  So a trace that holds only
-part of the restated launches and nothing else is taken again from the same state (see _traced); a kernel the
-restatement does not name fails at once, and eld_launch_count must match on every attempt."""
+(pytest -s); the file runs in about 80 s there.  The guards, traces and refusals are tests/abi_harness.py's."""
 import ctypes
-import re
-from collections import Counter, defaultdict
+from collections import defaultdict
 
 import numpy as np
 import pytest
 
+from tests import abi_harness as H
 from tests import elementwise_cases as EC
 from tests import elementwise_ref as R
+from tests.abi_harness import Guarded
 
 pytestmark = pytest.mark.gpu
 
-NAN32 = 0x7FC0A5A5             # fp32 NaN with a payload: what no launch may write
-E_ARG = -1
 F = np.float32
 FP = ctypes.POINTER(ctypes.c_float)
 
@@ -58,16 +52,7 @@ EPS_MEASURED = {
 STATS = defaultdict(lambda: defaultdict(float))
 LR, B1, B2, ADAM_EPS = 1e-3, 0.9, 0.999, 1e-8
 
-
-@pytest.fixture(scope='module')
-def torch():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no GPU')
-    yield torch
-    print('\nworst case per kernel (isp D: least window constant; adam eps: max (|x-x64| - ulp) / S)')
-    for k in sorted(STATS):
-        print('  %-24s %s' % (k, '  '.join('%s=%.3g' % kv for kv in sorted(STATS[k].items()))))
+torch = H.torch_fixture(STATS, 'worst case per kernel (isp D: least window constant; adam eps: max (|x-x64| - ulp) / S)')
 
 
 def _L():
@@ -77,95 +62,6 @@ def _L():
 
 def _st(torch):
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-class Guarded:
-    """a float32 view of `numel` elements at element offset `off` inside an allocation with `guard` NAN32 words on
-    each side (guard a multiple of 4, so that the view's alignment is set by `off`)"""
-
-    def __init__(self, torch, numel, guard, off=0):
-        self.full = torch.full((guard + off + numel + guard,), NAN32, dtype=torch.int32, device='cuda')
-        self.lo, self.hi = guard + off, guard + off + numel
-        self.view = self.full[self.lo:self.hi].view(torch.float32)
-
-    def written_guards(self):
-        b = self.full
-        return int((b[:self.lo] != NAN32).sum().item()) + int((b[self.hi:] != NAN32).sum().item())
-
-    @property
-    def ptr(self):                                   # the view's address, also for an empty view (data_ptr() 0)
-        return self.full.data_ptr() + 4 * self.lo
-
-    def untouched(self):
-        return int((self.full != NAN32).sum().item()) == 0
-
-
-def _input(torch, arr, off):
-    """a float32 array at element offset `off` inside its own allocation -> (allocation, view)"""
-    flat = torch.from_numpy(np.ascontiguousarray(arr, F).reshape(-1))
-    buf = torch.zeros(off + flat.numel(), dtype=torch.float32, device='cuda')
-    buf[off:] = flat.cuda()
-    return buf, buf[off:]
-
-
-def canonical(name):
-    m = re.search(r'(isp_kernel<(?:true|false)>|eval_\w+?_kernel|adam(?:_segments)?_kernel)', name)
-    return m.group(1) if m else None
-
-
-TRACE_ATTEMPTS = 4
-# later in a long run the profiler drops the first kernel records of a trace, trace after trace (seen on the H100 for
-# the first launch of a call, whatever it was): a few of torch's own kernels go first, and the cached device memory is
-# handed back before each trace
-LEAD_IN = 8
-
-
-def _trace_once(torch, fn):
-    """-> (fn(), {kernel: launches} of the kernels in its trace, launches counted by eld_launch_count)"""
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    n0 = _L().launch_count(0)
-    torch.cuda.empty_cache()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        lead = torch.ones(LEAD_IN, device='cuda')
-        for _ in range(LEAD_IN):
-            lead.add_(1)
-        torch.cuda.synchronize()
-        rc = fn()
-        torch.cuda.synchronize()
-    got = Counter()
-    for e in prof.key_averages():
-        k = canonical(e.key)
-        if k is not None:
-            got[k] += e.count
-    return rc, dict(got), _L().launch_count(0) - n0
-
-
-def _traced(torch, fn, expect, where, state=()):
-    """fn() under torch.profiler, held to the restated dispatch: eld_launch_count moves by the launches `expect` lists,
-    and the trace names exactly those kernels, as often.  A trace can lose kernel records (on the H100 a whole trace in
-    about 1 of 100, sometimes for long stretches of a run) but never invents one: a trace that holds only part of the
-    expected launches and nothing else is taken again from the same state - the tensors in `state` are restored first -
-    up to TRACE_ATTEMPTS times.  A kernel the restatement does not name, or one launched too often, fails at once.
-    -> fn()'s return code (the launches are checked only when it is ELD_OK)"""
-    saved = [t.clone() for t in state]
-    for attempt in range(TRACE_ATTEMPTS):
-        if attempt:
-            for t, v in zip(state, saved):
-                t.copy_(v)
-            STATS['trace']['retaken'] += 1
-        rc, got, launched = _trace_once(torch, fn)
-        if rc != 0:
-            return rc
-        assert launched == sum(expect.values()), '%s: eld_launch_count moved by %d, the dispatch restatement says %s' % (
-            where, launched, expect)
-        assert all(v <= expect.get(k, 0) for k, v in got.items()), \
-            '%s: launched %s, the dispatch restatement says %s' % (where, got, expect)
-        if got == expect:
-            STATS['trace']['complete'] += 1
-            return rc
-    raise AssertionError('%s: %d traces in a row lost kernel records, the last one holds %s of %s' % (
-        where, TRACE_ATTEMPTS, got, expect))
 
 
 def _err(rc, where):
@@ -214,7 +110,7 @@ def run_isp(torch, c, x_dev=None, check=None):
     plane = h * w
     if x_dev is None:
         x, wb, ccm = EC.isp_inputs(c)
-        _, inp = _input(torch, x, c.offs[0])
+        _, inp = H.place(torch, x, c.offs[0])
     else:
         x = None
         _, wb, ccm = EC.isp_inputs(EC.Isp(n, 1, 1, (0, 0), c.gamma, None, 'range'))
@@ -223,8 +119,8 @@ def run_isp(torch, c, x_dev=None, check=None):
     out = Guarded(torch, n * 3 * plane, 4 * (plane + 1), c.offs[1])
     where = EC.isp_case_id(c)
     expect = EC.isp_dispatch(n, h, w, inp.data_ptr(), out.view.data_ptr())
-    rc = _traced(torch, lambda: _isp_call(torch, inp.data_ptr(), out.view.data_ptr(), n, h, w, wb, ccm, c.gamma, crf),
-                 expect, where)
+    rc = H.traced(torch, lambda: _isp_call(torch, inp.data_ptr(), out.view.data_ptr(), n, h, w, wb, ccm, c.gamma, crf),
+                  expect, where, EC.canonical, stats=STATS)
     assert rc == 0, _err(rc, where)
     assert out.written_guards() == 0, '%s: %d guard words written' % (where, out.written_guards())
     kern = next(iter(expect))
@@ -264,8 +160,8 @@ def test_isp_empty(torch, nhw):
     out = Guarded(torch, 64, 64)
     inp = torch.zeros(64, device='cuda')
     wb, ccm = np.ones((max(n, 1), 4), F), np.ones((max(n, 1), 9), F)
-    rc = _traced(torch, lambda: _isp_call(torch, inp.data_ptr(), out.view.data_ptr(), n, h, w, wb, ccm, 2.2, None), {},
-                 'n%d_h%d_w%d' % nhw)
+    rc = H.traced(torch, lambda: _isp_call(torch, inp.data_ptr(), out.view.data_ptr(), n, h, w, wb, ccm, 2.2, None), {},
+                  'n%d_h%d_w%d' % nhw, EC.canonical, stats=STATS)
     assert rc == 0 and out.untouched(), rc
 
 
@@ -310,8 +206,8 @@ def run_eval(torch, c, dev=None):
     where = EC.eval_case_id(c)
     if dev is None:
         pred, target = eval_inputs(c)
-        pbuf, p_in = _input(torch, pred, c.offs[0])
-        _, t_in = _input(torch, target, c.offs[1])
+        _, p_in = H.place(torch, pred, c.offs[0])
+        _, t_in = H.place(torch, target, c.offs[1])
     else:
         p_in, t_in = dev
         pred, target = None, None
@@ -323,10 +219,10 @@ def run_eval(torch, c, dev=None):
     pred_before = p_in.clone() if c.out == 'pred' else None
     t_before = t_in.clone() if dev is None else None
     out_ptr = out.view.data_ptr() if out is not None else p_in.data_ptr() if c.out == 'pred' else None
-    rc = _traced(torch, lambda: _eval_call(
+    rc = H.traced(torch, lambda: _eval_call(
         torch, p_in.data_ptr(), t_in.data_ptr(), out_ptr, n, pf, c.correct, scratch.data_ptr(), ps.view.data_ptr(),
-        gn.view.data_ptr() if gn is not None else None), EC.eval_dispatch(c.correct), where,
-        state=(p_in,) if c.out == 'pred' else ())
+        gn.view.data_ptr() if gn is not None else None), EC.eval_dispatch(c.correct), where, EC.canonical,
+        (p_in,) if c.out == 'pred' else (), STATS)
     assert rc == 0, _err(rc, where)
     for b, what in ((out, 'out'), (ps, 'psnr'), (gn, 'gain')):
         assert b is None or b.written_guards() == 0, '%s: %s guard words written' % (where, what)
@@ -482,9 +378,9 @@ def test_adam(torch, c):
     for b, a in zip(bufs, (p, g, m, v)):
         b.view.copy_(torch.from_numpy(a).cuda())
     where = EC.adam_case_id(c)
-    rc = _traced(torch, lambda: lib.eld_adam_step(
+    rc = H.traced(torch, lambda: lib.eld_adam_step(
         L.ctx(0), *[b.ptr for b in bufs], c.n, *_hyper(), c.wd, c.step, c.scale, _st(torch)),
-        EC.adam_dispatch(c.n, None), where, state=[bufs[i].full for i in (0, 2, 3)])
+        EC.adam_dispatch(c.n, None), where, EC.canonical, [bufs[i].full for i in (0, 2, 3)], STATS)
     assert rc == 0, _err(rc, where)
     assert all(b.written_guards() == 0 for b in bufs), '%s: guard words written' % where
     assert np.array_equal(bufs[1].view.cpu().numpy().view(np.int32), g.view(np.int32)), '%s: grads changed' % where
@@ -504,7 +400,7 @@ def test_adam_segments(torch, wd, scale):
     inside = np.zeros(length, bool)
     for off, cnt, _ in table:
         inside[off:off + cnt] = True
-    sentinel = np.full(length, NAN32, np.int32).view(F)
+    sentinel = np.full(length, H.NAN32, np.int32).view(F)
     p, m, v = (np.where(inside, a, sentinel) for a in (p, m, v))
     bufs = [Guarded(torch, length, 1024) for _ in range(4)]
     for b, a in zip(bufs, (p, g, m, v)):
@@ -512,9 +408,10 @@ def test_adam_segments(torch, wd, scale):
     segs = (ctypes.c_size_t * 128)(*[x for off, cnt, _ in table for x in (off, cnt)])
     steps = (ctypes.c_int * 64)(*[s for _, _, s in table])
     where = 'segments wd %g scale %g' % (wd, scale)
-    rc = _traced(torch, lambda: lib.eld_adam_step_segments(
+    rc = H.traced(torch, lambda: lib.eld_adam_step_segments(
         L.ctx(0), *[b.view.data_ptr() for b in bufs], segs, steps, 64, *_hyper(), wd, scale, _st(torch)),
-        EC.adam_dispatch(sum(c for _, c, _ in table), table), where, state=[bufs[i].full for i in (0, 2, 3)])
+        EC.adam_dispatch(sum(c for _, c, _ in table), table), where, EC.canonical, [bufs[i].full for i in (0, 2, 3)],
+        STATS)
     assert rc == 0, _err(rc, where)
     assert all(b.written_guards() == 0 for b in bufs), '%s: guard words written' % where
     got = [bufs[i].view.cpu().numpy() for i in (0, 2, 3)]
@@ -533,8 +430,9 @@ def test_adam_segments_empty(torch):
     bufs = [Guarded(torch, 16, 64) for _ in range(4)]
     segs = (ctypes.c_size_t * 4)(3, 0, 9, 0)
     steps = (ctypes.c_int * 2)(1, 2)
-    rc = _traced(torch, lambda: lib.eld_adam_step_segments(
-        L.ctx(0), *[b.view.data_ptr() for b in bufs], segs, steps, 2, *_hyper(), 0.0, 1.0, _st(torch)), {}, 'empty ranges')
+    rc = H.traced(torch, lambda: lib.eld_adam_step_segments(
+        L.ctx(0), *[b.view.data_ptr() for b in bufs], segs, steps, 2, *_hyper(), 0.0, 1.0, _st(torch)), {}, 'empty ranges',
+        EC.canonical, stats=STATS)
     assert rc == 0 and all(b.untouched() for b in bufs)
 
 
@@ -548,11 +446,6 @@ SEG_REFUSALS = ['ctx', 'params', 'grads', 'm', 'v', 'segs', 'steps', 'step=0', '
                 'same offset']
 
 
-def _refused(torch, where, rc, launched, names, untouched):
-    assert rc == E_ARG and launched == 0 and not names and all(untouched), \
-        '%s: rc %d, %d launches (traced: %s), untouched %s' % (where, rc, launched, names, untouched)
-
-
 @pytest.mark.parametrize('what', ISP_REFUSALS)
 def test_isp_refused(torch, what):
     n, h, w = 3, 8, 8
@@ -561,7 +454,6 @@ def test_isp_refused(torch, what):
     x = np.random.RandomState(1).rand(n * 4 * plane).astype(F)
     packed = big.view[n * 3 * plane:n * 7 * plane]
     packed.copy_(torch.from_numpy(x).cuda())
-    before = big.full.clone()
     pp = packed.data_ptr()
     rp = {'rgb=packed': pp, 'rgb in packed': pp + 4 * (n * 4 * plane - 5),             # rgb starts inside packed
           'packed in rgb': big.view[1:].data_ptr()}.get(what, big.view[n * 7 * plane:].data_ptr())   # ends inside it
@@ -575,11 +467,11 @@ def test_isp_refused(torch, what):
               'gamma<0': dict(gamma=-2.2), 'gamma=nan': dict(gamma=float('nan')), 'crf_len=1': dict(L=1),
               'crf_len<0': dict(L=-4), 'crf_E': dict(E=None), 'crf_f': dict(f=None)}.get(what, {}))
     lib, L = _L().load(), _L()
-    rc, names, launched = _trace_once(torch, lambda: lib.eld_isp_process(
+    H.refused(torch, what, lambda: lib.eld_isp_process(
         None if what == 'ctx' else L.ctx(0), None if what == 'packed' else pp, None if what == 'rgb' else rp,
         a['n'], a['h'], a['w'], None if what == 'wb' else wb.ctypes.data_as(FP),
-        None if what == 'ccm' else ccm.ctypes.data_as(FP), a['gamma'], a['E'], a['f'], a['L'], _st(torch)))
-    _refused(torch, what, rc, launched, names, [torch.equal(big.full, before)])
+        None if what == 'ccm' else ccm.ctypes.data_as(FP), a['gamma'], a['E'], a['f'], a['L'], _st(torch)),
+        EC.canonical, big.full)
 
 
 @pytest.mark.parametrize('what', EVAL_REFUSALS)
@@ -588,20 +480,17 @@ def test_eval_refused(torch, what):
     buf = Guarded(torch, 3 * n * pf, 64)                          # pred, target, out side by side
     src = np.random.RandomState(2).rand(2 * n * pf).astype(F)
     buf.view[:2 * n * pf].copy_(torch.from_numpy(src).cuda())
-    before = buf.full.clone()
     pred, target, out = buf.view[:n * pf], buf.view[n * pf:2 * n * pf], buf.view[2 * n * pf:]
     op = {'out=target': target.data_ptr(), 'out in target': target.data_ptr() + 4 * (n * pf // 2),
           'out in pred': pred.data_ptr() + 4}.get(what, out.data_ptr())
     ps, gn = Guarded(torch, n, 64), Guarded(torch, n, 64)
     scratch = Guarded(torch, 8 * n, 64)
     lib, L = _L().load(), _L()
-    rc, names, launched = _trace_once(torch, lambda: lib.eld_eval_correct_psnr(
+    H.refused(torch, what, lambda: lib.eld_eval_correct_psnr(
         None if what == 'ctx' else L.ctx(0), None if what == 'pred' else pred.data_ptr(),
         None if what == 'target' else target.data_ptr(), op, 0 if what == 'n=0' else n, 0 if what == 'per_frame=0' else pf,
         1, None if what == 'scratch' else scratch.view.data_ptr(), None if what == 'psnr' else ps.view.data_ptr(),
-        gn.view.data_ptr(), _st(torch)))
-    _refused(torch, what, rc, launched, names, [torch.equal(buf.full, before), ps.untouched(), gn.untouched(),
-                                         scratch.untouched()])
+        gn.view.data_ptr(), _st(torch)), EC.canonical, buf.full, ps.full, gn.full, scratch.full)
 
 
 @pytest.mark.parametrize('what', ADAM_REFUSALS)
@@ -611,9 +500,9 @@ def test_adam_refused(torch, what):
     ptrs = [None if what == k else b.view.data_ptr() for k, b in zip(('params', 'grads', 'm', 'v'), bufs)]
     step = {'step=0': 0, 'step<0': -3}.get(what, 1)
     lib, L = _L().load(), _L()
-    rc, names, launched = _trace_once(torch, lambda: lib.eld_adam_step(
-        None if what == 'ctx' else L.ctx(0), *ptrs, n, *_hyper(), 0.0, step, 1.0, _st(torch)))
-    _refused(torch, what, rc, launched, names, [b.untouched() for b in bufs])
+    H.refused(torch, what, lambda: lib.eld_adam_step(
+        None if what == 'ctx' else L.ctx(0), *ptrs, n, *_hyper(), 0.0, step, 1.0, _st(torch)), EC.canonical,
+        *[b.full for b in bufs])
 
 
 @pytest.mark.parametrize('what', SEG_REFUSALS)
@@ -639,7 +528,6 @@ def test_adam_segments_refused(torch, what):
     segs = (ctypes.c_size_t * (2 * k))(*[x for off, cnt, _ in table for x in (off, cnt)])
     steps = (ctypes.c_int * k)(*[s for _, _, s in table])
     lib, L = _L().load(), _L()
-    rc, names, launched = _trace_once(torch, lambda: lib.eld_adam_step_segments(
+    H.refused(torch, what, lambda: lib.eld_adam_step_segments(
         None if what == 'ctx' else L.ctx(0), *ptrs, None if what == 'segs' else segs, None if what == 'steps' else steps,
-        k, *_hyper(), 0.0, 1.0, _st(torch)))
-    _refused(torch, what, rc, launched, names, [b.untouched() for b in bufs])
+        k, *_hyper(), 0.0, 1.0, _st(torch)), EC.canonical, *[b.full for b in bufs])

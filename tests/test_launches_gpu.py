@@ -395,6 +395,17 @@ def test_train_step_launches(torch, case):
     st.check(names)
 
 
+@pytest.mark.parametrize('frozen', [False, True], ids=['split-store', 'row-prefix'])
+def test_wide_tile_engine_concat_gradients(torch, frozen):
+    """one training step of a single 384 x 256 frame (the 1/16-resolution level has 3 pixel tiles per N tile): every
+    launch against its float64 reference, among them the concat dgrads of conv6_1 .. conv8_1 through the wide tile -
+    split stores into the planar concat gradients, or with the encoder frozen the row-prefix dgrads whose skip planes
+    must keep their NaN payload"""
+    st, names = _train(torch, 1, 4, 4, 384, 256, 'l1', ENC if frozen else ())
+    assert {'conv6_1.dgrad', 'conv7_1.dgrad', 'conv8_1.dgrad'} <= set(names)
+    st.check(names)
+
+
 def test_autograd_seam_launches_with_input_grad(torch):
     """eld_unet_forward + eld_unet_backward (the head's dOut-in mode) + eld_unet_input_grad (conv1_1's data gradient)"""
     from eld_b200 import _lib

@@ -1,8 +1,8 @@
 """The four noise entry points of the C ABI (eld_noise_packed, eld_noise_mosaic, eld_noise_packed_u16,
 eld_noise_packed_aug) against the float64 reference of tests/noise_ref.py, called directly through ctypes so that
 pointers, offsets and in-place aliasing are under the test's control.  The case table (tests/noise_cases.py) reaches
-all 25 kernel instantiations; each case also traces its launches with torch.profiler and requires the kernel name and
-template arguments that noise_cases.kernel() derives from the host dispatch.
+all 25 kernel instantiations; each call also traces its launches and requires the kernel name and template arguments
+that noise_cases.kernel() derives from the host dispatch, as often as noise_cases.launches() says.
 
 Every output is a view inside a larger allocation, between guard regions of one frame or more filled with an fp32 NaN
 payload that must come back bit-identical; a misaligned case offsets its view inside that allocation.
@@ -21,20 +21,20 @@ Gates: EPS is 4x the worst value measured per instantiation on an H100 80GB HBM3
 EPS_MEASURED: 2.8e-8 (Poisson, P only) to 5.7e-6 (the generic and aug kernels), and 2.9e-5 for vec<p|g> over the
 520-frame batch, whose 2M checked pixels reach Box-Muller radii closer to zero.  For comparison, test_noise_gpu.py
 allows 1e-3 of the total noise sigma.  No Poisson pixel left the rule there.  The file runs in about 25 s, 9 s of it
-the 520-frame batch.  The worst case per instantiation is printed at the end (pytest -s)."""
+the 520-frame batch.  The worst case per instantiation is printed at the end (pytest -s).  The guards, traces and
+refusals are tests/abi_harness.py's."""
 import ctypes
 from collections import defaultdict
 
 import numpy as np
 import pytest
 
+from tests import abi_harness as H
 from tests import noise_cases as T
 from tests import noise_ref as N
+from tests.abi_harness import Guarded
 
 pytestmark = pytest.mark.gpu
-
-NAN32 = 0x7FC0A5A5             # fp32 NaN with a payload: what no launch may write
-E_ARG = -1
 
 # worst max over elements of (|got - r| - ulp(r)) / S per instantiation, measured on the H100 over this file; the gate
 # EPS is 4x.  The largest values come from Box-Muller radii near zero (lg2.approx near u = 1): the generic kernel and
@@ -76,15 +76,8 @@ def EPS(kern):
     return 4 * EPS_MEASURED[kern]
 
 
-@pytest.fixture(scope='module')
-def torch():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no GPU')
-    yield torch
-    print('\nworst case per instantiation (eps: max (|got-r| - ulp) / S; mismatch: Poisson share off the rule)')
-    for k in sorted(STATS):
-        print('  %-46s %s' % (k, '  '.join('%s=%.3g' % kv for kv in sorted(STATS[k].items()))))
+torch = H.torch_fixture(STATS, 'worst case per instantiation (eps: max (|got-r| - ulp) / S; '
+                               'mismatch: Poisson share off the rule)')
 
 
 def _lib():
@@ -95,31 +88,6 @@ def _lib():
 def _params(plist):
     from eld_b200.noise import params_array
     return params_array(plist)
-
-
-class Guarded:
-    """a float32 view of `numel` elements at element offset `off` inside an allocation with `guard` NAN32 words on
-    each side"""
-
-    def __init__(self, torch, numel, guard, off=0):
-        self.full = torch.full((guard + off + numel + guard,), NAN32, dtype=torch.int32, device='cuda')
-        self.lo, self.hi = guard + off, guard + off + numel
-        self.view = self.full[self.lo:self.hi].view(torch.float32)
-
-    def written_guards(self):
-        b = self.full
-        return int((b[:self.lo] != NAN32).sum().item()) + int((b[self.hi:] != NAN32).sum().item())
-
-    def untouched(self):
-        return int((self.full != NAN32).sum().item()) == 0
-
-
-def _input(torch, arr, off):
-    """the input array at element offset `off` inside its own allocation"""
-    flat = torch.from_numpy(np.ascontiguousarray(arr).reshape(-1).view(np.int16 if arr.dtype == np.uint16 else arr.dtype))
-    buf = torch.zeros(off + flat.numel(), dtype=flat.dtype, device='cuda')
-    buf[off:] = flat.cuda()
-    return buf, buf[off:]
 
 
 def _call(torch, entry, inp, out, aux, n, h, w, plist, mask, seed, fid0, clip, dtype=1, black=0.0, white=1.0,
@@ -136,29 +104,6 @@ def _call(torch, entry, inp, out, aux, n, h, w, plist, mask, seed, fid0, clip, d
         return lib.eld_noise_packed_u16(L.ctx(0), inp, scale, out, aux, n, h, w, pa, mask, seed, fid0, clip, st)
     fl = None if flags is None else flags.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8))
     return lib.eld_noise_packed_aug(L.ctx(0), inp, out, aux, n, h, w, pa, mask, seed, fid0, clip, fl, st)
-
-
-TRACE_ATTEMPTS = 4
-# later in a long run the profiler drops the first kernel records of a trace, trace after trace (seen on the H100 for
-# the first launch of a call, whatever it was): a few of torch's own kernels go first, and the cached device memory is
-# handed back before each trace
-LEAD_IN = 8
-
-
-def _traced(torch, fn):
-    """-> (fn(), canonical names of the noise kernels it launched)"""
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    torch.cuda.empty_cache()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        lead = torch.ones(LEAD_IN, device='cuda')
-        for _ in range(LEAD_IN):
-            lead.add_(1)
-        torch.cuda.synchronize()
-        rc = fn()
-        torch.cuda.synchronize()
-    names = {T.canonical(e.key) for e in prof.key_averages() if 'noise_' in e.key}
-    return rc, names - {None}
 
 
 def _rule(kern, where, got, r, S, r0, clip, poisson, prm, mask):
@@ -215,24 +160,13 @@ def run_case(torch, oracle, c):
         out.view.copy_(torch.from_numpy(src.reshape(-1)).cuda())
         inp = out.view
     else:
-        _, inp = _input(torch, src, c.offs[0])
+        _, inp = H.place(torch, src, c.offs[0])
     flags = np.asarray(c.aug, np.uint8) if c.aug is not None else None
-    # torch.profiler can lose a trace's kernel records (about 1 trace in 100 on the H100) but never invents one: a trace
-    # that names no noise kernel is taken again, the in-place input restored first; a wrong kernel fails at once
-    for attempt in range(TRACE_ATTEMPTS):
-        if attempt and c.inplace:
-            out.view.copy_(torch.from_numpy(src.reshape(-1)).cuda())
-        n0 = _lib().launch_count(0)
-        rc, names = _traced(torch, lambda: _call(
-            torch, c.entry, inp.data_ptr(), out.view.data_ptr(), aux.view.data_ptr() if aux else None, n, h, w, plist,
-            c.mask, c.seed, c.fid0, c.clip, dtype=0 if c.dtype == 'u16' else 1, black=c.black, white=c.white,
-            scale=c.scale, flags=flags))
-        assert rc == 0, '%s: rc %d: %s' % (where, rc, _lib().load().eld_last_error())
-        assert names <= {kern}, '%s: launched %s, the dispatch restatement says %s' % (where, sorted(names), kern)
-        assert _lib().launch_count(0) - n0 == T.launches(c), where
-        if names:
-            break
-    assert names == {kern}, '%s: %d traces in a row lost their kernel records' % (where, TRACE_ATTEMPTS)
+    rc = H.traced(torch, lambda: _call(
+        torch, c.entry, inp.data_ptr(), out.view.data_ptr(), aux.view.data_ptr() if aux else None, n, h, w, plist,
+        c.mask, c.seed, c.fid0, c.clip, dtype=0 if c.dtype == 'u16' else 1, black=c.black, white=c.white,
+        scale=c.scale, flags=flags), {kern: T.launches(c)}, where, T.canonical, (out.view,) if c.inplace else (), STATS)
+    assert rc == 0, '%s: rc %d: %s' % (where, rc, _lib().load().eld_last_error())
     assert out.written_guards() == 0, '%s: %d output guard words written' % (where, out.written_guards())
     if aux is not None:
         assert aux.written_guards() == 0, '%s: %d clean_out / target_out guard words written' % (where, aux.written_guards())
@@ -241,8 +175,11 @@ def run_case(torch, oracle, c):
         # the same stream without the index map, checked against the reference, then the map bit for bit
         plain = Guarded(torch, total, guard)
         clean_t = torch.from_numpy(y.reshape(-1)).cuda()
-        assert _call(torch, 'packed', clean_t.data_ptr(), plain.view.data_ptr(), None, n, h, w, plist, c.mask, c.seed,
-                     c.fid0, c.clip) == 0
+        packed = c._replace(entry='packed', offs=(0, 0, 0), aug=None)
+        assert H.traced(torch, lambda: _call(torch, 'packed', clean_t.data_ptr(), plain.view.data_ptr(), None, n, h, w,
+                                             plist, c.mask, c.seed, c.fid0, c.clip),
+                        {T.kernel(packed)[0]: T.launches(packed)}, where + ' (eld_noise_packed)', T.canonical,
+                        stats=STATS) == 0
         pl = plain.view.cpu().numpy().reshape(n, 4, h, w)
         _check_frames(c, kern, where + ' (eld_noise_packed)', pl, y, plist, oracle)
         gt = aux.view.cpu().numpy().reshape(n, 4, h, w) if aux is not None else None
@@ -298,8 +235,7 @@ def test_refused(torch, what):
         src = rs.randint(0, 65536, size=(n, 4, h, w)).astype(np.uint16)
     else:
         src = rs.rand(n, 4, h, w).astype(np.float32)
-    ibuf, inp = _input(torch, src, a['offs'][0])
-    before = ibuf.clone()
+    ibuf, inp = H.place(torch, src, a['offs'][0])
     out = Guarded(torch, total, 64, a['offs'][1])
     aux = Guarded(torch, total, 64, a['offs'][2])
     flags = np.asarray(T.aug_flags(n), np.uint8) & 3
@@ -311,13 +247,8 @@ def test_refused(torch, what):
         out_ptr = inp.data_ptr()
     if a['inplace'] == 'target':
         aux_ptr = inp.data_ptr()
-    n0 = _lib().launch_count(0)
-    rc = _call(torch, entry, inp.data_ptr(), out_ptr, aux_ptr, a['n'], h, w, plist, a['mask'], a['seed'], a['fid0'],
-               a['clip'], dtype=a['dtype_code'], black=a['black'], white=a['white'], scale=1.0 / 65535.0,
-               flags=None if a['null'] == 'flags' else flags, H=2 * h + 1 if a['H_odd'] else None,
-               W=2 * w + 1 if a['W_odd'] else None)
-    torch.cuda.synchronize()
-    launched = _lib().launch_count(0) - n0
-    assert rc == E_ARG and launched == 0 and out.untouched() and aux.untouched() and torch.equal(ibuf, before), \
-        '%s: rc %d, %d launches, output untouched %s, aux untouched %s, input untouched %s' % (
-            what, rc, launched, out.untouched(), aux.untouched(), torch.equal(ibuf, before))
+    H.refused(torch, what, lambda: _call(
+        torch, entry, inp.data_ptr(), out_ptr, aux_ptr, a['n'], h, w, plist, a['mask'], a['seed'], a['fid0'], a['clip'],
+        dtype=a['dtype_code'], black=a['black'], white=a['white'], scale=1.0 / 65535.0,
+        flags=None if a['null'] == 'flags' else flags, H=2 * h + 1 if a['H_odd'] else None,
+        W=2 * w + 1 if a['W_odd'] else None), T.canonical, ibuf, out.full, aux.full)

@@ -33,6 +33,25 @@ def test_dispatch_restatement():
     assert T.tiles(T.case('deconv', 1, 8, 16, 64, 64)) == 2
 
 
+def test_canonical_names():
+    """the demangled names of the CUDA trace in kernel()'s form; anything else is not a tile kernel"""
+    assert T.canonical('void eld::conv3x3_wide_kernel<128, 64>(CUtensorMap_st, eld::ConvGemmParams)') == \
+        'conv3x3_wide<128,64>'
+    assert T.canonical('eld::conv3x3_thin_kernel<(int)32, (int)64>(CUtensorMap_st, eld::ConvGemmParams)') == \
+        'conv3x3_thin<32,64>'
+    assert T.canonical('void eld::conv3x3_wgrad_thin_kernel<64, 32>(CUtensorMap_st, CUtensorMap_st, '
+                       'eld::WgradThinParams)') == 'conv3x3_wgrad_thin<64,32>'
+    assert T.canonical('void eld::conv_gemm_kernel<128>(CUtensorMap_st, eld::ConvGemmParams)') == 'conv_gemm<128>'
+    assert T.canonical('void eld::wgrad_gemm_kernel<32>(CUtensorMap_st, CUtensorMap_st, eld::WgradParams)') == \
+        'wgrad_gemm<32>'
+    assert T.canonical('eld::pack_weights_kernel(float const*, __nv_bfloat16*, int, int, int)') == 'pack_weights_kernel'
+    for other in ('void eld::first_conv_kernel<false>(CUtensorMap_st, CUtensorMap_st, eld::FirstConvParams)',
+                  'void at::native::vectorized_elementwise_kernel<4, at::native::FillFunctor<float>, '
+                  'std::array<char*, 1ul> >(int, at::native::FillFunctor<float>, std::array<char*, 1ul>)',
+                  'void eld::noise_packed_generic_kernel(float const*, float*, eld::NoiseLaunch)'):
+        assert T.canonical(other) is None, other
+
+
 def test_cases_reach_every_instantiation():
     reached = {T.kernel(c)[0] for c in T.CASES}
     assert set(THIN + WIDE + WGRAD_THIN + GENERIC + WGRAD_GENERIC) == reached, reached
@@ -53,6 +72,20 @@ def test_every_instantiation_outnumbers_the_sms():
     """an odd tile count above 2 x 132, not a multiple of 132, for every instantiation"""
     for name in THIN + WIDE + WGRAD_THIN + GENERIC + WGRAD_GENERIC:
         assert any(T.kernel(c)[0] == name and T.many_tiles(c, T.SMS_H100) for c in T.CASES), name
+
+
+def test_wide_tile_cases():
+    """the wide tile meets an odd tile count within one round of SMs and one above two rounds, several channel chunks
+    at both kc, and four (N = 512) and three (N = 96) N tiles"""
+    wide = [c for c in T.CASES if T.kernel(c)[0].startswith('conv3x3_wide<')]
+    assert {(T.kernel(c)[1]['kc'], T.kernel(c)[1]['chunks'] > 1) for c in wide} >= {(32, True), (64, True)}
+    assert any(T.tiles(c) % 2 and T.tiles(c) < T.SMS_H100 for c in wide)
+    assert any(T.many_tiles(c, T.SMS_H100) for c in wide)
+    assert {c.co for c in wide} >= {512, 96}
+
+
+def test_case_ids_are_distinct():
+    assert len({T.case_id(c) for c in T.CASES}) == len(T.CASES)
 
 
 def test_cases_cover_partial_tiles_offsets_and_options():

@@ -7,14 +7,16 @@ than two rounds of SMs, partial 8 x 16 tiles (H % 8 in {1, 3, 4, 7}, W % 16 in {
 offsets and pitches on every operand, and batches whose odd images hold values 1000x larger than their neighbours (a
 halo row read from the wrong image is a large error).  Every output is a slice of a larger allocation: the guard image
 before and after it and the channels outside its range hold a bf16 NaN payload and must come back bit-identical; a
-weight gradient accumulates into a non-zero dW between two fp32 NaN guards.
+weight gradient accumulates into a non-zero dW between two fp32 NaN guards.  Every primitive call is traced and must
+launch the one kernel that tile_cases.kernel() names, so each case is judged by the gate of the kernel that ran
+(tests/abi_harness.py holds the guards, traces and refusals).
 
 Acceptance, the rules of test_launches_gpu.py:
   bf16  every element |got - r| <= ulp_bf16(r) + 2^-20 S (r = the float64 value before the kernel's single rounding,
         S = the same sum over |terms|), and at most MISMATCH[kernel] of the elements differ from round-to-nearest(r).
   fp32  (weight gradients) rel-L2 vs float64 <= WGRAD_REL_L2[kernel] and max |got - r| <= WGRAD_MAX_ABS[kernel] max|r|.
   exact the thin 3x3 tile equals the first N block of the generic tile bit for bit; eld_pack_weights equals the Python
-        restatement of packed_index bit for bit; a refused call writes nothing.
+        restatement of packed_index bit for bit; a refused call writes nothing and launches nothing.
 The gates are about 4x the worst case measured on an H100 80GB HBM3 (SXM, 132 SMs) at its 700 W power limit over this
 file and test_conv_gpu.py: a max |got-r| / (ulp + 2^-20 S) of 0.5 for every kernel (the final rounding alone); mismatch
 shares of 1.8e-4 to 4.3e-4 for the thin tiles, 4.3e-4 / 7.9e-4 / 2.8e-3 for the wide and deconv tiles of N tile 32 /
@@ -25,7 +27,9 @@ from collections import defaultdict
 
 import pytest
 
+from tests import abi_harness as H
 from tests import tile_cases as T
+from tests.abi_harness import NAN16, Guarded
 
 pytestmark = pytest.mark.gpu
 
@@ -39,22 +43,12 @@ WGRAD_REL_L2 = {'conv3x3_wgrad_thin<32,32>': 1.2e-6, 'conv3x3_wgrad_thin<32,64>'
 WGRAD_MAX_ABS = {'conv3x3_wgrad_thin<32,32>': 3.2e-6, 'conv3x3_wgrad_thin<32,64>': 2.3e-6,
                  'conv3x3_wgrad_thin<64,32>': 3e-6, 'conv3x3_wgrad_thin<64,64>': 2.9e-6,
                  'wgrad_gemm<32>': 2.4e-6, 'wgrad_gemm<64>': 1.7e-6, 'wgrad_gemm<128>': 1.3e-6}
-NAN16 = 0x7FA5                 # bf16 NaN with a payload: what no launch may write
-NAN32 = 0x7FC0A5A5             # its fp32 counterpart around a weight gradient
 BIG = 1000.0                   # scale of the odd images
 
 STATS = defaultdict(lambda: defaultdict(float))     # kernel -> worst measured value per statistic
 
-
-@pytest.fixture(scope='module')
-def torch():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no GPU')
-    yield torch
-    print('\nworst case per kernel (bf16: max |got-r| / (ulp + 2^-20 S), mismatch rate; fp32: rel-L2, max-abs / max|r|)')
-    for k in sorted(STATS):
-        print('  %-28s %s' % (k, '  '.join('%s=%.3g' % kv for kv in sorted(STATS[k].items()))))
+torch = H.torch_fixture(STATS, 'worst case per kernel (bf16: max |got-r| / (ulp + 2^-20 S), mismatch rate; '
+                               'fp32: rel-L2, max-abs / max|r|)')
 
 
 def _sms(torch):
@@ -68,18 +62,29 @@ def _operand(torch, g, n, h, w, pitch, big_odd=True):
     return (torch.randn(n, h, w, pitch, device='cuda', generator=g) * scale).bfloat16()
 
 
-def _guarded(torch, n, h, w, pitch):
-    """(the whole allocation [n+2,h,w,pitch] filled with NAN16, the output view = images 1..n)"""
-    full = torch.full((n + 2, h, w, pitch), NAN16, dtype=torch.int16, device='cuda').view(torch.bfloat16)
-    return full, full[1:n + 1]
+def _output(torch, n, h, w, pitch):
+    """bf16 NHWC [n,h,w,pitch] between two guard images of NAN16 -> (its Guarded allocation, the output tensor)"""
+    out = Guarded(torch, n * h * w * pitch, h * w * pitch, dtype=torch.bfloat16)
+    return out, out.view.view(n, h, w, pitch)
 
 
-def _untouched(torch, full, c0=None, c=None):
-    """bits of `full` that are not images 1..n, channels [c0, c0 + c) still NAN16 -> number of elements that are not"""
-    b = full.view(torch.int16).clone()
-    if c0 is not None:
-        b[1:-1, ..., c0:c0 + c] = NAN16
-    return int((b != NAN16).sum().item())
+def _written(torch, out, y, c0, c):
+    """elements written outside channels [c0, c0 + c) of the output y: in the guard images and in y's other channels"""
+    b = y.view(torch.int16).clone()
+    b[..., c0:c0 + c] = NAN16
+    return out.written_guards() + int((b != NAN16).sum().item())
+
+
+def _prims_traced(torch, call, expect, where, state=()):
+    """call(), an eld_b200.prims wrapper (it raises EldError where the C call fails), held to the launches `expect` by
+    abi_harness.traced -> what call() returned"""
+    got = []
+
+    def fn():
+        got.append(call())
+        return 0
+    H.traced(torch, fn, expect, where, T.canonical, state, STATS)
+    return got[-1]
 
 
 def _bf16_check(kernel, where, got, r, S):
@@ -103,7 +108,7 @@ def _f32_check(kernel, where, got, r, S):
 
 
 def run_case(torch, c, seed):
-    """one primitive call of case c, checked against its float64 reference and its guards"""
+    """one primitive call of case c, traced, then checked against its float64 reference and its guards"""
     from eld_b200 import prims
     import tests.launch_ref as R
     g = torch.Generator(device='cuda').manual_seed(seed)
@@ -116,51 +121,49 @@ def run_case(torch, c, seed):
         # the second operand is large on the EVEN images: a product across an image border is BIG^2
         q = _operand(torch, g, c.n, f * c.h, f * c.w, c.y_pitch, big_odd=False)
         xs, qs = x[..., c.x_c0:c.x_c0 + c.ci], q[..., c.y_c0:c.y_c0 + c.co]
-        if fine:
-            r, S, _, _ = R.deconv_wgrad(xs, qs)
-        else:
-            r, S, _, _ = R.conv_wgrad(xs, qs)
+        r, S, _, _ = (R.deconv_wgrad if fine else R.conv_wgrad)(xs, qs)
         dw0 = torch.randn(r.shape, device='cuda', generator=g) * r.abs().max().float()
-        k, G = r.numel(), 256
-        full = torch.full((k + 2 * G,), NAN32, dtype=torch.int32, device='cuda').view(torch.float32)
-        dw = full[G:G + k].view(r.shape)
+        out = Guarded(torch, r.numel(), 256)
+        dw = out.view.view(r.shape)
         dw.copy_(dw0)
-        if fine:
-            prims.deconv2x2_wgrad(x, c.x_c0, c.ci, q, c.y_c0, c.co, dw)
-        else:
-            prims.conv3x3_wgrad(x, c.x_c0, c.ci, q, c.y_c0, c.co, dw)
-        guard = full.view(torch.int32)
-        assert (guard[:G] == NAN32).all() and (guard[G + k:] == NAN32).all(), '%s: dW guard written' % where
+        wgrad = prims.deconv2x2_wgrad if fine else prims.conv3x3_wgrad
+        _prims_traced(torch, lambda: wgrad(x, c.x_c0, c.ci, q, c.y_c0, c.co, dw), {kern: 1}, where, state=(dw,))
+        assert out.written_guards() == 0, '%s: dW guard written' % where
         _f32_check(kern, where, dw, r + dw0.double(), S + dw0.double().abs())
         return
     ih, iw = (2 * c.h, 2 * c.w) if c.op == 'deconv.dgrad' else (c.h, c.w)
     oh, ow = (2 * c.h, 2 * c.w) if c.op == 'deconv' else (c.h, c.w)
     x = _operand(torch, g, c.n, ih, iw, c.x_pitch)
     xs = x[..., c.x_c0:c.x_c0 + c.ci]
-    full, y = _guarded(torch, c.n, oh, ow, c.y_pitch)
+    out, y = _output(torch, c.n, oh, ow, c.y_pitch)
     aux = _operand(torch, g, c.n, c.h, c.w, c.aux_pitch) if c.act == prims.ACT_MASK else None
     auxs = aux[..., c.aux_c0:c.aux_c0 + c.co] if aux is not None else None
     if c.op == 'conv':
         W = torch.randn(c.co, c.ci, 3, 3, device='cuda', generator=g) / (3 * c.ci ** 0.5)
         b = torch.randn(c.co, device='cuda', generator=g) if c.bias else None
-        prims.conv3x3(x, c.x_c0, c.ci, prims.pack_weights(W, prims.PACK_CONV_FPROP), b, y, c.y_c0, c.co, act=c.act)
+        wp = prims.pack_weights(W, prims.PACK_CONV_FPROP)
+        call = lambda: prims.conv3x3(x, c.x_c0, c.ci, wp, b, y, c.y_c0, c.co, act=c.act)  # noqa: E731
         r, S = R.conv_fprop(xs, W, b, act=c.act == prims.ACT_LRELU)
     elif c.op == 'conv.dgrad':
         W = torch.randn(c.ci, c.co, 3, 3, device='cuda', generator=g) / (3 * c.ci ** 0.5)
-        prims.conv3x3(x, c.x_c0, c.ci, prims.pack_weights(W, prims.PACK_CONV_DGRAD), None, y, c.y_c0, c.co, act=c.act,
-                      aux=aux, aux_c0=c.aux_c0)
+        wp = prims.pack_weights(W, prims.PACK_CONV_DGRAD)
+        call = lambda: prims.conv3x3(x, c.x_c0, c.ci, wp, None, y, c.y_c0, c.co, act=c.act, aux=aux,  # noqa: E731
+                                     aux_c0=c.aux_c0)
         r, S = R.conv_dgrad(xs, W, auxs)
     elif c.op == 'deconv':
         Wt = torch.randn(c.ci, c.co, 2, 2, device='cuda', generator=g) / c.ci ** 0.5
         b = torch.randn(c.co, device='cuda', generator=g) if c.bias else None
-        prims.deconv2x2(x, c.x_c0, c.ci, prims.pack_weights(Wt, prims.PACK_DECONV_FPROP), b, y, c.y_c0, c.co)
+        wp = prims.pack_weights(Wt, prims.PACK_DECONV_FPROP)
+        call = lambda: prims.deconv2x2(x, c.x_c0, c.ci, wp, b, y, c.y_c0, c.co)  # noqa: E731
         r, S = R.deconv_fprop(xs, Wt, b)
     else:
         Wt = torch.randn(c.co, c.ci, 2, 2, device='cuda', generator=g) / c.ci ** 0.5
-        prims.deconv2x2_dgrad(x, c.x_c0, c.ci, prims.pack_weights(Wt, prims.PACK_DECONV_DGRAD), y, c.y_c0, c.co,
-                              act=c.act, aux=aux, aux_c0=c.aux_c0)
+        wp = prims.pack_weights(Wt, prims.PACK_DECONV_DGRAD)
+        call = lambda: prims.deconv2x2_dgrad(x, c.x_c0, c.ci, wp, y, c.y_c0, c.co, act=c.act, aux=aux,  # noqa: E731
+                                             aux_c0=c.aux_c0)
         r, S = R.deconv_dgrad(xs, Wt, auxs)
-    bad = _untouched(torch, full, c.y_c0, c.co)
+    _prims_traced(torch, call, {kern: 1}, where)
+    bad = _written(torch, out, y, c.y_c0, c.co)
     assert bad == 0, '%s: %d guard elements written' % (where, bad)
     _bf16_check(kern, where, y[..., c.y_c0:c.y_c0 + c.co], r, S)
 
@@ -187,8 +190,6 @@ def test_thin_tile_equals_generic_tile_bitwise(torch, case):
     from eld_b200 import prims
     op, n, h, w, ci, co = case
     wide = 96 if co == 32 else 192
-    assert T.kernel(T.case(op, n, h, w, ci, co))[0] == 'conv3x3_thin<%d,%d>' % (co, ci)
-    assert T.kernel(T.case(op, n, h, w, ci, wide))[0] == 'conv3x3_wide<%d,%d>' % (co, ci)
     g = torch.Generator(device='cuda').manual_seed(7)
     x = _operand(torch, g, n, h, w, ci)
     y_thin = torch.empty(n, h, w, co, device='cuda', dtype=torch.bfloat16)
@@ -196,16 +197,18 @@ def test_thin_tile_equals_generic_tile_bitwise(torch, case):
     if op == 'conv':
         W = torch.randn(wide, ci, 3, 3, device='cuda', generator=g) / (3 * ci ** 0.5)
         b = torch.randn(wide, device='cuda', generator=g)
-        prims.conv3x3(x, 0, ci, prims.pack_weights(W[:co], prims.PACK_CONV_FPROP), b[:co].contiguous(), y_thin, 0, co,
-                      act=prims.ACT_LRELU)
-        prims.conv3x3(x, 0, ci, prims.pack_weights(W, prims.PACK_CONV_FPROP), b, y_wide, 0, wide, act=prims.ACT_LRELU)
+        packs = [prims.pack_weights(W[:co], prims.PACK_CONV_FPROP), prims.pack_weights(W, prims.PACK_CONV_FPROP)]
+        biases = [b[:co].contiguous(), b]
+        kw = dict(act=prims.ACT_LRELU)
     else:
         W = torch.randn(ci, wide, 3, 3, device='cuda', generator=g) / (3 * ci ** 0.5)
         aux = _operand(torch, g, n, h, w, wide)
-        prims.conv3x3(x, 0, ci, prims.pack_weights(W[:, :co], prims.PACK_CONV_DGRAD), None, y_thin, 0, co,
-                      act=prims.ACT_MASK, aux=aux, aux_c0=0)
-        prims.conv3x3(x, 0, ci, prims.pack_weights(W, prims.PACK_CONV_DGRAD), None, y_wide, 0, wide,
-                      act=prims.ACT_MASK, aux=aux, aux_c0=0)
+        packs = [prims.pack_weights(W[:, :co], prims.PACK_CONV_DGRAD), prims.pack_weights(W, prims.PACK_CONV_DGRAD)]
+        biases = [None, None]
+        kw = dict(act=prims.ACT_MASK, aux=aux, aux_c0=0)
+    for tile, wp, bias, y, cout in zip(('thin', 'wide'), packs, biases, (y_thin, y_wide), (co, wide)):
+        _prims_traced(torch, lambda: prims.conv3x3(x, 0, ci, wp, bias, y, 0, cout, **kw),
+                {'conv3x3_%s<%d,%d>' % (tile, co, ci): 1}, '%s %s tile' % (case, tile))
     a, b_ = y_thin.view(torch.int16), y_wide[..., :co].contiguous().view(torch.int16)
     diff = int((a != b_).sum().item())
     STATS['exact thin vs generic']['elements'] += a.numel()
@@ -224,31 +227,45 @@ def test_pack_weights_matches_packed_index(torch, shape):
     kind, cout, cin = shape
     g = torch.Generator(device='cuda').manual_seed(3)
     W = torch.randn(*((cout, cin, 3, 3) if kind < 2 else (cin, cout, 2, 2)), device='cuda', generator=g)
-    got = prims.pack_weights(W, kind).reshape(-1)
+    got = _prims_traced(torch, lambda: prims.pack_weights(W, kind), {'pack_weights_kernel': 1}, 'kind%d-%dx%d' % shape)
+    got = got.reshape(-1)
     src, dst = T.pack_order(kind, cout, cin)
     want = torch.empty_like(got)
     want[torch.from_numpy(dst).cuda()] = W.reshape(-1)[torch.from_numpy(src).cuda()].bfloat16()
     assert torch.equal(got.view(torch.int16), want.view(torch.int16))
 
 
-# ---- the contract: right, or refused with nothing written --------------------------------------------------------------
+@pytest.mark.parametrize('op', ['conv', 'conv.dgrad'])
+def test_wide_tile_repeats_bitwise(torch, op):
+    """the tile has no atomics and a fixed K order: the same call twice gives the same bits"""
+    from eld_b200 import prims
+    n, h, w, ci, co = 2, 19, 45, 256, 256
+    g = torch.Generator(device='cuda').manual_seed(11)
+    x = _operand(torch, g, n, h, w, ci)
+    ys = []
+    if op == 'conv':
+        W = torch.randn(co, ci, 3, 3, device='cuda', generator=g) / (3 * ci ** 0.5)
+        b = torch.randn(co, device='cuda', generator=g)
+        wp = prims.pack_weights(W, prims.PACK_CONV_FPROP)
+    else:
+        W = torch.randn(ci, co, 3, 3, device='cuda', generator=g) / (3 * ci ** 0.5)
+        aux = _operand(torch, g, n, h, w, co)
+        wp = prims.pack_weights(W, prims.PACK_CONV_DGRAD)
+    for _ in range(2):
+        out, y = _output(torch, n, h, w, co)
+        if op == 'conv':
+            prims.conv3x3(x, 0, ci, wp, b, y, 0, co, act=prims.ACT_LRELU)
+        else:
+            prims.conv3x3(x, 0, ci, wp, None, y, 0, co, act=prims.ACT_MASK, aux=aux, aux_c0=0)
+        assert _written(torch, out, y, 0, co) == 0
+        assert not (y.view(torch.int16) == NAN16).any()
+        ys.append(y.clone())
+    assert torch.equal(ys[0].view(torch.int16), ys[1].view(torch.int16))
+
+
+# ---- the contract: right, or refused with nothing written and nothing launched -----------------------------------------
 def _refused(torch, what, call, *guards):
-    """call() must raise EldError and leave every guard tensor (filled with NAN16 or NAN32) untouched; a guard is a
-    tensor or a (name, tensor) pair"""
-    from eld_b200 import _lib
-    raised = False
-    try:
-        call()
-    except _lib.EldError:
-        raised = True
-    torch.cuda.synchronize()
-    written = []
-    for i, t in enumerate(guards):
-        name, t = t if isinstance(t, tuple) else ('guard %d' % i, t)
-        bits = t.view(torch.int16 if t.element_size() == 2 else torch.int32)
-        written.append((name, int((bits != (NAN16 if t.element_size() == 2 else NAN32)).sum().item())))
-    assert raised and not any(k for _, k in written), '%s: %s; elements written: %s' % (
-        what, 'accepted' if not raised else 'refused', ', '.join('%s %d' % nk for nk in written))
+    H.refused(torch, what, call, T.canonical, *guards)
 
 
 @pytest.mark.parametrize('shape', [(0, 384, 32), (0, 320, 64), (1, 32, 384), (2, 96, 32), (3, 32, 320), (0, 48, 32),
@@ -265,10 +282,10 @@ def test_pack_refuses_partial_256_row_blocks(torch, shape):
     buf = torch.full((padded,), NAN16, dtype=torch.int16, device='cuda')
     W = torch.randn(*((cout, cin, 3, 3) if kind < 2 else (cin, cout, 2, 2)), device='cuda')
     lib = _lib.load()
-    _refused(torch, 'eld_pack_weights(kind %d, cout %d, cin %d): %d rows, operand %d elements' % (kind, cout, cin, rows, exact),
-             lambda: _lib.check(lib.eld_pack_weights(_lib.ctx(0), W.data_ptr(), buf.data_ptr(), cout, cin, kind,
-                                                     prims._st()), 'eld_pack_weights'),
-             ('in the operand', buf[:exact]), ('past its end', buf[exact:]))
+    _refused(torch, 'eld_pack_weights(kind %d, cout %d, cin %d): %d rows, operand %d elements (guard 0), padded '
+             'to %d (guard 1)' % (kind, cout, cin, rows, exact, padded),
+             lambda: lib.eld_pack_weights(_lib.ctx(0), W.data_ptr(), buf.data_ptr(), cout, cin, kind, prims._st()),
+             buf[:exact], buf[exact:])
 
 
 @pytest.mark.parametrize('cout', [8, 16, 96])
@@ -280,9 +297,9 @@ def test_deconv_refuses_cout_the_shuffle_cannot_store(torch, cout):
     Wt = torch.randn(cin, cout, 2, 2, device='cuda')
     wp = prims.pack_weights(Wt, prims.PACK_DECONV_FPROP) if cout != 96 else torch.zeros(4 * 256 * cin, device='cuda').bfloat16()
     b = torch.randn(cout, device='cuda')
-    full, y = _guarded(torch, n, 2 * h, 2 * w, 64)
+    out, y = _output(torch, n, 2 * h, 2 * w, 64)
     _refused(torch, 'eld_deconv2x2_bf16(cin %d, cout %d, y pitch 64)' % (cin, cout),
-             lambda: prims.deconv2x2(x, 0, cin, wp, b, y, 0, cout), full)
+             lambda: prims.deconv2x2(x, 0, cin, wp, b, y, 0, cout), out.full)
 
 
 def _conv_call(torch, n=1, h=8, w=16, ci=32, co=32, x_pitch=None, x_c0=0, y_pitch=None, y_c0=0, y_offset=0, act=0,
@@ -331,10 +348,10 @@ def test_deconv_dgrad_refuses_partial_tiles(torch, hw):
     Wt = torch.randn(cin, cout, 2, 2, device='cuda')
     dy = torch.randn(1, 2 * h, 2 * w, cout, device='cuda').bfloat16()
     aux = torch.randn(1, h, w, cin, device='cuda').bfloat16()
-    full, dx = _guarded(torch, 1, h, w, cin)
+    wp = prims.pack_weights(Wt, prims.PACK_DECONV_DGRAD)
+    out, dx = _output(torch, 1, h, w, cin)
     _refused(torch, 'eld_deconv2x2_dgrad_bf16 at %d x %d' % (h, w),
-             lambda: prims.deconv2x2_dgrad(dy, 0, cout, prims.pack_weights(Wt, prims.PACK_DECONV_DGRAD), dx, 0, cin,
-                                           act=prims.ACT_MASK, aux=aux), full)
+             lambda: prims.deconv2x2_dgrad(dy, 0, cout, wp, dx, 0, cin, act=prims.ACT_MASK, aux=aux), out.full)
 
 
 @pytest.mark.parametrize('shape', [(6, 16, 32, 32), (8, 24, 64, 64), (8, 16, 48, 32), (8, 16, 32, 40)],
@@ -346,9 +363,9 @@ def test_wgrad_refuses(torch, shape):
     x = torch.randn(1, h, w, cin, device='cuda').bfloat16()
     dz = torch.randn(1, h, w, cout, device='cuda').bfloat16()
     dy = torch.randn(1, 2 * h, 2 * w, cout, device='cuda').bfloat16()
-    dw = torch.full((cout * cin * 9,), NAN32, dtype=torch.int32, device='cuda').view(torch.float32)
+    dw = torch.full((cout * cin * 9,), H.NAN32, dtype=torch.int32, device='cuda').view(torch.float32)
     _refused(torch, 'eld_conv3x3_wgrad_bf16 %s' % (shape,),
              lambda: prims.conv3x3_wgrad(x, 0, cin, dz, 0, cout, dw.view(cout, cin, 3, 3)), dw)
-    dwt = torch.full((cin * cout * 4,), NAN32, dtype=torch.int32, device='cuda').view(torch.float32)
+    dwt = torch.full((cin * cout * 4,), H.NAN32, dtype=torch.int32, device='cuda').view(torch.float32)
     _refused(torch, 'eld_deconv2x2_wgrad_bf16 %s' % (shape,),
              lambda: prims.deconv2x2_wgrad(x, 0, cin, dy, 0, cout, dwt.view(cin, cout, 2, 2)), dwt)

@@ -16,6 +16,7 @@ channels per tap) and `co` the count it WRITES (or, for a weight gradient, the c
   conv.wgrad    x [n,h,w,ci], dz [n,h,w,co] -> dW OIHW [co][ci][3][3]
   deconv.wgrad  x [n,h,w,ci], dy [n,2h,2w,co] -> dWt IOHW [ci][co][2][2]
 (h, w) is always the grid the primitive is called with (the coarse one for the deconvolutions)."""
+import re
 from collections import namedtuple
 
 import numpy as np
@@ -77,6 +78,15 @@ def kernel(c):
             return 'conv3x3_thin<%d,%d>' % (n, k), {}
         return 'conv3x3_wide<%d,%d>' % (n_tile(n), kc), {'kc': kc, 'chunks': k // kc}
     return 'conv_gemm<%d>' % n_tile(n), {'kc': kc, 'chunks': k // kc, 'a_mode': a_mode, 'epi': epi}
+
+
+def canonical(demangled):
+    """a demangled kernel name (as the CUDA trace reports it) -> the form kernel() returns, 'pack_weights_kernel', or
+    None for a kernel that is not one of these: eld::conv3x3_wide_kernel<128, 64>(...) -> conv3x3_wide<128,64>"""
+    m = re.search(r'\b(conv3x3_thin|conv3x3_wide|conv3x3_wgrad_thin|conv_gemm|wgrad_gemm)_kernel<([^>]*)>', demangled)
+    if m is not None:
+        return '%s<%s>' % (m.group(1), ','.join(re.findall(r'\d+', re.sub(r'\([^)]*\)', ' ', m.group(2)))))
+    return 'pack_weights_kernel' if re.search(r'\bpack_weights_kernel\b', demangled) else None
 
 
 def tiles(c):
@@ -198,6 +208,27 @@ CASES = [
     case('deconv.wgrad', 1, 12, 32, 64, 96, x_c0=32, x_pitch=96),                 # M = 4 taps x 96 channels
     case('deconv.wgrad', 2, 8, 16, 128, 64),
     case('deconv.wgrad', 1, 8, 16, 512, 256),
+    # --- the wide tile: odd tile counts in one round of SMs (9 tiles) and in several (289), channel chunks of 32 and of
+    # 64 with partial border tiles, N = 512 (four N tiles across two 256-row operand blocks) and N = 96 (three) ---
+    case('conv', 1, 20, 40, 128, 128, act=1),                                     # 2 chunks of 64, 9 tiles
+    case('conv.dgrad', 1, 20, 44, 128, 128, act=2),                               # 9 tiles
+    case('conv', 1, 135, 263, 128, 128, act=1, x_c0=64, x_pitch=256, y_c0=128, y_pitch=384),   # 289 tiles
+    case('conv.dgrad', 1, 135, 263, 256, 128, act=2, aux_c0=32, aux_pitch=256),   # 4 chunks, 289 tiles
+    case('conv', 2, 21, 45, 96, 64, act=1),                                       # 3 chunks of 32
+    case('conv.dgrad', 1, 27, 77, 160, 128, act=2),                               # 5 chunks of 32
+    case('conv', 1, 30, 50, 192, 128, x_c0=64, x_pitch=256),                      # 3 chunks of 64
+    case('conv', 1, 21, 45, 64, 512),                                             # 9 pixel tiles x 4 N tiles
+    case('conv.dgrad', 1, 21, 45, 256, 512, act=2),
+    case('conv', 2, 11, 37, 128, 96, act=1),
+    case('conv.dgrad', 2, 11, 37, 64, 96, act=2),
+    # --- the thin weight-gradient tile: heights with a half tile at the bottom (h % 8 == 4, zero-filled rows), channel
+    # offsets on both operands, and more tiles than SMs, so that every CTA sums an uneven run of several tiles ---
+    case('conv.wgrad', 2, 12, 48, 32, 32),
+    case('conv.wgrad', 1, 20, 32, 64, 64, y_c0=64),
+    case('conv.wgrad', 3, 36, 16, 32, 64, x_c0=32, x_pitch=96),
+    case('conv.wgrad', 1, 44, 64, 64, 32, x_c0=64, y_c0=32),
+    case('conv.wgrad', 2, 132, 144, 64, 64),
+    case('conv.wgrad', 3, 100, 112, 32, 32, x_c0=32),
 ]
 
 # thin tile vs the first N block of the generic tile: (op, n, h, w, ci, co) of the thin call; the generic call appends
