@@ -104,6 +104,7 @@ class _EngineFunction(torch.autograd.Function):
         x = ctx.saved_tensors[0]                 # raises if x or a parameter was changed in place since the forward
         need = ctx.needs_input_grad[2:]          # frozen parameters: no weight-gradient launch, None returned
         net._set_trainable(eng[0], need, ctx.needs_input_grad[1])
+        net.join_allreduce()                     # autograd accumulates into .grad = flat_grads: after any pending exchange
         state = ctx.state
         if state is None and not eng.holds(ctx.claim):
             state = net._new_state(x)
@@ -288,10 +289,12 @@ class UNetSeeInDark(nn.Module):
         """forward + pixel loss + backward in one launch sequence.  Fills self.flat_grads (== every trainable
         parameter's .grad) and returns (out, loss) with loss a 0-dim cuda tensor (no host sync).  Parameters with
         requires_grad == False are frozen: no gradient is computed for them, their .grad is None and their range of
-        flat_grads reads zero."""
+        flat_grads reads zero.  An exchange an earlier train_step_ddp left in flight is joined first (a stream wait): the
+        step's memset and weight-gradient writes must not race with its all-reduces."""
         n, _, h, w = x.shape
         assert x.is_cuda and x.dtype == torch.float32 and x.shape[1] == self.in_channels
         assert target.shape == (n, self.out_channels, h, w) and target.dtype == torch.float32
+        self.join_allreduce()
         x, target = x.contiguous(), target.contiguous()
         out = torch.empty_like(target)
         loss = loss_out if loss_out is not None else torch.empty((), dtype=torch.float32, device=x.device)
@@ -318,8 +321,10 @@ class UNetSeeInDark(nn.Module):
     def train_step_ddp(self, x, target, loss_out=None, group=None, timeline=None):
         """train_step + SUM all-reduce of the flat gradient, bucket by bucket on a side stream: bucket k's NCCL kernel
         waits only for the event the engine records when that bucket is final, so the decoder and bottleneck
-        gradients travel while the encoder's backward still runs; the calling stream waits for all buckets at the end
-        (Adam follows).  No host synchronisation."""
+        gradients travel while the encoder's backward still runs.  The all-reduces are left in flight
+        (_pending_allreduce): the next FusedAdam.step joins them bucket by bucket, or the next train_step, autograd
+        backward or zero_grad joins them all, whichever comes first, so a step that skips the optimizer (a non-finite
+        loss) or a plain step after this one never races with the exchange.  No host synchronisation."""
         import torch.distributed as dist
         n, _, h, w = x.shape
         eng = self._engine(n, h, w, True)
@@ -485,6 +490,7 @@ class FusedAdam(torch.optim.Optimizer):
             adam(0, p.numel())
 
     def zero_grad(self, set_to_none=False):
+        self.net.join_allreduce()
         self.net.flat_grads.zero_()
 
     # checkpoint format of torch.optim.Adam ('opt_g' in ELD_model.py:516-523): per-parameter step; a parameter that has

@@ -5,6 +5,7 @@ import os
 import sys
 
 import numpy as np
+import pytest
 import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
@@ -94,3 +95,41 @@ def test_bucketed_allreduce_equals_one_allreduce(tmp_path):
     mp.spawn(_bucket_worker, args=(2, port, out), nprocs=2, join=True)
     r = torch.load(out, weights_only=False)
     assert r['same'] and r['all'] and r['k'] == 4
+
+
+@pytest.mark.parametrize('cin,cout', [(3, 3), (3, 4), (4, 3), (4, 4)])
+def test_grad_buckets_io_tile_the_flat_gradient(cin, cout):
+    """eld_unet_grad_buckets_io for every (in, out) channel pair the network takes: four contiguous ranges that cover the
+    flat gradient of that network exactly once, starting at upv6, conv5_1, conv2_1 and conv1_1 (backward-completion
+    order).  A bucket table of the 4 -> 4 network used for a 3-channel one misses or overlaps parameters."""
+    import ctypes as c
+    from eld_b200 import _lib
+    lib = _lib.load()
+    arr = (c.c_size_t * 8)()
+    assert lib.eld_unet_grad_buckets_io(cin, cout, arr, 8) == 4
+    b = [(int(arr[2 * i]), int(arr[2 * i + 1])) for i in range(4)]
+    n = lib.eld_unet_param_count_io(cin, cout)
+    cover = np.zeros(n, np.int32)
+    for off, cnt in b:
+        assert cnt > 0 and off + cnt <= n, (off, cnt, n)
+        cover[off:off + cnt] += 1
+    assert (cover == 1).all()
+    off, cnt = c.c_size_t(), c.c_size_t()
+    for (start, _), first in zip(b, (b'upv6', b'conv5_1', b'conv2_1', b'conv1_1')):
+        assert lib.eld_unet_param_offset_io(first, 0, cin, cout, c.byref(off), c.byref(cnt)) == 0
+        assert start == off.value, (first, start, off.value)
+    # the ranges end where the next one in state_dict order starts: the decoder bucket ends at the buffer's end
+    assert b[0][0] + b[0][1] == n and b[1][0] + b[1][1] == b[0][0] and b[2][0] + b[2][1] == b[1][0]
+    assert b[3][0] == 0 and b[3][1] == b[2][0]
+
+
+def test_grad_buckets_io_refusals():
+    import ctypes as c
+    from eld_b200 import _lib
+    lib = _lib.load()
+    arr = (c.c_size_t * 8)(*([12345] * 8))
+    assert lib.eld_unet_grad_buckets_io(3, 9, arr, 8) != 0            # 9-channel (X-Trans) frames are not taken
+    assert lib.eld_unet_grad_buckets_io(9, 4, arr, 8) != 0
+    assert lib.eld_unet_grad_buckets_io(4, 4, arr, 7) != 0            # room for fewer than 4 (offset, count) pairs
+    assert list(arr) == [12345] * 8                                   # a refused call writes nothing
+    assert lib.eld_unet_grad_buckets_io(4, 4, None, 0) == 4           # no array: only the bucket count

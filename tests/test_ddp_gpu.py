@@ -1,7 +1,7 @@
 """The data-parallel step on ONE GPU (NCCL group of world size 1): the engine's per-bucket path - a layout permute and an
 event per gradient bucket, all-reduces on the side stream, Adam in two launches - must leave the same gradients and the
-same updated weights as the plain step (SURVEY 8e; the N > 1 exchange itself is covered by tests/test_ddp_cpu.py on gloo
-and by tools/ddp_timeline.py on real GPUs)."""
+same updated weights as the plain step (SURVEY 8e; the exchange at world size 2 is held to the per-rank plain steps in
+tests/test_ddp_world2_gpu.py)."""
 import os
 
 import pytest
