@@ -1,23 +1,17 @@
 """The first cases the wgmma conv / deconv primitives were tested at, judged by the float64 references and rules of
-tests/test_tiles_gpu.py (run_case): the same bf16 operands, every bf16 element within ulp_bf16(r) + 2^-20 S plus a bounded
-share off round-to-nearest(r), weight gradients by rel-L2 and max-abs, guards around every output."""
+tests/test_tiles_gpu.py (tests/tile_check.py's run_case): the same bf16 operands, every bf16 element within
+ulp_bf16(r) + 2^-20 S plus a bounded share off round-to-nearest(r), weight gradients by rel-L2 and max-abs, guards
+around every output."""
 import pytest
 
 from tests import tile_cases as T
+from tests.engine_harness import torch  # noqa: F401 (the fixture)
+from tests.tile_check import run_case
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope='module')
-def torch():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no GPU')
-    return torch
-
-
 def _run(torch, c, case):
-    from tests.test_tiles_gpu import run_case
     run_case(torch, c, hash(case) % 2 ** 31)
 
 

@@ -6,6 +6,8 @@ import os
 
 import pytest
 
+from tests import engine_harness as E
+
 pytestmark = pytest.mark.gpu
 
 
@@ -20,8 +22,7 @@ def test_bucketed_step_equals_plain_step_world1():
     dist.init_process_group('nccl', init_method='tcp://127.0.0.1:%d' % port, rank=0, world_size=1,
                             device_id=torch.device('cuda', 0))
     try:
-        torch.manual_seed(2018)
-        net = arch.unet(4, 4).cuda()
+        net = E.net()
         opt = arch.FusedAdam(net, lr=1e-4)
         p0 = net.flat_params.clone()
         x = torch.rand(2, 4, 128, 256, device='cuda')

@@ -32,7 +32,7 @@ Gates, per step:
             three plain runs (the fp32-atomics noise of t); a tensor without atomics agrees to one rounding.
   lockstep  R, flat_params, m and v bitwise identical on both ranks.
   Adam      every trainable element of p, m and v within ulp(x64) + EPS S of tests/elementwise_ref.adam (float64,
-            scale 1/2) applied to the step's start state and R; EPS is 4x test_elementwise_gpu.EPS_MEASURED of the kernel
+            scale 1/2) applied to the step's start state and R; EPS is 4x elementwise_cases.EPS_MEASURED of the kernel
             FusedAdam dispatched.  An element updated twice or not at all is off by about S.
   frozen    frozen ranges of flat_params, m, v and the step counts bitwise unchanged, of R exactly zero; all-reduces
             issued for the live buckets only, in backward-completion order.
@@ -331,7 +331,7 @@ def _exchange(where, meta, R, gs, spreads):
 def _adam(where, meta, pre, R, post, scale):
     """Adam on the trainable elements against float64; frozen ranges and step counts untouched"""
     from tests import elementwise_ref as ER
-    from tests.test_elementwise_gpu import EPS_MEASURED
+    from tests.elementwise_cases import EPS_MEASURED
     flags, spans = meta['flags'], meta['spans']
     counts = [n for _, n in spans]
     mask = np.repeat(np.array(flags), counts)
@@ -420,7 +420,7 @@ def _sd_equal(a, b):
 def _check_model(torch, tmp, got):
     from eld_b200 import models
     from eld_b200.noise import NoiseModel
-    from tests.test_launches_gpu import WGRAD_REL_L2
+    from tests.launch_check import WGRAD_REL_L2
     r0, r1 = got
     assert r0['world'] == r1['world'] == 2
     meta = r0['meta']

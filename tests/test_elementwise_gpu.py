@@ -21,7 +21,7 @@ Rules
   refused ELD_E_ARG, nothing written (outputs, inputs, guards) and eld_launch_count unchanged.
 
 Gates: D and EPS are 4x the worst values measured on an H100 80GB HBM3 (SXM, 400 W power limit), listed in
-DELTA_MEASURED and EPS_MEASURED.  The Adam parameter error is set by powf's rounding of beta2^step before the
+DELTA_MEASURED and elementwise_cases.EPS_MEASURED.  The Adam parameter error is set by powf's rounding of beta2^step before the
 1 - beta2^step cancellation (1.9e-5 of the update at step 2); the moments stay within a few float32 roundings.  The ISP
 window needed at most 0.22 of its unit propagated bound.  The worst value per kernel and rule is printed at the end
 (pytest -s); the file runs in about 80 s there.  The guards, traces and refusals are tests/abi_harness.py's."""
@@ -44,11 +44,6 @@ FP = ctypes.POINTER(ctypes.c_float)
 # worst least window constant (elementwise_ref.isp_need) per kernel, measured on the H100 over this file; the gate is 4x
 # (both instantiations run the same arithmetic; the vectorised one met the larger value and it stands for both)
 DELTA_MEASURED = {'isp_kernel<true>': 0.218, 'isp_kernel<false>': 0.218}
-# worst max (|x - x64| - ulp(x64)) / S per kernel and quantity, measured on the H100 over this file; the gate is 4x
-EPS_MEASURED = {
-    'adam_kernel': {'p': 1.86e-5, 'm': 6.65e-8, 'v': 1.61e-7},
-    'adam_segments_kernel': {'p': 2.95e-6, 'm': 5.78e-8, 'v': 1.36e-7},
-}
 STATS = defaultdict(lambda: defaultdict(float))
 LR, B1, B2, ADAM_EPS = 1e-3, 0.9, 0.999, 1e-8
 
@@ -346,7 +341,7 @@ def _adam_state(rs, n, kind):
 def _adam_rule(kern, where, got, ref, scales):
     st = STATS[kern]
     for q, x, x64, S in zip('pmv', got, ref, scales):
-        eps = 4 * EPS_MEASURED[kern][q]
+        eps = 4 * EC.EPS_MEASURED[kern][q]
         d = np.abs(x.astype(np.float64) - x64)
         need = np.maximum(d - R.ulp32(x64), 0) / np.maximum(S, 1e-300)
         st['eps ' + q] = max(st['eps ' + q], float(need.max(initial=0)))

@@ -10,52 +10,11 @@ import ctypes
 
 import pytest
 
+from tests import engine_harness as E
+from tests.engine_harness import AUTOGRAD, ENC, FWD_NAMES, TRAIN_STEP, torch  # noqa: F401 (torch: the fixture)
+
 pytestmark = pytest.mark.gpu
 H, W = 128, 256
-ENC = ('conv1_1', 'conv1_2', 'conv2_1', 'conv2_2', 'conv3_1', 'conv3_2', 'conv4_1', 'conv4_2', 'conv5_1', 'conv5_2')
-_FWD = ['weights.pack'] + ['%s.fprop' % n for n in ENC] + [
-    'upv6.fprop', 'conv6_1.fprop', 'conv6_2.fprop', 'upv7.fprop', 'conv7_1.fprop', 'conv7_2.fprop',
-    'upv8.fprop', 'conv8_1.fprop', 'conv8_2.fprop', 'upv9.fprop', 'conv9_1.fprop', 'conv9_2.fprop']
-_BWD = []
-for _c in '9876':
-    _BWD += ['conv%s_2.wgrad' % _c, 'conv%s_2.dgrad' % _c, 'conv%s_1.wgrad' % _c, 'conv%s_1.dgrad' % _c,
-             'upv%s.wgrad' % _c, 'upv%s.dgrad' % _c]
-_BWD += ['conv5_2.wgrad', 'conv5_2.dgrad', 'conv5_1.wgrad', 'conv5_1.dgrad', 'pool.bwd']
-for _c in '432':
-    _BWD += ['conv%s_2.wgrad' % _c, 'conv%s_2.dgrad' % _c, 'conv%s_1.wgrad' % _c, 'conv%s_1.dgrad' % _c, 'pool.bwd']
-_BWD += ['conv1_2.wgrad', 'conv1_2.dgrad', 'conv1_1.wgrad', 'weights.gperm']
-# the per-launch profile of one fused train step and of one autograd forward + backward (x without grad), as the engine
-# has issued them since the single-GPU permute became one launch
-TRAIN_STEP = _FWD + ['conv10_1.fwd+loss+bwd'] + _BWD
-AUTOGRAD = _FWD + ['conv10_1.fprop', 'conv10_1.bwd'] + _BWD
-
-
-@pytest.fixture(scope='module')
-def torch():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no GPU')
-    return torch
-
-
-def _rel(a, b):
-    return ((a.double() - b.double()).norm() / (b.double().norm() + 1e-30)).item()
-
-
-def _net(torch, cin=4, cout=4):
-    from eld_b200 import arch
-    torch.manual_seed(2018)
-    return arch.unet(cin, cout).cuda()
-
-
-def _inputs(torch, n, h, w, seed):
-    g = torch.Generator().manual_seed(seed)
-    return torch.rand(n, 4, h, w, generator=g).cuda(), torch.rand(n, 4, h, w, generator=g).cuda()
-
-
-def _freeze(net, frozen_layers):
-    for name, p in net.named_parameters():
-        p.requires_grad_(name.split('.')[0] not in frozen_layers)
 
 
 def _decoder(net):
@@ -63,12 +22,12 @@ def _decoder(net):
 
 
 def _train_names(net, x, t):
-    return [r['name'] for r in net.profile(x, t, steps=1)]
+    return E.launch_names(net, net._engine(x.shape[0], x.shape[2], x.shape[3], True), lambda: net.train_step(x, t))
 
 
 def _autograd_names(torch, net, x, t):
     eng = net._engine(x.shape[0], x.shape[2], x.shape[3], True)
-    return [r['name'] for r in net._profile(eng, lambda: torch.nn.functional.l1_loss(net(x), t).backward(), 1)]
+    return E.launch_names(net, eng, lambda: torch.nn.functional.l1_loss(net(x), t).backward())
 
 
 def _grads(net):
@@ -76,65 +35,46 @@ def _grads(net):
     return {k: net.flat_grads[o:o + n].clone() for (k, _), (o, n) in zip(net.named_parameters(), net._spans)}
 
 
-def _set(lib, net, eng, flags, input_grad):
-    from eld_b200 import _lib
-    arr = (ctypes.c_uint8 * len(flags))(*flags)
-    _lib.check(lib.eld_unet_set_trainable(eng, arr, len(flags), input_grad), 'eld_unet_set_trainable')
-    net._masks[eng.value] = (tuple(bool(f) for f in flags), bool(input_grad))    # keep the module's cache truthful
-
-
-def _abi_train_names(torch, net, eng, x, t):
-    """profile of eld_unet_train_step called directly (the engine keeps whatever eld_unet_set_trainable gave it)"""
-    from eld_b200 import _lib
-    lib, out, loss = _lib.load(), torch.empty_like(t), torch.zeros((), device='cuda')
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    run = lambda: _lib.check(lib.eld_unet_train_step(eng, net.flat_params.data_ptr(), x.data_ptr(), t.data_ptr(),
-                                                     out.data_ptr(), net.flat_grads.data_ptr(), loss.data_ptr(), st),
-                             'eld_unet_train_step')
-    return [r['name'] for r in net._profile(eng, run, 1)]
-
-
-def _without(names, frozen_layers, drop=()):
-    """names minus the weight / data gradients of the frozen layers and minus `drop`"""
-    return [n for n in names if n not in drop and not (n.split('.')[0] in frozen_layers and n.split('.')[1] in ('wgrad', 'dgrad'))]
+def _abi_train_names(net, eng, x, t):
+    """profile of eld_unet_train_step called directly"""
+    return E.launch_names(net, eng, E.abi_train_step(net, eng, x, t))
 
 
 def test_default_launches_and_values_unchanged(torch):
-    from eld_b200 import _lib
-    net, lib = _net(torch), _lib.load()
-    x, t = _inputs(torch, 2, H, W, seed=1)
+    net = E.net()
+    x, t = E.frames(2, 4, 4, H, W, seed=1)
     eng = net._engine(2, H, W, True)
     xg = x.clone().requires_grad_()
-    before = (_abi_train_names(torch, net, eng, x, t), _train_names(net, x, t), _autograd_names(torch, net, x, t),
+    before = (_abi_train_names(net, eng, x, t), _train_names(net, x, t), _autograd_names(torch, net, x, t),
               _autograd_names(torch, net, xg, t))
     assert before == (TRAIN_STEP, TRAIN_STEP, AUTOGRAD, AUTOGRAD + ['conv1_1.dgrad'])
     o0, l0 = net.train_step(x, t)
     o0, l0, g0 = o0.clone(), l0.clone(), net.flat_grads.clone()
-    _set(lib, net, eng, [1] * 46, 1)
-    assert _abi_train_names(torch, net, eng, x, t) == TRAIN_STEP
+    E.set_trainable(net, eng, [1] * 46, 1)
+    assert _abi_train_names(net, eng, x, t) == TRAIN_STEP
     assert _autograd_names(torch, net, xg, t) == AUTOGRAD + ['conv1_1.dgrad']      # the mask x.grad asks for: no call
     assert _train_names(net, x, t) == TRAIN_STEP
     o1, l1 = net.train_step(x, t)
     assert torch.equal(o1, o0) and abs(l1.item() - l0.item()) <= 1e-6 * l0.item()
-    assert _rel(net.flat_grads, g0) <= 1e-4
+    assert E.rel(net.flat_grads, g0) <= 1e-4
 
 
 @pytest.mark.parametrize('shape', [(2, 128, 256), (8, 512, 512)])
 def test_frozen_encoder(torch, shape):
     n, h, w = shape
-    net = _net(torch)
-    x, t = _inputs(torch, n, h, w, seed=2)
+    net = E.net()
+    x, t = E.frames(n, 4, 4, h, w, seed=2)
     o_all, _ = net.train_step(x, t)
     o_all, g_all = o_all.clone(), _grads(net)
-    _freeze(net, ENC)
+    E.freeze_layers(net, ENC)
     names = _train_names(net, x, t)
-    assert names == _without(TRAIN_STEP, ENC, drop=('pool.bwd', 'upv6.dgrad'))
+    assert names == E.without(TRAIN_STEP, ENC, drop=('pool.bwd', 'upv6.dgrad'))
     out, _ = net.train_step(x, t)
     assert torch.equal(out, o_all)
     got = _grads(net)
     dec = [k for k, p in net.named_parameters() if p.requires_grad]
-    assert _rel(torch.cat([got[k] for k in dec]), torch.cat([g_all[k] for k in dec])) <= 1e-4
-    worst = max(_rel(got[k], g_all[k]) for k in dec)
+    assert E.rel(torch.cat([got[k] for k in dec]), torch.cat([g_all[k] for k in dec])) <= 1e-4
+    worst = max(E.rel(got[k], g_all[k]) for k in dec)
     assert worst <= 1e-2, worst
     for k, p in net.named_parameters():
         if not p.requires_grad:
@@ -147,7 +87,7 @@ def test_frozen_encoder(torch, shape):
         torch.manual_seed(2018)
         ref = UNetSeeInDarkRef(4, 4).cuda()
         _, _, gem = fp32_cuda(lambda: emulated_train_step(ref, x, t))
-        bad = [(k, _rel(got[k].view_as(gem[k]), gem[k])) for k in dec if _rel(got[k].view_as(gem[k]), gem[k]) > 1.5e-2]
+        bad = [(k, E.rel(got[k].view_as(gem[k]), gem[k])) for k in dec if E.rel(got[k].view_as(gem[k]), gem[k]) > 1.5e-2]
         assert not bad, bad
     # the autograd node: frozen parameters get no gradient at all
     for p in net.parameters():
@@ -155,35 +95,35 @@ def test_frozen_encoder(torch, shape):
     torch.nn.functional.l1_loss(net(x), t).backward()
     for (k, p), (o, c) in zip(net.named_parameters(), net._spans):
         if p.requires_grad:
-            assert _rel(p.grad.reshape(-1), g_all[k]) <= 1e-2, k
+            assert E.rel(p.grad.reshape(-1), g_all[k]) <= 1e-2, k
         else:
             assert p.grad is None, k
     assert 'upv6.dgrad' not in _autograd_names(torch, net, x, t)
 
 
 def test_frozen_decoder(torch):
-    net = _net(torch)
-    x, t = _inputs(torch, 2, H, W, seed=3)
+    net = E.net()
+    x, t = E.frames(2, 4, 4, H, W, seed=3)
     net.train_step(x, t)
     g_all = _grads(net)
     dec = _decoder(net)
-    _freeze(net, dec)
+    E.freeze_layers(net, dec)
     names = _train_names(net, x, t)
     assert [n for n in names if not n.endswith('.wgrad')] == [n for n in TRAIN_STEP if not n.endswith('.wgrad')]
     assert [n for n in names if n.endswith('.wgrad')] == [n for n in TRAIN_STEP if n.endswith('.wgrad') and n.split('.')[0] in ENC]
     net.train_step(x, t)
     got = _grads(net)
     enc = [k for k, p in net.named_parameters() if p.requires_grad]
-    assert _rel(torch.cat([got[k] for k in enc]), torch.cat([g_all[k] for k in enc])) <= 1e-4
-    assert max(_rel(got[k], g_all[k]) for k in enc) <= 1e-2
+    assert E.rel(torch.cat([got[k] for k in enc]), torch.cat([g_all[k] for k in enc])) <= 1e-4
+    assert max(E.rel(got[k], g_all[k]) for k in enc) <= 1e-2
     assert not any(got[k].any() for k, p in net.named_parameters() if not p.requires_grad)
 
 
 def test_frozen_network_input_grad(torch):
     """test-time optimisation of the input: no weight-gradient launch, x.grad bit-identical, nothing moves"""
     from eld_b200 import arch
-    net = _net(torch)
-    x, t = _inputs(torch, 2, H, W, seed=4)
+    net = E.net()
+    x, t = E.frames(2, 4, 4, H, W, seed=4)
 
     def dx_of():
         for p in net.parameters():
@@ -195,7 +135,7 @@ def test_frozen_network_input_grad(torch):
     d_all = dx_of()
     names_all = _autograd_names(torch, net, x.clone().requires_grad_(), t)
     opt = arch.FusedAdam(net, lr=1e-3, weight_decay=1e-4)
-    _freeze(net, ENC + _decoder(net))
+    E.freeze_layers(net, ENC + _decoder(net))
     p0, m0 = net.flat_params.clone(), opt.m.clone()
     d = dx_of()
     assert torch.equal(d, d_all)
@@ -205,7 +145,7 @@ def test_frozen_network_input_grad(torch):
     assert 'conv1_1.dgrad' in names and 'conv10_1.bwd' in names
     # the fused step of a fully frozen network is forward + loss; Adam has nothing to do
     names = _train_names(net, x, t)
-    assert names == _FWD + ['conv10_1.fwd+loss']
+    assert names == FWD_NAMES + ['conv10_1.fwd+loss']
     opt.step()
     torch.cuda.synchronize()
     assert torch.equal(net.flat_params, p0) and torch.equal(opt.m, m0) and opt.steps == [0] * 46
@@ -216,14 +156,14 @@ def test_adam_per_parameter_steps_match_torch(torch):
     """encoder frozen for steps 1-3, trainable for 4-6, weight decay on: FusedAdam against torch.optim.Adam fed the same
     flat gradients; frozen tensors bit-unchanged while frozen; checkpoints load both ways with per-parameter steps"""
     from eld_b200 import arch
-    net = _net(torch)
+    net = E.net()
     spans, names = net._spans, [k for k, _ in net.named_parameters()]
     plain = [p.detach().clone().requires_grad_() for p in net.parameters()]
     kw = dict(lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2)
     opt, topt = arch.FusedAdam(net, **kw), torch.optim.Adam(plain, **kw)
     g = torch.Generator(device='cuda').manual_seed(6)
     for step in range(6):
-        _freeze(net, ENC if step < 3 else ())
+        E.freeze_layers(net, ENC if step < 3 else ())
         before = net.flat_params.clone()
         grad = torch.randn(net.flat_params.shape, generator=g, device='cuda') * 1e-3
         net.flat_grads.copy_(grad)
@@ -258,11 +198,11 @@ def test_model_optimize_parameters_with_frozen_encoder(torch, tmp_path):
     from eld_b200 import models
     m = models.eld_model()
     m.initialize(models.default_opt(name='fz', checkpoints_dir=str(tmp_path)))
-    _freeze(m.netG, ENC)
+    E.freeze_layers(m.netG, ENC)
     enc0 = {k: p.detach().clone() for k, p in m.netG.named_parameters() if not p.requires_grad}
     dec0 = {k: p.detach().clone() for k, p in m.netG.named_parameters() if p.requires_grad}
     for i in range(5):
-        x, t = _inputs(torch, 1, H, W, seed=10 + i)
+        x, t = E.frames(1, 4, 4, H, W, seed=10 + i)
         m.set_input({'input': x.cpu(), 'target': t.cpu()}, 'train')
         m.optimize_parameters()
     params = dict(m.netG.named_parameters())
@@ -280,11 +220,11 @@ def test_ddp_world1_frozen_encoder(torch, monkeypatch):
     dist.init_process_group('nccl', init_method='tcp://127.0.0.1:%d' % port, rank=0, world_size=1,
                             device_id=torch.device('cuda', 0))
     try:
-        net = _net(torch)
-        _freeze(net, ENC)
+        net = E.net()
+        E.freeze_layers(net, ENC)
         opt = arch.FusedAdam(net, lr=1e-4)
         p0 = net.flat_params.clone()
-        x, t = _inputs(torch, 2, H, W, seed=7)
+        x, t = E.frames(2, 4, 4, H, W, seed=7)
         net.train_step(x, t)
         want = net.flat_grads.clone()
         opt.step()
@@ -299,33 +239,30 @@ def test_ddp_world1_frozen_encoder(torch, monkeypatch):
         torch.cuda.synchronize()
         buckets = net.grad_buckets()
         assert calls == [buckets[0][1]]                  # the decoder bucket; the three encoder buckets are wholly frozen
-        assert _rel(net.flat_grads, want) < 1e-3
+        assert E.rel(net.flat_grads, want) < 1e-3
         enc_end = buckets[0][0]
         assert torch.equal(net.flat_params[:enc_end], p0[:enc_end])
-        assert _rel(net.flat_params - p0, p_plain - p0) < 5e-2
+        assert E.rel(net.flat_params - p0, p_plain - p0) < 5e-2
     finally:
         dist.destroy_process_group()
 
 
 def test_contract(torch):
     from eld_b200 import _lib
-    net, lib = _net(torch), _lib.load()
+    net, lib = E.net(), _lib.load()
     eng = net._engine(2, H, W, True)
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     with pytest.raises(_lib.EldError):
-        _set(lib, net, eng, [1] * 45, 1)
+        E.set_trainable(net, eng, [1] * 45, 1)
     with pytest.raises(_lib.EldError):
         _lib.check(lib.eld_unet_set_trainable(eng, None, 46, 1), 'eld_unet_set_trainable')
-    x, t = _inputs(torch, 2, H, W, seed=8)
+    x, t = E.frames(2, 4, 4, H, W, seed=8)
     dx = torch.empty_like(x)
-    _freeze(net, ENC)
+    E.freeze_layers(net, ENC)
     net.train_step(x, t)                                 # input_grad = 0 and conv1_1 frozen: the chain stops at upv6
     with pytest.raises(_lib.EldError):
         _lib.check(lib.eld_unet_input_grad(eng, net.flat_params.data_ptr(), dx.data_ptr(), st), 'eld_unet_input_grad')
-    _set(lib, net, eng, [0] * 20 + [1] * 26, 1)          # input_grad = 1 keeps the chain running down to dz1_1
-    out = torch.empty_like(t)
-    loss = torch.zeros((), device='cuda')
-    _lib.check(lib.eld_unet_train_step(eng, net.flat_params.data_ptr(), x.data_ptr(), t.data_ptr(), out.data_ptr(),
-                                       net.flat_grads.data_ptr(), loss.data_ptr(), st), 'eld_unet_train_step')
+    E.set_trainable(net, eng, [0] * 20 + [1] * 26, 1)   # input_grad = 1 keeps the chain running down to dz1_1
+    E.abi_train_step(net, eng, x, t)()
     _lib.check(lib.eld_unet_input_grad(eng, net.flat_params.data_ptr(), dx.data_ptr(), st), 'eld_unet_input_grad')
     assert torch.isfinite(dx).all() and dx.abs().sum().item() > 0

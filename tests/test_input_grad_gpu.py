@@ -17,45 +17,11 @@ import warnings
 
 import pytest
 
+from tests import engine_harness as E
+from tests.engine_harness import torch  # noqa: F401 (the fixture)
+
 pytestmark = pytest.mark.gpu
 H, W = 128, 256          # smallest shape the training tiles accept
-
-
-@pytest.fixture(scope='module')
-def torch():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no GPU')
-    return torch
-
-
-def _rel(a, b):
-    return ((a.double() - b.double()).norm() / (b.double().norm() + 1e-30)).item()
-
-
-def _pair(torch, cin=4, cout=4):
-    """engine module and fp32 oracle module with the same weights; biases spread (both, identically) so that both sides
-    of every LeakyReLU kink - and both values of the backward masks - carry real weight"""
-    from eld_b200 import arch
-    from oracle.unet_ref import UNetSeeInDarkRef
-    torch.manual_seed(2018)
-    ours = arch.unet(cin, cout).cuda()
-    torch.manual_seed(2018)
-    ref = UNetSeeInDarkRef(cin, cout).cuda()
-    g = torch.Generator().manual_seed(5)
-    with torch.no_grad():
-        for (k, p), (k2, q) in zip(ref.named_parameters(), ours.named_parameters()):
-            assert k == k2 and torch.equal(p, q)
-            if k.endswith('.bias'):
-                d = ((torch.rand(p.shape, generator=g) - 0.5) * 0.2).cuda()
-                p.add_(d)
-                q.add_(d)
-    return ours, ref
-
-
-def _inputs(torch, n, cin, cout, h, w, seed):
-    g = torch.Generator().manual_seed(seed)
-    return torch.rand(n, cin, h, w, generator=g).cuda(), torch.rand(n, cout, h, w, generator=g).cuda()
 
 
 def _l1(torch, out, t):
@@ -103,23 +69,14 @@ def _check_tile(net, x, dx):
 
 def _check_vs_emulation(got, emu):
     assert got.shape == emu.shape
-    print('x.grad vs emulation: rel-L2 %.2e, border ring %.2e' % (_rel(got, emu), _rel(_ring(got), _ring(emu))))
-    assert _rel(got, emu) <= 5e-2, _rel(got, emu)
-    assert _rel(_ring(got), _ring(emu)) <= 5e-2, _rel(_ring(got), _ring(emu))
-
-
-def _profile_names(lib, eng):
-    from eld_b200 import _lib
-    cap = 512
-    names = ctypes.create_string_buffer(32 * cap)
-    cnt = ctypes.c_int(0)
-    _lib.check(lib.eld_unet_profile_read(eng, cap, names, None, None, None, ctypes.byref(cnt)), 'eld_unet_profile_read')
-    return [names.raw[32 * i:32 * i + 32].split(b'\0')[0].decode() for i in range(cnt.value)]
+    print('x.grad vs emulation: rel-L2 %.2e, border ring %.2e' % (E.rel(got, emu), E.rel(_ring(got), _ring(emu))))
+    assert E.rel(got, emu) <= 5e-2, E.rel(got, emu)
+    assert E.rel(_ring(got), _ring(emu)) <= 5e-2, E.rel(_ring(got), _ring(emu))
 
 
 def test_input_grad_matches_emulated_backward(torch):
-    ours, ref = _pair(torch)
-    x, t = _inputs(torch, 2, 4, 4, H, W, seed=1)
+    ours, ref = E.pair()
+    x, t = E.frames(2, 4, 4, H, W, seed=1)
     _, got = _engine_dx(torch, ours, x, t)
     assert torch.isfinite(got).all()
     _check_tile(ours, x, got)
@@ -129,8 +86,8 @@ def test_input_grad_matches_emulated_backward(torch):
 
 def test_input_grad_matches_fp32_oracle(torch):
     from tests.unet_emul import fp32_cuda
-    ours, ref = _pair(torch)
-    x, t = _inputs(torch, 2, 4, 4, H, W, seed=2)
+    ours, ref = E.pair()
+    x, t = E.frames(2, 4, 4, H, W, seed=2)
     _, got = _engine_dx(torch, ours, x, t)
     xr = x.clone().requires_grad_()
     fp32_cuda(lambda: _l1(torch, ref(xr), t).backward())
@@ -146,8 +103,8 @@ def test_input_grad_three_channel_frames(torch, io):
     """--stage_in srgb: x.grad has 3 planes; the padded B rows (c = 3 .. 7) are never stored."""
     from eld_b200 import _lib
     cin, cout = io
-    ours, ref = _pair(torch, cin, cout)
-    x, t = _inputs(torch, 2, cin, cout, H, W, seed=3)
+    ours, ref = E.pair(cin, cout)
+    x, t = E.frames(2, cin, cout, H, W, seed=3)
     _, got = _engine_dx(torch, ours, x, t)
     assert got.shape == (2, 3, H, W)
     _check_tile(ours, x, got)
@@ -167,9 +124,9 @@ def test_input_grad_leaves_the_rest_of_the_step_alone(torch):
     """The same step with and without x.requires_grad: the parameter gradients agree (fp32 atomics reorder the
     weight-gradient sums), and the conv1_1.dgrad launch is in the per-launch profile only when x asked for it."""
     from eld_b200 import _lib
-    ours, _ = _pair(torch)
+    ours, _ = E.pair()
     lib = _lib.load()
-    x, t = _inputs(torch, 2, 4, 4, H, W, seed=4)
+    x, t = E.frames(2, 4, 4, H, W, seed=4)
     eng = ours._engine(2, H, W, True)
     runs = []
     for want_dx in (False, True):
@@ -178,12 +135,12 @@ def test_input_grad_leaves_the_rest_of_the_step_alone(torch):
         xi = x.clone().requires_grad_(want_dx)
         _lib.check(lib.eld_unet_profile(eng, 1), 'eld_unet_profile')
         _l1(torch, ours(xi), t).backward()
-        names = _profile_names(lib, eng)
+        names = E.recorded(eng)
         _lib.check(lib.eld_unet_profile(eng, 0), 'eld_unet_profile')
         runs.append((torch.cat([p.grad.reshape(-1) for p in ours.parameters()]), names, xi.grad))
     (g0, n0, d0), (g1, n1, d1) = runs
     assert d0 is None and d1 is not None
-    assert _rel(g1, g0) <= 1e-4, _rel(g1, g0)
+    assert E.rel(g1, g0) <= 1e-4, E.rel(g1, g0)
     assert 'conv1_1.dgrad' not in n0 and n1.count('conv1_1.dgrad') == 1
     assert [n for n in n1 if n != 'conv1_1.dgrad'] == n0
     ours._flatten()
@@ -191,8 +148,8 @@ def test_input_grad_leaves_the_rest_of_the_step_alone(torch):
 
 def test_input_grad_composes_with_upstream_parameters(torch):
     """x = a * x0 with a learnable scalar a: autograd carries the engine's dx on to a, and a stock optimizer moves a."""
-    ours, _ = _pair(torch)
-    x0, t = _inputs(torch, 2, 4, 4, H, W, seed=5)
+    ours, _ = E.pair()
+    x0, t = E.frames(2, 4, 4, H, W, seed=5)
     a = torch.tensor(0.8, device='cuda', requires_grad=True)
     _l1(torch, ours(a * x0), t).backward()
     _, g = _engine_dx(torch, ours, (a * x0).detach(), t)
@@ -206,8 +163,8 @@ def test_input_grad_composes_with_upstream_parameters(torch):
 
 
 def test_input_grad_in_eval_mode(torch):
-    ours, _ = _pair(torch)
-    x, t = _inputs(torch, 2, 4, 4, H, W, seed=6)
+    ours, _ = E.pair()
+    x, t = E.frames(2, 4, 4, H, W, seed=6)
     out_t, g_t = _engine_dx(torch, ours, x, t)
     ours.eval()
     try:
@@ -221,7 +178,7 @@ def test_input_grad_in_eval_mode(torch):
 
 def test_input_grad_contract(torch):
     from eld_b200 import _lib
-    ours, _ = _pair(torch)
+    ours, _ = E.pair()
     lib = _lib.load()
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     # a shape the training tiles reject: today's inference result, detached, and ONE warning however often it is called
@@ -239,7 +196,7 @@ def test_input_grad_contract(torch):
     inf = ours._engine(2, H, W, False)
     with pytest.raises(_lib.EldError):
         _lib.check(lib.eld_unet_input_grad(inf, ours.flat_params.data_ptr(), dx.data_ptr(), st), 'eld_unet_input_grad')
-    xg, t = _inputs(torch, 2, 4, 4, H, W, seed=7)
+    xg, t = E.frames(2, 4, 4, H, W, seed=7)
     eng = ours._engine(2, H, W, True)
     _engine_dx(torch, ours, xg, t)
     with pytest.raises(_lib.EldError):
@@ -254,7 +211,7 @@ def test_input_grad_contract(torch):
 def test_input_grad_8x4x512x512(torch):
     """BASELINE's training shape (noisy smooth frames -> clean targets) against the emulated backward."""
     from tests.unet_emul import smooth_frames
-    ours, ref = _pair(torch)
+    ours, ref = E.pair()
     t = smooth_frames(8, 512, 512, seed=13, device='cuda')
     g = torch.Generator().manual_seed(8)
     x = (t + 0.05 * torch.randn(t.shape, generator=g).cuda()).clamp(0, 1)

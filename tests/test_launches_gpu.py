@@ -4,7 +4,8 @@ The end-to-end tests compare whole-network outputs and gradients at rel-L2 gates
 corrupted channels or one bad partial tile of one intermediate tensor can hide under.  Here each launch is judged in
 isolation: one step (or one forward) runs, the launch list comes from the engine's own profile (a launch without a
 check fails the test), and every launch's output is compared with a float64 reference fed with the exact tensors that
-launch read, as the engine stored them in its workspace (eld_unet_buffer).
+launch read, as the engine stored them in its workspace (eld_unet_buffer).  The check and its gates are
+tests/launch_check.py's.
 
 Acceptance, one rule per output kind:
   exact  pooled values (max of the stored values), pool codes, sign words, pack_all vs eld_pack_weights, the OIHW
@@ -21,345 +22,28 @@ from collections import defaultdict
 
 import pytest
 
+from tests import abi_harness as H
+from tests import engine_harness as E
+from tests.engine_harness import ENC
+from tests.launch_check import NAN_BITS, Step
+
 pytestmark = pytest.mark.gpu
-
-# fraction of bf16 elements allowed to differ from RNE(r) (fp32 accumulation order): about 4x the worst rate measured on
-# an H100 80GB HBM3 at a 400 W power limit over the cases below
-MISMATCH = {'conv.fprop': 0.01, 'conv.dgrad': 0.011, 'conv.dgrad.mask': 0.011, 'conv.dgrad.split': 0.006,
-            'conv.dgrad.prefix': 0.006, 'conv1_1.fprop': 1e-4, 'deconv.fprop': 1e-3, 'deconv.dgrad': 2e-3, 'pool.bwd': 8e-3,
-            'head.dz9_2.l1': 2e-4, 'head.dz9_2.l2': 2e-4, 'head.dz9_2.seam': 2e-4}
-REL_L2 = 1e-5
-MAX_ABS = 1e-4
-# The tensor-core weight gradients accumulate thousands of pixels per CTA in wgmma's fp32 accumulator (~80k for conv9_1 at
-# 8 x 512^2) and their error grows about linearly with that length.  Measured on the same H100: rel-L2 8.7e-6 at the
-# 2 x 128 x 256 shapes, 4.3e-4 (max-abs 4.7e-4 of max|r|, conv9_1) at 8 x 512^2.  Gates at about 4x those.
-WGRAD_KINDS = ('conv.wgrad', 'conv.bias_grad', 'deconv.wgrad', 'deconv.bias_grad', 'conv1_1.wgrad', 'conv1_1.bias_grad')
-WGRAD_REL_L2 = 4e-5
-PRODUCTION_WGRAD = 2e-3
-
-# the forward graph of Runner::forward (csrc/unet_engine.cu): layer -> (input tensor, its first channel, output, first channel)
-FWD = {'conv1_2': ('a1_1', 0, 'cat9', 32), 'conv2_1': ('p1', 0, 'a2_1', 0), 'conv2_2': ('a2_1', 0, 'cat8', 64),
-       'conv3_1': ('p2', 0, 'a3_1', 0), 'conv3_2': ('a3_1', 0, 'cat7', 128), 'conv4_1': ('p3', 0, 'a4_1', 0),
-       'conv4_2': ('a4_1', 0, 'cat6', 256), 'conv5_1': ('p4', 0, 'a5_1', 0), 'conv5_2': ('a5_1', 0, 'a5_2', 0),
-       'upv6': ('a5_2', 0, 'cat6', 0), 'conv6_1': ('cat6', 0, 'a6_1', 0), 'conv6_2': ('a6_1', 0, 'a6_2', 0),
-       'upv7': ('a6_2', 0, 'cat7', 0), 'conv7_1': ('cat7', 0, 'a7_1', 0), 'conv7_2': ('a7_1', 0, 'a7_2', 0),
-       'upv8': ('a7_2', 0, 'cat8', 0), 'conv8_1': ('cat8', 0, 'a8_1', 0), 'conv8_2': ('a8_1', 0, 'a8_2', 0),
-       'upv9': ('a8_2', 0, 'cat9', 0), 'conv9_1': ('cat9', 0, 'a9_1', 0), 'conv9_2': ('a9_1', 0, 'a9_2', 0)}
-POOLED = {'conv1_2': ('p1', 'pc1'), 'conv2_2': ('p2', 'pc2'), 'conv3_2': ('p3', 'pc3'), 'conv4_2': ('p4', 'pc4')}
-SIGNED = ('a1_1', 'a2_1', 'a3_1', 'a4_1', 'a5_1', 'a5_2', 'a6_1', 'a6_2', 'a7_1', 'a7_2', 'a8_1', 'a8_2', 'a9_1')
-# the pool backward launches in issue order: pooled activation (cat buffer, first channel), concat gradient, dp, output
-POOL_BWD = [('cat6', 256, 'dcat6', 'dp4', 'dz4_2'), ('cat7', 128, 'dcat7', 'dp3', 'dz3_2'),
-            ('cat8', 64, 'dcat8', 'dp2', 'dz2_2'), ('cat9', 32, 'dcat9', 'dp1', 'dz1_2')]
-ENC = ('conv1_1', 'conv1_2', 'conv2_1', 'conv2_2', 'conv3_1', 'conv3_2', 'conv4_1', 'conv4_2', 'conv5_1', 'conv5_2')
-NAN_BITS = 0x7FA5        # bf16 NaN with a payload: the sentinel of a plane no launch may write
 
 STATS = defaultdict(lambda: defaultdict(float))     # launch kind -> worst measured value per statistic
 
-
-@pytest.fixture(scope='module')
-def torch():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no GPU')
-    yield torch
-    print('\nworst case per launch kind (rule: bf16 = max |got-r| / (ulp + 2^-20 S), mismatch rate; '
-          'fp32 = rel-L2, max-abs / max|r|, max |got-r| / S; exact = elements compared)')
-    for kind in sorted(STATS):
-        print('  %-24s %s' % (kind, '  '.join('%s=%.3g' % kv for kv in sorted(STATS[kind].items()))))
-
-
-def _dz(layer):
-    """the stored gradient of a layer's pre-activation output: conv9_2 -> dz9_2"""
-    return 'dz' + layer[4:]
-
-
-def _level(cat):
-    """the grid level of a concat buffer: cat9 -> 0 (full resolution) .. cat6 -> 3"""
-    return 9 - int(cat[-1])
-
-
-class Step:
-    """One finished step (or forward) of engine `eng` and the checks of its launches.
-    skip_elided: the concat levels whose data gradient is a row-prefix launch (the up half only; the caller filled the
-    skip plane with NAN_BITS), split stores elsewhere.  frozen: the parameter names that do not train - a weight-gradient
-    launch still computes them (one launch per layer), but their range of grads must read zero."""
-
-    def __init__(self, torch, net, eng, ws, x, out, grads=None, target=None, loss=None, kind='l1', dout=None, dx=None,
-                 skip_elided=frozenset(), frozen=frozenset(), tag=''):
-        from eld_b200 import _lib
-        self.t, self.net, self.lib, self.eng, self.ws = torch, net, _lib.load(), eng, ws
-        self.x, self.out, self.grads, self.target, self.loss, self.kind = x, out, grads, target, loss, kind
-        self.dout, self.dx, self.skip_elided, self.frozen, self.tag = dout, dx, set(skip_elided), set(frozen), tag
-        self.dz9_2 = True       # the head wrote dz9_2 (something below conv10_1 needs it); set from the launch list
-        self.params = dict(net.named_parameters())
-        self.span = {k: sp for k, sp in zip(self.params, net._spans)}
-        self.fail = []
-        self.names = []
-
-    def V(self, name):
-        from tests.launch_ref import buffer
-        return buffer(self.lib, self.eng, self.ws, name)
-
-    def W(self, layer):
-        return self.params[layer + '.weight'].detach()
-
-    def B(self, layer):
-        return self.params[layer + '.bias'].detach()
-
-    def G(self, pname):
-        off, k = self.span[pname]
-        return self.grads[off:off + k].view(self.params[pname].shape)
-
-    def planes(self, dcat):
-        """the planar concat gradient buffer -> (up plane, skip plane), each [n, h, w, C/2]"""
-        v = self.V(dcat)
-        n, h, w, c = v.shape
-        flat = v.reshape(-1)
-        half = flat.numel() // 2
-        return flat[:half].view(n, h, w, c // 2), flat[half:].view(n, h, w, c // 2)
-
-    # ---- the three acceptance rules ----
-    def bf16(self, kind, where, got, r, S):
-        from tests.launch_ref import bf16_rule
-        assert got.shape == r.shape, (where, got.shape, r.shape)
-        ratio, mism, finite = bf16_rule(got, r, S)
-        st = STATS['bf16 ' + kind + self.tag]
-        st['ulp_ratio'] = max(st['ulp_ratio'], ratio)
-        st['mismatch'] = max(st['mismatch'], mism)
-        if not (ratio <= 1.0 and mism <= MISMATCH[kind]) or not finite:
-            self.fail.append('%s (%s): max |got-r|/(ulp+2^-20 S) = %.3g, mismatch %.3g' % (where, kind, ratio, mism))
-
-    def f32(self, kind, where, got, r, S):
-        from tests.launch_ref import f32_rule
-        rel, mx, ms = f32_rule(got, r, S)
-        st = STATS['fp32 ' + kind + self.tag]
-        st['rel_l2'] = max(st['rel_l2'], rel)
-        st['max_abs_rel'] = max(st['max_abs_rel'], mx)
-        st['err_over_S'] = max(st['err_over_S'], ms)
-        rel_max, abs_max = REL_L2, MAX_ABS
-        if kind in WGRAD_KINDS:
-            rel_max, abs_max = (PRODUCTION_WGRAD, PRODUCTION_WGRAD) if self.tag else (WGRAD_REL_L2, MAX_ABS)
-        if not (rel <= rel_max and mx <= abs_max):
-            self.fail.append('%s (%s): rel-L2 %.3g, max-abs / max|r| %.3g' % (where, kind, rel, mx))
-
-    def grad(self, kind, pname, r, S):
-        """a parameter's range of grads: the fp32 rule when it trains, all zero bits when it is frozen"""
-        got = self.G(pname)
-        if pname in self.frozen:
-            self.exact('frozen range', pname, got.view(self.t.int32), self.t.zeros_like(got).view(self.t.int32))
-        else:
-            self.f32(kind, pname, got, r, S)
-
-    def exact(self, kind, where, got, want):
-        STATS['exact ' + kind]['elements'] += got.numel()
-        if got.shape != want.shape or not self.t.equal(got, want):
-            bad = (got != want).sum().item() if got.shape == want.shape else -1
-            self.fail.append('%s (%s): %d elements differ' % (where, kind, bad))
-
-    def bits(self, t):
-        return t.contiguous().view(self.t.int16)
-
-    # ---- launch kinds ----
-    def pack(self):
-        from eld_b200 import prims
-        from tests.launch_ref import first_layer_image
-        self.exact('pack', 'wf:conv1_1', self.bits(self.V('wf:conv1_1').reshape(-1)), self.bits(first_layer_image(self.W('conv1_1'))))
-        for layer in FWD:
-            deconv = layer.startswith('upv')
-            kinds = (prims.PACK_DECONV_FPROP, prims.PACK_DECONV_DGRAD) if deconv else (prims.PACK_CONV_FPROP, prims.PACK_CONV_DGRAD)
-            for pre, kind in zip(('wf:', 'wd:'), kinds):
-                want = prims.pack_weights(self.W(layer), kind).reshape(-1)
-                self.exact('pack', pre + layer, self.bits(self.V(pre + layer).reshape(-1)), self.bits(want))
-
-    def fprop(self, layer):
-        import tests.launch_ref as R
-        src, sc0, dst, dc0 = FWD[layer]
-        if layer.startswith('upv'):
-            cout = self.W(layer).shape[1]
-            r, S = R.deconv_fprop(self.V(src), self.W(layer), self.B(layer))
-            self.bf16('deconv.fprop', layer, self.V(dst)[..., :cout], r, S)
-            return
-        cout, cin = self.W(layer).shape[:2]
-        x = self.V(src)[..., sc0:sc0 + cin]
-        r, S = R.conv_fprop(x, self.W(layer), self.B(layer))
-        got = self.V(dst)[..., dc0:dc0 + cout]
-        self.bf16('conv.fprop', layer, got, r, S)
-        self.epilogue_extras(layer, dst, got)
-
-    def epilogue_extras(self, layer, dst, got):
-        """the fused pool, its code and the sign words, all from the STORED output"""
-        import tests.launch_ref as R
-        if layer in POOLED:
-            p, pc = POOLED[layer]
-            m, _, _ = R.pool(got)
-            self.exact('pool', p, self.bits(self.V(p)), self.bits(m.bfloat16()))
-            if self.training:
-                n, h, w, c = self.V(pc).shape
-                self.exact('pool code', pc, self.V(pc).reshape(-1).view(self.t.int32).view(n, h, w, c // 32, 8), R.pool_code(got))
-        if self.training and dst in SIGNED:
-            self.exact('sign words', 'sign:' + dst, self.V('sign:' + dst), R.sign_words(got))
-
-    @property
-    def training(self):
-        return self.grads is not None
-
-    def first_fprop(self):
-        import tests.launch_ref as R
-        r, S = R.first_conv_fprop(self.x, self.W('conv1_1'), self.B('conv1_1'))
-        got = self.V('a1_1')
-        self.bf16('conv1_1.fprop', 'conv1_1', got, r, S)
-        self.epilogue_extras('conv1_1', 'a1_1', got)
-
-    def dgrad(self, layer):
-        import tests.launch_ref as R
-        src = FWD[layer][0]
-        if layer.startswith('upv'):
-            up, _ = self.planes('dcat' + layer[3:])
-            r, S = R.deconv_dgrad(up, self.W(layer), self.V(src))
-            self.bf16('deconv.dgrad', layer, self.V('dz' + src[1:]), r, S)
-            return
-        dz = self.V(_dz(layer))
-        if src.startswith('cat'):
-            up, skip = self.planes('d' + src)
-            r, S = R.conv_dgrad(dz, self.W(layer))
-            half = up.shape[-1]
-            if _level(src) in self.skip_elided:   # the row-prefix launch: the up half only, the skip plane keeps its sentinel
-                self.bf16('conv.dgrad.prefix', layer, up, r[..., :half], S[..., :half])
-                self.exact('sentinel', 'd%s skip plane' % src, self.bits(skip), self.t.full_like(self.bits(skip), NAN_BITS))
-            else:
-                self.bf16('conv.dgrad.split', layer, up, r[..., :half], S[..., :half])
-                self.bf16('conv.dgrad.split', layer + ' skip', skip, r[..., half:], S[..., half:])
-        elif src.startswith('p'):
-            r, S = R.conv_dgrad(dz, self.W(layer))
-            self.bf16('conv.dgrad', layer, self.V('d' + src), r, S)
-        else:
-            r, S = R.conv_dgrad(dz, self.W(layer), self.V(src))
-            self.bf16('conv.dgrad.mask', layer, self.V('dz' + src[1:]), r, S)
-
-    def pool_bwd(self, k):
-        import tests.launch_ref as R
-        cat, c0, dcat, dp, dst = POOL_BWD[k]
-        c = self.V(dp).shape[-1]
-        _, skip = self.planes(dcat)
-        r, S = R.pool_bwd(self.V(cat)[..., c0:c0 + c], skip, self.V(dp))
-        self.bf16('pool.bwd', dst, self.V(dst), r, S)
-
-    def wgrad(self, layer):
-        import tests.launch_ref as R
-        src, sc0 = FWD[layer][:2]
-        if layer.startswith('upv'):
-            up, _ = self.planes('dcat' + layer[3:])
-            dW, S, db, Sb = R.deconv_wgrad(self.V(src), up)
-            self.grad('deconv.wgrad', layer + '.weight', dW, S)
-            self.grad('deconv.bias_grad', layer + '.bias', db, Sb)
-            return
-        cout, cin = self.W(layer).shape[:2]
-        dW, S, db, Sb = R.conv_wgrad(self.V(src)[..., sc0:sc0 + cin], self.V(_dz(layer)))
-        off = self.span[layer + '.weight'][0]
-        staged = self.V('gtmp').reshape(-1)[off:off + dW.numel()].view(3, 3, cin, cout).permute(3, 2, 0, 1)
-        self.f32('conv.wgrad', layer + ' (gtmp)', staged, dW, S)    # staged whether or not the weight trains
-        self.grad('conv.bias_grad', layer + '.bias', db, Sb)
-
-    def gperm(self, trained):
-        """grads (OIHW) of every trained conv3x3 weight == its [tap][ci][co] staging, permuted; a frozen one's range zero"""
-        gtmp = self.V('gtmp').reshape(-1)
-        for layer in FWD:
-            if layer.startswith('upv'):
-                continue
-            off, k = self.span[layer + '.weight']
-            cout, cin = self.W(layer).shape[:2]
-            got = self.G(layer + '.weight')
-            want = gtmp[off:off + k].view(3, 3, cin, cout).permute(3, 2, 0, 1) if layer in trained else self.t.zeros_like(got)
-            self.exact('gperm', layer, got.view(self.t.int32), want.contiguous().view(self.t.int32))
-
-    def first_wgrad(self):
-        import tests.launch_ref as R
-        dW, S, db, Sb = R.first_conv_wgrad(self.x, self.V('dz1_1'))
-        self.grad('conv1_1.wgrad', 'conv1_1.weight', dW, S)
-        self.grad('conv1_1.bias_grad', 'conv1_1.bias', db, Sb)
-
-    def first_dgrad(self):
-        import tests.launch_ref as R
-        r, S = R.first_conv_dgrad(self.V('dz1_1'), self.W('conv1_1'))
-        self.f32('x.grad', 'conv1_1 dgrad', self.dx, r, S)
-
-    def head(self, what):
-        import tests.launch_ref as R
-        a, w = self.V('a9_2'), self.W('conv10_1')
-        if what != 'bwd':             # the seam's backward re-forms out into scratch: its forward launch is checked instead
-            r, S = R.head(a, w, self.B('conv10_1'))
-            self.f32('head.out', 'conv10_1 out', self.out, r, S)
-        if what == 'fprop':
-            return
-        if what != 'bwd':
-            lr = R.head_loss(self.out, self.target, self.kind)
-            self.f32('head.loss.' + self.kind, 'loss', self.loss.reshape(1), lr.reshape(1), lr.reshape(1))
-        if what == 'fwd+loss':
-            return
-        dout = self.dout if what == 'bwd' else R.head_dout(self.out, self.target, self.kind)
-        dz, S, dW, Sw, db, Sb = R.head_bwd(a, w, dout)
-        if self.dz9_2:
-            self.bf16('head.dz9_2' + ('.seam' if what == 'bwd' else '.' + self.kind), 'dz9_2', self.V('dz9_2'), dz, S)
-        self.grad('head.dW10', 'conv10_1.weight', dW, Sw)
-        self.grad('head.db10', 'conv10_1.bias', db, Sb)
-
-    def check(self, names):
-        """every launch in `names` (the engine's profile, in issue order)"""
-        self.names = names
-        pools = 0
-        trained = {n.split('.')[0] for n in names if n.endswith('.wgrad')} - {p.split('.')[0] for p in self.frozen
-                                                                               if p.endswith('.weight')}
-        self.dz9_2 = 'conv9_2.wgrad' in names or 'conv9_2.dgrad' in names
-        for name in names:
-            layer, what = name.split('.', 1)
-            if name == 'weights.pack':
-                self.pack()
-            elif name == 'weights.gperm':
-                self.gperm(trained)
-            elif name == 'pool.bwd':
-                self.pool_bwd(pools)
-                pools += 1
-            elif layer == 'conv10_1':
-                self.head(what)
-            elif layer == 'conv1_1':
-                {'fprop': self.first_fprop, 'wgrad': self.first_wgrad, 'dgrad': self.first_dgrad}[what]()
-            elif layer in FWD and what in ('fprop', 'dgrad', 'wgrad'):
-                getattr(self, what)(layer)
-            else:
-                self.fail.append('launch %s has no check' % name)
-        self.t.cuda.synchronize()
-        assert not self.fail, '\n'.join(self.fail)
-
-
-def _net(torch, cin=4, cout=4, seed=2018):
-    from eld_b200 import arch
-    torch.manual_seed(seed)
-    return arch.unet(cin, cout).cuda()
-
-
-def _frames(torch, n, c, h, w, seed):
-    g = torch.Generator().manual_seed(seed)
-    return torch.rand(n, c, h, w, generator=g).cuda()
-
-
-def _ws(net, n, h, w, train):
-    return net._engines[(n, h, w, train)][1]
-
-
-def _names(net, eng, run):
-    return [r['name'] for r in net._profile(eng, run, 1)]
+torch = H.torch_fixture(STATS, 'worst case per launch kind (rule: bf16 = max |got-r| / (ulp + 2^-20 S), mismatch rate; '
+                               'fp32 = rel-L2, max-abs / max|r|, max |got-r| / S; exact = elements compared)')
 
 
 def _train(torch, n, cin, cout, h, w, loss='l1', frozen=()):
-    net = _net(torch, cin, cout)
+    net = E.net(cin, cout)
     net.loss_kind = loss
-    for name, p in net.named_parameters():
-        p.requires_grad_(name.split('.')[0] not in frozen)
-    x, t = _frames(torch, n, cin, h, w, 1), _frames(torch, n, cout, h, w, 2)
+    E.freeze_layers(net, frozen)
+    x, t = E.frames(n, cin, cout, h, w, 1)[0], E.frames(n, cout, cout, h, w, 2)[0]    # x and t from seeds of their own
     eng = net._engine(n, h, w, True)
-    ws = _ws(net, n, h, w, True)
-    st = Step(torch, net, eng, ws, x, None, net.flat_grads, t, None, loss, skip_elided={0, 1, 2, 3} if frozen else (),
-              frozen={k for k, p in net.named_parameters() if not p.requires_grad},
+    ws = E.workspace(net, n, h, w, True)
+    st = Step(torch, net, eng, ws, x, None, net.flat_grads, t, None, loss, stats=STATS,
+              skip_elided={0, 1, 2, 3} if frozen else (), frozen={k for k, p in net.named_parameters() if not p.requires_grad},
               tag=' @8x512^2' if n * h * w >= 8 * 512 * 512 else '')
     if frozen:
         for d in ('dcat6', 'dcat7', 'dcat8', 'dcat9'):
@@ -368,7 +52,7 @@ def _train(torch, n, cin, cout, h, w, loss='l1', frozen=()):
 
     def run():
         res['out'], res['loss'] = net.train_step(x, t)
-    names = _names(net, eng, run)
+    names = E.launch_names(net, eng, run)
     st.out, st.loss = res['out'], res['loss']
     return st, names
 
@@ -410,12 +94,10 @@ def test_autograd_seam_launches_with_input_grad(torch):
     """eld_unet_forward + eld_unet_backward (the head's dOut-in mode) + eld_unet_input_grad (conv1_1's data gradient)"""
     from eld_b200 import _lib
     n, h, w = 2, 128, 256
-    net, lib = _net(torch), _lib.load()
-    x = _frames(torch, n, 4, h, w, 3)
+    net, lib = E.net(), _lib.load()
+    x = E.frames(n, 4, 4, h, w, 3)[0]
     eng = net._engine(n, h, w, True)
-    flags = (ctypes.c_uint8 * 46)(*([1] * 46))
-    _lib.check(lib.eld_unet_set_trainable(eng, flags, 46, 1), 'eld_unet_set_trainable')
-    net._masks[eng.value] = ((True,) * 46, True)
+    E.set_trainable(net, eng, [1] * 46, 1)
     g = torch.Generator(device='cuda').manual_seed(4)
     dout = torch.randn(n, 4, h, w, device='cuda', generator=g) * 1e-4
     out, grads, dx = torch.empty(n, 4, h, w, device='cuda'), torch.empty_like(net.flat_params), torch.empty_like(x)
@@ -426,9 +108,9 @@ def test_autograd_seam_launches_with_input_grad(torch):
         _lib.check(lib.eld_unet_forward(eng, p, x.data_ptr(), out.data_ptr(), s), 'eld_unet_forward')
         _lib.check(lib.eld_unet_backward(eng, p, x.data_ptr(), dout.data_ptr(), grads.data_ptr(), s), 'eld_unet_backward')
         _lib.check(lib.eld_unet_input_grad(eng, p, dx.data_ptr(), s), 'eld_unet_input_grad')
-    names = _names(net, eng, run)
+    names = E.launch_names(net, eng, run)
     assert names[-1] == 'conv1_1.dgrad' and 'conv10_1.bwd' in names
-    Step(torch, net, eng, _ws(net, n, h, w, True), x, out, grads, dout=dout, dx=dx).check(names)
+    Step(torch, net, eng, E.workspace(net, n, h, w, True), x, out, grads, dout=dout, dx=dx, stats=STATS).check(names)
 
 
 INFER_CASES = [  # n, cin, cout, h, w
@@ -445,16 +127,16 @@ def test_inference_launches_partial_tiles(torch, case):
     from eld_b200 import _lib
     from tests.launch_ref import buffer
     n, cin, cout, h, w = case
-    net, lib = _net(torch, cin, cout), _lib.load()
-    x = _frames(torch, n, cin, h, w, 5)
+    net, lib = E.net(cin, cout), _lib.load()
+    x = E.frames(n, cin, cout, h, w, 5)[0]
     eng = net._engine(n, h, w, False)
-    ws = _ws(net, n, h, w, False)
+    ws = E.workspace(net, n, h, w, False)
     out = torch.empty(n, cout, h, w, device='cuda')
     s = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    names = _names(net, eng, lambda: _lib.check(lib.eld_unet_forward(eng, net.flat_params.data_ptr(), x.data_ptr(),
-                                                                     out.data_ptr(), s), 'eld_unet_forward'))
+    names = E.launch_names(net, eng, lambda: _lib.check(lib.eld_unet_forward(eng, net.flat_params.data_ptr(), x.data_ptr(),
+                                                                             out.data_ptr(), s), 'eld_unet_forward'))
     assert names[0] == 'weights.pack' and names[-1] == 'conv10_1.fprop' and len(names) == 24
-    Step(torch, net, eng, ws, x, out).check(names)
+    Step(torch, net, eng, ws, x, out, stats=STATS).check(names)
     # an inference workspace holds no training tensors, and an unknown name is an error
     for bad in ('dz9_2', 'dcat6', 'pc1', 'sign:a1_1', 'gtmp', 'nonsense', 'wd:conv1_1', 'wf:conv10_1'):
         with pytest.raises(_lib.EldError):

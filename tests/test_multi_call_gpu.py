@@ -11,31 +11,11 @@ import ctypes
 
 import pytest
 
+from tests import engine_harness as E
+from tests.engine_harness import torch  # noqa: F401 (the fixture)
+
 pytestmark = pytest.mark.gpu
 H, W = 128, 256          # smallest shape the training tiles accept
-
-
-@pytest.fixture(scope='module')
-def torch():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no GPU')
-    return torch
-
-
-def _rel(a, b):
-    return ((a.double() - b.double()).norm() / (b.double().norm() + 1e-30)).item()
-
-
-def _net(torch, seed=2018):
-    from eld_b200 import arch
-    torch.manual_seed(seed)
-    return arch.unet(4, 4).cuda()
-
-
-def _frames(torch, n, seed, h=H, w=W):
-    g = torch.Generator().manual_seed(seed)
-    return torch.rand(n, 4, h, w, generator=g).cuda(), torch.rand(n, 4, h, w, generator=g).cuda()
 
 
 def _l1(torch, out, t):
@@ -61,14 +41,14 @@ def _single(torch, net, x, t):
 
 def _check(torch, net, dx, want_dx, want_g):
     assert torch.equal(dx, want_dx), (dx - want_dx).abs().max().item()
-    assert _rel(_pgrads(torch, net), want_g) <= 1e-5, _rel(_pgrads(torch, net), want_g)
+    assert E.rel(_pgrads(torch, net), want_g) <= 1e-5, E.rel(_pgrads(torch, net), want_g)
 
 
 def test_two_calls_one_backward(torch):
     """l1(net(x1), t1) + l1(net(x2), t2): each call back-propagates its own activations (the second call's state is its
     own), and the sum equals one call on cat([x1, x2]) with twice its mean loss"""
-    net = _net(torch)
-    x, t = _frames(torch, 2, seed=1)
+    net = E.net()
+    x, t = E.frames(2, 4, 4, H, W, seed=1)
     xc = x.clone().requires_grad_()
     _zero(net)
     out_c = net(xc)
@@ -81,13 +61,13 @@ def test_two_calls_one_backward(torch):
     assert torch.equal(torch.cat([o1, o2]).detach(), out_c.detach())
     (_l1(torch, o1, t[:1]) + _l1(torch, o2, t[1:])).backward()
     assert torch.equal(x1.grad, dx_c[:1]) and torch.equal(x2.grad, dx_c[1:])
-    assert _rel(_pgrads(torch, net), g_c) <= 1e-5, _rel(_pgrads(torch, net), g_c)
+    assert E.rel(_pgrads(torch, net), g_c) <= 1e-5, E.rel(_pgrads(torch, net), g_c)
 
 
 @pytest.mark.parametrize('order', [(0, 1), (1, 0)], ids=['first-call-first', 'second-call-first'])
 def test_separate_backwards_in_either_order(torch, order):
-    net = _net(torch)
-    data = [_frames(torch, 2, seed=s) for s in (2, 3)]
+    net = E.net()
+    data = [E.frames(2, 4, 4, H, W, seed=s) for s in (2, 3)]
     refs = [_single(torch, net, x, t) for x, t in data]
     xs = [x.clone().requires_grad_() for x, _ in data]
     losses = [_l1(torch, net(xe), t) for xe, (_, t) in zip(xs, data)]
@@ -100,8 +80,8 @@ def test_separate_backwards_in_either_order(torch, order):
 def test_other_calls_between_forward_and_backward(torch):
     """a train_step, a no_grad inference and a discarded training-mode call of the same shape between a forward and its
     backward: the train step overwrote the built-in state, so the backward runs the forward again into a state of its own"""
-    net = _net(torch)
-    (x1, t1), (x2, t2) = _frames(torch, 2, seed=4), _frames(torch, 2, seed=5)
+    net = E.net()
+    (x1, t1), (x2, t2) = E.frames(2, 4, 4, H, W, seed=4), E.frames(2, 4, 4, H, W, seed=5)
     ref = _single(torch, net, x1, t1)
     xe = x1.clone().requires_grad_()
     out = net(xe)
@@ -118,9 +98,9 @@ def test_other_calls_between_forward_and_backward(torch):
 
 def test_five_shapes_before_one_backward(torch):
     """more live shapes than the module caches plans for: the evicted plan lives on in the call that needs it"""
-    net = _net(torch)
+    net = E.net()
     shapes = [(1, 128, 256), (2, 128, 256), (1, 256, 256), (1, 128, 512), (2, 256, 256)]
-    data = [_frames(torch, n, seed=10 + i, h=h, w=w) for i, (n, h, w) in enumerate(shapes)]
+    data = [E.frames(n, 4, 4, h, w, seed=10 + i) for i, (n, h, w) in enumerate(shapes)]
     refs = [_single(torch, net, x, t) for x, t in data]
     xs = [x.clone().requires_grad_() for x, _ in data]
     loss = sum(_l1(torch, net(xe), t) for xe, (_, t) in zip(xs, data))
@@ -130,13 +110,13 @@ def test_five_shapes_before_one_backward(torch):
     for xe, (dx, _) in zip(xs, refs):
         assert torch.equal(xe.grad, dx)
     g_sum = sum(g for _, g in refs)
-    assert _rel(_pgrads(torch, net), g_sum) <= 1e-5, _rel(_pgrads(torch, net), g_sum)
+    assert E.rel(_pgrads(torch, net), g_sum) <= 1e-5, E.rel(_pgrads(torch, net), g_sum)
 
 
 def test_module_cuda_between_forward_and_backward(torch):
     """.cuda() re-flattens the parameters and drops every cached plan; the pending call keeps its own"""
-    net = _net(torch)
-    x, t = _frames(torch, 2, seed=6)
+    net = E.net()
+    x, t = E.frames(2, 4, 4, H, W, seed=6)
     ref = _single(torch, net, x, t)
     xe = x.clone().requires_grad_()
     loss = _l1(torch, net(xe), t)
@@ -154,8 +134,8 @@ def test_retain_graph(torch, between):
     """a second backward of a retained graph adds the same gradient again; with a same-shape forward in between, the
     built-in state belongs to that newer call, so the old one recomputes its forward - and leaves the newer call's state
     alone"""
-    net = _net(torch)
-    (x, t), (x2, t2) = _frames(torch, 2, seed=7), _frames(torch, 2, seed=8)
+    net = E.net()
+    (x, t), (x2, t2) = E.frames(2, 4, 4, H, W, seed=7), E.frames(2, 4, 4, H, W, seed=8)
     ref2 = _single(torch, net, x2, t2)
     xe = x.clone().requires_grad_()
     loss = _l1(torch, net(xe), t)
@@ -167,7 +147,7 @@ def test_retain_graph(torch, between):
         loss2 = _l1(torch, net(x2e), t2)
     loss.backward()
     assert torch.equal(xe.grad, 2 * dx1)
-    assert _rel(_pgrads(torch, net), 2 * g1) <= 1e-5, _rel(_pgrads(torch, net), 2 * g1)
+    assert E.rel(_pgrads(torch, net), 2 * g1) <= 1e-5, E.rel(_pgrads(torch, net), 2 * g1)
     with pytest.raises(RuntimeError):
         loss.backward()
     if between:
@@ -181,8 +161,8 @@ def test_checkpoint(torch, calls):
     """torch.utils.checkpoint (non-reentrant) around the module: the recomputed forward saves the same tensors as the
     original whichever forward state either of them got; with two calls, the backwards run first call first"""
     from torch.utils.checkpoint import checkpoint
-    net = _net(torch)
-    data = [_frames(torch, 2, seed=s) for s in (9, 10)][:calls]
+    net = E.net()
+    data = [E.frames(2, 4, 4, H, W, seed=s) for s in (9, 10)][:calls]
     refs = [_single(torch, net, x, t) for x, t in data]
     xs = [x.clone().requires_grad_() for x, _ in data]
     losses = [_l1(torch, checkpoint(net, xe, use_reentrant=False), t) for xe, (_, t) in zip(xs, data)]
@@ -194,9 +174,9 @@ def test_checkpoint(torch, calls):
 
 def test_inplace_weight_change_raises(torch):
     from eld_b200 import arch
-    net = _net(torch)
+    net = E.net()
     opt = arch.FusedAdam(net)
-    x, t = _frames(torch, 2, seed=11)
+    x, t = E.frames(2, 4, 4, H, W, seed=11)
     loss = _l1(torch, net(x), t)
     opt.step()                                   # FusedAdam rewrites the flat buffer in place
     with pytest.raises(RuntimeError, match='inplace'):
@@ -216,9 +196,9 @@ def test_one_call_per_backward_loop_stays_on_the_built_in_state(torch):
     """ELDModel's forward() / backward_G() / step loop, the previous output still referenced at the next forward: every
     call takes the built-in state, and the allocated memory does not grow after the first step"""
     from eld_b200 import arch
-    net = _net(torch)
+    net = E.net()
     opt = arch.FusedAdam(net)
-    data = [_frames(torch, 2, seed=20 + i) for i in range(5)]
+    data = [E.frames(2, 4, 4, H, W, seed=20 + i) for i in range(5)]
     output, mem = None, []
     for x, t in data:
         output = net(x)
@@ -235,8 +215,8 @@ def test_launch_list_is_the_single_call_list(torch):
     """an autograd step on the built-in state and one on a state of its own launch what eld_unet_forward +
     eld_unet_backward launch, in the same order"""
     from eld_b200 import _lib
-    net, lib = _net(torch), _lib.load()
-    x, t = _frames(torch, 2, seed=12)
+    net, lib = E.net(), _lib.load()
+    x, t = E.frames(2, 4, 4, H, W, seed=12)
     eng = net._engine(2, H, W, True)
     net._set_trainable(eng, [True] * 46, False)
     out, grads = torch.empty_like(t), torch.empty_like(net.flat_params)
@@ -253,9 +233,9 @@ def test_launch_list_is_the_single_call_list(torch):
         o = net(x)
         took.append(o.grad_fn.state is not None)
         _l1(torch, o, t).backward()
-    names = [[r['name'] for r in net._profile(eng, run, 1)] for run in (abi, step)]
+    names = [E.launch_names(net, eng, run) for run in (abi, step)]
     hold = net(x)                                # holds the built-in state: the profiled steps take states of their own
-    names.append([r['name'] for r in net._profile(eng, step, 1)])
+    names.append(E.launch_names(net, eng, step))
     assert took == [False, False, True, True] and hold.grad_fn.state is None
     assert names[0][0] == 'weights.pack' and 'conv10_1.bwd' in names[0]
     assert names[1] == names[0] and names[2] == names[0]
@@ -265,8 +245,8 @@ def test_state_entry_points(torch):
     """the C ABI directly: a caller state survives other forwards on the same object and stays valid after a backward
     read it; eld_unet_input_grad follows eld_unet_backward_state; the state calls refuse an inference object"""
     from eld_b200 import _lib
-    net, lib = _net(torch), _lib.load()
-    (x1, t1), (x2, _) = _frames(torch, 2, seed=13), _frames(torch, 2, seed=14)
+    net, lib = E.net(), _lib.load()
+    (x1, t1), (x2, _) = E.frames(2, 4, 4, H, W, seed=13), E.frames(2, 4, 4, H, W, seed=14)
     eng = net._engine(2, H, W, True)
     net._set_trainable(eng, [True] * 46, True)
     s = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
@@ -289,7 +269,7 @@ def test_state_entry_points(torch):
     for _ in range(2):
         got = backward(sp)
         assert torch.equal(got[0], want[0]) and torch.equal(got[2], want[2])
-        assert _rel(got[1], want[1]) <= 1e-5, _rel(got[1], want[1])
+        assert E.rel(got[1], want[1]) <= 1e-5, E.rel(got[1], want[1])
     inf = net._engine(2, H, W, False)
     with pytest.raises(_lib.EldError):
         _lib.check(lib.eld_unet_forward_state(inf, sp, p, x1.data_ptr(), out.data_ptr(), s), 'eld_unet_forward_state')

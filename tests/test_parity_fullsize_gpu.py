@@ -17,44 +17,11 @@ Gates (bf16 operands / activations / stored gradients, fp32 accumulation):
 import numpy as np
 import pytest
 
+from tests import engine_harness as E
+from tests.engine_harness import torch  # noqa: F401 (the fixture)
+
 pytestmark = pytest.mark.gpu
 SONY = (2.2881136684755243, 6.4508722699636545, 15583, 208.9766365993794)
-
-
-@pytest.fixture(scope='module')
-def torch():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no GPU')
-    return torch
-
-
-def _rel(a, b):
-    return ((a.double() - b.double()).norm() / (b.double().norm() + 1e-300)).item()
-
-
-def _pair(torch, seed=2018):
-    from eld_b200 import arch
-    from oracle.unet_ref import UNetSeeInDarkRef
-    torch.manual_seed(seed)
-    ours = arch.unet(4, 4).cuda()
-    torch.manual_seed(seed)
-    ref = UNetSeeInDarkRef(4, 4).cuda()
-    for (k, p), (k2, q) in zip(ref.named_parameters(), ours.named_parameters()):
-        assert k == k2 and torch.equal(p.detach(), q.detach())
-    return ours, ref
-
-
-def _spread_biases(torch, ours, ref):
-    """The default init leaves most pre-activations on one side of LeakyReLU's kink; widen the biases (both nets,
-    identically) so both branches - and both values of the backward mask - carry real weight."""
-    g = torch.Generator().manual_seed(5)
-    with torch.no_grad():
-        for (k, p), (_, q) in zip(ref.named_parameters(), ours.named_parameters()):
-            if k.endswith('.bias'):
-                d = (torch.rand(p.shape, generator=g) - 0.5).to(p.device) * 0.2
-                p.add_(d)
-                q.add_(d)
 
 
 def test_cuda_fp32_oracle_equals_the_pinned_cpu_oracle(torch):
@@ -72,17 +39,16 @@ def test_cuda_fp32_oracle_equals_the_pinned_cpu_oracle(torch):
     ref.cuda()
     out_g = fp32_cuda(lambda: ref(x.cuda()))
     fp32_cuda(lambda: torch.nn.functional.l1_loss(out_g, t.cuda()).backward())
-    assert _rel(out_g.detach().cpu(), out_c.detach()) <= 1e-5
+    assert E.rel(out_g.detach().cpu(), out_c.detach()) <= 1e-5
     for k, p in ref.named_parameters():
-        assert _rel(p.grad.cpu(), gc[k]) <= 2e-4, k
+        assert E.rel(p.grad.cpu(), gc[k]) <= 2e-4, k
 
 
 def test_inference_1x4x512x512_config1(torch):
     """BASELINE configs[1]: U-Net inference 1 x 4 x 512 x 512 with SonyA7S2 noise on a smooth frame."""
     from eld_b200.noise import NoiseModel
     from tests.unet_emul import emulated_forward, fp32_cuda, smooth_frames
-    ours, ref = _pair(torch)
-    _spread_biases(torch, ours, ref)
+    ours, ref = E.pair()
     clean = smooth_frames(1, 512, 512, seed=11, device='cuda')
     x = NoiseModel('P+g', include=4, verbose=False, seed=2018).batch_gpu(clean, params=SONY, frame_id0=0)
     with torch.no_grad():
@@ -90,16 +56,15 @@ def test_inference_1x4x512x512_config1(torch):
         emu = fp32_cuda(lambda: emulated_forward(ref, x))
     got = ours(x)
     assert torch.isfinite(got).all()
-    assert _rel(got, emu) <= 3e-3, _rel(got, emu)
-    assert _rel(got, want) <= 2e-2, _rel(got, want)
+    assert E.rel(got, emu) <= 3e-3, E.rel(got, emu)
+    assert E.rel(got, want) <= 2e-2, E.rel(got, want)
 
 
 def test_train_step_8x4x512x512_config2(torch):
     """BASELINE configs[2]: the batch-8 training step.  Every one of the 46 gradient tensors is gated."""
     from tests.unet_emul import emulated_train_step, fp32_cuda, smooth_frames
     from eld_b200.noise import NoiseModel
-    ours, ref = _pair(torch)
-    _spread_biases(torch, ours, ref)
+    ours, ref = E.pair()
     clean = smooth_frames(8, 512, 512, seed=12, device='cuda')
     x = NoiseModel('P+g', include=4, verbose=False, seed=2018).batch_gpu(clean, params=[SONY] * 8, frame_id0=0)
 
@@ -115,11 +80,11 @@ def test_train_step_8x4x512x512_config2(torch):
     o32, l32, g32 = fp32_cuda(fp32_step)
     oem, lem, gem = fp32_cuda(lambda: emulated_train_step(ref, x, clean))
 
-    assert _rel(out, oem) <= 3e-3, _rel(out, oem)
-    assert _rel(out, o32) <= 2e-2, _rel(out, o32)
+    assert E.rel(out, oem) <= 3e-3, E.rel(out, oem)
+    assert E.rel(out, o32) <= 2e-2, E.rel(out, o32)
     assert abs(loss.item() - lem.item()) <= 2e-3 * lem.item(), (loss.item(), lem.item())
     assert abs(loss.item() - l32.item()) <= 1e-2 * l32.item(), (loss.item(), l32.item())
-    table = [(k, _rel(mine[k], gem[k]), _rel(mine[k], g32[k])) for k in mine]
+    table = [(k, E.rel(mine[k], gem[k]), E.rel(mine[k], g32[k])) for k in mine]
     print('\n'.join('%-18s emu %.2e   fp32 %.2e' % r for r in table))
     bad = [r for r in table if not (r[1] <= 2e-3 and r[2] <= 5e-2)]
     assert not bad, bad
@@ -136,7 +101,7 @@ def test_dpsnr_after_200_adam_steps(torch):
     from tests.unet_emul import fp32_cuda, smooth_frames
     from eld_b200 import arch
     from eld_b200.noise import NoiseModel
-    ours, ref = _pair(torch)
+    ours, ref = E.pair(spread=False)
     nm = NoiseModel('P+g', include=4, verbose=False, seed=2018)
     opt_o = arch.FusedAdam(ours, lr=2e-4)
     opt_r = torch.optim.Adam(ref.parameters(), lr=2e-4, betas=(0.9, 0.999))
@@ -172,8 +137,7 @@ def test_dpsnr_after_200_adam_steps(torch):
 def test_mse_loss_train_step(torch):
     """--loss l2 (models/losses.py:33-34, nn.MSELoss): loss and every gradient tensor against the emulated backward."""
     from tests.unet_emul import emulated_train_step, fp32_cuda, smooth_frames
-    ours, ref = _pair(torch)
-    _spread_biases(torch, ours, ref)
+    ours, ref = E.pair()
     ours.loss_kind = 'l2'
     clean = smooth_frames(2, 256, 256, seed=21, device='cuda')
     x = (clean + 0.05 * torch.randn_like(clean)).clamp(0, 1)
@@ -183,6 +147,6 @@ def test_mse_loss_train_step(torch):
     want = fp32_cuda(lambda: torch.nn.functional.mse_loss(ref(x), clean))
     assert abs(loss.item() - lem.item()) <= 2e-3 * lem.item(), (loss.item(), lem.item())
     assert abs(loss.item() - want.item()) <= 1e-2 * want.item()
-    bad = [(k, _rel(mine[k], gem[k])) for k in mine if _rel(mine[k], gem[k]) > 5e-3]
+    bad = [(k, E.rel(mine[k], gem[k])) for k in mine if E.rel(mine[k], gem[k]) > 5e-3]
     assert not bad, bad
     ours.loss_kind = 'l1'

@@ -6,6 +6,7 @@ import pytest
 import torch
 
 from tests import plan_ref as P
+from tests.engine_harness import AUTOGRAD, ENC, FWD_NAMES, TRAIN_STEP, without
 
 # the masks test_plans_gpu.py runs, plus a few hundred more
 RANDOM = P.random_masks(300, seed=11)
@@ -75,8 +76,8 @@ def test_whole_block_plans(ref):
 
 
 def test_launch_lists_of_the_whole_block_plans():
-    """plan_ref's launch lists equal the ones test_frozen_gpu.py asserts the engine issues"""
-    from tests.test_frozen_gpu import AUTOGRAD, ENC, TRAIN_STEP, _FWD, _without
+    """plan_ref's launch lists equal the lists pinned in tests/engine_harness.py, which test_frozen_gpu.py asserts the
+    engine issues"""
     assert tuple(P.ENC) == ENC
     every = P.Plan(P.everything_but())
     assert every.launches() == TRAIN_STEP
@@ -84,14 +85,14 @@ def test_launch_lists_of_the_whole_block_plans():
     assert every.autograd_launches(x_grad=True) == AUTOGRAD + ['conv1_1.dgrad']
     assert every.prefix_levels() == set()
     enc = P.Plan(P.everything_but(ENC))
-    assert enc.launches() == _without(TRAIN_STEP, ENC, drop=('pool.bwd', 'upv6.dgrad'))
+    assert enc.launches() == without(TRAIN_STEP, ENC, drop=('pool.bwd', 'upv6.dgrad'))
     assert enc.prefix_levels() == {0, 1, 2, 3}
     dec = P.Plan(P.everything_but(P.NAMES[10:]))
     assert [n for n in dec.launches() if not n.endswith('.wgrad')] == [n for n in TRAIN_STEP if not n.endswith('.wgrad')]
     net = P.Plan(P.everything_but(P.NAMES), input_grad=True)     # (the ABI's train step after set_trainable(.., 1))
-    assert net.launches() == _FWD + ['conv10_1.fwd+loss+bwd'] + [n for n in TRAIN_STEP if n.endswith(('.dgrad', 'pool.bwd'))]
+    assert net.launches() == FWD_NAMES + ['conv10_1.fwd+loss+bwd'] + [n for n in TRAIN_STEP if n.endswith(('.dgrad', 'pool.bwd'))]
     assert net.autograd_launches() == [n for n in AUTOGRAD if not n.endswith('.wgrad') and n != 'weights.gperm'] + ['conv1_1.dgrad']
-    assert P.Plan(P.mask()).launches() == _FWD + ['conv10_1.fwd+loss']
+    assert P.Plan(P.mask()).launches() == FWD_NAMES + ['conv10_1.fwd+loss']
 
 
 def test_mixed_plans():

@@ -6,7 +6,7 @@ what those never do in one step: row-prefix concat gradients at some levels and 
 at some levels only, a weight frozen while its bias trains and the other way round, one layer deep inside the network
 training alone.  Per mask, on the weights and batch of one cached all-trainable step (2 x 4 x 128 x 256):
   a. the launch list of train_step and of the autograd forward + backward is plan_ref's;
-  b. every launch of the train step is checked on its own inputs (tests/test_launches_gpu.py's Step and gates);
+  b. every launch of the train step is checked on its own inputs (tests/launch_check.py's Step and gates);
   c. no stray writes: every dz / dcat plane / dp the plan does not produce keeps a NaN sentinel bit for bit, and every
      one it produces is finite;
   d. a frozen tensor's range of flat_grads is exactly zero and its .grad None; the trainable ones agree with the
@@ -14,10 +14,14 @@ training alone.  Per mask, on the weights and batch of one cached all-trainable 
      layer is reached, so x.grad and every data gradient are bit-identical to the all-trainable autograd step;
   e. FusedAdam leaves frozen tensors bit-unchanged.
 Then one mixed mask data parallel (NCCL, world size 1) and one at 8 x 4 x 512 x 512 under the production gates."""
+from collections import defaultdict
+
 import pytest
 
+from tests import engine_harness as E
 from tests import plan_ref as P
-from tests.test_launches_gpu import NAN_BITS, STATS, Step
+from tests.abi_harness import torch_fixture
+from tests.launch_check import NAN_BITS, Step
 
 pytestmark = pytest.mark.gpu
 N, H, W = 2, 128, 256
@@ -27,46 +31,13 @@ CASES = [pytest.param(f, g, id=name) for name, f, g in P.NAMED] + [pytest.param(
 # tensor trains in every kind of weight-gradient launch (conv3x3 bias, conv3x3 weight, deconv weight, head bias)
 MIXED = P.everything_but(['conv1_1', 'conv1_2', 'conv2_1', 'conv2_2'],
                          ['conv5_2.bias', 'conv7_1.weight', 'upv8.weight', 'conv10_1.bias'])
+STATS = defaultdict(lambda: defaultdict(float))     # launch kind -> worst measured value per statistic
 
-
-@pytest.fixture(scope='module')
-def torch():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no GPU')
-    STATS.clear()
-    yield torch
-    print('\nworst case per launch kind over the mixed plans (rules as in test_launches_gpu.py)')
-    for kind in sorted(STATS):
-        print('  %-24s %s' % (kind, '  '.join('%s=%.3g' % kv for kv in sorted(STATS[kind].items()))))
-
-
-def _rel(a, b):
-    return ((a.double() - b.double()).norm() / (b.double().norm() + 1e-30)).item()
-
-
-def _net(torch):
-    from eld_b200 import arch
-    torch.manual_seed(2018)
-    return arch.unet(4, 4).cuda()
-
-
-def _frames(torch, n, h, w, seed):
-    g = torch.Generator().manual_seed(seed)
-    return torch.rand(n, 4, h, w, generator=g).cuda(), torch.rand(n, 4, h, w, generator=g).cuda()
-
-
-def _apply(net, flags):
-    for p, f in zip(net.parameters(), flags):
-        p.requires_grad_(bool(f))
+torch = torch_fixture(STATS, 'worst case per launch kind over the mixed plans (rules as in test_launches_gpu.py)')
 
 
 def _ranges(net):
     return dict(zip(P.PARAMS, net._spans))
-
-
-def _names(net, eng, run):
-    return [r['name'] for r in net._profile(eng, run, 1)]
 
 
 def _scratch(torch, net, eng, ws):
@@ -90,10 +61,10 @@ class Base:
 
     def __init__(self, torch):
         import torch.nn.functional as F
-        self.net = net = _net(torch)
-        self.x, self.t = _frames(torch, N, H, W, seed=1)
+        self.net = net = E.net()
+        self.x, self.t = E.frames(N, 4, 4, H, W, seed=1)
         self.eng = net._engine(N, H, W, True)
-        self.ws = net._engines[(N, H, W, True)][1]
+        self.ws = E.workspace(net, N, H, W, True)
         self.p0 = net.flat_params.clone()
         out, _ = net.train_step(self.x, self.t)
         self.out, self.grads = out.clone(), net.flat_grads.clone()
@@ -124,17 +95,17 @@ def test_train_step(torch, base, flags, input_grad):
     net, x, t = base.net, base.x, base.t
     plan = P.Plan(flags, False)              # train_step never asks for x.grad
     net.flat_params.copy_(base.p0)           # (FusedAdam below moves them)
-    _apply(net, flags)
+    E.apply_flags(net, flags)
     bufs = _scratch(torch, net, base.eng, base.ws)
     for v in bufs.values():
         v.fill_(NAN_BITS)
-    st = Step(torch, net, base.eng, base.ws, x, None, net.flat_grads, t, None, 'l1', skip_elided=plan.prefix_levels(),
-              frozen=plan.frozen)
+    st = Step(torch, net, base.eng, base.ws, x, None, net.flat_grads, t, None, 'l1', stats=STATS,
+              skip_elided=plan.prefix_levels(), frozen=plan.frozen)
     res = {}
 
     def run():
         res['out'], res['loss'] = net.train_step(x, t)
-    names = _names(net, base.eng, run)
+    names = E.launch_names(net, base.eng, run)
     st.out, st.loss = res['out'], res['loss']
     # a. the launch list
     assert names == plan.launches()
@@ -158,8 +129,8 @@ def test_train_step(torch, base, flags, input_grad):
     if live:
         got = torch.cat([net.flat_grads[span[k][0]:sum(span[k])] for k in live])
         want = torch.cat([base.grads[span[k][0]:sum(span[k])] for k in live])
-        assert _rel(got, want) <= 1e-4
-        worst = max((_rel(net.flat_grads[span[k][0]:sum(span[k])], base.grads[span[k][0]:sum(span[k])]), k) for k in live)
+        assert E.rel(got, want) <= 1e-4
+        worst = max((E.rel(net.flat_grads[span[k][0]:sum(span[k])], base.grads[span[k][0]:sum(span[k])]), k) for k in live)
         assert worst[0] <= 1e-2, worst
     # e. Adam moves the trainable tensors only
     opt = arch.FusedAdam(net, lr=1e-3, weight_decay=1e-2)
@@ -178,7 +149,7 @@ def test_autograd(torch, base, flags, input_grad):
     net, t = base.net, base.t
     plan = P.Plan(flags, input_grad)
     net.flat_params.copy_(base.p0)
-    _apply(net, flags)
+    E.apply_flags(net, flags)
     xi = base.x.clone().requires_grad_(input_grad)
     if not plan.reach['conv10_1']:           # nothing asks for a gradient: the output is not part of a graph
         assert not net(xi).requires_grad
@@ -190,7 +161,7 @@ def test_autograd(torch, base, flags, input_grad):
         for p in net.parameters():
             p.grad = None
         F.l1_loss(net(xi), t).backward()
-    names = _names(net, base.eng, run)
+    names = E.launch_names(net, base.eng, run)
     assert names == plan.autograd_launches()
     span = _ranges(net)
     live = [k for k in P.PARAMS if plan.trains[k]]
@@ -199,10 +170,10 @@ def test_autograd(torch, base, flags, input_grad):
     if live:
         got = torch.cat([p.grad.reshape(-1) for k, p in zip(P.PARAMS, net.parameters()) if plan.trains[k]])
         want = torch.cat([base.grads[span[k][0]:sum(span[k])] for k in live])
-        assert _rel(got, want) <= 1e-4
+        assert E.rel(got, want) <= 1e-4
         for k, p in zip(P.PARAMS, net.parameters()):
             if plan.trains[k]:
-                assert _rel(p.grad.reshape(-1), base.grads[span[k][0]:sum(span[k])]) <= 1e-2, k
+                assert E.rel(p.grad.reshape(-1), base.grads[span[k][0]:sum(span[k])]) <= 1e-2, k
     if input_grad:
         # every layer is reached: the data-gradient chain is the all-trainable one, bit for bit
         assert torch.equal(xi.grad, base.dx)
@@ -224,9 +195,9 @@ def test_ddp_world1_mixed_mask(torch, monkeypatch):
     dist.init_process_group('nccl', init_method='tcp://127.0.0.1:%d' % port, rank=0, world_size=1,
                             device_id=torch.device('cuda', 0))
     try:
-        net = _net(torch)
-        _apply(net, flags)
-        x, t = _frames(torch, N, H, W, seed=7)
+        net = E.net()
+        E.apply_flags(net, flags)
+        x, t = E.frames(N, 4, 4, H, W, seed=7)
         net.train_step(x, t)
         want = net.flat_grads.clone()
         calls = []
@@ -237,12 +208,12 @@ def test_ddp_world1_mixed_mask(torch, monkeypatch):
         torch.cuda.synchronize()
         buckets = net.grad_buckets()
         assert calls == [buckets[0][1], buckets[1][1]]
-        assert _rel(net.flat_grads, want) < 1e-3
+        assert E.rel(net.flat_grads, want) < 1e-3
         for k, (o, c) in _ranges(net).items():
             if not plan.trains[k]:
                 assert not net.flat_grads[o:o + c].any(), k
         eng = net._engine(N, H, W, True)       # bucket events stay on: the permute runs per bucket
-        assert _names(net, eng, lambda: net.train_step(x, t)) == plan.launches(per_bucket=True)
+        assert E.launch_names(net, eng, lambda: net.train_step(x, t)) == plan.launches(per_bucket=True)
     finally:
         dist.destroy_process_group()
 
@@ -250,22 +221,22 @@ def test_ddp_world1_mixed_mask(torch, monkeypatch):
 def test_mixed_mask_production_shape(torch):
     """8 x 4 x 512 x 512 under the production weight-gradient gates"""
     n, h, w = 8, 512, 512
-    net = _net(torch)
+    net = E.net()
     plan = P.Plan(MIXED)
     assert plan.prefix_levels() == {0, 1}
-    _apply(net, MIXED)
-    x, t = _frames(torch, n, h, w, seed=9)
+    E.apply_flags(net, MIXED)
+    x, t = E.frames(n, 4, 4, h, w, seed=9)
     eng = net._engine(n, h, w, True)
-    ws = net._engines[(n, h, w, True)][1]
-    st = Step(torch, net, eng, ws, x, None, net.flat_grads, t, None, 'l1', skip_elided=plan.prefix_levels(),
-              frozen=plan.frozen, tag=' @8x512^2')
+    ws = E.workspace(net, n, h, w, True)
+    st = Step(torch, net, eng, ws, x, None, net.flat_grads, t, None, 'l1', stats=STATS,
+              skip_elided=plan.prefix_levels(), frozen=plan.frozen, tag=' @8x512^2')
     for lvl in plan.prefix_levels():
         st.bits(st.planes('dcat%d' % (9 - lvl))[1]).fill_(NAN_BITS)
     res = {}
 
     def run():
         res['out'], res['loss'] = net.train_step(x, t)
-    names = _names(net, eng, run)
+    names = E.launch_names(net, eng, run)
     st.out, st.loss = res['out'], res['loss']
     assert names == plan.launches()
     st.check(names)

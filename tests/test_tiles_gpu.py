@@ -22,155 +22,27 @@ file and test_conv_gpu.py: a max |got-r| / (ulp + 2^-20 S) of 0.5 for every kern
 shares of 1.8e-4 to 4.3e-4 for the thin tiles, 4.3e-4 / 7.9e-4 / 2.8e-3 for the wide and deconv tiles of N tile 32 /
 64 / 128 together (the deep K of the 512-channel layers), which share a gate per N tile; weight gradients at rel-L2
 2.8e-7 to 4.9e-7 and max-abs 3.0e-7 to 8.0e-7 of max|r|.  The whole file runs in about 8 s there.  The worst case per
-kernel is printed at the end (pytest -s)."""
-from collections import defaultdict
-
+kernel is printed at the end (pytest -s).  The gates and the check of one case are tests/tile_check.py's."""
 import pytest
 
 from tests import abi_harness as H
 from tests import tile_cases as T
-from tests.abi_harness import NAN16, Guarded
+from tests import tile_check as C
+from tests.abi_harness import NAN16
 
 pytestmark = pytest.mark.gpu
 
-MISMATCH = {'conv3x3_thin<32,32>': 1.1e-3, 'conv3x3_thin<32,64>': 1.7e-3, 'conv3x3_thin<64,32>': 7e-4,
-            'conv3x3_thin<64,64>': 1.7e-3, 'conv3x3_wide<32,32>': 1.7e-3, 'conv3x3_wide<32,64>': 1.7e-3,
-            'conv3x3_wide<64,32>': 3.2e-3, 'conv3x3_wide<64,64>': 3.2e-3, 'conv3x3_wide<128,32>': 1.1e-2,
-            'conv3x3_wide<128,64>': 1.1e-2, 'conv_gemm<32>': 1.7e-3, 'conv_gemm<64>': 3.2e-3, 'conv_gemm<128>': 1.1e-2}
-WGRAD_REL_L2 = {'conv3x3_wgrad_thin<32,32>': 1.2e-6, 'conv3x3_wgrad_thin<32,64>': 1.2e-6,
-                'conv3x3_wgrad_thin<64,32>': 1.2e-6, 'conv3x3_wgrad_thin<64,64>': 1.2e-6,
-                'wgrad_gemm<32>': 2e-6, 'wgrad_gemm<64>': 1.2e-6, 'wgrad_gemm<128>': 1.2e-6}
-WGRAD_MAX_ABS = {'conv3x3_wgrad_thin<32,32>': 3.2e-6, 'conv3x3_wgrad_thin<32,64>': 2.3e-6,
-                 'conv3x3_wgrad_thin<64,32>': 3e-6, 'conv3x3_wgrad_thin<64,64>': 2.9e-6,
-                 'wgrad_gemm<32>': 2.4e-6, 'wgrad_gemm<64>': 1.7e-6, 'wgrad_gemm<128>': 1.3e-6}
-BIG = 1000.0                   # scale of the odd images
-
-STATS = defaultdict(lambda: defaultdict(float))     # kernel -> worst measured value per statistic
-
-torch = H.torch_fixture(STATS, 'worst case per kernel (bf16: max |got-r| / (ulp + 2^-20 S), mismatch rate; '
-                               'fp32: rel-L2, max-abs / max|r|)')
+torch = H.torch_fixture(C.STATS, 'worst case per kernel (bf16: max |got-r| / (ulp + 2^-20 S), mismatch rate; '
+                                 'fp32: rel-L2, max-abs / max|r|)')
 
 
 def _sms(torch):
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-def _operand(torch, g, n, h, w, pitch, big_odd=True):
-    """bf16 NHWC [n,h,w,pitch]: standard normal, the odd (or even) images x BIG"""
-    scale = torch.ones(n, 1, 1, 1, device='cuda')
-    scale[(1 if big_odd else 0)::2] = BIG
-    return (torch.randn(n, h, w, pitch, device='cuda', generator=g) * scale).bfloat16()
-
-
-def _output(torch, n, h, w, pitch):
-    """bf16 NHWC [n,h,w,pitch] between two guard images of NAN16 -> (its Guarded allocation, the output tensor)"""
-    out = Guarded(torch, n * h * w * pitch, h * w * pitch, dtype=torch.bfloat16)
-    return out, out.view.view(n, h, w, pitch)
-
-
-def _written(torch, out, y, c0, c):
-    """elements written outside channels [c0, c0 + c) of the output y: in the guard images and in y's other channels"""
-    b = y.view(torch.int16).clone()
-    b[..., c0:c0 + c] = NAN16
-    return out.written_guards() + int((b != NAN16).sum().item())
-
-
-def _prims_traced(torch, call, expect, where, state=()):
-    """call(), an eld_b200.prims wrapper (it raises EldError where the C call fails), held to the launches `expect` by
-    abi_harness.traced -> what call() returned"""
-    got = []
-
-    def fn():
-        got.append(call())
-        return 0
-    H.traced(torch, fn, expect, where, T.canonical, state, STATS)
-    return got[-1]
-
-
-def _bf16_check(kernel, where, got, r, S):
-    from tests.launch_ref import bf16_rule
-    ratio, mism, finite = bf16_rule(got, r, S)
-    st = STATS['bf16 ' + kernel]
-    st['ulp_ratio'] = max(st['ulp_ratio'], ratio)
-    st['mismatch'] = max(st['mismatch'], mism)
-    assert ratio <= 1.0 and mism <= MISMATCH[kernel] and finite, \
-        '%s (%s): max |got-r|/(ulp+2^-20 S) = %.3g, mismatch %.3g, finite %s' % (where, kernel, ratio, mism, finite)
-
-
-def _f32_check(kernel, where, got, r, S):
-    from tests.launch_ref import f32_rule
-    rel, mx, _ = f32_rule(got, r, S)
-    st = STATS['fp32 ' + kernel]
-    st['rel_l2'] = max(st['rel_l2'], rel)
-    st['max_abs_rel'] = max(st['max_abs_rel'], mx)
-    assert rel <= WGRAD_REL_L2[kernel] and mx <= WGRAD_MAX_ABS[kernel], \
-        '%s (%s): rel-L2 %.3g, max-abs / max|r| %.3g' % (where, kernel, rel, mx)
-
-
-def run_case(torch, c, seed):
-    """one primitive call of case c, traced, then checked against its float64 reference and its guards"""
-    from eld_b200 import prims
-    import tests.launch_ref as R
-    g = torch.Generator(device='cuda').manual_seed(seed)
-    kern = T.kernel(c)[0]
-    where = T.case_id(c)
-    fine = c.op.startswith('deconv')
-    if c.op.endswith('wgrad'):
-        x = _operand(torch, g, c.n, c.h, c.w, c.x_pitch)
-        f = 2 if fine else 1
-        # the second operand is large on the EVEN images: a product across an image border is BIG^2
-        q = _operand(torch, g, c.n, f * c.h, f * c.w, c.y_pitch, big_odd=False)
-        xs, qs = x[..., c.x_c0:c.x_c0 + c.ci], q[..., c.y_c0:c.y_c0 + c.co]
-        r, S, _, _ = (R.deconv_wgrad if fine else R.conv_wgrad)(xs, qs)
-        dw0 = torch.randn(r.shape, device='cuda', generator=g) * r.abs().max().float()
-        out = Guarded(torch, r.numel(), 256)
-        dw = out.view.view(r.shape)
-        dw.copy_(dw0)
-        wgrad = prims.deconv2x2_wgrad if fine else prims.conv3x3_wgrad
-        _prims_traced(torch, lambda: wgrad(x, c.x_c0, c.ci, q, c.y_c0, c.co, dw), {kern: 1}, where, state=(dw,))
-        assert out.written_guards() == 0, '%s: dW guard written' % where
-        _f32_check(kern, where, dw, r + dw0.double(), S + dw0.double().abs())
-        return
-    ih, iw = (2 * c.h, 2 * c.w) if c.op == 'deconv.dgrad' else (c.h, c.w)
-    oh, ow = (2 * c.h, 2 * c.w) if c.op == 'deconv' else (c.h, c.w)
-    x = _operand(torch, g, c.n, ih, iw, c.x_pitch)
-    xs = x[..., c.x_c0:c.x_c0 + c.ci]
-    out, y = _output(torch, c.n, oh, ow, c.y_pitch)
-    aux = _operand(torch, g, c.n, c.h, c.w, c.aux_pitch) if c.act == prims.ACT_MASK else None
-    auxs = aux[..., c.aux_c0:c.aux_c0 + c.co] if aux is not None else None
-    if c.op == 'conv':
-        W = torch.randn(c.co, c.ci, 3, 3, device='cuda', generator=g) / (3 * c.ci ** 0.5)
-        b = torch.randn(c.co, device='cuda', generator=g) if c.bias else None
-        wp = prims.pack_weights(W, prims.PACK_CONV_FPROP)
-        call = lambda: prims.conv3x3(x, c.x_c0, c.ci, wp, b, y, c.y_c0, c.co, act=c.act)  # noqa: E731
-        r, S = R.conv_fprop(xs, W, b, act=c.act == prims.ACT_LRELU)
-    elif c.op == 'conv.dgrad':
-        W = torch.randn(c.ci, c.co, 3, 3, device='cuda', generator=g) / (3 * c.ci ** 0.5)
-        wp = prims.pack_weights(W, prims.PACK_CONV_DGRAD)
-        call = lambda: prims.conv3x3(x, c.x_c0, c.ci, wp, None, y, c.y_c0, c.co, act=c.act, aux=aux,  # noqa: E731
-                                     aux_c0=c.aux_c0)
-        r, S = R.conv_dgrad(xs, W, auxs)
-    elif c.op == 'deconv':
-        Wt = torch.randn(c.ci, c.co, 2, 2, device='cuda', generator=g) / c.ci ** 0.5
-        b = torch.randn(c.co, device='cuda', generator=g) if c.bias else None
-        wp = prims.pack_weights(Wt, prims.PACK_DECONV_FPROP)
-        call = lambda: prims.deconv2x2(x, c.x_c0, c.ci, wp, b, y, c.y_c0, c.co)  # noqa: E731
-        r, S = R.deconv_fprop(xs, Wt, b)
-    else:
-        Wt = torch.randn(c.co, c.ci, 2, 2, device='cuda', generator=g) / c.ci ** 0.5
-        wp = prims.pack_weights(Wt, prims.PACK_DECONV_DGRAD)
-        call = lambda: prims.deconv2x2_dgrad(x, c.x_c0, c.ci, wp, y, c.y_c0, c.co, act=c.act, aux=aux,  # noqa: E731
-                                             aux_c0=c.aux_c0)
-        r, S = R.deconv_dgrad(xs, Wt, auxs)
-    _prims_traced(torch, call, {kern: 1}, where)
-    bad = _written(torch, out, y, c.y_c0, c.co)
-    assert bad == 0, '%s: %d guard elements written' % (where, bad)
-    _bf16_check(kern, where, y[..., c.y_c0:c.y_c0 + c.co], r, S)
-
-
 @pytest.mark.parametrize('c', T.CASES, ids=T.case_id)
 def test_primitive(torch, c):
-    run_case(torch, c, T.CASES.index(c) + 1)
+    C.run_case(torch, c, T.CASES.index(c) + 1)
 
 
 def test_large_cases_outnumber_the_sms(torch):
@@ -191,7 +63,7 @@ def test_thin_tile_equals_generic_tile_bitwise(torch, case):
     op, n, h, w, ci, co = case
     wide = 96 if co == 32 else 192
     g = torch.Generator(device='cuda').manual_seed(7)
-    x = _operand(torch, g, n, h, w, ci)
+    x = C.operand(torch, g, n, h, w, ci)
     y_thin = torch.empty(n, h, w, co, device='cuda', dtype=torch.bfloat16)
     y_wide = torch.empty(n, h, w, wide, device='cuda', dtype=torch.bfloat16)
     if op == 'conv':
@@ -202,16 +74,16 @@ def test_thin_tile_equals_generic_tile_bitwise(torch, case):
         kw = dict(act=prims.ACT_LRELU)
     else:
         W = torch.randn(ci, wide, 3, 3, device='cuda', generator=g) / (3 * ci ** 0.5)
-        aux = _operand(torch, g, n, h, w, wide)
+        aux = C.operand(torch, g, n, h, w, wide)
         packs = [prims.pack_weights(W[:, :co], prims.PACK_CONV_DGRAD), prims.pack_weights(W, prims.PACK_CONV_DGRAD)]
         biases = [None, None]
         kw = dict(act=prims.ACT_MASK, aux=aux, aux_c0=0)
     for tile, wp, bias, y, cout in zip(('thin', 'wide'), packs, biases, (y_thin, y_wide), (co, wide)):
-        _prims_traced(torch, lambda: prims.conv3x3(x, 0, ci, wp, bias, y, 0, cout, **kw),
+        C.prims_traced(torch, lambda: prims.conv3x3(x, 0, ci, wp, bias, y, 0, cout, **kw),
                 {'conv3x3_%s<%d,%d>' % (tile, co, ci): 1}, '%s %s tile' % (case, tile))
     a, b_ = y_thin.view(torch.int16), y_wide[..., :co].contiguous().view(torch.int16)
     diff = int((a != b_).sum().item())
-    STATS['exact thin vs generic']['elements'] += a.numel()
+    C.STATS['exact thin vs generic']['elements'] += a.numel()
     assert diff == 0, '%s: %d of %d elements differ' % (case, diff, a.numel())
 
 
@@ -227,7 +99,7 @@ def test_pack_weights_matches_packed_index(torch, shape):
     kind, cout, cin = shape
     g = torch.Generator(device='cuda').manual_seed(3)
     W = torch.randn(*((cout, cin, 3, 3) if kind < 2 else (cin, cout, 2, 2)), device='cuda', generator=g)
-    got = _prims_traced(torch, lambda: prims.pack_weights(W, kind), {'pack_weights_kernel': 1}, 'kind%d-%dx%d' % shape)
+    got = C.prims_traced(torch, lambda: prims.pack_weights(W, kind), {'pack_weights_kernel': 1}, 'kind%d-%dx%d' % shape)
     got = got.reshape(-1)
     src, dst = T.pack_order(kind, cout, cin)
     want = torch.empty_like(got)
@@ -241,7 +113,7 @@ def test_wide_tile_repeats_bitwise(torch, op):
     from eld_b200 import prims
     n, h, w, ci, co = 2, 19, 45, 256, 256
     g = torch.Generator(device='cuda').manual_seed(11)
-    x = _operand(torch, g, n, h, w, ci)
+    x = C.operand(torch, g, n, h, w, ci)
     ys = []
     if op == 'conv':
         W = torch.randn(co, ci, 3, 3, device='cuda', generator=g) / (3 * ci ** 0.5)
@@ -249,15 +121,15 @@ def test_wide_tile_repeats_bitwise(torch, op):
         wp = prims.pack_weights(W, prims.PACK_CONV_FPROP)
     else:
         W = torch.randn(ci, co, 3, 3, device='cuda', generator=g) / (3 * ci ** 0.5)
-        aux = _operand(torch, g, n, h, w, co)
+        aux = C.operand(torch, g, n, h, w, co)
         wp = prims.pack_weights(W, prims.PACK_CONV_DGRAD)
     for _ in range(2):
-        out, y = _output(torch, n, h, w, co)
+        out, y = C.output(torch, n, h, w, co)
         if op == 'conv':
             prims.conv3x3(x, 0, ci, wp, b, y, 0, co, act=prims.ACT_LRELU)
         else:
             prims.conv3x3(x, 0, ci, wp, None, y, 0, co, act=prims.ACT_MASK, aux=aux, aux_c0=0)
-        assert _written(torch, out, y, 0, co) == 0
+        assert C.written(torch, out, y, 0, co) == 0
         assert not (y.view(torch.int16) == NAN16).any()
         ys.append(y.clone())
     assert torch.equal(ys[0].view(torch.int16), ys[1].view(torch.int16))
@@ -297,7 +169,7 @@ def test_deconv_refuses_cout_the_shuffle_cannot_store(torch, cout):
     Wt = torch.randn(cin, cout, 2, 2, device='cuda')
     wp = prims.pack_weights(Wt, prims.PACK_DECONV_FPROP) if cout != 96 else torch.zeros(4 * 256 * cin, device='cuda').bfloat16()
     b = torch.randn(cout, device='cuda')
-    out, y = _output(torch, n, 2 * h, 2 * w, 64)
+    out, y = C.output(torch, n, 2 * h, 2 * w, 64)
     _refused(torch, 'eld_deconv2x2_bf16(cin %d, cout %d, y pitch 64)' % (cin, cout),
              lambda: prims.deconv2x2(x, 0, cin, wp, b, y, 0, cout), out.full)
 
@@ -349,7 +221,7 @@ def test_deconv_dgrad_refuses_partial_tiles(torch, hw):
     dy = torch.randn(1, 2 * h, 2 * w, cout, device='cuda').bfloat16()
     aux = torch.randn(1, h, w, cin, device='cuda').bfloat16()
     wp = prims.pack_weights(Wt, prims.PACK_DECONV_DGRAD)
-    out, dx = _output(torch, 1, h, w, cin)
+    out, dx = C.output(torch, 1, h, w, cin)
     _refused(torch, 'eld_deconv2x2_dgrad_bf16 at %d x %d' % (h, w),
              lambda: prims.deconv2x2_dgrad(dy, 0, cout, wp, dx, 0, cin, act=prims.ACT_MASK, aux=aux), out.full)
 

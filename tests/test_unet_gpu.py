@@ -7,82 +7,36 @@ Stated tolerances (bf16 activations / bf16 GEMM operands, fp32 accumulation, fp3
   gradients : per tensor cosine >= 0.99 and norm ratio in [0.95, 1.05] vs the fp32 oracle autograd
   vs a bf16-EMULATED torch reference (same rounding points): rel-L2 <= 3e-3 - this is the bug detector.
 """
-import numpy as np
 import pytest
+
+from tests import engine_harness as E
+from tests.engine_harness import torch  # noqa: F401 (the fixture)
 
 pytestmark = pytest.mark.gpu
 H, W = 128, 256          # smallest shape the tiles accept (8x16 patches at 1/16 scale)
 
 
 @pytest.fixture(scope='module')
-def torch():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip('no GPU')
-    return torch
-
-
-@pytest.fixture(scope='module')
 def nets(torch):
-    from eld_b200 import arch
-    from oracle.unet_ref import UNetSeeInDarkRef
-    torch.manual_seed(2018)
-    ours = arch.unet(4, 4).cuda()
-    torch.manual_seed(2018)
-    ref = UNetSeeInDarkRef(4, 4)
-    # the default init leaves most pre-activations on one side of LeakyReLU's kink: spread the biases (both nets,
-    # identically) so that both branches - and both values of the backward mask - carry real weight
-    g = torch.Generator().manual_seed(5)
-    with torch.no_grad():
-        for (k, p), (_, q) in zip(ref.named_parameters(), ours.named_parameters()):
-            if k.endswith('.bias'):
-                d = (torch.rand(p.shape, generator=g) - 0.5) * 0.2
-                p.add_(d)
-                q.add_(d.to(q.device))
-    return ours, ref
-
-
-def _rel(a, b):
-    return ((a.double() - b.double()).norm() / (b.double().norm() + 1e-30)).item()
-
-
-def _q(t):
-    return t.bfloat16().float()
-
-
-def _emulated_forward(torch, net, x):
-    """fp32 torch math with the engine's rounding points: bf16 GEMM operands and bf16 activations."""
-    F = torch.nn.functional
-    lre = lambda v: torch.max(0.2 * v, v)
-    c = lambda name, v: _q(lre(F.conv2d(v, _q(getattr(net, name).weight), getattr(net, name).bias, padding=1)))
-    up = lambda name, v: _q(F.conv_transpose2d(v, _q(getattr(net, name).weight), getattr(net, name).bias, stride=2))
-    a = _q(lre(F.conv2d(_q(x), _q(net.conv1_1.weight), net.conv1_1.bias, padding=1)))   # first layer: bf16 operands too
-    c1 = c('conv1_2', a)
-    c2 = c('conv2_2', c('conv2_1', F.max_pool2d(c1, 2)))
-    c3 = c('conv3_2', c('conv3_1', F.max_pool2d(c2, 2)))
-    c4 = c('conv4_2', c('conv4_1', F.max_pool2d(c3, 2)))
-    c5 = c('conv5_2', c('conv5_1', F.max_pool2d(c4, 2)))
-    c6 = c('conv6_2', c('conv6_1', torch.cat([up('upv6', c5), c4], 1)))
-    c7 = c('conv7_2', c('conv7_1', torch.cat([up('upv7', c6), c3], 1)))
-    c8 = c('conv8_2', c('conv8_1', torch.cat([up('upv8', c7), c2], 1)))
-    c9 = c('conv9_2', c('conv9_1', torch.cat([up('upv9', c8), c1], 1)))
-    return F.conv2d(c9, net.conv10_1.weight, net.conv10_1.bias)
+    """the engine module and the CPU oracle, biases spread (tests/engine_harness.py)"""
+    return E.pair(device='cpu')
 
 
 def test_forward_parity(torch, nets):
     from oracle import ref_numpy
+    from tests.unet_emul import emulated_forward
     ours, ref = nets
     torch.manual_seed(7)
     x = torch.rand(2, 4, H, W)
     t = torch.rand(2, 4, H, W)
     with torch.no_grad():
         want = ref(x)
-        emu = _emulated_forward(torch, ref.cuda(), x.cuda()).cpu()
+        emu = emulated_forward(ref.cuda(), x.cuda()).cpu()
         ref.cpu()
     got = ours(x.cuda()).detach().cpu()          # (training mode: the output is an autograd node)
     assert torch.isfinite(got).all()
-    assert _rel(got, emu) <= 3e-3, _rel(got, emu)
-    assert _rel(got, want) <= 2e-2, _rel(got, want)
+    assert E.rel(got, emu) <= 3e-3, E.rel(got, emu)
+    assert E.rel(got, want) <= 2e-2, E.rel(got, want)
     d = abs(ref_numpy.psnr255(got.numpy(), t.numpy()) - ref_numpy.psnr255(want.numpy(), t.numpy()))
     assert d <= 0.05, d
 
@@ -98,7 +52,7 @@ def test_train_step_parity(torch, nets):
     loss_ref.backward()
     out, loss = ours.train_step(x.cuda(), t.cuda())
     assert abs(loss.item() - loss_ref.item()) <= 1e-2 * loss_ref.item()
-    assert _rel(out.cpu(), out_ref.detach()) <= 2e-2
+    assert E.rel(out.cpu(), out_ref.detach()) <= 2e-2
     bad = []
     for (k, p), (k2, q) in zip(ref.named_parameters(), ours.named_parameters()):
         assert k == k2
@@ -122,7 +76,7 @@ def test_train_step_deterministic_forward_and_grad_reset(torch, nets):
     o2, l2 = ours.train_step(x, t)
     assert torch.equal(o1, o2)
     # gradients are re-zeroed every step; fp32 atomics make the sum order vary -> tiny tolerance
-    assert _rel(ours.flat_grads, g1) <= 1e-4
+    assert E.rel(ours.flat_grads, g1) <= 1e-4
 
 
 def test_adam_matches_torch(torch, nets):
@@ -164,8 +118,8 @@ def test_inference_any_multiple_of_16(torch, nets, hw):
     with torch.no_grad():
         want = ref(x)
     got = ours(x.cuda()).cpu()
-    assert _rel(got, want) <= 2e-2, _rel(got, want)
-    assert _rel(got[:, :, -4:, -4:], want[:, :, -4:, -4:]) <= 5e-2          # bottom-right corner pixels
+    assert E.rel(got, want) <= 2e-2, E.rel(got, want)
+    assert E.rel(got[:, :, -4:, -4:], want[:, :, -4:, -4:]) <= 5e-2          # bottom-right corner pixels
 
 
 def test_shape_contract(torch, nets):
@@ -196,7 +150,7 @@ def test_autograd_seam_matches_the_fused_step(torch, nets):
     loss.backward()
     got = torch.cat([p.grad.reshape(-1) for p in ours.parameters()])
     assert abs(loss.item() - loss_f.item()) <= 1e-5 * loss_f.item()
-    assert _rel(got, fused) <= 1e-4, _rel(got, fused)
+    assert E.rel(got, fused) <= 1e-4, E.rel(got, fused)
     # a different loss through the same seam (the reference's --loss l2) and a stock torch optimizer on the parameters
     p0 = ours.flat_params.clone()
     opt = torch.optim.Adam(ours.parameters(), lr=1e-4)
@@ -212,16 +166,9 @@ def test_autograd_seam_matches_the_fused_step(torch, nets):
 def test_srgb_channel_variants(torch, io):
     """ELD_model.py:377-389: --stage_in / --stage_out srgb give a 3-channel first / last layer.  Forward, loss and every
     gradient tensor of the (cin, cout) network against the oracle module built with the same channels."""
-    from eld_b200 import arch
-    from oracle.unet_ref import UNetSeeInDarkRef
     from tests.unet_emul import emulated_train_step, fp32_cuda
     cin, cout = io
-    torch.manual_seed(2018)
-    ours = arch.unet(cin, cout).cuda()
-    torch.manual_seed(2018)
-    ref = UNetSeeInDarkRef(cin, cout).cuda()
-    for (k, p), (k2, q) in zip(ref.named_parameters(), ours.named_parameters()):
-        assert k == k2 and p.shape == q.shape and torch.equal(p.detach(), q.detach())
+    ours, ref = E.pair(cin, cout, spread=False)
     torch.manual_seed(9)
     x = torch.rand(2, cin, H, W, device='cuda')
     t = torch.rand(2, cout, H, W, device='cuda')
@@ -229,14 +176,14 @@ def test_srgb_channel_variants(torch, io):
     with torch.no_grad():
         want = fp32_cuda(lambda: ref(x))
         got = ours(x)
-    assert got.shape == (2, cout, H, W) and _rel(got, want) <= 2e-2, _rel(got, want)
+    assert got.shape == (2, cout, H, W) and E.rel(got, want) <= 2e-2, E.rel(got, want)
     out, loss = ours.train_step(x, t)
     mine = {k: p.grad.detach().clone() for k, p in ours.named_parameters()}
     oem, lem, gem = fp32_cuda(lambda: emulated_train_step(ref, x, t))
-    assert _rel(out, oem) <= 3e-3 and abs(loss.item() - lem.item()) <= 2e-3 * lem.item()
+    assert E.rel(out, oem) <= 3e-3 and abs(loss.item() - lem.item()) <= 2e-3 * lem.item()
     # 2 x 128 x 256 is a 2 x 8 x 16 pixel bottleneck: few terms per sum, so single bf16 rounding flips weigh more than at
     # BASELINE's shape (6.5e-4 there, up to 6.5e-3 here); an indexing / channel-count bug moves a tensor by >= 1e-1
-    bad = [(k, _rel(mine[k], gem[k])) for k in mine if _rel(mine[k], gem[k]) > 1.5e-2]
+    bad = [(k, E.rel(mine[k], gem[k])) for k in mine if E.rel(mine[k], gem[k]) > 1.5e-2]
     assert not bad, bad
 
 
@@ -245,19 +192,14 @@ def test_pool_ties_route_like_max_pool2d(torch):
     pool backward works from the 1-byte code the forward tile leaves (argmax + signs, conv_umma.cuh / unet_ew.cu) and
     must route the gradient of a tie to the first element in window order, as nn.MaxPool2d does (Unet.py:13); the
     LeakyReLU' masks come from the sign words.  Every gradient tensor against the bf16-emulated backward."""
-    from eld_b200 import arch
-    from oracle.unet_ref import UNetSeeInDarkRef
     from tests.unet_emul import emulated_train_step, fp32_cuda
-    torch.manual_seed(2018)
-    ours = arch.unet(4, 4).cuda()
-    torch.manual_seed(2018)
-    ref = UNetSeeInDarkRef(4, 4).cuda()
+    ours, ref = E.pair(spread=False)
     g = torch.Generator().manual_seed(3)
     x = torch.rand(2, 4, H // 8, W // 8, generator=g).repeat_interleave(8, 2).repeat_interleave(8, 3).cuda()
     t = torch.rand(2, 4, H, W, generator=g).cuda()
     out, loss = ours.train_step(x, t)
     mine = {k: p.grad.detach().clone() for k, p in ours.named_parameters()}
     oem, lem, gem = fp32_cuda(lambda: emulated_train_step(ref, x, t))
-    assert _rel(out, oem) <= 3e-3 and abs(loss.item() - lem.item()) <= 2e-3 * lem.item()
-    bad = [(k, _rel(mine[k], gem[k])) for k in mine if _rel(mine[k], gem[k]) > 1.5e-2]
+    assert E.rel(out, oem) <= 3e-3 and abs(loss.item() - lem.item()) <= 2e-3 * lem.item()
+    bad = [(k, E.rel(mine[k], gem[k])) for k in mine if E.rel(mine[k], gem[k]) > 1.5e-2]
     assert not bad, bad
