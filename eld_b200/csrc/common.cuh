@@ -76,7 +76,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), int grid, int block, siz
 }
 
 
-// device side of PDL (see umma.cuh for the wgmma tiles): wait for the predecessor, then release the successor
+// device side of PDL (see wgmma.cuh for the wgmma tiles): wait for the predecessor, then release the successor
 __device__ __forceinline__ void pdl_wait_and_release()
 {
     asm volatile("griddepcontrol.wait;" ::: "memory");

@@ -1,13 +1,11 @@
 // conv3x3_thin.cuh - wgmma tile for the thin 3x3 convolutions (fprop and dgrad with GEMM K = cin and N in {32, 64}):
-// the full- and half-resolution layers, which are bound by HBM and which the generic tile (conv_umma.cuh) feeds with
-// 9x the A bytes and a reload of the weights per tile.
+// the full- and half-resolution layers, which are bound by HBM.  Their weights fit in shared memory and stay there for
+// every tile; the other 3x3 convolutions stream theirs through a ring (conv3x3_wide.cuh).
 //
 //   D[128 pixels x NT] (f32, registers)  +=  A[128 pixels x 9 cin] (bf16, smem via TMA)  *  B[NT x 9 cin]^T
 //
-// A       = per 8 x 16 pixel tile three TMA boxes {kc, 16, 10} at columns x0 - 1, x0, x0 + 1 and rows y0 - 1 .. y0 + 8
-//           (zero-filled outside the image = the padding).  Tap (dy, dx) is box dx + 1 from pixel row 16 (dy + 1) on: a
-//           descriptor offset of 1 KB (kc = 32, SW64) or 2 KB (kc = 64, SW128) per row shift, whole swizzle atoms.  A tile
-//           moves 30 rows of 16 pixels instead of 9 x 8.
+// A       = the halo of each 8 x 16 pixel tile (tile.cuh): three TMA boxes {kc, 16, 10}, one load per tile for all nine
+//           taps, each tap a descriptor offset into them.
 // B       = the layer's whole packed operand for its one N block (9 tap blocks of NT x kc, unet_prims.h packed_index),
 //           bulk-copied once per CTA and resident for every tile (at most 72 KB).
 // K order = the wide tile's with one channel chunk (cin = kc): taps 0..8, k16 steps inside a tap, so every output row
@@ -18,11 +16,10 @@
 //           by r & 7 (conflict-free fragment writes and row reads without padding; 16 KB, so two 60 KB halo slots and
 //           72 KB of weights fit at K = N = 64).
 #pragma once
-#include "conv_umma.cuh"
+#include "conv_gemm.cuh"
 
 namespace eld {
 
-constexpr int kThinBoxRows = 10;                       // 8 tile rows + the halo row above and below
 constexpr int kThinStgBytes = 128 * 32 * 4;            // staging of one consumer warpgroup: 128 pixels x 32 f32 columns
 constexpr int kThinMaxSlots = 4;
 constexpr int kThinSmemBytes = 227 * 1024;             // the sm_90 per-block opt-in maximum
@@ -38,8 +35,7 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParam
 
     constexpr int row_bytes = KC * 2;
     constexpr int tap_bytes = NT * row_bytes;                       // one resident tap block of B
-    constexpr int box_bytes = kThinBoxRows * kConvTileW * row_bytes;
-    constexpr int slot_bytes = 3 * box_bytes;
+    constexpr int slot_bytes = halo_slot_bytes(KC);
     uint8_t* b_s = smem;
     uint8_t* slots = smem + 9 * tap_bytes;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.bar_smem_off);
@@ -81,7 +77,7 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParam
                 ptx::mbar_wait(&empty[s], ph ^ 1u);
                 uint8_t* sa = slots + (size_t)s * slot_bytes;
                 ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)slot_bytes);
-                for (int b = 0; b < 3; ++b) ptx::tma_load_5d(sa + b * box_bytes, &tmA, &full[s], p.a_c0, x0 + b - 1, y0 - 1, img, 0);
+                halo_load<KC>(sa, &tmA, &full[s], p.a_c0, x0, y0, img);
                 if (++s == p.stages) { s = 0; ph ^= 1u; }
             }
         }
@@ -110,14 +106,13 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParam
         ptx::wgmma_fence();
 #pragma unroll
         for (int tap = 0; tap < 9; ++tap) {
-            const int ty = tap / 3, tx = tap - 3 * ty;         // box tx, 16 ty pixel rows down
-            const uint32_t a_addr = sa + (uint32_t)(tx * box_bytes + ty * kConvTileW * row_bytes);
-            const uint64_t bd = desc0 | (uint64_t)(((b_base + (uint32_t)(tap * tap_bytes)) & 0x3FFFFu) >> 4);
+            const uint32_t a_addr = sa + halo_tap_off(KC, tap);
+            const uint64_t bd = ptx::desc_at(desc0, b_base + (uint32_t)(tap * tap_bytes));
 #pragma unroll
             for (int k = 0; k < KC / 16; ++k) {                   // +32 bytes along K inside the swizzle atom
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
-                    const uint64_t ad = desc0 | (uint64_t)(((a_addr + (uint32_t)(h * 64 * row_bytes)) & 0x3FFFFu) >> 4);
+                    const uint64_t ad = ptx::desc_at(desc0, a_addr + (uint32_t)(h * 64 * row_bytes));
                     ptx::wgmma_bf16<NT, 0, 0>(acc[h], ad + 2u * k, bd + 2u * k, (tap | k) != 0 ? 1u : 0u);
                 }
             }

@@ -4,17 +4,15 @@
 //
 //   D[128 pixels x NT] (f32, registers)  +=  A[128 pixels x 9 cin] (bf16, smem via TMA)  *  B[NT x 9 cin]^T
 //
-// A       = per 8 x 16 pixel tile and channel chunk of KC, three TMA boxes {KC, 16, 10} at columns x0 - 1, x0, x0 + 1 and
-//           rows y0 - 1 .. y0 + 8 (zero-filled outside the image = the padding); tap (dy, dx) is box dx + 1 from pixel
-//           row 16 (dy + 1) on, a descriptor offset of whole swizzle atoms.  30 rows of 16 pixels per chunk instead of the
-//           9 x 8 that one box per tap moves.
+// A       = per 8 x 16 pixel tile and channel chunk of KC, the halo of the tile (tile.cuh): three TMA boxes {KC, 16, 10},
+//           one load per chunk for all nine taps, each tap a descriptor offset into them.
 // B       = one [NT x KC] packed weight block per (tap, chunk) (unet_prims.h packed_index), one linear bulk copy each,
 //           through a ring of its own.
 // K order = chunk outer, taps 0..8 inside, k16 steps inside a tap.  With one chunk this is the thin tile's order (the
 //           thin tile equals the first N block of this one bit for bit); with more, the fp32 sums are reordered against
 //           a tap-outer walk, which moves bf16 outputs by at most the last-ulp rounding.
 // roles   = warpgroup 0: thread 0 loads the halo slots, thread 32 the weight blocks | warpgroups 1, 2: wgmma on pixel rows
-//           0-63 / 64-127 of the tile, then the shared epilogue of those rows (conv_umma.cuh conv_tile_epilogue).  The
+//           0-63 / 64-127 of the tile, then the shared epilogue of those rows (conv_gemm.cuh conv_tile_epilogue).  The
 //           producers run ahead across tiles, so the next tile's operands load while the consumers run the epilogue.
 #pragma once
 #include "conv3x3_thin.cuh"
@@ -34,8 +32,7 @@ conv3x3_wide_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParam
 
     constexpr int row_bytes = KC * 2;
     constexpr int b_bytes = NT * row_bytes;                         // one (tap, chunk) weight block of this N tile
-    constexpr int box_bytes = kThinBoxRows * kConvTileW * row_bytes;
-    constexpr int slot_bytes = 3 * box_bytes;
+    constexpr int slot_bytes = halo_slot_bytes(KC);
     uint8_t* slots = smem;
     uint8_t* b_s = smem + kWideHaloSlots * slot_bytes;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.bar_smem_off);   // weight ring
@@ -78,8 +75,7 @@ conv3x3_wide_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParam
                     ptx::mbar_wait(&h_empty[s], ph ^ 1u);
                     uint8_t* sa = slots + (size_t)s * slot_bytes;
                     ptx::mbar_arrive_expect_tx(&h_full[s], (uint32_t)slot_bytes);
-                    for (int b = 0; b < 3; ++b)
-                        ptx::tma_load_5d(sa + b * box_bytes, &tmA, &h_full[s], p.a_c0 + ch * KC, x0 + b - 1, y0 - 1, img, 0);
+                    halo_load<KC>(sa, &tmA, &h_full[s], p.a_c0 + ch * KC, x0, y0, img);
                     if (++s == kWideHaloSlots) { s = 0; ph ^= 1u; }
                 }
             }
@@ -124,10 +120,11 @@ conv3x3_wide_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParam
             const uint32_t sa = slot_base + (uint32_t)(hs * slot_bytes);
 #pragma unroll
             for (int tap = 0; tap < 9; ++tap) {
+                // halo_tap_off(KC, tap) written out: through the helper this loop compiles to a different schedule
                 const int ty = tap / 3, tx = tap - 3 * ty;     // box tx, 16 ty pixel rows down
                 ptx::mbar_wait(&full[s], ph);
-                const uint64_t ad = desc0 | (uint64_t)(((sa + (uint32_t)(tx * box_bytes + ty * kConvTileW * row_bytes)) & 0x3FFFFu) >> 4);
-                const uint64_t bd = desc0 | (uint64_t)(((b_base + (uint32_t)(s * b_bytes)) & 0x3FFFFu) >> 4);
+                const uint64_t ad = ptx::desc_at(desc0, sa + (uint32_t)(tx * halo_box_bytes(KC) + ty * kConvTileW * row_bytes));
+                const uint64_t bd = ptx::desc_at(desc0, b_base + (uint32_t)(s * b_bytes));
                 ptx::wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < KC / 16; ++k)              // +32 bytes along K inside the swizzle atom
@@ -142,7 +139,7 @@ conv3x3_wide_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParam
                 prev = s;
                 if (++s == p.stages) { s = 0; ph ^= 1u; }
             }
-            prev_h = hs;                                       // released after the next step's wait (or the tile's)
+            prev_h = hs;                                      // released after the next step's wait (or the tile's)
             if (++hs == kWideHaloSlots) { hs = 0; hph ^= 1u; }
         }
         ptx::wgmma_wait<0>();

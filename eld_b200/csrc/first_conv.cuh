@@ -1,7 +1,7 @@
 // first_conv.cuh - conv1_1 (4 -> 32 channels, 3x3, Unet.py:11) fprop and wgrad as wgmma tiles fed by a SOFTWARE im2col,
 // and its data gradient (the gradient of the input frame; see first_conv_dgrad_kernel at the end).
 //
-// The generic conv tile needs >= 32 input channels (one 64-byte TMA row per pixel); conv1_1 has 4.  Instead of a
+// The other conv tiles need >= 32 input channels (one 64-byte TMA row per pixel); conv1_1 has 4.  Instead of a
 // zero-padded 32-channel copy of the input (a pack pass, and 7/8 of the MMAs multiplying zeros), one thread per pixel
 // reads the fp32 NCHW frame (from a TMA-loaded halo patch in shared memory) and writes the im2col tile
 //     A[128 pixels][k = tap*4 + c  (36 real, k = 36 is a column of ones, the rest zero)]       bf16, 128-byte rows, SW128
@@ -14,7 +14,7 @@
 // builders undo that.  The box starts at column x0 - 4, not x0 - 1: the innermost start of a TMA box must be 16-byte
 // aligned in global memory.
 #pragma once
-#include "umma.cuh"
+#include "tile.cuh"
 #include <cuda_bf16.h>
 
 namespace eld {
@@ -29,7 +29,7 @@ struct FirstConvParams {
     __nv_bfloat16* out;         // fprop: NHWC bf16, 32 channels at out_pitch
     int out_pitch;
     uint32_t* sign_out;         // fprop, optional (training): one sign word per pixel (channel 2j -> bit j, 2j+1 -> bit 16+j), the
-                                // LeakyReLU' mask conv1_2's data gradient needs (conv_umma.cuh aux_sign)
+                                // LeakyReLU' mask conv1_2's data gradient needs (conv_gemm.cuh aux_sign)
     float* dw;                  // wgrad: f32 OIHW [32][4][3][3], accumulated into
     float* db;                  // wgrad: f32 [32]
     const float* w;             // dgrad: the f32 master weights, OIHW [32][cin][3][3]
@@ -78,15 +78,6 @@ __device__ __forceinline__ void fc_build_row(const float* raw, uint8_t* tile, in
     *reinterpret_cast<uint4*>(row + ((5 ^ sw) << 4)) = make_uint4(0u, 0u, 0u, 0u);
 }
 
-__device__ __forceinline__ void fc_tile_coords(const FirstConvParams& p, int tile, int& img, int& y0, int& x0)
-{
-    const int txy = p.tiles_x * p.tiles_y;
-    img = tile / txy;
-    const int rem = tile - img * txy;
-    const int ty = rem / p.tiles_x;
-    y0 = ty * 8; x0 = (rem - ty * p.tiles_x) * 16;
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
 // WGRAD = false: a1_1 = lrelu(conv1_1(x) + b)
 // WGRAD = true : dW[co][c][tap] += sum_px dZ[px][co] * x[px + tap][c] ; db[co] += sum_px dZ[px][co]
@@ -128,13 +119,12 @@ first_conv_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
     ptx::grid_dep_launch();
 
     auto issue = [&](int i) {      // TMA loads of this warpgroup's i-th tile into ring slot i % kFcRing
-        int img, y0, x0;
-        fc_tile_coords(p, (int)blockIdx.x + (wg + 2 * i) * (int)gridDim.x, img, y0, x0);
+        const TileCoord tc = tile_coord((int)blockIdx.x + (wg + 2 * i) * (int)gridDim.x, p.tiles_x, p.tiles_y);
         uint8_t* slot = ring + (size_t)(i % kFcRing) * slot_bytes;
         uint64_t* bar = &slot_full[i % kFcRing];
         ptx::mbar_arrive_expect_tx(bar, (uint32_t)slot_bytes);
-        ptx::tma_load_5d(slot, &tmX, bar, 2 * (x0 - 4), y0 - 1, 0, img, 0);
-        if (WGRAD) ptx::tma_load_5d(slot + kFcRaw, &tmQ, bar, 0, x0, y0, img, 0);
+        ptx::tma_load_5d(slot, &tmX, bar, 2 * (tc.x0 - 4), tc.y0 - 1, 0, tc.img, 0);
+        if (WGRAD) ptx::tma_load_5d(slot + kFcRaw, &tmQ, bar, 0, tc.x0, tc.y0, tc.img, 0);
     };
     if (m == 0) {
         if (!WGRAD && wg == 0) {
@@ -163,11 +153,11 @@ first_conv_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
             // D[px][co] for pixel rows 0-63 and 64-127: K-major A and W, SBO = 8 rows of 128 B
             if (m == 0 && i + kFcRing < n_mine) issue(i + kFcRing);     // the patch is consumed (it is in the A tile)
             const uint64_t dsc = ptx::make_gmma_desc(0, 16, 1024, ptx::GMMA_SW128);
-            const uint64_t bd = dsc | (uint64_t)((ptx::smem_u32(w_s) & 0x3FFFFu) >> 4);
+            const uint64_t bd = ptx::desc_at(dsc, ptx::smem_u32(w_s));
             ptx::wgmma_fence();
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const uint64_t ad = dsc | (uint64_t)(((a_addr + 8192u * h) & 0x3FFFFu) >> 4);
+                const uint64_t ad = ptx::desc_at(dsc, a_addr + 8192u * h);
 #pragma unroll
                 for (int k = 0; k < 3; ++k) ptx::wgmma_bf16<32, 0, 0>(acc[h], ad + 2u * k, bd + 2u * k, k != 0 ? 1u : 0u);
             }
@@ -186,8 +176,7 @@ first_conv_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
                         *reinterpret_cast<float2*>(stg + (64 * h + 16 * wq + (lane >> 2) + 8 * r) * kFcStg + 8 * j + 2 * (lane & 3)) =
                             make_float2(acc[h][4 * j + 2 * r], acc[h][4 * j + 2 * r + 1]);
             ptx::bar_sync(1 + wg, 128);
-            int img, y0, x0;
-            fc_tile_coords(p, (int)blockIdx.x + (wg + 2 * i) * (int)gridDim.x, img, y0, x0);
+            const TileCoord tc = tile_coord((int)blockIdx.x + (wg + 2 * i) * (int)gridDim.x, p.tiles_x, p.tiles_y);
             const float4* row = reinterpret_cast<const float4*>(stg + m * kFcStg);
             const float4* sb4 = reinterpret_cast<const float4*>(s_bias);
             uint32_t wv[16];
@@ -200,7 +189,7 @@ first_conv_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
                 wv[4 * g] = fc_pack(v[0], v[1]); wv[4 * g + 1] = fc_pack(v[2], v[3]);
                 wv[4 * g + 2] = fc_pack(v[4], v[5]); wv[4 * g + 3] = fc_pack(v[6], v[7]);
             }
-            const size_t pix = (size_t)(img * p.H + y0 + py) * p.W + (x0 + px);
+            const size_t pix = (size_t)(tc.img * p.H + tc.y0 + py) * p.W + (tc.x0 + px);
             __nv_bfloat16* dst = p.out + pix * p.out_pitch;
             ptx::st_global_32B(dst, wv);                   // 64 bytes = two full sectors
             ptx::st_global_32B(dst + 16, wv + 8);
@@ -247,21 +236,18 @@ first_conv_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
 // DGRAD: dx[c][y][x] = sum_{co, kh, kw} dZ[y + 1 - kh][x + 1 - kw][co] * W[co][c][kh][kw]   (d loss / d frame)
 //
 // Here the A operand needs no im2col: dZ (conv1_1's pre-activation gradient, bf16 NHWC, 32 channels) is one 64-byte SW64
-// row per pixel, and K = 9 taps x 32 channels.  Per 8 x 16 pixel tile the producer loads three TMA boxes
-// {32 ch, 16 px, 10 rows}, one per column shift -1 / 0 / +1, each with a one-row halo above and below; out-of-image
-// elements are zero-filled, which is the transposed padding.  A row shift is then 16 pixel rows = 1 KB inside a box,
-// whole 8-row swizzle atoms, so each of the nine taps is a descriptor offset, and a tile moves 30 KB instead of nine
-// 8 KB boxes.  B = the weights in the dgrad arrangement [tap][8 rows = c, zero for c >= cin][32 co] (taps flipped), bf16
-// SW64, built once per CTA from the fp32 master weights.  wgmma m64n8k16: N = cin padded to 8.
-// The wgmma tile of conv_umma.cuh is not reused: it bulk-loads B per stage and ends in a 32-column bf16 epilogue
-// (bias, masks, pool, sign words); an N = 8 fp32 NCHW store would make both halves branch on this one caller.
+// row per pixel, and K = 9 taps x 32 channels.  Per 8 x 16 pixel tile the producer loads the tile's halo of dZ (tile.cuh,
+// three boxes {32 ch, 16 px, 10 rows}; the zero fill outside the image is the transposed padding), and each of the nine
+// taps is a descriptor offset into it: a tile moves 30 KB instead of nine 8 KB boxes.  B = the weights in the dgrad
+// arrangement [tap][8 rows = c, zero for c >= cin][32 co] (taps flipped), bf16 SW64, built once per CTA from the fp32
+// master weights.  wgmma m64n8k16: N = cin padded to 8.
+// The thin 3x3 tile (conv3x3_thin.cuh) loads A the same way but is not reused: its N is 32 or 64, its B a packed bf16
+// operand, and it ends in the 32-column bf16 epilogue (bias, masks, pool, sign words), not an N = 8 fp32 NCHW store.
 // Warpgroup 0 is the TMA producer (one thread); warpgroups 1 and 2 take pixel rows 0-63 / 64-127 of every tile and store
 // their fragments straight to the fp32 planes: per store instruction a warp writes 8 consecutive pixels of one plane
 // per lane quad position (full 32-byte sectors).
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int kDgThreads = 384;
-constexpr int kDgBox = 10 * 16 * 64;      // one {32 ch, 16, 10} box of dZ: 10 KB
-constexpr int kDgStage = 3 * kDgBox;      // the three column shifts of one tile
 constexpr int kDgStages = 6;
 constexpr int kDgB = 9 * 8 * 64;          // B image: [tap][8 rows][32 co] bf16
 
@@ -271,7 +257,8 @@ first_conv_dgrad_kernel(const __grid_constant__ CUtensorMap tmZ, const FirstConv
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = ptx::smem_u32(smem_raw);
     uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
-    uint8_t* b_s = smem + kDgStages * kDgStage;
+    constexpr int slot_bytes = halo_slot_bytes(32);
+    uint8_t* b_s = smem + kDgStages * slot_bytes;
     uint64_t* full = reinterpret_cast<uint64_t*>(b_s + kDgB);
     uint64_t* empty = full + kDgStages;
     const int total_tiles = p.n_img * p.tiles_x * p.tiles_y;
@@ -299,12 +286,11 @@ first_conv_dgrad_kernel(const __grid_constant__ CUtensorMap tmZ, const FirstConv
             int s = 0;
             uint32_t ph = 0;
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                int img, y0, x0;
-                fc_tile_coords(p, tile, img, y0, x0);
+                const TileCoord tc = tile_coord(tile, p.tiles_x, p.tiles_y);
                 ptx::mbar_wait(&empty[s], ph ^ 1u);
-                uint8_t* sa = smem + (size_t)s * kDgStage;
-                ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)kDgStage);
-                for (int b = 0; b < 3; ++b) ptx::tma_load_5d(sa + b * kDgBox, &tmZ, &full[s], 0, x0 + b - 1, y0 - 1, img, 0);
+                uint8_t* sa = smem + (size_t)s * slot_bytes;
+                ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)slot_bytes);
+                halo_load<32>(sa, &tmZ, &full[s], 0, tc.x0, tc.y0, tc.img);
                 if (++s == kDgStages) { s = 0; ph ^= 1u; }
             }
         }
@@ -315,7 +301,7 @@ first_conv_dgrad_kernel(const __grid_constant__ CUtensorMap tmZ, const FirstConv
     const int cg = (threadIdx.x >> 7) - 1;
     const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
     const uint64_t desc0 = ptx::make_gmma_desc(0, 16, 512, ptx::GMMA_SW64);
-    const uint64_t bd0 = desc0 | (uint64_t)((ptx::smem_u32(b_s) & 0x3FFFFu) >> 4);
+    const uint64_t bd0 = ptx::desc_at(desc0, ptx::smem_u32(b_s));
     const uint32_t a0 = ptx::smem_u32(smem) + (uint32_t)(cg * 64 * 64);
     const size_t plane = (size_t)p.H * p.W;
     const int c0 = 2 * (lane & 3);                 // this lane's accumulator columns: input channels c0, c0 + 1
@@ -324,12 +310,11 @@ first_conv_dgrad_kernel(const __grid_constant__ CUtensorMap tmZ, const FirstConv
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         float acc[4] = { 0.f, 0.f, 0.f, 0.f };
         ptx::mbar_wait(&full[s], ph);
-        const uint32_t sa = a0 + (uint32_t)(s * kDgStage);
+        const uint32_t sa = a0 + (uint32_t)(s * slot_bytes);
         ptx::wgmma_fence();
 #pragma unroll
         for (int tap = 0; tap < 9; ++tap) {
-            const int ty = tap / 3, tx = tap - 3 * ty;     // box tx, 16 ty pixel rows down
-            const uint64_t ad = desc0 | (uint64_t)(((sa + (uint32_t)(tx * kDgBox + ty * 16 * 64)) & 0x3FFFFu) >> 4);
+            const uint64_t ad = ptx::desc_at(desc0, sa + halo_tap_off(32, tap));
             const uint64_t bd = bd0 + (uint64_t)((tap * 512) >> 4);
 #pragma unroll
             for (int k = 0; k < 2; ++k)                    // +32 bytes along K inside the swizzle atom
@@ -342,10 +327,9 @@ first_conv_dgrad_kernel(const __grid_constant__ CUtensorMap tmZ, const FirstConv
         if (++s == kDgStages) { s = 0; ph ^= 1u; }
 
         // ---- epilogue: acc[2i + j] = D[pixel row 16 wq + lane / 4 + 8 i][column c0 + j] ----
-        int img, y0, x0;
-        fc_tile_coords(p, tile, img, y0, x0);
+        const TileCoord tc = tile_coord(tile, p.tiles_x, p.tiles_y);
         const int m = cg * 64 + 16 * wq + (lane >> 2);
-        float* dst = p.dx + (size_t)img * p.cin * plane + (size_t)(y0 + (m >> 4)) * p.W + (x0 + (m & 15));
+        float* dst = p.dx + (size_t)tc.img * p.cin * plane + (size_t)(tc.y0 + (m >> 4)) * p.W + (tc.x0 + (m & 15));
 #pragma unroll
         for (int i = 0; i < 2; ++i)
 #pragma unroll

@@ -3,7 +3,7 @@
 //   fused Adam.
 #include "common.cuh"
 #include "unet_ew.h"
-#include "umma.cuh"
+#include "wgmma.cuh"
 #include <cuda_bf16.h>
 #include <algorithm>
 
@@ -22,7 +22,7 @@ __device__ __forceinline__ uint32_t pack_bf2(float a, float b)
 // 2x2 max-pool backward, NHWC bf16                                                      (Unet.py:51-63)
 // ---------------------------------------------------------------------------------------------------
 // dZ[full res] = ( dskip + (first arg-max of the window ? dP : 0) ) * lrelu'(A)
-//   A     : activation that was pooled - never read: the forward tile's epilogue (conv_umma.cuh) leaves a 1-byte-per-
+//   A     : activation that was pooled - never read: the forward tile's epilogue (conv_gemm.cuh) leaves a 1-byte-per-
 //           pooled-element code instead, per (pooled pixel, 32 channels) eight words - "not the maximum" masks of the
 //           window's four pixels, then their sign masks (channel 2j -> bit j, 2j+1 -> bit 16+j).  That is 1/16 of what
 //           the activation costs (and the level-1 skip half of an interleaved concat buffer cost double: 128-byte lines

@@ -4,10 +4,10 @@
 #include <algorithm>
 #include <cstdlib>
 #include <cstdio>
-#include "conv_umma.cuh"
+#include "conv_gemm.cuh"
 #include "conv3x3_thin.cuh"
 #include "conv3x3_wide.cuh"
-#include "wgrad_umma.cuh"
+#include "wgrad_gemm.cuh"
 #include "wgrad_thin.cuh"
 #include "first_conv.cuh"
 #include "unet_prims.h"
@@ -153,16 +153,16 @@ static int conv_gemm_params(const GemmOp& op, ConvGemmParams& p)
     return ELD_OK;
 }
 
-// the 3x3 convolutions read halo boxes {kc, 16, 10} around each 8 x 16 tile: the thin ones (one channel chunk, one N block)
-// with resident weights (conv3x3_thin.cuh), the others with a weight ring (conv3x3_wide.cuh)
+// the 3x3 convolutions read the halo boxes {kc, 16, 10} around each 8 x 16 tile (tile.cuh): the thin ones (one channel
+// chunk, one N block) with resident weights (conv3x3_thin.cuh), the others with a weight ring (conv3x3_wide.cuh)
 static int launch_conv3x3(eld_ctx* ctx, const GemmOp& op, ConvGemmParams& p, cudaStream_t st)
 {
     CUtensorMap tmA;
-    { int rc = encode_nhwc(ctx, &tmA, op.a, op.a_pitch, op.n_img, op.H, op.W, p.kc, 16, kThinBoxRows); if (rc) return rc; }
+    { int rc = encode_nhwc(ctx, &tmA, op.a, op.a_pitch, op.n_img, op.H, op.W, p.kc, kConvTileW, kHaloRows); if (rc) return rc; }
     const int rb = p.kc * 2;
+    const int slot_bytes = halo_slot_bytes(p.kc);
     if ((op.cin == 32 || op.cin == 64) && (p.n_total == 32 || p.n_total == 64)) {
         // [resident weights][halo slots][staging of both consumer warpgroups][bias][barriers] after the 1024-byte alignment
-        const int slot_bytes = 3 * kThinBoxRows * 16 * rb;
         const int fixed = 9 * p.n_tile * rb + 2 * kThinStgBytes + 256;
         int slots = (kThinSmemBytes - 1024 - fixed - 256) / slot_bytes;
         if (slots > kThinMaxSlots) slots = kThinMaxSlots;
@@ -179,7 +179,6 @@ static int launch_conv3x3(eld_ctx* ctx, const GemmOp& op, ConvGemmParams& p, cud
     // [halo slots][weight ring][staging of both consumer warpgroups][bias][barriers] after the 1024-byte alignment;
     // the weight ring takes what the opt-in maximum leaves
     const int stg_bytes = 2 * 64 * kConvStg * 4;
-    const int slot_bytes = 3 * kThinBoxRows * 16 * rb;
     const int b_bytes = p.n_tile * rb;
     const int fixed = kWideHaloSlots * slot_bytes + stg_bytes + 4096;
     int wstages = (kThinSmemBytes - 1024 - 256 - fixed) / b_bytes;
@@ -282,7 +281,7 @@ int launch_first_conv_wgrad(eld_ctx* ctx, const float* x, int cin, const void* d
 }
 
 // align slack, the TMA ring, the B image, full / empty barriers
-static size_t first_conv_dgrad_smem() { return 1024 + kDgStages * kDgStage + kDgB + 2 * kDgStages * 8; }
+static size_t first_conv_dgrad_smem() { return 1024 + kDgStages * halo_slot_bytes(32) + kDgB + 2 * kDgStages * 8; }
 
 int launch_first_conv_dgrad(eld_ctx* ctx, const void* dz, const float* w, int cin, float* dx, int n, int H, int W,
                             cudaStream_t st)
@@ -293,7 +292,7 @@ int launch_first_conv_dgrad(eld_ctx* ctx, const void* dz, const float* w, int ci
     p.n_img = n; p.H = H; p.W = W; p.tiles_x = W / 16; p.tiles_y = H / 8; p.cin = cin;
     p.w = w; p.dx = dx;
     CUtensorMap tmZ;
-    { int rc = encode_nhwc(ctx, &tmZ, dz, 32, n, H, W, 32, 16, 10); if (rc) return rc; }
+    { int rc = encode_nhwc(ctx, &tmZ, dz, 32, n, H, W, 32, kConvTileW, kHaloRows); if (rc) return rc; }
     const int total = n * p.tiles_x * p.tiles_y;
     return launch(ctx, first_conv_dgrad_kernel, std::min(total, ctx->num_sms), kDgThreads, first_conv_dgrad_smem(), st, tmZ, p);
 }
@@ -333,7 +332,7 @@ static int launch_wgrad_thin(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
     p.stages = stages;
 
     CUtensorMap tmP, tmQ;
-    { int rc = encode_nhwc(ctx, &tmP, op.p, op.p_pitch, op.n_img, op.H, op.W, op.p_ch, 16, kThinBoxRows); if (rc) return rc; }
+    { int rc = encode_nhwc(ctx, &tmP, op.p, op.p_pitch, op.n_img, op.H, op.W, op.p_ch, kConvTileW, kHaloRows); if (rc) return rc; }
     { int rc = encode_nhwc(ctx, &tmQ, op.q, op.q_pitch, op.n_img, op.H, op.W, op.q_ch, 16, 8); if (rc) return rc; }
     const size_t smem = 1024 + (size_t)stages * slot_bytes + 256;
     const int total_tiles = op.n_img * p.tiles_x * p.tiles_y;

@@ -1,15 +1,13 @@
 // wgrad_thin.cuh - wgmma weight-gradient tile for the thin 3x3 convolutions (cin and cout in {32, 64}): the
-// full- and half-resolution layers, where the generic tile (wgrad_umma.cuh) loads every pixel of X once per filter tap.
+// full- and half-resolution layers, where the generic tile (wgrad_gemm.cuh) loads every pixel of X once per filter tap.
 //
 //   D[(tap, ci) x co] (f32, registers)  =  sum over pixels p   X[p + tap shift, ci] * dZ[p, co]
 //
 // Grid    = one persistent CTA per SM; CTA b owns tiles [b T / G, (b + 1) T / G) of the T 8 x 16 pixel tiles (a
 //           contiguous run, so vertically neighbouring halos meet in L2) and the layer's whole dW (+ db) for them.
-// P (X)   = per tile three TMA boxes {KC, 16, 10} at columns x0 - 1, x0, x0 + 1 and rows y0 - 1 .. y0 + 8 (zero-filled
-//           outside the image = the padding), the fprop thin tile's geometry.  Consumed MN-major: tap (dy, dx) is box
-//           dx + 1 from pixel row 16 (dy + 1) on, a whole number of swizzle atoms (1 KB at SW64, 2 KB at SW128), and k16
-//           step k is tile row k.  KC = 64: one tap = one m64 unit (9 units).  KC = 32: two taps share one m64 unit, the
-//           second 32 rows at the descriptor's LBO: (dy = -1, dx) + (0, dx) at LBO = 1 KB for each dx, (1, -1) + (1, 0)
+// P (X)   = the halo of each tile (tile.cuh), as the fprop thin tile loads it.  Consumed MN-major: a tap starts a whole
+//           number of swizzle atoms into the slot (halo_tap_off), and k16 step k is tile row k.  KC = 64: one tap = one
+//           m64 unit (9 units).  KC = 32: two taps share one m64 unit, the second 32 rows at the descriptor's LBO: (dy = -1, dx) + (0, dx) at LBO = 1 KB for each dx, (1, -1) + (1, 0)
 //           and (1, 0) + (1, 1) at LBO = one box (5 units; the first half of the last duplicates a tap and is dropped).
 // Q (dZ)  = one {NT, 16, 8} box per tile, MN-major.  Its column sums are the bias gradient, summed from shared memory
 //           while the MMAs run.
@@ -18,7 +16,7 @@
 //           units into the gradient with vector red.global.add.  The 160 accumulator registers of (64 -> 64) need more
 //           than the 168 a 384-thread CTA gets evenly: setmaxnreg moves registers from the producer to the consumers.
 #pragma once
-#include "umma.cuh"
+#include "wgmma.cuh"
 #include "unet_prims.h"
 #include "conv3x3_thin.cuh"
 #include <cuda_bf16.h>
@@ -40,23 +38,21 @@ constexpr int kWgThinThreads = 384;
 constexpr int kWgThinProducerRegs = 40;
 constexpr int kWgThinConsumerRegs = 232;      // 128 x 40 + 256 x 232 <= 64 K registers
 
-// bytes of one pipeline slot: three halo boxes of X and the dZ box
-__host__ __device__ constexpr int wgrad_thin_box_bytes(int kc) { return kThinBoxRows * 16 * kc * 2; }
-__host__ __device__ constexpr int wgrad_thin_slot_bytes(int kc, int nt) { return 3 * wgrad_thin_box_bytes(kc) + 128 * nt * 2; }
+// bytes of one pipeline slot: the halo of X and the dZ box behind it
+__host__ __device__ constexpr int wgrad_thin_slot_bytes(int kc, int nt) { return halo_slot_bytes(kc) + 128 * nt * 2; }
 __host__ __device__ constexpr int wgrad_thin_units(int kc) { return kc == 64 ? 9 : 5; }
 
-// m64 unit u: byte offset of its first half inside a slot, and the LBO to its second 32 rows (KC = 32)
+// m64 unit u: byte offset of its first half inside a slot (tap u; at KC = 32 taps 0, 1, 2, 6, 7), and the LBO to its
+// second 32 rows (KC = 32): one tap row down for u < 3, one tap column right for the last two
 template <int KC>
 __device__ __forceinline__ constexpr uint32_t wg_unit_off(int u)
 {
-    constexpr int box = wgrad_thin_box_bytes(KC), row = KC * 2;
-    if (KC == 64) return (uint32_t)((u % 3) * box + (u / 3) * 16 * row);
-    return (uint32_t)(u < 3 ? u * box : (u - 3) * box + 32 * row);
+    return halo_tap_off(KC, KC == 64 || u < 3 ? u : u + 3);
 }
 template <int KC>
 __device__ __forceinline__ constexpr uint32_t wg_unit_lbo(int u)
 {
-    return KC == 64 ? 0u : (u < 3 ? 16u * KC * 2 : (uint32_t)wgrad_thin_box_bytes(KC));
+    return KC == 64 ? 0u : halo_tap_off(KC, u < 3 ? 3 : 1);
 }
 // filter tap (kh * 3 + kw) of row m of unit u, and its input channel; -1 = a duplicated half, dropped
 template <int KC>
@@ -72,7 +68,7 @@ template <int NT, int KC, int U0, int NU>
 __device__ __forceinline__ void wgrad_thin_consume(const WgradThinParams& p, uint8_t* smem, uint64_t* full, uint64_t* empty,
                                                    int ntiles, int bt)
 {
-    constexpr int box_bytes = wgrad_thin_box_bytes(KC), slot_bytes = wgrad_thin_slot_bytes(KC, NT);
+    constexpr int q_off = halo_slot_bytes(KC), slot_bytes = wgrad_thin_slot_bytes(KC, NT);   // dZ box / slot
     constexpr int p_row = KC * 2, q_row = NT * 2;
     constexpr uint32_t a_step = (16u * p_row) >> 4, b_step = (16u * q_row) >> 4;   // one k16 step = one tile row
     const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
@@ -103,18 +99,18 @@ __device__ __forceinline__ void wgrad_thin_consume(const WgradThinParams& p, uin
     for (int i = 0; i < ntiles; ++i) {
         ptx::mbar_wait(&full[s], ph);
         const uint32_t st = smem_base + (uint32_t)(s * slot_bytes);
-        const uint64_t bd = b_desc0 | (uint64_t)(((st + (uint32_t)(3 * box_bytes)) & 0x3FFFFu) >> 4);
+        const uint64_t bd = ptx::desc_at(b_desc0, st + (uint32_t)q_off);
         ptx::wgmma_fence();
 #pragma unroll
         for (int k = 0; k < 8; ++k)
 #pragma unroll
             for (int u = 0; u < NU; ++u) {
-                const uint64_t ad = a_desc0[u] | (uint64_t)(((st + wg_unit_off<KC>(U0 + u)) & 0x3FFFFu) >> 4);
+                const uint64_t ad = ptx::desc_at(a_desc0[u], st + wg_unit_off<KC>(U0 + u));
                 ptx::wgmma_bf16<NT, 1, 1>(acc[u], ad + (uint64_t)(k * a_step), bd + (uint64_t)(k * b_step), 1u);
             }
         ptx::wgmma_commit();
         if (bias_on) {
-            const uint8_t* q = smem + (size_t)s * slot_bytes + 3 * box_bytes;
+            const uint8_t* q = smem + (size_t)s * slot_bytes + q_off;
 #pragma unroll
             for (int r = 0; r < 128 / BR; ++r) {
                 const int row = br + r * BR;
@@ -193,7 +189,7 @@ conv3x3_wgrad_thin_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_
     const uint32_t raw = ptx::smem_u32(smem_raw);
     uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
 
-    constexpr int box_bytes = wgrad_thin_box_bytes(KC), slot_bytes = wgrad_thin_slot_bytes(KC, NT);
+    constexpr int slot_bytes = wgrad_thin_slot_bytes(KC, NT);
     constexpr int units = wgrad_thin_units(KC), u_first = (units + 1) / 2;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * slot_bytes);
     uint64_t* empty = full + p.stages;
@@ -227,8 +223,8 @@ conv3x3_wgrad_thin_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_
                 uint8_t* sa = smem + (size_t)s * slot_bytes;
                 ptx::mbar_wait(&empty[s], ph ^ 1u);
                 ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)slot_bytes);
-                for (int b = 0; b < 3; ++b) ptx::tma_load_5d(sa + b * box_bytes, &tmP, &full[s], p.p_c0, x0 + b - 1, y0 - 1, img, 0);
-                ptx::tma_load_5d(sa + 3 * box_bytes, &tmQ, &full[s], p.q_c0, x0, y0, img, 0);
+                halo_load<KC>(sa, &tmP, &full[s], p.p_c0, x0, y0, img);
+                ptx::tma_load_5d(sa + halo_slot_bytes(KC), &tmQ, &full[s], p.q_c0, x0, y0, img, 0);
                 if (++s == p.stages) { s = 0; ph ^= 1u; }
                 if (++tx == p.tiles_x) { tx = 0; if (++ty == p.tiles_y) { ty = 0; ++img; } }
             }

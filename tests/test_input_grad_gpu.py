@@ -4,7 +4,7 @@ behind eld_unet_input_grad and `_EngineFunction.backward`.
 Gates (bf16 stored dz1_1 and bf16 conv1_1 weights, fp32 accumulation, fp32 output), with the reference's L1 loss:
   the tile itself: conv1_1's data and weight gradients are read from the same stored dz1_1, so per input plane c
       <dx[:, c], bf16(x)[:, c]> = <bf16(W1)[:, c], dW1[:, c]>
-    holds up to fp32 summation order whatever the upstream rounding did: |difference| <= 2e-5 of the summed |terms|;
+    holds up to the order of the fp32 additions whatever the upstream rounding did: |difference| <= 2e-5 of the summed |terms|;
   vs the bf16-emulated backward (tests/unet_emul.py, same rounding points): rel-L2 <= 5e-2, on the whole gradient and on
     the 4-pixel border ring alone (padding and halo).  dx is a per-pixel quantity at the end of the whole backward chain,
     a sum of 288 signed terms per element: the engine's and the emulation's rounding and pool-argmax decisions drift

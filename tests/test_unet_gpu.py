@@ -189,7 +189,7 @@ def test_srgb_channel_variants(torch, io):
 
 def test_pool_ties_route_like_max_pool2d(torch):
     """Frames made of constant 8 x 8 blocks: a quarter of all 2 x 2 pool windows hold four EQUAL bf16 activations.  The
-    pool backward works from the 1-byte code the forward tile leaves (argmax + signs, conv_umma.cuh / unet_ew.cu) and
+    pool backward works from the 1-byte code the forward tile leaves (argmax + signs, conv_gemm.cuh / unet_ew.cu) and
     must route the gradient of a tie to the first element in window order, as nn.MaxPool2d does (Unet.py:13); the
     LeakyReLU' masks come from the sign words.  Every gradient tensor against the bf16-emulated backward."""
     from tests.unet_emul import emulated_train_step, fp32_cuda
