@@ -70,131 +70,7 @@ constexpr int kGradBuckets = 4;
 constexpr int kBucketFirst[kGradBuckets] = { I_UP6, I_C51, I_C21, I_C11 };
 static int bucket_end(int k) { return k == 0 ? kNumLayers : kBucketFirst[k - 1]; }
 
-// perm: the layer's weight trains, so the gradient permute moves its tiles (derive_needs)
-struct PackEntry { unsigned long long src, dst_f, dst_d; int cout, cin, type; int perm; };
-struct PackTable {
-    PackEntry e[kNumLayers];
-    int tile0[kNumLayers + 1];   // prefix sum of (cout/32 x cin/32) tiles per entry: one block per tile, whatever the layer
-    int n;
-    unsigned long long first_stage, first_dst, first_wf;
-    int first_cin;
-};
-
-// flattened tile id -> (entry, tile inside the entry)
-__device__ __forceinline__ int find_entry(const PackTable& T, int tile, int& local)
-{
-    int k = 0;
-    while (k + 1 < T.n && tile >= T.tile0[k + 1]) ++k;
-    local = tile - T.tile0[k];
-    return k;
-}
-
-// packed_index (unet_prims.h) with everything that is uniform over a 32 x 32 tile hoisted: rows n0..n0+31 and K
-// channels c0..c0+31 stay inside one n-tile and one channel chunk, so only the row / in-chunk channel vary.
-struct PackTileBase { size_t base0, tap_stride; int r0, cc0, kc; };
-__device__ __forceinline__ PackTileBase pack_tile_base(int rows, int ck, int taps, int n0, int c0)
-{
-    const int n_tile = rows <= 256 ? rows : 256;
-    const int kc = (ck % 64 == 0) ? 64 : 32;
-    const int kchunks = ck / kc;
-    const int nt = n0 / n_tile, chunk = c0 / kc;
-    PackTileBase b;
-    b.tap_stride = (size_t)kchunks * n_tile * kc;
-    b.base0 = ((size_t)nt * taps * kchunks + chunk) * ((size_t)n_tile * kc);
-    b.r0 = n0 - nt * n_tile; b.cc0 = c0 - chunk * kc; b.kc = kc;
-    return b;
-}
-__device__ __forceinline__ size_t pack_tile_index(const PackTileBase& b, int tap, int dn, int dc)
-{
-    const int r = b.r0 + dn, cc = b.cc0 + dc, rb = b.kc * 2;
-    const int swz = rb == 128 ? (r & 7) : ((r >> 1) & 3);
-    const int byte = r * rb + ((((cc * 2) >> 4) ^ swz) << 4) + ((cc * 2) & 15);
-    return b.base0 + (size_t)tap * b.tap_stride + (size_t)(byte >> 1);
-}
-
-// one launch packs every layer's fp32 master weights into both bf16 GEMM operands (fprop + dgrad).
-// A block moves a (32 x 32 x taps) tile through shared memory so that reads are 1 KB runs and writes are
-// 64-byte runs in both destination layouts.
-__global__ void __launch_bounds__(256)
-pack_all_kernel(const float* __restrict__ params, __nv_bfloat16* __restrict__ packed, const __grid_constant__ PackTable T)
-{
-    __shared__ float tile[32][32 * 9 + 1];
-    if ((int)blockIdx.x >= T.tile0[T.n]) {   // conv1_1: w[32][4][9] -> K-major operand [32 co][64 k], k = tap*4 + c (first_conv.cuh),
-        const float* w1 = params + T.first_dst;   // 128-byte rows with the SW128 swizzle; k >= 36 are zeros (k = 36 meets the ones column)
-        const int b = (int)blockIdx.x - T.tile0[T.n], nb = (int)gridDim.x - T.tile0[T.n];
-        for (int i = b * 256 + threadIdx.x; i < 32 * 64; i += nb * 256) {
-            const int co = i >> 6, k = i & 63, tap = k >> 2, c = k & 3;
-            const float v = (k < 36 && c < T.first_cin) ? w1[(co * T.first_cin + c) * 9 + tap] : 0.0f;
-            packed[T.first_wf + (size_t)co * 64 + ((((k >> 3) ^ (co & 7)) << 3) | (k & 7))] = __float2bfloat16_rn(v);
-        }
-        return;
-    }
-    int tl;
-    const PackEntry& e = T.e[find_entry(T, (int)blockIdx.x, tl)];
-    const float* w = params + e.src;
-    __nv_bfloat16* of = packed + e.dst_f;
-    __nv_bfloat16* od = packed + e.dst_d;
-    if (e.type == L_CONV3) {              // w[co][ci][t]
-        const int it = e.cin / 32;
-        {
-            const int co0 = (tl / it) * 32, ci0 = (tl % it) * 32;
-            if ((reinterpret_cast<uintptr_t>(params) & 15) == 0) {     // layer offsets are multiples of 4 floats: 16-byte loads
-                for (int i = threadIdx.x; i < 32 * 72; i += 256) {
-                    const int co = i / 72, r4 = i - co * 72;
-                    const float4 v = __ldg(reinterpret_cast<const float4*>(w + ((size_t)(co0 + co) * e.cin + ci0) * 9) + r4);
-                    float* t4 = &tile[co][4 * r4];
-                    t4[0] = v.x; t4[1] = v.y; t4[2] = v.z; t4[3] = v.w;
-                }
-            } else {
-                for (int i = threadIdx.x; i < 32 * 288; i += 256) {
-                    const int co = i / 288, r = i - co * 288;              // r = ci*9 + t
-                    tile[co][r] = w[((size_t)(co0 + co) * e.cin + ci0) * 9 + r];
-                }
-            }
-            __syncthreads();
-            // eight adjacent K elements per thread = one 16-byte chunk of the swizzled row (chunks are what the swizzle permutes)
-            const PackTileBase bf = pack_tile_base(e.cout, e.cin, 9, co0, ci0), bd = pack_tile_base(e.cin, e.cout, 9, ci0, co0);
-            for (int i = threadIdx.x; i < 32 * 36; i += 256) {        // fprop: [co][t][ci]
-                const int ci = (i & 3) * 8, t = (i >> 2) % 9, co = i / 36;
-                uint32_t q[4];
-#pragma unroll
-                for (int e2 = 0; e2 < 4; ++e2) {
-                    const __nv_bfloat162 v2 = __floats2bfloat162_rn(tile[co][(ci + 2 * e2) * 9 + t], tile[co][(ci + 2 * e2 + 1) * 9 + t]);
-                    q[e2] = *reinterpret_cast<const uint32_t*>(&v2);
-                }
-                *reinterpret_cast<uint4*>(of + pack_tile_index(bf, t, co, ci)) = make_uint4(q[0], q[1], q[2], q[3]);
-            }
-            for (int i = threadIdx.x; i < 32 * 36; i += 256) {        // dgrad: [ci][8-t][co]
-                const int co = (i & 3) * 8, t = (i >> 2) % 9, ci = i / 36;
-                uint32_t q[4];
-#pragma unroll
-                for (int e2 = 0; e2 < 4; ++e2) {
-                    const __nv_bfloat162 v2 = __floats2bfloat162_rn(tile[co + 2 * e2][ci * 9 + t], tile[co + 2 * e2 + 1][ci * 9 + t]);
-                    q[e2] = *reinterpret_cast<const uint32_t*>(&v2);
-                }
-                *reinterpret_cast<uint4*>(od + pack_tile_index(bd, 8 - t, ci, co)) = make_uint4(q[0], q[1], q[2], q[3]);
-            }
-        }
-    } else {                              // deconv wt[ci][co][s]
-        const int ct = e.cout / 32;
-        {
-            const int ci0 = (tl / ct) * 32, co0 = (tl % ct) * 32;
-            for (int i = threadIdx.x; i < 32 * 128; i += 256) {
-                const int ci = i / 128, r = i - ci * 128;              // r = co*4 + s
-                tile[ci][r] = w[((size_t)(ci0 + ci) * e.cout + co0) * 4 + r];
-            }
-            __syncthreads();
-            for (int i = threadIdx.x; i < 32 * 128; i += 256) {       // fprop: [(s*cout + co)][ci]
-                const int ci = i & 31, co = (i >> 5) & 31, sp = i >> 10;
-                of[packed_index(4 * e.cout, e.cin, 1, sp * e.cout + co0 + co, 0, ci0 + ci)] = __float2bfloat16_rn(tile[ci][co * 4 + sp]);
-            }
-            for (int i = threadIdx.x; i < 32 * 128; i += 256) {       // dgrad: [ci][s][co]
-                const int co = i & 31, sp = (i >> 5) & 3, ci = i >> 7;
-                od[packed_index(e.cin, e.cout, 4, ci0 + ci, sp, co0 + co)] = __float2bfloat16_rn(tile[ci][co * 4 + sp]);
-            }
-        }
-    }
-}
+static_assert(kNumLayers <= kPackMaxEntries, "the packing table (unet_prims.h) holds one entry per layer at most");
 
 // staging [tap][ci][co] -> PyTorch OIHW [co][ci][tap]; one block per (32 co x 32 ci) tile of one layer
 __global__ void __launch_bounds__(256)
@@ -207,7 +83,7 @@ wgrad_permute_kernel(const float* __restrict__ gtmp, float* __restrict__ grads, 
     if (gtile >= tile_end) return;
     int t;
     const PackEntry& e = T.e[find_entry(T, gtile, t)];
-    if (e.type != L_CONV3 || !e.perm) return;     // a frozen weight's range of grads keeps the zeros of the step's memset
+    if (e.deconv || !e.perm) return;     // a frozen weight's range of grads keeps the zeros of the step's memset
     const int ct = e.cout / 32;
     {
         const int co0 = (t % ct) * 32, ci0 = (t / ct) * 32;
@@ -477,7 +353,7 @@ extern "C" int eld_unet_create_io(eld_ctx* ctx, int n, int h, int w, int train, 
         const Layer& l = u->L[i];
         if (i == I_C11 || l.type == L_CONV1) continue;
         u->table.tile0[k] = k == 0 ? 0 : u->table.tile0[k - 1] + (u->table.e[k - 1].cout / 32) * (u->table.e[k - 1].cin / 32);
-        u->table.e[k++] = PackEntry{ l.w_off, l.wf_off, l.wd_off, l.cout, l.cin, l.type, 1 };
+        u->table.e[k++] = PackEntry{ l.w_off, l.wf_off, l.wd_off, l.cout, l.cin, l.type == L_DECONV, 1 };
     }
     u->table.tile0[k] = u->table.tile0[k - 1] + (u->table.e[k - 1].cout / 32) * (u->table.e[k - 1].cin / 32);
     u->table.n = k;
@@ -490,7 +366,7 @@ extern "C" int eld_unet_create_io(eld_ctx* ctx, int n, int h, int w, int train, 
         memset(all, 1, sizeof(all));
         derive_needs(u, all, true);
     }
-    // conv1_1's operand image: zero once (pack_all rewrites all of it every step anyway)
+    // conv1_1's operand image: zero once (the packer rewrites all of it every step anyway)
     ELD_CHECK_CUDA(cudaMemset(u->fs.packed + u->L[I_C11].wf_off, 0, 32 * 9 * 32 * sizeof(__nv_bfloat16)));
     // opt in to large dynamic shared memory once (not inside a captured region)
     { int rc = init_gemm_kernels(ctx); if (rc != ELD_OK) { delete u; return rc; } }
@@ -771,10 +647,7 @@ struct Runner {
     int pack() const
     {
         Scope sc(u, st, "weights", "pack", 0.0, (double)u->n_params * 8);
-        pack_all_kernel<<<u->table.tile0[u->table.n] + 2, 256, 0, st>>>(params, s->packed, u->table);
-        ELD_CHECK_CUDA(cudaGetLastError());
-        count_launch(ctx());
-        return ELD_OK;
+        return launch_pack(ctx(), params, s->packed, u->table, true, st);
     }
 
     int forward(const float* x) const

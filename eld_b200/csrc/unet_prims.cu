@@ -385,42 +385,125 @@ int launch_wgrad(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
     return launch(ctx, kWgradGemm[n_tile / 64], items * p.ksplit, kWgradThreads, smem, st, tmP, tmQ, p);
 }
 
-// ---- weight packing: fp32 master (PyTorch layout) -> bf16 K-major GEMM operand -------------------
-__global__ void pack_weights_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ out,
-                                    int cout, int cin, int kind)
+// ---- weight packing: fp32 master (PyTorch layout) -> bf16 K-major GEMM operands --------------------------------------
+// One launch packs every entry's fprop and dgrad operand (PACK_CONV_* / PACK_DECONV_*), whichever it names.
+// A block moves a (32 x 32 x taps) tile through shared memory so that reads are 1 KB runs and writes are
+// 64-byte runs in both destination layouts.
+// eight bf16 at dst: one 16-byte store, or eight 2-byte ones into an operand that is not 16-byte aligned (eld_pack_weights
+// takes any buffer)
+__device__ __forceinline__ void store_chunk(__nv_bfloat16* dst, const uint32_t (&q)[4], bool vec)
 {
-    const int ksz = (kind == PACK_CONV_FPROP || kind == PACK_CONV_DGRAD) ? 9 : 4;
-    const size_t total = (size_t)cout * cin * ksz;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        float v;
-        size_t dst;
-        if (kind == PACK_CONV_FPROP) {            // B[co][t][ci] = W[co][ci][kh][kw], t = kh*3+kw
-            const int ci = i % cin, t = (i / cin) % 9, co = i / ((size_t)cin * 9);
-            v = w[((size_t)co * cin + ci) * 9 + t];
-            dst = packed_index(cout, cin, 9, co, t, ci);
-        } else if (kind == PACK_CONV_DGRAD) {     // B[ci][t'][co] = W[co][ci][2-kh'][2-kw'] = W[..][8-t']
-            const int co = i % cout, t = (i / cout) % 9, ci = i / ((size_t)cout * 9);
-            v = w[((size_t)co * cin + ci) * 9 + (8 - t)];
-            dst = packed_index(cin, cout, 9, ci, t, co);
-        } else if (kind == PACK_DECONV_FPROP) {   // B[(s*cout + co)][ci] = Wt[ci][co][kh][kw], s = kh*2+kw
-            const int ci = i % cin, co = (i / cin) % cout, s = i / ((size_t)cin * cout);
-            v = w[((size_t)ci * cout + co) * 4 + s];
-            dst = packed_index(4 * cout, cin, 1, s * cout + co, 0, ci);
-        } else {                                  // PACK_DECONV_DGRAD: B[ci][s][co] = Wt[ci][co][s]
-            const int co = i % cout, s = (i / cout) % 4, ci = i / ((size_t)cout * 4);
-            v = w[((size_t)ci * cout + co) * 4 + s];
-            dst = packed_index(cin, cout, 4, ci, s, co);
+    if (vec) {
+        *reinterpret_cast<uint4*>(dst) = make_uint4(q[0], q[1], q[2], q[3]);
+        return;
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) dst[k] = __ushort_as_bfloat16((unsigned short)(q[k >> 1] >> (16 * (k & 1))));
+}
+
+__global__ void __launch_bounds__(256)
+pack_weights_kernel(const float* __restrict__ params, __nv_bfloat16* __restrict__ packed, const __grid_constant__ PackTable T)
+{
+    __shared__ float tile[32][32 * 9 + 1];
+    if ((int)blockIdx.x >= T.tile0[T.n]) {   // conv1_1: w[32][4][9] -> K-major operand [32 co][64 k], k = tap*4 + c (first_conv.cuh),
+        const float* w1 = params + T.first_dst;   // 128-byte rows with the SW128 swizzle; k >= 36 are zeros (k = 36 meets the ones column)
+        const int b = (int)blockIdx.x - T.tile0[T.n], nb = (int)gridDim.x - T.tile0[T.n];
+        for (int i = b * 256 + threadIdx.x; i < 32 * 64; i += nb * 256) {
+            const int co = i >> 6, k = i & 63, tap = k >> 2, c = k & 3;
+            const float v = (k < 36 && c < T.first_cin) ? w1[(co * T.first_cin + c) * 9 + tap] : 0.0f;
+            packed[T.first_wf + (size_t)co * 64 + ((((k >> 3) ^ (co & 7)) << 3) | (k & 7))] = __float2bfloat16_rn(v);
         }
-        out[dst] = __float2bfloat16_rn(v);
+        return;
+    }
+    int tl;
+    const PackEntry& e = T.e[find_entry(T, (int)blockIdx.x, tl)];
+    const float* w = params + e.src;
+    if (!e.deconv) {                      // w[co][ci][t]
+        const int it = e.cin / 32;
+        {
+            const int co0 = (tl / it) * 32, ci0 = (tl % it) * 32;
+            if ((reinterpret_cast<uintptr_t>(params) & 15) == 0) {     // layer offsets are multiples of 4 floats: 16-byte loads
+                for (int i = threadIdx.x; i < 32 * 72; i += 256) {
+                    const int co = i / 72, r4 = i - co * 72;
+                    const float4 v = __ldg(reinterpret_cast<const float4*>(w + ((size_t)(co0 + co) * e.cin + ci0) * 9) + r4);
+                    float* t4 = &tile[co][4 * r4];
+                    t4[0] = v.x; t4[1] = v.y; t4[2] = v.z; t4[3] = v.w;
+                }
+            } else {
+                for (int i = threadIdx.x; i < 32 * 288; i += 256) {
+                    const int co = i / 288, r = i - co * 288;              // r = ci*9 + t
+                    tile[co][r] = w[((size_t)(co0 + co) * e.cin + ci0) * 9 + r];
+                }
+            }
+            __syncthreads();
+            // eight adjacent K elements per thread = one 16-byte chunk of the swizzled row (chunks are what the swizzle permutes)
+            const PackTile bf = pack_tile(e.cout, e.cin, 9, co0, ci0), bd = pack_tile(e.cin, e.cout, 9, ci0, co0);
+            const bool vec = (reinterpret_cast<uintptr_t>(packed) & 15) == 0;   // operand offsets are multiples of 8
+            if (e.dst_f != kPackNone) {
+                __nv_bfloat16* of = packed + e.dst_f;
+                for (int i = threadIdx.x; i < 32 * 36; i += 256) {    // fprop: [co][t][ci]
+                    const int ci = (i & 3) * 8, t = (i >> 2) % 9, co = i / 36;
+                    uint32_t q[4];
+#pragma unroll
+                    for (int e2 = 0; e2 < 4; ++e2) {
+                        const __nv_bfloat162 v2 = __floats2bfloat162_rn(tile[co][(ci + 2 * e2) * 9 + t], tile[co][(ci + 2 * e2 + 1) * 9 + t]);
+                        q[e2] = *reinterpret_cast<const uint32_t*>(&v2);
+                    }
+                    store_chunk(of + pack_tile_index(bf, t, co, ci), q, vec);
+                }
+            }
+            if (e.dst_d != kPackNone) {
+                __nv_bfloat16* od = packed + e.dst_d;
+                for (int i = threadIdx.x; i < 32 * 36; i += 256) {    // dgrad: [ci][8-t][co]
+                    const int co = (i & 3) * 8, t = (i >> 2) % 9, ci = i / 36;
+                    uint32_t q[4];
+#pragma unroll
+                    for (int e2 = 0; e2 < 4; ++e2) {
+                        const __nv_bfloat162 v2 = __floats2bfloat162_rn(tile[co + 2 * e2][ci * 9 + t], tile[co + 2 * e2 + 1][ci * 9 + t]);
+                        q[e2] = *reinterpret_cast<const uint32_t*>(&v2);
+                    }
+                    store_chunk(od + pack_tile_index(bd, 8 - t, ci, co), q, vec);
+                }
+            }
+        }
+    } else {                              // deconv wt[ci][co][s]
+        const int ct = (e.cout + 31) / 32;
+        {
+            const int ci0 = (tl / ct) * 32, co0 = (tl % ct) * 32;
+            // the last co tile is partial when cout % 32 != 0 (PACK_DECONV_FPROP takes cout % 8 == 0)
+            const int nco = e.cout - co0 < 32 ? e.cout - co0 : 32;
+            for (int i = threadIdx.x; i < 32 * 128; i += 256) {
+                const int ci = i / 128, r = i - ci * 128;              // r = co*4 + s
+                if (r < 4 * nco) tile[ci][r] = w[((size_t)(ci0 + ci) * e.cout + co0) * 4 + r];
+            }
+            __syncthreads();
+            // rows sp*cout + co0 .. + nco stay inside one block: a block holds all 4*cout rows, or 256 with cout % 64 == 0
+            if (e.dst_f != kPackNone) {
+                __nv_bfloat16* of = packed + e.dst_f;
+#pragma unroll
+                for (int sp = 0; sp < 4; ++sp) {                       // fprop: [(s*cout + co)][ci]
+                    const PackTile bf = pack_tile(4 * e.cout, e.cin, 1, sp * e.cout + co0, ci0);
+                    for (int i = threadIdx.x; i < 32 * 32; i += 256) {
+                        const int ci = i & 31, co = i >> 5;
+                        if (co < nco) of[pack_tile_index(bf, 0, co, ci)] = __float2bfloat16_rn(tile[ci][co * 4 + sp]);
+                    }
+                }
+            }
+            if (e.dst_d != kPackNone) {
+                __nv_bfloat16* od = packed + e.dst_d;
+                const PackTile bd = pack_tile(e.cin, e.cout, 4, ci0, co0);
+                for (int i = threadIdx.x; i < 32 * 128; i += 256) {   // dgrad: [ci][s][co]
+                    const int co = i & 31, sp = (i >> 5) & 3, ci = i >> 7;
+                    if (co < nco) od[pack_tile_index(bd, sp, ci, co)] = __float2bfloat16_rn(tile[ci][co * 4 + sp]);
+                }
+            }
+        }
     }
 }
 
-int launch_pack_weights(eld_ctx* ctx, const float* w, void* out, int cout, int cin, int kind, cudaStream_t st)
+int launch_pack(eld_ctx* ctx, const float* params, void* packed, const PackTable& T, bool first_layer, cudaStream_t st)
 {
-    const size_t total = (size_t)cout * cin * ((kind == PACK_CONV_FPROP || kind == PACK_CONV_DGRAD) ? 9 : 4);
-    int blocks = (int)((total + 255) / 256);
-    if (blocks > 4 * ctx->num_sms) blocks = 4 * ctx->num_sms;
-    pack_weights_kernel<<<blocks, 256, 0, st>>>(w, static_cast<__nv_bfloat16*>(out), cout, cin, kind);
+    pack_weights_kernel<<<T.tile0[T.n] + (first_layer ? 2 : 0), 256, 0, st>>>(params, static_cast<__nv_bfloat16*>(packed), T);
     ELD_CHECK_CUDA(cudaGetLastError());
     count_launch(ctx);
     return ELD_OK;
@@ -447,7 +530,13 @@ extern "C" int eld_pack_weights(eld_ctx* ctx, const float* w, void* packed, int 
                 "eld_pack_weights: cout=%d, cin=%d (kind %d) gives %d operand rows; above 256 they must be a multiple of 256",
                 cout, cin, kind, rows);
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
-    return launch_pack_weights(ctx, w, packed, cout, cin, kind, static_cast<cudaStream_t>(stream));
+    const bool deconv = kind == PACK_DECONV_FPROP || kind == PACK_DECONV_DGRAD;
+    const bool fprop = kind == PACK_CONV_FPROP || kind == PACK_DECONV_FPROP;
+    PackTable T{};
+    T.e[0] = PackEntry{ 0, fprop ? 0 : kPackNone, fprop ? kPackNone : 0, cout, cin, deconv, 0 };
+    T.tile0[1] = (cout + 31) / 32 * (cin / 32);
+    T.n = 1;
+    return launch_pack(ctx, w, packed, T, false, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int eld_conv3x3_bf16(eld_ctx* ctx, const void* x, int x_pitch, int x_c0, int cin, const void* w_packed,

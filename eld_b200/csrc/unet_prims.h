@@ -11,22 +11,61 @@ enum { ACT_NONE = 0, ACT_LRELU = 1, ACT_MASK = 2 };
 enum { WG_CONV = 0, WG_DECONV = 1 };
 enum { PACK_CONV_FPROP = 0, PACK_CONV_DGRAD = 1, PACK_DECONV_FPROP = 2, PACK_DECONV_DGRAD = 3 };
 
-// Element index of logical B[n][tap][c] (n < rows, c < ck) inside the packed weight operand.
-// The operand is stored as the exact shared-memory IMAGE the conv tile consumes: contiguous blocks
-// [n_tile_idx][tap][channel chunk], each block = n_tile rows of kc channels (64 B / 128 B per row) with the
-// wgmma/TMA 64B / 128B swizzle already applied - so a whole block is
+// The packed weight operand of logical B[n][tap][c] (n < rows, c < ck) is stored as the exact shared-memory IMAGE the
+// conv tile consumes: contiguous blocks [n_tile_idx][tap][channel chunk], each block = n_tile rows of kc channels
+// (64 B / 128 B per row) with the wgmma/TMA 64B / 128B swizzle already applied - so a whole block is
 // ONE linear cp.async.bulk instead of n_tile TMA tensor rows.
-__host__ __device__ inline size_t packed_index(int rows, int ck, int taps, int n, int tap, int c)
+// PackTile holds what is uniform over the rows n0.. and K channels c0.. of one n_tile block and one channel chunk;
+// pack_tile_index gives the element index of B[n0 + dn][tap][c0 + dc] for the dn, dc that stay inside them.
+struct PackTile { size_t base0, tap_stride; int r0, cc0, kc; };
+__host__ __device__ __forceinline__ PackTile pack_tile(int rows, int ck, int taps, int n0, int c0)
 {
     const int n_tile = rows <= 256 ? rows : 256;
     const int kc = (ck % 64 == 0) ? 64 : 32;
-    const int kchunks = ck / kc, rb = kc * 2;
-    const int nt = n / n_tile, r = n - nt * n_tile;
-    const int chunk = c / kc, cc = c - chunk * kc;
-    const size_t block = ((size_t)nt * taps + tap) * kchunks + chunk;
+    const int kchunks = ck / kc;
+    const int nt = n0 / n_tile, chunk = c0 / kc;
+    PackTile b;
+    b.tap_stride = (size_t)kchunks * n_tile * kc;
+    b.base0 = ((size_t)nt * taps * kchunks + chunk) * ((size_t)n_tile * kc);
+    b.r0 = n0 - nt * n_tile; b.cc0 = c0 - chunk * kc; b.kc = kc;
+    return b;
+}
+__host__ __device__ __forceinline__ size_t pack_tile_index(const PackTile& b, int tap, int dn, int dc)
+{
+    const int r = b.r0 + dn, cc = b.cc0 + dc, rb = b.kc * 2;
     const int swz = rb == 128 ? (r & 7) : ((r >> 1) & 3);
     const int byte = r * rb + ((((cc * 2) >> 4) ^ swz) << 4) + ((cc * 2) & 15);
-    return block * ((size_t)n_tile * kc) + (size_t)(byte >> 1);
+    return b.base0 + (size_t)tap * b.tap_stride + (size_t)(byte >> 1);
+}
+// element index of B[n][tap][c] in the packed operand
+__host__ __device__ inline size_t packed_index(int rows, int ck, int taps, int n, int tap, int c)
+{
+    return pack_tile_index(pack_tile(rows, ck, taps, n, c), tap, 0, 0);
+}
+
+// One layer in a packing launch (launch_pack): its fp32 master weights at params + src (PyTorch layout: Conv2d OIHW
+// [cout][cin][3][3], ConvTranspose2d IOHW [cin][cout][2][2]) and its bf16 fprop / dgrad operands at packed + dst_f /
+// packed + dst_d (PACK_CONV_* or PACK_DECONV_*); kPackNone for an operand the launch does not write.
+// perm: the U-Net engine's gradient permute moves this layer's weight-gradient tiles (the layer's weight trains).
+constexpr unsigned long long kPackNone = ~0ull;
+struct PackEntry { unsigned long long src, dst_f, dst_d; int cout, cin, deconv; int perm; };
+constexpr int kPackMaxEntries = 23;   // the U-Net's layers
+struct PackTable {
+    PackEntry e[kPackMaxEntries];
+    int tile0[kPackMaxEntries + 1];   // prefix sum of (cout/32 x cin/32) tiles per entry, a deconv's last co tile partial
+    int n;
+    // with first_layer: conv1_1's weights at params + first_dst [32][first_cin][3][3] and its image at packed + first_wf
+    unsigned long long first_stage, first_dst, first_wf;
+    int first_cin;
+};
+
+// flattened tile id -> (entry, tile inside the entry)
+__device__ __forceinline__ int find_entry(const PackTable& T, int tile, int& local)
+{
+    int k = 0;
+    while (k + 1 < T.n && tile >= T.tile0[k + 1]) ++k;
+    local = tile - T.tile0[k];
+    return k;
 }
 
 // what a GemmOp computes: a 3x3 conv (fprop or dgrad: 9 taps around each pixel, GEMM N = cout), a 2x2 stride-2 deconv
@@ -81,6 +120,7 @@ int launch_first_conv_wgrad(eld_ctx* ctx, const float* x, int cin, const void* d
 // conv1_1's data gradient: dz bf16 NHWC [n][H][W][32], w f32 OIHW [32][cin][3][3] -> dx f32 NCHW [n][cin][H][W]
 int launch_first_conv_dgrad(eld_ctx* ctx, const void* dz, const float* w, int cin, float* dx, int n, int H, int W,
                             cudaStream_t st);
-int launch_pack_weights(eld_ctx* ctx, const float* w, void* out, int cout, int cin, int kind, cudaStream_t st);
+// packs the T.n entries of T (one block per tile of T.tile0) and, with first_layer, conv1_1's operand image
+int launch_pack(eld_ctx* ctx, const float* params, void* packed, const PackTable& T, bool first_layer, cudaStream_t st);
 
 }  // namespace eld

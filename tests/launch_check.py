@@ -128,12 +128,13 @@ class Step:
     def pack(self):
         from eld_b200 import prims
         from tests.launch_ref import first_layer_image
+        from tests.tile_cases import packed_operand
         self.exact('pack', 'wf:conv1_1', self.bits(self.V('wf:conv1_1').reshape(-1)), self.bits(first_layer_image(self.W('conv1_1'))))
         for layer in FWD:
             deconv = layer.startswith('upv')
             kinds = (prims.PACK_DECONV_FPROP, prims.PACK_DECONV_DGRAD) if deconv else (prims.PACK_CONV_FPROP, prims.PACK_CONV_DGRAD)
             for pre, kind in zip(('wf:', 'wd:'), kinds):
-                want = prims.pack_weights(self.W(layer), kind).reshape(-1)
+                want = packed_operand(self.t, self.W(layer), kind)
                 self.exact('pack', pre + layer, self.bits(self.V(pre + layer).reshape(-1)), self.bits(want))
 
     def fprop(self, layer):

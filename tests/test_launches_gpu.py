@@ -8,8 +8,9 @@ launch read, as the engine stored them in its workspace (eld_unet_buffer).  The 
 tests/launch_check.py's.
 
 Acceptance, one rule per output kind:
-  exact  pooled values (max of the stored values), pool codes, sign words, pack_all vs eld_pack_weights, the OIHW
-         gradients vs the permuted [tap][ci][co] staging, untouched sentinels: bit for bit.
+  exact  pooled values (max of the stored values), pool codes, sign words, the packed operands vs the Python
+         restatement of their layout (tests/tile_cases.py pack_order) and conv1_1's image, the OIHW gradients vs the
+         permuted [tap][ci][co] staging, untouched sentinels: bit for bit.
   bf16   activations, dz, dcat, dp, pool backward: every element |got - r| <= ulp_bf16(r) + 2^-20 S (r = the float64 value
          before the kernel's single rounding, S = the same sum over |terms|), and at most MISMATCH of the elements differ
          from round-to-nearest-even(r).  A wrong tap, channel, swizzle phase, stale tile or dropped K slice moves

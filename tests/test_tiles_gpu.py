@@ -87,24 +87,46 @@ def test_thin_tile_equals_generic_tile_bitwise(torch, case):
     assert diff == 0, '%s: %d of %d elements differ' % (case, diff, a.numel())
 
 
+# (64, 96) and (128, 256) span several 32-channel tiles on both sides in every kind; the deconv fprop kind takes
+# cout % 8 == 0, and cout 8, 16 and 40 end in a partial co tile
 PACK_SHAPES = [(k, co, ci) for k in range(4) for (co, ci) in [(32, 32), (64, 96), (96, 64), (256, 160), (512, 64),
                                                                (64, 512), (128, 256)]
-               if T.pack_accepts(k, co, ci)]
+               if T.pack_accepts(k, co, ci)] + [(2, 8, 32), (2, 16, 96), (2, 40, 64)]
+
+
+def _pack_weights(torch, kind, cout, cin):
+    g = torch.Generator(device='cuda').manual_seed(3)
+    return torch.randn(*((cout, cin, 3, 3) if kind < 2 else (cin, cout, 2, 2)), device='cuda', generator=g)
 
 
 @pytest.mark.parametrize('shape', PACK_SHAPES, ids=lambda s: 'kind%d-%dx%d' % s)
 def test_pack_weights_matches_packed_index(torch, shape):
     """eld_pack_weights against the Python restatement of packed_index, bit for bit"""
     from eld_b200 import prims
-    kind, cout, cin = shape
-    g = torch.Generator(device='cuda').manual_seed(3)
-    W = torch.randn(*((cout, cin, 3, 3) if kind < 2 else (cin, cout, 2, 2)), device='cuda', generator=g)
-    got = C.prims_traced(torch, lambda: prims.pack_weights(W, kind), {'pack_weights_kernel': 1}, 'kind%d-%dx%d' % shape)
-    got = got.reshape(-1)
-    src, dst = T.pack_order(kind, cout, cin)
-    want = torch.empty_like(got)
-    want[torch.from_numpy(dst).cuda()] = W.reshape(-1)[torch.from_numpy(src).cuda()].bfloat16()
-    assert torch.equal(got.view(torch.int16), want.view(torch.int16))
+    W = _pack_weights(torch, *shape)
+    got = C.prims_traced(torch, lambda: prims.pack_weights(W, shape[0]), {'pack_weights_kernel': 1}, 'kind%d-%dx%d' % shape)
+    want = T.packed_operand(torch, W, shape[0])
+    assert torch.equal(got.reshape(-1).view(torch.int16), want.view(torch.int16))
+
+
+@pytest.mark.parametrize('kind', range(4), ids=lambda k: 'kind%d' % k)
+def test_pack_weights_from_and_into_unaligned_buffers(torch, kind):
+    """w one float and the operand one bf16 past a 16-byte boundary (element-wise loads and stores): the same bits,
+    and the guard elements on both sides of the operand unchanged"""
+    from eld_b200 import _lib, prims
+    cout, cin = 64, 96
+    W = _pack_weights(torch, kind, cout, cin)
+    w = torch.empty(W.numel() + 1, device='cuda')
+    w[1:] = W.reshape(-1)
+    want = T.packed_operand(torch, W, kind)
+    buf = torch.full((want.numel() + 2,), NAN16, dtype=torch.int16, device='cuda')
+    lib = _lib.load()
+    rc = H.traced(torch, lambda: lib.eld_pack_weights(_lib.ctx(0), w[1:].data_ptr(), buf[1:].data_ptr(), cout, cin, kind,
+                                                      prims._st()),
+                  {'pack_weights_kernel': 1}, 'kind%d unaligned' % kind, T.canonical)
+    assert rc == 0
+    assert torch.equal(buf[1:-1], want.view(torch.int16))
+    assert buf[0].item() == NAN16 and buf[-1].item() == NAN16
 
 
 @pytest.mark.parametrize('op', ['conv', 'conv.dgrad'])

@@ -139,7 +139,7 @@ def packed_index(rows, ck, taps, n, tap, c):
 def pack_order(kind, cout, cin):
     """-> (flat index into the fp32 source tensor, index into the packed operand), one pair per weight"""
     rows, ck, taps = pack_geometry(kind, cout, cin)
-    n, tap, c = np.meshgrid(np.arange(rows), np.arange(taps), np.arange(ck), indexing='ij')
+    n, tap, c = np.ix_(np.arange(rows), np.arange(taps), np.arange(ck))
     if kind == 0:       # B[co][t][ci] = W[co][ci][t]
         src = (n * cin + c) * 9 + tap
     elif kind == 1:     # B[ci][t][co] = W[co][ci][8 - t]
@@ -148,7 +148,18 @@ def pack_order(kind, cout, cin):
         src = (c * cout + n % cout) * 4 + n // cout
     else:               # B[ci][s][co] = Wt[ci][co][s]
         src = (n * cout + c) * 4 + tap
-    return src.reshape(-1), packed_index(rows, ck, taps, n, tap, c).reshape(-1)
+    dst = packed_index(rows, ck, taps, n, tap, c)
+    return tuple(np.broadcast_to(v, (rows, taps, ck)).flatten() for v in (src, dst))
+
+
+def packed_operand(torch, W, kind):
+    """the bf16 operand pack_order builds from fp32 weights W (OIHW for the conv kinds, IOHW for the deconv kinds),
+    flat, on W's device"""
+    cout, cin = (W.shape[0], W.shape[1]) if kind < 2 else (W.shape[1], W.shape[0])
+    src, dst = (torch.from_numpy(v).to(W.device) for v in pack_order(kind, cout, cin))
+    out = torch.empty(dst.numel(), dtype=torch.bfloat16, device=W.device)
+    out[dst] = W.reshape(-1)[src].bfloat16()
+    return out
 
 
 # ---- the case table ------------------------------------------------------------------------------------------------
