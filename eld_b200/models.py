@@ -6,6 +6,8 @@ Differences that are the point of this repo
   * netG is eld_b200.arch.unet (wgmma engine); forward+L1+backward is ONE C-ABI call, Adam another;
   * noise can be synthesised ON THE TRAINING STREAM (opt.noise_on_gpu / a batch without 'input'):
     only the clean frame crosses PCIe, the fused CUDA kernel makes the noisy input (SURVEY F4);
+  * stored (input, target) pairs can be decoded ON THE TRAINING STREAM (opt.pairs_on_gpu): uint16 pairs cross PCIe
+    as stored and one kernel de-quantises, augments and clips them (eld_b200.datasets);
   * data parallel: if torch.distributed is initialised the flat gradient buffer is all-reduced
     (NCCL over NVLink) between backward and Adam - one collective, U-Net weights only;
   * get_current_errors() keeps the reference's `.item()` host sync but can be told to defer it.
@@ -27,7 +29,7 @@ def default_opt(**kw):
              resume_epoch=None, seed=2018, chop=False, no_log=True, no_verbose=True, netG='unet', channels=4,
              stage_in='raw', stage_out='raw', model_path=None, include=4, crf=False, batchSize=1, lr=1e-4,
              beta1=0.9, wd=0.0, loss='l1', noise='g', isTrain=True, save_epoch_freq=100, noise_on_gpu=False,
-             augment_on_gpu=False, defer_loss_sync=False, prefetch_noise=False, num_burst=1)
+             augment_on_gpu=False, defer_loss_sync=False, prefetch_noise=False, num_burst=1, pairs_on_gpu=False)
     o.update(kw)
     return SimpleNamespace(**o)
 
@@ -103,6 +105,9 @@ class ELDModel(BaseModel):
         BaseModel.initialize(self, opt)
         if self.device is None:
             raise RuntimeError('ELDModel (eld_b200) needs a CUDA device: no CPU fallback')
+        if getattr(opt, 'pairs_on_gpu', False) and getattr(opt, 'noise_on_gpu', False):
+            raise ValueError('pairs_on_gpu trains from stored (input, target) pairs, noise_on_gpu synthesises the input: '
+                             'set one of them')
         if len(opt.gpu_ids) > 0:
             self.device = torch.device('cuda', opt.gpu_ids[0])
         if getattr(opt, 'crf', False) and getattr(self, 'CRF', None) is None:
@@ -148,11 +153,14 @@ class ELDModel(BaseModel):
             input, data_name = data['input'], data['fn']
         else:
             raise NotImplementedError('Mode [%s] is not implemented' % mode)
-        synth = mode == 'train' and (input is None or getattr(self.opt, 'noise_on_gpu', False))
+        pairs = mode == 'train' and input is not None and getattr(self.opt, 'pairs_on_gpu', False)
+        synth = mode == 'train' and not pairs and (input is None or getattr(self.opt, 'noise_on_gpu', False))
         pre = self._prefetched if synth else None
-        if target is not None and not (pre is not None and pre[0] is data):
+        if target is not None and not pairs and not (pre is not None and pre[0] is data):
             target = target.to(device=self.device, dtype=torch.float32, non_blocking=True)
-        if synth:
+        if pairs:
+            input, target = self._ingest_pairs(input, target)
+        elif synth:
             self._prefetched = None
             if pre is not None and pre[0] is data:
                 # made ahead by prefetch_input() on the side stream while the previous step's network ran
@@ -183,8 +191,7 @@ class ELDModel(BaseModel):
         (a resumed run does not replay the Philox streams from frame 0)."""
         assert self.noise_maker is not None, 'noise_on_gpu needs a noise_maker (eld_b200.noise.NoiseModel)'
         n = target.shape[0]
-        fid0 = self._frames_seen + self.rank * n
-        self._frames_seen += self.world * n
+        fid0 = self._take_frame_ids(n)
         # per-frame (K, g_scale, ratio, ...) and flip flags are drawn from a generator keyed by (seed, global frame id):
         # W ranks draw W*n DIFFERENT tuples (not W copies of the same n), and frame f gets the same tuple at any GPU
         # count.  The draw itself is noise.py:201-225's call order on that per-frame RandomState.
@@ -195,6 +202,27 @@ class ELDModel(BaseModel):
             return self.noise_maker.batch_gpu_augmented(target, aug=self.noise_maker.frame_augment(fid0, n),
                                                         params=params, frame_id0=fid0, clip=True)
         return self.noise_maker.batch_gpu(target, params=params, frame_id0=fid0, clip=True), target
+
+    def _take_frame_ids(self, n):
+        """the global id of this rank's first frame of the step; advances the running count by the whole step"""
+        fid0 = self._frames_seen + self.rank * n
+        self._frames_seen += self.world * n
+        return fid0
+
+    def _ingest_pairs(self, input, target):
+        """ELDTrainDataset.__getitem__ (sid_dataset.py:337-356) over LMDBDataset (lmdb_dataset.py:28-41) for a batch
+        of stored pairs (uint16 or float32, as eld_b200.datasets hands them out): both tensors cross PCIe as stored and
+        one eld_pair_ingest launch on the current stream de-quantises, flips / transposes and clips them.  The flags
+        of a frame are drawn from (opt.seed, its global frame id), counted as in _synthesize, so the data does not
+        depend on the GPU count and a resumed run continues the stream.  sRGB databases are already rendered: no ISP."""
+        from . import datasets
+        from .noise import augment_flags
+        n = input.shape[0]
+        fid0 = self._take_frame_ids(n)
+        flags = augment_flags(self.opt.seed, fid0, n) if getattr(self.opt, 'augment_on_gpu', False) else None
+        input, target = ((t.view(torch.int16) if t.dtype == torch.uint16 else t).to(device=self.device, non_blocking=True)
+                         for t in (input, target))
+        return datasets.ingest(input, target, flags)
 
     def prefetch_input(self, data):
         """Start synthesising the NEXT step's noisy input on a side stream (Engine.train calls this right after it has

@@ -78,6 +78,25 @@ def _cur_stream(torch):
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def frame_rng(seed, fid):
+    """the RandomState of global frame `fid` under `seed`: the same frame draws the same values whatever the GPU count"""
+    return np.random.RandomState(np.random.SeedSequence([int(seed) & 0xFFFFFFFF, int(seed) >> 32,
+                                                         int(fid) & 0xFFFFFFFF, int(fid) >> 32]).generate_state(4))
+
+
+def augment_flags(seed, fid0, n):
+    """ELDTrainDataset's three coin flips (sid_dataset.py:344-350), in its order, for global frames fid0 .. fid0+n-1:
+    uint8 [n], bit 0 flip rows, bit 1 flip columns, bit 2 transpose.  Each frame draws from its own RandomState keyed
+    by (seed, frame id), in a domain apart from the frame's noise parameters."""
+    flags = np.zeros(n, dtype=np.uint8)
+    for i in range(n):
+        rng = frame_rng(seed, (fid0 + i) ^ (1 << 62))
+        for bit in (1, 2, 4):
+            if rng.randint(2, size=1)[0] == 1:
+                flags[i] |= bit
+    return flags
+
+
 class NoiseModelBase:
     model = 'g'
     seed = 0
@@ -96,8 +115,7 @@ class NoiseModelBase:
 
     # ---- per-frame draws keyed by (seed, global frame id): invariant to how frames are sharded over GPUs ----------
     def _frame_rng(self, fid):
-        return np.random.RandomState(np.random.SeedSequence([int(self.seed) & 0xFFFFFFFF, int(self.seed) >> 32,
-                                                             int(fid) & 0xFFFFFFFF, int(fid) >> 32]).generate_state(4))
+        return frame_rng(self.seed, fid)
 
     def frame_params(self, fid0, n, burst=1):
         """_sample_params (noise.py:201-225, same call order and distributions) for global frames fid0 .. fid0+n-1, each
@@ -109,13 +127,7 @@ class NoiseModelBase:
 
     def frame_augment(self, fid0, n):
         """ELDTrainDataset's three coin flips (sid_dataset.py:344-350) per global frame id, same order."""
-        flags = np.zeros(n, dtype=np.uint8)
-        for i in range(n):
-            rng = self._frame_rng((fid0 + i) ^ (1 << 62))
-            for bit in (1, 2, 4):
-                if rng.randint(2, size=1)[0] == 1:
-                    flags[i] |= bit
-        return flags
+        return augment_flags(self.seed, fid0, n)
 
     def _sample_params_any(self, rng=None):
         if _lib.is_full_model(self.model):

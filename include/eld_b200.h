@@ -119,6 +119,27 @@ int eld_noise_packed_aug(eld_ctx* ctx, const float* clean, float* noisy, float* 
                          int clip01, const uint8_t* aug_flags, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Paired training frames: the per-pixel work of ELDTrainDataset.__getitem__ (dataset/sid_dataset.py:337-356) over
+ * LMDBDataset.__getitem__ (dataset/lmdb_dataset.py:28-41), the path of train_real.py:44-58 and of train_syn.py:66-70's
+ * offline-noise database, for a batch of n frames in one launch:
+ *   input_out[f]  = clip(aug_f(deq(input[f])))      input  [n][cin][h][w],  input_out  f32 [n][cin][h][w]
+ *   target_out[f] = aug_f(deq(target[f]))           target [n][cout][h][w], target_out f32 [n][cout][h][w]
+ *   deq   ELD_DT_U16: v / 65535 as a correctly rounded float division (lmdb_dataset.py:38-39: the float64 quotient
+ *         rounded to float is the same number for every code; the clip to [0, 1] changes nothing);
+ *         ELD_DT_F32: identity, NaN and -0.0 included (LMDBDataset does not clip float databases).
+ *   aug_f the coin flips of sid_dataset.py:344-352 in their order: bit 0 (ELD_AUG_FLIP_H) flips rows (np.flip axis 1),
+ *         bit 1 (ELD_AUG_FLIP_W) columns (axis 2), bit 2 (ELD_AUG_TRANSPOSE) transposes (0, 2, 1); aug_flags is a HOST
+ *         array of n bytes copied into the launch (no device sync), NULL for no augmentation.
+ *   clip  np.maximum(np.minimum(x, 1), 0) (sid_dataset.py:354): NaN stays NaN, -0.0 becomes +0.0, +Inf 1, -Inf 0.
+ * cin, cout: 3 (sRGB databases) or 4 (raw); the two dtypes are independent.  Any element offset; partial tiles masked.
+ * ELD_E_ARG, nothing written and nothing launched: a NULL ctx or buffer, a negative size, a channel count other than 3
+ * or 4, a dtype other than ELD_DT_U16 / ELD_DT_F32, a flag byte with bits above 2, a transpose flag with h != w, flags
+ * for more than 2048 frames (the table the launch carries), either output overlapping either input or the other output.
+ * n, h or w == 0: ELD_OK, nothing launched. */
+int eld_pair_ingest(eld_ctx* ctx, const void* input, int in_dtype, int cin, const void* target, int tgt_dtype, int cout,
+                    float* input_out, float* target_out, int n, int h, int w, const uint8_t* aug_flags, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Raw -> sRGB rendering of the `--stage_in srgb` branch (train_syn.py:55-58): replaces util/process.py:51-68
  * `process` - apply_gains (:15-19), clip, binning RGBG->RGB (:41-48), apply_ccms (:22-31), clip,
  * gamma_compression (:34-39) or camera_response_function (:71-84) with its 8-bit quantisation - and the clips of
