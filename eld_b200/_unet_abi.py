@@ -45,6 +45,9 @@ def declare_engine(lib):
     lib.eld_unet_set_trainable.argtypes = [vp, c.POINTER(c.c_uint8), i32, i32]
     lib.eld_adam_step_segments.argtypes = [vp, vp, vp, vp, vp, c.POINTER(sz), c.POINTER(i32), i32, f32, f32, f32, f32, f32,
                                            f32, vp]
+    lib.eld_adam_step_capturable.argtypes = [vp, vp, vp, vp, vp, sz, vp, vp, f32, f32, f32, f32, f32, vp]
+    lib.eld_adam_step_segments_capturable.argtypes = [vp, vp, vp, vp, vp, c.POINTER(sz), c.POINTER(vp), i32, vp, f32, f32,
+                                                      f32, f32, f32, vp]
     lib.eld_unet_set_loss.argtypes = [vp, i32]
     lib.eld_clock_probe.argtypes = [vp, vp, vp]
     lib.eld_unet_profile.argtypes = [vp, i32]

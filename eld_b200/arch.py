@@ -374,7 +374,16 @@ class UNetSeeInDark(nn.Module):
             wk.wait()
         self._pending_allreduce = []
 
+    _profiling = False    # inside _profile: the engine records per-launch events (ELDModel refuses to capture a step then)
+
     def _profile(self, eng, run, steps):
+        try:
+            self._profiling = True
+            return self._profile_on(eng, run, steps)
+        finally:
+            self._profiling = False
+
+    def _profile_on(self, eng, run, steps):
         import numpy as np
         lib = _lib.load()
         run()
@@ -419,15 +428,50 @@ class FusedAdam(torch.optim.Optimizer):
     """torch.optim.Adam semantics (ELD_model.py:400-401) as ONE kernel over the flat buffers.
     Keeps `param_groups` so Engine.set_learning_rate / util.set_opt_param keep working.  Frozen parameters
     (requires_grad == False) are skipped: the trainable runs of the buffer go to eld_adam_step_segments, each with the
-    per-parameter step count torch keeps in state['step']."""
+    per-parameter step count torch keeps in state['step'].
+    capturable=True (torch.optim.Adam's option of that name): the step counts and the learning rate live in device memory
+    and the kernels read them when they run (eld_adam_step_segments_capturable), so a CUDA graph that captured step()
+    stays right on every replay.  Before each replay, graph_step() does the host half of a step: param_groups[0]['lr']
+    into device memory (outside the graph) and the parameters' version bump."""
 
-    def __init__(self, net, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
+    def __init__(self, net, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, capturable=False):
         super().__init__(list(net.parameters()), dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
         self.net = net
         self.m = torch.zeros_like(net.flat_params)
         self.v = torch.zeros_like(net.flat_params)
         self.t = 0                                     # step() calls
-        self.steps = [0] * len(net._spans)             # Adam steps taken by each parameter (torch's state['step'])
+        self.capturable = capturable
+        if capturable:
+            dev = net.flat_params.device
+            self.step_dev = torch.zeros(len(net._spans), dtype=torch.int32, device=dev)   # state['step'] per parameter
+            self.lr_dev = torch.zeros(1, dtype=torch.float32, device=dev)
+            self._lr_sent = None                       # the lr last written to lr_dev
+        else:
+            self.steps = [0] * len(net._spans)         # Adam steps taken by each parameter (torch's state['step'])
+
+    def _params_stepped(self, flags):
+        # the kernels write the flat buffer behind autograd's back: mark the parameters modified in place, so that a
+        # retained graph that saved them raises torch's usual error instead of back-propagating through new weights
+        torch.autograd.graph.increment_version([q for q, f in zip(self.net.parameters(), flags) if f])
+
+    def _send_lr(self):
+        """param_groups[0]['lr'] into lr_dev (a fill launch, no host synchronisation) when it changed"""
+        lr = float(self.param_groups[0]['lr'])
+        if lr != self._lr_sent:
+            self.lr_dev.fill_(lr)
+            self._lr_sent = lr
+
+    def graph_step(self):
+        """the host half of a capturable step whose kernels a CUDA graph replays: the learning rate into device memory
+        (call it before the replay), the parameter versions bumped"""
+        assert self.capturable
+        self.t += 1
+        self._send_lr()
+        self._params_stepped([q.requires_grad for q in self.net.parameters()])
+
+    def host_steps(self):
+        """Adam steps taken by each parameter, in state_dict order (reads the device counters when capturable)"""
+        return [int(s) for s in self.step_dev.tolist()] if self.capturable else list(self.steps)
 
     @torch.no_grad()
     def step(self, closure=None, grad_scale=1.0):
@@ -440,17 +484,33 @@ class FusedAdam(torch.optim.Optimizer):
         self.t += 1
         params = list(self.net.parameters())
         flags = [q.requires_grad for q in params]
-        for i, f in enumerate(flags):
-            self.steps[i] += 1 if f else 0
-        # the kernels write the flat buffer behind autograd's back: mark the parameters modified in place, so that a
-        # retained graph that saved them raises torch's usual error instead of back-propagating through new weights
-        torch.autograd.graph.increment_version([q for q, f in zip(params, flags) if f])
-        uniform = all(flags) and len(set(self.steps)) == 1
+        if self.capturable:
+            if not torch.cuda.is_current_stream_capturing():
+                self._send_lr()                        # a capture reads lr_dev as graph_step leaves it before each replay
+        else:
+            for i, f in enumerate(flags):
+                self.steps[i] += 1 if f else 0
+        self._params_stepped(flags)
+        uniform = not self.capturable and all(flags) and len(set(self.steps)) == 1
         p = self.net.flat_params
         hp = (float(g['lr']), float(g['betas'][0]), float(g['betas'][1]), float(g['eps']), float(g['weight_decay']))
 
         def adam(lo, hi):
             lib, dev = _lib.load(), _lib.ctx(p.device.index or 0)
+            if self.capturable:                        # one range per trainable parameter, each with its own counter
+                segs, ctrs = [], []
+                for i, ((off, n), f) in enumerate(zip(self.net._spans, flags)):
+                    if f and lo <= off and off + n <= hi:
+                        segs += [off, n]
+                        ctrs.append(self.step_dev.data_ptr() + 4 * i)
+                    assert not (f and lo < off + n and off < hi and not (lo <= off and off + n <= hi)), \
+                        'a capturable step range must hold whole parameters'
+                k = len(ctrs)
+                _lib.check(lib.eld_adam_step_segments_capturable(
+                    dev, p.data_ptr(), self.net.flat_grads.data_ptr(), self.m.data_ptr(), self.v.data_ptr(),
+                    (ctypes.c_size_t * (2 * k))(*segs), (ctypes.c_void_p * k)(*ctrs), k, self.lr_dev.data_ptr(), *hp[1:],
+                    float(grad_scale), _st()), 'eld_adam_step_segments_capturable')
+                return
             if uniform:                                # one range, one step count
                 _lib.check(lib.eld_adam_step(dev, p.data_ptr() + 4 * lo, self.net.flat_grads.data_ptr() + 4 * lo,
                                              self.m.data_ptr() + 4 * lo, self.v.data_ptr() + 4 * lo, hi - lo, *hp,
@@ -494,31 +554,37 @@ class FusedAdam(torch.optim.Optimizer):
         self.net.flat_grads.zero_()
 
     # checkpoint format of torch.optim.Adam ('opt_g' in ELD_model.py:516-523): per-parameter step; a parameter that has
-    # never taken a step has no state entry
+    # never taken a step has no state entry.  Capturable: 'step' is a float32 tensor on the parameter's device, as torch's
+    # capturable Adam stores it.
     def state_dict(self):
         state = {}
         params = list(self.net.parameters())
-        for i, (p, (off, n), s) in enumerate(zip(params, self.net._spans, self.steps)):
+        for i, (p, (off, n), s) in enumerate(zip(params, self.net._spans, self.host_steps())):
             if s == 0:
                 continue
-            state[i] = {'step': torch.tensor(float(s)), 'exp_avg': self.m[off:off + n].view(p.shape).clone(),
+            step = torch.tensor(float(s), device=p.device) if self.capturable else torch.tensor(float(s))
+            state[i] = {'step': step, 'exp_avg': self.m[off:off + n].view(p.shape).clone(),
                         'exp_avg_sq': self.v[off:off + n].view(p.shape).clone()}
         groups = [dict((k, v) for k, v in self.param_groups[0].items() if k != 'params')]
         groups[0]['params'] = list(range(len(params)))
         return {'state': state, 'param_groups': groups}
 
     def load_state_dict(self, sd):
+        steps = [0] * len(self.net._spans)
         for i, (off, n) in enumerate(self.net._spans):
             st = sd['state'].get(i)
             if st is not None:
                 self.m[off:off + n].copy_(st['exp_avg'].reshape(-1))
                 self.v[off:off + n].copy_(st['exp_avg_sq'].reshape(-1))
-                self.steps[i] = int(float(st['step']))
+                steps[i] = int(float(st['step']))
             else:
                 self.m[off:off + n].zero_()
                 self.v[off:off + n].zero_()
-                self.steps[i] = 0
-        self.t = max(self.steps)
+        if self.capturable:
+            self.step_dev.copy_(torch.tensor(steps, dtype=torch.int32))      # in place: a captured step keeps its address
+        else:
+            self.steps[:] = steps
+        self.t = max(steps)
         for k, v in sd['param_groups'][0].items():
             if k != 'params':
                 self.param_groups[0][k] = v

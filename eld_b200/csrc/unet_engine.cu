@@ -876,6 +876,29 @@ extern "C" int eld_adam_step_segments(eld_ctx* ctx, float* params, const float* 
                                 static_cast<cudaStream_t>(stream));
 }
 
+extern "C" int eld_adam_step_capturable(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, size_t n,
+                                        const float* lr, int* step, float beta1, float beta2, float eps, float weight_decay,
+                                        float grad_scale, void* stream)
+{
+    ELD_REQUIRE(ctx && params && grads && m && v && lr && step, "eld_adam_step_capturable: NULL argument");
+    ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
+    const size_t seg[2] = { 0, n };
+    return launch_adam_dev(ctx, params, grads, m, v, seg, &step, 1, lr, beta1, beta2, eps, weight_decay, grad_scale,
+                           static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int eld_adam_step_segments_capturable(eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
+                                                 const size_t* segs, int* const* steps, int n_segs, const float* lr,
+                                                 float beta1, float beta2, float eps, float weight_decay, float grad_scale,
+                                                 void* stream)
+{
+    ELD_REQUIRE(ctx && params && grads && m && v && lr && (n_segs == 0 || (segs && steps)),
+                "eld_adam_step_segments_capturable: NULL argument");
+    ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
+    return launch_adam_dev(ctx, params, grads, m, v, segs, steps, n_segs, lr, beta1, beta2, eps, weight_decay, grad_scale,
+                           static_cast<cudaStream_t>(stream));
+}
+
 extern "C" int eld_unet_set_loss(eld_unet* u, int kind)
 {
     ELD_REQUIRE(u && (kind == 0 || kind == 1), "eld_unet_set_loss: kind must be 0 (L1) or 1 (MSE)");

@@ -307,6 +307,43 @@ adam_segments_kernel(float* __restrict__ p, const float* __restrict__ g, float* 
     }
 }
 
+// The capturable update: lr and every range's step counter are read from device memory when the kernel runs, so one
+// captured launch is right on every replay.  A counter holds the steps its range has taken; this step is counter + 1.
+// Thread s of each block derives range s's bias corrections into shared memory (the host-side arithmetic of
+// launch_adam_segments, on the device).  The counters are only read here: adam_bump_kernel, the next launch on the
+// stream, increments them once this grid has finished.
+__global__ void __launch_bounds__(256)
+adam_dev_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                const __grid_constant__ AdamSegmentsDev S, const float* __restrict__ lr, float b1, float b2, float eps,
+                float wd, float gscale)
+{
+    __shared__ float bc1[kAdamMaxSegments], bc2_sqrt[kAdamMaxSegments];
+    if (threadIdx.x < S.n) {
+        const float t = (float)(*S.step[threadIdx.x] + 1);
+        bc1[threadIdx.x] = 1.0f - powf(b1, t);
+        bc2_sqrt[threadIdx.x] = sqrtf(1.0f - powf(b2, t));
+    }
+    __syncthreads();
+    const float rate = *lr;
+    const size_t t0 = blockIdx.x * (size_t)blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
+    for (int s = 0; s < S.n; ++s) {
+        const size_t off = S.off[s], end = S.off[s] + S.cnt[s];
+        for (size_t i = off + t0; i < end; i += stride)
+            adam_elem(p, g, m, v, i, rate, b1, b2, eps, wd, bc1[s], bc2_sqrt[s], gscale);
+    }
+}
+
+// One step more on every counter the ranges name; a counter named by several ranges takes one step (thread s skips a
+// counter an earlier range names).
+__global__ void adam_bump_kernel(const __grid_constant__ AdamSegmentsDev S)
+{
+    const int s = threadIdx.x;
+    if (s >= S.n) return;
+    for (int r = 0; r < s; ++r)
+        if (S.step[r] == S.step[s]) return;
+    *S.step[s] += 1;
+}
+
 // ---- launch helpers ---------------------------------------------------------------------------------
 static inline int grid_for(size_t work, int per_block, int cap)
 {
@@ -381,6 +418,24 @@ int launch_adam(eld_ctx* ctx, float* p, const float* g, float* m, float* v, size
     return ELD_OK;
 }
 
+// an element in two ranges would be updated twice, by two threads, without ordering: refuse overlapping ranges
+// (off / cnt: the n_segs ranges as the launchers copied them)
+static int check_disjoint(const unsigned long long* off, const unsigned long long* cnt, int n_segs)
+{
+    int order[kAdamMaxSegments];
+    for (int s = 0; s < n_segs; ++s) order[s] = s;
+    std::sort(order, order + n_segs, [&](int a, int b) { return off[a] < off[b]; });
+    unsigned long long end = 0;
+    for (int k = 0; k < n_segs; ++k) {
+        const int s = order[k];
+        if (cnt[s] == 0) continue;
+        ELD_REQUIRE(off[s] >= end && cnt[s] <= ~0ull - off[s], "adam: segment %d [%llu, +%llu) overlaps another", s,
+                    off[s], cnt[s]);
+        end = off[s] + cnt[s];
+    }
+    return ELD_OK;
+}
+
 int launch_adam_segments(eld_ctx* ctx, float* p, const float* g, float* m, float* v, const size_t* segs, const int* steps,
                          int n_segs, float lr, float b1, float b2, float eps, float wd, float gscale, cudaStream_t st)
 {
@@ -394,21 +449,35 @@ int launch_adam_segments(eld_ctx* ctx, float* p, const float* g, float* m, float
         S.bc2_sqrt[s] = sqrtf(1.0f - powf(b2, (float)steps[s]));
         total += S.cnt[s];
     }
-    // an element in two ranges would be updated twice, by two threads, without ordering: refuse overlapping ranges
-    int order[kAdamMaxSegments];
-    for (int s = 0; s < n_segs; ++s) order[s] = s;
-    std::sort(order, order + n_segs, [&](int a, int b) { return S.off[a] < S.off[b]; });
-    unsigned long long end = 0;
-    for (int k = 0; k < n_segs; ++k) {
-        const int s = order[k];
-        if (S.cnt[s] == 0) continue;
-        ELD_REQUIRE(S.off[s] >= end && S.cnt[s] <= ~0ull - S.off[s], "adam: segment %d [%llu, +%llu) overlaps another", s,
-                    S.off[s], S.cnt[s]);
-        end = S.off[s] + S.cnt[s];
-    }
+    { const int rc = check_disjoint(S.off, S.cnt, n_segs); if (rc != ELD_OK) return rc; }
     S.n = n_segs;
     if (total == 0) return ELD_OK;
     adam_segments_kernel<<<grid_for(total, 256 * 4, 8 * ctx->num_sms), 256, 0, st>>>(p, g, m, v, S, lr, b1, b2, eps, wd, gscale);
+    ELD_CHECK_CUDA(cudaGetLastError());
+    count_launch(ctx);
+    return ELD_OK;
+}
+
+int launch_adam_dev(eld_ctx* ctx, float* p, const float* g, float* m, float* v, const size_t* segs, int* const* steps,
+                    int n_segs, const float* lr, float b1, float b2, float eps, float wd, float gscale, cudaStream_t st)
+{
+    ELD_REQUIRE(n_segs >= 0 && n_segs <= kAdamMaxSegments, "adam: %d segments (at most %d)", n_segs, kAdamMaxSegments);
+    AdamSegmentsDev S{};
+    size_t total = 0;
+    for (int s = 0; s < n_segs; ++s) {
+        ELD_REQUIRE(steps[s], "adam: segment %d: NULL step counter", s);
+        S.off[s] = segs[2 * s]; S.cnt[s] = segs[2 * s + 1]; S.step[s] = steps[s];
+        total += S.cnt[s];
+    }
+    { const int rc = check_disjoint(S.off, S.cnt, n_segs); if (rc != ELD_OK) return rc; }
+    S.n = n_segs;
+    if (n_segs == 0) return ELD_OK;
+    if (total > 0) {
+        adam_dev_kernel<<<grid_for(total, 256 * 4, 8 * ctx->num_sms), 256, 0, st>>>(p, g, m, v, S, lr, b1, b2, eps, wd, gscale);
+        ELD_CHECK_CUDA(cudaGetLastError());
+        count_launch(ctx);
+    }
+    adam_bump_kernel<<<1, kAdamMaxSegments, 0, st>>>(S);
     ELD_CHECK_CUDA(cudaGetLastError());
     count_launch(ctx);
     return ELD_OK;

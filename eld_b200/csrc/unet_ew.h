@@ -19,4 +19,12 @@ struct AdamSegments {
 };
 int launch_adam_segments(eld_ctx* ctx, float* p, const float* g, float* m, float* v, const size_t* segs, const int* steps,
                          int n_segs, float lr, float b1, float b2, float eps, float wd, float gscale, cudaStream_t st);
+// The capturable variants: lr and the step counters live in device memory, each range names its own counter
+struct AdamSegmentsDev {
+    unsigned long long off[kAdamMaxSegments], cnt[kAdamMaxSegments];
+    int* step[kAdamMaxSegments];
+    int n;
+};
+int launch_adam_dev(eld_ctx* ctx, float* p, const float* g, float* m, float* v, const size_t* segs, int* const* steps,
+                    int n_segs, const float* lr, float b1, float b2, float eps, float wd, float gscale, cudaStream_t st);
 }  // namespace eld

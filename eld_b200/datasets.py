@@ -70,18 +70,21 @@ def _dtype_code(torch, t, what):
     raise TypeError('%s: uint16 (or its int16 bit pattern) or float32, not %s' % (what, t.dtype))
 
 
-def ingest(input, target, flags=None):
+def ingest(input, target, flags=None, out=None, target_out=None):
     """input [n, cin, h, w], target [n, cout, h, w] on the GPU, each uint16 (or int16 holding its bits) or float32,
     cin and cout 3 or 4 -> float32 (clip(aug(deq(input))), aug(deq(target))) in one launch on the current stream.
-    flags: None, or uint8 [n] per frame - bit 0 flip rows, bit 1 flip columns, bit 2 transpose (needs h == w)."""
+    flags: None, or uint8 [n] per frame - bit 0 flip rows, bit 1 flip columns, bit 2 transpose (needs h == w).
+    out / target_out: contiguous float32 tensors of input's / target's shape to write into (new ones if None)."""
     import torch
     assert input.is_cuda and target.is_cuda and input.dim() == 4 and target.dim() == 4
     n, cin, h, w = input.shape
     assert target.shape[0] == n and target.shape[2:] == (h, w), (input.shape, target.shape)
     din, dtg = _dtype_code(torch, input, 'input'), _dtype_code(torch, target, 'target')
     input, target = input.contiguous(), target.contiguous()
-    out_in = torch.empty((n, cin, h, w), dtype=torch.float32, device=input.device)
-    out_tg = torch.empty(target.shape, dtype=torch.float32, device=input.device)
+    out_in = torch.empty((n, cin, h, w), dtype=torch.float32, device=input.device) if out is None else out
+    out_tg = torch.empty(target.shape, dtype=torch.float32, device=input.device) if target_out is None else target_out
+    for t, like in ((out_in, input), (out_tg, target)):
+        assert t.is_contiguous() and t.shape == like.shape and t.dtype == torch.float32 and t.device == input.device
     fp = None
     if flags is not None:
         flags = np.ascontiguousarray(flags, dtype=np.uint8)

@@ -10,7 +10,8 @@ Differences that are the point of this repo
     as stored and one kernel de-quantises, augments and clips them (eld_b200.datasets);
   * data parallel: if torch.distributed is initialised the flat gradient buffer is all-reduced
     (NCCL over NVLink) between backward and Adam - one collective, U-Net weights only;
-  * get_current_errors() keeps the reference's `.item()` host sync but can be told to defer it.
+  * get_current_errors() keeps the reference's `.item()` host sync but can be told to defer it;
+  * opt.cuda_graph captures the fused step (train_step + Adam) in a CUDA graph and replays it (ELDModel._graph_step).
 """
 import os
 from collections import OrderedDict
@@ -29,7 +30,8 @@ def default_opt(**kw):
              resume_epoch=None, seed=2018, chop=False, no_log=True, no_verbose=True, netG='unet', channels=4,
              stage_in='raw', stage_out='raw', model_path=None, include=4, crf=False, batchSize=1, lr=1e-4,
              beta1=0.9, wd=0.0, loss='l1', noise='g', isTrain=True, save_epoch_freq=100, noise_on_gpu=False,
-             augment_on_gpu=False, defer_loss_sync=False, prefetch_noise=False, num_burst=1, pairs_on_gpu=False)
+             augment_on_gpu=False, defer_loss_sync=False, prefetch_noise=False, num_burst=1, pairs_on_gpu=False,
+             cuda_graph=False)
     o.update(kw)
     return SimpleNamespace(**o)
 
@@ -94,6 +96,10 @@ class ELDModel(BaseModel):
         self.CRF = None
         self._prefetched = None
         self._noise_stream = None
+        self._graphed = False
+        self._static = None          # (input, target) buffers the captured step reads
+        self._graph = None           # the captured step (_capture)
+        self._eager_left = 0         # eager warm-up steps before the next capture
 
     def _eval(self):
         self.netG.eval()
@@ -120,16 +126,25 @@ class ELDModel(BaseModel):
             raise NotImplementedError('Invalid Output Stage: {}'.format(opt.stage_out))
         self.netG = arch.__dict__[opt.netG](chan[opt.stage_in], chan[opt.stage_out]).to(self.device)     # ELD_model.py:391
         self.noise_maker = noise_maker
+        self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+        self.rank = dist.get_rank() if self.world > 1 else 0
+        self._graphed = bool(getattr(opt, 'cuda_graph', False)) and self.isTrain
+        if self._graphed:
+            if self.world > 1:
+                raise NotImplementedError('cuda_graph: the data-parallel step (NCCL all-reduces) is not captured; '
+                                          'train with world size 1 or without cuda_graph')
+            if getattr(opt, 'prefetch_noise', False):
+                raise NotImplementedError('cuda_graph with prefetch_noise: the side stream would overwrite the static '
+                                          'input buffers while a replay reads them')
         if self.isTrain:
             if opt.loss not in ('l1', 'l2'):
                 raise NotImplementedError("pixel losses of models/losses.py:29-36: 'l1' (nn.L1Loss) or 'l2' (nn.MSELoss)")
             self.netG.loss_kind = opt.loss
-            self.optimizer_G = arch.FusedAdam(self.netG, lr=opt.lr, betas=(opt.beta1, 0.999), weight_decay=opt.wd)
+            self.optimizer_G = arch.FusedAdam(self.netG, lr=opt.lr, betas=(opt.beta1, 0.999), weight_decay=opt.wd,
+                                              capturable=self._graphed)
             self._init_optimizer([self.optimizer_G])
         if opt.resume:
             self.load(self, opt.resume_epoch)
-        self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
-        self.rank = dist.get_rank() if self.world > 1 else 0
         self._sync_replicas()
 
     def _sync_replicas(self):
@@ -155,11 +170,21 @@ class ELDModel(BaseModel):
             raise NotImplementedError('Mode [%s] is not implemented' % mode)
         pairs = mode == 'train' and input is not None and getattr(self.opt, 'pairs_on_gpu', False)
         synth = mode == 'train' and not pairs and (input is None or getattr(self.opt, 'noise_on_gpu', False))
+        isp = synth and self.opt.stage_in == 'srgb' and target.shape[1] == 4
+        aug = synth and getattr(self.opt, 'augment_on_gpu', False)
+        # a graphed step reads its frames from static buffers: every launch below writes its result straight into them
+        xs = ts = None
+        if self._graphed and mode == 'train':
+            n, c, h, w = target.shape
+            xs, ts = self._static_io((n, 3 if isp else (c if input is None else input.shape[1]), h, w), (n, c, h, w))
         pre = self._prefetched if synth else None
         if target is not None and not pairs and not (pre is not None and pre[0] is data):
-            target = target.to(device=self.device, dtype=torch.float32, non_blocking=True)
+            if ts is not None and not aug:
+                target = ts.copy_(target, non_blocking=True)
+            else:
+                target = target.to(device=self.device, dtype=torch.float32, non_blocking=True)
         if pairs:
-            input, target = self._ingest_pairs(input, target)
+            input, target = self._ingest_pairs(input, target, out=xs, target_out=ts)
         elif synth:
             self._prefetched = None
             if pre is not None and pre[0] is data:
@@ -170,12 +195,14 @@ class ELDModel(BaseModel):
                 input.record_stream(cur)
                 target.record_stream(cur)
             else:
-                input, target = self._synthesize(target)
-            if self.opt.stage_in == 'srgb' and input.shape[1] == 4:
+                input, target = self._synthesize(target, out=None if isp else xs, target_out=ts if aug else None)
+            if isp:
                 # ISPDataset.__getitem__ (sid_dataset.py:306-312) on the stream: noise -> clip -> raw2rgb_v2(wb, ccm) -> clip
                 from . import process
                 assert 'wb' in data and 'ccm' in data, "--stage_in srgb needs the frames' (wb, ccm) meta in the batch"
-                input = process.isp_dataset_item(input, data['wb'], data['ccm'], CRF=getattr(self, 'CRF', None))
+                input = process.isp_dataset_item(input, data['wb'], data['ccm'], CRF=getattr(self, 'CRF', None), out=xs)
+        elif xs is not None:
+            input = xs.copy_(input, non_blocking=True)
         else:
             input = input.to(device=self.device, dtype=torch.float32, non_blocking=True)
         self.input, self.target, self.data_name = input, target, data_name
@@ -183,12 +210,13 @@ class ELDModel(BaseModel):
         self.cfa = data['cfa'][0] if 'cfa' in data else 'bayer'
         self.aligned = False if 'unaligned' in data else True
 
-    def _synthesize(self, target):
+    def _synthesize(self, target, out=None, target_out=None):
         """On-the-fly synthesis (SynDataset semantics, sid_dataset.py:259-280, incl. the [0,1] clip) on the CURRENT stream.
         Frame ids count GLOBAL frames: step s of a W-GPU job owns ids [F, F + sum of the ranks' batch sizes), rank r the
         r-th slice.  Batches are equal-sized except possibly the last one of an epoch (DataLoader without drop_last), so F
         advances by the batch actually seen times W - ids never repeat, and the running count is part of the checkpoint
-        (a resumed run does not replay the Philox streams from frame 0)."""
+        (a resumed run does not replay the Philox streams from frame 0).  out / target_out: where the input / the
+        augmented target go (new tensors if None)."""
         assert self.noise_maker is not None, 'noise_on_gpu needs a noise_maker (eld_b200.noise.NoiseModel)'
         n = target.shape[0]
         fid0 = self._take_frame_ids(n)
@@ -200,8 +228,9 @@ class ELDModel(BaseModel):
             # ELDTrainDataset's flips / transpose / clip (sid_dataset.py:340-356) fused into the noise kernel:
             # both the synthesised input and the target come back augmented, one pass over the frames
             return self.noise_maker.batch_gpu_augmented(target, aug=self.noise_maker.frame_augment(fid0, n),
-                                                        params=params, frame_id0=fid0, clip=True)
-        return self.noise_maker.batch_gpu(target, params=params, frame_id0=fid0, clip=True), target
+                                                        params=params, frame_id0=fid0, clip=True, out=out,
+                                                        target_out=target_out)
+        return self.noise_maker.batch_gpu(target, params=params, frame_id0=fid0, clip=True, out=out), target
 
     def _take_frame_ids(self, n):
         """the global id of this rank's first frame of the step; advances the running count by the whole step"""
@@ -209,7 +238,7 @@ class ELDModel(BaseModel):
         self._frames_seen += self.world * n
         return fid0
 
-    def _ingest_pairs(self, input, target):
+    def _ingest_pairs(self, input, target, out=None, target_out=None):
         """ELDTrainDataset.__getitem__ (sid_dataset.py:337-356) over LMDBDataset (lmdb_dataset.py:28-41) for a batch
         of stored pairs (uint16 or float32, as eld_b200.datasets hands them out): both tensors cross PCIe as stored and
         one eld_pair_ingest launch on the current stream de-quantises, flips / transposes and clips them.  The flags
@@ -222,7 +251,7 @@ class ELDModel(BaseModel):
         flags = augment_flags(self.opt.seed, fid0, n) if getattr(self.opt, 'augment_on_gpu', False) else None
         input, target = ((t.view(torch.int16) if t.dtype == torch.uint16 else t).to(device=self.device, non_blocking=True)
                          for t in (input, target))
-        return datasets.ingest(input, target, flags)
+        return datasets.ingest(input, target, flags, out=out, target_out=target_out)
 
     def prefetch_input(self, data):
         """Start synthesising the NEXT step's noisy input on a side stream (Engine.train calls this right after it has
@@ -282,11 +311,87 @@ class ELDModel(BaseModel):
     def optimize_parameters(self):
         """forward, zero_grad, L1 backward, (all-reduce), Adam - ELD_model.py:469-475."""
         self._train()
+        if self._graphed:
+            return self._graph_step()
         if self.world > 1:
             self.output, self.loss_pixel = self.netG.train_step_ddp(self.input, self.target)
         else:
             self.output, self.loss_pixel = self.netG.train_step(self.input, self.target)
         self.optimizer_G.step(grad_scale=1.0 / self.world)
+
+    # ---- the fused step in a CUDA graph (opt.cuda_graph) ----------------------------------------------------------------
+    graph_warmup = 3      # eager steps (on a side stream, as torch's capture recipe runs them) before each capture
+
+    def _static_io(self, x_shape, t_shape):
+        """the input and target buffers the captured step reads; a shape change allocates new ones and drops the graph"""
+        s = self._static
+        if s is None or tuple(s[0].shape) != tuple(x_shape) or tuple(s[1].shape) != tuple(t_shape):
+            self._drop_graph()
+            s = self._static = (torch.empty(x_shape, dtype=torch.float32, device=self.device),
+                                torch.empty(t_shape, dtype=torch.float32, device=self.device))
+        return s
+
+    def _drop_graph(self):
+        self._graph = None
+        self._eager_left = self.graph_warmup
+
+    def _graph_key(self):
+        """what a captured step bakes in besides its buffers: re-captured when any of it changes"""
+        g = self.optimizer_G.param_groups[0]
+        return (tuple(self._static[0].shape), tuple(self._static[1].shape), self.netG.loss_kind,
+                tuple(p.requires_grad for p in self.netG.parameters()), tuple(float(b) for b in g['betas']),
+                float(g['eps']), float(g['weight_decay']))
+
+    def _fused_step(self, x, t):
+        out, loss = self.netG.train_step(x, t)
+        self.optimizer_G.step()
+        return out, loss
+
+    def _graph_step(self):
+        """One training step through the captured graph.  The frames reach the static buffers (set_input writes them
+        there); a step whose key (_graph_key) differs from the captured one runs eagerly on a side stream, graph_warmup
+        times, and the next one is captured and replayed.  The graph holds the _Engine plan it launches on, so the
+        engine cache's eviction cannot free a workspace it addresses.  No host synchronisation."""
+        xs, ts = self._static_io(self.input.shape, self.target.shape)
+        if self.input.data_ptr() != xs.data_ptr():
+            xs.copy_(self.input)
+        if self.target.data_ptr() != ts.data_ptr():
+            ts.copy_(self.target)
+        self.input, self.target = xs, ts
+        key = self._graph_key()
+        if self._graph is not None and self._graph[0] != key:
+            self._drop_graph()
+        if self._graph is None and self._eager_left > 0:
+            self._eager_left -= 1
+            cur = torch.cuda.current_stream()
+            side = torch.cuda.Stream(device=self.device)
+            side.wait_stream(cur)
+            with torch.cuda.stream(side):
+                out, loss = self._fused_step(xs, ts)
+            cur.wait_stream(side)
+            for tensor in (out, loss):
+                tensor.record_stream(cur)
+            self.output, self.loss_pixel = out, loss
+            return
+        if self._graph is None:
+            self._capture(key, xs, ts)
+        _, graph, plan, out, loss = self._graph
+        plan.owner = None              # the replay overwrites the built-in forward state, as train_step does
+        self.optimizer_G.graph_step()
+        graph.replay()
+        self.output = out              # overwritten by the next replay
+        self.loss_pixel = loss.clone()
+
+    def _capture(self, key, xs, ts):
+        if self.netG._profiling:
+            raise NotImplementedError('cuda_graph: an engine with per-launch profiling on cannot be captured')
+        n, _, h, w = xs.shape
+        plan = self.netG._plan(n, h, w, True)      # created (or kept most recent) outside the capture
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            out, loss = self._fused_step(xs, ts)
+        self.optimizer_G.t -= 1                    # the capture ran no step; graph_step counts each replay
+        self._graph = (key, graph, plan, out, loss)
 
     def backward_G(self):
         """ELD_model.py:411-420 as written in the reference: loss on self.output, .backward() through the netG autograd

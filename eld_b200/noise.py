@@ -165,10 +165,12 @@ class NoiseModelBase:
                     flags[f] |= bit
         return flags
 
-    def batch_gpu_augmented(self, clean, aug=None, params=None, frame_id0=None, clip=True, seed=None):
+    def batch_gpu_augmented(self, clean, aug=None, params=None, frame_id0=None, clip=True, seed=None, out=None,
+                            target_out=None):
         """SynDataset + ELDTrainDataset in one kernel (sid_dataset.py:269-277, 340-356): returns
         (input, target) = (aug(clip(noise(clean))), aug(clean)), aug = per-frame flip rows / flip columns / transpose.
-        `aug`: uint8 flags per frame (bit 0 rows, 1 columns, 2 transpose) or None to draw them like the reference."""
+        `aug`: uint8 flags per frame (bit 0 rows, 1 columns, 2 transpose) or None to draw them like the reference.
+        `out` / `target_out`: contiguous f32 tensors of clean's shape to write input / target into (new ones if None)."""
         import ctypes
         import torch
         assert clean.is_cuda and clean.dtype == torch.float32 and clean.dim() == 4 and clean.shape[1] == 4
@@ -181,8 +183,10 @@ class NoiseModelBase:
         assert aug.shape == (n,)
         if frame_id0 is None:
             frame_id0 = int(np.random.randint(0, 2 ** 62))
-        noisy = torch.empty_like(clean)
-        target = torch.empty_like(clean)
+        noisy = torch.empty_like(clean) if out is None else out
+        target = torch.empty_like(clean) if target_out is None else target_out
+        for t in (noisy, target):
+            assert t.is_contiguous() and t.shape == clean.shape and t.dtype == torch.float32
         lib = _lib.load()
         rc = lib.eld_noise_packed_aug(_lib.ctx(clean.device.index or 0), clean.data_ptr(), noisy.data_ptr(), target.data_ptr(),
                                       n, h, w, params_array(plist), _lib.model_mask(self.model),

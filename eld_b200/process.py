@@ -21,16 +21,19 @@ def _f32_host(a, shape):
     return a
 
 
-def process(bayer_images, wbs, cam2rgbs, gamma=2.2, CRF=None):
+def process(bayer_images, wbs, cam2rgbs, gamma=2.2, CRF=None, out=None):
     """bayer_images: cuda f32 [N,4,h,w] RGBG; wbs [N,4]; cam2rgbs [N,3,3]; CRF = (E [3,L] or [L], fs [3,L]) or None.
-    Returns cuda f32 [N,3,h,w] in [0,1], quantised to 8 bits like the reference (process.py:38,83)."""
+    Returns cuda f32 [N,3,h,w] in [0,1], quantised to 8 bits like the reference (process.py:38,83); written into `out`
+    (contiguous f32 [N,3,h,w]) when given."""
     import torch
     assert bayer_images.is_cuda and bayer_images.dtype == torch.float32 and bayer_images.dim() == 4 and bayer_images.shape[1] == 4
     x = bayer_images.contiguous()
     n, _, h, w = x.shape
     wb = _f32_host(wbs.detach().cpu().numpy() if hasattr(wbs, 'detach') else wbs, (n, 4))
     ccm = _f32_host(cam2rgbs.detach().cpu().numpy() if hasattr(cam2rgbs, 'detach') else cam2rgbs, (n, 3, 3)).reshape(n, 9)
-    out = torch.empty((n, 3, h, w), dtype=torch.float32, device=x.device)
+    if out is None:
+        out = torch.empty((n, 3, h, w), dtype=torch.float32, device=x.device)
+    assert out.is_contiguous() and out.shape == (n, 3, h, w) and out.dtype == torch.float32
     E_ptr = f_ptr = None
     L = 0
     keep = None
@@ -60,12 +63,13 @@ def raw2rgb_v2(packed_raw, wb, ccm, CRF=None, gamma=2.2):
     return out[0].cpu().numpy()
 
 
-def isp_dataset_item(noisy_packed, wb, ccm, CRF=None):
+def isp_dataset_item(noisy_packed, wb, ccm, CRF=None, out=None):
     """ISPDataset.__getitem__ after the noise call (dataset/sid_dataset.py:309-312): clip, raw2rgb_v2, clip.  The kernel
-    clips its input after the white balance exactly like `process`; the leading clip to [0,1] is applied here."""
+    clips its input after the white balance exactly like `process`; the leading clip to [0,1] is applied here.
+    `out`: as for `process`."""
     import torch
     x = torch.clamp(noisy_packed, 0.0, 1.0)
-    return process(x, wb, ccm, CRF=CRF)
+    return process(x, wb, ccm, CRF=CRF, out=out)
 
 
 def read_emor(path):

@@ -78,7 +78,12 @@ size_t eld_unet_workspace_bytes(int n, int h, int w, int train);     /* activati
                                                                       * words (1 bit per masked activation element) and pool codes
                                                                       * (1 byte per pooled element: argmax + signs) */
 /* Inference (train = 0): h % 16 == 0 and w % 16 == 0, as for the reference network.  Training (train = 1):
- * h % 128 == 0, w % 256 == 0.  The caller owns `workspace` (device memory) for the lifetime of the object. */
+ * h % 128 == 0, w % 256 == 0.  The caller owns `workspace` (device memory) for the lifetime of the object.
+ * Creation synchronises (a cudaMemset of the workspace, the kernels' shared-memory opt-in): create the object outside any
+ * CUDA graph capture.  eld_unet_train_step (per-launch profiling off, eld_unet_profile) neither synchronises nor
+ * allocates - memsets on `stream`, kernels with
+ * programmatic stream serialization - so it captures into a graph (programmatic edges) and replays; the graph keeps
+ * addressing this object's workspace, which must outlive it. */
 int    eld_unet_create(eld_ctx* ctx, int n, int h, int w, int train, void* workspace, size_t bytes, eld_unet** out);
 void   eld_unet_destroy(eld_unet* u);
 /* The same network with 3-channel frames on either side (ELDModel.initialize, ELD_model.py:377-389: in_channels = 3 for
@@ -172,5 +177,26 @@ int    eld_adam_step(eld_ctx* ctx, float* params, const float* grads, float* m, 
 int    eld_adam_step_segments(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, const size_t* segs,
                               const int* steps, int n_segs, float lr, float beta1, float beta2, float eps,
                               float weight_decay, float grad_scale, void* stream);
+/* Capturable Adam (torch.optim.Adam(capturable=True)): the same update, with the learning rate and the step counters in
+ * DEVICE memory, read when the kernels run, so that a CUDA graph that captured the call is right on every replay.
+ * *lr (device float) is the learning rate; a step counter (device int) holds the steps its elements have taken so far
+ * (>= 0), and this call updates them with the bias corrections of step counter + 1 (1 - beta^t by device powf, which may
+ * differ from the host powf of eld_adam_step by an ulp) and leaves counter + 1 behind.
+ * Mechanism: two launches on `stream`.  The update kernel reads lr and the counters (thread s of each block derives range
+ * s's bias corrections into shared memory) and never writes a counter; a one-block kernel issued after it increments
+ * each counter once.  No thread reads a counter after it has been incremented.
+ * eld_adam_step_capturable: elements [0, n), one counter `step`.
+ * eld_adam_step_segments_capturable: n_segs ranges as for eld_adam_step_segments (segs, host), steps (host) = one device
+ * counter per range; a counter named by several ranges takes one step.  Ranges holding no element still step their
+ * counters; n_segs == 0 launches nothing.
+ * ELD_E_ARG, nothing written and nothing launched: a NULL argument (a NULL counter among steps included), more than 64
+ * ranges, two ranges that share an element. */
+int    eld_adam_step_capturable(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, size_t n,
+                                const float* lr, int* step, float beta1, float beta2, float eps, float weight_decay,
+                                float grad_scale, void* stream);
+int    eld_adam_step_segments_capturable(eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
+                                         const size_t* segs, int* const* steps, int n_segs, const float* lr,
+                                         float beta1, float beta2, float eps, float weight_decay, float grad_scale,
+                                         void* stream);
 
 #endif
