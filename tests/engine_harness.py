@@ -38,6 +38,58 @@ def frames(n, cin, cout, h, w, seed):
     return torch.rand(n, cin, h, w, generator=g).cuda(), torch.rand(n, cout, h, w, generator=g).cuda()
 
 
+def integer_weights(module, fan_in, seed):
+    """Fill the U-Net `module` (arch.unet or the oracle module: the same parameter names) with an integer network:
+    every output of every layer is the sum of `fan_in` inputs picked at seeded positions (a conv3x3 output channel:
+    (tap, input channel) pairs; a deconv output channel: input channels per sub-pixel; the head: input channels), that
+    is weights in {0, 1}.  Biases are 0 except conv9_2's, which are 1: the head's LeakyReLU' is a > 0, so a9_2 must not
+    hold a zero (a slope of 0.2f would take dz9_2 off the dyadic grid).  On integer frames every activation is then a
+    non-negative integer, LeakyReLU's negative branch is never taken, and every gradient stays on the grid of dOut."""
+    import torch
+    g = torch.Generator().manual_seed(seed)
+    with torch.no_grad():
+        for name, p in module.named_parameters():
+            layer, kind = name.split('.')
+            if kind == 'bias':
+                p.fill_(1.0 if layer == 'conv9_2' else 0.0)
+                continue
+            w = torch.zeros(p.shape)
+            if layer.startswith('upv'):            # IOHW: per (co, sub-pixel), fan_in input channels
+                ci, co = p.shape[:2]
+                for o in range(co):
+                    for s in range(4):
+                        pick = torch.randperm(ci, generator=g)[:fan_in]
+                        w[pick, o, s // 2, s % 2] = 1.0
+            else:                                  # OIHW: per output channel, fan_in (input channel, tap) pairs
+                co = p.shape[0]
+                k = p[0].numel()
+                for o in range(co):
+                    w[o].view(-1)[torch.randperm(k, generator=g)[:fan_in]] = 1.0
+            p.copy_(w.to(p.device))
+    return module
+
+
+def integer_net(cin=4, cout=4, fan_in=1, seed=7):
+    """net(cin, cout) with integer_weights(fan_in, seed)"""
+    return integer_weights(net(cin, cout), fan_in, seed)
+
+
+def integer_frames(n, cin, h, w, seed):
+    """integer frames 0..3 as fp32 [n, cin, h, w] on the GPU"""
+    import torch
+    g = torch.Generator().manual_seed(seed)
+    return torch.randint(0, 4, (n, cin, h, w), generator=g).float().cuda()
+
+
+def half_off(out, seed):
+    """a target 0.5 above or below each element of the integer output `out`, the side drawn from `seed`: the L1 loss
+    never sits on a tie, |e| = 1/2 keeps the loss's sum provable at any size, and MSE's 2 e is +-1"""
+    import torch
+    g = torch.Generator().manual_seed(seed)
+    side = torch.randint(0, 2, out.shape, generator=g).float().to(out.device)
+    return out + side - 0.5
+
+
 def spread_biases(ours, ref, seed=5):
     """The default init leaves most pre-activations on one side of LeakyReLU's kink: add the same seeded spread to the
     biases of both modules, so that both branches - and both values of the backward mask - carry real weight."""

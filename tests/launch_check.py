@@ -2,6 +2,8 @@
 finished step or forward on the exact tensors it read, as the engine stored them in its workspace (eld_unet_buffer),
 against the float64 references of tests/launch_ref.py, by the acceptance rules and gates below, and records the worst
 case per launch kind in the caller's table."""
+import math
+
 # fraction of bf16 elements allowed to differ from RNE(r) (fp32 accumulation order): about 4x the worst rate measured on
 # an H100 80GB HBM3 at a 400 W power limit over the cases below
 MISMATCH = {'conv.fprop': 0.01, 'conv.dgrad': 0.011, 'conv.dgrad.mask': 0.011, 'conv.dgrad.split': 0.006,
@@ -60,6 +62,18 @@ class Step:
         self.span = {k: sp for k, sp in zip(self.params, net._spans)}
         self.fail = []
         self.names = []
+        self.n_elements = self.n_provable = 0     # elements under the exact rule, and those provably exact
+
+    @property
+    def share(self):
+        """the share of this step's checked outputs (bf16 and fp32 elements) that the exact rule covered"""
+        return self.n_provable / max(self.n_elements, 1)
+
+    def q(self, *ts, bias=None):
+        """the grid of the products of operands ts (launch_ref.grid), capped by the bias's own grid"""
+        from tests.launch_ref import grid
+        q = sum(grid(t) for t in ts)
+        return q if bias is None else min(q, grid(bias))
 
     def V(self, name):
         from tests.launch_ref import buffer
@@ -83,8 +97,26 @@ class Step:
         half = flat.numel() // 2
         return flat[:half].view(n, h, w, c // 2), flat[half:].view(n, h, w, c // 2)
 
-    # ---- the three acceptance rules ----
-    def bf16(self, kind, where, got, r, S):
+    # ---- the acceptance rules ----
+    def provable(self, kind, where, got, want, S, q):
+        """the exact rule: every element whose accumulation is exact (launch_ref.exact_mask(S, q), q the grid of the
+        launch's products) equals `want` bit for bit - the kernel's epilogue emulated in float32 for a bf16 output, r
+        for an fp32 one.  Counts the elements compared and those provable, per launch kind."""
+        from tests.launch_ref import exact_mask, exact_rule
+        mask = exact_mask(S, q)
+        n = int(mask.sum().item())
+        st = self.stats['provable ' + kind + self.tag]
+        st['elements'] += mask.numel()
+        st['exact'] += n
+        st['share'] = st['exact'] / st['elements']
+        self.n_elements += mask.numel()
+        self.n_provable += n
+        bad = exact_rule(got, want, mask) if n else 0
+        if bad:
+            self.fail.append('%s (%s): %d of %d provable elements differ' % (where, kind, bad, n))
+
+    def bf16(self, kind, where, got, r, S, exact=None):
+        """exact: (the emulated bf16 output, q) for the exact rule on the provable elements"""
         from tests.launch_ref import bf16_rule
         assert got.shape == r.shape, (where, got.shape, r.shape)
         ratio, mism, finite = bf16_rule(got, r, S)
@@ -93,8 +125,11 @@ class Step:
         st['mismatch'] = max(st['mismatch'], mism)
         if not (ratio <= 1.0 and mism <= MISMATCH[kind]) or not finite:
             self.fail.append('%s (%s): max |got-r|/(ulp+2^-20 S) = %.3g, mismatch %.3g' % (where, kind, ratio, mism))
+        if exact is not None:
+            self.provable(kind, where, got, exact[0], S, exact[1])
 
-    def f32(self, kind, where, got, r, S):
+    def f32(self, kind, where, got, r, S, q=None):
+        """q: the grid of the launch's products, for the exact rule on the provable elements"""
         from tests.launch_ref import f32_rule
         rel, mx, ms = f32_rule(got, r, S)
         st = self.stats['fp32 ' + kind + self.tag]
@@ -106,14 +141,16 @@ class Step:
             rel_max, abs_max = (PRODUCTION_WGRAD, PRODUCTION_WGRAD) if self.tag else (WGRAD_REL_L2, MAX_ABS)
         if not (rel <= rel_max and mx <= abs_max):
             self.fail.append('%s (%s): rel-L2 %.3g, max-abs / max|r| %.3g' % (where, kind, rel, mx))
+        if q is not None:
+            self.provable(kind, where, got.reshape(r.shape), r, S, q)
 
-    def grad(self, kind, pname, r, S):
+    def grad(self, kind, pname, r, S, q=None):
         """a parameter's range of grads: the fp32 rule when it trains, all zero bits when it is frozen"""
         got = self.G(pname)
         if pname in self.frozen:
             self.exact('frozen range', pname, got.view(self.t.int32), self.t.zeros_like(got).view(self.t.int32))
         else:
-            self.f32(kind, pname, got, r, S)
+            self.f32(kind, pname, got, r, S, q)
 
     def exact(self, kind, where, got, want):
         self.stats['exact ' + kind]['elements'] += got.numel()
@@ -142,14 +179,17 @@ class Step:
         src, sc0, dst, dc0 = FWD[layer]
         if layer.startswith('upv'):
             cout = self.W(layer).shape[1]
-            r, S = R.deconv_fprop(self.V(src), self.W(layer), self.B(layer))
-            self.bf16('deconv.fprop', layer, self.V(dst)[..., :cout], r, S)
+            x = self.V(src)
+            r, S = R.deconv_fprop(x, self.W(layer), self.B(layer))
+            q = self.q(x, R.bf(self.W(layer)), bias=self.B(layer))
+            self.bf16('deconv.fprop', layer, self.V(dst)[..., :cout], r, S, (R.epi_store(r), q))
             return
         cout, cin = self.W(layer).shape[:2]
         x = self.V(src)[..., sc0:sc0 + cin]
-        r, S = R.conv_fprop(x, self.W(layer), self.B(layer))
+        z, S = R.conv_fprop(x, self.W(layer), self.B(layer), act=False)
         got = self.V(dst)[..., dc0:dc0 + cout]
-        self.bf16('conv.fprop', layer, got, r, S)
+        q = self.q(x, R.bf(self.W(layer)), bias=self.B(layer))
+        self.bf16('conv.fprop', layer, got, R.lrelu(z), S, (R.epi_store(z, act=True), q))
         self.epilogue_extras(layer, dst, got)
 
     def epilogue_extras(self, layer, dst, got):
@@ -171,60 +211,71 @@ class Step:
 
     def first_fprop(self):
         import tests.launch_ref as R
-        r, S = R.first_conv_fprop(self.x, self.W('conv1_1'), self.B('conv1_1'))
+        frame = R.bf(self.x).permute(0, 2, 3, 1)
+        z, S = R.conv_fprop(frame, self.W('conv1_1'), self.B('conv1_1'), act=False)
         got = self.V('a1_1')
-        self.bf16('conv1_1.fprop', 'conv1_1', got, r, S)
+        q = self.q(frame, R.bf(self.W('conv1_1')), bias=self.B('conv1_1'))
+        self.bf16('conv1_1.fprop', 'conv1_1', got, R.lrelu(z), S, (R.epi_store(z, act=True), q))
         self.epilogue_extras('conv1_1', 'a1_1', got)
 
     def dgrad(self, layer):
         import tests.launch_ref as R
         src = FWD[layer][0]
+        wq = R.bf(self.W(layer))
         if layer.startswith('upv'):
             up, _ = self.planes('dcat' + layer[3:])
-            r, S = R.deconv_dgrad(up, self.W(layer), self.V(src))
-            self.bf16('deconv.dgrad', layer, self.V('dz' + src[1:]), r, S)
+            act = self.V(src)
+            z, S = R.deconv_dgrad(up, self.W(layer))
+            s = R.slope(act)
+            self.bf16('deconv.dgrad', layer, self.V('dz' + src[1:]), z * s, S * s, (R.epi_mask(z, act), self.q(up, wq)))
             return
         dz = self.V(_dz(layer))
+        z, S = R.conv_dgrad(dz, self.W(layer))
+        q = self.q(dz, wq)
         if src.startswith('cat'):
             up, skip = self.planes('d' + src)
-            r, S = R.conv_dgrad(dz, self.W(layer))
             half = up.shape[-1]
+            want = R.epi_mask(z, None)
             if _level(src) in self.skip_elided:   # the row-prefix launch: the up half only, the skip plane keeps its sentinel
-                self.bf16('conv.dgrad.prefix', layer, up, r[..., :half], S[..., :half])
+                self.bf16('conv.dgrad.prefix', layer, up, z[..., :half], S[..., :half], (want[..., :half], q))
                 self.exact('sentinel', 'd%s skip plane' % src, self.bits(skip), self.t.full_like(self.bits(skip), NAN_BITS))
             else:
-                self.bf16('conv.dgrad.split', layer, up, r[..., :half], S[..., :half])
-                self.bf16('conv.dgrad.split', layer + ' skip', skip, r[..., half:], S[..., half:])
+                self.bf16('conv.dgrad.split', layer, up, z[..., :half], S[..., :half], (want[..., :half], q))
+                self.bf16('conv.dgrad.split', layer + ' skip', skip, z[..., half:], S[..., half:], (want[..., half:], q))
         elif src.startswith('p'):
-            r, S = R.conv_dgrad(dz, self.W(layer))
-            self.bf16('conv.dgrad', layer, self.V('d' + src), r, S)
+            self.bf16('conv.dgrad', layer, self.V('d' + src), z, S, (R.epi_mask(z, None), q))
         else:
-            r, S = R.conv_dgrad(dz, self.W(layer), self.V(src))
-            self.bf16('conv.dgrad.mask', layer, self.V('dz' + src[1:]), r, S)
+            act = self.V(src)
+            s = R.slope(act)
+            self.bf16('conv.dgrad.mask', layer, self.V('dz' + src[1:]), z * s, S * s, (R.epi_mask(z, act), q))
 
     def pool_bwd(self, k):
         import tests.launch_ref as R
         cat, c0, dcat, dp, dst = POOL_BWD[k]
         c = self.V(dp).shape[-1]
         _, skip = self.planes(dcat)
-        r, S = R.pool_bwd(self.V(cat)[..., c0:c0 + c], skip, self.V(dp))
-        self.bf16('pool.bwd', dst, self.V(dst), r, S)
+        a, d = self.V(cat)[..., c0:c0 + c], self.V(dp)
+        r, S = R.pool_bwd(a, skip, d)
+        q = min(self.q(skip), self.q(d))
+        self.bf16('pool.bwd', dst, self.V(dst), r, S, (R.epi_pool_bwd(a, skip, d), q))
 
     def wgrad(self, layer):
         import tests.launch_ref as R
         src, sc0 = FWD[layer][:2]
         if layer.startswith('upv'):
             up, _ = self.planes('dcat' + layer[3:])
-            dW, S, db, Sb = R.deconv_wgrad(self.V(src), up)
-            self.grad('deconv.wgrad', layer + '.weight', dW, S)
-            self.grad('deconv.bias_grad', layer + '.bias', db, Sb)
+            x = self.V(src)
+            dW, S, db, Sb = R.deconv_wgrad(x, up)
+            self.grad('deconv.wgrad', layer + '.weight', dW, S, self.q(x, up))
+            self.grad('deconv.bias_grad', layer + '.bias', db, Sb, self.q(up))
             return
         cout, cin = self.W(layer).shape[:2]
-        dW, S, db, Sb = R.conv_wgrad(self.V(src)[..., sc0:sc0 + cin], self.V(_dz(layer)))
+        x, dz = self.V(src)[..., sc0:sc0 + cin], self.V(_dz(layer))
+        dW, S, db, Sb = R.conv_wgrad(x, dz)
         off = self.span[layer + '.weight'][0]
         staged = self.V('gtmp').reshape(-1)[off:off + dW.numel()].view(3, 3, cin, cout).permute(3, 2, 0, 1)
-        self.f32('conv.wgrad', layer + ' (gtmp)', staged, dW, S)    # staged whether or not the weight trains
-        self.grad('conv.bias_grad', layer + '.bias', db, Sb)
+        self.f32('conv.wgrad', layer + ' (gtmp)', staged, dW, S, self.q(x, dz))    # staged whether or not the weight trains
+        self.grad('conv.bias_grad', layer + '.bias', db, Sb, self.q(dz))
 
     def gperm(self, trained):
         """grads (OIHW) of every trained conv3x3 weight == its [tap][ci][co] staging, permuted; a frozen one's range zero"""
@@ -240,34 +291,44 @@ class Step:
 
     def first_wgrad(self):
         import tests.launch_ref as R
-        dW, S, db, Sb = R.first_conv_wgrad(self.x, self.V('dz1_1'))
-        self.grad('conv1_1.wgrad', 'conv1_1.weight', dW, S)
-        self.grad('conv1_1.bias_grad', 'conv1_1.bias', db, Sb)
+        dz = self.V('dz1_1')
+        dW, S, db, Sb = R.first_conv_wgrad(self.x, dz)
+        self.grad('conv1_1.wgrad', 'conv1_1.weight', dW, S, self.q(R.bf(self.x), dz))
+        self.grad('conv1_1.bias_grad', 'conv1_1.bias', db, Sb, self.q(dz))
 
     def first_dgrad(self):
         import tests.launch_ref as R
-        r, S = R.first_conv_dgrad(self.V('dz1_1'), self.W('conv1_1'))
-        self.f32('x.grad', 'conv1_1 dgrad', self.dx, r, S)
+        dz = self.V('dz1_1')
+        r, S = R.first_conv_dgrad(dz, self.W('conv1_1'))
+        self.f32('x.grad', 'conv1_1 dgrad', self.dx, r, S, self.q(dz, R.bf(self.W('conv1_1'))))
 
     def head(self, what):
         import tests.launch_ref as R
         a, w = self.V('a9_2'), self.W('conv10_1')
         if what != 'bwd':             # the seam's backward re-forms out into scratch: its forward launch is checked instead
             r, S = R.head(a, w, self.B('conv10_1'))
-            self.f32('head.out', 'conv10_1 out', self.out, r, S)
+            self.f32('head.out', 'conv10_1 out', self.out, r, S, self.q(a, w, bias=self.B('conv10_1')))
         if what == 'fprop':
             return
         if what != 'bwd':
             lr = R.head_loss(self.out, self.target, self.kind)
-            self.f32('head.loss.' + self.kind, 'loss', self.loss.reshape(1), lr.reshape(1), lr.reshape(1))
+            # the kernel sums |e| (e^2) exactly when the sum is on the grid of e and scales by 1 / numel, exact when that
+            # is a power of two
+            numel = self.out.numel()
+            qe = self.q(self.out.double() - self.target.double()) * (1 if self.kind == 'l1' else 2)
+            q = qe - math.log2(numel) if numel & (numel - 1) == 0 else -math.inf
+            self.f32('head.loss.' + self.kind, 'loss', self.loss.reshape(1), lr.reshape(1), lr.reshape(1), q)
         if what == 'fwd+loss':
             return
         dout = self.dout if what == 'bwd' else R.head_dout(self.out, self.target, self.kind)
         dz, S, dW, Sw, db, Sb = R.head_bwd(a, w, dout)
+        qd = self.q(dout)
         if self.dz9_2:
-            self.bf16('head.dz9_2' + ('.seam' if what == 'bwd' else '.' + self.kind), 'dz9_2', self.V('dz9_2'), dz, S)
-        self.grad('head.dW10', 'conv10_1.weight', dW, Sw)
-        self.grad('head.db10', 'conv10_1.bias', db, Sb)
+            z = dout.double().permute(0, 2, 3, 1) @ w.double().reshape(w.shape[0], -1)
+            self.bf16('head.dz9_2' + ('.seam' if what == 'bwd' else '.' + self.kind), 'dz9_2', self.V('dz9_2'), dz, S,
+                      (R.epi_head_dz(z, a), qd + self.q(w)))
+        self.grad('head.dW10', 'conv10_1.weight', dW, Sw, qd + self.q(a))
+        self.grad('head.db10', 'conv10_1.bias', db, Sb, qd)
 
     def check(self, names):
         """every launch in `names` (the engine's profile, in issue order)"""

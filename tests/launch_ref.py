@@ -10,7 +10,9 @@ reference lines up with the workspace view element for element; the convolutions
 (eld_unet_buffer), never restated here.
 """
 import ctypes
+import math
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -53,6 +55,17 @@ def bf16_rule(got, r, S):
     return ratio, mism, bool(torch.isfinite(g).all())
 
 
+def exact_rule(got, want, mask):
+    """the number of elements inside `mask` where got differs from want bit for bit; +0 and -0 count as equal (the sign
+    of an exact zero sum of products depends on the order when every product is -0).  want: a bf16 tensor, or the
+    float64 r of an fp32 output."""
+    if want.dtype == torch.float64:
+        same = got.double().reshape(want.shape) == want
+    else:
+        same = (got.view(torch.int16) == want.view(torch.int16)) | ((got == 0) & (want == 0))
+    return int((mask & ~same).sum().item())
+
+
 def f32_rule(got, r, S):
     """the statistics of the fp32 rule: (rel-L2 of got - r, max |got - r| / max |r|, max |got - r| / S)"""
     d = got.double().reshape(r.shape) - r
@@ -65,6 +78,80 @@ def f32_rule(got, r, S):
 def slope(a):
     """LeakyReLU' from the sign of the stored activation: 1, or 0.2 where the sign bit is set (+0 counts positive)"""
     return 1.0 - 0.8 * torch.signbit(a.float()).double()
+
+
+# ---- exactly summable operands ---------------------------------------------------------------------------------------
+# If every element of operand A is a multiple of 2^qa, every element of B a multiple of 2^qb (and a bias a multiple of
+# 2^(qa+qb)), every product and every partial sum of an output element, in any order, is an integer multiple of
+# 2^(qa+qb) no larger in magnitude than S, the sum of |terms|.  Below 2^(qa+qb+24) each such number is an fp32 number:
+# the fp32 accumulation is exact whatever its order, split or atomics, and the kernel's result is fully determined -
+# r itself for an fp32 output, the kernel's epilogue applied to r in float32 for a bf16 output.
+def grid(t):
+    """the largest q such that every element of t is a multiple of 2^q: +inf for an all-zero tensor, -inf when an
+    element is not finite"""
+    t = t.double().reshape(-1)
+    if not bool(torch.isfinite(t).all()):
+        return -math.inf
+    t = t[t != 0]
+    if t.numel() == 0:
+        return math.inf
+    m, e = torch.frexp(t)                              # t = m 2^e, 0.5 <= |m| < 1: m 2^53 is an integer
+    mant = torch.ldexp(m, torch.full_like(e, 53)).long()
+    _, low = torch.frexp((mant & -mant).double())     # its lowest set bit, 2^(low - 1)
+    return int((e + low - 54).min().item())
+
+
+def exact_mask(S, q):
+    """the output elements whose accumulation is exact in fp32 in any order: S < 2^(q + 24)"""
+    if q == math.inf:
+        return torch.ones_like(S, dtype=torch.bool)
+    if q == -math.inf or q + 24 < -1000:
+        return torch.zeros_like(S, dtype=torch.bool)
+    return S < 2.0 ** min(q + 24, 1000)
+
+
+# the float32 constants of the kernels' epilogues (csrc/conv_gemm.cuh conv_epilogue32, csrc/unet_ew.cu)
+F32_02 = float(np.float32(0.2))                                # fmaxf(v, 0.2f * v), the head's 0.2f
+MASK_NEG = float(np.float32(0.6) - np.float32(0.4))            # fmaf(-1, 0.4f, 0.6f): exact (Sterbenz), not 0.2f
+
+
+def _f32(t, c):
+    return torch.tensor(c, dtype=torch.float32, device=t.device)
+
+
+def epi_store(z, b=None, act=False):
+    """conv / deconv fprop epilogue on the exact accumulator z (float64, no bias): fp32 bias add, fmaxf(v, 0.2f v),
+    round to bf16"""
+    v = z.float()
+    if b is not None:
+        v = v + b.float()
+    if act:
+        v = torch.maximum(v, v * _f32(v, F32_02))
+    return v.bfloat16()
+
+
+def epi_mask(z, act):
+    """dgrad epilogue: the exact accumulator z times fmaf(+-1, 0.4f, 0.6f) from the sign bit of the stored activation
+    (+0 counts positive; None: no mask), round to bf16"""
+    v = z.float()
+    if act is not None:
+        v = v * torch.where(torch.signbit(act.float()), _f32(v, MASK_NEG), _f32(v, 1.0))
+    return v.bfloat16()
+
+
+def epi_pool_bwd(a, dskip, dp):
+    """maxpool_bwd_code_kernel: (dskip + (first arg-max ? dp : +0)) * fmaf(+-1, 0.4f, 0.6f) in float32, round to bf16"""
+    _, _, first = pool(a)
+    n, h, w, c = a.shape
+    g = torch.where(first, dp.float().unsqueeze(-1), _f32(a, 0.0)).reshape(n, h // 2, w // 2, c, 2, 2)
+    g = g.permute(0, 1, 4, 2, 5, 3).reshape(n, h, w, c)
+    return epi_mask((dskip.float() + g).double(), a)
+
+
+def epi_head_dz(z, a):
+    """head_kernel's dz9_2: the exact sum z over the four outputs times (a > 0 ? 1 : 0.2f), round to bf16"""
+    v = z.float()
+    return (v * torch.where(a.float() > 0, _f32(v, 1.0), _f32(v, F32_02))).bfloat16()
 
 
 def lrelu(v):

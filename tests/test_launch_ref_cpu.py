@@ -1,6 +1,9 @@
 """The float64 references of tests/launch_ref.py checked against torch's own float64 convolutions and autograd, and
 the bit layouts of the sign words and pool codes against a hand-built window - on the CPU, so that the per-launch GPU
 suite measures the kernels with a yardstick that is itself tested."""
+import math
+
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -115,6 +118,146 @@ def test_reference_variants_without_bias_or_mask():
     rm, _ = R.deconv_dgrad(dy, wt, x)
     s = torch.where(torch.signbit(x.float()), torch.tensor(0.2, dtype=torch.float64), torch.tensor(1.0, dtype=torch.float64))
     assert torch.allclose(rm, r * s, rtol=1e-12, atol=1e-12)
+
+
+def test_grid_on_hand_made_tensors():
+    assert R.grid(torch.tensor([1.0, 2.0, 3.0])) == 0
+    assert R.grid(torch.tensor([4.0, -8.0, 12.0])) == 2
+    assert R.grid(torch.tensor([0.75, 0.0, -1.5])) == -2
+    assert R.grid(torch.tensor([2.0 ** -23, 1.0])) == -23
+    assert R.grid(torch.tensor([3.0 * 2 ** 40])) == 40
+    assert R.grid(torch.zeros(5)) == math.inf and R.grid(torch.tensor([-0.0, 0.0])) == math.inf
+    assert R.grid(torch.tensor([1.0, float('nan')])) == -math.inf
+    assert R.grid(torch.tensor([0.2]).float()) == -26            # 0.2f = 13421773 x 2^-26
+    assert R.grid(torch.tensor([1.5, 2.5]).bfloat16()) == -1
+    S = torch.tensor([2.0 ** 24 - 1, 2.0 ** 24, 3.0], dtype=torch.float64)
+    assert R.exact_mask(S, 0).tolist() == [True, False, True]
+    assert R.exact_mask(S, -2).tolist() == [False, False, True]
+    assert R.exact_mask(S, math.inf).all() and not R.exact_mask(S, -math.inf).any()
+
+
+def _bits(t):
+    return t.view(torch.int16).tolist()
+
+
+def test_epilogue_emulations_by_hand():
+    # 0.2f: fmaxf(v, 0.2f v) multiplies by 13421773 x 2^-26, not 0.2; v = -5 -> -1.0000000149 -> bf16 -1.0
+    assert R.F32_02 == 13421773 * 2.0 ** -26
+    got = R.epi_store(torch.tensor([-5.0, -1280.0, 7.0, 0.0], dtype=torch.float64), act=True)
+    assert got.float().tolist() == [-1.0, -256.0, 7.0, 0.0]
+    v = torch.tensor([-3.0], dtype=torch.float64)                 # -0.6000000089 -> bf16 -0.6015625 (RNE)
+    assert R.epi_store(v, act=True).float().item() == float(torch.tensor(-3.0 * R.F32_02).float().bfloat16())
+    # RNE ties to even: 257 lies between 256 and 258 -> 256; 259 between 258 and 260 -> 260; 1 + 2^-8 -> 1
+    assert R.epi_store(torch.tensor([257.0, 259.0, 1 + 2 ** -8, -257.0], dtype=torch.float64)).float().tolist() == \
+        [256.0, 260.0, 1.0, -256.0]
+    # the bias is added in fp32 before the rounding
+    assert R.epi_store(torch.tensor([256.0], dtype=torch.float64), torch.tensor([1.0])).float().item() == 256.0
+    assert R.epi_store(torch.tensor([256.0], dtype=torch.float64), torch.tensor([3.0])).float().item() == 260.0
+    # fmaf(-1, 0.4f, 0.6f) = 0.6f - 0.4f exactly, which is neither 0.2 nor 0.2f; fmaf(1, 0.4f, 0.6f) rounds to 1.0f
+    m = (-1.0 * float(np.float32(0.4)) + float(np.float32(0.6)))
+    assert R.MASK_NEG == m == float(np.float32(m)) == 6710887 * 2.0 ** -25 and R.MASK_NEG != R.F32_02
+    assert float(np.float32(1.0 * float(np.float32(0.4)) + float(np.float32(0.6)))) == 1.0
+    act = torch.tensor([-1.0, 0.0, -0.0, 2.0]).bfloat16()       # +0 counts positive, -0 negative (its sign bit)
+    z = torch.tensor([5.0, 5.0, 5.0, 5.0], dtype=torch.float64)
+    want = float(torch.tensor(5.0 * R.MASK_NEG).float().bfloat16())
+    assert R.epi_mask(z, act).float().tolist() == [want, 5.0, want, 5.0]
+    assert R.epi_mask(z, None).float().tolist() == [5.0] * 4
+    # head: (a > 0 ? 1 : 0.2f) - there +0 takes 0.2f, unlike the sign-bit masks
+    a = torch.tensor([0.0, 1.0]).bfloat16()
+    assert R.epi_head_dz(torch.tensor([5.0, 5.0], dtype=torch.float64), a).float().tolist() == \
+        [float(torch.tensor(5.0 * R.F32_02).float().bfloat16()), 5.0]
+    # pool backward: dp goes to the first maximum of each window, -0 + (+0) = +0, then the sign mask
+    a = torch.tensor([[1.0, 3.0], [3.0, -1.0]]).reshape(1, 2, 2, 1).expand(1, 2, 2, 32).contiguous().bfloat16()
+    dskip = torch.tensor([[-0.0, 1.0], [2.0, 4.0]]).reshape(1, 2, 2, 1).expand(1, 2, 2, 32).contiguous().bfloat16()
+    dp = torch.full((1, 1, 1, 32), 8.0).bfloat16()
+    got = R.epi_pool_bwd(a, dskip, dp)[0, :, :, 0]
+    assert _bits(got.reshape(-1)) == _bits(torch.tensor([0.0, 9.0, 2.0, float(torch.tensor(4.0 * R.MASK_NEG).float())
+                                                          ]).bfloat16())
+    # the exact rule: +0 and -0 are equal, one ulp is not, a NaN never is
+    want = torch.tensor([0.0, 1.0, 2.0]).bfloat16()
+    got = torch.tensor([-0.0, 1.0 + 2 ** -7, float('nan')]).bfloat16()
+    mask = torch.tensor([True, True, True])
+    assert R.exact_rule(got, want, mask) == 2 and R.exact_rule(got, want, torch.tensor([True, False, False])) == 0
+
+
+def _sum_f32(vals, order):
+    """vals (float64, exactly float32) summed in float32 in one of three orders"""
+    v = vals.float()
+    if order == 'forward':
+        acc = torch.zeros((), dtype=torch.float32)
+        for t in v:
+            acc = acc + t
+        return acc.item()
+    if order == 'reversed':
+        return _sum_f32(vals.flip(0), 'forward')
+    while v.numel() > 1:                                           # pairwise
+        if v.numel() % 2:
+            v = torch.cat([v, torch.zeros(1)])
+        v = v[0::2] + v[1::2]
+    return v.item()
+
+
+def test_exactness_witness_at_the_bound():
+    """integers with S just below 2^24 sum exactly in float32 in every order; just above, some order rounds"""
+    g = torch.Generator().manual_seed(9)
+    for trial in range(20):
+        k = 256
+        vals = torch.randint(1, 2 ** 16, (k,), generator=g).double() * torch.where(torch.rand(k, generator=g) < 0.5, -1.0, 1.0)
+        vals *= (2.0 ** 24 - 1 - 8 * trial) / vals.abs().sum()
+        vals = vals.trunc()
+        S = vals.abs().sum()
+        assert S < 2 ** 24 and R.exact_mask(S.reshape(1), R.grid(vals)).item()
+        for order in ('forward', 'reversed', 'pairwise'):
+            assert _sum_f32(vals, order) == vals.sum().item(), (trial, order)
+    # past the bound: 2^24 + 1 is not a float32, so 2^24 - 1 + 1 + 1 in order rounds and reversed does not
+    vals = torch.tensor([2.0 ** 24 - 1, 1.0, 1.0, -2.0 ** 23], dtype=torch.float64)
+    assert not R.exact_mask(vals.abs().sum().reshape(1), R.grid(vals)).item()
+    sums = {o: _sum_f32(vals, o) for o in ('forward', 'reversed', 'pairwise')}
+    assert sums['forward'] != vals.sum().item() or sums['reversed'] != vals.sum().item() or \
+        sums['pairwise'] != vals.sum().item(), sums
+
+
+def test_planted_faults_fail_the_exact_rule():
+    """float64 references of integer data with a planted fault: the exact rule rejects each one; the tolerance gates'
+    view of the same fault is printed (pytest -s)"""
+    g = torch.Generator().manual_seed(10)
+    x = torch.randint(0, 4, (2, 32, 64, 64), generator=g).double().bfloat16()
+    dz = (torch.randint(0, 2, (2, 32, 64, 32), generator=g).double() * 2 - 1) * 2.0 ** -16
+    dz = dz.bfloat16()
+    dW, S, db, Sb = R.conv_wgrad(x, dz)
+    q = R.grid(x) + R.grid(dz)
+    assert R.exact_mask(S, q).all() and R.exact_mask(Sb, R.grid(dz)).all()
+    faults = {}
+    # one 16-pixel row dropped from the weight-gradient sum
+    dzd = dz.clone()
+    dzd[1, 20, 16:32, :] = 0
+    faults['wgrad: one 16-pixel row dropped'] = (R.conv_wgrad(x, dzd)[0].float(), dW, S, q)
+    # one bias-gradient column zeroed
+    dbf = db.clone()
+    dbf[7] = 0
+    faults['bias grad: one column zeroed'] = (dbf.float(), db, Sb, R.grid(dz))
+    # one tap swapped in one 32-channel block (of a conv fprop)
+    w = torch.randint(0, 2, (32, 32, 3, 3), generator=g).float()
+    z, Sz = R.conv_fprop(x[..., :32], w, None, act=False)
+    ws = w.clone()
+    ws[:, :, 0, 0], ws[:, :, 2, 2] = w[:, :, 2, 2], w[:, :, 0, 0]
+    zs, _ = R.conv_fprop(x[..., :32], ws, None, act=False)
+    qz = R.grid(x) + R.grid(R.bf(w))
+    faults['fprop: taps (0,0) and (2,2) swapped'] = (R.epi_store(zs, act=True), R.epi_store(z, act=True), Sz, qz)
+    # one bf16 element off by one ulp
+    y = R.epi_store(z, act=True)
+    yb = y.clone()
+    yb.view(torch.int16)[0, 5, 5, 3] += 1
+    faults['bf16: one element one ulp off'] = (yb, y, Sz, qz)
+    for what, (got, want, S_, q_) in faults.items():
+        mask = R.exact_mask(S_, q_)
+        assert mask.all(), what
+        bad = R.exact_rule(got, want.double() if got.dtype == torch.float32 else want, mask)
+        assert bad > 0, what
+        r = want.double() if want.dtype != torch.float64 else want
+        rel, mx, _ = R.f32_rule(got.double(), r, S_)
+        print('%-40s exact rule: %d elements differ; tolerance view: rel-L2 %.3g, max-abs / max|r| %.3g'
+              % (what, bad, rel, mx))
 
 
 def test_rules_on_known_errors():

@@ -21,6 +21,7 @@ WGRAD_MAX_ABS = {'conv3x3_wgrad_thin<32,32>': 3.2e-6, 'conv3x3_wgrad_thin<32,64>
                  'conv3x3_wgrad_thin<64,32>': 3e-6, 'conv3x3_wgrad_thin<64,64>': 2.9e-6,
                  'wgrad_gemm<32>': 2.4e-6, 'wgrad_gemm<64>': 1.7e-6, 'wgrad_gemm<128>': 1.3e-6}
 BIG = 1000.0                   # scale of the odd images
+BIG_EXACT = 1024.0             # the same on integer operands: a power of two keeps them on the integer grid
 
 STATS = defaultdict(lambda: defaultdict(float))     # kernel -> worst measured value per statistic
 
@@ -30,6 +31,21 @@ def operand(torch, g, n, h, w, pitch, big_odd=True):
     scale = torch.ones(n, 1, 1, 1, device='cuda')
     scale[(1 if big_odd else 0)::2] = BIG
     return (torch.randn(n, h, w, pitch, device='cuda', generator=g) * scale).bfloat16()
+
+
+def int_operand(torch, g, n, h, w, pitch, big_odd=True, p=2.0 / 3):
+    """bf16 NHWC [n,h,w,pitch] of integers in {-1, 0, 1}, each non-zero with probability p, the odd (or even) images
+    x BIG_EXACT"""
+    scale = torch.ones(n, 1, 1, 1, device='cuda')
+    scale[(1 if big_odd else 0)::2] = BIG_EXACT
+    u = torch.rand(n, h, w, pitch, device='cuda', generator=g)
+    v = torch.where(u < p / 2, -1.0, torch.where(u < p, 1.0, 0.0))
+    return (v * scale).bfloat16()
+
+
+def int_weights(torch, g, *shape):
+    """fp32 integers in {-1, 0, 1}"""
+    return torch.randint(-1, 2, shape, device='cuda', generator=g).float()
 
 
 def output(torch, n, h, w, pitch):
@@ -57,6 +73,20 @@ def prims_traced(torch, call, expect, where, state=()):
     return got[-1]
 
 
+def _provable(kernel, where, got, want, S, q):
+    """the exact rule (tests/launch_check.py Step.provable) -> the share of the output that was provable"""
+    from tests.launch_ref import exact_mask, exact_rule
+    mask = exact_mask(S, q)
+    n = int(mask.sum().item())
+    st = STATS['provable ' + kernel]
+    st['elements'] += mask.numel()
+    st['exact'] += n
+    st['share'] = st['exact'] / st['elements']
+    bad = exact_rule(got, want, mask) if n else 0
+    assert bad == 0, '%s (%s): %d of %d provable elements differ' % (where, kernel, bad, n)
+    return n / mask.numel()
+
+
 def _bf16_check(kernel, where, got, r, S):
     from tests.launch_ref import bf16_rule
     ratio, mism, finite = bf16_rule(got, r, S)
@@ -77,62 +107,87 @@ def _f32_check(kernel, where, got, r, S):
         '%s (%s): rel-L2 %.3g, max-abs / max|r| %.3g' % (where, kernel, rel, mx)
 
 
-def run_case(torch, c, seed):
-    """one primitive call of case c, traced, then checked against its float64 reference and its guards"""
+def run_case(torch, c, seed, integer=False):
+    """one primitive call of case c, traced, then checked against its float64 reference and its guards; with `integer`
+    on integer operands (int_operand, int_weights), sparse enough that every output element is provable.  -> the share
+    of the output the exact rule covered"""
     from eld_b200 import prims
     import tests.launch_ref as R
     g = torch.Generator(device='cuda').manual_seed(seed)
     kern = T.kernel(c)[0]
     where = T.case_id(c)
     fine = c.op.startswith('deconv')
+    if integer:
+        dense = lambda *a, **k: int_operand(torch, g, *a, **k)                     # noqa: E731
+        weights = lambda *shape, div: int_weights(torch, g, *shape)                # noqa: E731
+    else:
+        dense = lambda *a, big_odd=True, p=None: operand(torch, g, *a, big_odd=big_odd)  # noqa: E731
+        weights = lambda *shape, div: torch.randn(*shape, device='cuda', generator=g) / div  # noqa: E731
     if c.op.endswith('wgrad'):
-        x = operand(torch, g, c.n, c.h, c.w, c.x_pitch)
+        # every product is at most BIG_EXACT and an output sums n h w of them: sparse enough for S < 2^22 or so
+        p = min(2.0 / 3, (2.0 ** 22 / (c.n * c.h * c.w * BIG_EXACT)) ** 0.5)
+        x = dense(c.n, c.h, c.w, c.x_pitch, p=p)
         f = 2 if fine else 1
         # the second operand is large on the EVEN images: a product across an image border is BIG^2
-        q = operand(torch, g, c.n, f * c.h, f * c.w, c.y_pitch, big_odd=False)
+        q = dense(c.n, f * c.h, f * c.w, c.y_pitch, big_odd=False, p=p)
         xs, qs = x[..., c.x_c0:c.x_c0 + c.ci], q[..., c.y_c0:c.y_c0 + c.co]
         r, S, _, _ = (R.deconv_wgrad if fine else R.conv_wgrad)(xs, qs)
-        dw0 = torch.randn(r.shape, device='cuda', generator=g) * r.abs().max().float()
+        if integer:
+            dw0 = torch.randint(-8, 9, r.shape, device='cuda', generator=g).float()
+        else:
+            dw0 = torch.randn(r.shape, device='cuda', generator=g) * r.abs().max().float()
         out = Guarded(torch, r.numel(), 256)
         dw = out.view.view(r.shape)
         dw.copy_(dw0)
         wgrad = prims.deconv2x2_wgrad if fine else prims.conv3x3_wgrad
         prims_traced(torch, lambda: wgrad(x, c.x_c0, c.ci, q, c.y_c0, c.co, dw), {kern: 1}, where, state=(dw,))
         assert out.written_guards() == 0, '%s: dW guard written' % where
-        _f32_check(kern, where, dw, r + dw0.double(), S + dw0.double().abs())
-        return
+        r, S = r + dw0.double(), S + dw0.double().abs()
+        _f32_check(kern, where, dw, r, S)
+        return _provable(kern, where, dw, r, S, min(R.grid(xs) + R.grid(qs), R.grid(dw0)))
     ih, iw = (2 * c.h, 2 * c.w) if c.op == 'deconv.dgrad' else (c.h, c.w)
     oh, ow = (2 * c.h, 2 * c.w) if c.op == 'deconv' else (c.h, c.w)
-    x = operand(torch, g, c.n, ih, iw, c.x_pitch)
+    x = dense(c.n, ih, iw, c.x_pitch)
     xs = x[..., c.x_c0:c.x_c0 + c.ci]
     out, y = output(torch, c.n, oh, ow, c.y_pitch)
-    aux = operand(torch, g, c.n, c.h, c.w, c.aux_pitch) if c.act == prims.ACT_MASK else None
+    aux = dense(c.n, c.h, c.w, c.aux_pitch) if c.act == prims.ACT_MASK else None
     auxs = aux[..., c.aux_c0:c.aux_c0 + c.co] if aux is not None else None
+    b = None
     if c.op == 'conv':
-        W = torch.randn(c.co, c.ci, 3, 3, device='cuda', generator=g) / (3 * c.ci ** 0.5)
-        b = torch.randn(c.co, device='cuda', generator=g) if c.bias else None
+        W = weights(c.co, c.ci, 3, 3, div=3 * c.ci ** 0.5)
+        b = weights(c.co, div=1.0) if c.bias else None
         wp = prims.pack_weights(W, prims.PACK_CONV_FPROP)
         call = lambda: prims.conv3x3(x, c.x_c0, c.ci, wp, b, y, c.y_c0, c.co, act=c.act)  # noqa: E731
-        r, S = R.conv_fprop(xs, W, b, act=c.act == prims.ACT_LRELU)
+        z, S = R.conv_fprop(xs, W, b, act=False)
+        lrelu = c.act == prims.ACT_LRELU
+        r, want = (R.lrelu(z) if lrelu else z), R.epi_store(z, act=lrelu)
     elif c.op == 'conv.dgrad':
-        W = torch.randn(c.ci, c.co, 3, 3, device='cuda', generator=g) / (3 * c.ci ** 0.5)
+        W = weights(c.ci, c.co, 3, 3, div=3 * c.ci ** 0.5)
         wp = prims.pack_weights(W, prims.PACK_CONV_DGRAD)
         call = lambda: prims.conv3x3(x, c.x_c0, c.ci, wp, None, y, c.y_c0, c.co, act=c.act, aux=aux,  # noqa: E731
                                      aux_c0=c.aux_c0)
-        r, S = R.conv_dgrad(xs, W, auxs)
+        z, S = R.conv_dgrad(xs, W)
     elif c.op == 'deconv':
-        Wt = torch.randn(c.ci, c.co, 2, 2, device='cuda', generator=g) / c.ci ** 0.5
-        b = torch.randn(c.co, device='cuda', generator=g) if c.bias else None
-        wp = prims.pack_weights(Wt, prims.PACK_DECONV_FPROP)
+        W = weights(c.ci, c.co, 2, 2, div=c.ci ** 0.5)
+        b = weights(c.co, div=1.0) if c.bias else None
+        wp = prims.pack_weights(W, prims.PACK_DECONV_FPROP)
         call = lambda: prims.deconv2x2(x, c.x_c0, c.ci, wp, b, y, c.y_c0, c.co)  # noqa: E731
-        r, S = R.deconv_fprop(xs, Wt, b)
+        r, S = R.deconv_fprop(xs, W, b)
+        want = R.epi_store(r)
     else:
-        Wt = torch.randn(c.co, c.ci, 2, 2, device='cuda', generator=g) / c.ci ** 0.5
-        wp = prims.pack_weights(Wt, prims.PACK_DECONV_DGRAD)
+        W = weights(c.co, c.ci, 2, 2, div=c.ci ** 0.5)
+        wp = prims.pack_weights(W, prims.PACK_DECONV_DGRAD)
         call = lambda: prims.deconv2x2_dgrad(x, c.x_c0, c.ci, wp, y, c.y_c0, c.co, act=c.act, aux=aux,  # noqa: E731
                                              aux_c0=c.aux_c0)
-        r, S = R.deconv_dgrad(xs, Wt, auxs)
+        z, S = R.deconv_dgrad(xs, W)
+    if c.op.endswith('dgrad'):
+        want = R.epi_mask(z, auxs)
+        s = R.slope(auxs) if auxs is not None else 1.0
+        r, S = z * s, S * s
     prims_traced(torch, call, {kern: 1}, where)
     bad = written(torch, out, y, c.y_c0, c.co)
     assert bad == 0, '%s: %d guard elements written' % (where, bad)
-    _bf16_check(kern, where, y[..., c.y_c0:c.y_c0 + c.co], r, S)
+    got = y[..., c.y_c0:c.y_c0 + c.co]
+    _bf16_check(kern, where, got, r, S)
+    q = R.grid(xs) + R.grid(R.bf(W))
+    return _provable(kern, where, got, want, S, q if b is None else min(q, R.grid(b)))
