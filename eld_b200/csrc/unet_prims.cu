@@ -312,7 +312,11 @@ int init_gemm_kernels(eld_ctx* ctx)
     return ELD_OK;
 }
 
-// the thin 3x3 weight gradients (cin, cout in {32, 64}): one halo load per pixel tile for all nine taps (wgrad_thin.cuh)
+// the thin 3x3 weight gradients (cin, cout each 32 or 64) and the engine's deep ones (multiples of 64): one halo load per
+// pixel tile for all nine taps (wgrad_thin.cuh), in KC x NT channel blocks of at most 64 x 64 (the nine taps' f32
+// accumulators fill the consumers' registers at 64 x 64).  Grid = blocks x splits: each block gets the same number of
+// pixel-tile ranges, as many as fill one wave of CTAs (blocks are powers of two up to 64 in the U-Net: 128 to 132
+// CTAs), and no range is empty.
 static int launch_wgrad_thin(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
 {
     // the [tap][ci][co] flush and the bias gradient add four contiguous floats at a time
@@ -323,21 +327,24 @@ static int launch_wgrad_thin(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
     WgradThinParams p{};
     p.n_img = op.n_img; p.H = op.H; p.W = op.W;
     p.tiles_x = op.W / 16; p.tiles_y = (op.H + 7) / 8;       // H % 8 == 4: the last tile row overhangs, zero-filled
-    p.p_c0 = op.p_c0; p.q_c0 = op.q_c0; p.p_ch = op.p_ch; p.q_ch = op.q_ch;
+    p.p_c0 = op.p_c0; p.q_c0 = op.q_c0; p.cin = op.p_ch; p.cout = op.q_ch;
+    const int kc = std::min(op.p_ch, 64), nt = std::min(op.q_ch, 64);
+    p.ci_blocks = op.p_ch / kc; p.co_blocks = op.q_ch / nt;
     p.dw = op.dw; p.out_tco = op.out_tco; p.db = op.db;
-    const int slot_bytes = wgrad_thin_slot_bytes(op.p_ch, op.q_ch);
+    const int slot_bytes = wgrad_thin_slot_bytes(kc, nt);
     int stages = (kThinSmemBytes - 1024 - 256) / slot_bytes;
     if (stages > kThinMaxSlots) stages = kThinMaxSlots;
     ELD_REQUIRE(stages >= 2, "thin wgrad tile: no room for two stages");
     p.stages = stages;
 
     CUtensorMap tmP, tmQ;
-    { int rc = encode_nhwc(ctx, &tmP, op.p, op.p_pitch, op.n_img, op.H, op.W, op.p_ch, kConvTileW, kHaloRows); if (rc) return rc; }
-    { int rc = encode_nhwc(ctx, &tmQ, op.q, op.q_pitch, op.n_img, op.H, op.W, op.q_ch, 16, 8); if (rc) return rc; }
+    { int rc = encode_nhwc(ctx, &tmP, op.p, op.p_pitch, op.n_img, op.H, op.W, kc, kConvTileW, kHaloRows); if (rc) return rc; }
+    { int rc = encode_nhwc(ctx, &tmQ, op.q, op.q_pitch, op.n_img, op.H, op.W, nt, 16, 8); if (rc) return rc; }
     const size_t smem = 1024 + (size_t)stages * slot_bytes + 256;
     const int total_tiles = op.n_img * p.tiles_x * p.tiles_y;
-    return launch(ctx, kWgradThin[op.q_ch / 64][op.p_ch / 64], std::min(total_tiles, ctx->num_sms), kWgThinThreads, smem, st,
-                  tmP, tmQ, p);
+    const int blocks = p.ci_blocks * p.co_blocks;
+    p.splits = std::min(std::max(1, ctx->num_sms / blocks), total_tiles);
+    return launch(ctx, kWgradThin[nt / 64][kc / 64], blocks * p.splits, kWgThinThreads, smem, st, tmP, tmQ, p);
 }
 
 int launch_wgrad(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
@@ -345,7 +352,13 @@ int launch_wgrad(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
     ELD_REQUIRE(op.H % 4 == 0 && op.W % 16 == 0, "wgrad tile: H=%d must be a multiple of 4 and W=%d of 16", op.H, op.W);
     ELD_REQUIRE(op.p_ch % 32 == 0 && op.q_ch % 32 == 0, "wgrad tile: channel counts must be multiples of 32");
     ELD_REQUIRE(op.out_tco == 0 || op.mode == WG_CONV, "wgrad tile: the [tap][ci][co] layout is a conv layout");
-    if (op.mode == WG_CONV && (op.p_ch == 32 || op.p_ch == 64) && (op.q_ch == 32 || op.q_ch == 64))
+    // the 3x3 tile of one halo per pixel tile: the thin layers, and the deep ones (cin, cout multiples of 64) in 64 x 64
+    // channel blocks when the gradient is the engine's [tap][ci][co] staging, where a block flushes rows of 64
+    // contiguous floats with 16-byte red.add.  wgrad_gemm: the deconvolutions, and the other 3x3 shapes of the C ABI,
+    // whose OIHW gradient would take a block's flush as scalar atomics at a stride of 9 floats.
+    const bool thin = (op.p_ch == 32 || op.p_ch == 64) && (op.q_ch == 32 || op.q_ch == 64);
+    const bool blocked = op.out_tco && op.p_ch % 64 == 0 && op.q_ch % 64 == 0;
+    if (op.mode == WG_CONV && (thin || blocked))
         return launch_wgrad_thin(ctx, op, st);
     WgradParams p{};
     p.n_img = op.n_img; p.H = op.H; p.W = op.W;

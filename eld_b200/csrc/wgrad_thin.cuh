@@ -1,16 +1,22 @@
-// wgrad_thin.cuh - wgmma weight-gradient tile for the thin 3x3 convolutions (cin and cout in {32, 64}): the
-// full- and half-resolution layers, where the generic tile (wgrad_gemm.cuh) loads every pixel of X once per filter tap.
+// wgrad_thin.cuh - wgmma weight-gradient tile of the 3x3 convolutions whose cin and cout are each 32, 64 or a multiple of
+// 64: one halo load per pixel tile for all nine taps, where the generic tile (wgrad_gemm.cuh) loads every pixel of X once
+// per filter tap.
 //
 //   D[(tap, ci) x co] (f32, registers)  =  sum over pixels p   X[p + tap shift, ci] * dZ[p, co]
 //
-// Grid    = one persistent CTA per SM; CTA b owns tiles [b T / G, (b + 1) T / G) of the T 8 x 16 pixel tiles (a
-//           contiguous run, so vertically neighbouring halos meet in L2) and the layer's whole dW (+ db) for them.
-// P (X)   = the halo of each tile (tile.cuh), as the fprop thin tile loads it.  Consumed MN-major: a tap starts a whole
-//           number of swizzle atoms into the slot (halo_tap_off), and k16 step k is tile row k.  KC = 64: one tap = one
-//           m64 unit (9 units).  KC = 32: two taps share one m64 unit, the second 32 rows at the descriptor's LBO: (dy = -1, dx) + (0, dx) at LBO = 1 KB for each dx, (1, -1) + (1, 0)
+// blocks  = a CTA computes one KC x NT channel block (ci0 .. ci0 + KC - 1) x (co0 .. co0 + NT - 1) of the layer's
+//           (cin / KC) x (cout / NT) blocks; the thin layers (cin, cout in {32, 64}) are one block.
+// Grid    = blocks x splits, the block index fastest: CTA b computes block b % blocks over split s = b / blocks, which owns
+//           tiles [s T / splits, (s + 1) T / splits) of the T 8 x 16 pixel tiles (a contiguous run, so vertically
+//           neighbouring halos meet in L2).  The CTAs resident together walk the same pixel range, so one halo / dZ tile
+//           read from HBM serves every channel block from L2.
+// P (X)   = the halo of each tile (tile.cuh), as the fprop thin tile loads it, at channel p_c0 + ci0.  Consumed MN-major:
+//           a tap starts a whole number of swizzle atoms into the slot (halo_tap_off), and k16 step k is tile row k.
+//           KC = 64: one tap = one m64 unit (9 units).  KC = 32: two taps share one m64 unit, the second 32 rows at the
+//           descriptor's LBO: (dy = -1, dx) + (0, dx) at LBO = 1 KB for each dx, (1, -1) + (1, 0)
 //           and (1, 0) + (1, 1) at LBO = one box (5 units; the first half of the last duplicates a tap and is dropped).
-// Q (dZ)  = one {NT, 16, 8} box per tile, MN-major.  Its column sums are the bias gradient, summed from shared memory
-//           while the MMAs run.
+// Q (dZ)  = one {NT, 16, 8} box per tile at channel q_c0 + co0, MN-major.  Its column sums are the bias gradient, summed
+//           from shared memory while the MMAs run (by the ci-block-0 CTAs only).
 // roles   = warpgroup 0: TMA producer (one thread) | warpgroups 1, 2 consume every stage and split the m64 units
 //           (5 / 4 at KC = 64, 3 / 2 at KC = 32).  There is no per-tile epilogue: at the end each consumer adds its f32
 //           units into the gradient with vector red.global.add.  The 160 accumulator registers of (64 -> 64) need more
@@ -27,9 +33,11 @@ struct WgradThinParams {
     int n_img, H, W;
     int tiles_x, tiles_y;
     int p_c0, q_c0;
-    int p_ch, q_ch;           // cin, cout (= KC, NT)
+    int cin, cout;            // the layer's channel counts: the strides of dw
+    int ci_blocks, co_blocks; // cin / KC, cout / NT
+    int splits;               // pixel-tile ranges per channel block
     int stages;
-    float* dw;                // out_tco: [tap][ci][co]; otherwise OIHW [co][ci][3][3]
+    float* dw;                // out_tco: [tap][cin][cout]; otherwise OIHW [cout][cin][3][3]
     int out_tco;
     float* db;                // optional: db[co] += sum over pixels of dZ
 };
@@ -63,10 +71,11 @@ __device__ __forceinline__ int wg_unit_tap(int u, int m)
     return u < 3 ? 3 * half + u : (u == 3 ? 6 + half : (half ? 8 : -1));
 }
 
-// One consumer warpgroup: units U0 .. U0 + NU - 1 of every stage, accumulated over the CTA's tiles, then flushed.
+// One consumer warpgroup: units U0 .. U0 + NU - 1 of every stage, accumulated over the CTA's tiles, then flushed into
+// channel block (ci0, co0) of the gradient.
 template <int NT, int KC, int U0, int NU>
 __device__ __forceinline__ void wgrad_thin_consume(const WgradThinParams& p, uint8_t* smem, uint64_t* full, uint64_t* empty,
-                                                   int ntiles, int bt)
+                                                   int ntiles, int bt, int ci0, int co0)
 {
     constexpr int q_off = halo_slot_bytes(KC), slot_bytes = wgrad_thin_slot_bytes(KC, NT);   // dZ box / slot
     constexpr int p_row = KC * 2, q_row = NT * 2;
@@ -83,7 +92,7 @@ __device__ __forceinline__ void wgrad_thin_consume(const WgradThinParams& p, uin
     constexpr int CH = NT / 8, BR = 256 / CH;
     const int bc = bt % CH, br = bt / CH;
     const uint32_t bswz = NT == 64 ? (uint32_t)(br & 7) : (uint32_t)((br >> 1) & 3);   // BR is a multiple of 8
-    const bool bias_on = p.db != nullptr;
+    const bool bias_on = p.db != nullptr && ci0 == 0;     // one ci block sums db, or it would count cin / KC times
     float bsum[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) bsum[i] = 0.f;
@@ -139,7 +148,7 @@ __device__ __forceinline__ void wgrad_thin_consume(const WgradThinParams& p, uin
 #pragma unroll
             for (int i = 0; i < 8; ++i) bsum[i] += __shfl_xor_sync(0xffffffffu, bsum[i], o);
         if (lane < CH) {
-            float4* d = reinterpret_cast<float4*>(p.db + 8 * bc);
+            float4* d = reinterpret_cast<float4*>(p.db + co0 + 8 * bc);
             atomicAdd(d, make_float4(bsum[0], bsum[1], bsum[2], bsum[3]));
             atomicAdd(d + 1, make_float4(bsum[4], bsum[5], bsum[6], bsum[7]));
         }
@@ -161,25 +170,25 @@ __device__ __forceinline__ void wgrad_thin_consume(const WgradThinParams& p, uin
                 const int m = 16 * wq + (lane >> 2) + (odd ? 8 : 0);
                 const int tap = wg_unit_tap<KC>(U0 + u, m);
                 if (tap < 0) continue;
-                const int ci = m & (KC - 1), co = 8 * j + 2 * ((lane & 3) & ~1);
+                const int ci = ci0 + (m & (KC - 1)), co = co0 + 8 * j + 2 * ((lane & 3) & ~1);
                 const float4 v = odd ? make_float4(s0, s1, v10, v11) : make_float4(v00, v01, s0, s1);
-                atomicAdd(reinterpret_cast<float4*>(p.dw + ((size_t)tap * KC + ci) * NT + co), v);
+                atomicAdd(reinterpret_cast<float4*>(p.dw + ((size_t)tap * p.cin + ci) * p.cout + co), v);
             } else {
 #pragma unroll
                 for (int i = 0; i < 2; ++i) {
                     const int m = 16 * wq + (lane >> 2) + 8 * i;
                     const int tap = wg_unit_tap<KC>(U0 + u, m);
                     if (tap < 0) continue;
-                    const int ci = m & (KC - 1), co = 8 * j + 2 * (lane & 3);
-                    atomicAdd(p.dw + ((size_t)co * KC + ci) * 9 + tap, i ? v10 : v00);
-                    atomicAdd(p.dw + ((size_t)(co + 1) * KC + ci) * 9 + tap, i ? v11 : v01);
+                    const int ci = ci0 + (m & (KC - 1)), co = co0 + 8 * j + 2 * (lane & 3);
+                    atomicAdd(p.dw + ((size_t)co * p.cin + ci) * 9 + tap, i ? v10 : v00);
+                    atomicAdd(p.dw + ((size_t)(co + 1) * p.cin + ci) * 9 + tap, i ? v11 : v01);
                 }
             }
         }
     }
 }
 
-// NT = cout, KC = cin, each 32 or 64
+// NT x KC = the channel block (cout x cin of a thin layer), each 32 or 64
 template <int NT, int KC>
 __global__ void __launch_bounds__(kWgThinThreads, 1)
 conv3x3_wgrad_thin_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmQ,
@@ -194,10 +203,13 @@ conv3x3_wgrad_thin_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * slot_bytes);
     uint64_t* empty = full + p.stages;
 
+    const int blocks = p.ci_blocks * p.co_blocks;
+    const int blk = (int)blockIdx.x % blocks, split = (int)blockIdx.x / blocks;
+    const int ci0 = (blk / p.co_blocks) * KC, co0 = (blk % p.co_blocks) * NT;
     const int tiles_xy = p.tiles_x * p.tiles_y;
     const int total_tiles = p.n_img * tiles_xy;
-    const int t_begin = (int)((long long)blockIdx.x * total_tiles / gridDim.x);
-    const int t_end = (int)((long long)(blockIdx.x + 1) * total_tiles / gridDim.x);
+    const int t_begin = (int)((long long)split * total_tiles / p.splits);
+    const int t_end = (int)((long long)(split + 1) * total_tiles / p.splits);
 
     if (threadIdx.x == 0) {
         ptx::prefetch_tmap(&tmP);
@@ -223,8 +235,8 @@ conv3x3_wgrad_thin_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_
                 uint8_t* sa = smem + (size_t)s * slot_bytes;
                 ptx::mbar_wait(&empty[s], ph ^ 1u);
                 ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)slot_bytes);
-                halo_load<KC>(sa, &tmP, &full[s], p.p_c0, x0, y0, img);
-                ptx::tma_load_5d(sa + halo_slot_bytes(KC), &tmQ, &full[s], p.q_c0, x0, y0, img, 0);
+                halo_load<KC>(sa, &tmP, &full[s], p.p_c0 + ci0, x0, y0, img);
+                ptx::tma_load_5d(sa + halo_slot_bytes(KC), &tmQ, &full[s], p.q_c0 + co0, x0, y0, img, 0);
                 if (++s == p.stages) { s = 0; ph ^= 1u; }
                 if (++tx == p.tiles_x) { tx = 0; if (++ty == p.tiles_y) { ty = 0; ++img; } }
             }
@@ -236,8 +248,8 @@ conv3x3_wgrad_thin_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_
     // broadcast from lane 0: the compiler then knows cg to be warp-uniform (no wgmma serialisation)
     const int cg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7) - 1, 0);
     const int bt = threadIdx.x - 128;
-    if (cg == 0) wgrad_thin_consume<NT, KC, 0, u_first>(p, smem, full, empty, t_end - t_begin, bt);
-    else wgrad_thin_consume<NT, KC, u_first, units - u_first>(p, smem, full, empty, t_end - t_begin, bt);
+    if (cg == 0) wgrad_thin_consume<NT, KC, 0, u_first>(p, smem, full, empty, t_end - t_begin, bt, ci0, co0);
+    else wgrad_thin_consume<NT, KC, u_first, units - u_first>(p, smem, full, empty, t_end - t_begin, bt, ci0, co0);
 }
 
 }  // namespace eld
