@@ -49,6 +49,7 @@ def declare_engine(lib):
     lib.eld_adam_step_segments_capturable.argtypes = [vp, vp, vp, vp, vp, c.POINTER(sz), c.POINTER(vp), i32, vp, f32, f32,
                                                       f32, f32, f32, vp]
     lib.eld_unet_set_loss.argtypes = [vp, i32]
+    lib.eld_unet_set_accumulate.argtypes = [vp, i32]
     lib.eld_clock_probe.argtypes = [vp, vp, vp]
     lib.eld_unet_profile.argtypes = [vp, i32]
     lib.eld_unet_profile_read.argtypes = [vp, i32, c.c_char_p, vp, vp, vp, c.POINTER(i32)]

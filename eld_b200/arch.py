@@ -285,25 +285,35 @@ class UNetSeeInDark(nn.Module):
 
     loss_kind = 'l1'      # 'l1' (nn.L1Loss, the reference default) or 'l2' (nn.MSELoss) - models/losses.py:29-36
 
-    def train_step(self, x, target, loss_out=None):
+    def train_step(self, x, target, loss_out=None, accumulate=False):
         """forward + pixel loss + backward in one launch sequence.  Fills self.flat_grads (== every trainable
         parameter's .grad) and returns (out, loss) with loss a 0-dim cuda tensor (no host sync).  Parameters with
         requires_grad == False are frozen: no gradient is computed for them, their .grad is None and their range of
         flat_grads reads zero.  An exchange an earlier train_step_ddp left in flight is joined first (a stream wait): the
-        step's memset and weight-gradient writes must not race with its all-reduces."""
+        step's memset and weight-gradient writes must not race with its all-reduces.
+        accumulate=True adds this call's gradients to flat_grads instead (gradient accumulation over micro-batches, as
+        loss.backward() adds into .grad); `loss` is still this call's own.  The launches are those of a plain step
+        without the memset of flat_grads.  A frozen range is never written, so a window of accumulating calls must keep
+        the previous call's freeze mask: ValueError if the trainable flags changed."""
         n, _, h, w = x.shape
         assert x.is_cuda and x.dtype == torch.float32 and x.shape[1] == self.in_channels
         assert target.shape == (n, self.out_channels, h, w) and target.dtype == torch.float32
+        flags = [p.requires_grad for p in self.parameters()]
+        prev = getattr(self, '_last_flags', None)
+        if accumulate and prev is not None and prev != flags:
+            raise ValueError('train_step(accumulate=True): the trainable parameters changed since the previous call; '
+                             'a window of accumulated gradients uses one freeze mask')
         self.join_allreduce()
         x, target = x.contiguous(), target.contiguous()
         out = torch.empty_like(target)
         loss = loss_out if loss_out is not None else torch.empty((), dtype=torch.float32, device=x.device)
-        flags = self._last_flags = [p.requires_grad for p in self.parameters()]
+        self._last_flags = flags
         plan = self._plan(n, h, w, True)
         plan.owner = None              # the step overwrites the built-in forward state: a call still needing it recomputes
         self._set_trainable(plan[0], flags, False)
         self._sync_grads(flags)
         _lib.check(_lib.load().eld_unet_set_loss(plan[0], 1 if self.loss_kind == 'l2' else 0), 'eld_unet_set_loss')
+        _lib.check(_lib.load().eld_unet_set_accumulate(plan[0], int(bool(accumulate))), 'eld_unet_set_accumulate')
         _lib.check(_lib.load().eld_unet_train_step(plan[0], self._flat.data_ptr(), x.data_ptr(),
                                                    target.data_ptr(), out.data_ptr(), self._flat_grad.data_ptr(),
                                                    loss.data_ptr(), _st()), 'eld_unet_train_step')
@@ -318,13 +328,16 @@ class UNetSeeInDark(nn.Module):
         k = _lib.load().eld_unet_grad_buckets_io(self.in_channels, self.out_channels, arr, 16)
         return [(int(arr[2 * i]), int(arr[2 * i + 1])) for i in range(k)]
 
-    def train_step_ddp(self, x, target, loss_out=None, group=None, timeline=None):
+    def train_step_ddp(self, x, target, loss_out=None, group=None, timeline=None, accumulate=False, sync=True):
         """train_step + SUM all-reduce of the flat gradient, bucket by bucket on a side stream: bucket k's NCCL kernel
         waits only for the event the engine records when that bucket is final, so the decoder and bottleneck
         gradients travel while the encoder's backward still runs.  The all-reduces are left in flight
         (_pending_allreduce): the next FusedAdam.step joins them bucket by bucket, or the next train_step, autograd
         backward or zero_grad joins them all, whichever comes first, so a step that skips the optimizer (a non-finite
-        loss) or a plain step after this one never races with the exchange.  No host synchronisation."""
+        loss) or a plain step after this one never races with the exchange.  No host synchronisation.
+        Gradient accumulation (DistributedDataParallel.no_sync()): accumulate as in train_step; sync=False runs the
+        local step alone, with no bucket wait and no all-reduce, so a window of k micro-batches calls this k - 1 times
+        with sync=False and once with sync=True, which exchanges the accumulated sum bucket by bucket."""
         import torch.distributed as dist
         n, _, h, w = x.shape
         eng = self._engine(n, h, w, True)
@@ -334,10 +347,12 @@ class UNetSeeInDark(nn.Module):
             self._ddp_ready = eng.value
             self._ddp_stream = torch.cuda.Stream(device=x.device)
             self._ddp_buckets = self.grad_buckets()
+        if not sync:
+            return self.train_step(x, target, loss_out=loss_out, accumulate=accumulate)
         ev = (lambda: torch.cuda.Event(enable_timing=True)) if timeline is not None else None
         if ev:
             timeline['step_start'] = ev(); timeline['step_start'].record()
-        out, loss = self.train_step(x, target, loss_out=loss_out)
+        out, loss = self.train_step(x, target, loss_out=loss_out, accumulate=accumulate)
         if ev:
             timeline['backward_end'] = ev(); timeline['backward_end'].record()
             timeline['buckets'] = []

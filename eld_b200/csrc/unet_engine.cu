@@ -72,10 +72,12 @@ static int bucket_end(int k) { return k == 0 ? kNumLayers : kBucketFirst[k - 1];
 
 static_assert(kNumLayers <= kPackMaxEntries, "the packing table (unet_prims.h) holds one entry per layer at most");
 
-// staging [tap][ci][co] -> PyTorch OIHW [co][ci][tap]; one block per (32 co x 32 ci) tile of one layer
+// staging [tap][ci][co] -> PyTorch OIHW [co][ci][tap]; one block per (32 co x 32 ci) tile of one layer.  accumulate: add
+// the staged gradient to what grads holds (eld_unet_set_accumulate) instead of storing it.  Each element of a layer's
+// weight range has one owner thread and no other launch of the step writes that range, so a plain read-modify-write.
 __global__ void __launch_bounds__(256)
 wgrad_permute_kernel(const float* __restrict__ gtmp, float* __restrict__ grads, const __grid_constant__ PackTable T,
-                     int tile_begin, int tile_end)
+                     int tile_begin, int tile_end, bool accumulate)
 {
     // blocks [0, tile_end - tile_begin) move the table tiles [tile_begin, tile_end) (one gradient bucket)
     __shared__ float tile[9][32][33];
@@ -83,7 +85,7 @@ wgrad_permute_kernel(const float* __restrict__ gtmp, float* __restrict__ grads, 
     if (gtile >= tile_end) return;
     int t;
     const PackEntry& e = T.e[find_entry(T, gtile, t)];
-    if (e.deconv || !e.perm) return;     // a frozen weight's range of grads keeps the zeros of the step's memset
+    if (e.deconv || !e.perm) return;     // a frozen weight's range of grads is never written
     const int ct = e.cout / 32;
     {
         const int co0 = (t % ct) * 32, ci0 = (t / ct) * 32;
@@ -104,13 +106,19 @@ wgrad_permute_kernel(const float* __restrict__ gtmp, float* __restrict__ grads, 
                     const int r = 4 * r4 + k, ci = r / 9, tap = r - ci * 9;
                     q[k] = tile[tap][ci][co];
                 }
-                *(reinterpret_cast<float4*>(grads + e.src + ((size_t)(co0 + co) * e.cin + ci0) * 9) + r4) = make_float4(q[0], q[1], q[2], q[3]);
+                float4* d = reinterpret_cast<float4*>(grads + e.src + ((size_t)(co0 + co) * e.cin + ci0) * 9) + r4;
+                if (accumulate) {
+                    const float4 p = *d;
+                    q[0] += p.x; q[1] += p.y; q[2] += p.z; q[3] += p.w;
+                }
+                *d = make_float4(q[0], q[1], q[2], q[3]);
             }
         } else {
             for (int i = threadIdx.x; i < 32 * 288; i += 256) {
                 const int co = i / 288, r = i - co * 288;
                 const int ci = r / 9, tap = r - ci * 9;
-                grads[e.src + ((size_t)(co0 + co) * e.cin + ci0 + ci) * 9 + tap] = tile[tap][ci][co];
+                float* d = grads + e.src + ((size_t)(co0 + co) * e.cin + ci0 + ci) * 9 + tap;
+                *d = accumulate ? *d + tile[tap][ci][co] : tile[tap][ci][co];
             }
         }
     }
@@ -152,6 +160,7 @@ struct eld_unet {
     cudaEvent_t bucket_ev[kGradBuckets] = { nullptr, nullptr, nullptr, nullptr };
     int cin0 = 4, cout_last = 4; // channels of the frame in / out: 4 = packed raw, 3 = sRGB (ELD_model.py:377-389)
     int l2_loss = 0;             // 0: nn.L1Loss (the reference default, losses.py:31-32), 1: nn.MSELoss (losses.py:33-34)
+    bool accumulate = false;     // eld_unet_train_step adds into grads instead of overwriting it (eld_unet_set_accumulate)
     bool dz1_1_final = false;    // dz1_1 holds the last backward's conv1_1 gradient: set by a backward, cleared by a forward
     // what the backward computes (eld_unet_set_trainable; default: everything).  train_w[l] / train_b[l]: layer l's
     // weight / bias requires grad; wgrad[l]: either does (one launch computes both).  reach[l]: the gradient of layer l's
@@ -447,6 +456,7 @@ struct Runner {
     const FwdState* s;           // the forward state this call writes (forward) or reads (backward)
     const float* params;
     cudaStream_t st;
+    bool accumulate = false;     // the permute adds the conv3x3 weight gradients into grads (an accumulating train step)
     eld_ctx* ctx() const { return u->ctx; }
     const __nv_bfloat16* wf(int i) const { return s->packed + u->L[i].wf_off; }
     const __nv_bfloat16* wd(int i) const { return s->packed + u->L[i].wd_off; }
@@ -636,7 +646,7 @@ struct Runner {
         const int t1 = u->perm_t1[per_bucket ? k : kGradBuckets];
         if (t1 > t0) {
             Scope sc(u, st, "weights", "gperm", 0.0, 0.0);
-            wgrad_permute_kernel<<<t1 - t0, 256, 0, st>>>(u->gtmp, g, u->table, t0, t1);
+            wgrad_permute_kernel<<<t1 - t0, 256, 0, st>>>(u->gtmp, g, u->table, t0, t1, accumulate);
             ELD_CHECK_CUDA(cudaGetLastError());
             count_launch(ctx());
         }
@@ -720,8 +730,8 @@ extern "C" int eld_unet_train_step(eld_unet* u, const float* params, const float
     ELD_REQUIRE(u->train, "eld_unet_train_step: the eld_unet was created with train = 0");
     u->dz1_1_final = false;
     ELD_CHECK_CUDA(cudaSetDevice(u->ctx->device));
-    Runner r{ u, &u->fs, params, static_cast<cudaStream_t>(stream) };
-    ELD_CHECK_CUDA(cudaMemsetAsync(grads, 0, u->n_params * sizeof(float), r.st));
+    Runner r{ u, &u->fs, params, static_cast<cudaStream_t>(stream), u->accumulate };
+    if (!u->accumulate) ELD_CHECK_CUDA(cudaMemsetAsync(grads, 0, u->n_params * sizeof(float), r.st));
     ELD_CHECK_CUDA(cudaMemsetAsync(u->gtmp, 0, u->n_params * sizeof(float), r.st));
     ELD_CHECK_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), r.st));
     TRY(r.forward(x));
@@ -903,6 +913,23 @@ extern "C" int eld_unet_set_loss(eld_unet* u, int kind)
 {
     ELD_REQUIRE(u && (kind == 0 || kind == 1), "eld_unet_set_loss: kind must be 0 (L1) or 1 (MSE)");
     u->l2_loss = kind;
+    return ELD_OK;
+}
+
+// Gradient accumulation for eld_unet_train_step: with `on`, the step adds its gradients to what grads holds.  The one
+// memset of grads is skipped, and the permute adds the staged conv3x3 weight gradients (Runner::finish_bucket, single-GPU
+// and per-bucket alike).  Every other writer into grads already adds into it with red.add / atomicAdd:
+//   first_conv_kernel<WGRAD>      conv1_1 dW / db      (first_conv.cuh)
+//   wgrad_gemm_kernel             deconv dW / db       (wgrad_gemm.cuh)
+//   conv3x3_wgrad_thin_kernel     conv3x3 db, fused    (wgrad_thin.cuh; its dW goes to the gtmp staging)
+//   head_kernel                   dW10 / db10          (unet_ew.cu)
+// A frozen tensor's gradient still goes to gtmp (dw_to / db_to) and the permute skips a frozen conv3x3 weight, so a
+// frozen range of grads is never written.  The launches are those of the plain step, in the same order.
+// eld_unet_backward / eld_unet_backward_state do not read the flag.
+extern "C" int eld_unet_set_accumulate(eld_unet* u, int on)
+{
+    ELD_REQUIRE(u && u->train, "eld_unet_set_accumulate: needs an eld_unet created with train = 1");
+    u->accumulate = on != 0;
     return ELD_OK;
 }
 

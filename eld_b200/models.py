@@ -11,7 +11,9 @@ Differences that are the point of this repo
   * data parallel: if torch.distributed is initialised the flat gradient buffer is all-reduced
     (NCCL over NVLink) between backward and Adam - one collective, U-Net weights only;
   * get_current_errors() keeps the reference's `.item()` host sync but can be told to defer it;
-  * opt.cuda_graph captures the fused step (train_step + Adam) in a CUDA graph and replays it (ELDModel._graph_step).
+  * opt.cuda_graph captures the fused step (train_step + Adam) in a CUDA graph and replays it (ELDModel._graph_step);
+  * opt.accum_steps = k accumulates the gradients of k optimize_parameters() calls and takes one Adam step (and, data
+    parallel, one all-reduce) per window of k: the update of a W-GPU job at batch n is that of batch k W n.
 """
 import os
 from collections import OrderedDict
@@ -31,7 +33,7 @@ def default_opt(**kw):
              stage_in='raw', stage_out='raw', model_path=None, include=4, crf=False, batchSize=1, lr=1e-4,
              beta1=0.9, wd=0.0, loss='l1', noise='g', isTrain=True, save_epoch_freq=100, noise_on_gpu=False,
              augment_on_gpu=False, defer_loss_sync=False, prefetch_noise=False, num_burst=1, pairs_on_gpu=False,
-             cuda_graph=False)
+             cuda_graph=False, accum_steps=1)
     o.update(kw)
     return SimpleNamespace(**o)
 
@@ -100,6 +102,8 @@ class ELDModel(BaseModel):
         self._static = None          # (input, target) buffers the captured step reads
         self._graph = None           # the captured step (_capture)
         self._eager_left = 0         # eager warm-up steps before the next capture
+        self._accum = 1              # optimize_parameters() calls per optimizer step (opt.accum_steps)
+        self._micro = 0              # calls of the current accumulation window so far
 
     def _eval(self):
         self.netG.eval()
@@ -129,7 +133,15 @@ class ELDModel(BaseModel):
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         self.rank = dist.get_rank() if self.world > 1 else 0
         self._graphed = bool(getattr(opt, 'cuda_graph', False)) and self.isTrain
+        accum = getattr(opt, 'accum_steps', 1)
+        if int(accum) != accum or accum < 1:
+            raise ValueError('accum_steps must be a positive integer; got %r' % (accum,))
+        self._accum, self._micro = int(accum), 0
         if self._graphed:
+            if self._accum > 1:
+                raise NotImplementedError('cuda_graph with accum_steps > 1: a window needs an accumulating and a '
+                                          'final step, and only one step graph is captured; set accum_steps = 1 or '
+                                          'train without cuda_graph')
             if self.world > 1:
                 raise NotImplementedError('cuda_graph: the data-parallel step (NCCL all-reduces) is not captured; '
                                           'train with world size 1 or without cuda_graph')
@@ -309,15 +321,23 @@ class ELDModel(BaseModel):
         return self.netG(x.contiguous())[:, :, :h, :w]
 
     def optimize_parameters(self):
-        """forward, zero_grad, L1 backward, (all-reduce), Adam - ELD_model.py:469-475."""
+        """forward, zero_grad, L1 backward, (all-reduce), Adam - ELD_model.py:469-475.
+        With opt.accum_steps = k, call j of each window of k adds its gradients to those of calls 0 .. j-1 (call 0
+        starts from zero), and only call k-1 all-reduces (data parallel) and takes the Adam step, on the mean gradient
+        (grad_scale 1 / (k world): every call's loss is its own micro-batch's mean).  Frame ids advance per call, so call
+        j of a 1-GPU job gets the frames rank j of a k-GPU job gets.  get_current_errors() reports each call's loss."""
         self._train()
         if self._graphed:
             return self._graph_step()
+        j, k = self._micro, self._accum
+        last = j == k - 1
         if self.world > 1:
-            self.output, self.loss_pixel = self.netG.train_step_ddp(self.input, self.target)
+            self.output, self.loss_pixel = self.netG.train_step_ddp(self.input, self.target, accumulate=j > 0, sync=last)
         else:
-            self.output, self.loss_pixel = self.netG.train_step(self.input, self.target)
-        self.optimizer_G.step(grad_scale=1.0 / self.world)
+            self.output, self.loss_pixel = self.netG.train_step(self.input, self.target, accumulate=j > 0)
+        self._micro = 0 if last else j + 1
+        if last:
+            self.optimizer_G.step(grad_scale=1.0 / (k * self.world))
 
     # ---- the fused step in a CUDA graph (opt.cuda_graph) ----------------------------------------------------------------
     graph_warmup = 3      # eager steps (on a side stream, as torch's capture recipe runs them) before each capture
@@ -473,10 +493,14 @@ class ELDModel(BaseModel):
         if model.isTrain and 'opt_g' in state_dict:
             model.optimizer_G.load_state_dict(state_dict['opt_g'])
         model._frames_seen = int(state_dict.get('frames_seen', 0))
+        model._micro = 0             # a partial accumulation window is not saved: the resumed run starts a new one
         print('Resume from epoch %d, iteration %d' % (model.epoch, model.iterations))
         return state_dict
 
     def state_dict(self):
+        """Taken in the middle of an accumulation window (opt.accum_steps), it holds the weights and Adam state of the
+        last update and the running frame count; the window's partial gradients are not saved, and load() starts a new
+        window."""
         return {'netG': {k: v.detach().cpu().clone() for k, v in self.netG.state_dict().items()},
                 'opt_g': self.optimizer_G.state_dict(), 'epoch': self.epoch, 'iterations': self.iterations,
                 'frames_seen': self._frames_seen}

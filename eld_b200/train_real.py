@@ -60,6 +60,8 @@ def main():
     ap.add_argument('--nThreads', type=int, default=2); ap.add_argument('--name', default='eld_b200_real')
     ap.add_argument('--loss', default='l1', choices=['l1', 'l2'])
     ap.add_argument('--no-augment', action='store_true', help='skip the flips / transpose (sid_dataset.py:340-352)')
+    ap.add_argument('--accum_steps', type=int, default=1, help='micro-batches per optimizer step: one Adam step (and one '
+                    'all-reduce) per window of k steps, on the gradients of k * world * batchSize frames')
     a = ap.parse_args()
     world = int(os.environ.get('WORLD_SIZE', '1'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
@@ -83,7 +85,7 @@ def main():
                                 [LMDBDataset(join(a.traindir, _db_name('input', a.stage_in, a.crf)))])
     opt = models.default_opt(name=a.name, gpu_ids=[local], batchSize=a.batchSize, lr=1e-4, pairs_on_gpu=True,
                              augment_on_gpu=not a.no_augment, defer_loss_sync=True, loss=a.loss, stage_in=a.stage_in,
-                             stage_out=a.stage_out, seed=a.seed)
+                             stage_out=a.stage_out, seed=a.seed, accum_steps=a.accum_steps)
     sampler = torch.utils.data.distributed.DistributedSampler(train, world, rank, shuffle=True) if world > 1 else None
     loader = torch.utils.data.DataLoader(train, batch_size=a.batchSize, shuffle=sampler is None, sampler=sampler,
                                          num_workers=a.nThreads, pin_memory=True)

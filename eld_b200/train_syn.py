@@ -48,6 +48,8 @@ def main():
     ap.add_argument('--stage_in', default='raw', choices=['raw', 'srgb'])     # train_syn.py:55-58 (ISPDataset branch)
     ap.add_argument('--stage_out', default='raw', choices=['raw'])            # an sRGB TARGET needs the rendered LMDB
     ap.add_argument('--num_burst', type=int, default=1)                       # SynDataset(num_burst=...), sid_dataset.py:269-275
+    ap.add_argument('--accum_steps', type=int, default=1, help='micro-batches per optimizer step: one Adam step (and one '
+                    'all-reduce) per window of k steps, on the gradients of k * world * batchSize frames')
     a = ap.parse_args()
     world = int(os.environ.get('WORLD_SIZE', '1'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
@@ -58,7 +60,8 @@ def main():
     torch.manual_seed(a.seed); np.random.seed(a.seed)                        # base_options.py:31-34
     opt = models.default_opt(name=a.name, gpu_ids=[local], noise=a.noise, include=a.include, batchSize=a.batchSize,
                              lr=a.lr, noise_on_gpu=True, augment_on_gpu=not a.no_augment and a.stage_in == 'raw', defer_loss_sync=True,
-                             loss=a.loss, stage_in=a.stage_in, stage_out=a.stage_out, num_burst=a.num_burst)
+                             loss=a.loss, stage_in=a.stage_in, stage_out=a.stage_out, num_burst=a.num_burst,
+                             accum_steps=a.accum_steps)
     noise_model = NoiseModel(model=opt.noise, include=opt.include, seed=a.seed, verbose=rank == 0)   # train_syn.py:38
     ds = SyntheticClean(a.iters * a.batchSize * world, a.seed, meta=a.stage_in == 'srgb')
     sampler = torch.utils.data.distributed.DistributedSampler(ds, world, rank, shuffle=True) if world > 1 else None

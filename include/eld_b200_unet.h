@@ -98,7 +98,8 @@ int    eld_unet_grad_buckets_io(int cin, int cout, size_t* offsets, int max_offs
 /* ELDModel.forward (ELD_model.py:422-432): x f32 NCHW [n][4][h][w] -> out f32 NCHW [n][4][h][w] */
 int    eld_unet_forward(eld_unet* u, const float* params, const float* x, float* out, void* stream);
 /* forward + pixel loss (L1: mean |out-target|, losses.py:32; or MSE, see eld_unet_set_loss) + backward (ELD_model.py:411-420): grads is zeroed
- * and filled; *loss (device float) receives the mean absolute error.  No optimizer step, no host sync. */
+ * and filled - or, after eld_unet_set_accumulate(u, 1), this call's gradients are added to what grads holds; *loss (device
+ * float) receives this call's mean absolute error either way.  No optimizer step, no host sync. */
 int    eld_unet_train_step(eld_unet* u, const float* params, const float* x, const float* target,
                            float* out, float* grads, float* loss, void* stream);
 /* The autograd seam (ELDModel.backward_G, ELD_model.py:411-420: `loss.backward()` through netG): after an
@@ -137,6 +138,15 @@ int    eld_unet_set_trainable(eld_unet* u, const uint8_t* flags, int n_flags, in
 #define ELD_LOSS_L1 0
 #define ELD_LOSS_L2 1
 int    eld_unet_set_loss(eld_unet* u, int kind);
+/* Gradient accumulation over micro-batches (loss.backward() adding into .grad, DistributedDataParallel.no_sync()): with
+ * on != 0, every following eld_unet_train_step adds its gradients to `grads` instead of zeroing it first, so k steps on k
+ * micro-batches leave the sum of their gradients (scale it in the optimizer step: each step's loss is its own batch's
+ * mean).  The step launches the kernels of a plain step in the same order, without the memset of `grads`; bucket events
+ * mark the accumulated sum final.  A frozen tensor's range of `grads` is never written, so it keeps what it held: keep
+ * one eld_unet_set_trainable mask over a window.  Governs eld_unet_train_step only (eld_unet_backward still zeroes and
+ * fills).  Default off.  Host-side only: no launch, no synchronisation.  ELD_E_ARG for NULL or an object created with
+ * train = 0. */
+int    eld_unet_set_accumulate(eld_unet* u, int on);
 /* Data-parallel overlap (SURVEY 8e; the reference is single-GPU, ELD_model.py:187-190): the flat gradient is final in
  * eld_unet_grad_buckets() = 4 contiguous ranges in backward-completion order (decoder upv6..conv10_1, bottleneck
  * conv5_*, encoder conv2_1..conv4_2, first layer conv1_1..conv1_2); offsets[2k], offsets[2k+1] = first element, element
