@@ -342,6 +342,9 @@ extern "C" int eld_unet_create_io(eld_ctx* ctx, int n, int h, int w, int train, 
     ELD_REQUIRE(io_ok(cin, cout), "eld_unet_create: channels in / out must be 3 (sRGB) or 4 (packed raw); got %d -> %d", cin, cout);
     ELD_REQUIRE(n > 0 && h > 0 && w > 0, "eld_unet_create: bad shape");
     ELD_REQUIRE(h % 16 == 0 && w % 16 == 0, "eld_unet_create: H and W must be multiples of 16 (four 2x2 pools, like the reference); got %dx%d", h, w);
+    // the head's 32-bit index (launch_head): refused here, before the workspace check, rather than after 23 launches
+    ELD_REQUIRE((size_t)n * h * w < kHeadMaxPixels,
+                "eld_unet_create: n*H*W = %zu pixels; the head needs fewer than 2^26 (n*H*W*32 < 2^31)", (size_t)n * h * w);
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     ELD_REQUIRE(!train || (h % 128 == 0 && w % 256 == 0),
                 "eld_unet_create: TRAINING needs H %% 128 == 0 and W %% 256 == 0 (whole 8x16 / 8x8 gradient tiles at 1/16 scale); got %dx%d", h, w);

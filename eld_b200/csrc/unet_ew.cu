@@ -210,7 +210,10 @@ head_kernel(const __nv_bfloat16* __restrict__ a, const float* __restrict__ w, co
             ploss += l2_loss == 1 ? e * e : fabsf(e);
             const float d = l2_loss == 2 ? ((valid && live) ? tg : 0.f)
                           : l2_loss == 1 ? 2.0f * e * inv_numel : (e > 0.f ? inv_numel : (e < 0.f ? -inv_numel : 0.f));
-            pdb += d;
+            // L1: count the signs (an exact integer in fp32 up to 2^24 pixels per thread) and scale once at the end -
+            // adding the constant inv_numel ~2000 times rounds the same way within each binade of the running sum, a
+            // bias that grows with the pixels per thread (rel 2e-5 at 10 x 1408 x 2048)
+            pdb += l2_loss == 0 ? (e > 0.f ? 1.f : (e < 0.f ? -1.f : 0.f)) : d;
             // the pixel's four dOut values (one per lane of the 4-lane group)
             const int base = lane & ~3;
             float dd[4];
@@ -249,7 +252,7 @@ head_kernel(const __nv_bfloat16* __restrict__ a, const float* __restrict__ w, co
                     x += __shfl_xor_sync(0xffffffffu, x, 16);
                     if (lane < 4) atomicAdd(&red[co * 32 + q * 8 + j], x);
                 }
-            float x = pdb;
+            float x = l2_loss == 0 ? pdb * inv_numel : pdb;
             x += __shfl_xor_sync(0xffffffffu, x, 4); x += __shfl_xor_sync(0xffffffffu, x, 8); x += __shfl_xor_sync(0xffffffffu, x, 16);
             if (lane < 4) atomicAdd(&red[128 + q], x);
         }
@@ -372,7 +375,7 @@ int launch_head(eld_ctx* ctx, const void* a, const float* w, const float* b, flo
                 float* dw, float* db, float* loss, int n, size_t plane, int cout, int l2_loss, cudaStream_t st)
 {
     const size_t total = (size_t)n * plane;
-    ELD_REQUIRE(total * 32 < (1ull << 31), "head kernel: %zu pixels exceed its 32-bit index range", total);
+    ELD_REQUIRE(total < kHeadMaxPixels, "head kernel: %zu pixels exceed its 32-bit index range", total);
     const float inv = 1.0f / (float)(total * cout);
     if (target) {
         head_kernel<true><<<grid_for(total, 32 * 16, 4 * ctx->num_sms), kHeadThreads, 0, st>>>(

@@ -5,6 +5,8 @@
 namespace eld {
 int launch_maxpool_bwd_code(eld_ctx* ctx, const void* code, const void* dskip, int s_pitch, int s_c0,
                             const void* dP, void* dZ, int C, int n, int Ho, int Wo, cudaStream_t st);
+// the head kernel indexes a9_2 with 32-bit offsets (n*H*W*32 bf16 elements < 2^31): fewer than 2^26 pixels per launch
+constexpr size_t kHeadMaxPixels = size_t(1) << 26;
 int launch_head(eld_ctx* ctx, const void* a, const float* w, const float* b, float* out, const float* target, void* dz,
                 float* dw, float* db, float* loss, int n, size_t plane, int cout, int l2_loss, cudaStream_t st);
 int launch_clock_probe(eld_ctx* ctx, float* out_mhz, cudaStream_t st);

@@ -78,7 +78,9 @@ size_t eld_unet_workspace_bytes(int n, int h, int w, int train);     /* activati
                                                                       * words (1 bit per masked activation element) and pool codes
                                                                       * (1 byte per pooled element: argmax + signs) */
 /* Inference (train = 0): h % 16 == 0 and w % 16 == 0, as for the reference network.  Training (train = 1):
- * h % 128 == 0, w % 256 == 0.  The caller owns `workspace` (device memory) for the lifetime of the object.
+ * h % 128 == 0, w % 256 == 0.  Both: n * h * w < 2^26 pixels (the head's 32-bit index), or ELD_E_ARG before the
+ * workspace is looked at - e.g. at most 255 frames of 512 x 512.  The caller owns `workspace` (device memory) for the
+ * lifetime of the object.
  * Creation synchronises (a cudaMemset of the workspace, the kernels' shared-memory opt-in): create the object outside any
  * CUDA graph capture.  eld_unet_train_step (per-launch profiling off, eld_unet_profile) neither synchronises nor
  * allocates - memsets on `stream`, kernels with

@@ -274,3 +274,43 @@ def test_rules_on_known_errors():
     rel, mx, ms = R.f32_rule(torch.tensor([1.0, 2.0]), torch.tensor([1.0, 2.5], dtype=torch.float64),
                              torch.tensor([1.0, 1.0], dtype=torch.float64))
     assert abs(rel - 0.5 / (1 + 2.5 ** 2) ** 0.5) < 1e-12 and mx == 0.2 and ms == 0.5
+
+
+def test_batch_sums_built_from_pieces_equal_the_whole_batch():
+    """tests/batch_ref.py: the weight / bias gradients, dW10 / db10 and the loss summed piece by piece (2-frame chunks of
+    a 5-frame batch and 16-row bands of 40 rows, both with an uneven last piece; the 3x3 pieces read a one-row halo)
+    equal the launch_ref references of the whole batch"""
+    import tests.batch_ref as B
+    g = torch.Generator().manual_seed(11)
+    n, h, w = 5, 40, 16
+    x = torch.randn(n, h, w, 32, generator=g).bfloat16()
+    dz = torch.randn(n, h, w, 64, generator=g).bfloat16()
+    parts = B.parts(n, h, 2, 16)
+    assert len(parts) == 9 and parts[-1] == (slice(4, 5), slice(32, 40))
+    close = lambda a, b: all(torch.allclose(u, v, rtol=1e-12, atol=1e-12) for u, v in zip(a, b))
+    whole = R.conv_wgrad(x, dz)
+    assert close(B.summed(B.conv_wgrad_piece(x, dz, fr, rows) for fr, rows in parts), whole)
+    # a wrong halo is visible: dropping it loses the taps that cross a band edge
+    cut = B.summed(R.conv_wgrad(x[fr, rows], dz[fr, rows]) for fr, rows in parts)
+    assert not torch.allclose(cut[0], whole[0], rtol=1e-6, atol=1e-6) and torch.allclose(cut[2], whole[2], rtol=1e-12)
+    frame = torch.rand(n, 4, h, w, generator=g)                          # conv1_1: the fp32 frame, rounded to bf16
+    dz1 = torch.randn(n, h, w, 32, generator=g).bfloat16()
+    assert close(B.summed(B.conv_wgrad_piece(frame.permute(0, 2, 3, 1), dz1, fr, rows, round_x=True) for fr, rows in parts),
+                 R.first_conv_wgrad(frame, dz1))
+    up = torch.randn(n, 2 * h, 2 * w, 32, generator=g).bfloat16()       # a deconv: dy at twice x's rows
+    assert close(B.summed(B.deconv_wgrad_piece(x, up, fr, rows) for fr, rows in parts), R.deconv_wgrad(x, up))
+    a = torch.randn(n, h, w, 32, generator=g).bfloat16()
+    w10 = torch.randn(4, 32, 1, 1, generator=g)
+    out, tgt = torch.randn(n, 4, h, w, generator=g), torch.randn(n, 4, h, w, generator=g)
+    for kind in ('l1', 'l2'):
+        dout = R.head_dout(out, tgt, kind)
+        pieces = [B.head_dout(out[fr, :, rows], tgt[fr, :, rows], kind, out.numel()) for fr, rows in parts]
+        assert all(torch.equal(p, dout[fr, :, rows]) for p, (fr, rows) in zip(pieces, parts))
+        assert close(B.summed(B.head_wgrad(a[fr, rows], w10, p) for p, (fr, rows) in zip(pieces, parts)),
+                     R.head_bwd(a, w10, dout)[2:])
+        lr, = B.summed((B.head_loss(out[fr, :, rows], tgt[fr, :, rows], kind, out.numel()).reshape(1),) for fr, rows in parts)
+        assert torch.allclose(lr, R.head_loss(out, tgt, kind).reshape(1), rtol=1e-14)
+    # grid over pieces of 2^24 elements: the minimum of the pieces' grids
+    t = torch.ones((1 << 24) + 3, dtype=torch.float32)
+    t[-1] = 0.25
+    assert B.grid(t) == R.grid(t) == -2 and B.grid(torch.zeros(0)) == math.inf
