@@ -37,26 +37,28 @@ struct ConvGemmParams {
     const float* bias;    // per GEMM column (EPI_SHUFFLE: per cout, column % cout)
     const __nv_bfloat16* aux;
     int aux_pitch, aux_c0;
-    const uint32_t* aux_sign;  // ACT_MASK from sign words instead of the activation: uint32 [pixel][n_total / 32], channel 2j -> bit j,
-                               // 2j+1 -> bit 16+j of its 32-channel chunk (what `sign_out` of the producing forward tile wrote)
-    uint32_t* sign_out;        // optional (training): sign words of the activated output, same layout
+    const uint32_t* aux_slope; // ACT_MASK from slope words instead of the activation: two planes of uint32 [pixel][n_total / 32],
+                               // the neg words, then the tie words (wgmma.cuh slope_words; channel 2j -> bit j, 2j+1 -> bit
+                               // 16+j of its 32-channel chunk), what `slope_out` of the producing forward tile wrote
+    uint32_t* slope_out;       // optional (training): slope words of the activated output, same layout
     int cout;             // EPI_SHUFFLE: channels per sub-pixel
     int cout_shift;       // EPI_SHUFFLE: log2(cout) (cout must be a power of two)
     int stages;
     const uint8_t* b_ptr; // packed weights
     __nv_bfloat16* pool_out;   // optional fused MaxPool2d(2) of the (activated) output: bf16 NHWC [n][H/2][W/2][pool_pitch]
     int pool_pitch;
-    uint32_t* pool_code;       // optional (training): 32 bytes per (pooled pixel, 32 channels) = which window element won and the
-                               // four signs, all the pool backward needs of the activation (unet_ew.cu maxpool_bwd_code_kernel)
+    uint32_t* pool_code;       // optional (training): per (pooled pixel, 32 channels) 32 bytes = which window elements are the
+                               // maximum and their four neg words, then in a second plane 16 bytes = their four tie words:
+                               // all the pool backward needs of the activation (unet_ew.cu maxpool_bwd_code_kernel)
     __nv_bfloat16* out2;  // EPI_STORE split store: GEMM columns >= out_split go to out2[pix * out2_pitch + (col - out_split)]
     int out2_pitch, out_split;   // (planar halves of a concat gradient); out_split % 32 == 0, 0 = off
     int bias_smem_off, stg_smem_off, bar_smem_off;   // byte offsets from the 1024-aligned base
 };
 
-// max of two packed bf16 pairs
+// max of two packed bf16 pairs, NaN if either is NaN (MaxPool2d propagates NaN)
 __device__ __forceinline__ uint32_t bf2_max(uint32_t a, uint32_t b)
 {
-    const __nv_bfloat162 m = __hmax2(*reinterpret_cast<const __nv_bfloat162*>(&a), *reinterpret_cast<const __nv_bfloat162*>(&b));
+    const __nv_bfloat162 m = __hmax2_nan(*reinterpret_cast<const __nv_bfloat162*>(&a), *reinterpret_cast<const __nv_bfloat162*>(&b));
     return *reinterpret_cast<const uint32_t*>(&m);
 }
 
@@ -93,29 +95,23 @@ __device__ __forceinline__ void conv_epilogue32(const ConvGemmParams& p, const f
     if (p.act == ACT_LRELU) {
 #pragma unroll
         for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.2f * v[j]);
-    } else if (p.act == ACT_MASK && in_img && p.aux_sign) {
-        const uint32_t sgw = __ldg(p.aux_sign + (size_t)pix * (size_t)(p.n_total >> 5) + (size_t)(col >> 5));
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            // slope = 0.6 + 0.4 * (+-1) = 1 or 0.2
-            const float s_lo = __uint_as_float(((sgw << (31 - j)) & 0x80000000u) | 0x3F800000u);
-            const float s_hi = __uint_as_float(((sgw << (15 - j)) & 0x80000000u) | 0x3F800000u);
-            v[2 * j] *= __fmaf_rn(s_lo, 0.4f, 0.6f);
-            v[2 * j + 1] *= __fmaf_rn(s_hi, 0.4f, 0.6f);
-        }
     } else if (p.act == ACT_MASK && in_img) {
-        uint32_t mk[16];
-        const __nv_bfloat16* ap = p.aux + (size_t)pix * p.aux_pitch + (p.aux_c0 + col);
-        ptx::ld_global_nc_32B(ap, mk);
-        ptx::ld_global_nc_32B(ap + 16, mk + 8);
+        uint32_t neg, tie;
+        if (p.aux_slope) {
+            const size_t plane = (size_t)p.n_img * p.H * p.W * (size_t)(p.n_total >> 5);
+            const uint32_t* sw = p.aux_slope + (size_t)pix * (size_t)(p.n_total >> 5) + (size_t)(col >> 5);
+            neg = __ldg(sw); tie = __ldg(sw + plane);
+        } else {
+            uint32_t mk[16];
+            const __nv_bfloat16* ap = p.aux + (size_t)pix * p.aux_pitch + (p.aux_c0 + col);
+            ptx::ld_global_nc_32B(ap, mk);
+            ptx::ld_global_nc_32B(ap + 16, mk + 8);
+            ptx::slope_words(mk, neg, tie);
+        }
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
-            // LeakyReLU keeps the sign: slope = 0.6 + 0.4 * sign(activation) = 1 or 0.2
-            // (activation == +0 counts as positive; the reference's tie is a measure-zero event)
-            const float s_lo = __uint_as_float(((mk[j] << 16) & 0x80000000u) | 0x3F800000u);
-            const float s_hi = __uint_as_float((mk[j] & 0x80000000u) | 0x3F800000u);
-            v[2 * j] *= __fmaf_rn(s_lo, 0.4f, 0.6f);
-            v[2 * j + 1] *= __fmaf_rn(s_hi, 0.4f, 0.6f);
+            v[2 * j] *= lrelu_slope(neg, tie, j, kMaskNeg);
+            v[2 * j + 1] *= lrelu_slope(neg, tie, 16 + j, kMaskNeg);
         }
     }
     // round once; the pool below works on the rounded (= stored) values
@@ -125,9 +121,13 @@ __device__ __forceinline__ void conv_epilogue32(const ConvGemmParams& p, const f
         const __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
         wv[j] = *reinterpret_cast<const uint32_t*>(&h);
     }
-    if (p.sign_out && in_img) {
-        // sign words of the stored activation: all a later LeakyReLU' needs (1/16 of the tensor)
-        p.sign_out[(size_t)pix * (size_t)(p.n_total >> 5) + (size_t)(col >> 5)] = ptx::gather_msb16(wv);
+    uint32_t neg = 0, tie = 0;
+    if (p.slope_out || p.pool_code) ptx::slope_words(wv, neg, tie);
+    if (p.slope_out && in_img) {
+        // slope words of the stored activation: all a later LeakyReLU' needs (1/8 of the tensor)
+        const size_t plane = (size_t)p.n_img * p.H * p.W * (size_t)(p.n_total >> 5);
+        uint32_t* sw = p.slope_out + (size_t)pix * (size_t)(p.n_total >> 5) + (size_t)(col >> 5);
+        sw[0] = neg; sw[plane] = tie;
     }
     if (p.pool_out) {
         // MaxPool2d(2) fused: the 2x2 window of pixel (x, y) lives in lanes ^1 (x) and ^16 (y) of this warp; packed bf16x2
@@ -146,20 +146,29 @@ __device__ __forceinline__ void conv_epilogue32(const ConvGemmParams& p, const f
             ptx::st_global_32B(q4 + 16, pw + 8);
         }
         if (p.pool_code) {
-            // per lane two 32-bit masks over its 32 channels: "is not the window's maximum" and "is negative"
-            // (channel 2j -> bit j, channel 2j+1 -> bit 16+j); the window's origin lane collects the four lanes'
-            // masks in the order the backward walks the window: (0,0) (0,1) (1,0) (1,1)
+            // per lane, over its 32 channels: "is not the window's maximum" (all clear in a window holding NaN, where the
+            // backward picks the last NaN from the slope words) and the slope-word pair (channel 2j -> bit j, channel
+            // 2j+1 -> bit 16+j); the window's origin lane collects the four lanes' words in the order the backward walks
+            // the window: (0,0) (0,1) (1,0) (1,1)
             uint32_t ne[16];
 #pragma unroll
             for (int j = 0; j < 16; ++j)
                 ne[j] = __hne2_mask(*reinterpret_cast<const __nv_bfloat162*>(&wv[j]), *reinterpret_cast<const __nv_bfloat162*>(&pw[j]));
-            const uint32_t nm = ptx::gather_msb16(ne), sg = ptx::gather_msb16(wv);
-            uint32_t code[8];
-            code[0] = nm; code[4] = sg;
-            code[1] = __shfl_xor_sync(0xffffffffu, nm, 1);                code[5] = __shfl_xor_sync(0xffffffffu, sg, 1);
-            code[2] = __shfl_xor_sync(0xffffffffu, nm, kConvTileW);       code[6] = __shfl_xor_sync(0xffffffffu, sg, kConvTileW);
-            code[3] = __shfl_xor_sync(0xffffffffu, nm, kConvTileW | 1);   code[7] = __shfl_xor_sync(0xffffffffu, sg, kConvTileW | 1);
-            if (origin) ptx::st_global_32B(p.pool_code + (ppix * (size_t)(p.pool_pitch >> 5) + (size_t)(col >> 5)) * 8, code);
+            const uint32_t own[3] = { ptx::gather_msb16(ne), neg, tie };
+            uint32_t code[12];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                code[4 * k] = own[k];
+                code[4 * k + 1] = __shfl_xor_sync(0xffffffffu, own[k], 1);
+                code[4 * k + 2] = __shfl_xor_sync(0xffffffffu, own[k], kConvTileW);
+                code[4 * k + 3] = __shfl_xor_sync(0xffffffffu, own[k], kConvTileW | 1);
+            }
+            if (origin) {
+                const size_t rec = ppix * (size_t)(p.pool_pitch >> 5) + (size_t)(col >> 5);
+                const size_t recs = (size_t)p.n_img * (p.H >> 1) * (p.W >> 1) * (size_t)(p.pool_pitch >> 5);
+                ptx::st_global_32B(p.pool_code + rec * 8, code);
+                *reinterpret_cast<uint4*>(p.pool_code + recs * 8 + rec * 4) = make_uint4(code[8], code[9], code[10], code[11]);
+            }
         }
     }
     if (!in_img) return;

@@ -28,8 +28,8 @@ struct FirstConvParams {
     const float* bias;          // fprop
     __nv_bfloat16* out;         // fprop: NHWC bf16, 32 channels at out_pitch
     int out_pitch;
-    uint32_t* sign_out;         // fprop, optional (training): one sign word per pixel (channel 2j -> bit j, 2j+1 -> bit 16+j), the
-                                // LeakyReLU' mask conv1_2's data gradient needs (conv_gemm.cuh aux_sign)
+    uint32_t* slope_out;        // fprop, optional (training): a neg word per pixel, then a plane of tie words (wgmma.cuh
+                                // slope_words), the LeakyReLU' mask conv1_2's data gradient needs (conv_gemm.cuh aux_slope)
     float* dw;                  // wgrad: f32 OIHW [32][4][3][3], accumulated into
     float* db;                  // wgrad: f32 [32]
     const float* w;             // dgrad: the f32 master weights, OIHW [32][cin][3][3]
@@ -193,7 +193,12 @@ first_conv_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
             __nv_bfloat16* dst = p.out + pix * p.out_pitch;
             ptx::st_global_32B(dst, wv);                   // 64 bytes = two full sectors
             ptx::st_global_32B(dst + 16, wv + 8);
-            if (p.sign_out) p.sign_out[pix] = ptx::gather_msb16(wv);
+            if (p.slope_out) {
+                uint32_t neg, tie;
+                ptx::slope_words(wv, neg, tie);
+                p.slope_out[pix] = neg;
+                p.slope_out[(size_t)p.n_img * p.H * p.W + pix] = tie;
+            }
             // the next tile's staging writes come after its build barrier: every thread has read its row by then
         } else {
             // D[k][co] += A^T (MN-major, k = 64 slots per 128-byte row) * dZ (MN-major, 32 co per 64-byte row);

@@ -128,16 +128,16 @@ wgrad_permute_kernel(const float* __restrict__ gtmp, float* __restrict__ grads, 
 
 using namespace eld;
 
-// Everything a forward leaves for the backward of the same call: activations and concat buffers, pool codes, sign words
+// Everything a forward leaves for the backward of the same call: activations and concat buffers, pool codes, slope words
 // and the packed weights.  layout() places one inside the workspace (the built-in state, eld_unet_forward) or in memory
 // the caller owns (eld_unet_forward_state).  The backward writes none of it, so a state stays valid after a backward
 // that read it.
 struct FwdState {
     __nv_bfloat16* act[kNumLayers] = {};     // the output of each layer that has a buffer of its own
-    // sign words (1 bit per element) of the activations whose LeakyReLU' a data gradient applies (training): the dgrad
+    // slope words (2 bits per element) of the activations whose LeakyReLU' a data gradient applies (training): the dgrad
     // tiles read these instead of the activation itself
-    uint32_t* sign[kNumLayers] = {};
-    // per level: the concat buffer, and the pooled tensor with its pool codes (1 byte per pooled element, training)
+    uint32_t* slope[kNumLayers] = {};
+    // per level: the concat buffer, and the pooled tensor with its pool codes (1.5 bytes per pooled element, training)
     __nv_bfloat16 *cat[kLevels] = {}, *pool[kLevels] = {}, *code[kLevels] = {};
     __nv_bfloat16* packed = nullptr;
 };
@@ -206,12 +206,12 @@ static size_t layout(eld_unet* u, FwdState* s, char* base, bool train, bool scra
     }
     if (train) {
         for (int i = 0; i < kNumLayers; ++i)
-            if (pooled(i)) s->code[u->L[i].lvl + 1] = take(u->L[i].lvl + 1, u->L[i].cout / 2);
+            if (pooled(i)) s->code[u->L[i].lvl + 1] = take(u->L[i].lvl + 1, u->L[i].cout * 3 / 4);   // 48 B per 32 channels
         // every activation with a buffer of its own, except the head's input: the head applies that LeakyReLU'
         for (int i = 0; i < kNumLayers; ++i) {
             const Layer& l = u->L[i];
             if (l.type == L_CONV3 && !pooled(i) && i != u->L[I_C10].src)
-                s->sign[i] = reinterpret_cast<uint32_t*>(take(l.lvl, l.cout / 16));   // cout / 32 words per pixel
+                s->slope[i] = reinterpret_cast<uint32_t*>(take(l.lvl, l.cout / 8));   // cout / 16 words per pixel
         }
     }
     // packed weights
@@ -504,7 +504,7 @@ struct Runner {
         op.act = ACT_LRELU; op.out = y.p; op.out_pitch = y.pitch; op.out_c0 = y.c0; op.bias = bias(li);
         if (pooled(li)) { op.pool_out = s->pool[l.lvl + 1]; op.pool_code = s->code[l.lvl + 1]; }
         op.pool_pitch = l.cout;
-        op.sign_out = s->sign[li];
+        op.slope_out = s->slope[li];
         const double px = (double)u->n * op.H * op.W;
         Scope sc(u, st, l.name, "fprop", 2.0 * px * l.cout * 9 * l.cin, px * 2 * (l.cin + l.cout) + 18.0 * l.cin * l.cout);
         return launch_conv_gemm(ctx(), op, st);
@@ -528,7 +528,7 @@ struct Runner {
     //   bytes (ncu r01: level-1 pool.bwd 570 MB for 300, upv9 dgrad/wgrad 336 MB for 200).  When nothing needs the skip
     //   half (reach[skip]), only the up half's cin/2 columns, read as a row prefix of every block of the same packed operand.
     // - a pooled input: into dp of its level, unmasked (pool_bwd applies the pool code)
-    // - else: into the producer's dz, with the LeakyReLU' mask from the producer's sign words
+    // - else: into the producer's dz, with the LeakyReLU' mask from the producer's slope words
     int conv_dgrad(int li) const
     {
         const Layer& l = u->L[li];
@@ -549,8 +549,8 @@ struct Runner {
         op.n_img = u->n; op.H = u->H >> l.lvl; op.W = u->W >> l.lvl;
         op.b = wd(li); op.cout = nc;
         op.act = mask ? ACT_MASK : ACT_NONE; op.out_c0 = 0; op.bias = nullptr;
-        op.aux_sign = mask ? s->sign[l.src] : nullptr;
-        ELD_REQUIRE(!mask || op.aux_sign, "eld_unet: %s dgrad: no sign words for its LeakyReLU' mask", l.name);
+        op.aux_slope = mask ? s->slope[l.src] : nullptr;
+        ELD_REQUIRE(!mask || op.aux_slope, "eld_unet: %s dgrad: no slope words for its LeakyReLU' mask", l.name);
         const double px = (double)u->n * op.H * op.W;
         Scope sc(u, st, l.name, "dgrad", 2.0 * px * l.cout * 9 * nc, px * 2 * (nc * (mask ? 2 : 1) + l.cout) + 18.0 * nc * l.cout);
         return launch_conv_gemm(ctx(), op, st);
@@ -564,8 +564,8 @@ struct Runner {
         op.n_img = u->n; op.H = u->H >> (l.lvl + 1); op.W = u->W >> (l.lvl + 1);
         op.b = wd(li); op.cout = l.cin;
         op.act = ACT_MASK; op.out = u->dz[l.src]; op.out_pitch = l.cin; op.out_c0 = 0;
-        op.aux_sign = s->sign[l.src];
-        ELD_REQUIRE(op.aux_sign, "eld_unet: %s dgrad: no sign words for its LeakyReLU' mask", l.name);
+        op.aux_slope = s->slope[l.src];
+        ELD_REQUIRE(op.aux_slope, "eld_unet: %s dgrad: no slope words for its LeakyReLU' mask", l.name);
         const double px = (double)u->n * op.H * op.W;
         Scope sc(u, st, l.name, "dgrad", 2.0 * px * 4 * l.cout * l.cin, px * 2 * (2 * l.cin + 4 * l.cout) + 8.0 * l.cin * l.cout);
         return launch_conv_gemm(ctx(), op, st);
@@ -605,14 +605,14 @@ struct Runner {
         return launch_first_conv_wgrad(ctx(), x, u->cin0, u->dz[I_C11], l.cout, dw_to(I_C11, grads), db_to(I_C11, grads), u->n,
                                        u->H, u->W, st);
     }
-    // pooled layer li's pool backward, from the argmax + sign code the forward tile left (the activation is not read
+    // pooled layer li's pool backward, from the maxima + slope code the forward tile left (the activation is not read
     // again): dp and the PLANAR skip half of the concat gradient -> li's dz
     int pool_bwd(int li) const
     {
         const Layer& l = u->L[li];
         const int lvl = l.lvl + 1, C = l.cout;
         const double pxo = (double)u->n * (u->H >> lvl) * (u->W >> lvl);
-        Scope sc(u, st, "pool", "bwd", 0.0, pxo * C * (2 * 9 + 1));
+        Scope sc(u, st, "pool", "bwd", 0.0, pxo * C * (2 * 9 + 1.5));
         return launch_maxpool_bwd_code(ctx(), s->code[lvl], skip_half(u->dcat[l.lvl], l.lvl, C), C, 0, u->dp[lvl], u->dz[li],
                                        C, u->n, u->H >> lvl, u->W >> lvl, st);
     }
@@ -671,7 +671,7 @@ struct Runner {
             const double px = (double)u->n * u->H * u->W;
             Scope sc(u, st, "conv1_1", "fprop", 2.0 * px * 32 * 9 * u->cin0, px * (4 * u->cin0 + 64));
             TRY(launch_first_conv(ctx(), x, u->cin0, wf(I_C11), bias(I_C11), s->act[I_C11], u->L[I_C11].cout, u->n, u->H, u->W,
-                                  st, s->sign[I_C11]));
+                                  st, s->slope[I_C11]));
         }
         for (int li = I_C11 + 1; li < I_C10; ++li) TRY(u->L[li].type == L_DECONV ? deconv(li) : conv(li));
         return ELD_OK;
@@ -805,9 +805,9 @@ extern "C" int eld_unet_input_grad(eld_unet* u, const float* params, float* dx, 
 }
 
 /* Host-side view of the workspace for tests and debugging: where tensor `name` of the last step lives.  No launch.
-   The names come from the layer table: aX_Y / dzX_Y / sign:aX_Y for convX_Y's own output, its gradient and its sign words;
-   catN / dcatN for the concat buffer upvN writes into and its gradient; pN / pcN / dpN for the pooled tensor at level N,
-   its pool codes and its gradient.  Activations belong to the built-in forward state; the gradients are backward scratch. */
+   The names come from the layer table: aX_Y / dzX_Y / sign:aX_Y / tie:aX_Y for convX_Y's own output, its gradient and its two planes of slope words;
+   catN / dcatN for the concat buffer upvN writes into and its gradient; pN / pcN / ptN / dpN for the pooled tensor at
+   level N, its pool codes (maxima and neg words, then the plane of tie words) and its gradient.  Activations belong to the built-in forward state; the gradients are backward scratch. */
 extern "C" int eld_unet_buffer(const eld_unet* u, const char* name, void** ptr, int dims[4], int* elem_bytes)
 {
     ELD_REQUIRE(u && name && ptr && dims && elem_bytes, "eld_unet_buffer: NULL argument");
@@ -820,6 +820,9 @@ extern "C" int eld_unet_buffer(const eld_unet* u, const char* name, void** ptr, 
     auto train_only = [&](const void* p, int lvl, int units, int eb) {
         ELD_REQUIRE(u->train, "eld_unet_buffer: '%s' exists only in a training workspace", name);
         return at(p, lvl, units, eb);
+    };
+    auto pool_ties = [&](const void* code, int lvl, int c) {   // the tie plane behind 32 bytes per (pixel, 32 channels)
+        return static_cast<const char*>(code) + (size_t)u->n * (u->H >> lvl) * (u->W >> lvl) * (c / 32) * 32;
     };
     auto is = [name](const char* prefix, const char* id) {     // name == prefix followed by id
         const size_t k = strlen(prefix);
@@ -838,14 +841,17 @@ extern "C" int eld_unet_buffer(const eld_unet* u, const char* name, void** ptr, 
             const char pool_lvl[2] = { char('1' + l.lvl), 0 };
             if (is("p", pool_lvl)) return at(fs.pool[l.lvl + 1], l.lvl + 1, l.cout, 2);
             if (is("pc", pool_lvl)) return train_only(fs.code[l.lvl + 1], l.lvl + 1, l.cout, 1);
+            if (is("pt", pool_lvl)) return train_only(pool_ties(fs.code[l.lvl + 1], l.lvl + 1, l.cout), l.lvl + 1, l.cout / 2, 1);
             if (is("dp", pool_lvl)) return train_only(u->dp[l.lvl + 1], l.lvl + 1, l.cout, 2);
         } else {
             if (is("a", l.name + 4)) return at(fs.act[i], l.lvl, l.cout, 2);
-            if (is("sign:a", l.name + 4) && fs.sign[i]) return at(fs.sign[i], l.lvl, l.cout / 32, 4);
+            if (is("sign:a", l.name + 4) && fs.slope[i]) return at(fs.slope[i], l.lvl, l.cout / 32, 4);
+            if (is("tie:a", l.name + 4) && fs.slope[i])
+                return at(fs.slope[i] + (size_t)u->n * (u->H >> l.lvl) * (u->W >> l.lvl) * (l.cout / 32), l.lvl, l.cout / 32, 4);
         }
     }
-    if (strncmp(name, "sign:", 5) == 0) {
-        set_error("eld_unet_buffer: no sign words '%s' in this workspace", name);
+    if (strncmp(name, "sign:", 5) == 0 || strncmp(name, "tie:", 4) == 0) {
+        set_error("eld_unet_buffer: no slope words '%s' in this workspace", name);
         return ELD_E_ARG;
     }
     if (strncmp(name, "wf:", 3) == 0 || strncmp(name, "wd:", 3) == 0) {   // packed bf16 operands of one layer

@@ -12,6 +12,11 @@ namespace eld {
 __device__ __forceinline__ float lrelu(float v) { return fmaxf(v, 0.2f * v); }
 __device__ __forceinline__ float bf_lo(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bf_hi(uint32_t w) { return __uint_as_float(w & 0xFFFF0000u); }
+// LeakyReLU' of a stored activation for the head's dz: 1, 0.2f, 0.6f at +-0 and +-Inf, 1.2f at NaN (wgmma.cuh lrelu_slope)
+__device__ __forceinline__ float head_slope(float a)
+{
+    return a > 0.f ? (a < INFINITY ? 1.0f : 0.6f) : a < 0.f ? (a > -INFINITY ? 0.2f : 0.6f) : a == 0.f ? 0.6f : 1.2f;
+}
 __device__ __forceinline__ uint32_t pack_bf2(float a, float b)
 {
     const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
@@ -21,15 +26,16 @@ __device__ __forceinline__ uint32_t pack_bf2(float a, float b)
 // ---------------------------------------------------------------------------------------------------
 // 2x2 max-pool backward, NHWC bf16                                                      (Unet.py:51-63)
 // ---------------------------------------------------------------------------------------------------
-// dZ[full res] = ( dskip + (first arg-max of the window ? dP : 0) ) * lrelu'(A)
-//   A     : activation that was pooled - never read: the forward tile's epilogue (conv_gemm.cuh) leaves a 1-byte-per-
+// dZ[full res] = ( dskip + (the window element MaxPool2d routes to ? dP : 0) ) * lrelu'(A)
+//   A     : activation that was pooled - never read: the forward tile's epilogue (conv_gemm.cuh) leaves a 1.5-byte-per-
 //           pooled-element code instead, per (pooled pixel, 32 channels) eight words - "not the maximum" masks of the
-//           window's four pixels, then their sign masks (channel 2j -> bit j, 2j+1 -> bit 16+j).  That is 1/16 of what
-//           the activation costs (and the level-1 skip half of an interleaved concat buffer cost double: 128-byte lines
-//           for 64 useful bytes).
+//           window's four pixels, then their `neg` slope words - and in a second plane four words, their `tie` slope
+//           words (wgmma.cuh slope_words; channel 2j -> bit j, 2j+1 -> bit 16+j).  That is 3/32 of what the activation costs (and the level-1 skip half of an interleaved
+//           concat buffer cost double: 128-byte lines for 64 useful bytes).
 //   dskip : gradient that reached A through the skip connection (pitch s_pitch, offset s_c0)
 //   dP    : gradient of the pooled tensor (compact)
-// PyTorch's max_pool2d backward routes to the FIRST maximum in window scan order; so do we.
+// PyTorch's max_pool2d propagates NaN and its backward routes to the LAST NaN of a window in scan order, else to the
+// FIRST maximum; so do we (a NaN element is the one whose neg and tie bits are both set).
 // 16 channels (32 bytes) per thread, moved as whole 32-byte sectors - C % 32 == 0, 32-byte aligned tensors.
 __global__ void __launch_bounds__(256)
 maxpool_bwd_code_kernel(const uint32_t* __restrict__ code, const __nv_bfloat16* __restrict__ dskip, int s_pitch, int s_c0,
@@ -46,27 +52,35 @@ maxpool_bwd_code_kernel(const uint32_t* __restrict__ code, const __nv_bfloat16* 
         const uint32_t n = r / (uint32_t)Ho;
         const size_t pix00 = ((size_t)n * 2 * Ho + 2 * yo) * (2 * Wo) + 2 * xo;
         const size_t offs[4] = { pix00, pix00 + 1, pix00 + (size_t)2 * Wo, pix00 + (size_t)2 * Wo + 1 };
-        uint32_t cw[8], s[4][8], dp[8];
-        ptx::ld_global_nc_32B(code + ((size_t)ppix * (groups >> 1) + (gch >> 1)) * 8, cw);
+        uint32_t cw[12], s[4][8], dp[8];
+        const size_t rec = (size_t)ppix * (groups >> 1) + (gch >> 1);
+        ptx::ld_global_nc_32B(code + rec * 8, cw);
+        const uint4 ct = __ldg(reinterpret_cast<const uint4*>(code + (size_t)total / 2 * 8 + rec * 4));   // total / 2 records
+        cw[8] = ct.x; cw[9] = ct.y; cw[10] = ct.z; cw[11] = ct.w;
 #pragma unroll
         for (int k = 0; k < 4; ++k) ptx::ld_global_nc_32B(dskip + offs[k] * s_pitch + s_c0 + gch * 16, s[k]);
         ptx::ld_global_nc_32B(dP + (size_t)ppix * C + gch * 16, dp);
         // this thread's 16 channels are pairs 8*(gch&1) .. +7 of the chunk: bring their bits to positions 0..7 / 16..23
         const uint32_t sh = (gch & 1u) * 8u;
         const uint32_t m0 = cw[0] >> sh, m1 = cw[1] >> sh, m2 = cw[2] >> sh;
-        // one-hot "first maximum in window order" (a NaN window has no maximum: the last pixel takes it)
-        const uint32_t sel[4] = { ~m0, m0 & ~m1, m0 & m1 & ~m2, m0 & m1 & m2 };
-        const uint32_t neg[4] = { cw[4] >> sh, cw[5] >> sh, cw[6] >> sh, cw[7] >> sh };
+        uint32_t neg[4], tie[4], nan[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) { neg[k] = cw[4 + k] >> sh; tie[k] = cw[8 + k] >> sh; nan[k] = neg[k] & tie[k]; }
+        // one-hot: the last NaN of a window that holds one, else the first maximum in window order
+        const uint32_t num = ~(nan[0] | nan[1] | nan[2] | nan[3]);
+        const uint32_t sel[4] = { (~m0 & num) | (nan[0] & ~(nan[1] | nan[2] | nan[3])),
+                                  (m0 & ~m1 & num) | (nan[1] & ~(nan[2] | nan[3])),
+                                  (m0 & m1 & ~m2 & num) | (nan[2] & ~nan[3]),
+                                  (m0 & m1 & m2 & num) | nan[3] };
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
             uint32_t o[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                // all-ones where this pixel won; slope = 0.6 + 0.4 * (+-1) = 1 or 0.2 from the sign
+                // all-ones where this pixel won
                 const uint32_t t_lo = (uint32_t)((int32_t)(sel[k] << (31 - j)) >> 31), t_hi = (uint32_t)((int32_t)(sel[k] << (15 - j)) >> 31);
                 const float g_lo = __uint_as_float((dp[j] << 16) & t_lo), g_hi = __uint_as_float((dp[j] & 0xFFFF0000u) & t_hi);
-                const float f_lo = __fmaf_rn(__uint_as_float(((neg[k] << (31 - j)) & 0x80000000u) | 0x3F800000u), 0.4f, 0.6f);
-                const float f_hi = __fmaf_rn(__uint_as_float(((neg[k] << (15 - j)) & 0x80000000u) | 0x3F800000u), 0.4f, 0.6f);
+                const float f_lo = lrelu_slope(neg[k], tie[k], j, kMaskNeg), f_hi = lrelu_slope(neg[k], tie[k], 16 + j, kMaskNeg);
                 const __nv_bfloat162 h = __floats2bfloat162_rn((bf_lo(s[k][j]) + g_lo) * f_lo, (bf_hi(s[k][j]) + g_hi) * f_hi);
                 o[j] = *reinterpret_cast<const uint32_t*>(&h);
             }
@@ -79,7 +93,8 @@ maxpool_bwd_code_kernel(const uint32_t* __restrict__ code, const __nv_bfloat16* 
 // head: conv10_1 (1x1, 32 -> 4, no activation; Unet.py:46,88) + L1 loss (losses.py:32) + its backward.
 //   out[n][co][y][x] (f32 NCHW) = b[co] + sum_ci a[p][ci] w[co][ci]
 //   loss += sum |out - t| / numel ;  dout = sign(out - t)/numel
-//   dz[p][ci] = (sum_co dout[co] w[co][ci]) * lrelu'(a[p][ci])     (bf16 NHWC, feeds conv9_2's backward)
+//   dz[p][ci] = (sum_co dout[co] w[co][ci]) * lrelu'(a[p][ci])     (bf16 NHWC, feeds conv9_2's backward; the slopes of
+//                                                                  wgmma.cuh lrelu_slope with 0.2f)
 //   dw[co][ci] += dout[co] a[p][ci] ; db[co] += dout[co]
 // One pixel per thread per iteration, persistent blocks; per-thread partial dW in registers.
 // ---------------------------------------------------------------------------------------------------
@@ -230,8 +245,8 @@ head_kernel(const __nv_bfloat16* __restrict__ a, const float* __restrict__ w, co
                     g0 = fmaf(dd[co], w4[co][j], g0);
                     g1 = fmaf(dd[co], w4[co][j + 1], g1);
                 }
-                g0 *= (av[j] > 0.f ? 1.0f : 0.2f);
-                g1 *= (av[j + 1] > 0.f ? 1.0f : 0.2f);
+                g0 *= head_slope(av[j]);
+                g1 *= head_slope(av[j + 1]);
                 zo[j >> 1] = pack_bf2(g0, g1);
             }
             if (valid && dz) reinterpret_cast<uint4*>(dz + (size_t)p * 32)[q] = make_uint4(zo[0], zo[1], zo[2], zo[3]);

@@ -113,10 +113,10 @@ static int conv_gemm_params(const GemmOp& op, ConvGemmParams& p)
     p.out = static_cast<__nv_bfloat16*>(op.out); p.out_pitch = op.out_pitch; p.out_c0 = op.out_c0;
     p.bias = op.bias;
     p.aux = static_cast<const __nv_bfloat16*>(op.aux); p.aux_pitch = op.aux_pitch; p.aux_c0 = op.aux_c0;
-    ELD_REQUIRE(op.aux_sign == nullptr || (op.act == ACT_MASK && store), "conv tile: sign words are a mask source of a plain store epilogue");
-    ELD_REQUIRE(op.sign_out == nullptr || (op.act == ACT_LRELU && store && op.out_split == 0),
-                "conv tile: sign words are written behind LeakyReLU by a plain store epilogue");
-    p.aux_sign = static_cast<const uint32_t*>(op.aux_sign); p.sign_out = static_cast<uint32_t*>(op.sign_out);
+    ELD_REQUIRE(op.aux_slope == nullptr || (op.act == ACT_MASK && store), "conv tile: slope words are a mask source of a plain store epilogue");
+    ELD_REQUIRE(op.slope_out == nullptr || (op.act == ACT_LRELU && store && op.out_split == 0),
+                "conv tile: slope words are written behind LeakyReLU by a plain store epilogue");
+    p.aux_slope = static_cast<const uint32_t*>(op.aux_slope); p.slope_out = static_cast<uint32_t*>(op.slope_out);
     p.cout = op.cout;
     ELD_REQUIRE(op.pool_out == nullptr || (store && op.H % 2 == 0 && op.W % 2 == 0),
                 "conv tile: the fused max pool needs a plain store epilogue and even H, W");
@@ -132,8 +132,8 @@ static int conv_gemm_params(const GemmOp& op, ConvGemmParams& p)
     // A prefix starts at row 0 of every block and covers whole 32-row groups, so each tile's rows keep the swizzle
     // phase (row & 7, or (row >> 1) & 3) they were packed with.
     ELD_REQUIRE(op.b_block_rows == 0 || (op.b_block_rows % 32 == 0 && op.b_block_rows <= 256 &&
-                                         (n_total <= op.b_block_rows || op.b_block_rows == 256) && op.aux_sign == nullptr),
-                "conv tile: a row prefix of the packed operand needs whole 32-row groups of its blocks and no sign-word mask");
+                                         (n_total <= op.b_block_rows || op.b_block_rows == 256) && op.aux_slope == nullptr),
+                "conv tile: a row prefix of the packed operand needs whole 32-row groups of its blocks and no slope-word mask");
     // a whole operand of more than 256 rows is whole 256-row blocks (packed_index gives every block a full 256-row slot)
     ELD_REQUIRE(op.b_block_rows != 0 || n_total <= 256 || n_total % 256 == 0,
                 "conv tile: GEMM N=%d above 256 must be a multiple of 256", n_total);
@@ -252,13 +252,13 @@ static size_t first_conv_smem(bool wgrad)
 
 // conv1_1 (4 -> 32): software-im2col wgmma tiles on the fp32 NCHW frame (first_conv.cuh)
 int launch_first_conv(eld_ctx* ctx, const float* x, int cin, const void* w_img, const float* bias, void* out, int out_pitch,
-                      int n, int H, int W, cudaStream_t st, void* sign_out)
+                      int n, int H, int W, cudaStream_t st, void* slope_out)
 {
     ELD_REQUIRE(H % 8 == 0 && W % 16 == 0, "first conv tile: H=%d must be a multiple of 8 and W=%d of 16", H, W);
     FirstConvParams p{};
     p.x = x; p.n_img = n; p.H = H; p.W = W; p.tiles_x = W / 16; p.tiles_y = H / 8; p.cin = cin;
     p.w_img = static_cast<const uint8_t*>(w_img); p.bias = bias;
-    p.out = static_cast<__nv_bfloat16*>(out); p.out_pitch = out_pitch; p.sign_out = static_cast<uint32_t*>(sign_out);
+    p.out = static_cast<__nv_bfloat16*>(out); p.out_pitch = out_pitch; p.slope_out = static_cast<uint32_t*>(slope_out);
     const int total = n * p.tiles_x * p.tiles_y;
     CUtensorMap tmX;
     { int rc = encode_frame(ctx, &tmX, x, cin, n, H, W); if (rc) return rc; }

@@ -87,11 +87,11 @@ struct GemmOp {
     const float* bias;
     const void* aux;
     int aux_pitch, aux_c0;
-    const void* aux_sign = nullptr;   // ACT_MASK from sign words (uint32 [pixel][GEMM N / 32]) instead of `aux`
-    void* sign_out = nullptr;         // ACT_LRELU, not the deconv: also write the output's sign words
+    const void* aux_slope = nullptr;   // ACT_MASK from slope words (uint32 pairs [pixel][GEMM N / 32]) instead of `aux`
+    void* slope_out = nullptr;         // ACT_LRELU, not the deconv: also write the output's slope words
     void* pool_out = nullptr;   // optional fused 2x2 max pool of the activated output (not the deconv)
     int pool_pitch = 0;
-    void* pool_code = nullptr;  // optional with pool_out: 1 byte per pooled element (argmax + signs) for the pool backward
+    void* pool_code = nullptr;  // optional with pool_out: 1.5 bytes per pooled element (maxima + slope words) for the pool backward
     void* out2 = nullptr;       // split store (not the deconv): columns >= out_split go to out2 (planar halves of a concat
                                 // gradient)
     int out2_pitch = 0, out_split = 0;
@@ -114,7 +114,7 @@ int init_gemm_kernels(eld_ctx* ctx);   // opt in to large dynamic smem (call onc
 int launch_wgrad(eld_ctx* ctx, const WgradOp& op, cudaStream_t st);
 int launch_conv_gemm(eld_ctx* ctx, const GemmOp& op, cudaStream_t st);
 int launch_first_conv(eld_ctx* ctx, const float* x, int cin, const void* w_img, const float* bias, void* out, int out_pitch,
-                      int n, int H, int W, cudaStream_t st, void* sign_out = nullptr);
+                      int n, int H, int W, cudaStream_t st, void* slope_out = nullptr);
 int launch_first_conv_wgrad(eld_ctx* ctx, const float* x, int cin, const void* dz, int dz_pitch, float* dw, float* db,
                             int n, int H, int W, cudaStream_t st);
 // conv1_1's data gradient: dz bf16 NHWC [n][H][W][32], w f32 OIHW [32][cin][3][3] -> dx f32 NCHW [n][cin][H][W]

@@ -187,5 +187,35 @@ __device__ __forceinline__ uint32_t gather_msb16(const uint32_t (&w)[16])
     return (a[0] | a[1]) | (a[2] | a[3]);
 }
 
+// ---- LeakyReLU' of a stored activation ----------------------------------------------------------------------------
+// The reference's LeakyReLU is torch.max(0.2 x, x); autograd of the max gives d/dx = 1 for x > 0, 0.2 for x < 0, 0.6 where
+// its two arguments tie (x = +-0 or +-Inf: each takes half the gradient) and 1.2 for NaN (both take all of it).  The
+// stored bf16 activation has the class of x.  Two bits per element carry it: `neg` = negative and finite, or NaN, and
+// `tie` = +-0, +-Inf or NaN.  slope_words turns 16 packed bf16x2 words into the two words, in the channel layout of
+// gather_msb16 (the slope words and pool codes).
+__device__ __forceinline__ void slope_words(const uint32_t (&w)[16], uint32_t& neg, uint32_t& tie)
+{
+    // per 16-bit half, in its top bit (all gather_msb16 reads; the 15-bit magnitudes never carry or borrow across
+    // halves): magnitude >= 0x7F80 (Inf, NaN) | magnitude == 0, and magnitude > 0x7F80 (NaN)
+    uint32_t n[16], t[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        const uint32_t mag = w[j] & 0x7FFF7FFFu;
+        t[j] = (mag + 0x00800080u) | (0x80008000u - mag);
+        n[j] = (mag + 0x007F007Fu) | (w[j] & ~t[j]);
+    }
+    neg = gather_msb16(n);
+    tie = gather_msb16(t);
+}
+
 }  // namespace ptx
+
+// the slope of bit `b` of a (neg, tie) pair; neg_slope: the kernel's constant for the negative branch
+__device__ __forceinline__ float lrelu_slope(uint32_t neg, uint32_t tie, int b, float neg_slope)
+{
+    const bool n = (neg >> b) & 1u, t = (tie >> b) & 1u;
+    return t ? (n ? 1.2f : 0.6f) : (n ? neg_slope : 1.0f);
+}
+// the conv and pool masks' negative slope: fmaf(-1, 0.4f, 0.6f), exact (Sterbenz), one ulp above 0.2f
+constexpr float kMaskNeg = 0.6f - 0.4f;
 }  // namespace eld

@@ -25,7 +25,8 @@ int eld_pack_weights(eld_ctx* ctx, const float* w, void* packed_bf16, int cout, 
 
 #define ELD_ACT_NONE  0
 #define ELD_ACT_LRELU 1  /* max(0.2x, x)  (Unet.py:102-104), fused into the producing tile           */
-#define ELD_ACT_MASK  2  /* multiply by d lrelu/dx of `aux` (1 if aux>0 else 0.2): backward of lrelu */
+#define ELD_ACT_MASK  2  /* multiply by d lrelu/dx of `aux`, autograd of max(0.2x, x): 1 if aux > 0, 0.2 if aux < 0,
+                          * 0.6 at +-0 and +-Inf (the arguments tie), 1.2 at NaN: backward of lrelu */
 
 /* y[n,h,w,y_c0:y_c0+cout] = act( conv3x3_pad1(x[n,h,w,x_c0:x_c0+cin]) + bias )   nn.Conv2d(k=3,p=1), Unet.py:11-44.
  * With ELD_PACK_CONV_DGRAD weights (cin/cout swapped) the same tile is the data gradient.
@@ -74,9 +75,9 @@ typedef struct eld_unet eld_unet;
 size_t eld_unet_param_count(void);                                   /* 7,760,484 for UNetSeeInDark(4,4) */
 int    eld_unet_param_offset(const char* layer, int is_bias, size_t* offset, size_t* count);
 size_t eld_unet_workspace_bytes(int n, int h, int w, int train);     /* activations (+gradients) + packed weights; train = 1 also
-                                                                      * holds what the forward tiles leave for the backward: sign
-                                                                      * words (1 bit per masked activation element) and pool codes
-                                                                      * (1 byte per pooled element: argmax + signs) */
+                                                                      * holds what the forward tiles leave for the backward: slope
+                                                                      * words (2 bits per masked activation element) and pool codes
+                                                                      * (1.5 bytes per pooled element: maxima + slope bits) */
 /* Inference (train = 0): h % 16 == 0 and w % 16 == 0, as for the reference network.  Training (train = 1):
  * h % 128 == 0, w % 256 == 0.  Both: n * h * w < 2^26 pixels (the head's 32-bit index), or ELD_E_ARG before the
  * workspace is looked at - e.g. at most 255 frames of 512 x 512.  The caller owns `workspace` (device memory) for the
@@ -114,7 +115,7 @@ int    eld_unet_backward(eld_unet* u, const float* params, const float* x, const
  * created with train = 0 and when no backward or train step has run since the last forward. */
 int    eld_unet_input_grad(eld_unet* u, const float* params, float* dx, void* stream);
 /* Several forwards before their backwards (a loss that calls the network twice, torch.utils.checkpoint, a retained
- * graph): what a forward leaves for its backward - activations, pool codes, sign words, packed weights - is its FORWARD
+ * graph): what a forward leaves for its backward - activations, pool codes, slope words, packed weights - is its FORWARD
  * STATE.  A train = 1 object holds one in its workspace (the built-in state, which eld_unet_forward / eld_unet_backward /
  * eld_unet_train_step use); a caller may give a forward a state of its own and later back-propagate from that state,
  * whatever ran on the object in between.  state == NULL means the built-in state, so eld_unet_forward(u, ...) is
@@ -171,8 +172,9 @@ int    eld_unet_profile_read(eld_unet* u, int max, char* names32, float* ms, dou
 /* Where intermediate tensor `name` of the last step lives in the caller's workspace (for tests and debugging; no launch,
  * no synchronisation).  dims = {n, h, w, units per pixel}, *elem_bytes = 2 (bf16) / 4 (f32, uint32) / 1 (bytes).
  * Names: activations a1_1, cat9, p1, ... a9_2; gradients dz9_2 ... dz1_1, dcat9 ... dcat6 (the whole planar buffer: up
- * plane [n][h][w][units/2], then the skip plane), dp1 ... dp4; pool codes pc1 ... pc4 (one byte per pooled element);
- * sign words sign:<activation> (uint32, one per pixel and 32 channels); packed operands wf:<layer>, wd:<layer> (dims
+ * plane [n][h][w][units/2], then the skip plane), dp1 ... dp4; pool codes pc1 ... pc4 (one byte per pooled element:
+ * maxima and neg bits) and pt1 ... pt4 (half a byte: tie bits); slope words sign:<activation> (neg bits) and
+ * tie:<activation> (uint32, one per pixel and 32 channels each); packed operands wf:<layer>, wd:<layer> (dims
  * {1, 1, 1, element count}); the [tap][ci][co] staging of the conv weight gradients gtmp (f32, parameter offsets).
  * ELD_E_ARG for an unknown name and, on an object created with train = 0, for a training-only one. */
 int    eld_unet_buffer(const eld_unet* u, const char* name, void** ptr, int dims[4], int* elem_bytes);

@@ -42,16 +42,18 @@ def integer_weights(module, fan_in, seed):
     """Fill the U-Net `module` (arch.unet or the oracle module: the same parameter names) with an integer network:
     every output of every layer is the sum of `fan_in` inputs picked at seeded positions (a conv3x3 output channel:
     (tap, input channel) pairs; a deconv output channel: input channels per sub-pixel; the head: input channels), that
-    is weights in {0, 1}.  Biases are 0 except conv9_2's, which are 1: the head's LeakyReLU' is a > 0, so a9_2 must not
-    hold a zero (a slope of 0.2f would take dz9_2 off the dyadic grid).  On integer frames every activation is then a
-    non-negative integer, LeakyReLU's negative branch is never taken, and every gradient stays on the grid of dOut."""
+    is weights in {0, 1}.  The biases of the convolutions are 1 (a 3x3 tap may pick the zero padding), those of the
+    deconvolutions and the head 0 (the smallest activations, and the sums every gradient runs over, stay small).  On
+    non-negative integer frames every LeakyReLU input is then an integer >= 1: none sits on the kink (at 0 the
+    reference's slope is 0.6, off the dyadic grid) or on the negative branch, every slope is 1, and every gradient
+    stays on the grid of dOut."""
     import torch
     g = torch.Generator().manual_seed(seed)
     with torch.no_grad():
         for name, p in module.named_parameters():
             layer, kind = name.split('.')
             if kind == 'bias':
-                p.fill_(1.0 if layer == 'conv9_2' else 0.0)
+                p.fill_(0.0 if layer.startswith('upv') or layer == 'conv10_1' else 1.0)
                 continue
             w = torch.zeros(p.shape)
             if layer.startswith('upv'):            # IOHW: per (co, sub-pixel), fan_in input channels
@@ -75,19 +77,23 @@ def integer_net(cin=4, cout=4, fan_in=1, seed=7):
 
 
 def integer_frames(n, cin, h, w, seed):
-    """integer frames 0..3 as fp32 [n, cin, h, w] on the GPU"""
+    """integer frames 0..1 as fp32 [n, cin, h, w] on the GPU (small: the integer network's biases add 1 per layer, and
+    the weight gradients of the 8 x 512^2 step must stay provably exact)"""
     import torch
     g = torch.Generator().manual_seed(seed)
-    return torch.randint(0, 4, (n, cin, h, w), generator=g).float().cuda()
+    return torch.randint(0, 2, (n, cin, h, w), generator=g).float().cuda()
 
 
 def half_off(out, seed):
-    """a target 0.5 above or below each element of the integer output `out`, the side drawn from `seed`: the L1 loss
-    never sits on a tie, |e| = 1/2 keeps the loss's sum provable at any size, and MSE's 2 e is +-1"""
+    """a target 0.5 above or below a quarter of the elements of the integer output `out` and equal to the rest, drawn
+    from `seed`: |e| = 1/2 or 0 keeps the loss's sum provable at any size, MSE's 2 e is +-1 or 0, and the L1 head's
+    sign(0) = 0, as torch's.  The zeros keep the sums of the weight gradients below 2^24 units of their grid at the
+    8 x 512^2 step, where the integer network's activations (1 more per layer) reach 20 and more."""
     import torch
     g = torch.Generator().manual_seed(seed)
-    side = torch.randint(0, 2, out.shape, generator=g).float().to(out.device)
-    return out + side - 0.5
+    side = torch.randint(0, 8, out.shape, generator=g).float()
+    side = torch.where(side == 0, -0.5, torch.where(side == 1, 0.5, 0.0)).to(out.device)
+    return out + side
 
 
 def spread_biases(ours, ref, seed=5):

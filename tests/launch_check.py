@@ -79,7 +79,7 @@ class Step:
     launch still computes them (one launch per layer), but their range of grads must read zero.
     stats: the caller's table {launch kind: {statistic: worst value}}, which every check raises to what it measured.
     frames: None - every output is checked on the whole batch at once.  Or the frames on which the outputs computed one
-    image at a time (fprop, dgrad, pool backward, sign words, pool codes, the head's out and dz9_2) are checked, one
+    image at a time (fprop, dgrad, pool backward, slope words, pool codes, the head's out and dz9_2) are checked, one
     frame and one band of at most BAND_PX pixels at a time; the batch sums (weight and bias gradients, the loss) are
     then built from pieces of at most SUM_FRAMES frames and SUM_PX pixels (tests/batch_ref.py), so that a batch whose
     float64 image would not fit beside its workspace can be checked."""
@@ -220,14 +220,18 @@ class Step:
         st['ulp_ratio'] = max(st['ulp_ratio'], ratio)
         st['mismatch'] = max(st['mismatch'], mism)
         if not (ratio <= 1.0 and mism <= MISMATCH[kind]) or not finite:
-            self.fail.append('%s (%s): max |got-r|/(ulp+2^-20 S) = %.3g, mismatch %.3g' % (where, kind, ratio, mism))
+            self.fail.append('%s (%s): max |got-r|/(ulp+2^-20 S) = %.3g, mismatch %.3g%s' % (
+                where, kind, ratio, mism, '' if finite else ', NaN / Inf positions differ'))
         if exact is not None:
             self.provable(kind, where, got, exact[0], S, exact[1])
 
     def f32(self, kind, where, got, r, S, q=None):
         """q: the grid of the launch's products, for the exact rule on the provable elements"""
-        from tests.launch_ref import f32_rule
+        from tests.launch_ref import f32_rule, nonfinite_mismatch
         rel, mx, ms = f32_rule(got, r, S)
+        bad = nonfinite_mismatch(got, r)
+        if bad:
+            self.fail.append('%s (%s): %d elements differ in NaN / Inf' % (where, kind, bad))
         st = self.stats['fp32 ' + kind + self.tag]
         st['rel_l2'] = max(st['rel_l2'], rel)
         st['max_abs_rel'] = max(st['max_abs_rel'], mx)
@@ -290,18 +294,26 @@ class Step:
         self.epilogue_extras(layer, dst, got)
 
     def epilogue_extras(self, layer, dst, got):
-        """the fused pool, its code and the sign words, all from the STORED output"""
+        """the fused pool, its code and the slope words, all from the STORED output"""
         import tests.launch_ref as R
         if layer in POOLED:
             p, pc = POOLED[layer]
             m, _, _ = R.pool(got)
-            self.exact('pool', p, self.bits(self.rows(self.V(p))), self.bits(m.bfloat16()))
+            # every NaN as the same one: a NaN's payload is not part of the result
+            nan = lambda t: self.t.where(self.t.isnan(t), self.t.full_like(t, float('nan')), t)   # noqa: E731
+            self.exact('pool', p, self.bits(nan(self.rows(self.V(p)))), self.bits(nan(m.bfloat16())))
             if self.training:
                 code = self.rows(self.V(pc))
                 n, h, w, c = code.shape
-                self.exact('pool code', pc, code.reshape(-1).view(self.t.int32).view(n, h, w, c // 32, 8), R.pool_code(got))
+                want = R.pool_code(got)
+                self.exact('pool code', pc, code.reshape(-1).view(self.t.int32).view(n, h, w, c // 32, 8), want[..., :8])
+                ties = self.rows(self.V('pt' + pc[2:]))
+                self.exact('pool code', 'pt' + pc[2:], ties.reshape(-1).view(self.t.int32).view(n, h, w, c // 32, 4),
+                           want[..., 8:])
         if self.training and dst in SIGNED:
-            self.exact('sign words', 'sign:' + dst, self.rows(self.V('sign:' + dst)), R.sign_words(got))
+            want = R.slope_words(got)
+            self.exact('sign words', 'sign:' + dst, self.rows(self.V('sign:' + dst)), want[..., 0])
+            self.exact('tie words', 'tie:' + dst, self.rows(self.V('tie:' + dst)), want[..., 1])
 
     @property
     def training(self):

@@ -20,15 +20,15 @@ _DT = {1: torch.uint8, 2: torch.bfloat16, 4: torch.float32}
 
 
 def buffer(lib, eng, ws, name):
-    """torch view [n, h, w, units] of tensor `name` inside workspace `ws` (uint8 tensor) of engine `eng`; sign words
-    are int32, pool codes uint8, gtmp float32, everything else bf16.  Raises EldError for a name the engine lacks."""
+    """torch view [n, h, w, units] of tensor `name` inside workspace `ws` (uint8 tensor) of engine `eng`; sign and tie
+    words are int32, pool codes uint8, gtmp float32, everything else bf16.  Raises EldError for a name the engine lacks."""
     from eld_b200 import _lib
     ptr, dims, eb = ctypes.c_void_p(), (ctypes.c_int * 4)(), ctypes.c_int()
     _lib.check(lib.eld_unet_buffer(eng, name.encode(), ctypes.byref(ptr), dims, ctypes.byref(eb)), 'eld_unet_buffer')
     n, h, w, u = list(dims)
     off, count = ptr.value - ws.data_ptr(), n * h * w * u * eb.value
     assert 0 <= off and off + count <= ws.numel(), (name, off, count, ws.numel())
-    dt = torch.int32 if name.startswith('sign:') else _DT[eb.value]
+    dt = torch.int32 if name.startswith(('sign:', 'tie:')) else _DT[eb.value]
     return ws[off:off + count].view(dt).view(n, h, w, u)
 
 
@@ -44,15 +44,27 @@ def ulp_bf16(r):
     return torch.ldexp(torch.ones_like(r), (e - 8).to(torch.int32))
 
 
+def nonfinite_mismatch(got, r):
+    """the number of elements where got and r differ in what is not a finite number: NaN must meet NaN, and +-Inf the
+    same infinity; a finite number must meet a finite number"""
+    g, r = got.double().reshape(r.shape), r.double()
+    fin = torch.isfinite(g) & torch.isfinite(r)
+    same = fin | (torch.isnan(g) & torch.isnan(r)) | (torch.isinf(g) & (g == r))
+    return int((~same).sum().item())
+
+
 def bf16_rule(got, r, S):
     """the statistics of the bf16 rule for a bf16 output `got` against the float64 value r before the kernel's single
-    rounding and its scale S: (max |got - r| / (ulp_bf16(r) + 2^-20 S), share of elements that differ from
-    round-to-nearest-even(r), every element finite)"""
+    rounding and its scale S: (max |got - r| / (ulp_bf16(r) + 2^-20 S) and the share of elements that differ from
+    round-to-nearest-even(r), both over the elements where got and r are finite; whether every other element matches
+    as nonfinite_mismatch asks)"""
     assert got.shape == r.shape, (got.shape, r.shape)
     g = got.double()
-    ratio = ((g - r).abs() / (ulp_bf16(r) + 2.0 ** -20 * S)).max().item()
-    mism = (got != r.float().bfloat16()).double().mean().item()
-    return ratio, mism, bool(torch.isfinite(g).all())
+    fin = torch.isfinite(g) & torch.isfinite(r) & torch.isfinite(S)
+    gf, rf, sf = g[fin], r[fin], S[fin]
+    ratio = ((gf - rf).abs() / (ulp_bf16(rf) + 2.0 ** -20 * sf)).max().item() if gf.numel() else 0.0
+    mism = (got[fin] != rf.float().bfloat16()).double().sum().item() / max(got.numel(), 1)
+    return ratio, mism, nonfinite_mismatch(got, r) == 0
 
 
 def exact_rule(got, want, mask):
@@ -62,22 +74,41 @@ def exact_rule(got, want, mask):
     if want.dtype == torch.float64:
         same = got.double().reshape(want.shape) == want
     else:
-        same = (got.view(torch.int16) == want.view(torch.int16)) | ((got == 0) & (want == 0))
+        same = (got.view(torch.int16) == want.view(torch.int16)) | ((got == 0) & (want == 0)) | \
+            (torch.isnan(got) & torch.isnan(want))
     return int((mask & ~same).sum().item())
 
 
 def f32_rule(got, r, S):
-    """the statistics of the fp32 rule: (rel-L2 of got - r, max |got - r| / max |r|, max |got - r| / S)"""
-    d = got.double().reshape(r.shape) - r
+    """the statistics of the fp32 rule over the elements where got and r are finite: (rel-L2 of got - r,
+    max |got - r| / max |r|, max |got - r| / S); the other elements are nonfinite_mismatch's"""
+    g = got.double().reshape(r.shape)
+    fin = torch.isfinite(g) & torch.isfinite(r) & torch.isfinite(S)
+    if not bool(fin.any()):
+        return 0.0, 0.0, 0.0
+    g, r, S = g[fin], r[fin], S[fin]
+    d = g - r
     rel = (d.norm() / r.norm().clamp_min(1e-300)).item()
     mx = (d.abs().max() / r.abs().max().clamp_min(1e-300)).item()
     ms = (d.abs() / S.clamp_min(1e-300)).max().item()
     return rel, mx, ms
 
 
-def slope(a):
-    """LeakyReLU' from the sign of the stored activation: 1, or 0.2 where the sign bit is set (+0 counts positive)"""
-    return 1.0 - 0.8 * torch.signbit(a.float()).double()
+def slope_class(a):
+    """(neg, tie) of the stored activation a: neg = negative and finite, or NaN; tie = +-0, +-Inf or NaN (where
+    0.2 a == a or the comparison is unordered)"""
+    a = a.double()
+    nan, tie = torch.isnan(a), (a == 0) | torch.isinf(a) | torch.isnan(a)
+    return nan | ((a < 0) & ~tie), tie
+
+
+def slope(a, neg=0.2):
+    """LeakyReLU' of the reference's torch.max(0.2 x, x) from the stored activation, as autograd of the max gives it:
+    1 (x > 0), `neg` (x < 0), 0.6 at +-0 and +-Inf (the two arguments tie and split the gradient), 1.2 at NaN (both
+    take all of it)"""
+    n, t = slope_class(a)
+    one = torch.ones_like(a, dtype=torch.float64)
+    return torch.where(t, torch.where(n, 1.2 * one, 0.6 * one), torch.where(n, neg * one, one))
 
 
 # ---- exactly summable operands ---------------------------------------------------------------------------------------
@@ -112,7 +143,14 @@ def exact_mask(S, q):
 
 # the float32 constants of the kernels' epilogues (csrc/conv_gemm.cuh conv_epilogue32, csrc/unet_ew.cu)
 F32_02 = float(np.float32(0.2))                                # fmaxf(v, 0.2f * v), the head's 0.2f
-MASK_NEG = float(np.float32(0.6) - np.float32(0.4))            # fmaf(-1, 0.4f, 0.6f): exact (Sterbenz), not 0.2f
+MASK_NEG = float(np.float32(0.6) - np.float32(0.4))            # the masks' kMaskNeg = 0.6f - 0.4f: exact (Sterbenz), not 0.2f
+F32_06, F32_12 = float(np.float32(0.6)), float(np.float32(1.2))   # lrelu_slope's 0.6f (tie) and 1.2f (NaN)
+
+
+def f32_slope(a, neg):
+    """the kernels' float32 LeakyReLU' of the stored activation a (wgmma.cuh lrelu_slope): 1, neg, 0.6f, 1.2f"""
+    n, t = slope_class(a)
+    return torch.where(t, torch.where(n, F32_12, F32_06), torch.where(n, neg, 1.0)).float()
 
 
 def _f32(t, c):
@@ -131,27 +169,33 @@ def epi_store(z, b=None, act=False):
 
 
 def epi_mask(z, act):
-    """dgrad epilogue: the exact accumulator z times fmaf(+-1, 0.4f, 0.6f) from the sign bit of the stored activation
-    (+0 counts positive; None: no mask), round to bf16"""
+    """dgrad epilogue: the exact accumulator z times f32_slope(act, MASK_NEG) of the stored activation (None: no
+    mask), round to bf16"""
     v = z.float()
     if act is not None:
-        v = v * torch.where(torch.signbit(act.float()), _f32(v, MASK_NEG), _f32(v, 1.0))
+        v = v * f32_slope(act, MASK_NEG).to(v.device)
     return v.bfloat16()
 
 
-def epi_pool_bwd(a, dskip, dp):
-    """maxpool_bwd_code_kernel: (dskip + (first arg-max ? dp : +0)) * fmaf(+-1, 0.4f, 0.6f) in float32, round to bf16"""
-    _, _, first = pool(a)
+def _route(a, dp, zero):
+    """dp [n,h/2,w/2,c] routed to the window element MaxPool2d's backward picks (pool's one-hot), `zero` elsewhere
+    -> [n,h,w,c] (a where, not a product: a NaN of dp must not reach the other three elements)"""
+    _, _, pick = pool(a)
     n, h, w, c = a.shape
-    g = torch.where(first, dp.float().unsqueeze(-1), _f32(a, 0.0)).reshape(n, h // 2, w // 2, c, 2, 2)
-    g = g.permute(0, 1, 4, 2, 5, 3).reshape(n, h, w, c)
+    g = torch.where(pick, dp.unsqueeze(-1), zero).reshape(n, h // 2, w // 2, c, 2, 2)
+    return g.permute(0, 1, 4, 2, 5, 3).reshape(n, h, w, c)
+
+
+def epi_pool_bwd(a, dskip, dp):
+    """maxpool_bwd_code_kernel: (dskip + (routed ? dp : +0)) * f32_slope(a, MASK_NEG) in float32, round to bf16"""
+    g = _route(a, dp.float(), _f32(a, 0.0))
     return epi_mask((dskip.float() + g).double(), a)
 
 
 def epi_head_dz(z, a):
-    """head_kernel's dz9_2: the exact sum z over the four outputs times (a > 0 ? 1 : 0.2f), round to bf16"""
+    """head_kernel's dz9_2: the exact sum z over the four outputs times f32_slope(a, 0.2f), round to bf16"""
     v = z.float()
-    return (v * torch.where(a.float() > 0, _f32(v, 1.0), _f32(v, F32_02))).bfloat16()
+    return (v * f32_slope(a, F32_02).to(v.device)).bfloat16()
 
 
 def lrelu(v):
@@ -243,14 +287,18 @@ def first_conv_fprop(frame, w, b):
 
 
 def pool(a):
-    """MaxPool2d(2) of the stored activation a [n,h,w,c] -> (pooled [n,h/2,w/2,c] exact, window [..., 4] in the order
-    (0,0) (0,1) (1,0) (1,1), one-hot first arg-max [..., 4])"""
+    """MaxPool2d(2) of the stored activation a [n,h,w,c] as F.max_pool2d computes it -> (pooled [n,h/2,w/2,c] exact,
+    NaN where the window holds one; window [..., 4] in the order (0,0) (0,1) (1,0) (1,1); the one-hot element the
+    backward routes to [..., 4]: the LAST NaN of a window that holds one, else the first maximum)"""
     n, h, w, c = a.shape
     win = a.float().reshape(n, h // 2, 2, w // 2, 2, c).permute(0, 1, 3, 5, 2, 4).reshape(n, h // 2, w // 2, c, 4)
-    m = win.amax(-1)
+    nan = torch.isnan(win)
+    has_nan = nan.any(-1)
+    m = torch.where(has_nan, float('nan'), torch.where(nan, -math.inf, win).amax(-1))
     eq = win == m.unsqueeze(-1)
     first = eq & (eq.int().cumsum(-1) == 1)
-    return m, win, first
+    last_nan = nan & (nan.flip(-1).int().cumsum(-1).flip(-1) == 1)
+    return m, win, torch.where(has_nan.unsqueeze(-1), last_nan, first)
 
 
 def _pack_bits(bits):
@@ -261,21 +309,26 @@ def _pack_bits(bits):
     return torch.where(w >= 2 ** 31, w - 2 ** 32, w).int()
 
 
-def sign_words(a):
-    """sign words of the stored activation a [n,h,w,c] -> int32 [n,h,w,c/32]"""
+def slope_words(a):
+    """slope words of the stored activation a [n,h,w,c] -> int32 [n,h,w,c/32,2]: the neg and tie bits of
+    slope_class (the engine's planes sign:<activation> and tie:<activation>)"""
     n, h, w, c = a.shape
-    return _pack_bits(torch.signbit(a.float()).reshape(n, h, w, c // 32, 32))
+    neg, tie = slope_class(a)
+    return torch.stack([_pack_bits(neg.reshape(n, h, w, c // 32, 32)), _pack_bits(tie.reshape(n, h, w, c // 32, 32))], -1)
 
 
 def pool_code(a):
-    """the 32-byte pool code per (pooled pixel, 32 channels) as int32 [n,h/2,w/2,c/32,8]: words 0-3 = "is not the
-    window's maximum" of the window elements (0,0) (0,1) (1,0) (1,1), words 4-7 = their sign bits (channel bits as in
-    sign_words).  The pool backward takes the first window element whose bit is clear."""
+    """the 48-byte pool code per (pooled pixel, 32 channels) as int32 [n,h/2,w/2,c/32,12]: words 0-3 = "is not the
+    window's maximum" of the window elements (0,0) (0,1) (1,0) (1,1) (an ordered comparison: all clear in a window that
+    holds NaN), words 4-7 their neg bits (the engine's pcN), words 8-11 their tie bits (ptN; channel bits as in
+    slope_words).  The pool
+    backward takes the last element whose neg and tie bits are both set (NaN), else the first whose "not" bit is
+    clear."""
     m, win, _ = pool(a)
     n, h2, w2, c, _ = win.shape
-    ne = (win != m.unsqueeze(-1)).reshape(n, h2, w2, c // 32, 32, 4)
-    sg = torch.signbit(win).reshape(n, h2, w2, c // 32, 32, 4)
-    return torch.stack([_pack_bits(ne[..., k]) for k in range(4)] + [_pack_bits(sg[..., k]) for k in range(4)], -1)
+    ne = ((win < m.unsqueeze(-1)) | (win > m.unsqueeze(-1))).reshape(n, h2, w2, c // 32, 32, 4)
+    neg, tie = (t.reshape(n, h2, w2, c // 32, 32, 4) for t in slope_class(win))
+    return torch.stack([_pack_bits(b[..., k]) for b in (ne, neg, tie) for k in range(4)], -1)
 
 
 def deconv_fprop(x, wt, b):
@@ -310,11 +363,8 @@ def deconv_dgrad(dy, wt, act=None):
 
 
 def pool_bwd(a, dskip, dp):
-    """dZ = (dskip + dp routed to the first arg-max of its window) * LeakyReLU'(a); a = the pooled activation"""
-    _, _, first = pool(a)
-    n, h, w, c = a.shape
-    g = (first.double() * dp.double().unsqueeze(-1)).reshape(n, h // 2, w // 2, c, 2, 2)
-    g = g.permute(0, 1, 4, 2, 5, 3).reshape(n, h, w, c)
+    """dZ = (dskip + dp routed as F.max_pool2d's backward routes it) * LeakyReLU'(a); a = the pooled activation"""
+    g = _route(a, dp.double(), torch.zeros((), dtype=torch.float64, device=a.device))
     s = slope(a)
     r = (dskip.double() + g) * s
     return r, (dskip.double().abs() + g.abs()) * s
@@ -364,10 +414,10 @@ def head_loss(out, target, kind):
 
 
 def head_bwd(a, w, dout):
-    """-> (dz9_2 r, S, dW10, S_w, db10, S_b): dout [n,co,h,w] (fp32), a stored bf16 a9_2; a9_2's LeakyReLU' is a > 0"""
+    """-> (dz9_2 r, S, dW10, S_w, db10, S_b): dout [n,co,h,w] (fp32), a stored bf16 a9_2, slope(a9_2) its LeakyReLU'"""
+    s = slope(a)
     a, w = a.double(), w.double().reshape(w.shape[0], -1)
     d = dout.double().permute(0, 2, 3, 1)
-    s = 1.0 - 0.8 * (a <= 0).double()
     dz, S = (d @ w) * s, (d.abs() @ w.abs()) * s
     p, q = a.reshape(-1, a.shape[-1]), d.reshape(-1, d.shape[-1])
     return dz, S, q.t() @ p, q.abs().t() @ p.abs(), q.sum(0), q.abs().sum(0)

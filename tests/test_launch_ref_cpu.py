@@ -1,5 +1,5 @@
 """The float64 references of tests/launch_ref.py checked against torch's own float64 convolutions and autograd, and
-the bit layouts of the sign words and pool codes against a hand-built window - on the CPU, so that the per-launch GPU
+the bit layouts of the slope words and pool codes against a hand-built window - on the CPU, so that the per-launch GPU
 suite measures the kernels with a yardstick that is itself tested."""
 import math
 
@@ -60,7 +60,82 @@ def test_head_and_pool_backward_match_autograd():
     assert torch.allclose(_nchw(r), z.grad, rtol=1e-12, atol=1e-12)
 
 
-def test_pool_code_and_sign_word_bit_layout():
+def _special_windows():
+    """z [1, 32, 4, 4] float64 (NCHW, 4 pooling windows per channel) holding +-0, +-Inf, NaN with both sign bits, equal
+    maxima, windows that mix NaN and numbers and all-NaN windows; the rest seeded normal numbers"""
+    inf, nan = math.inf, math.nan
+    g = torch.Generator().manual_seed(4)
+    z = torch.randn(1, 32, 4, 4, generator=g, dtype=torch.float64)
+    neg_nan = -torch.tensor(nan, dtype=torch.float64)
+    assert torch.signbit(neg_nan)
+    rows = [[0.0, -0.0, 1.0, 1.0], [-0.0, 0.0, 1.0, -2.0], [inf, -inf, -inf, -inf], [2.0, 2.0, nan, 1.0],
+            [nan, 5.0, nan, 1.0], [nan, nan, nan, nan], [-1.0, -3.0, -1.0, -1.0], [-inf, 0.0, -0.0, inf]]
+    for c, win in enumerate(rows):          # window (0, 0) of channel c, in the order (0,0) (0,1) (1,0) (1,1)
+        z[0, c, 0, 0], z[0, c, 0, 1], z[0, c, 1, 0], z[0, c, 1, 1] = (torch.tensor(v, dtype=torch.float64) for v in win)
+    z[0, 5, 1, 1] = neg_nan                 # the all-NaN window ends in a negative NaN
+    z[0, 8:16] = z[0, :8].flip(-1)          # the same windows elsewhere, mirrored
+    z[0, 16, 2:, 2:] = nan                  # an all-NaN window at (1, 1)
+    z[0, 17, 3, 3] = neg_nan
+    return z
+
+
+def test_slope_and_pool_match_autograd_at_ties_and_nan():
+    """LeakyReLU' = autograd of the reference's torch.max(0.2 x, x), F.max_pool2d's NaN propagation and routing, and
+    pool_bwd = autograd of (skip path + max_pool2d path) through that LeakyReLU, on hand-made windows"""
+    z = _special_windows().requires_grad_()
+    act = torch.max(0.2 * z, z)
+    act.backward(torch.ones_like(act))
+    a = _nhwc(act.detach())
+    assert torch.equal(_nchw(R.slope(a)), z.grad)
+    assert sorted(set(z.grad.reshape(-1).tolist())) == [0.2, 0.6, 1.0, 1.2]
+    # the pooled values: NaN where the window holds one, exactly where F.max_pool2d has it
+    m, _, pick = R.pool(a)
+    want = F.max_pool2d(act.detach().float(), 2)        # pool works on the stored values, in float32
+    assert torch.equal(torch.isnan(_nchw(m)), torch.isnan(want)) and torch.isnan(want).any()
+    assert torch.equal(_nchw(m).nan_to_num(7.0, 8.0, -8.0), want.nan_to_num(7.0, 8.0, -8.0))
+    _, idx = F.max_pool2d(act.detach(), 2, return_indices=True)
+    got_idx = pick.int().argmax(-1)            # window element 0..3 -> flat index in the 4 x 4 plane
+    got_idx = (2 * torch.arange(2).view(2, 1, 1) + got_idx // 2) * 4 + 2 * torch.arange(2).view(1, 2, 1) + got_idx % 2
+    assert torch.equal(_nchw(got_idx), idx) and (pick.sum(-1) == 1).all()
+    # the backward, NaN for NaN
+    z.grad = None
+    g = torch.Generator().manual_seed(5)
+    dskip, dp = torch.randn(1, 32, 4, 4, generator=g, dtype=torch.float64), torch.randn(1, 32, 2, 2, generator=g, dtype=torch.float64)
+    act = torch.max(0.2 * z, z)
+    torch.autograd.backward([act, F.max_pool2d(act, 2)], [dskip, dp])
+    r, S = R.pool_bwd(a, _nhwc(dskip), _nhwc(dp))
+    torch.testing.assert_close(_nchw(r), z.grad, rtol=1e-15, atol=0, equal_nan=True)
+    assert torch.isfinite(z.grad).sum() > 0 and torch.isnan(z.grad).sum() == 0      # dskip and dp are finite
+    # the head's LeakyReLU' in head_bwd is the same slope
+    w = torch.randn(4, 32, 1, 1, generator=g)
+    dout = torch.randn(1, 4, 4, 4, generator=g, dtype=torch.float64)
+    zh = z.detach().clone().requires_grad_()
+    F.conv2d(torch.max(0.2 * zh, zh), w.double()).backward(dout)
+    dz, _, _, _, _, _ = R.head_bwd(a, w, dout)
+    torch.testing.assert_close(_nchw(dz), zh.grad, rtol=1e-12, atol=1e-12, equal_nan=True)
+
+
+def test_sign_bit_slope_fails_the_reference():
+    """a planted fault: the engine's former rule (LeakyReLU' = 0.2 where the sign bit is set, else 1; pool routing that
+    ignores NaN) fails the checks the references feed, on the windows where it differs; the reference's rule passes"""
+    z = _special_windows()
+    a = _nhwc(torch.max(0.2 * z, z)).bfloat16()
+    g = torch.Generator().manual_seed(6)
+    zz = torch.randn(a.shape, generator=g, dtype=torch.float64)
+    r, S = zz * R.slope(a), zz.abs() * R.slope(a)
+    old = (zz.float() * torch.where(torch.signbit(a.float()), R.MASK_NEG, 1.0).float()).bfloat16()
+    ratio, _, finite = R.bf16_rule(old, r, S)
+    assert ratio > 1.0
+    ratio, mism, finite = R.bf16_rule(R.epi_mask(zz, a), r, S)
+    assert ratio <= 1.0 and mism == 0 and finite
+    # pool routing that skips NaN (the first numeric maximum) and keeps the pooled number
+    win = a.float().reshape(1, 2, 2, 2, 2, 32).permute(0, 1, 3, 5, 2, 4).reshape(1, 2, 2, 32, 4)
+    m_old = win.nan_to_num(-math.inf).amax(-1)
+    m, _, _ = R.pool(a)
+    assert R.nonfinite_mismatch(m_old, m.double()) > 0 and R.nonfinite_mismatch(m, m.double()) == 0
+
+
+def test_pool_code_and_slope_word_bit_layout():
     """one pooled pixel, 32 channels: channel c's window is (v0, v1, v2, v3) in the order (0,0) (0,1) (1,0) (1,1)"""
     win = torch.zeros(32, 4)
     win[0] = torch.tensor([1.0, 1.0, 0.5, -2.0])     # tie: the first element is the maximum, the second also equals it
@@ -77,11 +152,14 @@ def test_pool_code_and_sign_word_bit_layout():
     assert u[1] & 1 == 0 and (u[1] >> 16) & 1 == 1
     assert u[2] & 1 == 1 and (u[2] >> 16) & 1 == 0
     assert (u[3] >> 1) & 1 == 0 and (u[3] >> 16) & 1 == 0
-    # signs: element 3 of channel 0 is negative (bit 0); element 0 of channel 1 (bit 16); every element of channel 2 (bit 1)
+    # neg: element 3 of channel 0 is negative (bit 0); element 0 of channel 1 (bit 16); every element of channel 2 (bit 1)
     assert u[4 + 3] & 1 == 1 and u[4 + 0] & 1 == 0 and (u[4 + 0] >> 16) & 1 == 1
     assert all((u[4 + k] >> 1) & 1 == 1 for k in range(4))
-    sw = R.sign_words(a)[0, :, :, 0].reshape(-1).tolist()
-    assert [s & 0xFFFFFFFF for s in sw] == u[4:]
+    # tie: the zero windows of channels 3..31 (bits 1.. of the odd half, 2.. of the even half), none of channels 0..2
+    tie = 0xFFFFFFFF & ~((1 << 0) | (1 << 16) | (1 << 1))
+    assert u[8:12] == [tie] * 4 and all(u[4 + k] & tie == 0 for k in range(4))
+    sw = R.slope_words(a)[0, :, :, 0].reshape(4, 2).tolist()
+    assert [s & 0xFFFFFFFF for s, _ in sw] == u[4:8] and [t & 0xFFFFFFFF for _, t in sw] == u[8:12]
 
 
 def test_ulp_and_first_layer_image():
@@ -157,15 +235,18 @@ def test_epilogue_emulations_by_hand():
     m = (-1.0 * float(np.float32(0.4)) + float(np.float32(0.6)))
     assert R.MASK_NEG == m == float(np.float32(m)) == 6710887 * 2.0 ** -25 and R.MASK_NEG != R.F32_02
     assert float(np.float32(1.0 * float(np.float32(0.4)) + float(np.float32(0.6)))) == 1.0
-    act = torch.tensor([-1.0, 0.0, -0.0, 2.0]).bfloat16()       # +0 counts positive, -0 negative (its sign bit)
-    z = torch.tensor([5.0, 5.0, 5.0, 5.0], dtype=torch.float64)
-    want = float(torch.tensor(5.0 * R.MASK_NEG).float().bfloat16())
-    assert R.epi_mask(z, act).float().tolist() == [want, 5.0, want, 5.0]
-    assert R.epi_mask(z, None).float().tolist() == [5.0] * 4
-    # head: (a > 0 ? 1 : 0.2f) - there +0 takes 0.2f, unlike the sign-bit masks
-    a = torch.tensor([0.0, 1.0]).bfloat16()
-    assert R.epi_head_dz(torch.tensor([5.0, 5.0], dtype=torch.float64), a).float().tolist() == \
-        [float(torch.tensor(5.0 * R.F32_02).float().bfloat16()), 5.0]
+    # the masks: MASK_NEG below zero, 1 above, 0.6f at +-0 and +-Inf whatever the sign bit, 1.2f at NaN of either sign
+    inf, nan = math.inf, math.nan
+    act = torch.tensor([-1.0, 0.0, -0.0, 2.0, inf, -inf, nan, -nan]).bfloat16()
+    z = torch.full((8,), 5.0, dtype=torch.float64)
+    f = lambda c: float(torch.tensor(5.0 * c).float().bfloat16())      # noqa: E731
+    assert R.F32_06 == float(np.float32(0.6)) and R.F32_12 == float(np.float32(1.2))
+    assert R.epi_mask(z, act).float().tolist() == [f(R.MASK_NEG), f(R.F32_06), f(R.F32_06), 5.0, f(R.F32_06),
+                                                    f(R.F32_06), f(R.F32_12), f(R.F32_12)]
+    assert R.epi_mask(z, None).float().tolist() == [5.0] * 8
+    # head: the same classes with 0.2f below zero
+    assert R.epi_head_dz(z, act).float().tolist() == [f(R.F32_02), f(R.F32_06), f(R.F32_06), 5.0, f(R.F32_06),
+                                                       f(R.F32_06), f(R.F32_12), f(R.F32_12)]
     # pool backward: dp goes to the first maximum of each window, -0 + (+0) = +0, then the sign mask
     a = torch.tensor([[1.0, 3.0], [3.0, -1.0]]).reshape(1, 2, 2, 1).expand(1, 2, 2, 32).contiguous().bfloat16()
     dskip = torch.tensor([[-0.0, 1.0], [2.0, 4.0]]).reshape(1, 2, 2, 1).expand(1, 2, 2, 32).contiguous().bfloat16()
@@ -173,11 +254,16 @@ def test_epilogue_emulations_by_hand():
     got = R.epi_pool_bwd(a, dskip, dp)[0, :, :, 0]
     assert _bits(got.reshape(-1)) == _bits(torch.tensor([0.0, 9.0, 2.0, float(torch.tensor(4.0 * R.MASK_NEG).float())
                                                           ]).bfloat16())
-    # the exact rule: +0 and -0 are equal, one ulp is not, a NaN never is
-    want = torch.tensor([0.0, 1.0, 2.0]).bfloat16()
-    got = torch.tensor([-0.0, 1.0 + 2 ** -7, float('nan')]).bfloat16()
-    mask = torch.tensor([True, True, True])
-    assert R.exact_rule(got, want, mask) == 2 and R.exact_rule(got, want, torch.tensor([True, False, False])) == 0
+    # a NaN window routes dp to its last NaN, and the NaN's slope is 1.2f: dskip + dp = 10 at element 2
+    a = torch.tensor([[nan, 3.0], [nan, -1.0]]).reshape(1, 2, 2, 1).expand(1, 2, 2, 32).contiguous().bfloat16()
+    got = R.epi_pool_bwd(a, dskip, dp)[0, :, :, 0].reshape(-1)
+    assert got.float().tolist() == [f(0.0), 1.0, float(torch.tensor(10.0 * R.F32_12).float().bfloat16()),
+                                    float(torch.tensor(4.0 * R.MASK_NEG).float().bfloat16())]
+    # the exact rule: +0 and -0 are equal, one ulp is not, NaN only equals NaN
+    want = torch.tensor([0.0, 1.0, 2.0, nan, nan]).bfloat16()
+    got = torch.tensor([-0.0, 1.0 + 2 ** -7, nan, -nan, 4.0]).bfloat16()
+    mask = torch.tensor([True, True, True, True, True])
+    assert R.exact_rule(got, want, mask) == 3 and R.exact_rule(got, want, torch.tensor([True, False, False, True, False])) == 0
 
 
 def _sum_f32(vals, order):

@@ -26,6 +26,18 @@ BIG_EXACT = 1024.0             # the same on integer operands: a power of two ke
 STATS = defaultdict(lambda: defaultdict(float))     # kernel -> worst measured value per statistic
 
 
+def plant_slope_classes(torch, g, aux):
+    """the mask operand `aux` with +-0, +-Inf and NaN of both signs at 64 seeded elements each: the LeakyReLU' classes
+    0.6 and 1.2 besides the random operand's 1 and 0.2"""
+    inf, nan = float('inf'), float('nan')
+    vals = torch.tensor([0.0, -0.0, inf, -inf, nan, nan], device='cuda')
+    vals[5] = -vals[5]
+    flat = aux.view(-1)
+    idx = torch.randint(0, flat.numel(), (6 * 64,), device='cuda', generator=g)
+    flat[idx] = vals.repeat(64).to(aux.dtype)
+    return aux
+
+
 def operand(torch, g, n, h, w, pitch, big_odd=True):
     """bf16 NHWC [n,h,w,pitch]: standard normal, the odd (or even) images x BIG"""
     scale = torch.ones(n, 1, 1, 1, device='cuda')
@@ -150,7 +162,7 @@ def run_case(torch, c, seed, integer=False):
     x = dense(c.n, ih, iw, c.x_pitch)
     xs = x[..., c.x_c0:c.x_c0 + c.ci]
     out, y = output(torch, c.n, oh, ow, c.y_pitch)
-    aux = dense(c.n, c.h, c.w, c.aux_pitch) if c.act == prims.ACT_MASK else None
+    aux = plant_slope_classes(torch, g, dense(c.n, c.h, c.w, c.aux_pitch)) if c.act == prims.ACT_MASK else None
     auxs = aux[..., c.aux_c0:c.aux_c0 + c.co] if aux is not None else None
     b = None
     if c.op == 'conv':
