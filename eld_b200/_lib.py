@@ -24,6 +24,13 @@ class NoiseParams(ctypes.Structure):
                 ('saturation', ctypes.c_float), ('ratio', ctypes.c_float), ('color_bias', ctypes.c_float * 4)]
 
 
+class CameraCalib(ctypes.Structure):
+    """eld_camera_calib (440 bytes): one camera's calibration, as eld_noise_sample_params reads it."""
+    _fields_ = [(n, ctypes.c_double) for n in ('g_slope', 'g_bias', 'g_sigma', 'G_slope', 'G_bias', 'G_sigma',
+                                               'R_slope', 'R_bias', 'R_sigma')] + \
+               [('rows', ctypes.c_int), ('G_shape', ctypes.c_float * 18), ('color_bias', (ctypes.c_float * 4) * 18)]
+
+
 _lib = None
 
 
@@ -46,6 +53,9 @@ def _declare(lib):
                                          c.POINTER(c.c_uint8), vp]
     lib.eld_eval_correct_psnr.argtypes = [vp, vp, vp, vp, i32, c.c_size_t, i32, vp, vp, vp, vp]
     lib.eld_pair_ingest.argtypes = [vp, vp, i32, i32, vp, i32, i32, vp, vp, i32, i32, i32, c.POINTER(c.c_uint8), vp]
+    lib.eld_noise_sample_params.argtypes = [vp, c.POINTER(CameraCalib), i32, i32, u64, u64, vp, i32, i32, vp, vp, vp]
+    lib.eld_noise_packed_dev.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp, u32, u64, u64, vp, i32, vp, vp]
+    lib.eld_frame_counter_add.argtypes = [vp, vp, u64, vp]
     from . import _unet_abi
     _unet_abi.declare(lib)
 

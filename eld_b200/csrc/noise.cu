@@ -32,6 +32,15 @@ struct NoiseLaunch {
     int h, w;         // packed plane
     int clip01;
     uint8_t aug[kMaxFramesPerLaunch];   // AUG kernels: bit 0 flip rows, bit 1 flip columns, bit 2 transpose (sid_dataset.py:344-352)
+
+    // what the packed kernel bodies read per frame f of the launch
+    __device__ __forceinline__ const FrameConsts& consts(int f) const { return fr[f]; }
+    __device__ __forceinline__ Stream stream(int f) const
+    {
+        const uint64_t frame = frame0 + (uint64_t)f;
+        return Stream{ (uint32_t)seed, (uint32_t)(seed >> 32), (uint32_t)frame, (uint32_t)(frame >> 32) };
+    }
+    __device__ __forceinline__ uint32_t flags(int f) const { return aug[f]; }
 };
 
 static FrameConsts make_consts(const eld_noise_params& p)
@@ -204,10 +213,11 @@ __device__ __forceinline__ void row_normals(const Stream& s, uint32_t i, float& 
 
 // ---- packed in, aligned: w % 4 == 0 and 16-byte aligned planes ---------------------------------
 // Gaussian-only masks are issue/latency bound on MUFU chains: cap registers at 32 so 8 blocks (64 warps) fit.
-template <uint32_t MASK, int CLIP, int IN = 0, bool AUG = false>
-__global__ void __launch_bounds__(256, (MASK != kRuntimeMask && !(MASK & (ELD_NOISE_P | ELD_NOISE_G))) ? 8 : 1)
-noise_packed_vec_kernel(const float* __restrict__ clean, float* __restrict__ noisy,
-                        const __grid_constant__ NoiseLaunch L, const U16Src u16 = U16Src{}, float* __restrict__ target_out = nullptr)
+// The kernel bodies take the frame's constants, stream and flags from their caller: the host-table kernels read them from
+// the launch (NoiseLaunch), the device-table ones (NoiseLaunchDev) from a table in device memory.
+template <uint32_t MASK, int CLIP, int IN, bool AUG, class LP>
+__device__ __forceinline__ void packed_vec(const float* __restrict__ clean, float* __restrict__ noisy, const LP& L,
+                                           const U16Src u16, float* __restrict__ target_out)
 {
     const int f = blockIdx.y;
     const uint32_t plane = (uint32_t)L.h * (uint32_t)L.w;
@@ -215,8 +225,8 @@ noise_packed_vec_kernel(const float* __restrict__ clean, float* __restrict__ noi
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= quads) return;
     const uint32_t mask = (MASK == kRuntimeMask) ? L.mask : MASK;
-    const FrameConsts& fc = L.fr[f];
-    const Stream s = make_stream(L, f);
+    const FrameConsts& fc = L.consts(f);
+    const Stream s = L.stream(f);
     const size_t base = (size_t)f * 4 * plane + (size_t)t * 4;
 
     float4 v[4];
@@ -235,11 +245,19 @@ noise_packed_vec_kernel(const float* __restrict__ clean, float* __restrict__ noi
         if (AUG) {
             const uint32_t i = (t * 4u) / (uint32_t)L.w, j0 = t * 4u - i * (uint32_t)L.w;
             const size_t pbase = ((size_t)f * 4 + c) * plane;
-            store_aug(noisy + pbase, L.aug[f], i, j0, (uint32_t)L.h, (uint32_t)L.w, make_float4(y[0], y[1], y[2], y[3]));
-            if (target_out) store_aug(target_out + pbase, L.aug[f], i, j0, (uint32_t)L.h, (uint32_t)L.w, v[c]);
+            store_aug(noisy + pbase, L.flags(f), i, j0, (uint32_t)L.h, (uint32_t)L.w, make_float4(y[0], y[1], y[2], y[3]));
+            if (target_out) store_aug(target_out + pbase, L.flags(f), i, j0, (uint32_t)L.h, (uint32_t)L.w, v[c]);
         } else
         stg_stream(reinterpret_cast<float4*>(noisy + base + (size_t)c * plane), make_float4(y[0], y[1], y[2], y[3]));
     }
+}
+
+template <uint32_t MASK, int CLIP, int IN = 0, bool AUG = false>
+__global__ void __launch_bounds__(256, (MASK != kRuntimeMask && !(MASK & (ELD_NOISE_P | ELD_NOISE_G))) ? 8 : 1)
+noise_packed_vec_kernel(const float* __restrict__ clean, float* __restrict__ noisy,
+                        const __grid_constant__ NoiseLaunch L, const U16Src u16 = U16Src{}, float* __restrict__ target_out = nullptr)
+{
+    packed_vec<MASK, CLIP, IN, AUG>(clean, noisy, L, u16, target_out);
 }
 
 // ---- packed in, aligned, Poisson shot noise: lane-persistent sampler ---------------------------------
@@ -249,10 +267,9 @@ noise_packed_vec_kernel(const float* __restrict__ clean, float* __restrict__ noi
 // acceptance, so a warp iterates ~1.2 x 16 times instead of 16 x max-over-lanes.  The per-pixel arithmetic
 // and draw order are exactly poisson_px's (same values; oracle: eld_oracle_poisson_px).  The lane's 16 rates
 // and counts live in a private shared-memory column (dynamic indexing without local memory).
-template <uint32_t MASK, int IN = 0, bool AUG = false>
-__global__ void __launch_bounds__(256)
-noise_packed_poisson_kernel(const float* __restrict__ clean, float* __restrict__ noisy,
-                            const __grid_constant__ NoiseLaunch L, const U16Src u16 = U16Src{}, float* __restrict__ target_out = nullptr)
+template <uint32_t MASK, int IN, bool AUG, class LP>
+__device__ __forceinline__ void packed_poisson(const float* __restrict__ clean, float* __restrict__ noisy, const LP& L,
+                                               const U16Src u16, float* __restrict__ target_out)
 {
     __shared__ float s_buf[16][256];
     const int f = blockIdx.y;
@@ -261,8 +278,8 @@ noise_packed_poisson_kernel(const float* __restrict__ clean, float* __restrict__
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= quads) return;
     const uint32_t mask = (MASK == kRuntimeMask) ? L.mask : MASK;
-    const FrameConsts& fc = L.fr[f];
-    const Stream s = make_stream(L, f);
+    const FrameConsts& fc = L.consts(f);
+    const Stream s = L.stream(f);
     const size_t base = (size_t)f * 4 * plane + (size_t)t * 4;
     const int tid = threadIdx.x;
 
@@ -271,7 +288,7 @@ noise_packed_poisson_kernel(const float* __restrict__ clean, float* __restrict__
         const float4 v = load_clean<IN>(clean, u16, base + (size_t)c * plane);
         if (AUG && target_out) {
             const uint32_t i = (t * 4u) / (uint32_t)L.w, j0 = t * 4u - i * (uint32_t)L.w;
-            store_aug(target_out + ((size_t)f * 4 + c) * plane, L.aug[f], i, j0, (uint32_t)L.h, (uint32_t)L.w, v);
+            store_aug(target_out + ((size_t)f * 4 + c) * plane, L.flags(f), i, j0, (uint32_t)L.h, (uint32_t)L.w, v);
         }
         s_buf[c * 4 + 0][tid] = (v.x * fc.scale_in) * fc.invK;
         s_buf[c * 4 + 1][tid] = (v.y * fc.scale_in) * fc.invK;
@@ -383,24 +400,31 @@ noise_packed_poisson_kernel(const float* __restrict__ clean, float* __restrict__
         post_shot<MASK>(fc, s, L.mask, (uint32_t)cc, t * 4u, rown, L.clip01, z);
         if (AUG) {
             const uint32_t i = (t * 4u) / (uint32_t)L.w, j0 = t * 4u - i * (uint32_t)L.w;
-            store_aug(noisy + ((size_t)f * 4 + cc) * plane, L.aug[f], i, j0, (uint32_t)L.h, (uint32_t)L.w, make_float4(z[0], z[1], z[2], z[3]));
+            store_aug(noisy + ((size_t)f * 4 + cc) * plane, L.flags(f), i, j0, (uint32_t)L.h, (uint32_t)L.w, make_float4(z[0], z[1], z[2], z[3]));
         } else
         stg_stream(reinterpret_cast<float4*>(noisy + base + (size_t)cc * plane), make_float4(z[0], z[1], z[2], z[3]));
     }
 }
 
-// ---- packed in, generic shapes (scalar loads; quads may straddle rows) ------------------------------
+template <uint32_t MASK, int IN = 0, bool AUG = false>
 __global__ void __launch_bounds__(256)
-noise_packed_generic_kernel(const float* __restrict__ clean, float* __restrict__ noisy,
-                            const __grid_constant__ NoiseLaunch L)
+noise_packed_poisson_kernel(const float* __restrict__ clean, float* __restrict__ noisy,
+                            const __grid_constant__ NoiseLaunch L, const U16Src u16 = U16Src{}, float* __restrict__ target_out = nullptr)
+{
+    packed_poisson<MASK, IN, AUG>(clean, noisy, L, u16, target_out);
+}
+
+// ---- packed in, generic shapes (scalar loads; quads may straddle rows) ------------------------------
+template <class LP>
+__device__ __forceinline__ void packed_generic(const float* __restrict__ clean, float* __restrict__ noisy, const LP& L)
 {
     const int f = blockIdx.y;
     const uint32_t plane = (uint32_t)L.h * (uint32_t)L.w;
     const uint32_t quads = (plane + 3u) >> 2;
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= quads) return;
-    const FrameConsts& fc = L.fr[f];
-    const Stream s = make_stream(L, f);
+    const FrameConsts& fc = L.consts(f);
+    const Stream s = L.stream(f);
     for (int c = 0; c < 4; ++c) {
         const size_t base = ((size_t)f * 4 + c) * plane;
         float y[4], rown[4];
@@ -422,6 +446,13 @@ noise_packed_generic_kernel(const float* __restrict__ clean, float* __restrict__
             if (l < plane) noisy[base + l] = y[k];
         }
     }
+}
+
+__global__ void __launch_bounds__(256)
+noise_packed_generic_kernel(const float* __restrict__ clean, float* __restrict__ noisy,
+                            const __grid_constant__ NoiseLaunch L)
+{
+    packed_generic(clean, noisy, L);
 }
 
 // ---- mosaic in (fused Bayer pack + de-quantise), aligned: W % 8 == 0 --------------------------------
@@ -573,6 +604,116 @@ static void launch_mosaic_vec(dim3 grid, cudaStream_t st, const void* m, float* 
     X(ELD_NOISE_P | ELD_NOISE_g)                                                    \
     X(ELD_NOISE_P | ELD_NOISE_G | ELD_NOISE_R | ELD_NOISE_U)                        \
     X(ELD_NOISE_P | ELD_NOISE_G | ELD_NOISE_B | ELD_NOISE_R | ELD_NOISE_U)
+
+// ---- device parameter tables (eld_noise_packed_dev) --------------------------------------------------------------------
+// The frame's eld_noise_params and flags are read from device memory when the kernel runs, and the first frame id may come
+// from a device counter: what a captured step needs.  Thread 0 of each block forms the frame's FrameConsts in shared
+// memory with make_consts' operations, each rounded as on the host (no FMA contraction), so the constants - and the
+// noise - equal the host-table kernels' bit for bit.  The bodies are the host-table kernels'.
+constexpr int kMaxGridY = 65535;
+
+struct NoiseLaunchDev {
+    const eld_noise_params* params;   // [frames of the launch]
+    const uint8_t* flags;             // [frames of the launch] or NULL
+    const uint64_t* frame0_dev;       // added to frame0 if not NULL
+    uint64_t seed;
+    uint64_t frame0;
+    uint32_t mask;
+    int h, w;
+    int clip01;
+};
+
+__device__ __forceinline__ FrameConsts make_consts_dev(const eld_noise_params& p)
+{
+    FrameConsts c{};
+    c.K = p.K;
+    c.invK = __fdiv_rn(1.0f, p.K);
+    c.g = fmaxf(p.g_scale, 1e-10f);
+    c.Kbm = __fmul_rn(p.K, 1.3862943611198906f);
+    c.gbm = __fmul_rn(c.g, 1.1774100225154747f);
+    c.Gs = p.G_scale;
+    c.Gl = p.G_lambda;
+    c.Rs = p.R_scale;
+    c.q = p.q_step;
+    c.scale_in = __fdiv_rn(p.saturation, p.ratio);
+    c.scale_out = __fdiv_rn(p.ratio, p.saturation);
+    for (int i = 0; i < 4; ++i) c.bias[i] = p.color_bias[i];
+    return c;
+}
+
+struct DevFrame {                      // a block's frame, in shared memory
+    FrameConsts fc;
+    uint64_t frame;
+    uint32_t aug;
+};
+
+// NoiseLaunch's per-frame accessors over the block's DevFrame
+struct DevView {
+    const DevFrame* d;
+    uint64_t seed;
+    uint32_t mask;
+    int h, w, clip01;
+    __device__ __forceinline__ const FrameConsts& consts(int) const { return d->fc; }
+    __device__ __forceinline__ Stream stream(int) const
+    {
+        return Stream{ (uint32_t)seed, (uint32_t)(seed >> 32), (uint32_t)d->frame, (uint32_t)(d->frame >> 32) };
+    }
+    __device__ __forceinline__ uint32_t flags(int) const { return d->aug; }
+};
+
+__device__ __forceinline__ DevView dev_frame(const NoiseLaunchDev& L, DevFrame& sh)
+{
+    if (threadIdx.x == 0) {
+        const int f = blockIdx.y;
+        sh.fc = make_consts_dev(L.params[f]);
+        sh.frame = L.frame0 + (L.frame0_dev ? *L.frame0_dev : 0ull) + (uint64_t)f;
+        sh.aug = L.flags ? L.flags[f] : 0u;
+    }
+    __syncthreads();
+    return DevView{ &sh, L.seed, L.mask, L.h, L.w, L.clip01 };
+}
+
+template <uint32_t MASK, int CLIP, bool AUG>
+__global__ void __launch_bounds__(256, (MASK != kRuntimeMask && !(MASK & (ELD_NOISE_P | ELD_NOISE_G))) ? 8 : 1)
+noise_packed_vec_dev_kernel(const float* __restrict__ clean, float* __restrict__ noisy,
+                            const __grid_constant__ NoiseLaunchDev L, float* __restrict__ target_out)
+{
+    __shared__ DevFrame sh;
+    packed_vec<MASK, CLIP, 0, AUG>(clean, noisy, dev_frame(L, sh), U16Src{}, target_out);
+}
+
+template <uint32_t MASK, bool AUG>
+__global__ void __launch_bounds__(256)
+noise_packed_poisson_dev_kernel(const float* __restrict__ clean, float* __restrict__ noisy,
+                                const __grid_constant__ NoiseLaunchDev L, float* __restrict__ target_out)
+{
+    __shared__ DevFrame sh;
+    packed_poisson<MASK, 0, AUG>(clean, noisy, dev_frame(L, sh), U16Src{}, target_out);
+}
+
+__global__ void __launch_bounds__(256)
+noise_packed_generic_dev_kernel(const float* __restrict__ clean, float* __restrict__ noisy,
+                                const __grid_constant__ NoiseLaunchDev L)
+{
+    __shared__ DevFrame sh;
+    packed_generic(clean, noisy, dev_frame(L, sh));
+}
+
+// eld_noise_packed's aligned dispatch (launch_packed_vec) over a device table
+template <uint32_t MASK>
+static void launch_packed_vec_dev(dim3 grid, cudaStream_t st, const float* clean, float* noisy, const NoiseLaunchDev& L)
+{
+    if constexpr (MASK != kRuntimeMask && (MASK & ELD_NOISE_P)) {
+        noise_packed_poisson_dev_kernel<MASK, false><<<grid, 256, 0, st>>>(clean, noisy, L, nullptr);
+    } else {
+        if (MASK == kRuntimeMask && (L.mask & ELD_NOISE_P))
+            noise_packed_poisson_dev_kernel<kRuntimeMask, false><<<grid, 256, 0, st>>>(clean, noisy, L, nullptr);
+        else if (L.clip01)
+            noise_packed_vec_dev_kernel<MASK, 1, false><<<grid, 256, 0, st>>>(clean, noisy, L, nullptr);
+        else
+            noise_packed_vec_dev_kernel<MASK, 0, false><<<grid, 256, 0, st>>>(clean, noisy, L, nullptr);
+    }
+}
 
 static int check_common(eld_ctx* ctx, const void* in, const void* out, int n, int h, int w,
                         const eld_noise_params* params, uint32_t mask, const char* who)
@@ -743,6 +884,60 @@ extern "C" int eld_noise_packed_aug(eld_ctx* ctx, const float* clean, float* noi
         dim3 grid((uint32_t)((plane / 4 + 255) / 256), nf);
         if (model_mask & ELD_NOISE_P) noise_packed_poisson_kernel<kRuntimeMask, 0, true><<<grid, 256, 0, st>>>(src, dst, L, U16Src{}, tdst);
         else                          noise_packed_vec_kernel<kRuntimeMask, -1, 0, true><<<grid, 256, 0, st>>>(src, dst, L, U16Src{}, tdst);
+        ELD_CHECK_CUDA(cudaGetLastError());
+        count_launch(ctx);
+    }
+    return ELD_OK;
+}
+
+extern "C" int eld_noise_packed_dev(eld_ctx* ctx, const float* clean, float* noisy, float* target_out, int n, int h, int w,
+                                    const eld_noise_params* params_dev, uint32_t model_mask, uint64_t seed,
+                                    uint64_t frame_id0, const uint64_t* frame_id0_dev, int clip01,
+                                    const uint8_t* flags_dev, void* stream)
+{
+    const char* who = "eld_noise_packed_dev";
+    ELD_REQUIRE(ctx != nullptr, "%s: ctx is NULL", who);
+    ELD_REQUIRE(n >= 0 && h >= 0 && w >= 0, "%s: negative size n=%d h=%d w=%d", who, n, h, w);
+    ELD_REQUIRE((model_mask & ~0x7Fu) == 0, "%s: unknown model_mask bits 0x%x", who, model_mask);
+    if (n == 0 || h == 0 || w == 0) return ELD_OK;
+    ELD_REQUIRE(clean != nullptr && noisy != nullptr && params_dev != nullptr, "%s: NULL buffer", who);
+    ELD_REQUIRE((uint64_t)h * (uint64_t)w < (1ull << 32), "%s: plane of %d x %d exceeds 2^32 pixels", who, h, w);
+    const bool aug = flags_dev != nullptr;
+    if (aug) {
+        ELD_REQUIRE(h == w, "%s: a device flags table may transpose, which needs square frames (h=%d w=%d)", who, h, w);
+        ELD_REQUIRE(w % 4 == 0, "%s: w=%d must be a multiple of 4 with flags", who, w);
+        ELD_REQUIRE((reinterpret_cast<uintptr_t>(clean) | reinterpret_cast<uintptr_t>(noisy) |
+                     reinterpret_cast<uintptr_t>(target_out)) % 16 == 0, "%s: buffers must be 16-byte aligned with flags", who);
+        ELD_REQUIRE(clean != noisy && clean != target_out, "%s: the index map cannot run in place", who);
+    } else {
+        ELD_REQUIRE(target_out == nullptr, "%s: target_out is written on the augmenting path only (flags_dev != NULL)", who);
+    }
+    ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t plane = (size_t)h * w;
+    const bool aligned = (w % 4 == 0) && ((reinterpret_cast<uintptr_t>(clean) | reinterpret_cast<uintptr_t>(noisy)) % 16 == 0);
+    const uint32_t quads = (uint32_t)((plane + 3) / 4);
+    for (int f0 = 0; f0 < n; f0 += kMaxGridY) {
+        const int nf = (n - f0 < kMaxGridY) ? n - f0 : kMaxGridY;
+        NoiseLaunchDev L{ params_dev + f0, aug ? flags_dev + f0 : nullptr, frame_id0_dev, seed, frame_id0 + (uint64_t)f0,
+                          model_mask, h, w, clip01 };
+        const float* src = clean + (size_t)f0 * 4 * plane;
+        float* dst = noisy + (size_t)f0 * 4 * plane;
+        const dim3 grid((quads + 255) / 256, nf);
+        if (aug) {
+            float* tdst = target_out ? target_out + (size_t)f0 * 4 * plane : nullptr;
+            if (model_mask & ELD_NOISE_P) noise_packed_poisson_dev_kernel<kRuntimeMask, true><<<grid, 256, 0, st>>>(src, dst, L, tdst);
+            else                          noise_packed_vec_dev_kernel<kRuntimeMask, -1, true><<<grid, 256, 0, st>>>(src, dst, L, tdst);
+        } else if (aligned) {
+            switch (model_mask) {
+#define X(M) case (M): launch_packed_vec_dev<(M)>(grid, st, src, dst, L); break;
+                ELD_FOR_EACH_MASK(X)
+#undef X
+                default: launch_packed_vec_dev<kRuntimeMask>(grid, st, src, dst, L); break;
+            }
+        } else {
+            noise_packed_generic_dev_kernel<<<grid, 256, 0, st>>>(src, dst, L);
+        }
         ELD_CHECK_CUDA(cudaGetLastError());
         count_launch(ctx);
     }

@@ -5,13 +5,19 @@
 //     DOM_QUAD: a = linear pixel index in the plane >> 2; the 4 words serve the 4 pixels of the quad
 //     DOM_PIX : a = linear pixel index in the plane        (variable-length Poisson draws, call d)
 //     DOM_ROW : a = packed row index                        (row-noise normals of sensor rows 2a, 2a+1)
+//     DOM_PARAM: a = 0, c = 0, frame = f / burst           (a frame's eld_noise_params, csrc/noise_params.cu)
+//         d = 0: words (0,1) camera index, (2,3) log K       d = 1: Box-Muller (0,1) radius, (2,3) angle -> cos g_scale,
+//         d = 2: Box-Muller -> cos R_scale (full model)             sin G_scale (full model)
+//         d = 3: words (0,1) G_shape / color_bias row (full model), (2,3) ratio
+//         a word pair (hi, lo) is the 53-bit integer hi << 21 | lo >> 11
+//     DOM_FLAGS: a = 0, c = 0, d = 0, frame = f            (augmentation flags: bit b = top bit of word b, b = 0, 1, 2)
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
 
 namespace eld {
 
-constexpr uint32_t DOM_QUAD = 1u, DOM_PIX = 2u, DOM_ROW = 3u;
+constexpr uint32_t DOM_QUAD = 1u, DOM_PIX = 2u, DOM_ROW = 3u, DOM_PARAM = 4u, DOM_FLAGS = 5u;
 constexpr uint32_t D_SHOT = 0u, D_READ = 1u, D_TL = 2u, D_QUANT = 3u;
 
 struct Stream {

@@ -12,9 +12,12 @@ Differences that are the point of this repo
     (NCCL over NVLink) between backward and Adam - one collective, U-Net weights only;
   * get_current_errors() keeps the reference's `.item()` host sync but can be told to defer it;
   * opt.cuda_graph captures the fused step (train_step + Adam) in a CUDA graph and replays it (ELDModel._graph_step);
+  * opt.params_on_gpu draws each frame's noise parameters and flips on the device (keyed like the host draws, other
+    values): with opt.cuda_graph the synthesis is captured with the step, and a step's host work is one copy and a replay;
   * opt.accum_steps = k accumulates the gradients of k optimize_parameters() calls and takes one Adam step (and, data
     parallel, one all-reduce) per window of k: the update of a W-GPU job at batch n is that of batch k W n.
 """
+import ctypes
 import os
 from collections import OrderedDict
 from types import SimpleNamespace
@@ -33,7 +36,7 @@ def default_opt(**kw):
              stage_in='raw', stage_out='raw', model_path=None, include=4, crf=False, batchSize=1, lr=1e-4,
              beta1=0.9, wd=0.0, loss='l1', noise='g', isTrain=True, save_epoch_freq=100, noise_on_gpu=False,
              augment_on_gpu=False, defer_loss_sync=False, prefetch_noise=False, num_burst=1, pairs_on_gpu=False,
-             cuda_graph=False, accum_steps=1)
+             cuda_graph=False, accum_steps=1, params_on_gpu=False)
     o.update(kw)
     return SimpleNamespace(**o)
 
@@ -104,6 +107,9 @@ class ELDModel(BaseModel):
         self._eager_left = 0         # eager warm-up steps before the next capture
         self._accum = 1              # optimize_parameters() calls per optimizer step (opt.accum_steps)
         self._micro = 0              # calls of the current accumulation window so far
+        self._synth_bufs = None      # params_on_gpu under cuda_graph: (clean, parameter table, flags, frame counter)
+        self._deferred = None        # (first frame id, n) of a synthesis the captured step runs
+        self._counter_host = None    # what the device frame counter holds once the queued work has run
 
     def _eval(self):
         self.netG.eval()
@@ -115,6 +121,12 @@ class ELDModel(BaseModel):
         BaseModel.initialize(self, opt)
         if self.device is None:
             raise RuntimeError('ELDModel (eld_b200) needs a CUDA device: no CPU fallback')
+        if getattr(opt, 'params_on_gpu', False):
+            if getattr(opt, 'pairs_on_gpu', False):
+                raise ValueError('params_on_gpu draws the noise parameters of synthesised frames, pairs_on_gpu trains from '
+                                 'stored pairs: set one of them')
+            if not getattr(opt, 'noise_on_gpu', False):
+                raise ValueError('params_on_gpu feeds the noise kernel on the training stream: it needs noise_on_gpu')
         if getattr(opt, 'pairs_on_gpu', False) and getattr(opt, 'noise_on_gpu', False):
             raise ValueError('pairs_on_gpu trains from stored (input, target) pairs, noise_on_gpu synthesises the input: '
                              'set one of them')
@@ -190,12 +202,21 @@ class ELDModel(BaseModel):
             n, c, h, w = target.shape
             xs, ts = self._static_io((n, 3 if isp else (c if input is None else input.shape[1]), h, w), (n, c, h, w))
         pre = self._prefetched if synth else None
-        if target is not None and not pairs and not (pre is not None and pre[0] is data):
+        # params_on_gpu under cuda_graph: the captured step synthesises the input itself (_graph_step)
+        deferred = xs is not None and synth and not isp and pre is None and getattr(self.opt, 'params_on_gpu', False)
+        self._deferred = None
+        if target is not None and not pairs and not deferred and not (pre is not None and pre[0] is data):
             if ts is not None and not aug:
                 target = ts.copy_(target, non_blocking=True)
             else:
                 target = target.to(device=self.device, dtype=torch.float32, non_blocking=True)
-        if pairs:
+        if deferred:
+            # only the clean frame is copied, into the buffer the captured synthesis reads; the step's frame ids are
+            # taken here, as _synthesize takes them
+            self._synth_buffers(target.shape, aug, ts)[0].copy_(target, non_blocking=True)
+            self._deferred = (self._take_frame_ids(target.shape[0]), target.shape[0])
+            input, target = xs, ts
+        elif pairs:
             input, target = self._ingest_pairs(input, target, out=xs, target_out=ts)
         elif synth:
             self._prefetched = None
@@ -232,6 +253,9 @@ class ELDModel(BaseModel):
         assert self.noise_maker is not None, 'noise_on_gpu needs a noise_maker (eld_b200.noise.NoiseModel)'
         n = target.shape[0]
         fid0 = self._take_frame_ids(n)
+        if getattr(self.opt, 'params_on_gpu', False):
+            # the same frame ids, the parameters and flips drawn on the device (eld_noise_sample_params)
+            return self._synthesize_device(target, fid0, out=out, target_out=target_out)
         # per-frame (K, g_scale, ratio, ...) and flip flags are drawn from a generator keyed by (seed, global frame id):
         # W ranks draw W*n DIFFERENT tuples (not W copies of the same n), and frame f gets the same tuple at any GPU
         # count.  The draw itself is noise.py:201-225's call order on that per-frame RandomState.
@@ -243,6 +267,39 @@ class ELDModel(BaseModel):
                                                         params=params, frame_id0=fid0, clip=True, out=out,
                                                         target_out=target_out)
         return self.noise_maker.batch_gpu(target, params=params, frame_id0=fid0, clip=True, out=out), target
+
+    def _synthesize_device(self, clean, fid0, out=None, target_out=None, bufs=None, counter=None):
+        """the frames' parameters (and flips, opt.augment_on_gpu) drawn on the device for frame ids fid0 + (*counter if
+        counter is given), then the noise launch that reads them: two launches, nothing per frame on the host.
+        bufs: (parameter table, flags) to draw into (new tensors if None)."""
+        nm, n = self.noise_maker, clean.shape[0]
+        aug = getattr(self.opt, 'augment_on_gpu', False)
+        table, flags = nm.frame_params_gpu(fid0, n, burst=max(1, int(getattr(self.opt, 'num_burst', 1))), flags=aug,
+                                           out=bufs, counter=counter, device=clean.device.index)
+        return nm.noise_from_table(clean, table, flags, fid0, counter=counter, clip=True, out=out,
+                                   target_out=target_out if aug else None)
+
+    def _synth_buffers(self, shape, aug, ts):
+        """params_on_gpu under cuda_graph: the clean frame (the target buffer itself unless augmented), parameter table,
+        flags and frame counter the captured synthesis reads; new ones (and a new capture) when the shape changes"""
+        b = self._synth_bufs
+        # the clean buffer is the target buffer itself exactly when not augmenting (the noise launch then leaves the
+        # target as it is); augmented, the launch writes aug(clean) into the target buffer from a clean buffer of its own
+        if b is None or tuple(b[0].shape) != tuple(shape) or (b[0] is ts) != (not aug):
+            dev = self.device
+            cs = torch.empty(tuple(shape), dtype=torch.float32, device=dev) if aug else ts
+            b = self._synth_bufs = (cs, torch.empty((shape[0], 12), dtype=torch.float32, device=dev),
+                                    torch.empty(shape[0], dtype=torch.uint8, device=dev),
+                                    b[3] if b is not None else torch.zeros(1, dtype=torch.int64, device=dev))
+            self._drop_graph()
+        return b
+
+    def _graph_synth(self, fid0, counter=None):
+        """the deferred synthesis into the static buffers: eagerly with the host's frame ids (counter None), or reading
+        the device frame counter (in the captured step, fid0 = 0)"""
+        cs, table, flags, _ = self._synth_bufs
+        xs, ts = self._static
+        self._synthesize_device(cs, fid0, out=xs, target_out=ts, bufs=(table, flags), counter=counter)
 
     def _take_frame_ids(self, n):
         """the global id of this rank's first frame of the step; advances the running count by the whole step"""
@@ -358,9 +415,14 @@ class ELDModel(BaseModel):
     def _graph_key(self):
         """what a captured step bakes in besides its buffers: re-captured when any of it changes"""
         g = self.optimizer_G.param_groups[0]
+        synth = None
+        if self._deferred is not None:       # the captured synthesis bakes in the noise model and the flags
+            nm = self.noise_maker
+            synth = (id(nm), int(nm.seed), nm.model, bool(getattr(self.opt, 'augment_on_gpu', False)),
+                     max(1, int(getattr(self.opt, 'num_burst', 1))), self._synth_bufs[0].data_ptr())
         return (tuple(self._static[0].shape), tuple(self._static[1].shape), self.netG.loss_kind,
                 tuple(p.requires_grad for p in self.netG.parameters()), tuple(float(b) for b in g['betas']),
-                float(g['eps']), float(g['weight_decay']))
+                float(g['eps']), float(g['weight_decay']), synth)
 
     def _fused_step(self, x, t):
         out, loss = self.netG.train_step(x, t)
@@ -373,6 +435,7 @@ class ELDModel(BaseModel):
         times, and the next one is captured and replayed.  The graph holds the _Engine plan it launches on, so the
         engine cache's eviction cannot free a workspace it addresses.  No host synchronisation."""
         xs, ts = self._static_io(self.input.shape, self.target.shape)
+        d = self._deferred
         if self.input.data_ptr() != xs.data_ptr():
             xs.copy_(self.input)
         if self.target.data_ptr() != ts.data_ptr():
@@ -383,6 +446,8 @@ class ELDModel(BaseModel):
             self._drop_graph()
         if self._graph is None and self._eager_left > 0:
             self._eager_left -= 1
+            if d is not None:
+                self._graph_synth(d[0])
             cur = torch.cuda.current_stream()
             side = torch.cuda.Stream(device=self.device)
             side.wait_stream(cur)
@@ -397,6 +462,12 @@ class ELDModel(BaseModel):
             self._capture(key, xs, ts)
         _, graph, plan, out, loss = self._graph
         plan.owner = None              # the replay overwrites the built-in forward state, as train_step does
+        if d is not None:
+            # the captured synthesis reads its first frame id from the device counter and advances it by n: set it here
+            # (outside the graph, no host sync) whenever the host count moved otherwise - first replay, warm-up, load()
+            if self._counter_host != d[0]:
+                self._synth_bufs[3].fill_(d[0])
+            self._counter_host = d[0] + d[1]
         self.optimizer_G.graph_step()
         graph.replay()
         self.output = out              # overwritten by the next replay
@@ -409,6 +480,13 @@ class ELDModel(BaseModel):
         plan = self.netG._plan(n, h, w, True)      # created (or kept most recent) outside the capture
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
+            if self._deferred is not None:
+                from . import _lib
+                counter = self._synth_bufs[3]
+                self._graph_synth(0, counter=counter)
+                _lib.check(_lib.load().eld_frame_counter_add(
+                    _lib.ctx(counter.device.index or 0), counter.data_ptr(), n,
+                    ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), 'eld_frame_counter_add')
             out, loss = self._fused_step(xs, ts)
         self.optimizer_G.t -= 1                    # the capture ran no step; graph_step counts each replay
         self._graph = (key, graph, plan, out, loss)

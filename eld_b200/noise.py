@@ -13,6 +13,9 @@ calls reproducible exactly as it does for the reference.  There is no CPU path h
 GPU-native additions (used by ELDModel.set_input when noise runs on the training stream):
     batch_gpu(clean[N,4,h,w] cuda f32, params=None, frame_id0=None) -> noisy
     mosaic_gpu(mosaic[N,H,W] cuda u16|f32, black, white, ...)       -> (noisy, clean)
+    frame_params_gpu(fid0, n, burst=1, flags=False)                 -> (table[N,12] cuda f32, flags[N] cuda u8 | None)
+    batch_gpu(clean, params='device') / noise_from_table(clean, table, flags, fid0, ...): the parameters (and flags)
+        drawn and read on the device - same laws as frame_params, other values (csrc/noise_params.cu)
 """
 import ctypes
 import json
@@ -78,6 +81,36 @@ def _cur_stream(torch):
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def _counter_ptr(counter):
+    """the device address of a one-element int64 frame counter, or None"""
+    if counter is None:
+        return None
+    assert counter.is_cuda and counter.element_size() == 8 and counter.numel() == 1
+    return counter.data_ptr()
+
+
+def calib_array(camera_params, cameras):
+    """the cameras' calibration (the dictionaries of camera_params/release/<camera>_params.npy) -> ctypes array of
+    eld_camera_calib, in the order of `cameras`"""
+    arr = (_lib.CameraCalib * len(cameras))()
+    for c, cam in enumerate(cameras):
+        cp = camera_params[cam]
+        prof = cp['Profile-1']
+        for name, key in (('g', 'g_scale'), ('G', 'G_scale'), ('R', 'R_scale')):
+            for field in ('slope', 'bias', 'sigma'):
+                setattr(arr[c], '%s_%s' % (name, field), float(prof[key][field]))
+        shape, bias = np.asarray(cp['G_shape'], dtype=np.float64).reshape(-1), np.asarray(cp['color_bias'], dtype=np.float64)
+        if len(shape) > len(arr[c].G_shape):
+            raise ValueError('camera %s: %d G_shape rows, eld_noise_sample_params takes at most %d'
+                             % (cam, len(shape), len(arr[c].G_shape)))
+        arr[c].rows = len(shape)
+        for r in range(len(shape)):
+            arr[c].G_shape[r] = shape[r]
+            for k in range(4):
+                arr[c].color_bias[r][k] = bias[r][k]
+    return arr
+
+
 def frame_rng(seed, fid):
     """the RandomState of global frame `fid` under `seed`: the same frame draws the same values whatever the GPU count"""
     return np.random.RandomState(np.random.SeedSequence([int(seed) & 0xFFFFFFFF, int(seed) >> 32,
@@ -134,12 +167,71 @@ class NoiseModelBase:
             return self._sample_params_full(rng)
         return self._sample_params(rng)
 
-    def batch_gpu(self, clean, params=None, frame_id0=None, clip=True, out=None, seed=None):
-        """clean: cuda float32 [N,4,h,w] in [0,1] -> noisy, same shape (reference layout, SURVEY F3)."""
+    # ---- per-frame draws on the device (csrc/noise_params.cu) ----------------------------------------------------------
+    def _calib_table(self):
+        raise NotImplementedError
+
+    def frame_params_gpu(self, fid0, n, burst=1, flags=False, out=None, counter=None, device=None):
+        """frame_params (and, flags=True, frame_augment) for global frames fid0 .. fid0+n-1 drawn on the current stream by
+        eld_noise_sample_params: the same laws, keyed by (self.seed, frame id) in Philox domains of their own, no host
+        work per frame.  counter: a cuda int64 tensor of one element whose value is added to fid0 when the kernel runs.
+        out: (table, flags) to write into.  -> (table, flags): cuda float32 [n, 12] rows laid out as eld_noise_params,
+        cuda uint8 [n] or None."""
+        import torch
+        if out is not None:
+            table, fl = out
+        else:
+            dev = torch.device('cuda', torch.cuda.current_device() if device is None else device)
+            table = torch.empty((n, 12), dtype=torch.float32, device=dev)
+            fl = torch.empty(n, dtype=torch.uint8, device=dev) if flags else None
+        assert table.is_cuda and table.dtype == torch.float32 and table.shape == (n, 12) and table.is_contiguous()
+        assert not flags or (fl is not None and fl.dtype == torch.uint8 and fl.shape == (n,) and fl.is_contiguous())
+        cams, ncam = self._calib_table()
+        _lib.check(_lib.load().eld_noise_sample_params(
+            _lib.ctx(table.device.index or 0), cams, ncam, int(_lib.is_full_model(self.model)), int(self.seed), int(fid0),
+            _counter_ptr(counter), int(burst), int(n), table.data_ptr(), fl.data_ptr() if flags else None,
+            _cur_stream(torch)), 'eld_noise_sample_params')
+        return table, (fl if flags else None)
+
+    def noise_from_table(self, clean, table, flags, frame_id0, counter=None, clip=True, out=None, target_out=None,
+                         seed=None):
+        """batch_gpu (flags None) or batch_gpu_augmented (flags a cuda uint8 [N]) with the per-frame parameters read from
+        the cuda float32 [N, 12] table frame_params_gpu writes: eld_noise_packed_dev, one launch, nothing read on the
+        host.  counter as in frame_params_gpu.  -> (noisy, target): target = aug(clean) with flags, else clean."""
         import torch
         assert clean.is_cuda and clean.dtype == torch.float32 and clean.dim() == 4 and clean.shape[1] == 4
         clean = clean.contiguous()
         n, _, h, w = clean.shape
+        assert table.is_cuda and table.dtype == torch.float32 and table.shape == (n, 12) and table.is_contiguous()
+        noisy = torch.empty_like(clean) if out is None else out
+        target = None
+        if flags is not None:
+            assert flags.is_cuda and flags.dtype == torch.uint8 and flags.shape == (n,) and flags.is_contiguous()
+            target = torch.empty_like(clean) if target_out is None else target_out
+        for t in (noisy, target):
+            assert t is None or (t.is_contiguous() and t.shape == clean.shape and t.dtype == torch.float32)
+        rc = _lib.load().eld_noise_packed_dev(
+            _lib.ctx(clean.device.index or 0), clean.data_ptr(), noisy.data_ptr(), target.data_ptr() if target is not None
+            else None, n, h, w, table.data_ptr(), _lib.model_mask(self.model), int(self.seed if seed is None else seed),
+            int(frame_id0), _counter_ptr(counter), int(bool(clip)), flags.data_ptr() if flags is not None else None,
+            _cur_stream(torch))
+        _lib.check(rc, 'eld_noise_packed_dev')
+        return noisy, (clean if target is None else target)
+
+    def batch_gpu(self, clean, params=None, frame_id0=None, clip=True, out=None, seed=None):
+        """clean: cuda float32 [N,4,h,w] in [0,1] -> noisy, same shape (reference layout, SURVEY F3).
+        params='device': the frames' parameters drawn on the device (frame_params_gpu, frame ids from frame_id0)."""
+        import torch
+        assert clean.is_cuda and clean.dtype == torch.float32 and clean.dim() == 4 and clean.shape[1] == 4
+        clean = clean.contiguous()
+        n, _, h, w = clean.shape
+        if isinstance(params, str):
+            assert params == 'device', params
+            if frame_id0 is None:
+                frame_id0 = int(np.random.randint(0, 2 ** 62))
+            table, _ = self.frame_params_gpu(frame_id0, n, device=clean.device.index)
+            return self.noise_from_table(clean, table, None, frame_id0, clip=clip, out=out, seed=seed)[0]
+        # host route: the parameters first, then the frame id - the order numpy's global RNG is drawn in
         plist = self._frame_params(n, params)
         if frame_id0 is None:
             frame_id0 = int(np.random.randint(0, 2 ** 62))
@@ -170,12 +262,20 @@ class NoiseModelBase:
         """SynDataset + ELDTrainDataset in one kernel (sid_dataset.py:269-277, 340-356): returns
         (input, target) = (aug(clip(noise(clean))), aug(clean)), aug = per-frame flip rows / flip columns / transpose.
         `aug`: uint8 flags per frame (bit 0 rows, 1 columns, 2 transpose) or None to draw them like the reference.
-        `out` / `target_out`: contiguous f32 tensors of clean's shape to write input / target into (new ones if None)."""
+        `out` / `target_out`: contiguous f32 tensors of clean's shape to write input / target into (new ones if None).
+        params='device' (with aug None): parameters and flags drawn on the device (frame_params_gpu); square frames."""
         import ctypes
         import torch
         assert clean.is_cuda and clean.dtype == torch.float32 and clean.dim() == 4 and clean.shape[1] == 4
         clean = clean.contiguous()
         n, _, h, w = clean.shape
+        if isinstance(params, str):
+            assert params == 'device' and aug is None, (params, aug)
+            if frame_id0 is None:
+                frame_id0 = int(np.random.randint(0, 2 ** 62))
+            table, flags = self.frame_params_gpu(frame_id0, n, flags=True, device=clean.device.index)
+            return self.noise_from_table(clean, table, flags, frame_id0, clip=clip, out=out, target_out=target_out,
+                                         seed=seed)
         plist = self._frame_params(n, params)
         if aug is None:
             aug = self.sample_augment(n)
@@ -304,6 +404,12 @@ class NoiseModel(NoiseModelBase):
         g_scale = np.exp(log_g_scale)
         ratio = np.random.uniform(low=100, high=300)
         return (K, g_scale, saturation_level, ratio)
+
+    def _calib_table(self):
+        """the camera list's calibration as eld_noise_sample_params reads it, built once"""
+        if getattr(self, '_calib', None) is None:
+            self._calib = (calib_array(self.camera_params, self.cameras), len(self.cameras))
+        return self._calib
 
     def _sample_params_full(self, rng=None):
         """Per-frame scalars of the full (paper-restated) model: the calibrated fields the released

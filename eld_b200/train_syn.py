@@ -50,6 +50,8 @@ def main():
     ap.add_argument('--num_burst', type=int, default=1)                       # SynDataset(num_burst=...), sid_dataset.py:269-275
     ap.add_argument('--accum_steps', type=int, default=1, help='micro-batches per optimizer step: one Adam step (and one '
                     'all-reduce) per window of k steps, on the gradients of k * world * batchSize frames')
+    ap.add_argument('--params_on_gpu', action='store_true', help="draw each frame's noise parameters and flips on the GPU "
+                    '(same laws and frame ids as the host draws, other values): no host work per frame')
     a = ap.parse_args()
     world = int(os.environ.get('WORLD_SIZE', '1'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
@@ -61,7 +63,7 @@ def main():
     opt = models.default_opt(name=a.name, gpu_ids=[local], noise=a.noise, include=a.include, batchSize=a.batchSize,
                              lr=a.lr, noise_on_gpu=True, augment_on_gpu=not a.no_augment and a.stage_in == 'raw', defer_loss_sync=True,
                              loss=a.loss, stage_in=a.stage_in, stage_out=a.stage_out, num_burst=a.num_burst,
-                             accum_steps=a.accum_steps)
+                             accum_steps=a.accum_steps, params_on_gpu=a.params_on_gpu)
     noise_model = NoiseModel(model=opt.noise, include=opt.include, seed=a.seed, verbose=rank == 0)   # train_syn.py:38
     ds = SyntheticClean(a.iters * a.batchSize * world, a.seed, meta=a.stage_in == 'srgb')
     sampler = torch.utils.data.distributed.DistributedSampler(ds, world, rank, shuffle=True) if world > 1 else None

@@ -119,6 +119,65 @@ int eld_noise_packed_aug(eld_ctx* ctx, const float* clean, float* noisy, float* 
                          int clip01, const uint8_t* aug_flags, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Per-frame parameters drawn on the GPU, and the noise kernels fed from device tables: the synthesis of a training step
+ * with no host work per frame, so that it can be captured in a CUDA graph and replayed on fresh frames.
+ *
+ * Random stream: the Philox4x32-10 stream above, two more domains (csrc/philox.cuh has the word layout):
+ *   domain 4 (parameters), counter frame word = f / burst: the frames of a burst share one tuple, as
+ *     NoiseModel.frame_params(burst=k) and SynDataset (dataset/sid_dataset.py:269-275) share one _sample_params();
+ *   domain 5 (augmentation flags), counter frame word = f.
+ * f = the global frame id: frame_id0 + i, plus *frame_id0_dev when frame_id0_dev != NULL (a device counter, so that a
+ * replayed graph draws new frames; see eld_frame_counter_add).
+ *
+ * The laws are NoiseModel._sample_params' (noise.py:201-225) and, full_model != 0, those of the paper-restated model
+ * (eld_b200.noise.NoiseModel._sample_params_full), computed in float64 from 53-bit uniforms and rounded to the float
+ * fields at the end:
+ *   camera uniform over cameras[0 .. n_cameras);  log K ~ U(ln 0.1, ln 30);  log s = N(0,1) sigma + slope log K + bias
+ *   for s = g_scale (and, full model, G_scale and R_scale; Box-Muller normals);  ratio ~ U(100, 300);
+ *   saturation 15583;  q_step 1;  full model: one row index uniform over the camera's `rows`, shared by G_lambda =
+ *   G_shape[row] and color_bias = color_bias[row].  Fields a model does not draw are 0.
+ * The per-frame values differ from the host draws (numpy's RandomState) but follow the same laws. */
+#define ELD_MAX_CAMERAS     5
+#define ELD_MAX_CALIB_ROWS  18
+typedef struct eld_camera_calib {
+    double g_slope, g_bias, g_sigma;      /* Profile-1 'g_scale': log g_scale = N(0,1) g_sigma + g_slope log K + g_bias */
+    double G_slope, G_bias, G_sigma;      /* Profile-1 'G_scale' (full model)                                           */
+    double R_slope, R_bias, R_sigma;      /* Profile-1 'R_scale' (full model)                                           */
+    int    rows;                          /* number of G_shape / color_bias rows, 1 .. ELD_MAX_CALIB_ROWS               */
+    float  G_shape[ELD_MAX_CALIB_ROWS];   /* Tukey-lambda shapes                                                         */
+    float  color_bias[ELD_MAX_CALIB_ROWS][4];
+} eld_camera_calib;                       /* 440 bytes */
+
+/* Draws the parameters of frames i = 0 .. n-1 into params_out[i] (DEVICE, n entries) and, if flags_out != NULL, their
+ * augmentation flags into flags_out[i] (DEVICE, n bytes: bit 0 rows, 1 columns, 2 transpose, three fair coins, the
+ * byte eld_noise_packed_aug takes).  cameras: HOST array of n_cameras entries, copied into the launch.  One launch.
+ * ELD_E_ARG, nothing written and nothing launched: a NULL ctx or cameras, n < 0, burst < 1, n_cameras < 1 or > 5, a
+ * camera's rows < 1 or > 18, a NULL params_out with n > 0.  n == 0: ELD_OK, nothing launched.
+ * The caller's: device buffers of n entries, and a frame_id0_dev that stays valid until the launch has run. */
+int eld_noise_sample_params(eld_ctx* ctx, const eld_camera_calib* cameras, int n_cameras, int full_model, uint64_t seed,
+                            uint64_t frame_id0, const uint64_t* frame_id0_dev, int burst, int n,
+                            eld_noise_params* params_out, uint8_t* flags_out, void* stream);
+
+/* eld_noise_packed (flags_dev == NULL) and eld_noise_packed_aug (flags_dev != NULL) with the parameters and flags read
+ * from DEVICE tables of n entries (eld_noise_sample_params writes them) when the kernel runs, and the first frame id
+ * frame_id0 (+ *frame_id0_dev if frame_id0_dev != NULL).  Given the same values as host tables, the output is the host
+ * entry points' bit for bit; every frame goes in one launch (two past 65535 frames).
+ *   flags_dev == NULL: eld_noise_packed's rules (any w, in place allowed); target_out must be NULL.
+ *   flags_dev != NULL: eld_noise_packed_aug's rules - h == w (the flags are not seen on the host, so any of them may
+ *   transpose), w % 4 == 0, 16-byte aligned buffers, not in place; target_out (may be NULL) receives aug(clean).
+ * ELD_E_ARG, nothing written and nothing launched: a NULL ctx, a negative size, unknown model_mask bits, a NULL clean,
+ * noisy or params_dev with n, h, w > 0, a plane of 2^32 pixels or more, the rules above.  n, h or w == 0: ELD_OK.
+ * The caller's: each table entry needs K, ratio and saturation > 0 (the sampler's entries have them; a hand-written
+ * table is not checked), flag bytes below 8, and tables that stay valid until the launch has run. */
+int eld_noise_packed_dev(eld_ctx* ctx, const float* clean, float* noisy, float* target_out, int n, int h, int w,
+                         const eld_noise_params* params_dev, uint32_t model_mask, uint64_t seed, uint64_t frame_id0,
+                         const uint64_t* frame_id0_dev, int clip01, const uint8_t* flags_dev, void* stream);
+
+/* *counter_dev += add on `stream` (one thread): advances the device frame counter of a captured step - the same pattern
+ * as the capturable Adam's step counters.  ELD_E_ARG, nothing launched: a NULL ctx or counter_dev. */
+int eld_frame_counter_add(eld_ctx* ctx, uint64_t* counter_dev, uint64_t add, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Paired training frames: the per-pixel work of ELDTrainDataset.__getitem__ (dataset/sid_dataset.py:337-356) over
  * LMDBDataset.__getitem__ (dataset/lmdb_dataset.py:28-41), the path of train_real.py:44-58 and of train_syn.py:66-70's
  * offline-noise database, for a batch of n frames in one launch:
