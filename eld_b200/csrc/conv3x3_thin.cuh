@@ -12,22 +12,32 @@
 //           accumulates the same wgmma sequence and the results are bit-identical to conv3x3_wide_kernel's.
 // roles   = warpgroup 0: TMA producer (one thread) | warpgroups 1, 2 take whole tiles in turn (ping-pong): per k16 step
 //           two m64nNTk16 (pixel rows 0-63 / 64-127), then the epilogue of the tile, while the other warpgroup runs its
-//           MMAs.  Each has its own staging area: 128 pixel rows x 32 floats per pass, the 16-byte chunks of row r XOR-ed
-//           by r & 7 (conflict-free fragment writes and row reads without padding; 16 KB, so two 60 KB halo slots and
-//           72 KB of weights fit at K = N = 64).
+//           MMAs.
+// epilogue = on the accumulator fragments in registers: bias, LeakyReLU or LeakyReLU' mask, bf16 rounding (the fp32
+//           operations of conv_epilogue32, in its order), slope words OR-ed over each lane quad; then `stmatrix` into this
+//           warpgroup's bf16 staging rows (one [128 px][32 ch] block per 32 columns, 64-byte rows with the TMA's 64-byte
+//           swizzle) and one TMA store per block, which clips at the image border.  The fused pool reads the staging
+//           rows: four lanes per (pooled pixel, 32 channels).  Staging is 8 / 16 KB per warpgroup, so at K = N = 64 two
+//           60 KB halo slots and 72 KB of weights fit.
 #pragma once
 #include "conv_gemm.cuh"
 
 namespace eld {
 
-constexpr int kThinStgBytes = 128 * 32 * 4;            // staging of one consumer warpgroup: 128 pixels x 32 f32 columns
+// bf16 staging of one consumer warpgroup: 128 pixels x NT columns
+__host__ __device__ constexpr int thin_stg_bytes(int nt) { return 128 * nt * 2; }
 constexpr int kThinMaxSlots = 4;
 constexpr int kThinSmemBytes = 227 * 1024;             // the sm_90 per-block opt-in maximum
 
-// NT = GEMM N = 32 or 64, KC = cin = 32 or 64 (the trip counts of the MMA loop are compile-time: no wgmma serialisation)
+// byte offset of 16-byte chunk `q` (0..3) of pixel row m in a [128 px][32 ch] bf16 staging block (SWIZZLE_64B)
+__device__ __forceinline__ uint32_t thin_stg_off(int m, int q) { return (uint32_t)(m * 64 + ((q ^ ((m >> 1) & 3)) << 4)); }
+
+// NT = GEMM N = 32 or 64, KC = cin = 32 or 64 (the trip counts of the MMA loop are compile-time: no wgmma serialisation).
+// tmOut / tmOut2: `out` / `out2` as boxes {32, 16, 8} (unet_prims.cu launch_conv3x3).
 template <int NT, int KC>
 __global__ void __launch_bounds__(kConvThreads, 1)
-conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParams p)
+conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmOut,
+                    const __grid_constant__ CUtensorMap tmOut2, const ConvGemmParams p)
 {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = ptx::smem_u32(smem_raw);
@@ -36,6 +46,7 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParam
     constexpr int row_bytes = KC * 2;
     constexpr int tap_bytes = NT * row_bytes;                       // one resident tap block of B
     constexpr int slot_bytes = halo_slot_bytes(KC);
+    constexpr int NC = NT / 32;                                     // 32-column blocks of the output
     uint8_t* b_s = smem;
     uint8_t* slots = smem + 9 * tap_bytes;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.bar_smem_off);
@@ -48,6 +59,7 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParam
 
     if (threadIdx.x == 0) {
         ptx::prefetch_tmap(&tmA);
+        ptx::prefetch_tmap(&tmOut);
         for (int s = 0; s < p.stages; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 4); }
         ptx::mbar_init(b_full, 1);
         ptx::fence_barrier_init();
@@ -93,14 +105,32 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParam
     const uint32_t layout = ptx::gmma_layout(row_bytes);
     const uint64_t desc0 = ptx::make_gmma_desc(0, 16, 8u * row_bytes, layout);     // everything but the address
     const uint32_t b_base = ptx::smem_u32(b_s), slot_base = ptx::smem_u32(slots);
-    float* stg = reinterpret_cast<float*>(smem + p.stg_smem_off + cg * kThinStgBytes);
-    const int wq = t >> 5, r0 = 16 * wq + (lane >> 2), c0 = 2 * (lane & 3);
+    uint8_t* stg = smem + p.stg_smem_off + cg * thin_stg_bytes(NT);
+    const uint32_t stg_base = ptx::smem_u32(stg);
+    // fragment of this thread (wgmma.cuh): pixel rows m = 64 h + 16 wq + lr + 8 i, i.e. tile pixel (lr + 8 i, 4 h + wq),
+    // columns 8 j + 2 q + c, i.e. bf16 pair k = 4 (j % 4) + q of 32-column block j / 4
+    const int wq = t >> 5, lr = lane >> 2, q = lane & 3;
+    const size_t n_pix = (size_t)p.n_img * p.H * p.W;
+    float bias[NT / 8][2];
+#pragma unroll
+    for (int j = 0; j < NT / 8; ++j) { bias[j][0] = p.bias ? s_bias[8 * j + 2 * q] : 0.f; bias[j][1] = p.bias ? s_bias[8 * j + 2 * q + 1] : 0.f; }
     ptx::mbar_wait(b_full, 0);
-    for (int j = cg;; j += 2) {
-        const int tile = blockIdx.x + j * gridDim.x;
+    for (int jt = cg;; jt += 2) {
+        const int tile = blockIdx.x + jt * gridDim.x;
         if (tile >= total_tiles) break;
-        const int s = j % p.stages;
-        ptx::mbar_wait(&full[s], (uint32_t)(j / p.stages) & 1u);
+        const int s = jt % p.stages;
+        const int img = tile / tiles_xy;
+        const int rem = tile - img * tiles_xy;
+        const int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
+        const int x0 = tx * kConvTileW, y0 = ty * 8;
+        // this thread's four pixels u = 2 h + i: image flat index, or -1 outside the image (partial tiles)
+        long long pix[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const int x = x0 + lr + 8 * (u & 1), y = y0 + 4 * (u >> 1) + wq;
+            pix[u] = (x < p.W && y < p.H) ? ((long long)(img * p.H + y) * p.W + x) : -1;
+        }
+        ptx::mbar_wait(&full[s], (uint32_t)(jt / p.stages) & 1u);
         float acc[2][NT / 2];
         const uint32_t sa = slot_base + (uint32_t)(s * slot_bytes);
         ptx::wgmma_fence();
@@ -118,40 +148,185 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const ConvGemmParam
             }
         }
         ptx::wgmma_commit();
+        // LeakyReLU' classes of this thread's elements (slope-word layout, this thread's bits only), the slope words
+        // loaded while the MMAs run
+        uint32_t mneg[4][NC], mtie[4][NC];
+        if (p.act == ACT_MASK && p.aux_slope) {
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+#pragma unroll
+                for (int c = 0; c < NC; ++c) {
+                    const uint32_t* sw = p.aux_slope + (size_t)pix[u] * NC + c;
+                    mneg[u][c] = pix[u] >= 0 ? __ldg(sw) : 0u;
+                    mtie[u][c] = pix[u] >= 0 ? __ldg(sw + n_pix * NC) : 0u;
+                }
+        }
         ptx::wgmma_wait<0>();
         ptx::reg_fence(acc[0]);
         ptx::reg_fence(acc[1]);
         if (lane == 0) ptx::mbar_arrive(&empty[s]);
 
-        // ---- epilogue: 32 columns of all 128 pixels per pass; thread t -> pixel t ----
-        const int img = tile / tiles_xy;
-        const int rem = tile - img * tiles_xy;
-        const int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
-        const int x = tx * kConvTileW + (t & 15), y = ty * 8 + (t >> 4);
+        if (p.act == ACT_MASK && !p.aux_slope) {
+            // the C-ABI mask source: the activation itself, this thread's bf16 pairs
 #pragma unroll
-        for (int pass = 0; pass < NT / 32; ++pass) {
-            ptx::bar_sync(1 + cg, 128);                        // the previous pass / tile is done reading the staging rows
+            for (int u = 0; u < 4; ++u)
 #pragma unroll
-            for (int h = 0; h < 2; ++h)
+                for (int c = 0; c < NC; ++c) {
+                    mneg[u][c] = 0u; mtie[u][c] = 0u;
 #pragma unroll
-                for (int jj = 0; jj < 4; ++jj)
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        const int r = 64 * h + r0 + 8 * i, q = 2 * jj + (c0 >> 2);
-                        *reinterpret_cast<float2*>(stg + r * 32 + ((q ^ (r & 7)) << 2) + (c0 & 3)) =
-                            make_float2(acc[h][4 * (4 * pass + jj) + 2 * i], acc[h][4 * (4 * pass + jj) + 2 * i + 1]);
+                    for (int jj = 0; jj < 4; ++jj) {
+                        if (pix[u] < 0) continue;
+                        const int k = 4 * jj + q;
+                        const uint32_t w = __ldg(reinterpret_cast<const uint32_t*>(
+                            p.aux + (size_t)pix[u] * p.aux_pitch + (p.aux_c0 + 32 * c + 2 * k)));
+                        uint32_t n, tc;
+                        ptx::slope_classes(w, n, tc);
+                        mneg[u][c] |= (n >> (15 - k)) & (0x00010001u << k);
+                        mtie[u][c] |= (tc >> (15 - k)) & (0x00010001u << k);
                     }
-            ptx::bar_sync(1 + cg, 128);
-            float v[32];
-            const float4* src = reinterpret_cast<const float4*>(stg + t * 32);
+                }
+        }
+
+        // ---- bias, activation / mask and rounding on the fragments (conv_epilogue32's operations, in its order) ----
+        uint32_t wv[2][NT / 8][2];                     // [h][j][i]: the bf16 pair of columns 8 j + 2 q, + 1
 #pragma unroll
-            for (int q = 0; q < 8; ++q) {
-                const float4 f = src[q ^ (t & 7)];
-                v[4 * q] = f.x; v[4 * q + 1] = f.y; v[4 * q + 2] = f.z; v[4 * q + 3] = f.w;
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int j = 0; j < NT / 8; ++j)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    float v[2] = { acc[h][4 * j + 2 * i], acc[h][4 * j + 2 * i + 1] };
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        if (p.bias) v[c] += bias[j][c];
+                        if (p.act == ACT_LRELU) {
+                            v[c] = fmaxf(v[c], 0.2f * v[c]);
+                        } else if (p.act == ACT_MASK) {
+                            const int u = 2 * h + i, b = 4 * (j & 3) + q + 16 * c;
+                            v[c] *= lrelu_slope(mneg[u][j >> 2], mtie[u][j >> 2], b, kMaskNeg);
+                        }
+                    }
+                    const __nv_bfloat162 b2 = __floats2bfloat162_rn(v[0], v[1]);
+                    wv[h][j][i] = *reinterpret_cast<const uint32_t*>(&b2);
+                }
+        if (p.slope_out) {
+            // slope words of the stored activation: each lane's pairs, OR-ed over the quad; lane q stores pixel u = q
+            uint32_t sn[4][NC], st[4][NC];
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+#pragma unroll
+                for (int c = 0; c < NC; ++c) {
+                    sn[u][c] = 0u; st[u][c] = 0u;
+#pragma unroll
+                    for (int jj = 0; jj < 4; ++jj) {
+                        const int k = 4 * jj + q;
+                        uint32_t n, tc;
+                        ptx::slope_classes(wv[u >> 1][4 * c + jj][u & 1], n, tc);
+                        sn[u][c] |= (n >> (15 - k)) & (0x00010001u << k);
+                        st[u][c] |= (tc >> (15 - k)) & (0x00010001u << k);
+                    }
+#pragma unroll
+                    for (int o = 1; o <= 2; o <<= 1) {
+                        sn[u][c] |= __shfl_xor_sync(0xffffffffu, sn[u][c], o);
+                        st[u][c] |= __shfl_xor_sync(0xffffffffu, st[u][c], o);
+                    }
+                }
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+                if (u == q && pix[u] >= 0) {
+                    uint32_t* sw = p.slope_out + (size_t)pix[u] * NC;
+#pragma unroll
+                    for (int c = 0; c < NC; ++c) { sw[c] = sn[u][c]; sw[n_pix * NC + c] = st[u][c]; }
+                }
+        }
+
+        // ---- bf16 staging rows and the TMA stores ----
+        if (t == 0) ptx::bulk_wait_read<0>();           // the previous tile's stores have read the staging rows
+        ptx::bar_sync(1 + cg, 128);                    // ... and its pool threads are done with them
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int c = 0; c < NC; ++c)
+#pragma unroll
+                for (int jp = 0; jp < 2; ++jp) {
+                    // matrices g = lane / 8: (i, j) = (g % 2, 4 c + 2 jp + g / 2)
+                    const int g = lane >> 3;
+                    const int m = 64 * h + 16 * wq + 8 * (g & 1) + (lane & 7);
+                    const int j0 = 4 * c + 2 * jp;
+                    ptx::stmatrix_x4(stg_base + (uint32_t)(c * 128 * 64) + thin_stg_off(m, 2 * jp + (g >> 1)),
+                                     wv[h][j0][0], wv[h][j0][1], wv[h][j0 + 1][0], wv[h][j0 + 1][1]);
+                }
+        ptx::fence_proxy_async();
+        ptx::bar_sync(1 + cg, 128);
+        if (t == 0) {
+#pragma unroll
+            for (int c = 0; c < NC; ++c) {
+                const bool second = p.out_split && 32 * c >= p.out_split;
+                ptx::tma_store_5d(second ? &tmOut2 : &tmOut, stg + c * 128 * 64,
+                                  second ? 32 * c - p.out_split : p.out_c0 + 32 * c, x0, y0, img, 0);
             }
-            conv_epilogue32(p, s_bias, v, img, x, y, 32 * pass);
+            ptx::bulk_commit();
+        }
+        if (p.pool_out) {
+            // MaxPool2d(2) of the stored values: four lanes per (32-column block c, pooled pixel (px, py)), lane qq
+            // taking channels 8 qq .. 8 qq + 7; the window's rows (0,0) (0,1) (1,0) (1,1) in the order the backward
+            // walks it.  H, W and the tile origin are even: a window is wholly in or out.
+#pragma unroll
+            for (int it = t; it < 128 * NC; it += 128) {         // whole warps (the code words' shuffles)
+                const int qq = it & 3, px = (it >> 2) & 7, py = (it >> 5) & 3, c = it >> 7;
+                const uint8_t* blk = stg + c * 128 * 64;
+                uint32_t w[4][4];
+#pragma unroll
+                for (int d = 0; d < 4; ++d) {
+                    const uint4 v = *reinterpret_cast<const uint4*>(blk + thin_stg_off(16 * (2 * py + (d >> 1)) + 2 * px + (d & 1), qq));
+                    w[d][0] = v.x; w[d][1] = v.y; w[d][2] = v.z; w[d][3] = v.w;
+                }
+                uint32_t pw[4];
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) pw[jj] = bf2_max(bf2_max(w[0][jj], w[1][jj]), bf2_max(w[2][jj], w[3][jj]));
+                const int x = x0 + 2 * px, y = y0 + 2 * py;
+                const bool in_img = x < p.W && y < p.H;
+                const size_t ppix = (size_t)(img * (p.H >> 1) + (y >> 1)) * (p.W >> 1) + (x >> 1);
+                if (in_img)
+                    *reinterpret_cast<uint4*>(p.pool_out + ppix * p.pool_pitch + 32 * c + 8 * qq) = make_uint4(pw[0], pw[1], pw[2], pw[3]);
+                if (p.pool_code) {
+                    // per window element, over the 32 channels: "is not the window's maximum" (all clear in a window
+                    // holding NaN, where the backward picks the last NaN from the slope words) and its slope words;
+                    // each lane's pairs k = 4 qq + jj, OR-ed over the four lanes
+                    uint32_t code[12];
+#pragma unroll
+                    for (int d = 0; d < 4; ++d) {
+                        code[d] = 0u; code[4 + d] = 0u; code[8 + d] = 0u;
+#pragma unroll
+                        for (int jj = 0; jj < 4; ++jj) {
+                            const int k = 4 * qq + jj;
+                            const uint32_t ne = __hne2_mask(*reinterpret_cast<const __nv_bfloat162*>(&w[d][jj]),
+                                                            *reinterpret_cast<const __nv_bfloat162*>(&pw[jj]));
+                            uint32_t n, tc;
+                            ptx::slope_classes(w[d][jj], n, tc);
+                            code[d] |= (ne >> (15 - k)) & (0x00010001u << k);
+                            code[4 + d] |= (n >> (15 - k)) & (0x00010001u << k);
+                            code[8 + d] |= (tc >> (15 - k)) & (0x00010001u << k);
+                        }
+                    }
+#pragma unroll
+                    for (int e = 0; e < 12; ++e) {
+                        code[e] |= __shfl_xor_sync(0xffffffffu, code[e], 1);
+                        code[e] |= __shfl_xor_sync(0xffffffffu, code[e], 2);
+                    }
+                    // lane 0: the maxima masks, lane 1: the neg words (the 32-byte record), lane 2: the tie words
+                    const size_t rec = ppix * (size_t)(p.pool_pitch >> 5) + (size_t)c;
+                    const size_t recs = (size_t)p.n_img * (p.H >> 1) * (p.W >> 1) * (size_t)(p.pool_pitch >> 5);
+                    uint32_t* dst = qq == 2 ? p.pool_code + recs * 8 + rec * 4 : p.pool_code + rec * 8 + 4 * qq;
+#pragma unroll
+                    for (int g = 0; g < 3; ++g)
+                        if (in_img && qq == g)
+                            *reinterpret_cast<uint4*>(dst) = make_uint4(code[4 * g], code[4 * g + 1], code[4 * g + 2], code[4 * g + 3]);
+                }
+            }
         }
     }
+    if (t == 0) ptx::bulk_wait<0>();                   // the staging rows live until the last stores are done
 }
 
 }  // namespace eld

@@ -1,6 +1,6 @@
 // conv_gemm.cuh - persistent, warp-specialised wgmma implicit-GEMM tile for the U-Net's deconv2x2 (fprop and dgrad) on
-// NHWC bf16 activations, and the epilogue every conv / deconv tile shares.  The 3x3 convolutions run the halo tiles of
-// conv3x3_thin.cuh and conv3x3_wide.cuh.
+// NHWC bf16 activations, and the epilogue it shares with the wide 3x3 tile (conv3x3_wide.cuh).  The 3x3 convolutions run
+// the halo tiles of conv3x3_thin.cuh (which has its own epilogue on the accumulator fragments) and conv3x3_wide.cuh.
 //
 //   D[128 pixels x n_tile] (f32, registers)  +=  A[128 pixels x K] (bf16, smem via TMA)  *  B[n_tile x K]^T
 //

@@ -552,7 +552,8 @@ struct Runner {
         op.aux_slope = mask ? s->slope[l.src] : nullptr;
         ELD_REQUIRE(!mask || op.aux_slope, "eld_unet: %s dgrad: no slope words for its LeakyReLU' mask", l.name);
         const double px = (double)u->n * op.H * op.W;
-        Scope sc(u, st, l.name, "dgrad", 2.0 * px * l.cout * 9 * nc, px * 2 * (nc * (mask ? 2 : 1) + l.cout) + 18.0 * nc * l.cout);
+        // the mask is the producer's slope words: two uint32 planes per 32 channels, nc / 4 bytes per pixel
+        Scope sc(u, st, l.name, "dgrad", 2.0 * px * l.cout * 9 * nc, px * (2.0 * (nc + l.cout) + (mask ? nc / 4.0 : 0.0)) + 18.0 * nc * l.cout);
         return launch_conv_gemm(ctx(), op, st);
     }
     // data gradient of a deconv: the up half of its level's dcat -> the producer's dz, with its LeakyReLU' mask
@@ -567,7 +568,7 @@ struct Runner {
         op.aux_slope = s->slope[l.src];
         ELD_REQUIRE(op.aux_slope, "eld_unet: %s dgrad: no slope words for its LeakyReLU' mask", l.name);
         const double px = (double)u->n * op.H * op.W;
-        Scope sc(u, st, l.name, "dgrad", 2.0 * px * 4 * l.cout * l.cin, px * 2 * (2 * l.cin + 4 * l.cout) + 8.0 * l.cin * l.cout);
+        Scope sc(u, st, l.name, "dgrad", 2.0 * px * 4 * l.cout * l.cin, px * (2.0 * (l.cin + 4 * l.cout) + l.cin / 4.0) + 8.0 * l.cin * l.cout);
         return launch_conv_gemm(ctx(), op, st);
     }
     int conv_wgrad(int li, float* grads) const

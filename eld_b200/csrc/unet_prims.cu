@@ -21,8 +21,9 @@ using WgradKernel = void (*)(CUtensorMap, CUtensorMap, WgradParams);
 using WgradThinKernel = void (*)(CUtensorMap, CUtensorMap, WgradThinParams);
 using FirstConvKernel = void (*)(CUtensorMap, CUtensorMap, FirstConvParams);
 static const ConvKernel kConvGemm[3] = { conv_gemm_kernel<32>, conv_gemm_kernel<64>, conv_gemm_kernel<128> };
-static const ConvKernel kConvThin[2][2] = { { conv3x3_thin_kernel<32, 32>, conv3x3_thin_kernel<32, 64> },
-                                            { conv3x3_thin_kernel<64, 32>, conv3x3_thin_kernel<64, 64> } };
+using ConvThinKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, ConvGemmParams);
+static const ConvThinKernel kConvThin[2][2] = { { conv3x3_thin_kernel<32, 32>, conv3x3_thin_kernel<32, 64> },
+                                                { conv3x3_thin_kernel<64, 32>, conv3x3_thin_kernel<64, 64> } };
 static const ConvKernel kConvWide[3][2] = { { conv3x3_wide_kernel<32, 32>, conv3x3_wide_kernel<32, 64> },
                                             { conv3x3_wide_kernel<64, 32>, conv3x3_wide_kernel<64, 64> },
                                             { conv3x3_wide_kernel<128, 32>, conv3x3_wide_kernel<128, 64> } };
@@ -162,19 +163,26 @@ static int launch_conv3x3(eld_ctx* ctx, const GemmOp& op, ConvGemmParams& p, cud
     const int rb = p.kc * 2;
     const int slot_bytes = halo_slot_bytes(p.kc);
     if ((op.cin == 32 || op.cin == 64) && (p.n_total == 32 || p.n_total == 64)) {
-        // [resident weights][halo slots][staging of both consumer warpgroups][bias][barriers] after the 1024-byte alignment
-        const int fixed = 9 * p.n_tile * rb + 2 * kThinStgBytes + 256;
+        // [resident weights][halo slots][staging of both consumer warpgroups][bias][barriers] after the 1024-byte
+        // alignment; every part a multiple of 1 KB, so each staging block sits on its 64-byte swizzle's 512-byte period
+        const int stg = thin_stg_bytes(p.n_tile);
+        const int fixed = 9 * p.n_tile * rb + 2 * stg + 256;
         int slots = (kThinSmemBytes - 1024 - fixed - 256) / slot_bytes;
         if (slots > kThinMaxSlots) slots = kThinMaxSlots;
         ELD_REQUIRE(slots >= 2, "thin conv tile: no room for two halo slots");
         p.stages = slots;
         p.stg_smem_off = 9 * p.n_tile * rb + slots * slot_bytes;
-        p.bias_smem_off = p.stg_smem_off + 2 * kThinStgBytes;
+        p.bias_smem_off = p.stg_smem_off + 2 * stg;
         p.bar_smem_off = p.bias_smem_off + 256;
         const size_t smem = 1024 + (size_t)p.bar_smem_off + 256;
+        // the epilogue's TMA stores: 32 channels x 16 x 8 pixels per box, clipped at the image border
+        CUtensorMap tmOut, tmOut2;
+        { int rc = encode_nhwc(ctx, &tmOut, op.out, op.out_pitch, op.n_img, op.H, op.W, 32, kConvTileW, 8); if (rc) return rc; }
+        tmOut2 = tmOut;
+        if (op.out_split) { int rc = encode_nhwc(ctx, &tmOut2, op.out2, op.out2_pitch, op.n_img, op.H, op.W, 32, kConvTileW, 8); if (rc) return rc; }
         const int total_tiles = op.n_img * p.tiles_x * p.tiles_y;
         return launch(ctx, kConvThin[p.n_tile / 64][p.kc / 64], std::min(total_tiles, ctx->num_sms), kConvThreads, smem, st,
-                      tmA, p);
+                      tmA, tmOut, tmOut2, p);
     }
     // [halo slots][weight ring][staging of both consumer warpgroups][bias][barriers] after the 1024-byte alignment;
     // the weight ring takes what the opt-in maximum leaves

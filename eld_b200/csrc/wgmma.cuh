@@ -80,6 +80,28 @@ __device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t b
                  ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
+// tensor store shared -> global of one box (out-of-tensor elements are not written), tracked by the bulk async-groups
+__device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3, int c4)
+{
+    asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
+                 ::"l"(m), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// wait until at most N committed bulk groups are pending: `read` = until they have read their shared-memory source
+// (it may be overwritten), else until their writes are done
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+
+// four 8 x 8 b16 matrices to shared memory: lane l holds row l / 4, columns 2 (l % 4) .. + 1 of matrix i in r[i] (the
+// layout of a wgmma accumulator fragment's 8-column groups); lanes 8i .. 8i + 7 give the row addresses of matrix i
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3)
+{
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};"
+                 ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
+}
+
 // ---- 32-byte global accesses (two 128-bit instructions; 32-byte aligned) ----------------------------------------
 // An epilogue thread owns 64 contiguous bytes of its pixel: it writes them as two full 32-byte sectors.
 __device__ __forceinline__ void st_global_32B(void* p, const uint32_t w[8])
@@ -193,17 +215,20 @@ __device__ __forceinline__ uint32_t gather_msb16(const uint32_t (&w)[16])
 // stored bf16 activation has the class of x.  Two bits per element carry it: `neg` = negative and finite, or NaN, and
 // `tie` = +-0, +-Inf or NaN.  slope_words turns 16 packed bf16x2 words into the two words, in the channel layout of
 // gather_msb16 (the slope words and pool codes).
-__device__ __forceinline__ void slope_words(const uint32_t (&w)[16], uint32_t& neg, uint32_t& tie)
+// slope_classes: the two classes of one packed bf16x2 word, in the top bit of each 16-bit half.
+__device__ __forceinline__ void slope_classes(uint32_t w, uint32_t& n, uint32_t& t)
 {
     // per 16-bit half, in its top bit (all gather_msb16 reads; the 15-bit magnitudes never carry or borrow across
     // halves): magnitude >= 0x7F80 (Inf, NaN) | magnitude == 0, and magnitude > 0x7F80 (NaN)
+    const uint32_t mag = w & 0x7FFF7FFFu;
+    t = (mag + 0x00800080u) | (0x80008000u - mag);
+    n = (mag + 0x007F007Fu) | (w & ~t);
+}
+__device__ __forceinline__ void slope_words(const uint32_t (&w)[16], uint32_t& neg, uint32_t& tie)
+{
     uint32_t n[16], t[16];
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-        const uint32_t mag = w[j] & 0x7FFF7FFFu;
-        t[j] = (mag + 0x00800080u) | (0x80008000u - mag);
-        n[j] = (mag + 0x007F007Fu) | (w[j] & ~t[j]);
-    }
+    for (int j = 0; j < 16; ++j) slope_classes(w[j], n[j], t[j]);
     neg = gather_msb16(n);
     tie = gather_msb16(t);
 }
