@@ -10,34 +10,51 @@
 //           bulk-copied once per CTA and resident for every tile (at most 72 KB).
 // K order = the wide tile's with one channel chunk (cin = kc): taps 0..8, k16 steps inside a tap, so every output row
 //           accumulates the same wgmma sequence and the results are bit-identical to conv3x3_wide_kernel's.
-// roles   = warpgroup 0: TMA producer (one thread) | warpgroups 1, 2 take whole tiles in turn (ping-pong): per k16 step
-//           two m64nNTk16 (pixel rows 0-63 / 64-127), then the epilogue of the tile, while the other warpgroup runs its
-//           MMAs.
+// roles   = warpgroup 0: TMA producer (one thread) | consumer warpgroups 1, 2, 3 take whole tiles in turn (tile j of the
+//           CTA goes to warpgroup j % 3): per k16 step two m64nNTk16 (pixel rows 0-63 / 64-127), then the epilogue of
+//           the tile, while the other warpgroups run their MMAs.  The epilogue costs 1.5-3x a tile's MMAs, so with two
+//           consumers the tensor pipe idled for most of each tile.  A 512-thread CTA gets 128 registers per thread
+//           evenly; setmaxnreg gives the producer 24 and the consumers 152 (NT = 32) or 160 (NT = 64).
 // epilogue = on the accumulator fragments in registers: bias, LeakyReLU or LeakyReLU' mask, bf16 rounding (the fp32
 //           operations of conv_epilogue32, in its order), slope words OR-ed over each lane quad; then `stmatrix` into this
-//           warpgroup's bf16 staging rows (one [128 px][32 ch] block per 32 columns, 64-byte rows with the TMA's 64-byte
-//           swizzle) and one TMA store per block, which clips at the image border.  The fused pool reads the staging
-//           rows: four lanes per (pooled pixel, 32 channels).  Staging is 8 / 16 KB per warpgroup, so at K = N = 64 two
-//           60 KB halo slots and 72 KB of weights fit.
+//           warpgroup's bf16 staging rows ([128 px][32 ch] blocks, 64-byte rows with the TMA's 64-byte swizzle) and one
+//           TMA store per block, which clips at the image border.  The fused pool reads the staging rows: four lanes per
+//           (pooled pixel, 32 channels).  A warpgroup stages all NT / 32 blocks of a tile at once, except at <64, 64>:
+//           its 72 KB of weights and two 60 KB halo slots leave room for one 8 KB block per warpgroup, which then
+//           takes the tile's two 32-column halves in two passes.
+// mask    = the slope words of the training dgrads (aux_slope): the producer loads the tile's {16 NC, 8} words of both
+//           planes as one TMA box into the stage, with the halo on the same `full` barrier (1-2 KB per stage); global
+//           loads issued under the MMAs outlasted them.  The C-ABI mask (the activation itself, `aux`) is read from
+//           global memory.
 #pragma once
 #include "conv_gemm.cuh"
 
 namespace eld {
 
-// bf16 staging of one consumer warpgroup: 128 pixels x NT columns
-__host__ __device__ constexpr int thin_stg_bytes(int nt) { return 128 * nt * 2; }
+// consumer warpgroups (the header's roles) and the CTA size
+constexpr int kThinConsumers = 3;
+constexpr int kThinThreads = 128 * (1 + kThinConsumers);
+// 32-column staging blocks of one consumer warpgroup, each [128 px][32 ch] bf16 (8 KB): all NT / 32 of a tile, but one
+// at <64, 64>, whose 72 KB of weights and two 60 KB halo slots leave room for three 8 KB blocks only
+__host__ __device__ constexpr int thin_stg_blocks(int nt, int kc) { return nt == 64 && kc == 64 ? 1 : nt / 32; }
+__host__ __device__ constexpr int thin_stg_bytes(int nt, int kc) { return thin_stg_blocks(nt, kc) * 128 * 32 * 2; }
+// bytes per stage of the slope-word box (the header's mask): two planes of 8 rows x 16 pixels x nt / 32 words
+__host__ __device__ constexpr int thin_slope_bytes(int nt) { return 2 * 8 * 16 * (nt / 32) * 4; }
 constexpr int kThinMaxSlots = 4;
 constexpr int kThinSmemBytes = 227 * 1024;             // the sm_90 per-block opt-in maximum
+constexpr int kThinProducerRegs = 24;
 
 // byte offset of 16-byte chunk `q` (0..3) of pixel row m in a [128 px][32 ch] bf16 staging block (SWIZZLE_64B)
 __device__ __forceinline__ uint32_t thin_stg_off(int m, int q) { return (uint32_t)(m * 64 + ((q ^ ((m >> 1) & 3)) << 4)); }
 
 // NT = GEMM N = 32 or 64, KC = cin = 32 or 64 (the trip counts of the MMA loop are compile-time: no wgmma serialisation).
-// tmOut / tmOut2: `out` / `out2` as boxes {32, 16, 8} (unet_prims.cu launch_conv3x3).
+// tmOut / tmOut2: `out` / `out2` as boxes {32, 16, 8}; tmSlope: `aux_slope` as boxes {16 NC, 8, 2} (unet_prims.cu
+// launch_conv3x3).
 template <int NT, int KC>
-__global__ void __launch_bounds__(kConvThreads, 1)
+__global__ void __launch_bounds__(kThinThreads, 1)
 conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmOut,
-                    const __grid_constant__ CUtensorMap tmOut2, const ConvGemmParams p)
+                    const __grid_constant__ CUtensorMap tmOut2, const __grid_constant__ CUtensorMap tmSlope,
+                    const ConvGemmParams p)
 {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = ptx::smem_u32(smem_raw);
@@ -47,10 +64,19 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     constexpr int tap_bytes = NT * row_bytes;                       // one resident tap block of B
     constexpr int slot_bytes = halo_slot_bytes(KC);
     constexpr int NC = NT / 32;                                     // 32-column blocks of the output
+    constexpr int CG = kThinConsumers;
+    constexpr int SB = thin_stg_blocks(NT, KC);
+    constexpr int slope_bytes = thin_slope_bytes(NT);
+    // the slope-word box: plane 0 (neg) then plane 1 (tie), each [8 rows][16 pixels][NC]
+    const bool slope_box = p.act == ACT_MASK && p.aux_slope;
     uint8_t* b_s = smem;
     uint8_t* slots = smem + 9 * tap_bytes;
+    uint8_t* slope_s = slots + p.stages * slot_bytes;               // [stage] slope-word boxes
+    // full[stage][consumer]: a consumer waits only on its own barriers, so each phase it waits for is its next fill.
+    // One barrier per stage would let a consumer whose previous tile of the stage was another's (CG does not divide
+    // the stage count) see that earlier fill's phase parity as its own fill done.
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.bar_smem_off);
-    uint64_t* empty = full + p.stages;
+    uint64_t* empty = full + p.stages * CG;
     uint64_t* b_full = empty + p.stages;
     float* s_bias = reinterpret_cast<float*>(smem + p.bias_smem_off);
 
@@ -60,12 +86,16 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     if (threadIdx.x == 0) {
         ptx::prefetch_tmap(&tmA);
         ptx::prefetch_tmap(&tmOut);
-        for (int s = 0; s < p.stages; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 4); }
+        if (slope_box) ptx::prefetch_tmap(&tmSlope);
+        for (int s = 0; s < p.stages; ++s) {
+            for (int c = 0; c < CG; ++c) ptx::mbar_init(&full[s * CG + c], 1);
+            ptx::mbar_init(&empty[s], 4);
+        }
         ptx::mbar_init(b_full, 1);
         ptx::fence_barrier_init();
     }
     if (p.bias)
-        for (int i = threadIdx.x; i < p.n_total; i += kConvThreads) s_bias[i] = __ldg(p.bias + i);
+        for (int i = threadIdx.x; i < p.n_total; i += kThinThreads) s_bias[i] = __ldg(p.bias + i);
     __syncthreads();
     // PDL: the activations, the mask sources, the output and (for the C-ABI primitive) the weights belong to the
     // previous kernels
@@ -74,12 +104,13 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 
     if (threadIdx.x < 128) {
         // ===================== TMA producer (warpgroup 0; one thread works) =====================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kThinProducerRegs));
         if (threadIdx.x == 0) {
             // rows 0 .. NT-1 of every tap block (a prefix when the operand has b_rows > NT rows per block)
             ptx::mbar_arrive_expect_tx(b_full, (uint32_t)(9 * tap_bytes));
             for (int tap = 0; tap < 9; ++tap)
                 ptx::bulk_load(b_s + tap * tap_bytes, p.b_ptr + (size_t)tap * p.b_rows * row_bytes, (uint32_t)tap_bytes, b_full);
-            int s = 0;
+            int s = 0, c = 0;
             uint32_t ph = 0;
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const int img = tile / tiles_xy;
@@ -88,15 +119,19 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 const int x0 = tx * kConvTileW, y0 = ty * 8;
                 ptx::mbar_wait(&empty[s], ph ^ 1u);
                 uint8_t* sa = slots + (size_t)s * slot_bytes;
-                ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)slot_bytes);
-                halo_load<KC>(sa, &tmA, &full[s], p.a_c0, x0, y0, img);
+                uint64_t* bar = &full[s * CG + c];
+                ptx::mbar_arrive_expect_tx(bar, (uint32_t)(slot_bytes + (slope_box ? slope_bytes : 0)));
+                halo_load<KC>(sa, &tmA, bar, p.a_c0, x0, y0, img);
+                if (slope_box) ptx::tma_load_3d(slope_s + s * slope_bytes, &tmSlope, bar, x0 * NC, img * p.H + y0, 0);
                 if (++s == p.stages) { s = 0; ph ^= 1u; }
+                if (++c == CG) c = 0;
             }
         }
         return;
     }
 
-    // ===================== consumers: warpgroup cg = 0 / 1 owns tiles j = cg, cg + 2, ... of this CTA =====================
+    // ===================== consumers: warpgroup cg = 0 .. CG-1 owns tiles j = cg, cg + CG, ... of this CTA =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(NT == 32 ? 152 : 160));
     // broadcast from lane 0: the compiler then knows cg, and every tile index and descriptor derived from it, to be
     // warp-uniform (without it the wgmma loop counts as a divergent path and ptxas serialises the MMAs)
     const int cg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7) - 1, 0);
@@ -105,7 +140,7 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     const uint32_t layout = ptx::gmma_layout(row_bytes);
     const uint64_t desc0 = ptx::make_gmma_desc(0, 16, 8u * row_bytes, layout);     // everything but the address
     const uint32_t b_base = ptx::smem_u32(b_s), slot_base = ptx::smem_u32(slots);
-    uint8_t* stg = smem + p.stg_smem_off + cg * thin_stg_bytes(NT);
+    uint8_t* stg = smem + p.stg_smem_off + cg * thin_stg_bytes(NT, KC);
     const uint32_t stg_base = ptx::smem_u32(stg);
     // fragment of this thread (wgmma.cuh): pixel rows m = 64 h + 16 wq + lr + 8 i, i.e. tile pixel (lr + 8 i, 4 h + wq),
     // columns 8 j + 2 q + c, i.e. bf16 pair k = 4 (j % 4) + q of 32-column block j / 4
@@ -115,7 +150,8 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 #pragma unroll
     for (int j = 0; j < NT / 8; ++j) { bias[j][0] = p.bias ? s_bias[8 * j + 2 * q] : 0.f; bias[j][1] = p.bias ? s_bias[8 * j + 2 * q + 1] : 0.f; }
     ptx::mbar_wait(b_full, 0);
-    for (int jt = cg;; jt += 2) {
+    uint32_t full_ph = 0;                              // bit s: the parity of this consumer's next fill of stage s
+    for (int jt = cg;; jt += CG) {
         const int tile = blockIdx.x + jt * gridDim.x;
         if (tile >= total_tiles) break;
         const int s = jt % p.stages;
@@ -130,7 +166,8 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             const int x = x0 + lr + 8 * (u & 1), y = y0 + 4 * (u >> 1) + wq;
             pix[u] = (x < p.W && y < p.H) ? ((long long)(img * p.H + y) * p.W + x) : -1;
         }
-        ptx::mbar_wait(&full[s], (uint32_t)(jt / p.stages) & 1u);
+        ptx::mbar_wait(&full[s * CG + cg], (full_ph >> s) & 1u);
+        full_ph ^= 1u << s;
         float acc[2][NT / 2];
         const uint32_t sa = slot_base + (uint32_t)(s * slot_bytes);
         ptx::wgmma_fence();
@@ -148,22 +185,24 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             }
         }
         ptx::wgmma_commit();
-        // LeakyReLU' classes of this thread's elements (slope-word layout, this thread's bits only), the slope words
-        // loaded while the MMAs run
+        // LeakyReLU' classes of this thread's elements (slope-word layout, this thread's bits only), read from the
+        // stage's slope-word box while the MMAs run
         uint32_t mneg[4][NC], mtie[4][NC];
-        if (p.act == ACT_MASK && p.aux_slope) {
+        if (slope_box) {
+            const uint32_t* sw = reinterpret_cast<const uint32_t*>(slope_s + s * slope_bytes);
 #pragma unroll
             for (int u = 0; u < 4; ++u)
 #pragma unroll
                 for (int c = 0; c < NC; ++c) {
-                    const uint32_t* sw = p.aux_slope + (size_t)pix[u] * NC + c;
-                    mneg[u][c] = pix[u] >= 0 ? __ldg(sw) : 0u;
-                    mtie[u][c] = pix[u] >= 0 ? __ldg(sw + n_pix * NC) : 0u;
+                    const int w = ((4 * (u >> 1) + wq) * kConvTileW + lr + 8 * (u & 1)) * NC + c;
+                    mneg[u][c] = sw[w];
+                    mtie[u][c] = sw[128 * NC + w];
                 }
         }
         ptx::wgmma_wait<0>();
         ptx::reg_fence(acc[0]);
         ptx::reg_fence(acc[1]);
+        if (slope_box) __syncwarp();                   // every lane's reads of the stage's slope words are done
         if (lane == 0) ptx::mbar_arrive(&empty[s]);
 
         if (p.act == ACT_MASK && !p.aux_slope) {
@@ -240,29 +279,31 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 }
         }
 
-        // ---- bf16 staging rows and the TMA stores ----
-        if (t == 0) ptx::bulk_wait_read<0>();           // the previous tile's stores have read the staging rows
+        // ---- bf16 staging rows and the TMA stores: SB 32-column blocks per pass ----
+#pragma unroll
+        for (int c0 = 0; c0 < NC; c0 += SB) {
+        if (t == 0) ptx::bulk_wait_read<0>();           // the previous pass's stores have read the staging rows
         ptx::bar_sync(1 + cg, 128);                    // ... and its pool threads are done with them
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int c = 0; c < NC; ++c)
+            for (int c = c0; c < c0 + SB; ++c)
 #pragma unroll
                 for (int jp = 0; jp < 2; ++jp) {
                     // matrices g = lane / 8: (i, j) = (g % 2, 4 c + 2 jp + g / 2)
                     const int g = lane >> 3;
                     const int m = 64 * h + 16 * wq + 8 * (g & 1) + (lane & 7);
                     const int j0 = 4 * c + 2 * jp;
-                    ptx::stmatrix_x4(stg_base + (uint32_t)(c * 128 * 64) + thin_stg_off(m, 2 * jp + (g >> 1)),
+                    ptx::stmatrix_x4(stg_base + (uint32_t)((c - c0) * 128 * 64) + thin_stg_off(m, 2 * jp + (g >> 1)),
                                      wv[h][j0][0], wv[h][j0][1], wv[h][j0 + 1][0], wv[h][j0 + 1][1]);
                 }
         ptx::fence_proxy_async();
         ptx::bar_sync(1 + cg, 128);
         if (t == 0) {
 #pragma unroll
-            for (int c = 0; c < NC; ++c) {
+            for (int c = c0; c < c0 + SB; ++c) {
                 const bool second = p.out_split && 32 * c >= p.out_split;
-                ptx::tma_store_5d(second ? &tmOut2 : &tmOut, stg + c * 128 * 64,
+                ptx::tma_store_5d(second ? &tmOut2 : &tmOut, stg + (c - c0) * 128 * 64,
                                   second ? 32 * c - p.out_split : p.out_c0 + 32 * c, x0, y0, img, 0);
             }
             ptx::bulk_commit();
@@ -272,9 +313,9 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             // taking channels 8 qq .. 8 qq + 7; the window's rows (0,0) (0,1) (1,0) (1,1) in the order the backward
             // walks it.  H, W and the tile origin are even: a window is wholly in or out.
 #pragma unroll
-            for (int it = t; it < 128 * NC; it += 128) {         // whole warps (the code words' shuffles)
-                const int qq = it & 3, px = (it >> 2) & 7, py = (it >> 5) & 3, c = it >> 7;
-                const uint8_t* blk = stg + c * 128 * 64;
+            for (int it = t; it < 128 * SB; it += 128) {         // whole warps (the code words' shuffles)
+                const int qq = it & 3, px = (it >> 2) & 7, py = (it >> 5) & 3, c = c0 + (it >> 7);
+                const uint8_t* blk = stg + (it >> 7) * 128 * 64;
                 uint32_t w[4][4];
 #pragma unroll
                 for (int d = 0; d < 4; ++d) {
@@ -324,6 +365,7 @@ conv3x3_thin_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                             *reinterpret_cast<uint4*>(dst) = make_uint4(code[4 * g], code[4 * g + 1], code[4 * g + 2], code[4 * g + 3]);
                 }
             }
+        }
         }
     }
     if (t == 0) ptx::bulk_wait<0>();                   // the staging rows live until the last stores are done

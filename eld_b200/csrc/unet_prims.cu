@@ -21,7 +21,7 @@ using WgradKernel = void (*)(CUtensorMap, CUtensorMap, WgradParams);
 using WgradThinKernel = void (*)(CUtensorMap, CUtensorMap, WgradThinParams);
 using FirstConvKernel = void (*)(CUtensorMap, CUtensorMap, FirstConvParams);
 static const ConvKernel kConvGemm[3] = { conv_gemm_kernel<32>, conv_gemm_kernel<64>, conv_gemm_kernel<128> };
-using ConvThinKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, ConvGemmParams);
+using ConvThinKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, ConvGemmParams);
 static const ConvThinKernel kConvThin[2][2] = { { conv3x3_thin_kernel<32, 32>, conv3x3_thin_kernel<32, 64> },
                                                 { conv3x3_thin_kernel<64, 32>, conv3x3_thin_kernel<64, 64> } };
 static const ConvKernel kConvWide[3][2] = { { conv3x3_wide_kernel<32, 32>, conv3x3_wide_kernel<32, 64> },
@@ -163,16 +163,18 @@ static int launch_conv3x3(eld_ctx* ctx, const GemmOp& op, ConvGemmParams& p, cud
     const int rb = p.kc * 2;
     const int slot_bytes = halo_slot_bytes(p.kc);
     if ((op.cin == 32 || op.cin == 64) && (p.n_total == 32 || p.n_total == 64)) {
-        // [resident weights][halo slots][staging of both consumer warpgroups][bias][barriers] after the 1024-byte
-        // alignment; every part a multiple of 1 KB, so each staging block sits on its 64-byte swizzle's 512-byte period
-        const int stg = thin_stg_bytes(p.n_tile);
-        const int fixed = 9 * p.n_tile * rb + 2 * stg + 256;
-        int slots = (kThinSmemBytes - 1024 - fixed - 256) / slot_bytes;
+        // [resident weights][halo slots][slope-word boxes][staging of the consumer warpgroups][bias][barriers] after
+        // the 1024-byte alignment; every part a multiple of 1 KB, so each staging block sits on its 64-byte swizzle's
+        // 512-byte period
+        const int cg = kThinConsumers, slope_bytes = thin_slope_bytes(p.n_tile);
+        const int stg = thin_stg_bytes(p.n_tile, p.kc);
+        const int fixed = 9 * p.n_tile * rb + cg * stg + 256;
+        int slots = (kThinSmemBytes - 1024 - fixed - 256) / (slot_bytes + slope_bytes);
         if (slots > kThinMaxSlots) slots = kThinMaxSlots;
         ELD_REQUIRE(slots >= 2, "thin conv tile: no room for two halo slots");
         p.stages = slots;
-        p.stg_smem_off = 9 * p.n_tile * rb + slots * slot_bytes;
-        p.bias_smem_off = p.stg_smem_off + 2 * stg;
+        p.stg_smem_off = 9 * p.n_tile * rb + slots * (slot_bytes + slope_bytes);
+        p.bias_smem_off = p.stg_smem_off + cg * stg;
         p.bar_smem_off = p.bias_smem_off + 256;
         const size_t smem = 1024 + (size_t)p.bar_smem_off + 256;
         // the epilogue's TMA stores: 32 channels x 16 x 8 pixels per box, clipped at the image border
@@ -180,9 +182,23 @@ static int launch_conv3x3(eld_ctx* ctx, const GemmOp& op, ConvGemmParams& p, cud
         { int rc = encode_nhwc(ctx, &tmOut, op.out, op.out_pitch, op.n_img, op.H, op.W, 32, kConvTileW, 8); if (rc) return rc; }
         tmOut2 = tmOut;
         if (op.out_split) { int rc = encode_nhwc(ctx, &tmOut2, op.out2, op.out2_pitch, op.n_img, op.H, op.W, 32, kConvTileW, 8); if (rc) return rc; }
+        // the slope words loaded with the halo: the two planes [n H][W nc] as (word, row, plane), boxes of one tile's
+        // {16 nc, 8} words of both, unswizzled.  Images share the row dimension, so the tiles must be whole.
+        CUtensorMap tmSlope = tmA;
+        if (p.aux_slope) {
+            const int nc = p.n_tile / 32;
+            ELD_REQUIRE(op.H % 8 == 0 && op.W % kConvTileW == 0 && (reinterpret_cast<uintptr_t>(op.aux_slope) & 15) == 0,
+                        "thin conv tile: a slope-word mask needs whole 8 x 16 tiles (H=%d, W=%d) and 16-byte aligned words",
+                        op.H, op.W);
+            const cuuint64_t dims[3] = { (cuuint64_t)op.W * nc, (cuuint64_t)op.n_img * op.H, 2 };
+            const cuuint64_t str[2] = { (cuuint64_t)op.W * nc * 4, (cuuint64_t)op.n_img * op.H * op.W * nc * 4 };
+            const cuuint32_t box[3] = { (cuuint32_t)(kConvTileW * nc), 8, 2 };
+            int rc = encode(ctx, &tmSlope, op.aux_slope, 3, dims, str, box, 0 /* unswizzled */, CU_TENSOR_MAP_DATA_TYPE_UINT32);
+            if (rc) return rc;
+        }
         const int total_tiles = op.n_img * p.tiles_x * p.tiles_y;
-        return launch(ctx, kConvThin[p.n_tile / 64][p.kc / 64], std::min(total_tiles, ctx->num_sms), kConvThreads, smem, st,
-                      tmA, tmOut, tmOut2, p);
+        return launch(ctx, kConvThin[p.n_tile / 64][p.kc / 64], std::min(total_tiles, ctx->num_sms),
+                      kThinThreads, smem, st, tmA, tmOut, tmOut2, tmSlope, p);
     }
     // [halo slots][weight ring][staging of both consumer warpgroups][bias][barriers] after the 1024-byte alignment;
     // the weight ring takes what the opt-in maximum leaves
