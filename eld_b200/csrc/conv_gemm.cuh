@@ -1,6 +1,6 @@
 // conv_gemm.cuh - persistent, warp-specialised wgmma implicit-GEMM tile for the U-Net's deconv2x2 (fprop and dgrad) on
-// NHWC bf16 activations, and the epilogue it shares with the wide 3x3 tile (conv3x3_wide.cuh).  The 3x3 convolutions run
-// the halo tiles of conv3x3_thin.cuh (which has its own epilogue on the accumulator fragments) and conv3x3_wide.cuh.
+// NHWC bf16 activations, and its epilogue through shared memory.  The 3x3 convolutions run the halo tiles of
+// conv3x3_thin.cuh and conv3x3_wide.cuh, which share an epilogue on the accumulator fragments.
 //
 //   D[128 pixels x n_tile] (f32, registers)  +=  A[128 pixels x K] (bf16, smem via TMA)  *  B[n_tile x K]^T
 //
@@ -12,7 +12,7 @@
 //           swizzled shared-memory image, one linear bulk copy each.
 // roles   = warpgroup 0: TMA producer (one thread) | warpgroups 1, 2: wgmma on pixel rows 0-63 / 64-127 of the tile,
 //           then the epilogue of those rows (accumulators -> smem -> one pixel x 32 channels per thread ->
-//           bias / LeakyReLU / mask -> bf16 -> global).  The producer runs ahead across tiles, so the next tile's
+//           bias / mask -> bf16 -> global).  The producer runs ahead across tiles, so the next tile's
 //           operands load while the consumers run the epilogue.
 #pragma once
 #include "tile.cuh"
@@ -65,8 +65,8 @@ __device__ __forceinline__ uint32_t bf2_max(uint32_t a, uint32_t b)
 constexpr int kConvThreads = 384;
 constexpr int kConvStg = 68;          // floats per staged pixel row (64 columns + 4: conflict-free 16-byte reads)
 
-// One pixel x 32 GEMM columns of the epilogue: bias, activation / mask, bf16 rounding, sign words, fused pool, store.
-// All 32 lanes of the warp call it together (the pool's 2x2 window lives in lanes ^1 and ^16).
+// One pixel x 32 GEMM columns of the deconvolutions' epilogue: bias, LeakyReLU' mask, bf16 rounding, store (the
+// dgrad's plain store, or the fprop's pixel shuffle).
 __device__ __forceinline__ void conv_epilogue32(const ConvGemmParams& p, const float* s_bias, float (&v)[32],
                                                 int img, int x, int y, int col)
 {
@@ -75,8 +75,7 @@ __device__ __forceinline__ void conv_epilogue32(const ConvGemmParams& p, const f
     __nv_bfloat16* dst;
     int bcol;
     if (p.epi_mode == EPI_STORE) {
-        dst = (p.out_split && col >= p.out_split) ? p.out2 + (size_t)pix * p.out2_pitch + (col - p.out_split)
-                                                  : p.out + (size_t)pix * p.out_pitch + (p.out_c0 + col);
+        dst = p.out + (size_t)pix * p.out_pitch + (p.out_c0 + col);
         bcol = col;
     } else {
         const int sub = col >> p.cout_shift, co = col & (p.cout - 1);   // sub = kh*2 + kw
@@ -92,10 +91,7 @@ __device__ __forceinline__ void conv_epilogue32(const ConvGemmParams& p, const f
             v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
         }
     }
-    if (p.act == ACT_LRELU) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.2f * v[j]);
-    } else if (p.act == ACT_MASK && in_img) {
+    if (p.act == ACT_MASK && in_img) {
         uint32_t neg, tie;
         if (p.aux_slope) {
             const size_t plane = (size_t)p.n_img * p.H * p.W * (size_t)(p.n_total >> 5);
@@ -114,64 +110,13 @@ __device__ __forceinline__ void conv_epilogue32(const ConvGemmParams& p, const f
             v[2 * j + 1] *= lrelu_slope(neg, tie, 16 + j, kMaskNeg);
         }
     }
-    // round once; the pool below works on the rounded (= stored) values
+    if (!in_img) return;
     uint32_t wv[16];
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
         const __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
         wv[j] = *reinterpret_cast<const uint32_t*>(&h);
     }
-    uint32_t neg = 0, tie = 0;
-    if (p.slope_out || p.pool_code) ptx::slope_words(wv, neg, tie);
-    if (p.slope_out && in_img) {
-        // slope words of the stored activation: all a later LeakyReLU' needs (1/8 of the tensor)
-        const size_t plane = (size_t)p.n_img * p.H * p.W * (size_t)(p.n_total >> 5);
-        uint32_t* sw = p.slope_out + (size_t)pix * (size_t)(p.n_total >> 5) + (size_t)(col >> 5);
-        sw[0] = neg; sw[plane] = tie;
-    }
-    if (p.pool_out) {
-        // MaxPool2d(2) fused: the 2x2 window of pixel (x, y) lives in lanes ^1 (x) and ^16 (y) of this warp; packed bf16x2
-        // max of the stored values.  H, W and the tile origin are even: a window is wholly in or out.
-        uint32_t pw[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            const uint32_t a = bf2_max(wv[j], __shfl_xor_sync(0xffffffffu, wv[j], 1));
-            pw[j] = bf2_max(a, __shfl_xor_sync(0xffffffffu, a, kConvTileW));
-        }
-        const bool origin = in_img && !((x | y) & 1);
-        const size_t ppix = (size_t)(img * (p.H >> 1) + (y >> 1)) * (p.W >> 1) + (x >> 1);
-        if (origin) {
-            __nv_bfloat16* q4 = p.pool_out + ppix * p.pool_pitch + col;
-            ptx::st_global_32B(q4, pw);
-            ptx::st_global_32B(q4 + 16, pw + 8);
-        }
-        if (p.pool_code) {
-            // per lane, over its 32 channels: "is not the window's maximum" (all clear in a window holding NaN, where the
-            // backward picks the last NaN from the slope words) and the slope-word pair (channel 2j -> bit j, channel
-            // 2j+1 -> bit 16+j); the window's origin lane collects the four lanes' words in the order the backward walks
-            // the window: (0,0) (0,1) (1,0) (1,1)
-            uint32_t ne[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-                ne[j] = __hne2_mask(*reinterpret_cast<const __nv_bfloat162*>(&wv[j]), *reinterpret_cast<const __nv_bfloat162*>(&pw[j]));
-            const uint32_t own[3] = { ptx::gather_msb16(ne), neg, tie };
-            uint32_t code[12];
-#pragma unroll
-            for (int k = 0; k < 3; ++k) {
-                code[4 * k] = own[k];
-                code[4 * k + 1] = __shfl_xor_sync(0xffffffffu, own[k], 1);
-                code[4 * k + 2] = __shfl_xor_sync(0xffffffffu, own[k], kConvTileW);
-                code[4 * k + 3] = __shfl_xor_sync(0xffffffffu, own[k], kConvTileW | 1);
-            }
-            if (origin) {
-                const size_t rec = ppix * (size_t)(p.pool_pitch >> 5) + (size_t)(col >> 5);
-                const size_t recs = (size_t)p.n_img * (p.H >> 1) * (p.W >> 1) * (size_t)(p.pool_pitch >> 5);
-                ptx::st_global_32B(p.pool_code + rec * 8, code);
-                *reinterpret_cast<uint4*>(p.pool_code + recs * 8 + rec * 4) = make_uint4(code[8], code[9], code[10], code[11]);
-            }
-        }
-    }
-    if (!in_img) return;
     ptx::st_global_32B(dst, wv);                       // 64 bytes per pixel = two full 32-byte sectors
     ptx::st_global_32B(dst + 16, wv + 8);
 }
@@ -200,7 +145,7 @@ __device__ __forceinline__ void conv_tile_epilogue(const ConvGemmParams& p, cons
                     make_float2(acc[4 * (8 * pass + j) + 2 * i], acc[4 * (8 * pass + j) + 2 * i + 1]);
         ptx::bar_sync(1 + cg, 128);
         const int half = t >> 6;
-        if (64 * pass + 32 * half < NT) {               // whole warps take part (the pool shuffles)
+        if (64 * pass + 32 * half < NT) {
             float v[32];
             const float4* src = reinterpret_cast<const float4*>(stg + (t & 63) * kConvStg + 32 * half);
 #pragma unroll

@@ -21,12 +21,13 @@ using WgradKernel = void (*)(CUtensorMap, CUtensorMap, WgradParams);
 using WgradThinKernel = void (*)(CUtensorMap, CUtensorMap, WgradThinParams);
 using FirstConvKernel = void (*)(CUtensorMap, CUtensorMap, FirstConvParams);
 static const ConvKernel kConvGemm[3] = { conv_gemm_kernel<32>, conv_gemm_kernel<64>, conv_gemm_kernel<128> };
+// the 3x3 halo tiles: the input, `out`, `out2` and the slope-word mask as tensor maps
 using ConvThinKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, ConvGemmParams);
 static const ConvThinKernel kConvThin[2][2] = { { conv3x3_thin_kernel<32, 32>, conv3x3_thin_kernel<32, 64> },
                                                 { conv3x3_thin_kernel<64, 32>, conv3x3_thin_kernel<64, 64> } };
-static const ConvKernel kConvWide[3][2] = { { conv3x3_wide_kernel<32, 32>, conv3x3_wide_kernel<32, 64> },
-                                            { conv3x3_wide_kernel<64, 32>, conv3x3_wide_kernel<64, 64> },
-                                            { conv3x3_wide_kernel<128, 32>, conv3x3_wide_kernel<128, 64> } };
+static const ConvThinKernel kConvWide[3][2] = { { conv3x3_wide_kernel<32, 32>, conv3x3_wide_kernel<32, 64> },
+                                                { conv3x3_wide_kernel<64, 32>, conv3x3_wide_kernel<64, 64> },
+                                                { conv3x3_wide_kernel<128, 32>, conv3x3_wide_kernel<128, 64> } };
 static const WgradKernel kWgradGemm[3] = { wgrad_gemm_kernel<32>, wgrad_gemm_kernel<64>, wgrad_gemm_kernel<128> };
 static const WgradThinKernel kWgradThin[2][2] = { { conv3x3_wgrad_thin_kernel<32, 32>, conv3x3_wgrad_thin_kernel<32, 64> },
                                                   { conv3x3_wgrad_thin_kernel<64, 32>, conv3x3_wgrad_thin_kernel<64, 64> } };
@@ -162,7 +163,15 @@ static int launch_conv3x3(eld_ctx* ctx, const GemmOp& op, ConvGemmParams& p, cud
     { int rc = encode_nhwc(ctx, &tmA, op.a, op.a_pitch, op.n_img, op.H, op.W, p.kc, kConvTileW, kHaloRows); if (rc) return rc; }
     const int rb = p.kc * 2;
     const int slot_bytes = halo_slot_bytes(p.kc);
-    if ((op.cin == 32 || op.cin == 64) && (p.n_total == 32 || p.n_total == 64)) {
+    const bool thin = (op.cin == 32 || op.cin == 64) && (p.n_total == 32 || p.n_total == 64);
+    // the epilogue's TMA stores: 32 channels x 16 pixels x 8 rows per box (thin) or 4 rows, one 64-pixel half of a
+    // tile (wide), clipped at the image border
+    const int out_rows = thin ? 8 : 4;
+    CUtensorMap tmOut, tmOut2;
+    { int rc = encode_nhwc(ctx, &tmOut, op.out, op.out_pitch, op.n_img, op.H, op.W, 32, kConvTileW, out_rows); if (rc) return rc; }
+    tmOut2 = tmOut;
+    if (op.out_split) { int rc = encode_nhwc(ctx, &tmOut2, op.out2, op.out2_pitch, op.n_img, op.H, op.W, 32, kConvTileW, out_rows); if (rc) return rc; }
+    if (thin) {
         // [resident weights][halo slots][slope-word boxes][staging of the consumer warpgroups][bias][barriers] after
         // the 1024-byte alignment; every part a multiple of 1 KB, so each staging block sits on its 64-byte swizzle's
         // 512-byte period
@@ -177,11 +186,6 @@ static int launch_conv3x3(eld_ctx* ctx, const GemmOp& op, ConvGemmParams& p, cud
         p.bias_smem_off = p.stg_smem_off + cg * stg;
         p.bar_smem_off = p.bias_smem_off + 256;
         const size_t smem = 1024 + (size_t)p.bar_smem_off + 256;
-        // the epilogue's TMA stores: 32 channels x 16 x 8 pixels per box, clipped at the image border
-        CUtensorMap tmOut, tmOut2;
-        { int rc = encode_nhwc(ctx, &tmOut, op.out, op.out_pitch, op.n_img, op.H, op.W, 32, kConvTileW, 8); if (rc) return rc; }
-        tmOut2 = tmOut;
-        if (op.out_split) { int rc = encode_nhwc(ctx, &tmOut2, op.out2, op.out2_pitch, op.n_img, op.H, op.W, 32, kConvTileW, 8); if (rc) return rc; }
         // the slope words loaded with the halo: the two planes [n H][W nc] as (word, row, plane), boxes of one tile's
         // {16 nc, 8} words of both, unswizzled.  Images share the row dimension, so the tiles must be whole.
         CUtensorMap tmSlope = tmA;
@@ -200,22 +204,50 @@ static int launch_conv3x3(eld_ctx* ctx, const GemmOp& op, ConvGemmParams& p, cud
         return launch(ctx, kConvThin[p.n_tile / 64][p.kc / 64], std::min(total_tiles, ctx->num_sms),
                       kThinThreads, smem, st, tmA, tmOut, tmOut2, tmSlope, p);
     }
-    // [halo slots][weight ring][staging of both consumer warpgroups][bias][barriers] after the 1024-byte alignment;
-    // the weight ring takes what the opt-in maximum leaves
-    const int stg_bytes = 2 * 64 * kConvStg * 4;
+    // [halo slots][slope-word boxes][weight ring][staging of the consumer warpgroups][bias][barriers] after the
+    // 1024-byte alignment; every part but the last two a multiple of 1 KB, so each staging block sits on its 64-byte
+    // swizzle's 512-byte period.  The weight ring takes what the opt-in maximum leaves.
+    const int nc = p.n_tile / 32, n_blocks = p.n_total / p.n_tile;
+    const bool slope_box = op.act == ACT_MASK && op.aux_slope;
+    const int slope_bytes = slope_box ? kWideHaloSlots * thin_slope_bytes(p.n_tile) : 0;
+    const int stg = kWideConsumers * wide_stg_bytes(p.n_tile, p.kc);
+    const int bias_bytes = op.bias ? (p.n_total * 4 + 255) & ~255 : 0;
     const int b_bytes = p.n_tile * rb;
-    const int fixed = kWideHaloSlots * slot_bytes + stg_bytes + 4096;
-    int wstages = (kThinSmemBytes - 1024 - 256 - fixed) / b_bytes;
-    if (wstages > 8) wstages = 8;
+    const int fixed = kWideHaloSlots * slot_bytes + slope_bytes + stg + bias_bytes + 256;
+    int wstages = (kThinSmemBytes - 1024 - fixed) / b_bytes;
+    if (wstages > kWideMaxStages) wstages = kWideMaxStages;
     ELD_REQUIRE(wstages >= 2, "wide conv tile: no room for two weight stages");
     p.stages = wstages;
-    p.stg_smem_off = kWideHaloSlots * slot_bytes + wstages * b_bytes;
-    p.bias_smem_off = p.stg_smem_off + stg_bytes;
-    p.bar_smem_off = p.bias_smem_off + 4096;
+    p.stg_smem_off = kWideHaloSlots * slot_bytes + slope_bytes + wstages * b_bytes;
+    p.bias_smem_off = p.stg_smem_off + stg;
+    p.bar_smem_off = p.bias_smem_off + bias_bytes;
     const size_t smem = 1024 + (size_t)p.bar_smem_off + 256;
-    const int total_tiles = op.n_img * p.tiles_x * p.tiles_y * (p.n_total / p.n_tile);
-    return launch(ctx, kConvWide[p.n_tile / 64][p.kc / 64], std::min(total_tiles, ctx->num_sms), kConvThreads, smem, st,
-                  tmA, p);
+    // the slope words loaded with the halo of a tile's first chunk: the two planes [n H][W][n_total / 32] as (word,
+    // x, row, plane), unswizzled boxes of one tile's {nc, 16, 8} words of both.  With one N block a pixel row's words
+    // are contiguous, so the box is {16 nc, 1, 8, 2} of (word, -, row, plane); with several, nc = 4 words (16 bytes, the
+    // least TMA box row) per pixel.  Images share the row dimension, so the tiles must be whole.
+    CUtensorMap tmSlope = tmA;
+    if (slope_box) {
+        const int nw = p.n_total / 32;
+        ELD_REQUIRE(op.H % 8 == 0 && op.W % kConvTileW == 0 && (reinterpret_cast<uintptr_t>(op.aux_slope) & 15) == 0,
+                    "wide conv tile: a slope-word mask needs whole 8 x 16 tiles (H=%d, W=%d) and 16-byte aligned words",
+                    op.H, op.W);
+        ELD_REQUIRE(n_blocks == 1 || nc == 4,
+                    "wide conv tile: a slope-word mask over several N blocks needs 128-column blocks (N=%d)", p.n_total);
+        const cuuint64_t rows = (cuuint64_t)op.n_img * op.H, plane = rows * op.W * nw * 4;
+        const cuuint64_t dims1[4] = { (cuuint64_t)op.W * nw, 1, rows, 2 };
+        const cuuint64_t str1[3] = { (cuuint64_t)op.W * nw * 4, (cuuint64_t)op.W * nw * 4, plane };
+        const cuuint32_t box1[4] = { (cuuint32_t)(kConvTileW * nc), 1, 8, 2 };
+        const cuuint64_t dims[4] = { (cuuint64_t)nw, (cuuint64_t)op.W, rows, 2 };
+        const cuuint64_t str[3] = { (cuuint64_t)nw * 4, (cuuint64_t)op.W * nw * 4, plane };
+        const cuuint32_t box[4] = { (cuuint32_t)nc, (cuuint32_t)kConvTileW, 8, 2 };
+        int rc = n_blocks == 1 ? encode(ctx, &tmSlope, op.aux_slope, 4, dims1, str1, box1, 0, CU_TENSOR_MAP_DATA_TYPE_UINT32)
+                               : encode(ctx, &tmSlope, op.aux_slope, 4, dims, str, box, 0, CU_TENSOR_MAP_DATA_TYPE_UINT32);
+        if (rc) return rc;
+    }
+    const int total_tiles = op.n_img * p.tiles_x * p.tiles_y * n_blocks;
+    return launch(ctx, kConvWide[p.n_tile / 64][p.kc / 64], std::min(total_tiles, ctx->num_sms), kWideThreads, smem, st,
+                  tmA, tmOut, tmOut2, tmSlope, p);
 }
 
 // the deconv fprop (one {kc, 16, 8} box of the coarse tile) and the deconv dgrad (the sub-pixel gather of the fine
@@ -226,6 +258,9 @@ static int launch_deconv(eld_ctx* ctx, const GemmOp& op, ConvGemmParams& p, cuda
     // merges (image, row) into one tensor-map dimension and therefore needs whole 8-row tiles
     ELD_REQUIRE(op.kind == GEMM_DECONV || (op.H % 8 == 0 && op.W % 16 == 0),
                 "deconv dgrad tile: H=%d must be a multiple of 8 and W=%d of 16", op.H, op.W);
+    // its epilogue (conv_gemm.cuh conv_epilogue32) applies bias and the LeakyReLU' mask only
+    ELD_REQUIRE(op.act != ACT_LRELU && !op.pool_out && !op.slope_out && !op.out_split,
+                "deconv tile: no LeakyReLU, fused pool, slope-word output or split store");
     CUtensorMap tmA;
     { int rc = op.kind == GEMM_DECONV ? encode_nhwc(ctx, &tmA, op.a, op.a_pitch, op.n_img, op.H, op.W, p.kc, 16, 8)
                                       : encode_subpixel(ctx, &tmA, op.a, op.a_pitch, op.n_img, op.H, op.W, p.kc, 8);
