@@ -4,6 +4,18 @@ import ctypes as c
 vp, i32 = c.c_void_p, c.c_int
 
 
+class AdamRange(c.Structure):
+    """eld_adam_range"""
+    _fields_ = [('offset', c.c_size_t), ('count', c.c_size_t), ('step', i32), ('lr', c.c_float), ('beta1', c.c_float),
+                ('beta2', c.c_float), ('eps', c.c_float), ('weight_decay', c.c_float)]
+
+
+class AdamRangeDev(c.Structure):
+    """eld_adam_range_dev (step: device int*, lr: device float*)"""
+    _fields_ = [('offset', c.c_size_t), ('count', c.c_size_t), ('step', vp), ('lr', vp), ('beta1', c.c_float),
+                ('beta2', c.c_float), ('eps', c.c_float), ('weight_decay', c.c_float)]
+
+
 def declare(lib):
     lib.eld_pack_weights.argtypes = [vp, vp, vp, i32, i32, i32, vp]
     lib.eld_conv3x3_bf16.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32,
@@ -48,6 +60,8 @@ def declare_engine(lib):
     lib.eld_adam_step_capturable.argtypes = [vp, vp, vp, vp, vp, sz, vp, vp, f32, f32, f32, f32, f32, vp]
     lib.eld_adam_step_segments_capturable.argtypes = [vp, vp, vp, vp, vp, c.POINTER(sz), c.POINTER(vp), i32, vp, f32, f32,
                                                       f32, f32, f32, vp]
+    lib.eld_adam_step_ranges.argtypes = [vp, vp, vp, vp, vp, c.POINTER(AdamRange), i32, f32, vp]
+    lib.eld_adam_step_ranges_capturable.argtypes = [vp, vp, vp, vp, vp, c.POINTER(AdamRangeDev), i32, f32, vp]
     lib.eld_unet_set_loss.argtypes = [vp, i32]
     lib.eld_unet_set_accumulate.argtypes = [vp, i32]
     lib.eld_clock_probe.argtypes = [vp, vp, vp]

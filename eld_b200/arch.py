@@ -13,7 +13,7 @@ import weakref
 import torch
 import torch.nn as nn
 
-from . import _lib
+from . import _lib, _unet_abi
 
 _SPEC = [('conv1_1', 'c', 4, 32), ('conv1_2', 'c', 32, 32), ('conv2_1', 'c', 32, 64), ('conv2_2', 'c', 64, 64),
          ('conv3_1', 'c', 64, 128), ('conv3_2', 'c', 128, 128), ('conv4_1', 'c', 128, 256), ('conv4_2', 'c', 256, 256),
@@ -444,25 +444,68 @@ class FusedAdam(torch.optim.Optimizer):
     Keeps `param_groups` so Engine.set_learning_rate / util.set_opt_param keep working.  Frozen parameters
     (requires_grad == False) are skipped: the trainable runs of the buffer go to eld_adam_step_segments, each with the
     per-parameter step count torch keeps in state['step'].
-    capturable=True (torch.optim.Adam's option of that name): the step counts and the learning rate live in device memory
-    and the kernels read them when they run (eld_adam_step_segments_capturable), so a CUDA graph that captured step()
-    stays right on every replay.  Before each replay, graph_step() does the host half of a step: param_groups[0]['lr']
-    into device memory (outside the graph) and the parameters' version bump."""
+    param_groups: what torch.optim.Adam's first argument takes - parameters of `net`, or dicts {'params': ..., and any
+    of 'lr', 'betas', 'eps', 'weight_decay'} whose missing keys take the defaults given here; None is one group over
+    every parameter.  A parameter of `net` in no group is never stepped (its moments and step count stay zero).  With
+    two or more hyperparameter sets in use, or a parameter in no group, the step goes to eld_adam_step_ranges: still
+    one launch, each range with its group's hyperparameters.
+    capturable=True (torch.optim.Adam's option of that name): the step counts and the learning rates (lr_dev, one per
+    group) live in device memory and the kernels read them when they run (eld_adam_step_segments_capturable /
+    eld_adam_step_ranges_capturable), so a CUDA graph that captured step() stays right on every replay.  Before each
+    replay, graph_step() does the host half of a step: each group's 'lr' into device memory (outside the graph) and
+    the parameters' version bump."""
 
-    def __init__(self, net, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, capturable=False):
-        super().__init__(list(net.parameters()), dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
+    def __init__(self, net, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, capturable=False,
+                 param_groups=None):
         self.net = net
+        self.capturable = capturable
+        self._index = {id(q): i for i, q in enumerate(net.parameters())}     # a parameter's place in the flat buffer
+        super().__init__(list(net.parameters()) if param_groups is None else param_groups,
+                         dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
         self.m = torch.zeros_like(net.flat_params)
         self.v = torch.zeros_like(net.flat_params)
         self.t = 0                                     # step() calls
-        self.capturable = capturable
         if capturable:
             dev = net.flat_params.device
             self.step_dev = torch.zeros(len(net._spans), dtype=torch.int32, device=dev)   # state['step'] per parameter
-            self.lr_dev = torch.zeros(1, dtype=torch.float32, device=dev)
-            self._lr_sent = None                       # the lr last written to lr_dev
+            self.lr_dev = torch.zeros(len(self.param_groups), dtype=torch.float32, device=dev)
+            self._lr_sent = [None] * len(self.param_groups)    # the lr last written to each element of lr_dev
         else:
             self.steps = [0] * len(net._spans)         # Adam steps taken by each parameter (torch's state['step'])
+
+    def add_param_group(self, param_group):
+        """torch's add_param_group, and every parameter must be one of net's, in one group at most (ValueError).  A
+        capturable optimizer gets a new lr_dev: capture after adding groups."""
+        super().add_param_group(param_group)
+        params = self.param_groups[-1]['params']
+        if any(id(q) not in self._index for q in params) or len({id(q) for q in params}) != len(params):
+            self.param_groups.pop()
+            raise ValueError('FusedAdam: a parameter group holds a parameter that is not one of net\'s, or holds one '
+                             'twice')
+        if hasattr(self, 'lr_dev'):
+            self.lr_dev = torch.cat([self.lr_dev, self.lr_dev.new_zeros(1)])
+            self._lr_sent.append(None)
+
+    def _owners(self):
+        """the group of each parameter, in state_dict order (None: in no group)"""
+        owner = [None] * len(self._index)
+        for k, group in enumerate(self.param_groups):
+            for q in group['params']:
+                owner[self._index[id(q)]] = k
+        return owner
+
+    def _stepped(self, owner):
+        """which parameters this step updates: the trainable ones that are in a group"""
+        return [q.requires_grad and o is not None for q, o in zip(self.net.parameters(), owner)]
+
+    def capture_key(self):
+        """what a captured step() bakes in besides the device values it reads: the buffers, each parameter's group and
+        whether it is stepped, and every group's betas, eps and weight decay"""
+        owner = self._owners()
+        return (id(self), self.m.data_ptr(), self.v.data_ptr(), self.lr_dev.data_ptr() if self.capturable else None,
+                tuple(owner), tuple(self._stepped(owner)),
+                tuple((tuple(float(b) for b in g['betas']), float(g['eps']), float(g['weight_decay']))
+                      for g in self.param_groups))
 
     def _params_stepped(self, flags):
         # the kernels write the flat buffer behind autograd's back: mark the parameters modified in place, so that a
@@ -470,35 +513,35 @@ class FusedAdam(torch.optim.Optimizer):
         torch.autograd.graph.increment_version([q for q, f in zip(self.net.parameters(), flags) if f])
 
     def _send_lr(self):
-        """param_groups[0]['lr'] into lr_dev (a fill launch, no host synchronisation) when it changed"""
-        lr = float(self.param_groups[0]['lr'])
-        if lr != self._lr_sent:
-            self.lr_dev.fill_(lr)
-            self._lr_sent = lr
+        """each group's 'lr' into its element of lr_dev (a fill launch, no host synchronisation) when it changed"""
+        for k, group in enumerate(self.param_groups):
+            lr = float(group['lr'])
+            if lr != self._lr_sent[k]:
+                self.lr_dev[k].fill_(lr)
+                self._lr_sent[k] = lr
 
     def graph_step(self):
-        """the host half of a capturable step whose kernels a CUDA graph replays: the learning rate into device memory
+        """the host half of a capturable step whose kernels a CUDA graph replays: the learning rates into device memory
         (call it before the replay), the parameter versions bumped"""
         assert self.capturable
         self.t += 1
         self._send_lr()
-        self._params_stepped([q.requires_grad for q in self.net.parameters()])
+        self._params_stepped(self._stepped(self._owners()))
 
     def host_steps(self):
-        """Adam steps taken by each parameter, in state_dict order (reads the device counters when capturable)"""
+        """Adam steps taken by each parameter, in net.parameters() order (reads the device counters when capturable)"""
         return [int(s) for s in self.step_dev.tolist()] if self.capturable else list(self.steps)
 
     @torch.no_grad()
     def step(self, closure=None, grad_scale=1.0):
-        """One Adam step on every parameter that requires grad; a frozen parameter, its moments and its step count stay
-        as they are (torch.optim.Adam skips a parameter whose .grad is None)."""
-        g = self.param_groups[0]
+        """One Adam step on every parameter that requires grad and is in a group; a frozen parameter, its moments and
+        its step count stay as they are (torch.optim.Adam skips a parameter whose .grad is None)."""
         if self.m.data_ptr() == 0 or self.m.device != self.net.flat_params.device:
             self.m = torch.zeros_like(self.net.flat_params)
             self.v = torch.zeros_like(self.net.flat_params)
         self.t += 1
-        params = list(self.net.parameters())
-        flags = [q.requires_grad for q in params]
+        owner = self._owners()
+        flags = self._stepped(owner)
         if self.capturable:
             if not torch.cuda.is_current_stream_capturing():
                 self._send_lr()                        # a capture reads lr_dev as graph_step leaves it before each replay
@@ -506,48 +549,68 @@ class FusedAdam(torch.optim.Optimizer):
             for i, f in enumerate(flags):
                 self.steps[i] += 1 if f else 0
         self._params_stepped(flags)
-        uniform = not self.capturable and all(flags) and len(set(self.steps)) == 1
+        hps = [(float(g['lr']), float(g['betas'][0]), float(g['betas'][1]), float(g['eps']), float(g['weight_decay']))
+               for g in self.param_groups]
+        live = sorted({o for o, f in zip(owner, flags) if f})
+        # one hyperparameter set (a captured step: one group, whose lr may change between replays) over every
+        # parameter: the single-group entry points, as without groups
+        if None in owner or (len(live) > 1 if self.capturable else len({hps[k] for k in live}) > 1):
+            single = None
+        else:
+            single = live[0] if live else 0
+        uniform = not self.capturable and single is not None and all(flags) and len(set(self.steps)) == 1
         p = self.net.flat_params
-        hp = (float(g['lr']), float(g['betas'][0]), float(g['betas'][1]), float(g['eps']), float(g['weight_decay']))
 
         def adam(lo, hi):
             lib, dev = _lib.load(), _lib.ctx(p.device.index or 0)
+            bufs = (dev, p.data_ptr(), self.net.flat_grads.data_ptr(), self.m.data_ptr(), self.v.data_ptr())
             if self.capturable:                        # one range per trainable parameter, each with its own counter
-                segs, ctrs = [], []
+                mine = []
                 for i, ((off, n), f) in enumerate(zip(self.net._spans, flags)):
                     if f and lo <= off and off + n <= hi:
-                        segs += [off, n]
-                        ctrs.append(self.step_dev.data_ptr() + 4 * i)
+                        mine.append(i)
                     assert not (f and lo < off + n and off < hi and not (lo <= off and off + n <= hi)), \
                         'a capturable step range must hold whole parameters'
-                k = len(ctrs)
-                _lib.check(lib.eld_adam_step_segments_capturable(
-                    dev, p.data_ptr(), self.net.flat_grads.data_ptr(), self.m.data_ptr(), self.v.data_ptr(),
-                    (ctypes.c_size_t * (2 * k))(*segs), (ctypes.c_void_p * k)(*ctrs), k, self.lr_dev.data_ptr(), *hp[1:],
-                    float(grad_scale), _st()), 'eld_adam_step_segments_capturable')
+                k = len(mine)
+                ctrs = [self.step_dev.data_ptr() + 4 * i for i in mine]
+                if single is not None:
+                    segs = [x for i in mine for x in self.net._spans[i]]
+                    _lib.check(lib.eld_adam_step_segments_capturable(
+                        *bufs, (ctypes.c_size_t * (2 * k))(*segs), (ctypes.c_void_p * k)(*ctrs), k,
+                        self.lr_dev.data_ptr() + 4 * single, *hps[single][1:], float(grad_scale), _st()),
+                        'eld_adam_step_segments_capturable')
+                    return
+                rates = self.lr_dev.data_ptr()
+                table = (_unet_abi.AdamRangeDev * k)(*[_unet_abi.AdamRangeDev(
+                    *self.net._spans[i], c, rates + 4 * owner[i], *hps[owner[i]][1:]) for i, c in zip(mine, ctrs)])
+                _lib.check(lib.eld_adam_step_ranges_capturable(*bufs, table, k, float(grad_scale), _st()),
+                           'eld_adam_step_ranges_capturable')
                 return
             if uniform:                                # one range, one step count
                 _lib.check(lib.eld_adam_step(dev, p.data_ptr() + 4 * lo, self.net.flat_grads.data_ptr() + 4 * lo,
-                                             self.m.data_ptr() + 4 * lo, self.v.data_ptr() + 4 * lo, hi - lo, *hp,
-                                             self.steps[0], float(grad_scale), _st()), 'eld_adam_step')
+                                             self.m.data_ptr() + 4 * lo, self.v.data_ptr() + 4 * lo, hi - lo,
+                                             *hps[single], self.steps[0], float(grad_scale), _st()), 'eld_adam_step')
                 return
-            segs = []                                  # trainable runs inside [lo, hi), merged while the step count agrees
-            for (off, n), f, s in zip(self.net._spans, flags, self.steps):
+            segs = []                                  # trainable runs inside [lo, hi), merged while step and group agree
+            for (off, n), f, s, o in zip(self.net._spans, flags, self.steps, owner):
                 a, b = max(off, lo), min(off + n, hi)
                 if not f or a >= b:
                     continue
-                if segs and segs[-1][2] == s and segs[-1][0] + segs[-1][1] == a:
+                if segs and segs[-1][2] == s and segs[-1][3] == o and segs[-1][0] + segs[-1][1] == a:
                     segs[-1][1] += b - a
                 else:
-                    segs.append([a, b - a, s])
+                    segs.append([a, b - a, s, o])
             if not segs:
                 return
             k = len(segs)
-            table = (ctypes.c_size_t * (2 * k))(*[x for a, c, _ in segs for x in (a, c)])
-            steps = (ctypes.c_int * k)(*[s for _, _, s in segs])
-            _lib.check(lib.eld_adam_step_segments(dev, p.data_ptr(), self.net.flat_grads.data_ptr(), self.m.data_ptr(),
-                                                  self.v.data_ptr(), table, steps, k, *hp, float(grad_scale), _st()),
-                       'eld_adam_step_segments')
+            if single is not None:
+                table = (ctypes.c_size_t * (2 * k))(*[x for a, c, _, _ in segs for x in (a, c)])
+                steps = (ctypes.c_int * k)(*[s for _, _, s, _ in segs])
+                _lib.check(lib.eld_adam_step_segments(*bufs, table, steps, k, *hps[single], float(grad_scale), _st()),
+                           'eld_adam_step_segments')
+                return
+            table = (_unet_abi.AdamRange * k)(*[_unet_abi.AdamRange(a, c, s, *hps[o]) for a, c, s, o in segs])
+            _lib.check(lib.eld_adam_step_ranges(*bufs, table, k, float(grad_scale), _st()), 'eld_adam_step_ranges')
         pend = getattr(self.net, '_pending_allreduce', None)
         if pend:
             # data parallel: buckets arrive in backward-completion order and tile the buffer from its end towards its start;
@@ -568,41 +631,60 @@ class FusedAdam(torch.optim.Optimizer):
         self.net.join_allreduce()
         self.net.flat_grads.zero_()
 
-    # checkpoint format of torch.optim.Adam ('opt_g' in ELD_model.py:516-523): per-parameter step; a parameter that has
-    # never taken a step has no state entry.  Capturable: 'step' is a float32 tensor on the parameter's device, as torch's
-    # capturable Adam stores it.
+    # checkpoint format of torch.optim.Adam ('opt_g' in ELD_model.py:516-523): parameters numbered group by group, in
+    # group order; per-parameter step; a parameter that has never taken a step has no state entry.  Capturable: 'step' is
+    # a float32 tensor on the parameter's device, as torch's capturable Adam stores it.
     def state_dict(self):
-        state = {}
-        params = list(self.net.parameters())
-        for i, (p, (off, n), s) in enumerate(zip(params, self.net._spans, self.host_steps())):
-            if s == 0:
-                continue
-            step = torch.tensor(float(s), device=p.device) if self.capturable else torch.tensor(float(s))
-            state[i] = {'step': step, 'exp_avg': self.m[off:off + n].view(p.shape).clone(),
-                        'exp_avg_sq': self.v[off:off + n].view(p.shape).clone()}
-        groups = [dict((k, v) for k, v in self.param_groups[0].items() if k != 'params')]
-        groups[0]['params'] = list(range(len(params)))
+        state, groups = {}, []
+        steps, spans, i = self.host_steps(), self.net._spans, 0
+        for group in self.param_groups:
+            ids = []
+            for q in group['params']:
+                j = self._index[id(q)]
+                off, n = spans[j]
+                if steps[j]:
+                    s = float(steps[j])
+                    state[i] = {'step': torch.tensor(s, device=q.device) if self.capturable else torch.tensor(s),
+                                'exp_avg': self.m[off:off + n].view(q.shape).clone(),
+                                'exp_avg_sq': self.v[off:off + n].view(q.shape).clone()}
+                ids.append(i)
+                i += 1
+            groups.append(dict((k, v) for k, v in group.items() if k != 'params'))
+            groups[-1]['params'] = ids
         return {'state': state, 'param_groups': groups}
 
     def load_state_dict(self, sd):
+        """torch.optim.Adam's load_state_dict: the saved groups must match this optimizer's in number and size
+        (ValueError); saved parameter k of the saved numbering is this optimizer's parameter k of its own"""
+        saved = sd['param_groups']
+        if len(saved) != len(self.param_groups):
+            raise ValueError('loaded state dict has %d parameter groups, the optimizer %d' % (
+                len(saved), len(self.param_groups)))
+        if any(len(a['params']) != len(b['params']) for a, b in zip(saved, self.param_groups)):
+            raise ValueError("loaded state dict contains a parameter group that doesn't match the size of optimizer's "
+                             "group")
         steps = [0] * len(self.net._spans)
-        for i, (off, n) in enumerate(self.net._spans):
-            st = sd['state'].get(i)
-            if st is not None:
+        self.m.zero_()
+        self.v.zero_()
+        for a, b in zip(saved, self.param_groups):
+            for key, q in zip(a['params'], b['params']):
+                st = sd['state'].get(key)
+                if st is None:
+                    continue
+                j = self._index[id(q)]
+                off, n = self.net._spans[j]
                 self.m[off:off + n].copy_(st['exp_avg'].reshape(-1))
                 self.v[off:off + n].copy_(st['exp_avg_sq'].reshape(-1))
-                steps[i] = int(float(st['step']))
-            else:
-                self.m[off:off + n].zero_()
-                self.v[off:off + n].zero_()
+                steps[j] = int(float(st['step']))
         if self.capturable:
             self.step_dev.copy_(torch.tensor(steps, dtype=torch.int32))      # in place: a captured step keeps its address
         else:
             self.steps[:] = steps
-        self.t = max(steps)
-        for k, v in sd['param_groups'][0].items():
-            if k != 'params':
-                self.param_groups[0][k] = v
+        self.t = max(steps, default=0)
+        for a, b in zip(saved, self.param_groups):
+            for k, v in a.items():
+                if k != 'params':
+                    b[k] = v
 
 
 def unet(in_channels, out_channels, **kwargs):

@@ -9,6 +9,8 @@
 #include "unet_prims.h"
 #include "unet_ew.h"
 #include <cuda_bf16.h>
+#include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <vector>
 #include <new>
@@ -892,7 +894,42 @@ extern "C" int eld_adam_step_segments(eld_ctx* ctx, float* params, const float* 
 {
     ELD_REQUIRE(ctx && params && grads && m && v && (n_segs == 0 || (segs && steps)), "eld_adam_step_segments: NULL argument");
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
-    return launch_adam_segments(ctx, params, grads, m, v, segs, steps, n_segs, lr, beta1, beta2, eps, weight_decay, grad_scale,
+    AdamHyper hyper[kAdamMaxSegments];                  // every range takes the one set (n_segs > 64 is refused below)
+    std::fill(hyper, hyper + kAdamMaxSegments, AdamHyper{ lr, beta1, beta2, eps, weight_decay });
+    return launch_adam_segments(ctx, params, grads, m, v, segs, steps, hyper, n_segs, grad_scale,
+                                static_cast<cudaStream_t>(stream));
+}
+
+// a range's hyperparameters as eld_adam_step_ranges(_capturable) accept them (lr only where it is on the host)
+static int check_adam_hyper(const char* fn, int s, const float* lr, float beta1, float beta2, float eps, float wd)
+{
+    ELD_REQUIRE(!lr || (std::isfinite(*lr) && *lr >= 0.f), "%s: range %d: lr %g is not a finite number >= 0", fn, s,
+                lr ? (double)*lr : 0.0);
+    ELD_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f, "%s: range %d: betas (%g, %g) outside [0, 1)",
+                fn, s, (double)beta1, (double)beta2);
+    ELD_REQUIRE(std::isfinite(eps) && eps >= 0.f, "%s: range %d: eps %g is not a finite number >= 0", fn, s, (double)eps);
+    ELD_REQUIRE(std::isfinite(wd) && wd >= 0.f, "%s: range %d: weight_decay %g is not a finite number >= 0", fn, s,
+                (double)wd);
+    return ELD_OK;
+}
+
+extern "C" int eld_adam_step_ranges(eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
+                                    const eld_adam_range* ranges, int n_ranges, float grad_scale, void* stream)
+{
+    ELD_REQUIRE(ctx && params && grads && m && v && (n_ranges <= 0 || ranges), "eld_adam_step_ranges: NULL argument");
+    size_t segs[2 * kAdamMaxSegments];
+    int steps[kAdamMaxSegments];
+    AdamHyper hyper[kAdamMaxSegments];
+    const int k = n_ranges < kAdamMaxSegments ? n_ranges : kAdamMaxSegments;     // more than 64 is refused below
+    for (int s = 0; s < k; ++s) {
+        const eld_adam_range& r = ranges[s];
+        const int rc = check_adam_hyper("eld_adam_step_ranges", s, &r.lr, r.beta1, r.beta2, r.eps, r.weight_decay);
+        if (rc != ELD_OK) return rc;
+        segs[2 * s] = r.offset; segs[2 * s + 1] = r.count; steps[s] = r.step;
+        hyper[s] = AdamHyper{ r.lr, r.beta1, r.beta2, r.eps, r.weight_decay };
+    }
+    ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
+    return launch_adam_segments(ctx, params, grads, m, v, segs, steps, hyper, n_ranges, grad_scale,
                                 static_cast<cudaStream_t>(stream));
 }
 
@@ -903,8 +940,8 @@ extern "C" int eld_adam_step_capturable(eld_ctx* ctx, float* params, const float
     ELD_REQUIRE(ctx && params && grads && m && v && lr && step, "eld_adam_step_capturable: NULL argument");
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     const size_t seg[2] = { 0, n };
-    return launch_adam_dev(ctx, params, grads, m, v, seg, &step, 1, lr, beta1, beta2, eps, weight_decay, grad_scale,
-                           static_cast<cudaStream_t>(stream));
+    const AdamHyper hyper{ 0.f, beta1, beta2, eps, weight_decay };
+    return launch_adam_dev(ctx, params, grads, m, v, seg, &step, &lr, &hyper, 1, grad_scale, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int eld_adam_step_segments_capturable(eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
@@ -915,7 +952,35 @@ extern "C" int eld_adam_step_segments_capturable(eld_ctx* ctx, float* params, co
     ELD_REQUIRE(ctx && params && grads && m && v && lr && (n_segs == 0 || (segs && steps)),
                 "eld_adam_step_segments_capturable: NULL argument");
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
-    return launch_adam_dev(ctx, params, grads, m, v, segs, steps, n_segs, lr, beta1, beta2, eps, weight_decay, grad_scale,
+    const float* rates[kAdamMaxSegments];               // every range takes the one set (n_segs > 64 is refused below)
+    AdamHyper hyper[kAdamMaxSegments];
+    std::fill(rates, rates + kAdamMaxSegments, lr);
+    std::fill(hyper, hyper + kAdamMaxSegments, AdamHyper{ 0.f, beta1, beta2, eps, weight_decay });
+    return launch_adam_dev(ctx, params, grads, m, v, segs, steps, rates, hyper, n_segs, grad_scale,
+                           static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int eld_adam_step_ranges_capturable(eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
+                                               const eld_adam_range_dev* ranges, int n_ranges, float grad_scale,
+                                               void* stream)
+{
+    ELD_REQUIRE(ctx && params && grads && m && v && (n_ranges <= 0 || ranges),
+                "eld_adam_step_ranges_capturable: NULL argument");
+    size_t segs[2 * kAdamMaxSegments];
+    int* steps[kAdamMaxSegments];
+    const float* rates[kAdamMaxSegments];
+    AdamHyper hyper[kAdamMaxSegments];
+    const int k = n_ranges < kAdamMaxSegments ? n_ranges : kAdamMaxSegments;     // more than 64 is refused below
+    for (int s = 0; s < k; ++s) {
+        const eld_adam_range_dev& r = ranges[s];
+        const int rc = check_adam_hyper("eld_adam_step_ranges_capturable", s, nullptr, r.beta1, r.beta2, r.eps,
+                                        r.weight_decay);
+        if (rc != ELD_OK) return rc;
+        segs[2 * s] = r.offset; segs[2 * s + 1] = r.count; steps[s] = r.step; rates[s] = r.lr;
+        hyper[s] = AdamHyper{ 0.f, r.beta1, r.beta2, r.eps, r.weight_decay };
+    }
+    ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
+    return launch_adam_dev(ctx, params, grads, m, v, segs, steps, rates, hyper, n_ranges, grad_scale,
                            static_cast<cudaStream_t>(stream));
 }
 

@@ -311,41 +311,46 @@ adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restric
 }
 
 // The same update on a list of (offset, count) ranges, each with its own step count (torch.optim.Adam keeps
-// state['step'] per parameter: a tensor that was frozen for a while has taken fewer steps than its neighbours).
-// Every segment is walked by the whole grid; the table travels in the kernel parameters.
+// state['step'] per parameter: a tensor that was frozen for a while has taken fewer steps than its neighbours) and its
+// own hyperparameters (its parameter group's).  Every segment is walked by the whole grid; the table travels in the
+// kernel parameters, so a range's values are uniform constant-bank loads.
 __global__ void __launch_bounds__(256)
 adam_segments_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                     const __grid_constant__ AdamSegments S, float lr, float b1, float b2, float eps, float wd, float gscale)
+                     const __grid_constant__ AdamSegments S, float gscale)
 {
     const size_t t0 = blockIdx.x * (size_t)blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
     for (int s = 0; s < S.n; ++s) {
         const size_t off = S.off[s], end = S.off[s] + S.cnt[s];
+        if (off + t0 >= end)
+            continue;
+        const AdamRangeConst h = S.h[s];
         for (size_t i = off + t0; i < end; i += stride)
-            adam_elem(p, g, m, v, i, lr, b1, b2, eps, wd, S.bc1[s], S.bc2_sqrt[s], gscale);
+            adam_elem(p, g, m, v, i, h.lr, h.b1, h.b2, h.eps, h.wd, h.bc1, h.bc2_sqrt, gscale);
     }
 }
 
-// The capturable update: lr and every range's step counter are read from device memory when the kernel runs, so one
-// captured launch is right on every replay.  A counter holds the steps its range has taken; this step is counter + 1.
-// Thread s of each block derives range s's bias corrections into shared memory (the host-side arithmetic of
-// launch_adam_segments, on the device).  The counters are only read here: adam_bump_kernel, the next launch on the
-// stream, increments them once this grid has finished.
+// The capturable update: the learning rates and every range's step counter are read from device memory when the kernel
+// runs, so one captured launch is right on every replay.  A counter holds the steps its range has taken; this step is
+// counter + 1.  Thread s of each block derives range s's bias corrections from its betas into shared memory (the
+// host-side arithmetic of launch_adam_segments, on the device).  The counters are only read here: adam_bump_kernel, the
+// next launch on the stream, increments them once this grid has finished.
 __global__ void __launch_bounds__(256)
 adam_dev_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                const __grid_constant__ AdamSegmentsDev S, const float* __restrict__ lr, float b1, float b2, float eps,
-                float wd, float gscale)
+                const __grid_constant__ AdamSegmentsDev S, float gscale)
 {
     __shared__ float bc1[kAdamMaxSegments], bc2_sqrt[kAdamMaxSegments];
     if (threadIdx.x < S.n) {
         const float t = (float)(*S.step[threadIdx.x] + 1);
-        bc1[threadIdx.x] = 1.0f - powf(b1, t);
-        bc2_sqrt[threadIdx.x] = sqrtf(1.0f - powf(b2, t));
+        bc1[threadIdx.x] = 1.0f - powf(S.b1[threadIdx.x], t);
+        bc2_sqrt[threadIdx.x] = sqrtf(1.0f - powf(S.b2[threadIdx.x], t));
     }
     __syncthreads();
-    const float rate = *lr;
     const size_t t0 = blockIdx.x * (size_t)blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
     for (int s = 0; s < S.n; ++s) {
         const size_t off = S.off[s], end = S.off[s] + S.cnt[s];
+        if (off + t0 >= end)
+            continue;
+        const float rate = *S.lr[s], b1 = S.b1[s], b2 = S.b2[s], eps = S.eps[s], wd = S.wd[s];
         for (size_t i = off + t0; i < end; i += stride)
             adam_elem(p, g, m, v, i, rate, b1, b2, eps, wd, bc1[s], bc2_sqrt[s], gscale);
     }
@@ -455,43 +460,48 @@ static int check_disjoint(const unsigned long long* off, const unsigned long lon
 }
 
 int launch_adam_segments(eld_ctx* ctx, float* p, const float* g, float* m, float* v, const size_t* segs, const int* steps,
-                         int n_segs, float lr, float b1, float b2, float eps, float wd, float gscale, cudaStream_t st)
+                         const AdamHyper* hyper, int n_segs, float gscale, cudaStream_t st)
 {
     ELD_REQUIRE(n_segs >= 0 && n_segs <= kAdamMaxSegments, "adam: %d segments (at most %d)", n_segs, kAdamMaxSegments);
     AdamSegments S{};
     size_t total = 0;
     for (int s = 0; s < n_segs; ++s) {
         ELD_REQUIRE(steps[s] >= 1, "adam: segment %d: step counts from 1", s);
+        const AdamHyper& h = hyper[s];
         S.off[s] = segs[2 * s]; S.cnt[s] = segs[2 * s + 1];
-        S.bc1[s] = 1.0f - powf(b1, (float)steps[s]);                 // the bias corrections of launch_adam, per segment
-        S.bc2_sqrt[s] = sqrtf(1.0f - powf(b2, (float)steps[s]));
+        S.h[s] = AdamRangeConst{ h.lr, h.b1, h.b2, h.eps, h.wd,
+                                 1.0f - powf(h.b1, (float)steps[s]),                 // the bias corrections of
+                                 sqrtf(1.0f - powf(h.b2, (float)steps[s])), 0.f };   // launch_adam, per segment
         total += S.cnt[s];
     }
     { const int rc = check_disjoint(S.off, S.cnt, n_segs); if (rc != ELD_OK) return rc; }
     S.n = n_segs;
     if (total == 0) return ELD_OK;
-    adam_segments_kernel<<<grid_for(total, 256 * 4, 8 * ctx->num_sms), 256, 0, st>>>(p, g, m, v, S, lr, b1, b2, eps, wd, gscale);
+    adam_segments_kernel<<<grid_for(total, 256 * 4, 8 * ctx->num_sms), 256, 0, st>>>(p, g, m, v, S, gscale);
     ELD_CHECK_CUDA(cudaGetLastError());
     count_launch(ctx);
     return ELD_OK;
 }
 
 int launch_adam_dev(eld_ctx* ctx, float* p, const float* g, float* m, float* v, const size_t* segs, int* const* steps,
-                    int n_segs, const float* lr, float b1, float b2, float eps, float wd, float gscale, cudaStream_t st)
+                    const float* const* lr, const AdamHyper* hyper, int n_segs, float gscale, cudaStream_t st)
 {
     ELD_REQUIRE(n_segs >= 0 && n_segs <= kAdamMaxSegments, "adam: %d segments (at most %d)", n_segs, kAdamMaxSegments);
     AdamSegmentsDev S{};
     size_t total = 0;
     for (int s = 0; s < n_segs; ++s) {
         ELD_REQUIRE(steps[s], "adam: segment %d: NULL step counter", s);
+        ELD_REQUIRE(lr[s], "adam: segment %d: NULL learning rate", s);
+        const AdamHyper& h = hyper[s];
         S.off[s] = segs[2 * s]; S.cnt[s] = segs[2 * s + 1]; S.step[s] = steps[s];
+        S.lr[s] = lr[s]; S.b1[s] = h.b1; S.b2[s] = h.b2; S.eps[s] = h.eps; S.wd[s] = h.wd;
         total += S.cnt[s];
     }
     { const int rc = check_disjoint(S.off, S.cnt, n_segs); if (rc != ELD_OK) return rc; }
     S.n = n_segs;
     if (n_segs == 0) return ELD_OK;
     if (total > 0) {
-        adam_dev_kernel<<<grid_for(total, 256 * 4, 8 * ctx->num_sms), 256, 0, st>>>(p, g, m, v, S, lr, b1, b2, eps, wd, gscale);
+        adam_dev_kernel<<<grid_for(total, 256 * 4, 8 * ctx->num_sms), 256, 0, st>>>(p, g, m, v, S, gscale);
         ELD_CHECK_CUDA(cudaGetLastError());
         count_launch(ctx);
     }

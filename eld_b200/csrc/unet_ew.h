@@ -12,21 +12,35 @@ int launch_head(eld_ctx* ctx, const void* a, const float* w, const float* b, flo
 int launch_clock_probe(eld_ctx* ctx, float* out_mhz, cudaStream_t st);
 int launch_adam(eld_ctx* ctx, float* p, const float* g, float* m, float* v, size_t n, float lr, float b1, float b2,
                 float eps, float wd, int step, float gscale, cudaStream_t st);
-// Adam over (offset, count) ranges of the flat buffers with one step count per range, one launch
+// Adam over (offset, count) ranges of the flat buffers in one launch, each range with its own step count and its own
+// hyperparameters (torch.optim.Adam's parameter groups).  The tables travel in the kernel parameters (4 KB at most).
 constexpr int kAdamMaxSegments = 64;    // one per parameter tensor of the U-Net (46) fits
+struct AdamHyper {                      // one range's hyperparameters, as the launchers take them from the host
+    float lr, b1, b2, eps, wd;
+};
+struct alignas(16) AdamRangeConst {     // one range's values in the kernel, side by side: four constant loads, not seven
+    float lr, b1, b2, eps, wd, bc1, bc2_sqrt, unused;
+};
 struct AdamSegments {
     unsigned long long off[kAdamMaxSegments], cnt[kAdamMaxSegments];
-    float bc1[kAdamMaxSegments], bc2_sqrt[kAdamMaxSegments];
+    AdamRangeConst h[kAdamMaxSegments];
     int n;
 };
+static_assert(sizeof(AdamSegments) + 4 * sizeof(void*) + sizeof(float) <= 4096, "adam_segments_kernel: parameters over 4 KB");
+// segs: (offset, count) pairs; steps, hyper: one entry per range
 int launch_adam_segments(eld_ctx* ctx, float* p, const float* g, float* m, float* v, const size_t* segs, const int* steps,
-                         int n_segs, float lr, float b1, float b2, float eps, float wd, float gscale, cudaStream_t st);
-// The capturable variants: lr and the step counters live in device memory, each range names its own counter
+                         const AdamHyper* hyper, int n_segs, float gscale, cudaStream_t st);
+// The capturable variant: the learning rates and the step counters live in device memory, each range names its own
+// counter and its own rate (ranges of one parameter group share one rate)
 struct AdamSegmentsDev {
     unsigned long long off[kAdamMaxSegments], cnt[kAdamMaxSegments];
     int* step[kAdamMaxSegments];
+    const float* lr[kAdamMaxSegments];
+    float b1[kAdamMaxSegments], b2[kAdamMaxSegments], eps[kAdamMaxSegments], wd[kAdamMaxSegments];
     int n;
 };
+static_assert(sizeof(AdamSegmentsDev) + 4 * sizeof(void*) + sizeof(float) <= 4096, "adam_dev_kernel: parameters over 4 KB");
+// steps, lr: one device pointer per range; hyper: one entry per range, its lr unused
 int launch_adam_dev(eld_ctx* ctx, float* p, const float* g, float* m, float* v, const size_t* segs, int* const* steps,
-                    int n_segs, const float* lr, float b1, float b2, float eps, float wd, float gscale, cudaStream_t st);
+                    const float* const* lr, const AdamHyper* hyper, int n_segs, float gscale, cudaStream_t st);
 }  // namespace eld

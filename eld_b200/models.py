@@ -111,6 +111,19 @@ class ELDModel(BaseModel):
         self._deferred = None        # (first frame id, n) of a synthesis the captured step runs
         self._counter_host = None    # what the device frame counter holds once the queued work has run
 
+    @property
+    def optimizer_G(self):
+        return self._optimizer_G
+
+    @optimizer_G.setter
+    def optimizer_G(self, opt):
+        """an optimizer assigned after initialize (a grouped FusedAdam, say) also takes the old one's place in
+        self.optimizers, so set_learning_rate and update_learning_rate reach it"""
+        old = getattr(self, '_optimizer_G', None)
+        self._optimizer_G = opt
+        if old is not None and getattr(self, 'optimizers', None):
+            self.optimizers = [opt if o is old else o for o in self.optimizers]
+
     def _eval(self):
         self.netG.eval()
 
@@ -414,15 +427,13 @@ class ELDModel(BaseModel):
 
     def _graph_key(self):
         """what a captured step bakes in besides its buffers: re-captured when any of it changes"""
-        g = self.optimizer_G.param_groups[0]
         synth = None
         if self._deferred is not None:       # the captured synthesis bakes in the noise model and the flags
             nm = self.noise_maker
             synth = (id(nm), int(nm.seed), nm.model, bool(getattr(self.opt, 'augment_on_gpu', False)),
                      max(1, int(getattr(self.opt, 'num_burst', 1))), self._synth_bufs[0].data_ptr())
         return (tuple(self._static[0].shape), tuple(self._static[1].shape), self.netG.loss_kind,
-                tuple(p.requires_grad for p in self.netG.parameters()), tuple(float(b) for b in g['betas']),
-                float(g['eps']), float(g['weight_decay']), synth)
+                tuple(p.requires_grad for p in self.netG.parameters()), self.optimizer_G.capture_key(), synth)
 
     def _fused_step(self, x, t):
         out, loss = self.netG.train_step(x, t)

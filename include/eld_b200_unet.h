@@ -212,5 +212,35 @@ int    eld_adam_step_segments_capturable(eld_ctx* ctx, float* params, const floa
                                          const size_t* segs, int* const* steps, int n_segs, const float* lr,
                                          float beta1, float beta2, float eps, float weight_decay, float grad_scale,
                                          void* stream);
+/* torch.optim.Adam's parameter groups: the update of eld_adam_step_segments with each range's own hyperparameters, in
+ * ONE launch.  ranges (host): n_ranges entries, each the elements [offset, offset + count) of the flat buffers, their
+ * step count (>= 1) and their group's lr, betas, eps and weight decay; grad_scale applies to every range.  The same
+ * hyperparameters in every range give eld_adam_step_segments' result bit for bit.  Elements outside the ranges are not
+ * touched.  n_ranges <= 64.
+ * ELD_E_ARG, nothing written and nothing launched: a NULL argument, a step count < 1, more than 64 ranges, two ranges that
+ * share an element (empty ranges share none), an lr, eps or weight_decay that is negative or not finite, a beta outside
+ * [0, 1). */
+typedef struct {
+    size_t offset, count;
+    int    step;
+    float  lr, beta1, beta2, eps, weight_decay;
+} eld_adam_range;
+int    eld_adam_step_ranges(eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
+                            const eld_adam_range* ranges, int n_ranges, float grad_scale, void* stream);
+/* The capturable form (as eld_adam_step_segments_capturable): each range names its own device step counter and its own
+ * device learning rate, read when the kernels run; ranges of one parameter group share one lr pointer, so a replay reads
+ * each group's current rate.  A range's bias corrections use its own betas.  Two launches on `stream` (the update, then
+ * the counters' increment); a counter named by several ranges takes one step; n_ranges == 0 launches nothing.
+ * ELD_E_ARG, nothing written and nothing launched: a NULL argument (a NULL counter or lr among the ranges included),
+ * more than 64 ranges, two ranges that share an element, an eps or weight_decay that is negative or not finite, a beta
+ * outside [0, 1).  The device lr is not read on the host: the caller keeps it a finite number >= 0. */
+typedef struct {
+    size_t       offset, count;
+    int*         step;          /* device */
+    const float* lr;            /* device */
+    float        beta1, beta2, eps, weight_decay;
+} eld_adam_range_dev;
+int    eld_adam_step_ranges_capturable(eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
+                                       const eld_adam_range_dev* ranges, int n_ranges, float grad_scale, void* stream);
 
 #endif
