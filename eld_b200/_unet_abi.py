@@ -16,6 +16,19 @@ class AdamRangeDev(c.Structure):
                 ('beta2', c.c_float), ('eps', c.c_float), ('weight_decay', c.c_float)]
 
 
+AMSGRAD, MAXIMIZE, DECOUPLED = 1, 2, 4     # ELD_ADAM_*
+
+
+class AdamRangeEx(c.Structure):
+    """eld_adam_range_ex"""
+    _fields_ = AdamRange._fields_ + [('flags', c.c_uint)]
+
+
+class AdamRangeDevEx(c.Structure):
+    """eld_adam_range_dev_ex (step: device int*, lr: device float*)"""
+    _fields_ = AdamRangeDev._fields_ + [('flags', c.c_uint)]
+
+
 def declare(lib):
     lib.eld_pack_weights.argtypes = [vp, vp, vp, i32, i32, i32, vp]
     lib.eld_conv3x3_bf16.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32,
@@ -62,6 +75,8 @@ def declare_engine(lib):
                                                       f32, f32, f32, vp]
     lib.eld_adam_step_ranges.argtypes = [vp, vp, vp, vp, vp, c.POINTER(AdamRange), i32, f32, vp]
     lib.eld_adam_step_ranges_capturable.argtypes = [vp, vp, vp, vp, vp, c.POINTER(AdamRangeDev), i32, f32, vp]
+    lib.eld_adam_step_ranges_ex.argtypes = [vp, vp, vp, vp, vp, vp, c.POINTER(AdamRangeEx), i32, f32, vp]
+    lib.eld_adam_step_ranges_ex_capturable.argtypes = [vp, vp, vp, vp, vp, vp, c.POINTER(AdamRangeDevEx), i32, f32, vp]
     lib.eld_unet_set_loss.argtypes = [vp, i32]
     lib.eld_unet_set_accumulate.argtypes = [vp, i32]
     lib.eld_clock_probe.argtypes = [vp, vp, vp]

@@ -439,6 +439,16 @@ class UNetSeeInDark(nn.Module):
         return self._profile(self._engine(n, h, w, False), lambda: self.forward(x), steps)
 
 
+# torch.optim.Adam's other update rules: a parameter group's key and its ELD_ADAM_* bit
+_OPTIONS = (('amsgrad', _unet_abi.AMSGRAD), ('maximize', _unet_abi.MAXIMIZE),
+            ('decoupled_weight_decay', _unet_abi.DECOUPLED))
+
+
+def _flags(group):
+    """a group's ELD_ADAM_* flags; a key the group lacks (a checkpoint written before it existed) reads as False"""
+    return sum(bit for key, bit in _OPTIONS if group.get(key, False))
+
+
 class FusedAdam(torch.optim.Optimizer):
     """torch.optim.Adam semantics (ELD_model.py:400-401) as ONE kernel over the flat buffers.
     Keeps `param_groups` so Engine.set_learning_rate / util.set_opt_param keep working.  Frozen parameters
@@ -453,17 +463,28 @@ class FusedAdam(torch.optim.Optimizer):
     group) live in device memory and the kernels read them when they run (eld_adam_step_segments_capturable /
     eld_adam_step_ranges_capturable), so a CUDA graph that captured step() stays right on every replay.  Before each
     replay, graph_step() does the host half of a step: each group's 'lr' into device memory (outside the graph) and
-    the parameters' version bump."""
+    the parameters' version bump.
+    amsgrad, maximize, decoupled_weight_decay: torch.optim.Adam's options of those names, per group like the other
+    hyperparameters (torch.optim.AdamW is decoupled_weight_decay=True: FusedAdamW).  While no stepped group has one on,
+    step() launches what it launched before they existed; otherwise every step goes to eld_adam_step_ranges_ex (or its
+    capturable form), still one launch.  amsgrad keeps torch's max_exp_avg_sq of every parameter in `vmax`, a buffer
+    like m and v allocated once some group has amsgrad; as in torch, a parameter gets its max_exp_avg_sq at its first
+    step under amsgrad, and one that has stepped without it cannot go on under amsgrad (ValueError)."""
 
     def __init__(self, net, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, capturable=False,
-                 param_groups=None):
+                 param_groups=None, amsgrad=False, maximize=False, decoupled_weight_decay=False):
         self.net = net
         self.capturable = capturable
         self._index = {id(q): i for i, q in enumerate(net.parameters())}     # a parameter's place in the flat buffer
         super().__init__(list(net.parameters()) if param_groups is None else param_groups,
-                         dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
+                         dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=amsgrad,
+                              maximize=maximize, decoupled_weight_decay=decoupled_weight_decay))
         self.m = torch.zeros_like(net.flat_params)
         self.v = torch.zeros_like(net.flat_params)
+        self.vmax = None                               # max_exp_avg_sq of every parameter, once some group has amsgrad
+        self._begun = [False] * len(net._spans)        # a parameter has taken a step (torch: it has state)
+        self._has_vmax = [False] * len(net._spans)     # ... and has a max_exp_avg_sq (its first step was under amsgrad)
+        self._buffers()
         self.t = 0                                     # step() calls
         if capturable:
             dev = net.flat_params.device
@@ -485,6 +506,19 @@ class FusedAdam(torch.optim.Optimizer):
         if hasattr(self, 'lr_dev'):
             self.lr_dev = torch.cat([self.lr_dev, self.lr_dev.new_zeros(1)])
             self._lr_sent.append(None)
+        if hasattr(self, 'vmax'):
+            self._buffers()
+
+    def _buffers(self):
+        """m and v, and vmax once some group has amsgrad, on the flat buffer's device (new zero buffers after a move)"""
+        p = self.net.flat_params
+        if self.m.data_ptr() == 0 or self.m.device != p.device:
+            self.m = torch.zeros_like(p)
+            self.v = torch.zeros_like(p)
+        if self.vmax is not None and (self.vmax.data_ptr() == 0 or self.vmax.device != p.device):
+            self.vmax = torch.zeros_like(p)
+        if self.vmax is None and any(g.get('amsgrad', False) for g in self.param_groups):
+            self.vmax = torch.zeros_like(p)
 
     def _owners(self):
         """the group of each parameter, in state_dict order (None: in no group)"""
@@ -499,12 +533,14 @@ class FusedAdam(torch.optim.Optimizer):
         return [q.requires_grad and o is not None for q, o in zip(self.net.parameters(), owner)]
 
     def capture_key(self):
-        """what a captured step() bakes in besides the device values it reads: the buffers, each parameter's group and
-        whether it is stepped, and every group's betas, eps and weight decay"""
+        """what a captured step() bakes in besides the device values it reads: the buffers (vmax allocated here if a
+        group has just turned amsgrad on, so that no capture allocates it), each parameter's group and whether it is
+        stepped, and every group's betas, eps, weight decay and options"""
+        self._buffers()
         owner = self._owners()
-        return (id(self), self.m.data_ptr(), self.v.data_ptr(), self.lr_dev.data_ptr() if self.capturable else None,
-                tuple(owner), tuple(self._stepped(owner)),
-                tuple((tuple(float(b) for b in g['betas']), float(g['eps']), float(g['weight_decay']))
+        return (id(self), self.m.data_ptr(), self.v.data_ptr(), None if self.vmax is None else self.vmax.data_ptr(),
+                self.lr_dev.data_ptr() if self.capturable else None, tuple(owner), tuple(self._stepped(owner)),
+                tuple((tuple(float(b) for b in g['betas']), float(g['eps']), float(g['weight_decay']), _flags(g))
                       for g in self.param_groups))
 
     def _params_stepped(self, flags):
@@ -536,12 +572,18 @@ class FusedAdam(torch.optim.Optimizer):
     def step(self, closure=None, grad_scale=1.0):
         """One Adam step on every parameter that requires grad and is in a group; a frozen parameter, its moments and
         its step count stay as they are (torch.optim.Adam skips a parameter whose .grad is None)."""
-        if self.m.data_ptr() == 0 or self.m.device != self.net.flat_params.device:
-            self.m = torch.zeros_like(self.net.flat_params)
-            self.v = torch.zeros_like(self.net.flat_params)
-        self.t += 1
+        self._buffers()
         owner = self._owners()
         flags = self._stepped(owner)
+        opts = [_flags(g) for g in self.param_groups]
+        for i, (f, o) in enumerate(zip(flags, owner)):
+            if f and opts[o] & _unet_abi.AMSGRAD and self._begun[i] and not self._has_vmax[i]:
+                raise ValueError("FusedAdam: parameter %d of net has stepped without amsgrad, so it has no "
+                                 "max_exp_avg_sq for its group's amsgrad (torch.optim.Adam raises KeyError)" % i)
+        for i, (f, o) in enumerate(zip(flags, owner)):
+            if f and not self._begun[i]:
+                self._begun[i], self._has_vmax[i] = True, bool(opts[o] & _unet_abi.AMSGRAD)
+        self.t += 1
         if self.capturable:
             if not torch.cuda.is_current_stream_capturing():
                 self._send_lr()                        # a capture reads lr_dev as graph_step leaves it before each replay
@@ -552,9 +594,10 @@ class FusedAdam(torch.optim.Optimizer):
         hps = [(float(g['lr']), float(g['betas'][0]), float(g['betas'][1]), float(g['eps']), float(g['weight_decay']))
                for g in self.param_groups]
         live = sorted({o for o, f in zip(owner, flags) if f})
+        ex = any(opts[k] for k in live)              # amsgrad, maximize or decoupled weight decay: the _ex entry points
         # one hyperparameter set (a captured step: one group, whose lr may change between replays) over every
         # parameter: the single-group entry points, as without groups
-        if None in owner or (len(live) > 1 if self.capturable else len({hps[k] for k in live}) > 1):
+        if ex or None in owner or (len(live) > 1 if self.capturable else len({hps[k] for k in live}) > 1):
             single = None
         else:
             single = live[0] if live else 0
@@ -564,6 +607,7 @@ class FusedAdam(torch.optim.Optimizer):
         def adam(lo, hi):
             lib, dev = _lib.load(), _lib.ctx(p.device.index or 0)
             bufs = (dev, p.data_ptr(), self.net.flat_grads.data_ptr(), self.m.data_ptr(), self.v.data_ptr())
+            vmax = None if self.vmax is None else self.vmax.data_ptr()
             if self.capturable:                        # one range per trainable parameter, each with its own counter
                 mine = []
                 for i, ((off, n), f) in enumerate(zip(self.net._spans, flags)):
@@ -581,6 +625,13 @@ class FusedAdam(torch.optim.Optimizer):
                         'eld_adam_step_segments_capturable')
                     return
                 rates = self.lr_dev.data_ptr()
+                if ex:
+                    table = (_unet_abi.AdamRangeDevEx * k)(*[_unet_abi.AdamRangeDevEx(
+                        *self.net._spans[i], c, rates + 4 * owner[i], *hps[owner[i]][1:], opts[owner[i]])
+                        for i, c in zip(mine, ctrs)])
+                    _lib.check(lib.eld_adam_step_ranges_ex_capturable(*bufs, vmax, table, k, float(grad_scale), _st()),
+                               'eld_adam_step_ranges_ex_capturable')
+                    return
                 table = (_unet_abi.AdamRangeDev * k)(*[_unet_abi.AdamRangeDev(
                     *self.net._spans[i], c, rates + 4 * owner[i], *hps[owner[i]][1:]) for i, c in zip(mine, ctrs)])
                 _lib.check(lib.eld_adam_step_ranges_capturable(*bufs, table, k, float(grad_scale), _st()),
@@ -609,6 +660,12 @@ class FusedAdam(torch.optim.Optimizer):
                 _lib.check(lib.eld_adam_step_segments(*bufs, table, steps, k, *hps[single], float(grad_scale), _st()),
                            'eld_adam_step_segments')
                 return
+            if ex:
+                table = (_unet_abi.AdamRangeEx * k)(*[_unet_abi.AdamRangeEx(a, c, s, *hps[o], opts[o])
+                                                      for a, c, s, o in segs])
+                _lib.check(lib.eld_adam_step_ranges_ex(*bufs, vmax, table, k, float(grad_scale), _st()),
+                           'eld_adam_step_ranges_ex')
+                return
             table = (_unet_abi.AdamRange * k)(*[_unet_abi.AdamRange(a, c, s, *hps[o]) for a, c, s, o in segs])
             _lib.check(lib.eld_adam_step_ranges(*bufs, table, k, float(grad_scale), _st()), 'eld_adam_step_ranges')
         pend = getattr(self.net, '_pending_allreduce', None)
@@ -632,8 +689,9 @@ class FusedAdam(torch.optim.Optimizer):
         self.net.flat_grads.zero_()
 
     # checkpoint format of torch.optim.Adam ('opt_g' in ELD_model.py:516-523): parameters numbered group by group, in
-    # group order; per-parameter step; a parameter that has never taken a step has no state entry.  Capturable: 'step' is
-    # a float32 tensor on the parameter's device, as torch's capturable Adam stores it.
+    # group order; per-parameter step; a parameter that has never taken a step has no state entry; 'max_exp_avg_sq' for a
+    # parameter whose first step was under amsgrad.  Capturable: 'step' is a float32 tensor on the parameter's device, as
+    # torch's capturable Adam stores it.
     def state_dict(self):
         state, groups = {}, []
         steps, spans, i = self.host_steps(), self.net._spans, 0
@@ -647,6 +705,8 @@ class FusedAdam(torch.optim.Optimizer):
                     state[i] = {'step': torch.tensor(s, device=q.device) if self.capturable else torch.tensor(s),
                                 'exp_avg': self.m[off:off + n].view(q.shape).clone(),
                                 'exp_avg_sq': self.v[off:off + n].view(q.shape).clone()}
+                    if self._has_vmax[j]:
+                        state[i]['max_exp_avg_sq'] = self.vmax[off:off + n].view(q.shape).clone()
                 ids.append(i)
                 i += 1
             groups.append(dict((k, v) for k, v in group.items() if k != 'params'))
@@ -655,7 +715,9 @@ class FusedAdam(torch.optim.Optimizer):
 
     def load_state_dict(self, sd):
         """torch.optim.Adam's load_state_dict: the saved groups must match this optimizer's in number and size
-        (ValueError); saved parameter k of the saved numbering is this optimizer's parameter k of its own"""
+        (ValueError); saved parameter k of the saved numbering is this optimizer's parameter k of its own.  The saved
+        groups' hyperparameters and options replace this optimizer's (an option the checkpoint lacks is False); a
+        parameter with state in an amsgrad group must have its max_exp_avg_sq (ValueError, nothing loaded)."""
         saved = sd['param_groups']
         if len(saved) != len(self.param_groups):
             raise ValueError('loaded state dict has %d parameter groups, the optimizer %d' % (
@@ -663,9 +725,21 @@ class FusedAdam(torch.optim.Optimizer):
         if any(len(a['params']) != len(b['params']) for a, b in zip(saved, self.param_groups)):
             raise ValueError("loaded state dict contains a parameter group that doesn't match the size of optimizer's "
                              "group")
+        for a in saved:
+            if a.get('amsgrad', False) and any(k in sd['state'] and 'max_exp_avg_sq' not in sd['state'][k]
+                                               for k in a['params']):
+                raise ValueError('loaded state dict has an amsgrad group with a stepped parameter but no '
+                                 'max_exp_avg_sq for it')
+        if self.vmax is None and (any(a.get('amsgrad', False) for a in saved) or
+                                  any('max_exp_avg_sq' in st for st in sd['state'].values())):
+            self.vmax = torch.zeros_like(self.net.flat_params)
         steps = [0] * len(self.net._spans)
         self.m.zero_()
         self.v.zero_()
+        if self.vmax is not None:
+            self.vmax.zero_()
+        self._begun = [False] * len(self.net._spans)
+        self._has_vmax = [False] * len(self.net._spans)
         for a, b in zip(saved, self.param_groups):
             for key, q in zip(a['params'], b['params']):
                 st = sd['state'].get(key)
@@ -675,6 +749,10 @@ class FusedAdam(torch.optim.Optimizer):
                 off, n = self.net._spans[j]
                 self.m[off:off + n].copy_(st['exp_avg'].reshape(-1))
                 self.v[off:off + n].copy_(st['exp_avg_sq'].reshape(-1))
+                if 'max_exp_avg_sq' in st:
+                    self.vmax[off:off + n].copy_(st['max_exp_avg_sq'].reshape(-1))
+                    self._has_vmax[j] = True
+                self._begun[j] = True
                 steps[j] = int(float(st['step']))
         if self.capturable:
             self.step_dev.copy_(torch.tensor(steps, dtype=torch.int32))      # in place: a captured step keeps its address
@@ -685,6 +763,23 @@ class FusedAdam(torch.optim.Optimizer):
             for k, v in a.items():
                 if k != 'params':
                     b[k] = v
+            for k, _ in _OPTIONS:
+                b[k] = a.get(k, False)
+
+
+class FusedAdamW(FusedAdam):
+    """torch.optim.AdamW: FusedAdam with decoupled weight decay, and AdamW's default weight decay of 1e-2.  As AdamW,
+    it keeps decoupled_weight_decay=True in every group through a checkpoint load."""
+
+    def __init__(self, net, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, capturable=False,
+                 param_groups=None, amsgrad=False, maximize=False):
+        super().__init__(net, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, capturable=capturable,
+                         param_groups=param_groups, amsgrad=amsgrad, maximize=maximize, decoupled_weight_decay=True)
+
+    def load_state_dict(self, sd):
+        super().load_state_dict(sd)
+        for group in self.param_groups:
+            group['decoupled_weight_decay'] = True
 
 
 def unet(in_channels, out_channels, **kwargs):

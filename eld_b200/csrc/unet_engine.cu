@@ -896,7 +896,7 @@ extern "C" int eld_adam_step_segments(eld_ctx* ctx, float* params, const float* 
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     AdamHyper hyper[kAdamMaxSegments];                  // every range takes the one set (n_segs > 64 is refused below)
     std::fill(hyper, hyper + kAdamMaxSegments, AdamHyper{ lr, beta1, beta2, eps, weight_decay });
-    return launch_adam_segments(ctx, params, grads, m, v, segs, steps, hyper, n_segs, grad_scale,
+    return launch_adam_segments(ctx, params, grads, m, v, nullptr, segs, steps, hyper, n_segs, grad_scale,
                                 static_cast<cudaStream_t>(stream));
 }
 
@@ -913,24 +913,56 @@ static int check_adam_hyper(const char* fn, int s, const float* lr, float beta1,
     return ELD_OK;
 }
 
-extern "C" int eld_adam_step_ranges(eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
-                                    const eld_adam_range* ranges, int n_ranges, float grad_scale, void* stream)
+// a range's ELD_ADAM_* flags: none in the plain records
+static unsigned adam_flags(const eld_adam_range&) { return 0; }
+static unsigned adam_flags(const eld_adam_range_dev&) { return 0; }
+static unsigned adam_flags(const eld_adam_range_ex& r) { return r.flags; }
+static unsigned adam_flags(const eld_adam_range_dev_ex& r) { return r.flags; }
+
+// a range's flags as the _ex calls accept them: known bits, and a vmax where AMSGRAD needs one
+static int check_adam_flags(const char* fn, int s, unsigned flags, const float* vmax)
 {
-    ELD_REQUIRE(ctx && params && grads && m && v && (n_ranges <= 0 || ranges), "eld_adam_step_ranges: NULL argument");
+    ELD_REQUIRE(!(flags & ~(ELD_ADAM_AMSGRAD | ELD_ADAM_MAXIMIZE | ELD_ADAM_DECOUPLED)), "%s: range %d: unknown flags 0x%x",
+                fn, s, flags);
+    ELD_REQUIRE(vmax || !(flags & ELD_ADAM_AMSGRAD), "%s: range %d: ELD_ADAM_AMSGRAD with a NULL vmax", fn, s);
+    return ELD_OK;
+}
+
+// eld_adam_step_ranges and its _ex form: every record checked, then one launch_adam_segments
+template <class Range>
+static int adam_step_ranges(const char* fn, eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
+                            float* vmax, const Range* ranges, int n_ranges, float grad_scale, void* stream)
+{
+    ELD_REQUIRE(ctx && params && grads && m && v && (n_ranges <= 0 || ranges), "%s: NULL argument", fn);
     size_t segs[2 * kAdamMaxSegments];
     int steps[kAdamMaxSegments];
     AdamHyper hyper[kAdamMaxSegments];
     const int k = n_ranges < kAdamMaxSegments ? n_ranges : kAdamMaxSegments;     // more than 64 is refused below
     for (int s = 0; s < k; ++s) {
-        const eld_adam_range& r = ranges[s];
-        const int rc = check_adam_hyper("eld_adam_step_ranges", s, &r.lr, r.beta1, r.beta2, r.eps, r.weight_decay);
+        const Range& r = ranges[s];
+        int rc = check_adam_hyper(fn, s, &r.lr, r.beta1, r.beta2, r.eps, r.weight_decay);
+        if (rc == ELD_OK) rc = check_adam_flags(fn, s, adam_flags(r), vmax);
         if (rc != ELD_OK) return rc;
         segs[2 * s] = r.offset; segs[2 * s + 1] = r.count; steps[s] = r.step;
-        hyper[s] = AdamHyper{ r.lr, r.beta1, r.beta2, r.eps, r.weight_decay };
+        hyper[s] = AdamHyper{ r.lr, r.beta1, r.beta2, r.eps, r.weight_decay, adam_flags(r) };
     }
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
-    return launch_adam_segments(ctx, params, grads, m, v, segs, steps, hyper, n_ranges, grad_scale,
+    return launch_adam_segments(ctx, params, grads, m, v, vmax, segs, steps, hyper, n_ranges, grad_scale,
                                 static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int eld_adam_step_ranges(eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
+                                    const eld_adam_range* ranges, int n_ranges, float grad_scale, void* stream)
+{
+    return adam_step_ranges("eld_adam_step_ranges", ctx, params, grads, m, v, nullptr, ranges, n_ranges, grad_scale,
+                            stream);
+}
+
+extern "C" int eld_adam_step_ranges_ex(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, float* vmax,
+                                       const eld_adam_range_ex* ranges, int n_ranges, float grad_scale, void* stream)
+{
+    return adam_step_ranges("eld_adam_step_ranges_ex", ctx, params, grads, m, v, vmax, ranges, n_ranges, grad_scale,
+                            stream);
 }
 
 extern "C" int eld_adam_step_capturable(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, size_t n,
@@ -941,7 +973,8 @@ extern "C" int eld_adam_step_capturable(eld_ctx* ctx, float* params, const float
     ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
     const size_t seg[2] = { 0, n };
     const AdamHyper hyper{ 0.f, beta1, beta2, eps, weight_decay };
-    return launch_adam_dev(ctx, params, grads, m, v, seg, &step, &lr, &hyper, 1, grad_scale, static_cast<cudaStream_t>(stream));
+    return launch_adam_dev(ctx, params, grads, m, v, nullptr, seg, &step, &lr, &hyper, 1, grad_scale,
+                           static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int eld_adam_step_segments_capturable(eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
@@ -956,7 +989,31 @@ extern "C" int eld_adam_step_segments_capturable(eld_ctx* ctx, float* params, co
     AdamHyper hyper[kAdamMaxSegments];
     std::fill(rates, rates + kAdamMaxSegments, lr);
     std::fill(hyper, hyper + kAdamMaxSegments, AdamHyper{ 0.f, beta1, beta2, eps, weight_decay });
-    return launch_adam_dev(ctx, params, grads, m, v, segs, steps, rates, hyper, n_segs, grad_scale,
+    return launch_adam_dev(ctx, params, grads, m, v, nullptr, segs, steps, rates, hyper, n_segs, grad_scale,
+                           static_cast<cudaStream_t>(stream));
+}
+
+// eld_adam_step_ranges_capturable and its _ex form: every record checked, then one launch_adam_dev
+template <class Range>
+static int adam_step_ranges_dev(const char* fn, eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
+                                float* vmax, const Range* ranges, int n_ranges, float grad_scale, void* stream)
+{
+    ELD_REQUIRE(ctx && params && grads && m && v && (n_ranges <= 0 || ranges), "%s: NULL argument", fn);
+    size_t segs[2 * kAdamMaxSegments];
+    int* steps[kAdamMaxSegments];
+    const float* rates[kAdamMaxSegments];
+    AdamHyper hyper[kAdamMaxSegments];
+    const int k = n_ranges < kAdamMaxSegments ? n_ranges : kAdamMaxSegments;     // more than 64 is refused below
+    for (int s = 0; s < k; ++s) {
+        const Range& r = ranges[s];
+        int rc = check_adam_hyper(fn, s, nullptr, r.beta1, r.beta2, r.eps, r.weight_decay);
+        if (rc == ELD_OK) rc = check_adam_flags(fn, s, adam_flags(r), vmax);
+        if (rc != ELD_OK) return rc;
+        segs[2 * s] = r.offset; segs[2 * s + 1] = r.count; steps[s] = r.step; rates[s] = r.lr;
+        hyper[s] = AdamHyper{ 0.f, r.beta1, r.beta2, r.eps, r.weight_decay, adam_flags(r) };
+    }
+    ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
+    return launch_adam_dev(ctx, params, grads, m, v, vmax, segs, steps, rates, hyper, n_ranges, grad_scale,
                            static_cast<cudaStream_t>(stream));
 }
 
@@ -964,24 +1021,16 @@ extern "C" int eld_adam_step_ranges_capturable(eld_ctx* ctx, float* params, cons
                                                const eld_adam_range_dev* ranges, int n_ranges, float grad_scale,
                                                void* stream)
 {
-    ELD_REQUIRE(ctx && params && grads && m && v && (n_ranges <= 0 || ranges),
-                "eld_adam_step_ranges_capturable: NULL argument");
-    size_t segs[2 * kAdamMaxSegments];
-    int* steps[kAdamMaxSegments];
-    const float* rates[kAdamMaxSegments];
-    AdamHyper hyper[kAdamMaxSegments];
-    const int k = n_ranges < kAdamMaxSegments ? n_ranges : kAdamMaxSegments;     // more than 64 is refused below
-    for (int s = 0; s < k; ++s) {
-        const eld_adam_range_dev& r = ranges[s];
-        const int rc = check_adam_hyper("eld_adam_step_ranges_capturable", s, nullptr, r.beta1, r.beta2, r.eps,
-                                        r.weight_decay);
-        if (rc != ELD_OK) return rc;
-        segs[2 * s] = r.offset; segs[2 * s + 1] = r.count; steps[s] = r.step; rates[s] = r.lr;
-        hyper[s] = AdamHyper{ 0.f, r.beta1, r.beta2, r.eps, r.weight_decay };
-    }
-    ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
-    return launch_adam_dev(ctx, params, grads, m, v, segs, steps, rates, hyper, n_ranges, grad_scale,
-                           static_cast<cudaStream_t>(stream));
+    return adam_step_ranges_dev("eld_adam_step_ranges_capturable", ctx, params, grads, m, v, nullptr, ranges, n_ranges,
+                                grad_scale, stream);
+}
+
+extern "C" int eld_adam_step_ranges_ex_capturable(eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
+                                                  float* vmax, const eld_adam_range_dev_ex* ranges, int n_ranges,
+                                                  float grad_scale, void* stream)
+{
+    return adam_step_ranges_dev("eld_adam_step_ranges_ex_capturable", ctx, params, grads, m, v, vmax, ranges, n_ranges,
+                                grad_scale, stream);
 }
 
 extern "C" int eld_unet_set_loss(eld_unet* u, int kind)

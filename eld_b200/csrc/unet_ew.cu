@@ -287,20 +287,41 @@ head_kernel(const __nv_bfloat16* __restrict__ a, const float* __restrict__ w, co
 // ---------------------------------------------------------------------------------------------------
 // Adam (torch.optim.Adam semantics, ELD_model.py:400-401): one pass over the flat parameter buffer.
 // ---------------------------------------------------------------------------------------------------
+// kOptions: torch.optim.Adam's other update rules, `flags` (ELD_ADAM_*) uniform over a range:
+//   MAXIMIZE   the gradient's sign flipped after the scaling;
+//   DECOUPLED  a non-zero weight decay shrinks the parameter by `decay` = 1 - lr wd (torch.optim.AdamW) instead of
+//              adding wd p to the gradient;
+//   AMSGRAD    vmax <- max(vmax, v) (NaN if either is, as torch.maximum), and the denominator takes vmax.
+// Without kOptions, or with flags 0, the operations are the plain update's, in its order: the same bits.
+template <bool kOptions = false>
 __device__ __forceinline__ void adam_elem(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                           float* __restrict__ v, size_t i, float lr, float b1, float b2, float eps, float wd,
-                                          float bc1, float bc2_sqrt, float gscale)
+                                          float bc1, float bc2_sqrt, float gscale, float* __restrict__ vmax = nullptr,
+                                          unsigned flags = 0, float decay = 1.f)
 {
     float gi = g[i] * gscale;
-    const float pi = p[i];
-    if (wd != 0.f) gi = fmaf(wd, pi, gi);
+    float pi = p[i];
+    if (kOptions && (flags & ELD_ADAM_MAXIMIZE)) gi = -gi;
+    if (wd != 0.f) {
+        if (kOptions && (flags & ELD_ADAM_DECOUPLED)) pi = __fmul_rn(pi, decay);   // rounded on its own, as torch's mul_
+        else gi = fmaf(wd, pi, gi);
+    }
     const float mi = fmaf(b1, m[i], (1.f - b1) * gi);
     const float vi = fmaf(b2, v[i], (1.f - b2) * gi * gi);
     m[i] = mi;
     v[i] = vi;
-    const float denom = sqrtf(vi) / bc2_sqrt + eps;
+    float vd = vi;
+    if (kOptions && (flags & ELD_ADAM_AMSGRAD)) {
+        const float vo = vmax[i];
+        vd = isnan(vo) ? vo : (vo > vi ? vo : vi);       // not fmaxf: that one drops a NaN
+        vmax[i] = vd;
+    }
+    const float denom = sqrtf(vd) / bc2_sqrt + eps;
     p[i] = pi - (lr / bc1) * (mi / denom);
 }
+
+// 1 - lr wd in fp32, rounded once: the factor a DECOUPLED range multiplies its parameters by
+__device__ __forceinline__ float adam_decay(float lr, float wd) { return fmaf(-lr, wd, 1.f); }
 
 __global__ void __launch_bounds__(256)
 adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
@@ -314,9 +335,12 @@ adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restric
 // state['step'] per parameter: a tensor that was frozen for a while has taken fewer steps than its neighbours) and its
 // own hyperparameters (its parameter group's).  Every segment is walked by the whole grid; the table travels in the
 // kernel parameters, so a range's values are uniform constant-bank loads.
+// kOptions: each range's ELD_ADAM_* flags (the record's `flags`) select its update rules, and vmax is read and written
+// on AMSGRAD ranges; without, the flags and vmax are not read.
+template <bool kOptions>
 __global__ void __launch_bounds__(256)
 adam_segments_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                     const __grid_constant__ AdamSegments S, float gscale)
+                     float* __restrict__ vmax, const __grid_constant__ AdamSegments S, float gscale)
 {
     const size_t t0 = blockIdx.x * (size_t)blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
     for (int s = 0; s < S.n; ++s) {
@@ -324,8 +348,10 @@ adam_segments_kernel(float* __restrict__ p, const float* __restrict__ g, float* 
         if (off + t0 >= end)
             continue;
         const AdamRangeConst h = S.h[s];
+        const float decay = adam_decay(h.lr, h.wd);
         for (size_t i = off + t0; i < end; i += stride)
-            adam_elem(p, g, m, v, i, h.lr, h.b1, h.b2, h.eps, h.wd, h.bc1, h.bc2_sqrt, gscale);
+            adam_elem<kOptions>(p, g, m, v, i, h.lr, h.b1, h.b2, h.eps, h.wd, h.bc1, h.bc2_sqrt, gscale, vmax, h.flags,
+                                decay);
     }
 }
 
@@ -333,10 +359,12 @@ adam_segments_kernel(float* __restrict__ p, const float* __restrict__ g, float* 
 // runs, so one captured launch is right on every replay.  A counter holds the steps its range has taken; this step is
 // counter + 1.  Thread s of each block derives range s's bias corrections from its betas into shared memory (the
 // host-side arithmetic of launch_adam_segments, on the device).  The counters are only read here: adam_bump_kernel, the
-// next launch on the stream, increments them once this grid has finished.
+// next launch on the stream, increments them once this grid has finished.  kOptions as adam_segments_kernel's, with
+// each range's flags in S.flags and the decoupled decay from the device lr.
+template <bool kOptions>
 __global__ void __launch_bounds__(256)
 adam_dev_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                const __grid_constant__ AdamSegmentsDev S, float gscale)
+                float* __restrict__ vmax, const __grid_constant__ AdamSegmentsDev S, float gscale)
 {
     __shared__ float bc1[kAdamMaxSegments], bc2_sqrt[kAdamMaxSegments];
     if (threadIdx.x < S.n) {
@@ -351,8 +379,10 @@ adam_dev_kernel(float* __restrict__ p, const float* __restrict__ g, float* __res
         if (off + t0 >= end)
             continue;
         const float rate = *S.lr[s], b1 = S.b1[s], b2 = S.b2[s], eps = S.eps[s], wd = S.wd[s];
+        const float decay = adam_decay(rate, wd);
         for (size_t i = off + t0; i < end; i += stride)
-            adam_elem(p, g, m, v, i, rate, b1, b2, eps, wd, bc1[s], bc2_sqrt[s], gscale);
+            adam_elem<kOptions>(p, g, m, v, i, rate, b1, b2, eps, wd, bc1[s], bc2_sqrt[s], gscale, vmax, S.flags[s],
+                                decay);
     }
 }
 
@@ -459,49 +489,62 @@ static int check_disjoint(const unsigned long long* off, const unsigned long lon
     return ELD_OK;
 }
 
-int launch_adam_segments(eld_ctx* ctx, float* p, const float* g, float* m, float* v, const size_t* segs, const int* steps,
-                         const AdamHyper* hyper, int n_segs, float gscale, cudaStream_t st)
+int launch_adam_segments(eld_ctx* ctx, float* p, const float* g, float* m, float* v, float* vmax, const size_t* segs,
+                         const int* steps, const AdamHyper* hyper, int n_segs, float gscale, cudaStream_t st)
 {
     ELD_REQUIRE(n_segs >= 0 && n_segs <= kAdamMaxSegments, "adam: %d segments (at most %d)", n_segs, kAdamMaxSegments);
     AdamSegments S{};
     size_t total = 0;
+    unsigned any = 0;
     for (int s = 0; s < n_segs; ++s) {
         ELD_REQUIRE(steps[s] >= 1, "adam: segment %d: step counts from 1", s);
         const AdamHyper& h = hyper[s];
         S.off[s] = segs[2 * s]; S.cnt[s] = segs[2 * s + 1];
         S.h[s] = AdamRangeConst{ h.lr, h.b1, h.b2, h.eps, h.wd,
                                  1.0f - powf(h.b1, (float)steps[s]),                 // the bias corrections of
-                                 sqrtf(1.0f - powf(h.b2, (float)steps[s])), 0.f };   // launch_adam, per segment
+                                 sqrtf(1.0f - powf(h.b2, (float)steps[s])), h.flags };   // launch_adam, per segment
         total += S.cnt[s];
+        any |= h.flags;
     }
     { const int rc = check_disjoint(S.off, S.cnt, n_segs); if (rc != ELD_OK) return rc; }
     S.n = n_segs;
     if (total == 0) return ELD_OK;
-    adam_segments_kernel<<<grid_for(total, 256 * 4, 8 * ctx->num_sms), 256, 0, st>>>(p, g, m, v, S, gscale);
+    const int grid = grid_for(total, 256 * 4, 8 * ctx->num_sms);
+    if (any)
+        adam_segments_kernel<true><<<grid, 256, 0, st>>>(p, g, m, v, vmax, S, gscale);
+    else
+        adam_segments_kernel<false><<<grid, 256, 0, st>>>(p, g, m, v, nullptr, S, gscale);
     ELD_CHECK_CUDA(cudaGetLastError());
     count_launch(ctx);
     return ELD_OK;
 }
 
-int launch_adam_dev(eld_ctx* ctx, float* p, const float* g, float* m, float* v, const size_t* segs, int* const* steps,
-                    const float* const* lr, const AdamHyper* hyper, int n_segs, float gscale, cudaStream_t st)
+int launch_adam_dev(eld_ctx* ctx, float* p, const float* g, float* m, float* v, float* vmax, const size_t* segs,
+                    int* const* steps, const float* const* lr, const AdamHyper* hyper, int n_segs, float gscale,
+                    cudaStream_t st)
 {
     ELD_REQUIRE(n_segs >= 0 && n_segs <= kAdamMaxSegments, "adam: %d segments (at most %d)", n_segs, kAdamMaxSegments);
     AdamSegmentsDev S{};
     size_t total = 0;
+    unsigned any = 0;
     for (int s = 0; s < n_segs; ++s) {
         ELD_REQUIRE(steps[s], "adam: segment %d: NULL step counter", s);
         ELD_REQUIRE(lr[s], "adam: segment %d: NULL learning rate", s);
         const AdamHyper& h = hyper[s];
         S.off[s] = segs[2 * s]; S.cnt[s] = segs[2 * s + 1]; S.step[s] = steps[s];
-        S.lr[s] = lr[s]; S.b1[s] = h.b1; S.b2[s] = h.b2; S.eps[s] = h.eps; S.wd[s] = h.wd;
+        S.lr[s] = lr[s]; S.b1[s] = h.b1; S.b2[s] = h.b2; S.eps[s] = h.eps; S.wd[s] = h.wd; S.flags[s] = h.flags;
         total += S.cnt[s];
+        any |= h.flags;
     }
     { const int rc = check_disjoint(S.off, S.cnt, n_segs); if (rc != ELD_OK) return rc; }
     S.n = n_segs;
     if (n_segs == 0) return ELD_OK;
     if (total > 0) {
-        adam_dev_kernel<<<grid_for(total, 256 * 4, 8 * ctx->num_sms), 256, 0, st>>>(p, g, m, v, S, gscale);
+        const int grid = grid_for(total, 256 * 4, 8 * ctx->num_sms);
+        if (any)
+            adam_dev_kernel<true><<<grid, 256, 0, st>>>(p, g, m, v, vmax, S, gscale);
+        else
+            adam_dev_kernel<false><<<grid, 256, 0, st>>>(p, g, m, v, nullptr, S, gscale);
         ELD_CHECK_CUDA(cudaGetLastError());
         count_launch(ctx);
     }

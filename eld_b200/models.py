@@ -36,7 +36,8 @@ def default_opt(**kw):
              stage_in='raw', stage_out='raw', model_path=None, include=4, crf=False, batchSize=1, lr=1e-4,
              beta1=0.9, wd=0.0, loss='l1', noise='g', isTrain=True, save_epoch_freq=100, noise_on_gpu=False,
              augment_on_gpu=False, defer_loss_sync=False, prefetch_noise=False, num_burst=1, pairs_on_gpu=False,
-             cuda_graph=False, accum_steps=1, params_on_gpu=False)
+             cuda_graph=False, accum_steps=1, params_on_gpu=False, amsgrad=False,
+             decoupled_weight_decay=False)
     o.update(kw)
     return SimpleNamespace(**o)
 
@@ -178,7 +179,8 @@ class ELDModel(BaseModel):
                 raise NotImplementedError("pixel losses of models/losses.py:29-36: 'l1' (nn.L1Loss) or 'l2' (nn.MSELoss)")
             self.netG.loss_kind = opt.loss
             self.optimizer_G = arch.FusedAdam(self.netG, lr=opt.lr, betas=(opt.beta1, 0.999), weight_decay=opt.wd,
-                                              capturable=self._graphed)
+                                              capturable=self._graphed, amsgrad=getattr(opt, 'amsgrad', False),
+                                              decoupled_weight_decay=getattr(opt, 'decoupled_weight_decay', False))
             self._init_optimizer([self.optimizer_G])
         if opt.resume:
             self.load(self, opt.resume_epoch)

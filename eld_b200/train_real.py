@@ -62,6 +62,10 @@ def main():
     ap.add_argument('--no-augment', action='store_true', help='skip the flips / transpose (sid_dataset.py:340-352)')
     ap.add_argument('--accum_steps', type=int, default=1, help='micro-batches per optimizer step: one Adam step (and one '
                     'all-reduce) per window of k steps, on the gradients of k * world * batchSize frames')
+    ap.add_argument('--wd', type=float, default=0, help='weight decay for adam')   # options/eld/train_options.py: --wd
+    ap.add_argument('--amsgrad', action='store_true', help="Adam's AMSGrad variant (torch.optim.Adam(amsgrad=True))")
+    ap.add_argument('--decoupled_weight_decay', action='store_true', help='decoupled weight decay: --wd shrinks the '
+                    'weights by 1 - lr * wd each step instead of adding wd * w to the gradient (torch.optim.AdamW)')
     a = ap.parse_args()
     world = int(os.environ.get('WORLD_SIZE', '1'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
@@ -85,7 +89,8 @@ def main():
                                 [LMDBDataset(join(a.traindir, _db_name('input', a.stage_in, a.crf)))])
     opt = models.default_opt(name=a.name, gpu_ids=[local], batchSize=a.batchSize, lr=1e-4, pairs_on_gpu=True,
                              augment_on_gpu=not a.no_augment, defer_loss_sync=True, loss=a.loss, stage_in=a.stage_in,
-                             stage_out=a.stage_out, seed=a.seed, accum_steps=a.accum_steps)
+                             stage_out=a.stage_out, seed=a.seed, accum_steps=a.accum_steps, wd=a.wd, amsgrad=a.amsgrad,
+                             decoupled_weight_decay=a.decoupled_weight_decay)
     sampler = torch.utils.data.distributed.DistributedSampler(train, world, rank, shuffle=True) if world > 1 else None
     loader = torch.utils.data.DataLoader(train, batch_size=a.batchSize, shuffle=sampler is None, sampler=sampler,
                                          num_workers=a.nThreads, pin_memory=True)

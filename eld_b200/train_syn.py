@@ -52,6 +52,10 @@ def main():
                     'all-reduce) per window of k steps, on the gradients of k * world * batchSize frames')
     ap.add_argument('--params_on_gpu', action='store_true', help="draw each frame's noise parameters and flips on the GPU "
                     '(same laws and frame ids as the host draws, other values): no host work per frame')
+    ap.add_argument('--wd', type=float, default=0, help='weight decay for adam')   # options/eld/train_options.py: --wd
+    ap.add_argument('--amsgrad', action='store_true', help="Adam's AMSGrad variant (torch.optim.Adam(amsgrad=True))")
+    ap.add_argument('--decoupled_weight_decay', action='store_true', help='decoupled weight decay: --wd shrinks the '
+                    'weights by 1 - lr * wd each step instead of adding wd * w to the gradient (torch.optim.AdamW)')
     a = ap.parse_args()
     world = int(os.environ.get('WORLD_SIZE', '1'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
@@ -63,7 +67,8 @@ def main():
     opt = models.default_opt(name=a.name, gpu_ids=[local], noise=a.noise, include=a.include, batchSize=a.batchSize,
                              lr=a.lr, noise_on_gpu=True, augment_on_gpu=not a.no_augment and a.stage_in == 'raw', defer_loss_sync=True,
                              loss=a.loss, stage_in=a.stage_in, stage_out=a.stage_out, num_burst=a.num_burst,
-                             accum_steps=a.accum_steps, params_on_gpu=a.params_on_gpu)
+                             accum_steps=a.accum_steps, params_on_gpu=a.params_on_gpu, wd=a.wd, amsgrad=a.amsgrad,
+                             decoupled_weight_decay=a.decoupled_weight_decay)
     noise_model = NoiseModel(model=opt.noise, include=opt.include, seed=a.seed, verbose=rank == 0)   # train_syn.py:38
     ds = SyntheticClean(a.iters * a.batchSize * world, a.seed, meta=a.stage_in == 'srgb')
     sampler = torch.utils.data.distributed.DistributedSampler(ds, world, rank, shuffle=True) if world > 1 else None

@@ -242,5 +242,39 @@ typedef struct {
 } eld_adam_range_dev;
 int    eld_adam_step_ranges_capturable(eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
                                        const eld_adam_range_dev* ranges, int n_ranges, float grad_scale, void* stream);
+/* torch.optim.Adam's other update rules, per range: eld_adam_step_ranges(_capturable) with `flags` in every record, a
+ * set of
+ *   ELD_ADAM_AMSGRAD     (amsgrad=True)   vmax <- max(vmax, v), NaN if either is (torch.maximum); the denominator is
+ *                                         sqrt(vmax) / sqrt(1 - beta2^t) + eps.  vmax is laid out like m and v.
+ *   ELD_ADAM_MAXIMIZE    (maximize=True)  the scaled gradient's sign flipped before the weight decay.
+ *   ELD_ADAM_DECOUPLED   (decoupled_weight_decay=True, torch.optim.AdamW) a non-zero weight decay multiplies the
+ *                                         parameters by 1 - lr * weight_decay (fp32, rounded once; the device lr in the
+ *                                         capturable form) instead of adding weight_decay * params to the gradient.
+ * Flags 0 in every range give eld_adam_step_ranges(_capturable)'s result bit for bit, and a range's flags 0 give that
+ * range the plain update's bits in any call.  vmax is read and written only on AMSGRAD ranges and may be NULL when no
+ * range has that flag.  One update launch (plus the counters' increment in the capturable form), as the plain calls.
+ * ELD_E_ARG, nothing written and nothing launched: every refusal of the plain call, flag bits other than these three,
+ * a NULL vmax while some range has ELD_ADAM_AMSGRAD. */
+#define ELD_ADAM_AMSGRAD   1u
+#define ELD_ADAM_MAXIMIZE  2u
+#define ELD_ADAM_DECOUPLED 4u
+typedef struct {
+    size_t   offset, count;
+    int      step;
+    float    lr, beta1, beta2, eps, weight_decay;
+    unsigned flags;
+} eld_adam_range_ex;
+typedef struct {
+    size_t       offset, count;
+    int*         step;          /* device */
+    const float* lr;            /* device */
+    float        beta1, beta2, eps, weight_decay;
+    unsigned     flags;
+} eld_adam_range_dev_ex;
+int    eld_adam_step_ranges_ex(eld_ctx* ctx, float* params, const float* grads, float* m, float* v, float* vmax,
+                               const eld_adam_range_ex* ranges, int n_ranges, float grad_scale, void* stream);
+int    eld_adam_step_ranges_ex_capturable(eld_ctx* ctx, float* params, const float* grads, float* m, float* v,
+                                          float* vmax, const eld_adam_range_dev_ex* ranges, int n_ranges,
+                                          float grad_scale, void* stream);
 
 #endif
