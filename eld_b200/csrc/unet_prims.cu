@@ -372,10 +372,10 @@ int init_gemm_kernels(eld_ctx* ctx)
 }
 
 // the thin 3x3 weight gradients (cin, cout each 32 or 64) and the engine's deep ones (multiples of 64): one halo load per
-// pixel tile for all nine taps (wgrad_thin.cuh), in KC x NT channel blocks of at most 64 x 64 (the nine taps' f32
-// accumulators fill the consumers' registers at 64 x 64).  Grid = blocks x splits: each block gets the same number of
-// pixel-tile ranges, as many as fill one wave of CTAs (blocks are powers of two up to 64 in the U-Net: 128 to 132
-// CTAs), and no range is empty.
+// pixel tile for all nine taps (wgrad_thin.cuh), in KC x NT channel blocks of at most 64 x 64 (a 64 x 64 block's nine
+// taps take 96 f32 accumulators in each of three consumer warpgroups).  Grid = blocks x splits: each block gets the
+// same number of pixel-tile ranges, as many as fill one wave of CTAs (blocks are powers of two up to 64 in the U-Net:
+// 128 to 132 CTAs), and no range is empty.
 static int launch_wgrad_thin(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
 {
     // the [tap][ci][co] flush and the bias gradient add four contiguous floats at a time
@@ -403,7 +403,7 @@ static int launch_wgrad_thin(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)
     const int total_tiles = op.n_img * p.tiles_x * p.tiles_y;
     const int blocks = p.ci_blocks * p.co_blocks;
     p.splits = std::min(std::max(1, ctx->num_sms / blocks), total_tiles);
-    return launch(ctx, kWgradThin[nt / 64][kc / 64], blocks * p.splits, kWgThinThreads, smem, st, tmP, tmQ, p);
+    return launch(ctx, kWgradThin[nt / 64][kc / 64], blocks * p.splits, wgrad_thin_threads(nt), smem, st, tmP, tmQ, p);
 }
 
 int launch_wgrad(eld_ctx* ctx, const WgradOp& op, cudaStream_t st)

@@ -2,7 +2,7 @@
 // 64: one halo load per pixel tile for all nine taps, where the generic tile (wgrad_gemm.cuh) loads every pixel of X once
 // per filter tap.
 //
-//   D[(tap, ci) x co] (f32, registers)  =  sum over pixels p   X[p + tap shift, ci] * dZ[p, co]
+//   dW[tap][ci][co] (f32)  =  sum over pixels p   X[p + tap shift, ci] * dZ[p, co]
 //
 // blocks  = a CTA computes one KC x NT channel block (ci0 .. ci0 + KC - 1) x (co0 .. co0 + NT - 1) of the layer's
 //           (cin / KC) x (cout / NT) blocks; the thin layers (cin, cout in {32, 64}) are one block.
@@ -10,17 +10,22 @@
 //           tiles [s T / splits, (s + 1) T / splits) of the T 8 x 16 pixel tiles (a contiguous run, so vertically
 //           neighbouring halos meet in L2).  The CTAs resident together walk the same pixel range, so one halo / dZ tile
 //           read from HBM serves every channel block from L2.
-// P (X)   = the halo of each tile (tile.cuh), as the fprop thin tile loads it, at channel p_c0 + ci0.  Consumed MN-major:
-//           a tap starts a whole number of swizzle atoms into the slot (halo_tap_off), and k16 step k is tile row k.
-//           KC = 64: one tap = one m64 unit (9 units).  KC = 32: two taps share one m64 unit, the second 32 rows at the
-//           descriptor's LBO: (dy = -1, dx) + (0, dx) at LBO = 1 KB for each dx, (1, -1) + (1, 0)
-//           and (1, 0) + (1, 1) at LBO = one box (5 units; the first half of the last duplicates a tap and is dropped).
+// P (X)   = the halo of each tile (tile.cuh), as the fprop thin tile loads it, at channel p_c0 + ci0, MN-major: tap
+//           (dy, dx) starts a whole number of swizzle atoms into the slot (halo_tap_off), and k16 step k is tile row k.
 // Q (dZ)  = one {NT, 16, 8} box per tile at channel q_c0 + co0, MN-major.  Its column sums are the bias gradient, summed
 //           from shared memory while the MMAs run (by the ci-block-0 CTAs only).
-// roles   = warpgroup 0: TMA producer (one thread) | warpgroups 1, 2 consume every stage and split the m64 units
-//           (5 / 4 at KC = 64, 3 / 2 at KC = 32).  There is no per-tile epilogue: at the end each consumer adds its f32
-//           units into the gradient with vector red.global.add.  The 160 accumulator registers of (64 -> 64) need more
-//           than the 168 a 384-thread CTA gets evenly: setmaxnreg moves registers from the producer to the consumers.
+//
+// NT = 64 (every launch with a 64-wide cout block): D[co][(dx, ci)] with dZ as the M operand (64 co) and the three dx
+//           boxes of one filter row as one N = 3 KC operand (the descriptor's LBO = one halo box), so a tile is 3 rows x
+//           8 k16 steps of m64n192k16 (m64n96k16 at KC = 32).  Warpgroup 0: TMA producer (one thread); consumer
+//           warpgroups 1-3 own filter rows dy = -1, 0, 1, all three consume every stage.  After the last tile each
+//           consumer stages its 64 x 3 KC block transposed into the free slots and adds it along co with vector
+//           red.global.add.
+// NT = 32:  D[(tap, ci)][co] with the halo as the M operand.  KC = 64: one tap = one m64 unit (9 units).  KC = 32: two
+//           taps share one m64 unit, the second 32 rows at the descriptor's LBO: (dy = -1, dx) + (0, dx) at LBO = 1 KB
+//           for each dx, (1, -1) + (1, 0) and (1, 0) + (1, 1) at LBO = one box (5 units; the first half of the last
+//           duplicates a tap and is dropped).  Warpgroups 1, 2 consume every stage and split the m64 units (5 / 4 at
+//           KC = 64, 3 / 2 at KC = 32), and at the end add their f32 units into the gradient from the fragments.
 #pragma once
 #include "wgmma.cuh"
 #include "unet_prims.h"
@@ -42,9 +47,10 @@ struct WgradThinParams {
     float* db;                // optional: db[co] += sum over pixels of dZ
 };
 
-constexpr int kWgThinThreads = 384;
 constexpr int kWgThinProducerRegs = 40;
-constexpr int kWgThinConsumerRegs = 232;      // 128 x 40 + 256 x 232 <= 64 K registers
+constexpr int kWgThinConsumerRegs = 232;      // NT = 32: 128 x 40 + 256 x 232 <= 64 K registers
+constexpr int kWgRowsConsumerRegs = 152;      // NT = 64: 128 x 40 + 384 x 152 <= 64 K registers
+__host__ __device__ constexpr int wgrad_thin_threads(int nt) { return nt == 64 ? 512 : 384; }
 
 // bytes of one pipeline slot: the halo of X and the dZ box behind it
 __host__ __device__ constexpr int wgrad_thin_slot_bytes(int kc, int nt) { return halo_slot_bytes(kc) + 128 * nt * 2; }
@@ -71,12 +77,129 @@ __device__ __forceinline__ int wg_unit_tap(int u, int m)
     return u < 3 ? 3 * half + u : (u == 3 ? 6 + half : (half ? 8 : -1));
 }
 
-// One consumer warpgroup: units U0 .. U0 + NU - 1 of every stage, accumulated over the CTA's tiles, then flushed into
+// NT = 64: filter tap (kh * 3 + kw) of N atom `atom` (= dx + 1, one halo box) of filter row `row` (= dy + 1)
+__host__ __device__ constexpr int wg_row_tap(int row, int atom) { return 3 * row + atom; }
+
+// One consumer warpgroup of the NT = 64 tile: filter row `row` of every stage, D[co][(dx, ci)] accumulated over the
+// CTA's tiles, then staged through shared memory and flushed into channel block (ci0, co0) of the gradient.
+template <int KC>
+__device__ __forceinline__ void wgrad_rows_consume(const WgradThinParams& p, uint8_t* smem, uint64_t* full, uint64_t* empty,
+                                                   int ntiles, int row, int ci0, int co0)
+{
+    constexpr int NT = 64, N = 3 * KC;
+    constexpr int q_off = halo_slot_bytes(KC), slot_bytes = wgrad_thin_slot_bytes(KC, NT);   // dZ box / slot
+    constexpr int p_row = KC * 2, q_row = NT * 2;
+    constexpr uint32_t a_step = (16u * q_row) >> 4, b_step = (16u * p_row) >> 4;   // one k16 step = one tile row
+    // the staged block (below) of the three consumers fits in the two slots a launch has at least
+    static_assert(3 * N * NT * 4 <= 2 * slot_bytes, "the staged gradient does not fit in two slots");
+    const int bt = threadIdx.x & 127, lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+    const uint32_t smem_base = ptx::smem_u32(smem);
+    const uint64_t a_desc0 = ptx::make_gmma_desc(0, 0, 8u * q_row, ptx::gmma_layout(q_row));
+    const uint64_t b_desc0 = ptx::make_gmma_desc(0, (uint32_t)halo_box_bytes(KC), 8u * p_row, ptx::gmma_layout(p_row));
+    const uint32_t b_off = halo_tap_off(KC, wg_row_tap(row, 0));
+
+    // bias gradient: thread bt sums 16-byte chunk bc (8 columns) of the dZ rows br + 16 r, the three consumers taking
+    // r = row, row + 3, ... of the 8 row groups
+    const int bc = bt & 7, br = bt >> 3;
+    const uint32_t bswz = (uint32_t)(br & 7);
+    const bool bias_on = p.db != nullptr && ci0 == 0;     // one ci block sums db, or it would count cin / KC times
+    float bsum[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) bsum[i] = 0.f;
+
+    float acc[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+
+    int s = 0;
+    uint32_t ph = 0;
+    for (int i = 0; i < ntiles; ++i) {
+        ptx::mbar_wait(&full[s], ph);
+        const uint32_t st = smem_base + (uint32_t)(s * slot_bytes);
+        const uint64_t ad = ptx::desc_at(a_desc0, st + (uint32_t)q_off);
+        const uint64_t bd = ptx::desc_at(b_desc0, st + b_off);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+            ptx::wgmma_bf16<N, 1, 1>(acc, ad + (uint64_t)(k * a_step), bd + (uint64_t)(k * b_step), 1u);
+        ptx::wgmma_commit();
+        if (bias_on) {
+            const uint8_t* q = smem + (size_t)s * slot_bytes + q_off;
+            for (int r = row; r < 8; r += 3) {
+                const uint4 v = *reinterpret_cast<const uint4*>(q + (br + 16 * r) * q_row + (((uint32_t)bc ^ bswz) << 4));
+                const uint32_t w[4] = { v.x, v.y, v.z, v.w };
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    bsum[2 * j] += __uint_as_float(w[j] << 16);
+                    bsum[2 * j + 1] += __uint_as_float(w[j] & 0xFFFF0000u);
+                }
+            }
+        }
+        // release the stage as soon as its MMAs are done, not after the next stage has arrived: with two stages the
+        // producer would otherwise wait for that arrival before it could start the load after it (the other two
+        // consumers' MMAs keep the tensor cores busy meanwhile)
+        ptx::wgmma_wait<0>();
+        if (lane == 0) ptx::mbar_arrive(&empty[s]);
+        if (++s == p.stages) { s = 0; ph ^= 1u; }
+    }
+    ptx::reg_fence(acc);
+
+    if (bias_on) {
+        // lanes with the same chunk: lane % 8; fold them onto lanes 0 .. 7, one pair of float4 reds each
+#pragma unroll
+        for (int o = 8; o < 32; o <<= 1)
+#pragma unroll
+            for (int i = 0; i < 8; ++i) bsum[i] += __shfl_xor_sync(0xffffffffu, bsum[i], o);
+        if (lane < 8) {
+            float4* d = reinterpret_cast<float4*>(p.db + co0 + 8 * bc);
+            atomicAdd(d, make_float4(bsum[0], bsum[1], bsum[2], bsum[3]));
+            atomicAdd(d + 1, make_float4(bsum[4], bsum[5], bsum[6], bsum[7]));
+        }
+    }
+
+    // ===================== flush: registers -> shared memory (transposed) -> red.add into dW =====================
+    // Every consumer has read its last stage: the slots are free.  Consumer `row` stages T[n][co] (f32, n = (dx, ci))
+    // at its third of them, co XOR 8 ((n / 2) % 4) so that neither the fragment stores nor the float4 loads conflict.
+    ptx::bar_sync(1, 384);
+    float* T = reinterpret_cast<float*>(smem) + row * N * NT;
+    // fragment: lane holds D[16 wq + lane / 4 + 8 i][8 j + 2 (lane % 4) + c] in acc[4 j + 2 i + c]
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                const int n = 8 * j + 2 * (lane & 3) + c, co = 16 * wq + (lane >> 2) + 8 * i;
+                T[n * NT + (co ^ (8 * ((n >> 1) & 3)))] = acc[4 * j + 2 * i + c];
+            }
+    ptx::bar_sync(2 + row, 128);
+    // thread bt: four contiguous co (chunk bt % 16) of rows n = bt / 16 + 8 m
+    const int co = 4 * (bt & 15);
+#pragma unroll 4
+    for (int m = 0; m < N / 8; ++m) {
+        const int n = (bt >> 4) + 8 * m;
+        const float4 v = *reinterpret_cast<const float4*>(T + n * NT + (co ^ (8 * ((n >> 1) & 3))));
+        const int tap = wg_row_tap(row, n / KC), ci = ci0 + n % KC;
+        if (p.out_tco) {
+            atomicAdd(reinterpret_cast<float4*>(p.dw + ((size_t)tap * p.cin + ci) * p.cout + co0 + co), v);
+        } else {
+            float* d = p.dw + ((size_t)(co0 + co) * p.cin + ci) * 9 + tap;
+            const size_t cs = (size_t)p.cin * 9;
+            atomicAdd(d, v.x);
+            atomicAdd(d + cs, v.y);
+            atomicAdd(d + 2 * cs, v.z);
+            atomicAdd(d + 3 * cs, v.w);
+        }
+    }
+}
+
+// NT = 32: one consumer warpgroup: units U0 .. U0 + NU - 1 of every stage, accumulated over the CTA's tiles, then flushed into
 // channel block (ci0, co0) of the gradient.
 template <int NT, int KC, int U0, int NU>
 __device__ __forceinline__ void wgrad_thin_consume(const WgradThinParams& p, uint8_t* smem, uint64_t* full, uint64_t* empty,
                                                    int ntiles, int bt, int ci0, int co0)
 {
+    static_assert(NT == 32, "NT = 64 runs wgrad_rows_consume");
     constexpr int q_off = halo_slot_bytes(KC), slot_bytes = wgrad_thin_slot_bytes(KC, NT);   // dZ box / slot
     constexpr int p_row = KC * 2, q_row = NT * 2;
     constexpr uint32_t a_step = (16u * p_row) >> 4, b_step = (16u * q_row) >> 4;   // one k16 step = one tile row
@@ -91,7 +214,7 @@ __device__ __forceinline__ void wgrad_thin_consume(const WgradThinParams& p, uin
     // bias gradient: consumer thread bt sums 16-byte chunk bc (8 columns) of the dZ rows br, br + BR, ...
     constexpr int CH = NT / 8, BR = 256 / CH;
     const int bc = bt % CH, br = bt / CH;
-    const uint32_t bswz = NT == 64 ? (uint32_t)(br & 7) : (uint32_t)((br >> 1) & 3);   // BR is a multiple of 8
+    const uint32_t bswz = (uint32_t)((br >> 1) & 3);   // BR is a multiple of 8
     const bool bias_on = p.db != nullptr && ci0 == 0;     // one ci block sums db, or it would count cin / KC times
     float bsum[8];
 #pragma unroll
@@ -190,7 +313,7 @@ __device__ __forceinline__ void wgrad_thin_consume(const WgradThinParams& p, uin
 
 // NT x KC = the channel block (cout x cin of a thin layer), each 32 or 64
 template <int NT, int KC>
-__global__ void __launch_bounds__(kWgThinThreads, 1)
+__global__ void __launch_bounds__(wgrad_thin_threads(NT), 1)
 conv3x3_wgrad_thin_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmQ,
                           const WgradThinParams p)
 {
@@ -214,7 +337,8 @@ conv3x3_wgrad_thin_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_
     if (threadIdx.x == 0) {
         ptx::prefetch_tmap(&tmP);
         ptx::prefetch_tmap(&tmQ);
-        for (int s = 0; s < p.stages; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 8); }
+        // empty: one arrival per consumer warp
+        for (int s = 0; s < p.stages; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], wgrad_thin_threads(NT) / 32 - 4); }
         ptx::fence_barrier_init();
     }
     __syncthreads();
@@ -243,13 +367,17 @@ conv3x3_wgrad_thin_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_
         }
         return;
     }
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kWgThinConsumerRegs));
-
     // broadcast from lane 0: the compiler then knows cg to be warp-uniform (no wgmma serialisation)
     const int cg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7) - 1, 0);
-    const int bt = threadIdx.x - 128;
-    if (cg == 0) wgrad_thin_consume<NT, KC, 0, u_first>(p, smem, full, empty, t_end - t_begin, bt, ci0, co0);
-    else wgrad_thin_consume<NT, KC, u_first, units - u_first>(p, smem, full, empty, t_end - t_begin, bt, ci0, co0);
+    if constexpr (NT == 64) {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kWgRowsConsumerRegs));
+        wgrad_rows_consume<KC>(p, smem, full, empty, t_end - t_begin, cg, ci0, co0);
+    } else {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kWgThinConsumerRegs));
+        const int bt = threadIdx.x - 128;
+        if (cg == 0) wgrad_thin_consume<NT, KC, 0, u_first>(p, smem, full, empty, t_end - t_begin, bt, ci0, co0);
+        else wgrad_thin_consume<NT, KC, u_first, units - u_first>(p, smem, full, empty, t_end - t_begin, bt, ci0, co0);
+    }
 }
 
 }  // namespace eld
