@@ -52,6 +52,8 @@ def _declare(lib):
     lib.eld_noise_packed_aug.argtypes = [vp, vp, vp, vp, i32, i32, i32, c.POINTER(NoiseParams), u32, u64, u64, i32,
                                          c.POINTER(c.c_uint8), vp]
     lib.eld_eval_correct_psnr.argtypes = [vp, vp, vp, vp, i32, c.c_size_t, i32, vp, vp, vp, vp]
+    lib.eld_eval_srgb_psnr.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, c.POINTER(c.c_float), c.POINTER(c.c_float), i32,
+                                       vp, vp, vp, vp, vp]
     lib.eld_pair_ingest.argtypes = [vp, vp, i32, i32, vp, i32, i32, vp, vp, i32, i32, i32, c.POINTER(c.c_uint8), vp]
     lib.eld_noise_sample_params.argtypes = [vp, c.POINTER(CameraCalib), i32, i32, u64, u64, vp, i32, i32, vp, vp, vp]
     lib.eld_noise_packed_dev.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp, u32, u64, u64, vp, i32, vp, vp]

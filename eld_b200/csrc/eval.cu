@@ -8,7 +8,12 @@
 //   quality_assess -> skimage peak_signal_noise_ratio(data_range = 255) (util/index.py:76-79):
 //       PSNR = 10 log10(255^2 / mean((a - b)^2))
 // Three launches (two reductions + a finalise), double accumulation, no host synchronisation.
-#include "common.cuh"
+//
+// The sRGB metric (--stage_out raw --stage_eval srgb, ELD_model.py:226-233): output, target and input are rendered by
+// postprocess_bayer_v2 -> raw2rgb_postprocess -> `process` (util/process.py:51-68, gamma 2.2, no CRF) before tensor2im.
+// eval_srgb_kernel renders each packed pixel position of the three frames in registers with isp_render (the arithmetic
+// of isp_kernel, isp_pixel.cuh) and keeps only the squared errors: no rendered frame reaches memory.
+#include "isp_pixel.cuh"
 
 namespace eld {
 
@@ -84,6 +89,100 @@ __global__ void eval_finalize_kernel(const double* __restrict__ acc, size_t per_
     if (gain) gain[f] = correct ? (float)acc[f * 4 + 0] / (float)acc[f * 4 + 1] : 1.0f;
 }
 
+// the per-frame table of one eval_srgb_kernel launch: frames f0 .. f0 + gridDim.y - 1
+struct SrgbEvalLaunch {
+    IspFrame fr[kIspMaxFrames];
+    float inv_gamma;
+    int f0;
+    int h, w;
+};
+
+__device__ __forceinline__ double srgb_sq(const float (&a)[3], const float (&b)[3])      // tensor2im on both, then (a - b)^2
+{
+    double s = 0.0;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const double d = (double)clamp_nan(a[c] * 255.0f, 0.0f, 255.0f) - (double)clamp_nan(b[c] * 255.0f, 0.0f, 255.0f);
+        s += d * d;
+    }
+    return s;
+}
+
+// x = gain * clamp(pred) (correct) or pred, written to `out` if out != NULL; acc[f][2] += sum over the rendered pixels
+// of (tensor2im(render(x)) - tensor2im(render(target)))^2, acc[f][3] the same for input (if input != NULL)
+template <bool VEC>
+__global__ void __launch_bounds__(256)
+eval_srgb_kernel(const float* __restrict__ pred, const float* __restrict__ target, const float* __restrict__ input,
+                 float* __restrict__ out, int correct, double* __restrict__ acc, const __grid_constant__ SrgbEvalLaunch L)
+{
+    __shared__ double sh[8];
+    constexpr int K = VEC ? 4 : 1;
+    const int crf_len = 0;                                        // raw2rgb_postprocess passes no CRF
+    const int f = L.f0 + blockIdx.y;
+    const IspFrame& F = L.fr[blockIdx.y];
+    const size_t plane = (size_t)L.h * L.w;
+    const size_t frame = (size_t)f * 4 * plane;
+    // the reference forms num / den in fp32 (torch.dot) and multiplies in fp32, as eval_apply_kernel
+    const float gain = correct ? (float)acc[f * 4 + 0] / (float)acc[f * 4 + 1] : 1.0f;
+    double sq = 0.0, sq_in = 0.0;
+    for (size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x; t * K < plane; t += (size_t)gridDim.x * blockDim.x) {
+        const size_t at = frame + t * K;
+        float x[4][K], s[4][K], u[4][K];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            if (VEC) {
+                const float4 a = __ldg(reinterpret_cast<const float4*>(pred + at + c * plane));
+                const float4 b = __ldg(reinterpret_cast<const float4*>(target + at + c * plane));
+                x[c][0] = a.x; x[c][1] = a.y; x[c][2] = a.z; x[c][3] = a.w;
+                s[c][0] = b.x; s[c][1] = b.y; s[c][2] = b.z; s[c][3] = b.w;
+                if (input) {
+                    const float4 d = __ldg(reinterpret_cast<const float4*>(input + at + c * plane));
+                    u[c][0] = d.x; u[c][1] = d.y; u[c][2] = d.z; u[c][3] = d.w;
+                }
+            } else {
+                x[c][0] = __ldg(pred + at + c * plane);
+                s[c][0] = __ldg(target + at + c * plane);
+                if (input) u[c][0] = __ldg(input + at + c * plane);
+            }
+#pragma unroll
+            for (int k = 0; k < K; ++k)
+                if (correct) x[c][k] = gain * clamp_nan(x[c][k], 0.0f, 1.0f);
+            if (out) {
+                if (VEC) *reinterpret_cast<float4*>(out + at + c * plane) = make_float4(x[c][0], x[c][1], x[c][2], x[c][3]);
+                else out[at + c * plane] = x[c][0];
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+            float ro[3], rt[3];
+            isp_render(x[0][k], x[1][k], x[2][k], x[3][k], F, L.inv_gamma, crf_len, nullptr, nullptr, ro);
+            isp_render(s[0][k], s[1][k], s[2][k], s[3][k], F, L.inv_gamma, crf_len, nullptr, nullptr, rt);
+            sq += srgb_sq(ro, rt);
+            if (input) {
+                float ri[3];
+                isp_render(u[0][k], u[1][k], u[2][k], u[3][k], F, L.inv_gamma, crf_len, nullptr, nullptr, ri);
+                sq_in += srgb_sq(ri, rt);
+            }
+        }
+    }
+    const double a = block_sum(sq, sh);
+    const double b = block_sum(sq_in, sh);
+    if (threadIdx.x == 0) {
+        atomicAdd(acc + f * 4 + 2, a);
+        if (input) atomicAdd(acc + f * 4 + 3, b);
+    }
+}
+
+__global__ void eval_srgb_finalize_kernel(const double* __restrict__ acc, size_t count, int n, int correct,
+                                          float* __restrict__ psnr, float* __restrict__ psnr_in, float* __restrict__ gain)
+{
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n) return;
+    psnr[f] = (float)(10.0 * log10(255.0 * 255.0 / (acc[f * 4 + 2] / (double)count)));
+    if (psnr_in) psnr_in[f] = (float)(10.0 * log10(255.0 * 255.0 / (acc[f * 4 + 3] / (double)count)));
+    if (gain) gain[f] = correct ? (float)acc[f * 4 + 0] / (float)acc[f * 4 + 1] : 1.0f;
+}
+
 }  // namespace eld
 
 using namespace eld;
@@ -115,5 +214,74 @@ extern "C" int eld_eval_correct_psnr(eld_ctx* ctx, const float* pred, const floa
     eval_finalize_kernel<<<(n + 63) / 64, 64, 0, st>>>(scratch, per_frame, n, correct, psnr, gain);
     ELD_CHECK_CUDA(cudaGetLastError());
     count_launch(ctx, 2);
+    return ELD_OK;
+}
+
+extern "C" int eld_eval_srgb_psnr(eld_ctx* ctx, const float* pred, const float* target, const float* input, float* out,
+                                  int n, int h, int w, const float* wb, const float* ccm, int correct, double* scratch,
+                                  float* psnr, float* psnr_in, float* gain, void* stream)
+{
+    ELD_REQUIRE(ctx && pred && target && wb && ccm && scratch && psnr, "eld_eval_srgb_psnr: NULL argument");
+    ELD_REQUIRE(!input == !psnr_in, "eld_eval_srgb_psnr: input and psnr_in go together");
+    ELD_REQUIRE(n > 0 && n <= 65535, "eld_eval_srgb_psnr: %d frames (1 to 65535, one grid row each)", n);
+    ELD_REQUIRE(h > 0 && w > 0, "eld_eval_srgb_psnr: empty frame %d x %d", h, w);
+    const size_t plane = (size_t)h * w;
+    const size_t frames = (size_t)n * 4 * plane * sizeof(float);
+    const void* ins[3] = {pred, target, input};
+    const void* outs[5] = {out, scratch, psnr, psnr_in, gain};
+    const size_t out_bytes[5] = {frames, (size_t)n * 4 * sizeof(double), n * sizeof(float), n * sizeof(float),
+                                 n * sizeof(float)};
+    // the outputs are written while other blocks still read the frames: only the element-for-element out == pred is safe
+    for (int i = 0; i < 3; ++i)
+        for (int o = 0; o < 5; ++o)
+            ELD_REQUIRE(!ins[i] || !outs[o] || (i == 0 && o == 0 && out == pred) ||
+                        !ranges_overlap(ins[i], frames, outs[o], out_bytes[o]),
+                        "eld_eval_srgb_psnr: an output overlaps %s", i == 0 ? "pred" : i == 1 ? "target" : "input");
+    for (int o = 0; o < 5; ++o)
+        for (int p = o + 1; p < 5; ++p)
+            ELD_REQUIRE(!outs[o] || !outs[p] || !ranges_overlap(outs[o], out_bytes[o], outs[p], out_bytes[p]),
+                        "eld_eval_srgb_psnr: two outputs overlap");
+    ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    ELD_CHECK_CUDA(cudaMemsetAsync(scratch, 0, (size_t)n * 4 * sizeof(double), st));
+    if (correct) {                               // the gain of eld_eval_correct_psnr: the same reduction on the same grid
+        const size_t per_frame = 4 * plane;
+        int bx = (int)((per_frame + 256 * 8 - 1) / (256 * 8));
+        const int cap = (4 * ctx->num_sms + n - 1) / n;
+        if (bx > cap) bx = cap;
+        if (bx < 1) bx = 1;
+        eval_dots_kernel<<<dim3((unsigned)bx, (unsigned)n), 256, 0, st>>>(pred, target, per_frame, scratch);
+        ELD_CHECK_CUDA(cudaGetLastError());
+        count_launch(ctx);
+    }
+    const uintptr_t addr = reinterpret_cast<uintptr_t>(pred) | reinterpret_cast<uintptr_t>(target) |
+                           reinterpret_cast<uintptr_t>(input) | reinterpret_cast<uintptr_t>(out);
+    const bool vec = plane % 4 == 0 && addr % 16 == 0;
+    const size_t items = vec ? plane / 4 : plane;
+    int per_sm = 0;
+    if (vec) ELD_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, eval_srgb_kernel<true>, 256, 0));
+    else     ELD_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, eval_srgb_kernel<false>, 256, 0));
+    if (per_sm < 1) per_sm = 1;
+    for (int f0 = 0; f0 < n; f0 += kIspMaxFrames) {
+        const int nf = n - f0 < kIspMaxFrames ? n - f0 : kIspMaxFrames;
+        SrgbEvalLaunch L{};
+        for (int f = 0; f < nf; ++f) {
+            for (int i = 0; i < 4; ++i) L.fr[f].wb[i] = wb[(size_t)(f0 + f) * 4 + i];
+            for (int i = 0; i < 9; ++i) L.fr[f].ccm[i] = ccm[(size_t)(f0 + f) * 9 + i];
+        }
+        L.inv_gamma = 1.0f / 2.2f;               // gamma_compression's default, as eld_isp_process forms it from gamma
+        L.f0 = f0; L.h = h; L.w = w;
+        int bx = (int)((items + 255) / 256);
+        const int cap = (per_sm * ctx->num_sms + nf - 1) / nf;        // one wave of resident blocks over the launch
+        if (bx > cap) bx = cap;
+        const dim3 grid((unsigned)bx, (unsigned)nf);
+        if (vec) eval_srgb_kernel<true><<<grid, 256, 0, st>>>(pred, target, input, out, correct, scratch, L);
+        else     eval_srgb_kernel<false><<<grid, 256, 0, st>>>(pred, target, input, out, correct, scratch, L);
+        ELD_CHECK_CUDA(cudaGetLastError());
+        count_launch(ctx);
+    }
+    eval_srgb_finalize_kernel<<<(n + 63) / 64, 64, 0, st>>>(scratch, 3 * plane, n, correct, psnr, psnr_in, gain);
+    ELD_CHECK_CUDA(cudaGetLastError());
+    count_launch(ctx);
     return ELD_OK;
 }

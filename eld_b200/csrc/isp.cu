@@ -4,48 +4,17 @@
 // Replaces util/process.py:41-68 `process` (apply_gains :15-19, binning :41-48, apply_ccms :22-31,
 // gamma_compression :34-39, camera_response_function :71-84) and the two clips of ISPDataset.__getitem__
 // (dataset/sid_dataset.py:309,311).  HBM-bound: 16 B in + 12 B out per packed pixel position.
-// The arithmetic keeps torch's CPU operation order (separate fp32 multiplies, no FMA contraction, the 3-term colour
-// sum in a double accumulator) so that only pow / the interpolation differ from the reference by rounding.
-#include "common.cuh"
+// The per-pixel arithmetic is isp_render (isp_pixel.cuh), which the sRGB eval metric (eval.cu) runs too.
+#include "isp_pixel.cuh"
 
 namespace eld {
 
-constexpr int kIspMaxFrames = 48;
-
-struct IspFrame { float wb[4]; float ccm[9]; float pad[3]; };   // 64 bytes
 struct IspLaunch {
     IspFrame fr[kIspMaxFrames];
     float inv_gamma;
     int crf_len;            // 0: gamma curve
     int h, w;
 };
-
-// torch.clamp keeps NaN (process.py:56,61); a NaN then reaches the `.int()` of :38 / :83, whose INT_MIN the final clamp
-// turns into 0 - so a NaN in any of a pixel's four packed values makes all three of its outputs 0, here as there
-__device__ __forceinline__ float clamp01(float x) { return clamp_nan(x, 0.0f, 1.0f); }
-
-// torchinterp1d.Interp1d semantics: ind = clamp(searchsorted(x, v) - 1, 0, L-2); y[ind] + slope[ind] * (v - x[ind]),
-// slope = (y[i+1] - y[i]) / (eps + x[i+1] - x[i])
-__device__ __forceinline__ float crf_lookup(const float* __restrict__ E, const float* __restrict__ f, int L, float v)
-{
-    int lo = 0, hi = L;                                   // first index with E[idx] >= v  (searchsorted, side='left')
-    while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(E + mid) < v) lo = mid + 1; else hi = mid;
-    }
-    int ind = lo - 1;
-    ind = ind < 0 ? 0 : (ind > L - 2 ? L - 2 : ind);
-    const float x0 = __ldg(E + ind), x1 = __ldg(E + ind + 1), y0 = __ldg(f + ind), y1 = __ldg(f + ind + 1);
-    const float slope = __fdiv_rn(__fadd_rn(y1, -y0), __fadd_rn(1.1920929e-07f, __fadd_rn(x1, -x0)));
-    return __fadd_rn(y0, __fmul_rn(slope, __fadd_rn(v, -x0)));
-}
-
-__device__ __forceinline__ float quant8(float v)          // clamp((v*255).int(), 0, 255).float() / 255
-{
-    int q = (int)__fmul_rn(v, 255.0f);                    // truncation toward zero, like Tensor.int(); NaN -> 0
-    q = q < 0 ? 0 : (q > 255 ? 255 : q);
-    return __fdiv_rn((float)q, 255.0f);
-}
 
 template <bool VEC>
 __global__ void __launch_bounds__(256)
@@ -74,22 +43,10 @@ isp_kernel(const float* __restrict__ packed, float* __restrict__ rgb, const __gr
     float out[3][4];
 #pragma unroll
     for (int k = 0; k < (VEC ? 4 : 1); ++k) {
-        // white balance (process.py:15-19), clip (:56), RGBG -> RGB binning (:41-48)
-        const float r = clamp01(__fmul_rn(in[0][k], F.wb[0]));
-        const float g1 = clamp01(__fmul_rn(in[1][k], F.wb[1]));
-        const float b = clamp01(__fmul_rn(in[2][k], F.wb[2]));
-        const float g2 = clamp01(__fmul_rn(in[3][k], F.wb[3]));
-        const float g = __fmul_rn(__fadd_rn(g1, g2), 0.5f);
+        float px[3];
+        isp_render(in[0][k], in[1][k], in[2][k], in[3][k], F, L.inv_gamma, L.crf_len, crf_E, crf_f, px);
 #pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            // colour correction (:22-31): fp32 products, the three terms summed in a double accumulator and rounded once -
-            // what torch's CPU reduction does (pinned by tests/golden/isp_kat.npz, saturated pixels included)
-            float v = (float)(((double)__fmul_rn(r, F.ccm[3 * c]) + (double)__fmul_rn(g, F.ccm[3 * c + 1])) + (double)__fmul_rn(b, F.ccm[3 * c + 2]));
-            v = clamp01(v);                                               // :61
-            if (L.crf_len > 0) v = crf_lookup(crf_E, crf_f + (size_t)c * L.crf_len, L.crf_len, v);   // :71-84
-            else v = powf(fmax_nan(v, 1e-8f), L.inv_gamma);                // :34-36
-            out[c][k] = clamp01(quant8(v));                               // :38 / :83, ISPDataset's clip (sid_dataset.py:311)
-        }
+        for (int c = 0; c < 3; ++c) out[c][k] = px[c];
     }
     if (VEC) {
 #pragma unroll

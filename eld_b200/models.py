@@ -37,7 +37,7 @@ def default_opt(**kw):
              beta1=0.9, wd=0.0, loss='l1', noise='g', isTrain=True, save_epoch_freq=100, noise_on_gpu=False,
              augment_on_gpu=False, defer_loss_sync=False, prefetch_noise=False, num_burst=1, pairs_on_gpu=False,
              cuda_graph=False, accum_steps=1, params_on_gpu=False, amsgrad=False,
-             decoupled_weight_decay=False)
+             decoupled_weight_decay=False, stage_eval='raw')
     o.update(kw)
     return SimpleNamespace(**o)
 
@@ -538,6 +538,54 @@ class ELDModel(BaseModel):
             ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), 'eld_eval_correct_psnr')
         return out, psnr, gain
 
+    def eval_metrics_srgb(self, predict, target, input, wb, ccm, correct=False):
+        """eval_metrics in sRGB (ELD_model.py:226-233, --stage_eval srgb): the corrected prediction (or the prediction),
+        the target and the input are rendered with each frame's white balance wb [n, 4] and cam2rgb ccm [n, 3, 3]
+        (raw2rgb_postprocess: util/process.py `process`, gamma 2.2) and compared after tensor2im, all in one pass on the
+        device that keeps the renders in registers (csrc/eval.cu, eld_eval_srgb_psnr).  predict, target, input: packed
+        [n, 4, h, w]; a target (or wb / ccm) of one frame serves every frame; input may be None.  Returns (output,
+        psnr[n], psnr_input[n] or None, gain[n]) - output is the corrected raw prediction when correct=True, else
+        `predict` itself.  A NaN in a pixel renders it black, as the reference's `process` does, so the PSNR stays
+        finite where eval_metrics' is NaN."""
+        from . import _lib
+        predict = predict.contiguous()
+        n, c, h, w = predict.shape
+        if c != 4:
+            raise ValueError('eval_metrics_srgb renders packed RGBG frames [n, 4, h, w]; got %s' % (tuple(predict.shape),))
+
+        def frames(t):
+            t = t.to(device=predict.device, dtype=torch.float32)
+            if t.shape[0] == 1 and n != 1:
+                t = t.expand(n, *t.shape[1:])               # IlluminanceCorrect.forward's broadcast case (:147-149)
+            if tuple(t.shape) != (n, c, h, w):
+                raise ValueError('expected frames of shape %s, got %s' % ((n, c, h, w), tuple(t.shape)))
+            return t.contiguous()
+
+        def table(a, k):
+            a = np.asarray(a.detach().cpu().numpy() if hasattr(a, 'detach') else a, dtype=np.float32).reshape(-1, k)
+            if a.shape[0] == 1 and n != 1:
+                a = np.repeat(a, n, axis=0)
+            if a.shape[0] != n:
+                raise ValueError('expected %d rows of %d values, got %d' % (n, k, a.shape[0]))
+            return np.ascontiguousarray(a)
+
+        target = frames(target)
+        input = frames(input) if input is not None else None
+        wb, ccm = table(wb, 4), table(ccm, 9)
+        out = torch.empty_like(predict) if correct else predict
+        scratch = torch.empty(n * 4, dtype=torch.float64, device=predict.device)
+        psnr = torch.empty(n, dtype=torch.float32, device=predict.device)
+        psnr_in = torch.empty(n, dtype=torch.float32, device=predict.device) if input is not None else None
+        gain = torch.empty(n, dtype=torch.float32, device=predict.device)
+        fp = ctypes.POINTER(ctypes.c_float)
+        _lib.check(_lib.load().eld_eval_srgb_psnr(
+            _lib.ctx(predict.device.index or 0), predict.data_ptr(), target.data_ptr(),
+            input.data_ptr() if input is not None else None, out.data_ptr() if correct else None, n, h, w,
+            wb.ctypes.data_as(fp), ccm.ctypes.data_as(fp), int(bool(correct)), scratch.data_ptr(), psnr.data_ptr(),
+            psnr_in.data_ptr() if psnr_in is not None else None, gain.data_ptr(),
+            ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), 'eld_eval_srgb_psnr')
+        return out, psnr, psnr_in, gain
+
     def illuminance_correct(self, predict, source):
         return self.eval_metrics(predict, source, correct=True)[0]
 
@@ -545,7 +593,18 @@ class ELDModel(BaseModel):
         """ELDModelBase.eval (ELD_model.py:203-243) without the rawpy / PIL visualisation: centre 512x512 crop
         (util.crop_center), forward (or forward_chop), optional illuminance correction, PSNR of the output and of the
         input against the target exactly as tensor2im + quality_assess compute them - all on the device (csrc/eval.cu);
-        one host read of the final scalars.  Only the 1st frame is assessed, like the reference (tensor2im takes [0])."""
+        one host read of the final scalars.  Only the 1st frame is assessed, like the reference (tensor2im takes [0]).
+        opt.stage_eval == 'srgb' with opt.stage_out == 'raw' (ELD_model.py:226-233): output, input and target are
+        compared in sRGB, rendered with the batch's 'wb' [n, 4] and 'ccm' [n, 3, 3] (the reference reads them from the
+        target's RAW file: process.read_wb_ccm) - eval_metrics_srgb.  self.output stays the corrected raw output."""
+        srgb = self.opt.stage_out == 'raw' and getattr(self.opt, 'stage_eval', 'raw') == 'srgb'
+        if srgb:
+            if self.opt.stage_in == 'srgb':
+                raise NotImplementedError("stage_eval 'srgb' with stage_in 'srgb': the reference renders the input as a "
+                                          "4-channel raw frame (process.apply_gains) and cannot render a 3-channel one")
+            if 'wb' not in data or 'ccm' not in data:
+                raise ValueError("stage_eval 'srgb' renders with each frame's white balance and colour matrix: the batch "
+                                 "needs the keys 'wb' [n, 4] and 'ccm' [n, 3, 3]")
         self._eval()
         self.set_input(data, 'eval')
         with torch.no_grad():
@@ -555,8 +614,12 @@ class ELDModel(BaseModel):
                 y0, x0 = h // 2 - 256, w // 2 - 256                     # util.crop_center
                 x, t = x[:, :, y0:y0 + 512, x0:x0 + 512].contiguous(), t[:, :, y0:y0 + 512, x0:x0 + 512].contiguous()
             out = self.forward_chop(x) if self.opt.chop else self._padded_forward(x)
-            out, psnr, _ = self.eval_metrics(out.contiguous(), t, correct=correct)
-            _, psnr_in, _ = self.eval_metrics(x, t, correct=False)
+            if srgb:
+                out, psnr, psnr_in, _ = self.eval_metrics_srgb(out.contiguous(), t, x, data['wb'], data['ccm'],
+                                                               correct=correct)
+            else:
+                out, psnr, _ = self.eval_metrics(out.contiguous(), t, correct=correct)
+                _, psnr_in, _ = self.eval_metrics(x, t, correct=False)
             self.output = out
             both = torch.stack([psnr[0], psnr_in[0]]).cpu()
         return {'PSNR': float(both[0]), 'PSNR_input': float(both[1])}

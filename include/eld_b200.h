@@ -234,6 +234,30 @@ int eld_isp_process(eld_ctx* ctx, const float* packed, float* rgb, int n, int h,
 int eld_eval_correct_psnr(eld_ctx* ctx, const float* pred, const float* target, float* out, int n, size_t per_frame,
                           int correct, double* scratch, float* psnr, float* gain, void* stream);
 
+/* The same metric in sRGB: ELDModelBase.eval with --stage_out raw --stage_eval srgb (models/ELD_model.py:226-233), which
+ * renders output, target and input with postprocess_bayer_v2 -> raw2rgb_postprocess (util/process.py:116-126) before
+ * tensor2im.  Per frame f of n packed frames pred, target and input (device f32 [n][4][h][w], RGBG planes):
+ *   x = gain * clamp(pred, 0, 1) with eld_eval_correct_psnr's gain (the same reduction, so the same value) if
+ *       correct != 0, else x = pred; written to `out` (device f32 [n][4][h][w]) if out != NULL
+ *   R(.) = eld_isp_process's render with wb[f], ccm[f] and gamma 2.2, no CRF: three 8-bit levels / 255 per position
+ *   psnr[f]    = 10 log10(255^2 / mean((clip(255 R(x),0,255)   - clip(255 R(target),0,255))^2))
+ *   psnr_in[f] = 10 log10(255^2 / mean((clip(255 R(input),0,255) - clip(255 R(target),0,255))^2))   (input != NULL)
+ *   gain[f] (may be NULL) as eld_eval_correct_psnr writes it; the means are over the 3 h w rendered values.
+ * The renders stay in registers: one pass reads pred, target and input once (48 B per packed pixel position, 16 B
+ * more to write `out`, 32 B more for the gain's reduction when correct != 0).
+ * NaN as in the reference, and unlike eld_eval_correct_psnr: a NaN in any of a pixel's four packed values renders all
+ * three of its sRGB values 0 (eld_isp_process's rule), so a NaN prediction or a NaN gain (an empty correction mask)
+ * still gives a finite PSNR, as process + tensor2im do; gain[f] is then NaN.  Equal renders give PSNR +inf.
+ * wb: HOST [n][4], ccm: HOST [n][9] cam2rgb row-major (as eld_isp_process).  scratch: device, n * 4 doubles (zeroed
+ * here).  psnr, psnr_in: device f32 [n].  Launches: the gain's reduction (correct != 0), one render pass per 48 frames,
+ * one finalise.  No host synchronisation, no allocation.
+ * ELD_E_ARG, nothing written: a NULL ctx / pred / target / wb / ccm / scratch / psnr, input and psnr_in not both given or
+ * both NULL, n == 0 or n > 65535, h <= 0 or w <= 0, pred / target / input overlapping an output (out == pred is allowed),
+ * two outputs overlapping. */
+int eld_eval_srgb_psnr(eld_ctx* ctx, const float* pred, const float* target, const float* input, float* out,
+                       int n, int h, int w, const float* wb, const float* ccm, int correct, double* scratch,
+                       float* psnr, float* psnr_in, float* gain, void* stream);
+
 /* Number of kernels the library has launched through this ctx since creation (bench.py's
  * gpu_launches evidence). */
 int64_t eld_launch_count(const eld_ctx* ctx);
