@@ -54,6 +54,10 @@ def _declare(lib):
     lib.eld_eval_correct_psnr.argtypes = [vp, vp, vp, vp, i32, c.c_size_t, i32, vp, vp, vp, vp]
     lib.eld_eval_srgb_psnr.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, c.POINTER(c.c_float), c.POINTER(c.c_float), i32,
                                        vp, vp, vp, vp, vp]
+    lib.eld_eval_ssim_scratch_bytes.argtypes = [i32, i32, i32]
+    lib.eld_eval_ssim_scratch_bytes.restype = c.c_size_t
+    lib.eld_eval_ssim.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, vp, c.POINTER(c.c_float), c.POINTER(c.c_float), vp,
+                                  c.c_size_t, vp, vp, vp]
     lib.eld_pair_ingest.argtypes = [vp, vp, i32, i32, vp, i32, i32, vp, vp, i32, i32, i32, c.POINTER(c.c_uint8), vp]
     lib.eld_noise_sample_params.argtypes = [vp, c.POINTER(CameraCalib), i32, i32, u64, u64, vp, i32, i32, vp, vp, vp]
     lib.eld_noise_packed_dev.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp, u32, u64, u64, vp, i32, vp, vp]

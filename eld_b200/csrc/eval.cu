@@ -89,7 +89,7 @@ __global__ void eval_finalize_kernel(const double* __restrict__ acc, size_t per_
     if (gain) gain[f] = correct ? (float)acc[f * 4 + 0] / (float)acc[f * 4 + 1] : 1.0f;
 }
 
-// the per-frame table of one eval_srgb_kernel launch: frames f0 .. f0 + gridDim.y - 1
+// the per-frame table of one eval_srgb_kernel or eval_ssim_kernel<true, *> launch: frames f0 .. f0 + gridDim.y - 1
 struct SrgbEvalLaunch {
     IspFrame fr[kIspMaxFrames];
     float inv_gamma;
@@ -181,6 +181,203 @@ __global__ void eval_srgb_finalize_kernel(const double* __restrict__ acc, size_t
     psnr[f] = (float)(10.0 * log10(255.0 * 255.0 / (acc[f * 4 + 2] / (double)count)));
     if (psnr_in) psnr_in[f] = (float)(10.0 * log10(255.0 * 255.0 / (acc[f * 4 + 3] / (double)count)));
     if (gain) gain[f] = correct ? (float)acc[f * 4 + 0] / (float)acc[f * 4 + 1] : 1.0f;
+}
+
+// SSIM (util/index.py:80 -> skimage structural_similarity(Y, X, data_range=255, multichannel=True), default arguments):
+// per channel, on the tensor2im values in float64, the 7 x 7 uniform window means ux, uy, uxx, uyy, uxy, then
+//   vx = cov_norm (uxx - ux^2), vy likewise, vxy = cov_norm (uxy - ux uy), cov_norm = 49 / 48,
+//   S = (2 ux uy + C1)(2 vxy + C2) / ((ux^2 + uy^2 + C1)(vx + vy + C2)),  C1 = (0.01 * 255)^2, C2 = (0.03 * 255)^2,
+// averaged over the map without its 3-pixel border (every window inside the frame, so the filter's border mode never
+// matters), then over the channels.  A CTA takes kSsimTW x kSsimTH map positions (kSsimTW x kSsimTH windows whose
+// top-left corner is the position), stages the tensor2im values of their (kSsimTW + 6) x (kSsimTH + 6) pixels once in
+// shared memory as doubles, sums the moments along rows (7 taps) into shared memory and then along columns, and writes
+// its sum of S to its own scratch slot; eval_ssim_finalize_kernel adds a frame's slots in a fixed order, so the result
+// does not depend on scheduling.
+constexpr int kSsimTW = 32, kSsimTH = 16, kSsimWin = 7;
+constexpr int kSsimIW = kSsimTW + kSsimWin - 1, kSsimIH = kSsimTH + kSsimWin - 1, kSsimPix = kSsimIW * kSsimIH;
+constexpr int kSsimThreads = 256;
+static_assert(kSsimThreads == kSsimTW * kSsimTH / 2, "eval_ssim_kernel: one thread per column and pair of rows");
+
+// images staged per channel (estimate, target, input) and moments per position (sums of x, y, xx, yy, xy, then u, uu, uy)
+template <bool INPUT> struct SsimShape { static constexpr int images = INPUT ? 3 : 2, moments = INPUT ? 8 : 5; };
+
+template <bool SRGB, bool INPUT>
+constexpr size_t ssim_smem_bytes()
+{
+    return sizeof(double) * ((SRGB ? 3 : 1) * SsimShape<INPUT>::images * kSsimPix + SsimShape<INPUT>::moments * kSsimIH * kSsimTW);
+}
+
+__device__ __forceinline__ float t2im(float v) { return clamp_nan(v * 255.0f, 0.0f, 255.0f); }
+
+// S from the window sums, in numpy's operation order (no contraction), so equal images give exactly 1
+__device__ __forceinline__ double ssim_map(double sx, double sy, double sxx, double syy, double sxy)
+{
+    constexpr double inv = 1.0 / 49.0, cov = 49.0 / 48.0;
+    constexpr double C1 = (0.01 * 255.0) * (0.01 * 255.0), C2 = (0.03 * 255.0) * (0.03 * 255.0);
+    const double ux = __dmul_rn(sx, inv), uy = __dmul_rn(sy, inv);
+    const double uxx = __dmul_rn(sxx, inv), uyy = __dmul_rn(syy, inv), uxy = __dmul_rn(sxy, inv);
+    const double vx = __dmul_rn(cov, __dsub_rn(uxx, __dmul_rn(ux, ux)));
+    const double vy = __dmul_rn(cov, __dsub_rn(uyy, __dmul_rn(uy, uy)));
+    const double vxy = __dmul_rn(cov, __dsub_rn(uxy, __dmul_rn(ux, uy)));
+    const double a1 = __dadd_rn(__dmul_rn(__dmul_rn(2.0, ux), uy), C1), a2 = __dadd_rn(__dmul_rn(2.0, vxy), C2);
+    const double b1 = __dadd_rn(__dadd_rn(__dmul_rn(ux, ux), __dmul_rn(uy, uy)), C1);
+    const double b2 = __dadd_rn(__dadd_rn(vx, vy), C2);
+    return __dmul_rn(a1, a2) / __dmul_rn(b1, b2);
+}
+
+// grid = (tiles_y * tiles_x, frames of the launch); scratch[(f * tiles + tile) * 2 + {0, 1}] = the tile's sum of S over
+// its map positions and channels for (estimate, target) and (input, target).  x = gain[f] * clamp(pred, 0, 1) when
+// gain != NULL, else pred.  SRGB: the c = 4 packed planes rendered by isp_render (3 channels) before tensor2im.
+template <bool SRGB, bool INPUT>
+__global__ void __launch_bounds__(kSsimThreads)
+eval_ssim_kernel(const float* __restrict__ pred, const float* __restrict__ target, const float* __restrict__ input,
+                 const float* __restrict__ gain, int c, int tiles_x, double* __restrict__ scratch,
+                 const __grid_constant__ SrgbEvalLaunch L)
+{
+    constexpr int NI = SsimShape<INPUT>::images, NM = SsimShape<INPUT>::moments;
+    constexpr int NS = SRGB ? 3 : 1;                              // channels staged at once: a render yields all three
+    extern __shared__ double smem[];
+    double* const stg = smem;                                     // [NS][NI][kSsimIH][kSsimIW]
+    double* const hs = smem + NS * NI * kSsimPix;                 // [NM][kSsimIH][kSsimTW]: the row sums
+    __shared__ double sh[8];
+    const int crf_len = 0;
+    const int fl = blockIdx.y, f = L.f0 + fl;
+    const int h = L.h, w = L.w;
+    const int oy0 = (int)(blockIdx.x / tiles_x) * kSsimTH, ox0 = (int)(blockIdx.x % tiles_x) * kSsimTW;
+    const size_t plane = (size_t)h * w;
+    const size_t frame = (size_t)f * c * plane;
+    const bool corr = gain != nullptr;
+    const float g = corr ? __ldg(gain + f) : 1.0f;
+    const int lane = threadIdx.x & 31, r0 = 2 * (threadIdx.x >> 5);
+    const bool valid0 = ox0 + lane < w - (kSsimWin - 1) && oy0 + r0 < h - (kSsimWin - 1);
+    const bool valid1 = ox0 + lane < w - (kSsimWin - 1) && oy0 + r0 + 1 < h - (kSsimWin - 1);
+    double acc = 0.0, acc_in = 0.0;
+    for (int ch = 0; ch < (SRGB ? 3 : c); ++ch) {
+        __syncthreads();                                          // the previous channel's passes are done with stg, hs
+        if (!SRGB || ch == 0) {
+            for (int p = threadIdx.x; p < kSsimPix; p += kSsimThreads) {
+                const int y = oy0 + p / kSsimIW, x = ox0 + p % kSsimIW;
+                float vx[3] = {0.0f, 0.0f, 0.0f}, vy[3] = {0.0f, 0.0f, 0.0f}, vu[3] = {0.0f, 0.0f, 0.0f};
+                if (y < h && x < w) {                              // pixels past the frame feed no valid position
+                    const size_t at = frame + (size_t)y * w + x;
+                    if (SRGB) {
+                        float a[4], b[4], u[4];
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) {
+                            a[k] = __ldg(pred + at + k * plane);
+                            if (corr) a[k] = g * clamp_nan(a[k], 0.0f, 1.0f);
+                            b[k] = __ldg(target + at + k * plane);
+                            if (INPUT) u[k] = __ldg(input + at + k * plane);
+                        }
+                        const IspFrame& F = L.fr[fl];
+                        isp_render(a[0], a[1], a[2], a[3], F, L.inv_gamma, crf_len, nullptr, nullptr, vx);
+                        isp_render(b[0], b[1], b[2], b[3], F, L.inv_gamma, crf_len, nullptr, nullptr, vy);
+                        if (INPUT) isp_render(u[0], u[1], u[2], u[3], F, L.inv_gamma, crf_len, nullptr, nullptr, vu);
+                    } else {
+                        const size_t ac = at + ch * plane;
+                        vx[0] = __ldg(pred + ac);
+                        if (corr) vx[0] = g * clamp_nan(vx[0], 0.0f, 1.0f);
+                        vy[0] = __ldg(target + ac);
+                        if (INPUT) vu[0] = __ldg(input + ac);
+                    }
+#pragma unroll
+                    for (int k = 0; k < NS; ++k) { vx[k] = t2im(vx[k]); vy[k] = t2im(vy[k]); vu[k] = t2im(vu[k]); }
+                }
+#pragma unroll
+                for (int k = 0; k < NS; ++k) {
+                    double* s = stg + k * NI * kSsimPix + p;
+                    s[0] = (double)vx[k];
+                    s[kSsimPix] = (double)vy[k];
+                    if (INPUT) s[2 * kSsimPix] = (double)vu[k];
+                }
+            }
+            __syncthreads();
+        }
+        // row sums: position (r, j) of hs = the sums over pixels (r, j .. j + 6) of the staged tile
+        const double* img = stg + (SRGB ? ch : 0) * NI * kSsimPix;
+        for (int i = threadIdx.x; i < kSsimIH * kSsimTW; i += kSsimThreads) {
+            const int r = i / kSsimTW, j = i % kSsimTW;
+            const double* px = img + r * kSsimIW + j;
+            double m[NM];
+#pragma unroll
+            for (int k = 0; k < NM; ++k) m[k] = 0.0;
+#pragma unroll
+            for (int t = 0; t < kSsimWin; ++t) {
+                const double x = px[t], y = px[kSsimPix + t];
+                m[0] += x; m[1] += y; m[2] += x * x; m[3] += y * y; m[4] += x * y;
+                if constexpr (INPUT) { const double u = px[2 * kSsimPix + t]; m[5] += u; m[6] += u * u; m[7] += u * y; }
+            }
+#pragma unroll
+            for (int k = 0; k < NM; ++k) hs[k * kSsimIH * kSsimTW + i] = m[k];
+        }
+        __syncthreads();
+        // column sums for map rows r0 and r0 + 1 at column `lane`: rows r0 + 1 .. r0 + 6 are shared
+        double s0[NM], s1[NM];
+#pragma unroll
+        for (int k = 0; k < NM; ++k) {
+            const double* col = hs + k * kSsimIH * kSsimTW + r0 * kSsimTW + lane;
+            double inner = col[kSsimTW];
+#pragma unroll
+            for (int t = 2; t < kSsimWin; ++t) inner += col[t * kSsimTW];
+            s0[k] = col[0] + inner;
+            s1[k] = inner + col[kSsimWin * kSsimTW];
+        }
+        if (valid0) {
+            acc += ssim_map(s0[0], s0[1], s0[2], s0[3], s0[4]);
+            if constexpr (INPUT) acc_in += ssim_map(s0[5], s0[1], s0[6], s0[3], s0[7]);
+        }
+        if (valid1) {
+            acc += ssim_map(s1[0], s1[1], s1[2], s1[3], s1[4]);
+            if constexpr (INPUT) acc_in += ssim_map(s1[5], s1[1], s1[6], s1[3], s1[7]);
+        }
+    }
+    const double a = block_sum(acc, sh);
+    const double b = block_sum(acc_in, sh);
+    if (threadIdx.x == 0) {
+        double* slot = scratch + ((size_t)f * gridDim.x + blockIdx.x) * 2;
+        slot[0] = a;
+        if (INPUT) slot[1] = b;
+    }
+}
+
+// one CTA per frame: its tiles' slots summed in a fixed order (thread t takes slots t, t + 256, ..., then block_sum)
+__global__ void __launch_bounds__(256)
+eval_ssim_finalize_kernel(const double* __restrict__ scratch, int tiles, double count, double* __restrict__ ssim,
+                          double* __restrict__ ssim_in)
+{
+    __shared__ double sh[8];
+    const double* s = scratch + (size_t)blockIdx.x * tiles * 2;
+    double a = 0.0, b = 0.0;
+    for (int i = threadIdx.x; i < tiles; i += blockDim.x) {
+        a += s[2 * i];
+        if (ssim_in) b += s[2 * i + 1];
+    }
+    a = block_sum(a, sh);
+    b = block_sum(b, sh);
+    if (threadIdx.x == 0) {
+        ssim[blockIdx.x] = a / count;
+        if (ssim_in) ssim_in[blockIdx.x] = b / count;
+    }
+}
+
+// map tiles per frame; 0 for a frame below 7 x 7 (or a grid row wider than a launch can take)
+static int64_t ssim_tiles(int h, int w, int* tiles_x)
+{
+    if (h < kSsimWin || w < kSsimWin) return 0;
+    const int64_t tx = (w - (kSsimWin - 1) + kSsimTW - 1) / kSsimTW, ty = (h - (kSsimWin - 1) + kSsimTH - 1) / kSsimTH;
+    if (tiles_x) *tiles_x = (int)tx;
+    return tx * ty <= 0x7fffffff ? tx * ty : 0;
+}
+
+template <bool SRGB, bool INPUT>
+static cudaError_t launch_ssim(dim3 grid, cudaStream_t st, const float* pred, const float* target, const float* input,
+                               const float* gain, int c, int tiles_x, double* scratch, const SrgbEvalLaunch& L)
+{
+    constexpr size_t smem = ssim_smem_bytes<SRGB, INPUT>();
+    cudaError_t e = cudaFuncSetAttribute(eval_ssim_kernel<SRGB, INPUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    eval_ssim_kernel<SRGB, INPUT><<<grid, kSsimThreads, smem, st>>>(pred, target, input, gain, c, tiles_x, scratch, L);
+    return cudaGetLastError();
 }
 
 }  // namespace eld
@@ -281,6 +478,74 @@ extern "C" int eld_eval_srgb_psnr(eld_ctx* ctx, const float* pred, const float* 
         count_launch(ctx);
     }
     eval_srgb_finalize_kernel<<<(n + 63) / 64, 64, 0, st>>>(scratch, 3 * plane, n, correct, psnr, psnr_in, gain);
+    ELD_CHECK_CUDA(cudaGetLastError());
+    count_launch(ctx);
+    return ELD_OK;
+}
+
+extern "C" size_t eld_eval_ssim_scratch_bytes(int n, int h, int w)
+{
+    const int64_t tiles = ssim_tiles(h, w, nullptr);
+    return n > 0 && n <= 65535 ? (size_t)n * (size_t)tiles * 2 * sizeof(double) : 0;
+}
+
+extern "C" int eld_eval_ssim(eld_ctx* ctx, const float* pred, const float* target, const float* input, int n, int c, int h,
+                             int w, const float* gain, const float* wb, const float* ccm, double* scratch,
+                             size_t scratch_bytes, double* ssim, double* ssim_in, void* stream)
+{
+    ELD_REQUIRE(ctx && pred && target && scratch && ssim, "eld_eval_ssim: NULL argument");
+    ELD_REQUIRE(!input == !ssim_in, "eld_eval_ssim: input and ssim_in go together");
+    ELD_REQUIRE(!wb == !ccm, "eld_eval_ssim: wb and ccm go together (both given: the sRGB stage)");
+    const bool srgb = wb != nullptr;
+    ELD_REQUIRE(n > 0 && n <= 65535, "eld_eval_ssim: %d frames (1 to 65535, one grid row each)", n);
+    ELD_REQUIRE(srgb ? c == 4 : (c == 3 || c == 4), "eld_eval_ssim: %d channels (%s)", c,
+                srgb ? "the sRGB stage renders 4 packed planes" : "3 or 4");
+    ELD_REQUIRE(h >= kSsimWin && w >= kSsimWin, "eld_eval_ssim: frame %d x %d is smaller than the 7 x 7 window", h, w);
+    int tiles_x = 0;
+    const int64_t tiles = ssim_tiles(h, w, &tiles_x);
+    ELD_REQUIRE(tiles > 0, "eld_eval_ssim: frame %d x %d has more map tiles than a grid row takes", h, w);
+    const size_t need = eld_eval_ssim_scratch_bytes(n, h, w);
+    ELD_REQUIRE(scratch_bytes >= need, "eld_eval_ssim: scratch of %zu bytes, %zu needed (eld_eval_ssim_scratch_bytes)",
+                scratch_bytes, need);
+    const size_t frames = (size_t)n * c * h * w * sizeof(float);
+    const void* ins[4] = {pred, target, input, gain};
+    const size_t in_bytes[4] = {frames, frames, frames, n * sizeof(float)};
+    const void* outs[3] = {scratch, ssim, ssim_in};
+    const size_t out_bytes[3] = {need, n * sizeof(double), n * sizeof(double)};
+    // slots and results are written while other CTAs still read the frames and the gain
+    for (int i = 0; i < 4; ++i)
+        for (int o = 0; o < 3; ++o)
+            ELD_REQUIRE(!ins[i] || !outs[o] || !ranges_overlap(ins[i], in_bytes[i], outs[o], out_bytes[o]),
+                        "eld_eval_ssim: an output overlaps %s", i == 0 ? "pred" : i == 1 ? "target" : i == 2 ? "input" : "gain");
+    for (int o = 0; o < 3; ++o)
+        for (int p = o + 1; p < 3; ++p)
+            ELD_REQUIRE(!outs[o] || !outs[p] || !ranges_overlap(outs[o], out_bytes[o], outs[p], out_bytes[p]),
+                        "eld_eval_ssim: two outputs overlap");
+    ELD_CHECK_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SrgbEvalLaunch L{};
+    L.inv_gamma = 1.0f / 2.2f;                   // as eld_eval_srgb_psnr renders
+    L.h = h; L.w = w;
+    const int chunk = srgb ? kIspMaxFrames : n;  // the sRGB launch carries each frame's wb / ccm
+    for (int f0 = 0; f0 < n; f0 += chunk) {
+        const int nf = n - f0 < chunk ? n - f0 : chunk;
+        L.f0 = f0;
+        if (srgb)
+            for (int f = 0; f < nf; ++f) {
+                for (int i = 0; i < 4; ++i) L.fr[f].wb[i] = wb[(size_t)(f0 + f) * 4 + i];
+                for (int i = 0; i < 9; ++i) L.fr[f].ccm[i] = ccm[(size_t)(f0 + f) * 9 + i];
+            }
+        const dim3 grid((unsigned)tiles, (unsigned)nf);
+        cudaError_t e;
+        if (srgb) e = input ? launch_ssim<true, true>(grid, st, pred, target, input, gain, c, tiles_x, scratch, L)
+                            : launch_ssim<true, false>(grid, st, pred, target, input, gain, c, tiles_x, scratch, L);
+        else      e = input ? launch_ssim<false, true>(grid, st, pred, target, input, gain, c, tiles_x, scratch, L)
+                            : launch_ssim<false, false>(grid, st, pred, target, input, gain, c, tiles_x, scratch, L);
+        ELD_CHECK_CUDA(e);
+        count_launch(ctx);
+    }
+    const double count = (double)(srgb ? 3 : c) * (double)(h - (kSsimWin - 1)) * (double)(w - (kSsimWin - 1));
+    eval_ssim_finalize_kernel<<<n, 256, 0, st>>>(scratch, (int)tiles, count, ssim, ssim_in);
     ELD_CHECK_CUDA(cudaGetLastError());
     count_launch(ctx);
     return ELD_OK;

@@ -37,7 +37,7 @@ def default_opt(**kw):
              beta1=0.9, wd=0.0, loss='l1', noise='g', isTrain=True, save_epoch_freq=100, noise_on_gpu=False,
              augment_on_gpu=False, defer_loss_sync=False, prefetch_noise=False, num_burst=1, pairs_on_gpu=False,
              cuda_graph=False, accum_steps=1, params_on_gpu=False, amsgrad=False,
-             decoupled_weight_decay=False, stage_eval='raw')
+             decoupled_weight_decay=False, stage_eval='raw', eval_ssim=False)
     o.update(kw)
     return SimpleNamespace(**o)
 
@@ -552,26 +552,9 @@ class ELDModel(BaseModel):
         n, c, h, w = predict.shape
         if c != 4:
             raise ValueError('eval_metrics_srgb renders packed RGBG frames [n, 4, h, w]; got %s' % (tuple(predict.shape),))
-
-        def frames(t):
-            t = t.to(device=predict.device, dtype=torch.float32)
-            if t.shape[0] == 1 and n != 1:
-                t = t.expand(n, *t.shape[1:])               # IlluminanceCorrect.forward's broadcast case (:147-149)
-            if tuple(t.shape) != (n, c, h, w):
-                raise ValueError('expected frames of shape %s, got %s' % ((n, c, h, w), tuple(t.shape)))
-            return t.contiguous()
-
-        def table(a, k):
-            a = np.asarray(a.detach().cpu().numpy() if hasattr(a, 'detach') else a, dtype=np.float32).reshape(-1, k)
-            if a.shape[0] == 1 and n != 1:
-                a = np.repeat(a, n, axis=0)
-            if a.shape[0] != n:
-                raise ValueError('expected %d rows of %d values, got %d' % (n, k, a.shape[0]))
-            return np.ascontiguousarray(a)
-
-        target = frames(target)
-        input = frames(input) if input is not None else None
-        wb, ccm = table(wb, 4), table(ccm, 9)
+        target = _frames_like(target, predict)
+        input = _frames_like(input, predict) if input is not None else None
+        wb, ccm = _frame_table(wb, 4, n), _frame_table(ccm, 9, n)
         out = torch.empty_like(predict) if correct else predict
         scratch = torch.empty(n * 4, dtype=torch.float64, device=predict.device)
         psnr = torch.empty(n, dtype=torch.float32, device=predict.device)
@@ -586,6 +569,45 @@ class ELDModel(BaseModel):
             ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), 'eld_eval_srgb_psnr')
         return out, psnr, psnr_in, gain
 
+    def eval_ssim(self, predict, target, input=None, gain=None, wb=None, ccm=None):
+        """quality_assess's SSIM (util/index.py:80: skimage structural_similarity, data_range 255, 7 x 7 uniform window,
+        the 3-pixel border cropped, mean over the channels) of tensor2im(x) against tensor2im(target) per frame, on the
+        device (csrc/eval.cu, eld_eval_ssim: one stencil pass and a finalise, deterministic).  x = gain * clamp(predict,
+        0, 1) with gain [n] the float32 gain the PSNR call returned (eval_metrics / eval_metrics_srgb), or predict when
+        gain is None.  With wb [n, 4] and ccm [n, 3, 3] the packed frames are first rendered to sRGB as
+        eval_metrics_srgb renders them.  predict, target, input: [n, c, h, w] (c = 3 or 4; 4 to render), h, w >= 7; a
+        target (or wb / ccm) of one frame serves every frame.  Returns (ssim [n], ssim_input [n] or None), float64 on
+        the device.  A NaN makes a raw frame's SSIM NaN; rendered, it is black and the SSIM stays finite."""
+        from . import _lib
+        predict = predict.to(dtype=torch.float32).contiguous()
+        n, c, h, w = predict.shape
+        if h < 7 or w < 7:
+            raise ValueError('SSIM takes 7 x 7 windows: frame %d x %d is too small' % (h, w))
+        if (wb is None) != (ccm is None):
+            raise ValueError('the sRGB stage renders with both wb and ccm')
+        target = _frames_like(target, predict)
+        input = _frames_like(input, predict) if input is not None else None
+        dev = predict.device
+        if gain is not None:
+            gain = gain.to(device=dev, dtype=torch.float32).reshape(-1).contiguous()
+            if gain.numel() != n:
+                raise ValueError('expected %d gains, got %d' % (n, gain.numel()))
+        fp = ctypes.POINTER(ctypes.c_float)
+        if wb is not None:
+            wb, ccm = _frame_table(wb, 4, n), _frame_table(ccm, 9, n)
+        lib = _lib.load()
+        nbytes = lib.eld_eval_ssim_scratch_bytes(n, h, w)
+        scratch = torch.empty(max(nbytes // 8, 1), dtype=torch.float64, device=dev)
+        ssim = torch.empty(n, dtype=torch.float64, device=dev)
+        ssim_in = torch.empty(n, dtype=torch.float64, device=dev) if input is not None else None
+        _lib.check(lib.eld_eval_ssim(
+            _lib.ctx(dev.index or 0), predict.data_ptr(), target.data_ptr(), input.data_ptr() if input is not None else None,
+            n, c, h, w, gain.data_ptr() if gain is not None else None, wb.ctypes.data_as(fp) if wb is not None else None,
+            ccm.ctypes.data_as(fp) if ccm is not None else None, scratch.data_ptr(), nbytes,
+            ssim.data_ptr(), ssim_in.data_ptr() if ssim_in is not None else None,
+            ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), 'eld_eval_ssim')
+        return ssim, ssim_in
+
     def illuminance_correct(self, predict, source):
         return self.eval_metrics(predict, source, correct=True)[0]
 
@@ -596,7 +618,10 @@ class ELDModel(BaseModel):
         one host read of the final scalars.  Only the 1st frame is assessed, like the reference (tensor2im takes [0]).
         opt.stage_eval == 'srgb' with opt.stage_out == 'raw' (ELD_model.py:226-233): output, input and target are
         compared in sRGB, rendered with the batch's 'wb' [n, 4] and 'ccm' [n, 3, 3] (the reference reads them from the
-        target's RAW file: process.read_wb_ccm) - eval_metrics_srgb.  self.output stays the corrected raw output."""
+        target's RAW file: process.read_wb_ccm) - eval_metrics_srgb.  self.output stays the corrected raw output.
+        opt.eval_ssim adds quality_assess's SSIM of the output and of the input (util/index.py:80) as 'SSIM' and
+        'SSIM_input', in the same space as the PSNR, on the PSNR call's gain (eval_ssim); the four scalars come back
+        in one host read."""
         srgb = self.opt.stage_out == 'raw' and getattr(self.opt, 'stage_eval', 'raw') == 'srgb'
         if srgb:
             if self.opt.stage_in == 'srgb':
@@ -613,14 +638,19 @@ class ELDModel(BaseModel):
                 h, w = x.shape[2:]
                 y0, x0 = h // 2 - 256, w // 2 - 256                     # util.crop_center
                 x, t = x[:, :, y0:y0 + 512, x0:x0 + 512].contiguous(), t[:, :, y0:y0 + 512, x0:x0 + 512].contiguous()
-            out = self.forward_chop(x) if self.opt.chop else self._padded_forward(x)
+            raw = (self.forward_chop(x) if self.opt.chop else self._padded_forward(x)).contiguous()
             if srgb:
-                out, psnr, psnr_in, _ = self.eval_metrics_srgb(out.contiguous(), t, x, data['wb'], data['ccm'],
-                                                               correct=correct)
+                out, psnr, psnr_in, gain = self.eval_metrics_srgb(raw, t, x, data['wb'], data['ccm'], correct=correct)
             else:
-                out, psnr, _ = self.eval_metrics(out.contiguous(), t, correct=correct)
+                out, psnr, gain = self.eval_metrics(raw, t, correct=correct)
                 _, psnr_in, _ = self.eval_metrics(x, t, correct=False)
             self.output = out
+            if getattr(self.opt, 'eval_ssim', False):
+                ssim, ssim_in = self.eval_ssim(raw, t, x, gain=gain if correct else None,
+                                               **({'wb': data['wb'], 'ccm': data['ccm']} if srgb else {}))
+                four = torch.stack([psnr[0].double(), psnr_in[0].double(), ssim[0], ssim_in[0]]).cpu()
+                return {'PSNR': float(four[0]), 'PSNR_input': float(four[1]), 'SSIM': float(four[2]),
+                        'SSIM_input': float(four[3])}
             both = torch.stack([psnr[0], psnr_in[0]]).cpu()
         return {'PSNR': float(both[0]), 'PSNR_input': float(both[1])}
 
@@ -658,6 +688,28 @@ class ELDModel(BaseModel):
         return {'netG': {k: v.detach().cpu().clone() for k, v in self.netG.state_dict().items()},
                 'opt_g': self.optimizer_G.state_dict(), 'epoch': self.epoch, 'iterations': self.iterations,
                 'frames_seen': self._frames_seen}
+
+
+def _frames_like(t, predict):
+    """t as float32 frames of predict's shape on its device; one frame serves every frame (IlluminanceCorrect.forward's
+    broadcast case, ELD_model.py:147-149)"""
+    n = predict.shape[0]
+    t = t.to(device=predict.device, dtype=torch.float32)
+    if t.shape[0] == 1 and n != 1:
+        t = t.expand(n, *t.shape[1:])
+    if tuple(t.shape) != tuple(predict.shape):
+        raise ValueError('expected frames of shape %s, got %s' % (tuple(predict.shape), tuple(t.shape)))
+    return t.contiguous()
+
+
+def _frame_table(a, k, n):
+    """a host float32 table of n rows of k values (one row serves every frame)"""
+    a = np.asarray(a.detach().cpu().numpy() if hasattr(a, 'detach') else a, dtype=np.float32).reshape(-1, k)
+    if a.shape[0] == 1 and n != 1:
+        a = np.repeat(a, n, axis=0)
+    if a.shape[0] != n:
+        raise ValueError('expected %d rows of %d values, got %d' % (n, k, a.shape[0]))
+    return np.ascontiguousarray(a)
 
 
 def eld_model():

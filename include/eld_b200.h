@@ -258,6 +258,33 @@ int eld_eval_srgb_psnr(eld_ctx* ctx, const float* pred, const float* target, con
                        int n, int h, int w, const float* wb, const float* ccm, int correct, double* scratch,
                        float* psnr, float* psnr_in, float* gain, void* stream);
 
+/* SSIM, the other half of quality_assess (util/index.py:80): skimage's structural_similarity(Y, X, data_range=255,
+ * multichannel=True) with its defaults, on the tensor2im images of frame f (Y the target, X the estimate):
+ *   x = gain[f] * clamp(pred, 0, 1) if gain != NULL (device f32 [n]: the gain eld_eval_correct_psnr or
+ *       eld_eval_srgb_psnr wrote, so the same value), else x = pred
+ *   raw stage (wb == ccm == NULL): the c planes of x and target (c = 3 or 4), each clip(255 v, 0, 255) in f32;
+ *   sRGB stage (wb, ccm both given, c = 4): eld_eval_srgb_psnr's render R(.) first (gamma 2.2, no CRF; a NaN pixel
+ *       renders 0), three channels clip(255 R, 0, 255)
+ *   per channel, in float64: the 7 x 7 uniform-window means ux, uy, uxx, uyy, uxy, cov_norm = 49/48,
+ *   vx = cov_norm (uxx - ux^2), vy likewise, vxy = cov_norm (uxy - ux uy), C1 = (0.01 * 255)^2, C2 = (0.03 * 255)^2,
+ *   S = (2 ux uy + C1)(2 vxy + C2) / ((ux^2 + uy^2 + C1)(vx + vy + C2)) at every window inside the frame (the map
+ *   without its 3-pixel border); ssim[f] = the mean of S over those (h - 6)(w - 6) positions and the channels
+ *   ssim_in[f] the same for input against target (input != NULL).
+ * NaN: in the raw stage a NaN anywhere in a frame's x or target (a NaN gain included) makes ssim[f] NaN; in the sRGB
+ * stage it renders black, and ssim[f] stays finite.  Equal images give exactly 1.
+ * ssim, ssim_in: device f64 [n].  scratch: device, at least eld_eval_ssim_scratch_bytes(n, h, w) bytes, one slot per
+ * map tile of 32 x 16 positions, each written by one CTA and summed in a fixed order: two calls give the same bits.
+ * wb: HOST [n][4], ccm: HOST [n][9] (as eld_eval_srgb_psnr).  Launches: one stencil pass (one per 48 frames in the sRGB
+ * stage), one finalise.  No host synchronisation, no allocation.
+ * ELD_E_ARG, nothing written and nothing launched: a NULL ctx / pred / target / scratch / ssim, input and ssim_in not
+ * both given or both NULL, wb and ccm not both given or both NULL, n < 1 or n > 65535, c other than 3 or 4 (other than 4
+ * in the sRGB stage), h < 7 or w < 7 (skimage raises ValueError), scratch_bytes short, scratch / ssim / ssim_in
+ * overlapping pred, target, input, gain or each other. */
+size_t eld_eval_ssim_scratch_bytes(int n, int h, int w);     /* 0 for n, h, w eld_eval_ssim refuses */
+int eld_eval_ssim(eld_ctx* ctx, const float* pred, const float* target, const float* input, int n, int c, int h, int w,
+                  const float* gain, const float* wb, const float* ccm, double* scratch, size_t scratch_bytes,
+                  double* ssim, double* ssim_in, void* stream);
+
 /* Number of kernels the library has launched through this ctx since creation (bench.py's
  * gpu_launches evidence). */
 int64_t eld_launch_count(const eld_ctx* ctx);
